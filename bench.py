@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — CenterPoint frames/s on B200 (driver contract, see the task's Measurement rules).
+"""bench.py — CenterPoint frames/s on an H100.
 
   python bench.py [--gpus N] [--steps K] [--warmup W]            this repo's CUDA path
+  python bench.py ... --dump-outputs DIR                         + the last timed frame's boxes / scores / labels as .npy
   python bench.py --impl reference [--steps K] [--warmup W]      the reference's CPU arm on the host cores
 
 A step = one synthetic nuScenes-shaped frame (300k x 5 points, 1440 x 1440 x 40 grid, max 160000 voxels) through the
@@ -14,8 +15,7 @@ round-1 workload (resident synthetic head tensors).
 
 `value`  : frames/s with the frame's points already resident in HBM (CUDA-graph replay per frame), --in-flight frames
            (default 4) computing concurrently per GPU: CenterPointSweep lanes with their own buffers / graph / stream and a
-           shared model (measured: 605 / 709 / 740 / 754 / 735 frames/s with 1 / 2 / 3 / 4 / 6 lanes - the latency-bound
-           kernels of one frame fill the SMs the other frames leave idle).
+           shared model (the latency-bound kernels of one frame fill the SMs the other frames leave idle).
 `e2e`    : frames/s through the public API CenterPointSweep.infer_many(): pinned-host points -> H2D ->
            graph -> D2H of boxes/scores/labels/counts/status, every step; the H2D of a lane's next frame overlaps its
            compute (copy stream + two staging buffers per lane). `e2e.sync_value` is the one-frame-at-a-time
@@ -45,14 +45,14 @@ WORKLOAD = ("CenterPoint-voxel nuScenes-shape frame, 300k x 5 points, 1440x1440x
 HEAD_ON = "SecondBackbone + SecondFPN + CenterHead (2 x 6 + 2 + 1 + 36 + 36 convs, 234 GFLOP)"
 HEAD_OFF = "resident synthetic head tensors (dense RPN/head skipped: --no-head)"
 BN_GAIN = 6.0 ** 0.5  # seeded weights with BatchNorm gamma = sqrt(6): activations stay O(1) through the 21 + 54 convs
-POOL = 32  # distinct frames cycled through: 32 x 6 MB = 192 MB of inputs > 126 MB L2
+POOL = 32  # distinct frames cycled through: 32 x 6 MB = 192 MB of inputs > 50 MB L2 (H100)
 
 
 def make_config(geometry, with_head, in_flight=4):
     """The `config` object both arms print (identical dicts: the driver compares them)."""
     geo = "0.075 m voxels / +-54 m range" if geometry == "0075" else "0.1 m voxels / +-72 m range"
     return {"workload": WORKLOAD % (geo, HEAD_ON if with_head else HEAD_OFF), "geometry": geometry, "with_head": bool(with_head),
-            "frames_in_pool": POOL, "l2": "input pool 192 MB > 126 MB L2; no explicit flush",
+            "frames_in_pool": POOL, "l2": "input pool 192 MB > 50 MB L2; no explicit flush",
             "frames_in_flight_per_gpu": int(in_flight)}
 
 
@@ -75,7 +75,7 @@ def frame_pool(cfg, n_frames, seed0=0, base=4):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -123,8 +123,8 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
-    return 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+        return d.get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
+    return 3350.0, "H100 SXM data sheet 3.35 TB/s (not measured)"
 
 
 def cpu_threads_for_reference():
@@ -175,10 +175,7 @@ def run_reference(args):
     n_warm = min(args.warmup, 1)  # a frame costs ~10 s on the host: one untimed frame warms caches / page tables
     for i in range(n_warm):
         cf.run(frames[i % len(frames)])
-    per_frame = (time.perf_counter() - t_w) / max(n_warm, 1)
-    # bound the run: the number of timed frames is capped at what fits in about two minutes (the per-frame throughput
-    # is what is reported, not a total)
-    steps = max(1, min(args.steps, int(120.0 / max(per_frame, 1e-3))))
+    steps = args.steps  # a host frame takes seconds: pass a small --steps for a short run
     t0 = time.perf_counter()
     stages = {}
     for i in range(steps):
@@ -186,7 +183,6 @@ def run_reference(args):
         for k, v in r["times"].items():
             stages[k] = stages.get(k, 0.0) + v
     dt = time.perf_counter() - t0
-    requested, args.steps = args.steps, steps
     fps = args.steps / dt
     cores = oracle.num_threads()
     sample = ("%d full frames; voxelize = %s, voxel_mean / sparse conv / to_dense / dense RPN+head / postprocess = oracle "
@@ -199,8 +195,7 @@ def run_reference(args):
             "config": make_config(args.geometry, with_head, max(1, args.in_flight)),
             "cpu_baseline": {"value": fps, "unit": UNIT, "cores": cores, "kind": "port", "sample": sample},
             "e2e": {"value": fps, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
-            "stage_ms": {k: 1e3 * v / args.steps for k, v in stages.items()}, "gpu_launches": 0,
-            "steps_requested": requested}
+            "stage_ms": {k: 1e3 * v / args.steps for k, v in stages.items()}, "gpu_launches": 0}
     print(json.dumps(line))
 
 
@@ -222,44 +217,6 @@ def graph_time_ms(fn, stream, iters=5):
         e.record(stream)
     e.synchronize()
     return s.elapsed_time(e) / iters
-
-
-def ncu_dram_bytes(path_name):
-    """dram__bytes_read.sum + dram__bytes_write.sum summed over the launches of a committed ncu capture
-    (profiles/<path_name>: rows = launches of one frame); None when the capture is not in the tree."""
-    import csv
-    path = os.path.join(ROOT, "profiles", path_name)
-    if not os.path.exists(path):
-        return None
-    try:
-        rows = list(csv.reader(open(path)))
-        hdr, units = rows[0], rows[1]
-        scale = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-        total = 0.0
-        for name in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-            i = hdr.index(name)
-            total += sum(float(r[i]) for r in rows[2:]) * scale[units[i]]
-        return total
-    except (ValueError, KeyError, IndexError, OSError):
-        return None  # a malformed capture must not take the benchmark down
-
-
-def ncu_tensor_active(path_name):
-    """Time-weighted sm__pipe_tensor_cycles_active (% of peak sustained active) over the launches of a committed ncu capture
-    (tcgen05 and legacy HMMA launches alike); None when the capture is not in the tree."""
-    import csv
-    path = os.path.join(ROOT, "profiles", path_name)
-    if not os.path.exists(path):
-        return None
-    try:
-        rows = list(csv.reader(open(path)))
-        hdr = rows[0]
-        it, ia = hdr.index("gpu__time_duration.sum"), hdr.index("sm__pipe_tensor_cycles_active.avg.pct_of_peak_sustained_active")
-        t = [float(r[it]) for r in rows[2:]]
-        a = [float(r[ia]) for r in rows[2:]]
-        return sum(x * y for x, y in zip(t, a)) / sum(t) if sum(t) > 0 else None
-    except (ValueError, KeyError, IndexError, OSError):
-        return None
 
 
 def dense_flops(net, H, W):
@@ -286,9 +243,21 @@ def dense_flops(net, H, W):
     return total
 
 
-def measure(sweep, dev_frames, host_frames, args, world, dist, sample_clocks, local):
+def dump_outputs(lane, out_dir):
+    """What the timed path handed back for its last frame (the arrays CenterPointHotPath.infer returns): boxes [K, 9],
+    scores [K] as float32, labels [K] as float64 (exact small integers), one .npy each."""
+    o = lane.out
+    lane.check_status(o["status"].cpu())  # a frame that overflowed fp16 or dropped sites raises instead of being saved
+    k = int(o["counts"][-1].item())
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "boxes.npy"), o["boxes"][:k].float().cpu().numpy())
+    np.save(os.path.join(out_dir, "scores.npy"), o["scores"][:k].float().cpu().numpy())
+    np.save(os.path.join(out_dir, "labels.npy"), o["labels"][:k].cpu().numpy().astype(np.float64))
+
+
+def measure(sweep, dev_frames, host_frames, args, world, dist, sample_clocks, local, dump_dir=None):
     """Device-timed resident-input rate, e2e (pipelined and one-frame-at-a-time) for one sweep engine (len(sweep) frames in
-    flight, CenterPointSweep).  Returns a dict."""
+    flight, CenterPointSweep).  dump_dir: write the outputs of the last timed frame there.  Returns a dict."""
     import torch
     pipe = sweep.lanes[0]
     st = pipe.stream
@@ -324,6 +293,8 @@ def measure(sweep, dev_frames, host_frames, args, world, dist, sample_clocks, lo
     barrier()
     wall = time.perf_counter() - t0
     dev_ms = s.elapsed_time(e)
+    if dump_dir and args.steps > 0:
+        dump_outputs(sweep.lanes[(args.steps - 1) % len(sweep)], dump_dir)
     # ---- e2e through the public API (host in, host out), same K
     sweep.prepare_sweep()
     for i in range(3):
@@ -433,6 +404,8 @@ def main():
     ap.add_argument("--no-head", action="store_true", help="skip the dense RPN / neck / CenterHead (round-1 workload)")
     ap.add_argument("--no-second-geometry", action="store_true")
     ap.add_argument("--in-flight", type=int, default=4, help="frames computing concurrently per GPU (CenterPointSweep lanes)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the boxes / scores / labels of the last timed frame to DIR/*.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     if args.impl == "reference":
@@ -481,7 +454,8 @@ def main():
         p.capture()
     graph_nodes = pipe.graph_nodes["kernel"] if (rank == 0 and pipe.graph_nodes) else None
     st = pipe.stream
-    m = measure(sweep, dev_frames, host_frames, args, world, dist, True, local)
+    m = measure(sweep, dev_frames, host_frames, args, world, dist, True, local,
+                dump_dir=args.dump_outputs if rank == 0 else None)
 
     # ---- the other geometry, same model, shorter run (reported, not the headline)
     other = None
@@ -567,7 +541,7 @@ def main():
             layers.append({"cin": cin, "cout": cout, "rows": rows, "pairs": pairs, "ms": round(ms, 4),
                            "precision": {sp.F16X3: "f16x3", sp.FP32: "fp32"}.get(prec, "tf32x3"), "gflop": round(fl / 1e9, 3),
                            "kernel": ("wm::conv_wm_kernel (register gather + mma.sync)" if kern == "wm" else
-                                      "tcgen05" if prec in tcp else "small_cin (fp32 FMA)")})
+                                      "wgmma" if prec in tcp else "small_cin (fp32 FMA)")})
             if prec in tcp:
                 tc_ms += ms
                 tc_flops += fl
@@ -578,12 +552,12 @@ def main():
         extra["sparse_conv_layers"] = layers
         pkp = os.path.join(ROOT, "MEASURED_PEAKS.json")
         pk = json.load(open(pkp)) if os.path.exists(pkp) else {}
-        bf16_peak = pk.get("bf16_tflops", 1590.0)
-        tpeak_src = "MEASURED_PEAKS.json bf16_tflops (burst)" if pk else "fallback 1.59 PFLOP/s"
+        bf16_peak = pk.get("bf16_tflops", 989.0)
+        tpeak_src = "MEASURED_PEAKS.json bf16_tflops (burst)" if pk else "H100 SXM data sheet 989 TFLOP/s dense fp16/bf16 at 700 W (not measured)"
         rooflines = []
         rooflines.append({"bound": "hbm", "kernel": "hard_voxelize op (reference API: zero-padded [V, P, F] output)",
                           "achieved": vox_bytes / (ms_vox * 1e-3) / 1e9, "peak": hbm_peak, "unit": "GB/s",
-                          "frac": vox_bytes / (ms_vox * 1e-3) / 1e9 / hbm_peak, "traffic": ncu_dram_bytes("r02_voxelize_ncu_metrics.csv"),
+                          "frac": vox_bytes / (ms_vox * 1e-3) / 1e9 / hbm_peak,
                           "algorithmic_bytes": vox_bytes, "ms": ms_vox, "peak_source": peak_src})
         sparse_roof = None
         if tc_ms > 0:
@@ -593,14 +567,10 @@ def main():
                 kname += " (wide layers) + wm::conv_wm_kernel (16/32-channel layers, %.3f ms)" % wm_ms
             sparse_roof = {"bound": "tensor", "kernel": kname + " (the 20 tensor-core sparse convs of one frame)",
                            "achieved": ach, "peak": bf16_peak, "unit": "TFLOP/s", "frac": ach / bf16_peak,
-                           "traffic": ncu_dram_bytes("r02_sparse_ncu_metrics.csv"),
-                           "tensor_pipe_active_pct_ncu": ncu_tensor_active("r02_sparse_ncu_metrics.csv"),
                            "algorithmic_flops": tc_flops, "ms": tc_ms,
                            "peak_source": tpeak_src,
                            "note": "achieved counts ALGORITHMIC flops 2*pairs*Cin*Cout; the kernels execute 3 fp16 MMAs per "
-                                   "product on zero-padded row tiles; bound by the row gather (tcgen05 kernel: L1TEX wavefronts "
-                                   "per gathered row, profiles/r02_f16_sweep.md; warp-MMA kernel: L2 latency of the register "
-                                   "gather + issue slots, profiles/r02_wm_ncu_metrics.csv), not by the tensor pipe"}
+                                   "product on zero-padded row tiles"}
         dense_roof = None
         if pipe.dense is not None:
             if pipe.out["bev_h16"] is not None:
@@ -614,13 +584,11 @@ def main():
             ach = fl / (ms_dense * 1e-3) / 1e12
             dense_roof = {"bound": "tensor", "kernel": "dcf::dense_conv_f16_kernel (RPN + neck + CenterHead: 16 + 1 + 1 launches)",
                           "achieved": ach, "peak": bf16_peak, "unit": "TFLOP/s", "frac": ach / bf16_peak,
-                          "traffic": ncu_dram_bytes("r02_dense_ncu_metrics.csv"),
-                          "tensor_pipe_active_pct_ncu": ncu_tensor_active("r02_dense_ncu_metrics.csv"),
                           "algorithmic_flops": fl, "ms": ms_dense,
                           "peak_source": tpeak_src,
                           "note": "achieved counts ALGORITHMIC flops (2 x MACs of the convolutions); the kernel executes 3 fp16 "
                                   "MMAs per product (fp16-pair operands, 1e-4 parity), i.e. the tensor pipe runs at 3 x "
-                                  "this fraction of the measured fp16/bf16 peak"}
+                                  "this fraction of the fp16/bf16 peak"}
         cands = [r for r in (dense_roof, sparse_roof) if r is not None]
         cands.sort(key=lambda r: -r["ms"])
         if cands:

@@ -1,5 +1,5 @@
 /*
- * p3d_b200.h — C ABI of libp3d_b200.so: the B200 (sm_100a) implementation of Paddle3D's
+ * p3d_b200.h — C ABI of libp3d_b200.so: the H100 (sm_90a) implementation of Paddle3D's
  * point-cloud-to-BEV hot path.  This is the drop-in boundary: every entry point below is what a
  * Paddle custom-op kernel function (PD_BUILD_OP ... SetKernelFn) for this path binds to; the
  * reference interface each one replaces is cited as file:line under PaddlePaddle/Paddle3D @ 3259dabe.
@@ -201,8 +201,8 @@ int p3d_sparse_affine_act(const float *x, const int32_t *n_dev, int64_t n_cap, i
  *   in [n_in, Cin] fp32; W [K, Cin, Cout] fp32 (Paddle's [kD,kH,kW,Cin,Cout]); scale/shift [Cout]
  *   (BatchNorm(eval) and conv bias folded by the caller; NULL = identity); residual [n_out, Cout] or
  *   NULL; relu != 0 applies max(.,0).  n_out_dev: device row count (NULL = n_out_cap rows).
- *   precision: P3D_CONV_FP32 = fp32 FMA on CUDA cores; P3D_CONV_TF32X3 = tcgen05 tensor cores with
- *   3xTF32 split accumulation in TMEM (fp32-level accuracy). */
+ *   precision: P3D_CONV_FP32 = fp32 FMA on CUDA cores; P3D_CONV_TF32X3 = wgmma tensor cores with
+ *   3xTF32 split accumulation in registers (fp32-level accuracy). */
 enum p3d_conv_precision { P3D_CONV_FP32 = 0, P3D_CONV_TF32X3 = 1 };
 /* Weight pre-pack for P3D_CONV_TF32X3 (once per layer): splits W [K, Cin, Cout] into tf32 hi / lo and lays it out
  * as the shared-memory image the tensor-core kernel streams with cp.async.bulk.  Needs Cin, Cout multiples of
@@ -295,7 +295,7 @@ int p3d_sparse_conv_f16(const void *in_h16, const int32_t *nbr, const int32_t *n
 /* Narrow layers (Cin, Cout) in {(16,16), (16,32), (32,32)}: register gather + warp MMA (csrc/sparse_conv_wm.cu), same
  * H16 rows in and out, same fused epilogue and the same three-product arithmetic as p3d_sparse_conv_f16; only the weight
  * image differs (mma.sync fragment order, k permuted so that a lane's fragment is 4 contiguous channels of a row).
- * Missing neighbours cost nothing here (predicated-off loads), which is what bounds the tcgen05 kernel at these widths.
+ * Missing neighbours cost nothing here (predicated-off loads), unlike the staged gathers of the wgmma kernel.
  * Work is cut stream-K style into equal (tile, tap) ranges per warp; a tile cut by a range boundary is summed by the last
  * warp to finish it, pieces in warp order (deterministic).  workspace = p3d_sparse_conv_wm_workspace_bytes(...) bytes whose
  * first align_up(ceil(n_out_cap / 16) * 4) bytes (tickets) must be ZERO on first use (the kernel leaves them zero).
@@ -310,7 +310,7 @@ int p3d_sparse_conv_wm(const void *in_h16, const int32_t *nbr, const int32_t *n_
                        size_t workspace_bytes, int32_t *status_dev, p3d_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
- * SURVEY.md 8f-1 (parity-green, performance not measured yet): dense 2-D convolution on tcgen05 for the RPN / neck /
+ * SURVEY.md 8f-1: dense 2-D convolution on wgmma (tf32 pairs) for the RPN / neck /
  * CenterHead (reference: backbones/second_backbone.py:72-120, necks/second_fpn.py:99-160,
  * detection/centerpoint/center_head.py:43-220).  Images are "pixel split rows" [B*H*W][2][C] (the split-row format
  * of the sparse layers with row = pixel).
@@ -342,7 +342,7 @@ int p3d_head_final_conv_h16(const void *in_h16, int B, int H, int W, int in_C, i
 
 /* fp16-pair dense convolution (csrc/dense_conv_f16.cu): same layer contract as p3d_dense_conv2d_split on pixel H16
  * rows [B*H*W][C / 32 groups][hi 32 | lo' 32] halfs.  3x3 / stride 1 / pad 1 layers load the haloed tile once per
- * 32-channel group and read the 9 taps through shifted UMMA descriptors; everything else loads one box per tap.
+ * 32-channel group and read the 9 taps through shifted wgmma descriptors; everything else loads one box per tap.
  * mode 0 = auto, 1 = force per-tap loads; m_tiles 0 = auto, 1 or 2 M tiles (8 x 16 pixels each) per work item. */
 int p3d_nchw_to_pixel_h16(const float *in, int B, int C, int H, int W, void *out_h16, int32_t *status_dev,
                           p3d_stream_t stream);

@@ -22,8 +22,16 @@ u64p = np.ctypeslib.ndpointer(np.uint64, flags="C_CONTIGUOUS")
 
 
 def build(ref=True):
-    """(Re)build the oracle library and, when /root/reference is present, oracle/_ref."""
+    """(Re)build the oracle library and, when a Paddle3D checkout is named by $P3D_REFERENCE, oracle/_ref."""
     subprocess.run(["make", "-s", "-C", _HERE, "oracle"] + (["ref"] if ref else []), check=True)
+
+
+REF_LIBS = ("cpu", "iou3d_gpu", "cpp_gpu", "bevpool_gpu")
+
+
+def ref_missing():
+    """Names of the reference libraries (oracle/_ref) that are not built."""
+    return [n for n in REF_LIBS if not os.path.exists(os.path.join(_HERE, "_ref", "libp3d_ref_%s.so" % n))]
 
 
 def lib():

@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE ONLY — not part of the product.
 // extern "C" entry points around the UNMODIFIED reference CPU ops, which are
-// compiled from where they lie under /root/reference by oracle/Makefile:
+// compiled from where they lie in a Paddle3D checkout ($P3D_REFERENCE) by oracle/Makefile:
 //   paddle3d/ops/voxel/voxelize_op.cc:84-146   hard_voxelize_cpu
 //   paddle3d/ops/iou3d_nms/iou3d_cpu.cpp:241-264  boxes_iou_bev_cpu
 // The wrappers only marshal raw host pointers into the stub paddle::Tensor.

@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE ONLY — not part of the product.
 // extern "C" entry points around the UNMODIFIED reference CUDA launchers, compiled
-// for sm_100a from where they lie under /root/reference by oracle/Makefile.  These
+// for sm_90a from where they lie in a Paddle3D checkout ($P3D_REFERENCE) by oracle/Makefile.  These
 // are "the kernels to beat" and the GPU-side parity oracle (raw device pointers in/out):
 //   paddle3d/ops/iou3d_nms/iou3d_nms_kernel.cu:436-482   BoxesOverlap/BoxesIouBev/Nms/NmsNormal launchers
 //   paddle3d/ops/centerpoint_postprocess/iou3d_nms_kernel.cu:341-352  indexed NmsLauncher

@@ -2,7 +2,7 @@
 //
 // Minimal stand-in for PaddlePaddle's `paddle/extension.h`, written for this
 // repo so that the reference's *CPU* custom-op sources under
-// /root/reference/paddle3d/ops can be compiled unmodified into oracle/_ref/
+// $P3D_REFERENCE/paddle3d/ops can be compiled unmodified into oracle/_ref/
 // (PaddlePaddle itself is not installable in this image, SURVEY.md fact 2).
 // It models exactly the API surface those files touch:
 //   paddle3d/ops/voxel/voxelize_op.cc        (Tensor::shape/data/size/type/is_cpu, empty, full,

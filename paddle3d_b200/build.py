@@ -1,4 +1,4 @@
-"""Build libp3d_b200.so in-tree with nvcc for sm_100a (one object per .cu, in parallel)."""
+"""Build libp3d_b200.so in-tree with nvcc for sm_90a (one object per .cu, in parallel)."""
 import os
 import subprocess
 import sys
@@ -10,7 +10,8 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(CSRC, "_obj")
 LIB = os.path.join(HERE, "libp3d_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-Xcompiler", "-fPIC",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]  # Hopper (H100): wgmma, TMA
+FLAGS = ["-O3", "-std=c++17"] + ARCH + ["-lineinfo", "-Xcompiler", "-fPIC",
          "-I", os.path.join(ROOT, "include"), "-I", CSRC] + os.environ.get("P3D_NVCC_EXTRA", "").split()
 
 
@@ -47,7 +48,7 @@ def build(verbose=False, force=False):
         raise RuntimeError("nvcc failed")
     objs = [os.path.join(OBJ, s[:-3] + ".o") for s in srcs]
     if jobs or not os.path.exists(LIB):
-        cmd = [NVCC, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB] + objs
+        cmd = [NVCC, "-shared"] + ARCH + ["-o", LIB] + objs
         subprocess.run(cmd, check=True)
     return LIB
 

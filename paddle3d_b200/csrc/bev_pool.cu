@@ -1,4 +1,4 @@
-// bev_pool_v2 forward / backward for sm_100a.
+// bev_pool_v2 forward / backward for sm_90a.
 //
 // Replaces paddle3d/ops/bev_pool_v2/bev_pool_cuda.cu:18-116 (and the duplicate in
 // ops/bev_pool_v2_backward).  Same arithmetic in the same order — one fp32 FMA per point, summed in

@@ -1,4 +1,4 @@
-// Shared helpers for libp3d_b200 (sm_100a only).
+// Shared helpers for libp3d_b200 (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -47,7 +47,13 @@ inline uint32_t next_pow2(uint64_t x) {
   return static_cast<uint32_t>(p);
 }
 
-constexpr int kNumSMs = 148;  // B200
+// Multiprocessors of the current device (persistent grids are sized by it; 132 on an H100 SXM).
+inline int num_sms() {
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1)
+    return 132;
+  return n;
+}
 
 // Programmatic dependent launch: the grid may be scheduled while its predecessor in the stream drains.  Every kernel
 // launched this way executes pdl_wait() before it touches global memory (and pdl_trigger() first, so that ITS successor

@@ -1,4 +1,4 @@
-// Dense 2-D convolution on tcgen05 with fp16 (hi, lo') pair operands for the RPN / neck / CenterHead row (SURVEY.md §8f-1;
+// Dense 2-D convolution on wgmma with fp16 (hi, lo') pair operands for the RPN / neck / CenterHead row (SURVEY.md §8f-1;
 // reference: backbones/second_backbone.py:72-120, necks/second_fpn.py:99-160, detection/centerpoint/center_head.py:43-220).
 //
 // Images travel between layers as "pixel H16 rows": NHWC, each pixel's C channels as groups of 32 channels
@@ -6,21 +6,21 @@
 // One (32-channel group) x (pixel box) TMA load therefore lands in shared memory as a SWIZZLE_128B K-major operand tile
 // whose k-steps 0,1 are the hi halves and 2,3 the lo' halves; the three partial products run as
 //   D[0, N) += A_hi x B_hi          D[N, 2N) += A_hi x B_lo' + A_lo' x B_hi        out = D[0, N) + D[N, 2N) * 2^-11
-// with one MMA A_hi x [B_hi | B_lo'] (N' = 2N) and one MMA A_lo' x B_hi per 16-channel k-step (kind::f16).
+// (three m64nN wgmma per 16-channel k-step and warpgroup; the accumulators live in registers).
 //
-// The tf32 kernel this replaces (dense_conv_tc.cu) ran at the L2 -> SM bandwidth limit (measured 12.5 TB/s aggregate on the
-// 256 -> 128 layer): every 3x3 tap re-loaded its shifted 128-pixel window and the weights of the use.  Here
-//   * HALO mode (3x3, stride 1, pad 1 - 94 % of the flops): the haloed tile (10 x 18 pixels for an 8 x 16 output tile, or
-//     10 x 34 for 8 x 32 = two M tiles) of a 32-channel group is loaded ONCE; the A operand of tap (dy, dx) is the same
+//   * HALO mode (3x3, stride 1, pad 1): the haloed tile (10 x 18 pixels for an 8 x 16 output tile, or 10 x 34 for
+//     8 x 32 = two M tiles) of a 32-channel group is loaded ONCE; the A operand of tap (dy, dx) is the same
 //     shared-memory tile read through a descriptor whose start address is shifted by (dy * 10 + dx) rows and whose 8-row
-//     group stride (SBO) is one haloed image row (1280 bytes): 6.3x less activation traffic.  The swizzle is a function of
-//     the absolute shared-memory address bits, so TMA's writes and the shifted UMMA reads agree (descriptor base_offset 0;
-//     verified on the B200 for both row pitches, tests/test_gpu_dense.py).
-//   * TAP mode (1x1, stride 2, transposed k = s): one TMA box per (tap, group), as before, half the bytes.
-//   * MT = 2: two M tiles (8 x 32 pixels) share every weight block: half the weight traffic per flop.
+//     group stride (SBO) is one haloed image row (1280 bytes).  The swizzle is a function of the absolute shared-memory
+//     address bits, so TMA's writes and the shifted wgmma reads agree (descriptor base_offset 0, tests/test_gpu_dense.py).
+//   * TAP mode (1x1, stride 2, transposed k = s): one TMA box per (tap, group).
+//   * MT = 2 (N tile <= 64): two M tiles (8 x 32 pixels) share every weight block: half the weight traffic per flop.
 //
 //   work item   (batch, pixel tile, N tile[, tap of a k = s transposed conv]), N tile fastest
-//   warps 0-3   epilogue (TMEM lane quarter = warp)   4  MMA issue   5  activation TMA   6  weight blocks (cp.async.bulk)
+//   step        (A unit, tap): HALO one A unit per 32-channel group serves 9 steps, TAP one A unit per step.  Thread 0
+//               keeps an activation ring (NA) and a weight ring (NB) ahead of the consumers across work items (TMA /
+//               cp.async.bulk, mbarrier complete_tx); warpgroup g computes rows 64g .. 64g+63 of every M tile and runs
+//               their epilogue from its registers.
 #include <cuda.h>
 #include <cuda_fp16.h>
 
@@ -32,9 +32,8 @@ namespace dcf {
 
 using namespace tc;
 
-constexpr int kTW = 8, kTH = 16;        // output tile of one M = 128 UMMA: 8 x 16 pixels
-constexpr int kThreadsD = 7 * 32;
-constexpr int kMaxB = 12;               // weight ring depth limit
+constexpr int kTW = 8, kTH = 16;        // output tile of one M = 128 tile: 8 x 16 pixels
+constexpr int kMaxA = 6, kMaxB = 12;    // activation / weight ring depth limits
 constexpr float kLoScale = 2048.0f, kLoInv = 1.0f / 2048.0f;
 
 struct Params {
@@ -57,7 +56,7 @@ struct Params {
   // columns to the fp32 planes grp_plane0[nt] .. of out_nchw ([B, cout planes, out_H, out_W]); shift is [n_ntiles][N]
   int grouped, in_C;
   const int32_t *grp_plane0, *grp_cnt;
-  int base_offset_mode;       // 0 (default, measured correct): base_offset field zero; 1: address bits 7-9 (wrong results)
+  int base_offset_mode;       // 0 (default): base_offset field zero; 1: address bits 7-9 of the shifted start address
   int w_bytes;                // weight-stationary kernel: bytes of one N tile's weight image (taps * Cin / 16 k-blocks)
 };
 
@@ -70,66 +69,30 @@ template <int N, int MT, bool HALO, int PITCH, bool WS = false>
 struct Cfg {
   static constexpr int A_ROWS = HALO ? PITCH * (kTH * MT + 2) : kM * MT;     // rows of 128 bytes per activation buffer
   static constexpr int A_BYTES = ((A_ROWS * 128 + 1023) / 1024) * 1024;
-  static constexpr int NA = WS ? 3 : (HALO ? 2 : 3);                         // activation buffers
   static constexpr int B_BYTES = 128 * N;                                    // weight blocks of one (tap, group): 2 k-blocks
   static constexpr int B_BLK = 64 * N;
-  static constexpr int BUDGET = (227 - 6) * 1024 - NA * A_BYTES;  // 227 KB - alignment slack - static (barriers, scale / shift)
+  // TAP mode: every step needs a new activation buffer, so both rings get the same depth; HALO: 2 (WS: 3) buffers
+  static constexpr int NA_TAP_RAW = (227 - 6) * 1024 / (A_BYTES + B_BYTES);
+  static constexpr int NA = WS ? 3 : (HALO ? 2 : (NA_TAP_RAW > kMaxA ? kMaxA : NA_TAP_RAW));
+  static constexpr int BUDGET = (227 - 6) * 1024 - NA * A_BYTES;  // 227 KB - alignment slack - static (barriers)
   static constexpr int NB_RAW = BUDGET / B_BYTES;
   static constexpr int NB = NB_RAW > kMaxB ? kMaxB : NB_RAW;                 // weight ring depth
-  static constexpr int ACC_COLS = MT * 2 * N;                                // TMEM columns of one accumulator set
-  static constexpr int NBUF = (2 * ACC_COLS <= 512) ? 2 : 1;                 // double-buffered accumulators when they fit
-  static constexpr int TMEM_COLS = (NBUF * ACC_COLS <= 64) ? 64 : (NBUF * ACC_COLS <= 128) ? 128 : (NBUF * ACC_COLS <= 256) ? 256 : 512;
-  static constexpr uint32_t IDESC2 = (1u << 4) | (static_cast<uint32_t>((2 * N) >> 3) << 17) | (static_cast<uint32_t>(kM >> 4) << 24);
-  static constexpr uint32_t IDESC1 = (1u << 4) | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(kM >> 4) << 24);
+  static constexpr int ACC = MT * N;                                         // fp32 registers per thread
+  static constexpr int SPU = HALO ? 9 : 1;                                   // steps per activation buffer
   static_assert(N == 16 || N == 64 || N == 128, "N tile: 16 (grouped output convs), 64 or 128");
   static_assert(MT == 1 || MT == 2, "one or two M tiles");
-  static_assert(WS || NB >= 4, "weight ring too shallow");
+  static_assert(MT * N <= 128, "accumulators: at most 128 registers per thread");
+  static_assert(WS || NB >= 3, "weight ring too shallow");
+  static_assert(NA >= 2 && NA <= kMaxA, "activation ring depth");
   static_assert(!WS || (HALO && MT == 1), "weight-stationary: haloed 3x3 tiles, one M tile");
-  static_assert(ACC_COLS <= 512, "accumulators exceed TMEM");
 };
 
-// SWIZZLE_128B K-major descriptor with an explicit 8-row-group stride and the base offset of a start address that is not
-// 1024-byte aligned (bits 7-9 of the address: the row phase of the swizzle pattern)
-__device__ __forceinline__ uint64_t desc_sw128_at(uint32_t addr, uint32_t sbo_bytes, int bo_mode) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((addr & 0x3ffffu) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3fffu) << 32;
-  d |= 1ull << 46;
-  if (bo_mode) d |= static_cast<uint64_t>((addr >> 7) & 7u) << 49;
-  d |= 2ull << 61;
-  return d;
-}
-__device__ __forceinline__ void mma_f16_elect(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p, e;\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "@e tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void commit_elect(uint32_t bar) {
-  asm volatile(
-      "{\n\t.reg .pred e;\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(bar)
-      : "memory");
-}
 __device__ __forceinline__ void tma_tile4d(uint32_t dst, const CUtensorMap *map, int c, int x, int y, int b, uint32_t bar) {
   asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cta.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];" ::
+      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];" ::
           "r"(dst),
       "l"(reinterpret_cast<uint64_t>(map)), "r"(c), "r"(x), "r"(y), "r"(b), "r"(bar)
       : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&a)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-      "[%16];"
-      : "=r"(a[0]), "=r"(a[1]), "=r"(a[2]), "=r"(a[3]), "=r"(a[4]), "=r"(a[5]), "=r"(a[6]), "=r"(a[7]), "=r"(a[8]),
-        "=r"(a[9]), "=r"(a[10]), "=r"(a[11]), "=r"(a[12]), "=r"(a[13]), "=r"(a[14]), "=r"(a[15])
-      : "r"(taddr));
 }
 __device__ __forceinline__ void split_h16(float x, __half &hi, __half &lo, bool &ovf) {
   if (fabsf(x) > 65504.0f) {
@@ -169,11 +132,13 @@ __device__ __forceinline__ Item decode(long long w, const Params &p, int th) {
 }
 
 template <int N, int MT, bool HALO, int PITCH, bool WS = false>
-__global__ void __launch_bounds__(kThreadsD, 1)
+__global__ void __launch_bounds__(kThreads, 1)
     dense_conv_f16_kernel(const __grid_constant__ CUtensorMap in_map, const Params p) {
   using C = Cfg<N, MT, HALO, PITCH, WS>;
   constexpr int TH = kTH * MT;  // output tile height
+  constexpr int H = N / 2;      // accumulator registers of the hi products of one M tile; the cross products follow
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  asm volatile("griddepcontrol.wait;" ::: "memory");  // the input image is the previous layer's output
   const int up2 = p.up * p.up;
   const long long n_total = static_cast<long long>(p.B) * p.tiles_y * p.tiles_x * p.n_ntiles * (p.up > 1 ? up2 : 1);
   if (static_cast<long long>(blockIdx.x) >= n_total) return;
@@ -181,305 +146,179 @@ __global__ void __launch_bounds__(kThreadsD, 1)
   const long long w_first = WS ? (static_cast<long long>(blockIdx.x) * n_total) / gridDim.x : blockIdx.x;
   const long long n_work = WS ? (static_cast<long long>(blockIdx.x + 1) * n_total) / gridDim.x : n_total;
   const long long w_step = WS ? 1 : gridDim.x;
+  const long long n_items = (n_work - w_first + w_step - 1) / w_step;
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  __shared__ __align__(8) unsigned long long s_bar[2 * 3 + 2 * kMaxB + 4 + 2];
-  // activation buffers: full[NA] empty[NA] | weight ring: full[NB] empty[NB] | accumulators: full[2] empty[2] |
-  // weight-stationary image: landed, free
-  constexpr int kAF = 0, kAE = 3, kBF = 6, kBE = 6 + kMaxB, kTF = 6 + 2 * kMaxB, kTE = kTF + 2, kWF = kTE + 2, kWE = kWF + 1;
-  __shared__ uint32_t s_tmem_base;
-  __shared__ float s_scale[2][N], s_shift[2][N];  // per accumulator buffer: the item's N-tile slice
+  __shared__ __align__(8) unsigned long long s_bar[kMaxA + kMaxB + 1];  // activation full[NA] | weight full[NB] | image
+  constexpr int kAF = 0, kBF = kMaxA, kWF = kMaxA + kMaxB;
 
-  const int tid = threadIdx.x, wid = tid >> 5, lane = tid & 31;
-  if (tid == 4 * 32) {
-    for (int s = 0; s < C::NA; ++s) {
-      mbar_init(smem_u32(&s_bar[kAF + s]), 1);
-      mbar_init(smem_u32(&s_bar[kAE + s]), 1);
-    }
-    for (int s = 0; s < (WS ? 0 : C::NB); ++s) {
-      mbar_init(smem_u32(&s_bar[kBF + s]), 1);
-      mbar_init(smem_u32(&s_bar[kBE + s]), 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(smem_u32(&s_bar[kTF + b]), 1);
-      mbar_init(smem_u32(&s_bar[kTE + b]), 4);
-    }
+  const int tid = threadIdx.x, wg = tid >> 7, wtid = tid & 127;
+  if (tid == 0) {
+    for (int s = 0; s < C::NA; ++s) mbar_init(smem_u32(&s_bar[kAF + s]), 1);
+    for (int s = 0; s < (WS ? 0 : C::NB); ++s) mbar_init(smem_u32(&s_bar[kBF + s]), 1);
     mbar_init(smem_u32(&s_bar[kWF]), 1);
-    mbar_init(smem_u32(&s_bar[kWE]), 1);
     fence_mbar_init();
   }
-  if (wid == 4) {
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem_base)),
-                 "r"(static_cast<uint32_t>(C::TMEM_COLS))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem_base;
   const uint32_t a_ring = smem_u32(smem);
   const uint32_t b_ring = a_ring + C::NA * C::A_BYTES;
   const int G = p.Cin / 32;
-  // A-units per item: HALO: one per group (serves all taps); TAP: one per (tap, group)
+  // steps / activation units per item: HALO: one unit per group, 9 taps each; TAP: one unit per (tap, group)
   const int taps_item = p.up > 1 ? 1 : p.taps;
+  const int units_item = HALO ? G : taps_item * G;
+  const int steps_item = units_item * C::SPU;
+  const long long n_units = n_items * units_item, n_steps = n_items * steps_item;
+  auto item_w = [&](long long idx) { return w_first + idx * w_step; };
 
-  if (wid < 4) {
-    // ------------------------------------------------------------------------------------------ epilogue
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    bool ovf = false;
-    int it = 0;
-    for (long long w = w_first; w < n_work; w += w_step, ++it) {
-      const int buf = (C::NBUF == 2) ? (it & 1) : 0;
-      const int use = (C::NBUF == 2) ? (it >> 1) : it;
-      const Item im = decode<WS>(w, p, TH);
-      // this item's per-channel epilogue constants (one thread per channel of the N tile)
-      if (tid < N) {
-        const int ch = im.nt * N + tid;
-        const bool okc = p.grouped ? true : ch < p.cout;
-        s_scale[buf][tid] = (p.scale && okc) ? __ldg(p.scale + ch) : 1.0f;
-        s_shift[buf][tid] = (p.shift && okc) ? __ldg(p.shift + ch) : 0.0f;
+  // thread 0: activation buffer of global unit a / weight blocks of global step q
+  auto issue_a = [&](long long a) {
+    const Item im = decode<WS>(item_w(a / units_item), p, TH);
+    const int ua = static_cast<int>(a % units_item);
+    const int cg0 = p.grouped ? im.nt * G : 0;  // first 32-channel group of this item's input channels
+    const uint32_t slot = static_cast<uint32_t>(a % C::NA), bar = smem_u32(&s_bar[kAF + slot]);
+    mbar_arrive_expect_tx(bar, static_cast<uint32_t>(C::A_ROWS * 128));
+    if (HALO) {
+      tma_tile4d(a_ring + slot * C::A_BYTES, &in_map, (cg0 + ua) * 64, im.tx0 - 1, im.ty0 - 1, im.b, bar);
+    } else {
+      const int t = (p.up > 1 ? im.tap0 : ua / G), g = ua % G;
+      const int dy = p.up > 1 ? 0 : t / p.kw, dx = p.up > 1 ? 0 : t % p.kw;
+      const int x = im.tx0 * p.stride - p.pad + dx, y = im.ty0 * p.stride - p.pad + dy;  // may be negative: zero fill
+      tma_tile4d(a_ring + slot * C::A_BYTES, &in_map, (cg0 + g) * 64, x, y, im.b, bar);
+    }
+  };
+  auto issue_b = [&](long long q) {
+    const Item im = decode<WS>(item_w(q / steps_item), p, TH);
+    const int u = static_cast<int>(q % steps_item);
+    int t, g;
+    if (HALO) {
+      g = u / 9;
+      t = u % 9;
+    } else {
+      t = p.up > 1 ? im.tap0 : u / G;
+      g = u % G;
+    }
+    const uint8_t *w_tile = p.packed_w + static_cast<size_t>(im.nt) * p.taps * (p.Cin / 16) * C::B_BLK;
+    const uint32_t slot = static_cast<uint32_t>(q % C::NB), bar = smem_u32(&s_bar[kBF + slot]);
+    mbar_arrive_expect_tx(bar, static_cast<uint32_t>(C::B_BYTES));
+    bulk_g2s(b_ring + slot * C::B_BYTES, w_tile + (static_cast<size_t>(t) * (p.Cin / 16) + 2 * g) * C::B_BLK,
+             static_cast<uint32_t>(C::B_BYTES), bar);
+  };
+
+  bool ovf = false;
+  long long next_a = 0, next_b = 0;  // thread 0: next unit / step to load
+  int cur_nt = -1;                   // WS: N tile whose weight image is resident
+  uint32_t img = 0;                  // WS: images loaded so far
+  long long q = 0;                   // global step
+  float acc[C::ACC];
+  for (long long idx = 0; idx < n_items; ++idx) {
+    const Item im = decode<WS>(item_w(idx), p, TH);
+#pragma unroll
+    for (int i = 0; i < C::ACC; ++i) acc[i] = 0.f;
+    for (int ua = 0; ua < units_item; ++ua) {
+      for (int t = 0; t < C::SPU; ++t, ++q) {
+        __syncthreads();  // the wgmma of step q - 1 have retired in both warpgroups
+        if (WS && ua == 0 && t == 0 && im.nt != cur_nt) {
+          // first item of a run on this N tile: every step of the previous run has completed, replace the image
+          if (tid == 0) {
+            const uint32_t bar = smem_u32(&s_bar[kWF]);
+            mbar_arrive_expect_tx(bar, static_cast<uint32_t>(p.w_bytes));
+            const uint8_t *w_tile = p.packed_w + static_cast<size_t>(im.nt) * p.w_bytes;
+            for (int off = 0; off < p.w_bytes; off += 16384) {
+              const int bytes = p.w_bytes - off < 16384 ? p.w_bytes - off : 16384;
+              bulk_g2s(b_ring + static_cast<uint32_t>(off), w_tile + off, static_cast<uint32_t>(bytes), bar);
+            }
+          }
+          mbar_wait(smem_u32(&s_bar[kWF]), img & 1u);
+          ++img;
+          cur_nt = im.nt;
+        }
+        if (tid == 0) {
+          for (; next_a < n_units && (next_a - C::NA + 1) * C::SPU <= q; ++next_a) issue_a(next_a);
+          if (!WS)
+            for (; next_b < n_steps && next_b <= q + C::NB - 1; ++next_b) issue_b(next_b);
+        }
+        const long long ga = q / C::SPU;  // global unit of this step
+        const uint32_t sa = static_cast<uint32_t>(ga % C::NA), sb = static_cast<uint32_t>(q % C::NB);
+        mbar_wait(smem_u32(&s_bar[kAF + sa]), static_cast<uint32_t>((ga / C::NA) & 1));
+        if (!WS) mbar_wait(smem_u32(&s_bar[kBF + sb]), static_cast<uint32_t>((q / C::NB) & 1));
+        const uint32_t a_base = a_ring + sa * C::A_BYTES;
+        const uint32_t b_base = WS ? b_ring + static_cast<uint32_t>((t * (p.Cin / 16) + 2 * ua) * C::B_BLK)
+                                   : b_ring + sb * C::B_BYTES;
+        wg_fence();
+#pragma unroll
+        for (int kb = 0; kb < 2; ++kb) {
+          const uint32_t bk = b_base + static_cast<uint32_t>(kb * C::B_BLK);
+          const uint64_t dbh = smem_desc(bk, 2 * N * 16, 128), dbl = smem_desc(bk + N * 16, 2 * N * 16, 128);
+#pragma unroll
+          for (int mt = 0; mt < MT; ++mt) {
+            uint32_t a0, sbo;
+            if (HALO) {  // this warpgroup's 8 image rows of M tile mt, shifted by the tap
+              a0 = a_base + static_cast<uint32_t>(((mt * kTH + wg * 8 + t / 3) * PITCH + t % 3) * 128);
+              sbo = PITCH * 128;
+            } else {
+              a0 = a_base + static_cast<uint32_t>((mt * kM + wg * 64) * 128);
+              sbo = 1024;
+            }
+            const uint32_t ah = a0 + kb * 32, al = a0 + (2 + kb) * 32;
+            const uint32_t bo = p.base_offset_mode ? 1u : 0u;
+            const uint64_t dah = gmma_desc(ah, 16, sbo, 1, bo * ((ah >> 7) & 7u)), dal = gmma_desc(al, 16, sbo, 1, bo * ((al >> 7) & 7u));
+            float *d = acc + mt * N;
+            wg::mma_f16<N>(d, dah, dbh, 1u);      // A_hi x B_hi
+            wg::mma_f16<N>(d + H, dah, dbl, 1u);  // A_hi x B_lo'
+            wg::mma_f16<N>(d + H, dal, dbh, 1u);  // A_lo' x B_hi
+          }
+        }
+        wg_commit();
+        wg_wait<0>();
       }
-      const int g_cnt = p.grouped ? __ldg(p.grp_cnt + im.nt) : 0, g_p0 = p.grouped ? __ldg(p.grp_plane0 + im.nt) : 0;
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      mbar_wait(smem_u32(&s_bar[kTF + buf]), static_cast<uint32_t>(use & 1));
-      tc_fence_after();
-      const int m = tid;  // TMEM lane = pixel of the M tile
-      const int py = m / kTW, px = m % kTW;
-#pragma unroll 1
-      for (int mt = 0; mt < MT; ++mt) {
-        const int iy = im.ty0 + mt * kTH + py, ix = im.tx0 + px;
-        const bool live = iy < p.oH && ix < p.oW;
+    }
+    wg_fence_acc<C::ACC>(acc);
+
+    // ------------------------------------------------------------------------------------------ epilogue
+    const int g_cnt = p.grouped ? __ldg(p.grp_cnt + im.nt) : 0, g_p0 = p.grouped ? __ldg(p.grp_plane0 + im.nt) : 0;
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt) {
+#pragma unroll
+      for (int i = 0; i < H; i += 2) {
+        const int m = wg * 64 + frag_row(i, wtid), c = frag_col(i, wtid);  // pixel of the M tile, column of the N tile
+        const int iy = im.ty0 + mt * kTH + m / kTW, ix = im.tx0 + m % kTW;
+        const int ch = im.nt * N + c;  // output channel
+        if (iy >= p.oH || ix >= p.oW || (p.grouped ? c >= g_cnt : ch >= p.cout)) continue;
         const int Y = iy * p.up + (p.up > 1 ? im.tap0 / p.up : 0), X = ix * p.up + (p.up > 1 ? im.tap0 % p.up : 0);
         const size_t opix = (static_cast<size_t>(im.b) * p.out_H + Y) * p.out_W + X;
-        const uint32_t taddr = tmem_base + (static_cast<uint32_t>(wid * 32) << 16) + static_cast<uint32_t>(buf * C::ACC_COLS + mt * 2 * N);
-#pragma unroll 1
-        for (int c0 = 0; c0 < N; c0 += 16) {
-          uint32_t a[16], x[16];
-          tmem_ld16(taddr + static_cast<uint32_t>(c0), a);
-          tmem_ld16(taddr + static_cast<uint32_t>(N + c0), x);
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-          if (mt == MT - 1 && c0 + 16 >= N) {  // last read of the accumulators: hand the buffer back to the MMA warp
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(smem_u32(&s_bar[kTE + buf]));
-          }
-          const int ch0 = im.nt * N + c0;  // first output channel of this chunk
-          if (live && (p.grouped ? c0 < g_cnt : ch0 < p.cout)) {
-            float v[16];
+        float v[2];
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              float o = fmaf(__uint_as_float(x[j]), kLoInv, __uint_as_float(a[j]));
-              o = fmaf(o, s_scale[buf][c0 + j], s_shift[buf][c0 + j]);
-              if (p.relu) o = fmaxf(o, 0.f);
-              v[j] = o;
-            }
-            if (p.out_h16) {  // channel counts of H16 layers are multiples of 16: whole chunks
-              uint32_t hw[8], lw[8];
+        for (int e = 0; e < 2; ++e) {
+          const bool okc = p.grouped ? true : ch + e < p.cout;
+          const float sc = (p.scale && okc) ? __ldg(p.scale + ch + e) : 1.0f, sh = (p.shift && okc) ? __ldg(p.shift + ch + e) : 0.0f;
+          float o = fmaf(acc[mt * N + H + i + e], kLoInv, acc[mt * N + i + e]);
+          o = fmaf(o, sc, sh);
+          if (p.relu) o = fmaxf(o, 0.f);
+          v[e] = o;
+        }
+        if (p.out_h16) {  // channel counts of H16 layers are multiples of 16: whole pairs
+          __half h0, l0, h1, l1;
+          split_h16(v[0], h0, l0, ovf);
+          split_h16(v[1], h1, l1, ovf);
+          const int oc = p.out_c0 + ch;
+          uint8_t *op = p.out_h16 + opix * (4 * static_cast<size_t>(p.out_C)) + (oc / 32) * 128 + (oc % 32) * 2;
+          *reinterpret_cast<__half2 *>(op) = __halves2half2(h0, h1);
+          *reinterpret_cast<__half2 *>(op + 64) = __halves2half2(l0, l1);
+        }
+        if (p.out_nchw) {
 #pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                __half h0, l0, h1, l1;
-                split_h16(v[2 * j], h0, l0, ovf);
-                split_h16(v[2 * j + 1], h1, l1, ovf);
-                const __half2 hh = __halves2half2(h0, h1), ll = __halves2half2(l0, l1);
-                hw[j] = *reinterpret_cast<const uint32_t *>(&hh);
-                lw[j] = *reinterpret_cast<const uint32_t *>(&ll);
-              }
-              const int ch = p.out_c0 + ch0;
-              uint8_t *op = p.out_h16 + opix * (4 * static_cast<size_t>(p.out_C)) + (ch / 32) * 128 + (ch % 32) * 2;
-              reinterpret_cast<uint4 *>(op)[0] = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-              reinterpret_cast<uint4 *>(op)[1] = make_uint4(hw[4], hw[5], hw[6], hw[7]);
-              reinterpret_cast<uint4 *>(op + 64)[0] = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-              reinterpret_cast<uint4 *>(op + 64)[1] = make_uint4(lw[4], lw[5], lw[6], lw[7]);
-            }
-            if (p.out_nchw) {
-              if (p.grouped) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j)
-                  if (c0 + j < g_cnt)
-                    p.out_nchw[((static_cast<size_t>(im.b) * p.cout + g_p0 + c0 + j) * p.out_H + Y) * p.out_W + X] = v[j];
-              } else {
-#pragma unroll
-                for (int j = 0; j < 16; ++j)
-                  if (ch0 + j < p.cout)
-                    p.out_nchw[((static_cast<size_t>(im.b) * p.cout + ch0 + j) * p.out_H + Y) * p.out_W + X] = v[j];
-              }
+          for (int e = 0; e < 2; ++e) {
+            if (p.grouped) {
+              if (c + e < g_cnt) p.out_nchw[((static_cast<size_t>(im.b) * p.cout + g_p0 + c + e) * p.out_H + Y) * p.out_W + X] = v[e];
+            } else if (ch + e < p.cout) {
+              p.out_nchw[((static_cast<size_t>(im.b) * p.cout + ch + e) * p.out_H + Y) * p.out_W + X] = v[e];
             }
           }
         }
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");  // s_scale / s_shift of this buffer are rewritten two items later
-    }
-    if (ovf && p.status) atomicOr(p.status, 1);
-  } else if (wid == 4) {
-    // ------------------------------------------------------------------------------------------ MMA issuer
-    int sa = 0, sb = 0;
-    uint32_t pa = 0, pb = 0;  // parities to wait for on a_full[sa] / b_full[sb]
-    int it = 0;
-    int cur_nt = -1;
-    uint32_t pw = 0;
-    for (long long w = w_first; w < n_work; w += w_step, ++it) {
-      const int buf = (C::NBUF == 2) ? (it & 1) : 0;
-      const int use = (C::NBUF == 2) ? (it >> 1) : it;
-      mbar_wait(smem_u32(&s_bar[kTE + buf]), static_cast<uint32_t>((use & 1) ^ 1));  // epilogue of the previous use done
-      tc_fence_after();
-      int nt_next = -1;
-      if (WS) {
-        const int nt = decode<WS>(w, p, TH).nt;
-        if (nt != cur_nt) {  // first item of a run on this N tile: its weight image has to have landed
-          mbar_wait(smem_u32(&s_bar[kWF]), pw);
-          pw ^= 1u;
-          tc_fence_after();
-          cur_nt = nt;
-        }
-        nt_next = (w + w_step < n_work) ? decode<WS>(w + w_step, p, TH).nt : -1;
-      }
-      const uint32_t acc = tmem_base + static_cast<uint32_t>(buf * C::ACC_COLS);
-      const int n_a = HALO ? G : taps_item * G;
-      for (int ua = 0; ua < n_a; ++ua) {
-        mbar_wait(smem_u32(&s_bar[kAF + sa]), pa);
-        tc_fence_after();
-        const uint32_t a_base = a_ring + static_cast<uint32_t>(sa * C::A_BYTES);
-        const int n_t = HALO ? 9 : 1;
-        for (int t = 0; t < n_t; ++t) {
-          if (!WS) {
-            mbar_wait(smem_u32(&s_bar[kBF + sb]), pb);
-            tc_fence_after();
-          }
-          const uint32_t b_base = WS ? b_ring + static_cast<uint32_t>((t * (p.Cin / 16) + 2 * ua) * C::B_BLK)
-                                     : b_ring + static_cast<uint32_t>(sb * C::B_BYTES);
-#pragma unroll
-          for (int kb = 0; kb < 2; ++kb) {
-            const uint64_t db = smem_desc(b_base + static_cast<uint32_t>(kb * C::B_BLK), 2 * N * 16, 128);
-#pragma unroll
-            for (int mt = 0; mt < MT; ++mt) {
-              uint32_t a0;
-              uint32_t sbo;
-              if (HALO) {
-                a0 = a_base + static_cast<uint32_t>(((mt * kTH + t / 3) * PITCH + t % 3) * 128);
-                sbo = PITCH * 128;
-              } else {
-                a0 = a_base + static_cast<uint32_t>(mt * kM * 128);
-                sbo = 1024;
-              }
-              const uint32_t first = (ua | t | kb) ? 1u : 0u;
-              mma_f16_elect(acc + mt * 2 * N, desc_sw128_at(a0 + kb * 32, sbo, p.base_offset_mode), db, C::IDESC2, first);         // A_hi x [B_hi | B_lo']
-              mma_f16_elect(acc + mt * 2 * N + N, desc_sw128_at(a0 + (2 + kb) * 32, sbo, p.base_offset_mode), db, C::IDESC1, 1u);  // A_lo' x B_hi
-            }
-          }
-          if (!WS) {
-            commit_elect(smem_u32(&s_bar[kBE + sb]));
-            if (++sb == C::NB) {
-              sb = 0;
-              pb ^= 1u;
-            }
-          }
-        }
-        commit_elect(smem_u32(&s_bar[kAE + sa]));
-        if (ua == n_a - 1) {
-          commit_elect(smem_u32(&s_bar[kTF + buf]));
-          if (WS && nt_next != cur_nt) commit_elect(smem_u32(&s_bar[kWE]));  // last MMAs of this N tile: image may be replaced
-        }
-        if (++sa == C::NA) {
-          sa = 0;
-          pa ^= 1u;
-        }
-      }
-    }
-    tc_fence_before();
-  } else if (wid == 5) {
-    // ------------------------------------------------------------------------------------------ activation TMA (one lane)
-    if (lane == 0) {
-      asm volatile("griddepcontrol.wait;" ::: "memory");  // the input image is the previous layer's output
-      int sa = 0;
-      uint32_t pe = 1;
-      for (long long w = w_first; w < n_work; w += w_step) {
-        const Item im = decode<WS>(w, p, TH);
-        const int cg0 = p.grouped ? im.nt * G : 0;  // first 32-channel group of this item's input channels
-        if (HALO) {
-          for (int g = 0; g < G; ++g) {
-            mbar_wait(smem_u32(&s_bar[kAE + sa]), pe);
-            const uint32_t bar = smem_u32(&s_bar[kAF + sa]);
-            mbar_arrive_expect_tx(bar, static_cast<uint32_t>(C::A_ROWS * 128));
-            tma_tile4d(a_ring + static_cast<uint32_t>(sa * C::A_BYTES), &in_map, (cg0 + g) * 64, im.tx0 - 1, im.ty0 - 1, im.b, bar);
-            if (++sa == C::NA) {
-              sa = 0;
-              pe ^= 1u;
-            }
-          }
-        } else {
-          const int t_begin = p.up > 1 ? im.tap0 : 0, t_end = p.up > 1 ? im.tap0 + 1 : p.taps;
-          for (int t = t_begin; t < t_end; ++t) {
-            const int dy = p.up > 1 ? 0 : t / p.kw, dx = p.up > 1 ? 0 : t % p.kw;
-            const int x = im.tx0 * p.stride - p.pad + dx, y = im.ty0 * p.stride - p.pad + dy;  // may be negative: zero fill
-            for (int g = 0; g < G; ++g) {
-              mbar_wait(smem_u32(&s_bar[kAE + sa]), pe);
-              const uint32_t bar = smem_u32(&s_bar[kAF + sa]);
-              mbar_arrive_expect_tx(bar, static_cast<uint32_t>(C::A_ROWS * 128));
-              tma_tile4d(a_ring + static_cast<uint32_t>(sa * C::A_BYTES), &in_map, (cg0 + g) * 64, x, y, im.b, bar);
-              if (++sa == C::NA) {
-                sa = 0;
-                pe ^= 1u;
-              }
-            }
-          }
-        }
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------------------------------ weight blocks (one lane)
-    if (lane == 0 && WS) {
-      int cur_nt = -1;
-      uint32_t pe = 1;
-      for (long long w = w_first; w < n_work; w += w_step) {
-        const int nt = decode<WS>(w, p, TH).nt;
-        if (nt == cur_nt) continue;
-        cur_nt = nt;
-        mbar_wait(smem_u32(&s_bar[kWE]), pe);  // the MMAs reading the previous image have completed
-        pe ^= 1u;
-        const uint32_t bar = smem_u32(&s_bar[kWF]);
-        mbar_arrive_expect_tx(bar, static_cast<uint32_t>(p.w_bytes));
-        const uint8_t *w_tile = p.packed_w + static_cast<size_t>(nt) * p.w_bytes;
-        for (int off = 0; off < p.w_bytes; off += 16384) {
-          const int bytes = p.w_bytes - off < 16384 ? p.w_bytes - off : 16384;
-          bulk_g2s(b_ring + static_cast<uint32_t>(off), w_tile + off, static_cast<uint32_t>(bytes), bar);
-        }
-      }
-    } else if (lane == 0) {
-      int sb = 0;
-      uint32_t pe = 1;
-      for (long long w = w_first; w < n_work; w += w_step) {
-        const Item im = decode<WS>(w, p, TH);
-        const uint8_t *w_tile = p.packed_w + static_cast<size_t>(im.nt) * p.taps * (p.Cin / 16) * C::B_BLK;
-        // same (A-unit, tap) order as the MMA warp: HALO: group-major, taps inside; TAP: tap-major, groups inside
-        const int t_begin = p.up > 1 ? im.tap0 : 0, t_end = p.up > 1 ? im.tap0 + 1 : p.taps;
-        const int outer = HALO ? G : (t_end - t_begin), inner = HALO ? 9 : G;
-        for (int o = 0; o < outer; ++o)
-          for (int i = 0; i < inner; ++i) {
-            const int t = HALO ? i : t_begin + o, g = HALO ? o : i;
-            mbar_wait(smem_u32(&s_bar[kBE + sb]), pe);
-            const uint32_t bar = smem_u32(&s_bar[kBF + sb]);
-            mbar_arrive_expect_tx(bar, static_cast<uint32_t>(C::B_BYTES));
-            bulk_g2s(b_ring + static_cast<uint32_t>(sb * C::B_BYTES),
-                     w_tile + (static_cast<size_t>(t) * (p.Cin / 16) + 2 * g) * C::B_BLK, static_cast<uint32_t>(C::B_BYTES), bar);
-            if (++sb == C::NB) {
-              sb = 0;
-              pe ^= 1u;
-            }
-          }
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (wid == 4) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"(static_cast<uint32_t>(C::TMEM_COLS))
-                 : "memory");
-  }
+  if (ovf && p.status) atomicOr(p.status, 1);
 }
 
 // fp32 NCHW image -> pixel H16 rows (32 x 32 tile transpose through shared memory)
@@ -558,8 +397,9 @@ int launch(const CUtensorMap &map, const Params &p, cudaStream_t st) {
   P3D_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   const long long work = static_cast<long long>(p.B) * p.tiles_y * p.tiles_x * p.n_ntiles * (p.up > 1 ? p.up * p.up : 1);
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(static_cast<unsigned int>(work < kNumSMs ? work : kNumSMs));
-  cfg.blockDim = dim3(kThreadsD);
+  const long long sms = num_sms();
+  cfg.gridDim = dim3(static_cast<unsigned int>(work < sms ? work : sms));
+  cfg.blockDim = dim3(kThreads);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
   cudaLaunchAttribute attr[1];
@@ -575,14 +415,14 @@ int launch(const CUtensorMap &map, const Params &p, cudaStream_t st) {
 // ---------------------------------------------------------------------------------------------------------------------
 // CenterHead output convs with the 9 taps in the N dimension ("tap-as-N", center_head.py:80-117 SeparateHead finals).
 //
-// A 3x3 conv with <= 3 output channels is 9 * Cin/16 k-steps of N = 16 UMMAs per 128 pixels in the generic kernel above:
-// 144 tiny MMAs per item, bound by the MMA issue latency (190 us for the 36 convs of the C3 head).  Here one item is a
-// 16 x 16-pixel haloed tile (256 rows = 2 M tiles) of one group's Cin channels and ONE GEMM
+// A 3x3 conv with <= 3 output channels is 9 * Cin/16 k-steps of N = 16 MMAs per 128 pixels in the generic kernel above.
+// Here one item is a 16 x 16-pixel haloed tile (256 rows = 2 M tiles) of one group's Cin channels and ONE GEMM
 //     P[pixel][tap * 3 + co] = sum_c  mid[pixel][c] * W[tap][c][co]            (N = 27 -> 32, K = Cin: 4 k-steps for 64)
-// = 16 MMAs; the epilogue parks P in shared memory and every output pixel of the 14 x 14 interior adds its 9 shifted
+// the epilogue parks P in shared memory and every output pixel of the 14 x 14 interior adds its 9 shifted
 // entries  out[y][x][co] = bias + sum_tap P[(y + dy) * 16 + x + dx][tap * 3 + co].  The kernel is then bound by reading
 // the intermediate image once (x 1.31 halo overhead, mostly L2 hits).
-//   warps 0-3 epilogue + tap sums   4 MMA issue   5 activation TMA   6 weight blocks
+//   step = one 32-channel group of an item (activation ring, NA); the item's weights (all groups) are one slot of a
+//   3-deep weight ring; thread 0 loads both ahead across items, warpgroup g computes rows 64g .. 64g+63 of both M tiles.
 namespace out9 {
 constexpr int kHT = 16, kOT = 14;                 // haloed / output tile side
 constexpr int kRows = kHT * kHT;                  // 256 rows of 128 bytes per 32-channel group
@@ -591,8 +431,7 @@ constexpr int kN = 32, kStride = 29;              // GEMM N, fp32 row stride of 
 constexpr int kWBlk = 64 * kN;                    // bytes of one 16-channel weight k-block ([2 chunks][2N rows][8 halfs])
 constexpr int kPBytes = kRows * kStride * 4;
 constexpr int kMaxNA = 5, kNW = 3;
-constexpr uint32_t IDESC2 = (1u << 4) | (static_cast<uint32_t>((2 * kN) >> 3) << 17) | (static_cast<uint32_t>(kM >> 4) << 24);
-constexpr uint32_t IDESC1 = (1u << 4) | (static_cast<uint32_t>(kN >> 3) << 17) | (static_cast<uint32_t>(kM >> 4) << 24);
+constexpr int kAcc = 2 * kN;                      // two M tiles x (hi | cross) x 16 registers
 
 struct Params {
   int B, H, W, G;              // image, 32-channel groups per conv group (Cin / 32)
@@ -604,43 +443,23 @@ struct Params {
   float *out;                  // [B, planes, H, W]
 };
 
-__global__ void __launch_bounds__(kThreadsD, 1) head_out9_kernel(const __grid_constant__ CUtensorMap in_map, const Params p) {
+__global__ void __launch_bounds__(kThreads, 1) head_out9_kernel(const __grid_constant__ CUtensorMap in_map, const Params p) {
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  asm volatile("griddepcontrol.wait;" ::: "memory");
   const long long n_work = static_cast<long long>(p.B) * p.tiles_y * p.tiles_x * p.groups;
   if (static_cast<long long>(blockIdx.x) >= n_work) return;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  __shared__ __align__(8) unsigned long long s_bar[2 * kMaxNA + 2 * kNW + 4];
-  constexpr int kAF = 0, kAE = kMaxNA, kWF = 2 * kMaxNA, kWE = kWF + kNW, kTF = kWE + kNW, kTE = kTF + 2;
-  __shared__ uint32_t s_tmem_base;
-  const int tid = threadIdx.x, wid = tid >> 5, lane = tid & 31;
+  __shared__ __align__(8) unsigned long long s_bar[kMaxNA + kNW];
+  constexpr int kAF = 0, kWF = kMaxNA;
+  const int tid = threadIdx.x, wg = tid >> 7, wtid = tid & 127;
   const int NA = p.NA, G = p.G;
   const uint32_t w_slot = static_cast<uint32_t>(2 * G * kWBlk);
-  if (tid == 4 * 32) {
-    for (int s = 0; s < kMaxNA; ++s) {
-      mbar_init(smem_u32(&s_bar[kAF + s]), 1);
-      mbar_init(smem_u32(&s_bar[kAE + s]), 1);
-    }
-    for (int s = 0; s < kNW; ++s) {
-      mbar_init(smem_u32(&s_bar[kWF + s]), 1);
-      mbar_init(smem_u32(&s_bar[kWE + s]), 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(smem_u32(&s_bar[kTF + b]), 1);
-      mbar_init(smem_u32(&s_bar[kTE + b]), 4);
-    }
+  if (tid == 0) {
+    for (int s = 0; s < NA; ++s) mbar_init(smem_u32(&s_bar[kAF + s]), 1);
+    for (int s = 0; s < kNW; ++s) mbar_init(smem_u32(&s_bar[kWF + s]), 1);
     fence_mbar_init();
   }
-  if (wid == 4) {
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem_base)), "r"(256u)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem_base;
   const uint32_t a_ring = smem_u32(smem);
   const uint32_t w_ring = a_ring + static_cast<uint32_t>(NA * kABytes);
   float *s_p = reinterpret_cast<float *>(smem + static_cast<size_t>(NA) * kABytes + static_cast<size_t>(kNW) * w_slot);
@@ -653,146 +472,93 @@ __global__ void __launch_bounds__(kThreadsD, 1) head_out9_kernel(const __grid_co
     ty0 = static_cast<int>(q % p.tiles_y) * kOT;
     b = static_cast<int>(q / p.tiles_y);
   };
+  const long long n_items = (n_work - blockIdx.x + gridDim.x - 1) / gridDim.x;
+  const long long n_steps = n_items * G;
+  // thread 0: activation tile of global step q (item q / G, group q % G) / weights of item i
+  auto issue_a = [&](long long q) {
+    int g, tx0, ty0, b;
+    decode(blockIdx.x + (q / G) * gridDim.x, g, tx0, ty0, b);
+    const int cg0 = (p.cin0 ? __ldg(p.cin0 + g) : g * G * 32) / 32;
+    const uint32_t slot = static_cast<uint32_t>(q % NA), bar = smem_u32(&s_bar[kAF + slot]);
+    mbar_arrive_expect_tx(bar, static_cast<uint32_t>(kABytes));
+    tma_tile4d(a_ring + slot * kABytes, &in_map, (cg0 + static_cast<int>(q % G)) * 64, tx0 - 1, ty0 - 1, b, bar);
+  };
+  auto issue_w = [&](long long i) {
+    const int g = static_cast<int>((blockIdx.x + i * gridDim.x) % p.groups);
+    const uint32_t slot = static_cast<uint32_t>(i % kNW), bar = smem_u32(&s_bar[kWF + slot]);
+    mbar_arrive_expect_tx(bar, w_slot);
+    bulk_g2s(w_ring + slot * w_slot, p.packed_w + static_cast<size_t>(g) * w_slot, w_slot, bar);
+  };
 
-  if (wid < 4) {
-    // ------------------------------------------------------------------------------------------ epilogue + tap sums
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    int it = 0;
-    for (long long w = blockIdx.x; w < n_work; w += gridDim.x, ++it) {
-      const int buf = it & 1, use = it >> 1;
-      int g, tx0, ty0, b;
-      decode(w, g, tx0, ty0, b);
-      const int cnt = __ldg(p.cnt + g), p0 = __ldg(p.plane0 + g);
-      const float4 bias = __ldg(reinterpret_cast<const float4 *>(p.bias) + g);
-      mbar_wait(smem_u32(&s_bar[kTF + buf]), static_cast<uint32_t>(use & 1));
-      tc_fence_after();
-#pragma unroll 1
-      for (int mt = 0; mt < 2; ++mt) {
-        const uint32_t taddr = tmem_base + (static_cast<uint32_t>(wid * 32) << 16) + static_cast<uint32_t>(buf * 128 + mt * 64);
-        uint32_t a0[16], a1[16], x0[16], x1[16];
-        tmem_ld16(taddr, a0);
-        tmem_ld16(taddr + 16, a1);
-        tmem_ld16(taddr + 32, x0);
-        tmem_ld16(taddr + 48, x1);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (mt == 1) {  // accumulators read: hand the buffer back to the MMA warp
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(smem_u32(&s_bar[kTE + buf]));
-        }
-        float *row = s_p + (mt * 128 + tid) * kStride;
+  long long next_a = 0, next_w = 0, q = 0;
+  float acc[kAcc];
+  for (long long idx = 0; idx < n_items; ++idx) {
+    int g, tx0, ty0, b;
+    decode(blockIdx.x + idx * gridDim.x, g, tx0, ty0, b);
+    const int cnt = __ldg(p.cnt + g), p0 = __ldg(p.plane0 + g);
+    const float4 bias = __ldg(reinterpret_cast<const float4 *>(p.bias) + g);
 #pragma unroll
-        for (int j = 0; j < 16; ++j) row[j] = fmaf(__uint_as_float(x0[j]), kLoInv, __uint_as_float(a0[j]));
-#pragma unroll
-        for (int j = 0; j < 11; ++j) row[16 + j] = fmaf(__uint_as_float(x1[j]), kLoInv, __uint_as_float(a1[j]));
+    for (int i = 0; i < kAcc; ++i) acc[i] = 0.f;
+    const uint32_t ws = static_cast<uint32_t>(idx % kNW);
+    for (int k = 0; k < G; ++k, ++q) {
+      __syncthreads();  // the wgmma of step q - 1 have retired in both warpgroups
+      if (tid == 0) {
+        for (; next_a < n_steps && next_a <= q + NA - 1; ++next_a) issue_a(next_a);
+        for (; next_w < n_items && (next_w - kNW + 1) * G <= q; ++next_w) issue_w(next_w);
       }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      for (int o = tid; o < kOT * kOT; o += 128) {
-        const int oy = o / kOT, ox = o - oy * kOT;
-        const int Y = ty0 + oy, X = tx0 + ox;
-        if (Y < p.H && X < p.W) {
-          float s0 = bias.x, s1 = bias.y, s2 = bias.z;
+      if (k == 0) mbar_wait(smem_u32(&s_bar[kWF + ws]), static_cast<uint32_t>((idx / kNW) & 1));
+      const uint32_t sa = static_cast<uint32_t>(q % NA);
+      mbar_wait(smem_u32(&s_bar[kAF + sa]), static_cast<uint32_t>((q / NA) & 1));
+      const uint32_t a_base = a_ring + sa * kABytes;
+      const uint32_t w_base = w_ring + ws * w_slot;
+      wg_fence();
 #pragma unroll
-          for (int t = 0; t < 9; ++t) {
-            const float *e = s_p + ((oy + t / 3) * kHT + ox + t % 3) * kStride + t * 3;
-            s0 += e[0];
-            s1 += e[1];
-            s2 += e[2];
-          }
-          float *op = p.out + ((static_cast<size_t>(b) * p.planes + p0) * p.H + Y) * p.W + X;
-          const size_t plane = static_cast<size_t>(p.H) * p.W;
-          op[0] = s0;
-          if (cnt > 1) op[plane] = s1;
-          if (cnt > 2) op[2 * plane] = s2;
+      for (int kb = 0; kb < 2; ++kb) {
+        const uint32_t bk = w_base + static_cast<uint32_t>((k * 2 + kb) * kWBlk);
+        const uint64_t dbh = smem_desc(bk, 2 * kN * 16, 128), dbl = smem_desc(bk + kN * 16, 2 * kN * 16, 128);
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt) {
+          const uint32_t a0 = a_base + static_cast<uint32_t>((mt * kM + wg * 64) * 128);
+          const uint64_t dah = desc_sw128(a0 + kb * 32), dal = desc_sw128(a0 + (2 + kb) * 32);
+          float *d = acc + mt * kN;
+          wg::mma_f16<kN>(d, dah, dbh, 1u);
+          wg::mma_f16<kN>(d + kN / 2, dah, dbl, 1u);
+          wg::mma_f16<kN>(d + kN / 2, dal, dbh, 1u);
         }
       }
-      asm volatile("bar.sync 1, 128;" ::: "memory");  // P is rewritten by the next item
+      wg_commit();
+      wg_wait<0>();
     }
-  } else if (wid == 4) {
-    // ------------------------------------------------------------------------------------------ MMA issuer
-    int sa = 0, sw = 0;
-    uint32_t pa = 0, pw = 0;
-    int it = 0;
-    for (long long w = blockIdx.x; w < n_work; w += gridDim.x, ++it) {
-      const int buf = it & 1, use = it >> 1;
-      mbar_wait(smem_u32(&s_bar[kTE + buf]), static_cast<uint32_t>((use & 1) ^ 1));
-      mbar_wait(smem_u32(&s_bar[kWF + sw]), pw);
-      tc_fence_after();
-      const uint32_t acc = tmem_base + static_cast<uint32_t>(buf * 128);
-      const uint32_t w_base = w_ring + static_cast<uint32_t>(sw) * w_slot;
-      for (int g = 0; g < G; ++g) {
-        mbar_wait(smem_u32(&s_bar[kAF + sa]), pa);
-        tc_fence_after();
-        const uint32_t a_base = a_ring + static_cast<uint32_t>(sa * kABytes);
+    wg_fence_acc<kAcc>(acc);
+    // P[row][col] = hi + cross * 2^-11 for the 27 used columns
 #pragma unroll
-        for (int kb = 0; kb < 2; ++kb) {
-          const uint64_t db = smem_desc(w_base + static_cast<uint32_t>((g * 2 + kb) * kWBlk), 2 * kN * 16, 128);
+    for (int mt = 0; mt < 2; ++mt) {
 #pragma unroll
-          for (int mt = 0; mt < 2; ++mt) {
-            const uint32_t a0 = a_base + static_cast<uint32_t>(mt * kM * 128);
-            mma_f16_elect(acc + mt * 64, desc_sw128_at(a0 + kb * 32, 1024, 0), db, IDESC2, (g | kb) ? 1u : 0u);
-            mma_f16_elect(acc + mt * 64 + kN, desc_sw128_at(a0 + (2 + kb) * 32, 1024, 0), db, IDESC1, 1u);
-          }
-        }
-        commit_elect(smem_u32(&s_bar[kAE + sa]));
-        if (++sa == NA) {
-          sa = 0;
-          pa ^= 1u;
-        }
-      }
-      commit_elect(smem_u32(&s_bar[kWE + sw]));
-      commit_elect(smem_u32(&s_bar[kTF + buf]));
-      if (++sw == kNW) {
-        sw = 0;
-        pw ^= 1u;
+      for (int i = 0; i < kN / 2; ++i) {
+        const int r = mt * kM + wg * 64 + frag_row(i, wtid), c = frag_col(i, wtid);
+        if (c < 27) s_p[r * kStride + c] = fmaf(acc[mt * kN + kN / 2 + i], kLoInv, acc[mt * kN + i]);
       }
     }
-    tc_fence_before();
-  } else if (wid == 5) {
-    // ------------------------------------------------------------------------------------------ activation TMA (one lane)
-    if (lane == 0) {
-      asm volatile("griddepcontrol.wait;" ::: "memory");
-      int sa = 0;
-      uint32_t pe = 1;
-      for (long long w = blockIdx.x; w < n_work; w += gridDim.x) {
-        int g, tx0, ty0, b;
-        decode(w, g, tx0, ty0, b);
-        const int cg0 = (p.cin0 ? __ldg(p.cin0 + g) : g * G * 32) / 32;
-        for (int k = 0; k < G; ++k) {
-          mbar_wait(smem_u32(&s_bar[kAE + sa]), pe);
-          const uint32_t bar = smem_u32(&s_bar[kAF + sa]);
-          mbar_arrive_expect_tx(bar, static_cast<uint32_t>(kABytes));
-          tma_tile4d(a_ring + static_cast<uint32_t>(sa * kABytes), &in_map, (cg0 + k) * 64, tx0 - 1, ty0 - 1, b, bar);
-          if (++sa == NA) {
-            sa = 0;
-            pe ^= 1u;
-          }
+    __syncthreads();
+    for (int o = tid; o < kOT * kOT; o += kThreads) {
+      const int oy = o / kOT, ox = o - oy * kOT;
+      const int Y = ty0 + oy, X = tx0 + ox;
+      if (Y < p.H && X < p.W) {
+        float s0 = bias.x, s1 = bias.y, s2 = bias.z;
+#pragma unroll
+        for (int t = 0; t < 9; ++t) {
+          const float *e = s_p + ((oy + t / 3) * kHT + ox + t % 3) * kStride + t * 3;
+          s0 += e[0];
+          s1 += e[1];
+          s2 += e[2];
         }
+        float *op = p.out + ((static_cast<size_t>(b) * p.planes + p0) * p.H + Y) * p.W + X;
+        const size_t plane = static_cast<size_t>(p.H) * p.W;
+        op[0] = s0;
+        if (cnt > 1) op[plane] = s1;
+        if (cnt > 2) op[2 * plane] = s2;
       }
     }
-  } else {
-    // ------------------------------------------------------------------------------------------ weights (one lane)
-    if (lane == 0) {
-      int sw = 0;
-      uint32_t pe = 1;
-      for (long long w = blockIdx.x; w < n_work; w += gridDim.x) {
-        const int g = static_cast<int>(w % p.groups);
-        mbar_wait(smem_u32(&s_bar[kWE + sw]), pe);
-        const uint32_t bar = smem_u32(&s_bar[kWF + sw]);
-        mbar_arrive_expect_tx(bar, w_slot);
-        bulk_g2s(w_ring + static_cast<uint32_t>(sw) * w_slot, p.packed_w + static_cast<size_t>(g) * w_slot, w_slot, bar);
-        if (++sw == kNW) {
-          sw = 0;
-          pe ^= 1u;
-        }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (wid == 4) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256u) : "memory");
   }
 }
 }  // namespace out9
@@ -876,8 +642,8 @@ static int dense_conv_f16(const void *in_h16, int B, int H, int W, int Cin, cons
   static const int env_mode = getenv("P3D_DENSE_MODE") ? atoi(getenv("P3D_DENSE_MODE")) : -1;  // tuning hooks
   static const int env_mt = getenv("P3D_DENSE_MT") ? atoi(getenv("P3D_DENSE_MT")) : -1;
   static const int env_pitch = getenv("P3D_DENSE_PITCH") ? atoi(getenv("P3D_DENSE_PITCH")) : 10;
-  // measured on the B200 (profiles/r02_dense_halo_probe.md): shifted tiles read correctly with base_offset = 0 (the swizzle
-  // is a function of the absolute shared-memory address) and wrongly with base_offset = address bits 7-9
+  // shifted tiles read correctly with base_offset = 0: the swizzle is a function of the absolute shared-memory address
+  // (tests/test_gpu_dense.py); P3D_DENSE_BO=1 sets it to the address bits 7-9 instead
   static const int env_bo = getenv("P3D_DENSE_BO") ? atoi(getenv("P3D_DENSE_BO")) : 0;
   p.base_offset_mode = env_bo;
   const int pitch = env_pitch == 16 ? 16 : 10;
@@ -889,16 +655,14 @@ static int dense_conv_f16(const void *in_h16, int B, int H, int W, int Cin, cons
   if (mt != 1 && mt != 2) {
     const long long tx = (p.oW + dcf::kTW - 1) / dcf::kTW, ty2 = (p.oH + 2 * dcf::kTH - 1) / (2 * dcf::kTH);
     const long long items2 = static_cast<long long>(B) * tx * ty2 * p.n_ntiles * (up > 1 ? up * up : 1);
-    // measured (profiles/r02_dense_bench.jsonl): two M tiles pay off for the narrow N = 64 layers (weights are a small
-    // share, the second tile amortises the per-item prologue); N = 128 is faster with one tile and double-buffered
-    // accumulators (the epilogue overlaps the next item)
-    mt = (n_tile <= 64 && items2 >= (kNumSMs * 9) / 10) ? 2 : 1;
+    // two M tiles for the narrow N = 64 layers (the second tile halves the weight traffic per flop and amortises the
+    // per-item prologue) when that still leaves every SM an item; N = 128 keeps one (register budget)
+    mt = (n_tile <= 64 && items2 >= (num_sms() * 9) / 10) ? 2 : 1;
   }
   // weight-stationary variant: haloed 3x3, N tile 64, the N tile's weight image + 3 activation tiles fit in shared memory,
   // and every CTA has enough pixel tiles per weight image to amortise loading it (mode 2 forces it, P3D_DENSE_WS=0 disables)
-  // Measured on the CenterHead's 64 -> 2304 layer (profiles/r02_dense_ws.md): 248 us against 236 us for the streaming
-  // N = 128 kernel - the layer is bound by the shared-memory reads of the MMA operands (N = 64 needs 128-192 B/clk), not by
-  // the weight ingest, so the variant is OFF unless asked for (mode 2 or P3D_DENSE_WS=1).
+  // The variant is OFF unless asked for (mode 2 or P3D_DENSE_WS=1): it was not faster than the streaming N = 128 kernel on
+  // the CenterHead's 64 -> 2304 layer.
   static const int env_ws = getenv("P3D_DENSE_WS") ? atoi(getenv("P3D_DENSE_WS")) : 0;
   p.w_bytes = p.taps * (Cin / 16) * 64 * n_tile;
   bool ws = false;
@@ -906,10 +670,10 @@ static int dense_conv_f16(const void *in_h16, int B, int H, int W, int Cin, cons
     const size_t need = 3 * static_cast<size_t>(dcf::Cfg<64, 1, true, 10, true>::A_BYTES) + p.w_bytes + 1024;
     const long long pix = static_cast<long long>(B) * ((p.oW + dcf::kTW - 1) / dcf::kTW) * ((p.oH + dcf::kTH - 1) / dcf::kTH);
     const long long items = pix * p.n_ntiles;
-    ws = need <= static_cast<size_t>(227 - 6) * 1024 && (mode == 2 || items >= 8ll * kNumSMs);
+    ws = need <= static_cast<size_t>(227 - 6) * 1024 && (mode == 2 || items >= 8ll * num_sms());
   }
   if (mode == 2 && !ws) return P3D_ERR_UNSUPPORTED;
-  if (ws) mt = 1;
+  if (ws || n_tile > 64) mt = 1;  // two M tiles of a 128-wide N tile would need 256 accumulator registers per thread
   p.tiles_x = (p.oW + dcf::kTW - 1) / dcf::kTW;
   p.tiles_y = (p.oH + dcf::kTH * mt - 1) / (dcf::kTH * mt);
   CUtensorMap map;
@@ -929,7 +693,6 @@ static int dense_conv_f16(const void *in_h16, int B, int H, int W, int Cin, cons
   P3D_DCF(64, 1)
   P3D_DCF(64, 2)
   P3D_DCF(128, 1)
-  P3D_DCF(128, 2)
 #undef P3D_DCF
   return P3D_ERR_UNSUPPORTED;
 }
@@ -995,8 +758,9 @@ extern "C" int p3d_head_out_conv_f16(const void *in_h16, int B, int H, int W, in
   P3D_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   const long long work = static_cast<long long>(B) * p.tiles_y * p.tiles_x * groups;
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(static_cast<unsigned int>(work < kNumSMs ? work : kNumSMs));
-  cfg.blockDim = dim3(dcf::kThreadsD);
+  const long long sms = num_sms();
+  cfg.gridDim = dim3(static_cast<unsigned int>(work < sms ? work : sms));
+  cfg.blockDim = dim3(tc::kThreads);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = static_cast<cudaStream_t>(stream);
   cudaLaunchAttribute attr[1];

@@ -1,19 +1,20 @@
-// Dense 2-D convolution on tcgen05 for the RPN / neck / CenterHead row (SURVEY.md §8f-1; reference:
+// Dense 2-D convolution on wgmma (tf32) for the RPN / neck / CenterHead row (SURVEY.md §8f-1; reference:
 // backbones/second_backbone.py:72-120, necks/second_fpn.py:99-160, detection/centerpoint/center_head.py:43-220).
-// Parity-green on a B200 (tests/test_gpu_dense.py) at the end of round 1; performance not measured yet, not on the
-// default bench path.
+// Kept for models whose activations leave fp16's range; the default dense path is dense_conv_f16.cu.
 //
 // The image is kept as "pixel split rows" [B*H*W][2][C] (NHWC with the tf32 hi half of all channels, then the lo half —
 // the row format of the sparse-conv layers with row = pixel), so a 3x3 tap of 32 input channels for a 16 x 8 pixel
 // tile is one 4-D TMA box {32 ch, 16 x, 8 y, 1 b} at the shifted coordinate: zero padding is the tensor map's
 // out-of-bounds fill, a stride-2 conv is the map's element stride, and the box lands in shared memory as the
-// SWIZZLE_128B K-major operand tile (128 rows x 128 B) that the sparse kernel builds with 64 cp.async per thread.
-// Everything after the load is the sparse kernel's pipeline: 3xTF32 with acc[0,2N) += A_hi x [B_hi | B_lo],
-// acc[2N,3N) += A_lo x B_hi in TMEM, weights of the use by cp.async.bulk, BN/bias/ReLU epilogue writing split rows
-// (at a column offset: channel concat for free) or fp32 NCHW planes (the head outputs centerpoint_postprocess reads).
+// SWIZZLE_128B K-major operand tile (128 rows x 128 B).  3xTF32: A_hi x B_hi into one register accumulator,
+// A_lo x B_hi + A_hi x B_lo into a second (warpgroup g: rows 64g .. 64g+63 of the tile), weights of the use by cp.async.bulk,
+// BN/bias/ReLU epilogue writing split rows (at a column offset: channel concat for free) or fp32 NCHW planes (the head
+// outputs centerpoint_postprocess reads).
 //
 //   work item   (batch, 16 x 8 output tile, N tile of the output channels[, tap of a k = s transposed conv])
-//   warps 0-3   epilogue        warp 4   MMA issue        warp 5   TMA (rows + weights), one lane
+//   step        one (tap, 32-channel group) of an item: image tile (hi, lo) + weight slice in one ring slot.  Thread 0
+//               keeps the ring STAGES - 1 steps ahead across work items (TMA, mbarrier complete_tx); all 256 threads
+//               issue the wgmma of their warpgroup and run its epilogue.
 #include <cuda.h>
 
 #include "p3d_b200.h"
@@ -24,7 +25,7 @@ namespace dc {
 
 using namespace tc;
 
-constexpr int kTW = 16, kTH = 8;  // output tile: 16 x 8 pixels = the 128 rows of one UMMA
+constexpr int kTW = 16, kTH = 8;  // output tile: 16 x 8 pixels = the 128 rows of one CTA tile
 static_assert(kTW * kTH == kM, "tile must have 128 pixels");
 
 struct Params {
@@ -50,47 +51,38 @@ struct Cfg {
   static constexpr int BUDGET = (N <= 64) ? 100 * 1024 : 192 * 1024;
   static constexpr int S_RAW = BUDGET / STAGE;
   static constexpr int STAGES = S_RAW > 8 ? 8 : (S_RAW < 2 ? 2 : S_RAW);
-  static constexpr int TMEM_COLS = (3 * N <= 64) ? 64 : (3 * N <= 128) ? 128 : (3 * N <= 256) ? 256 : 512;
-  static constexpr uint32_t IDESC2 = (1u << 4) | (2u << 7) | (2u << 10) | (static_cast<uint32_t>((2 * N) >> 3) << 17) |
-                                     (static_cast<uint32_t>(kM >> 4) << 24);
-  static constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | (static_cast<uint32_t>(N >> 3) << 17) |
-                                    (static_cast<uint32_t>(kM >> 4) << 24);
+  static constexpr int ACC = N / 2;
   static_assert(N % 16 == 0 && N >= 16 && N <= 128, "N tile: 16 .. 128 in steps of 16");
-  static_assert(MIN_CTAS * TMEM_COLS <= 512, "TMEM over-subscribed");
   static_assert(STAGE % 1024 == 0, "SWIZZLE_128B tiles need 1024-byte alignment");
 };
 
-__device__ __forceinline__ uint64_t desc_sw128(uint32_t addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((addr & 0x3ffffu) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= 1ull << 46;
-  d |= 2ull << 61;
-  return d;
-}
-__device__ __forceinline__ void mma_elect(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p, e;\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "@e tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void commit_elect(uint32_t bar) {
-  asm volatile(
-      "{\n\t.reg .pred e;\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(bar)
-      : "memory");
-}
 __device__ __forceinline__ void tma_tile4d(uint32_t dst, const CUtensorMap *map, int c, int x, int y, int b, uint32_t bar) {
   asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cta.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];" ::
+      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];" ::
           "r"(dst),
       "l"(reinterpret_cast<uint64_t>(map)), "r"(c), "r"(x), "r"(y), "r"(b), "r"(bar)
       : "memory");
+}
+
+struct Item {
+  int nt, tap0, tx0, ty0, b;
+};
+// N tile fastest (neighbouring CTAs share the image tile in L2), then tap (transposed conv), x, y, batch
+__device__ __forceinline__ Item decode(long long w, const Params &p) {
+  Item it;
+  long long q = w;
+  it.nt = static_cast<int>(q % p.n_ntiles);
+  q /= p.n_ntiles;
+  it.tap0 = 0;
+  if (p.up > 1) {
+    it.tap0 = static_cast<int>(q % (p.up * p.up));
+    q /= p.up * p.up;
+  }
+  it.tx0 = static_cast<int>(q % p.tiles_x) * kTW;
+  q /= p.tiles_x;
+  it.ty0 = static_cast<int>(q % p.tiles_y) * kTH;
+  it.b = static_cast<int>(q / p.tiles_y);
+  return it;
 }
 
 template <int N>
@@ -99,176 +91,109 @@ __global__ void __launch_bounds__(kThreads, Cfg<N>::MIN_CTAS)
                       const float *__restrict__ scale, const float *__restrict__ shift, float *__restrict__ out_split,
                       float *__restrict__ out_nchw) {
   using C = Cfg<N>;
+  constexpr int S = C::STAGES;
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  asm volatile("griddepcontrol.wait;" ::: "memory");  // the input image is the previous layer's output
   const int up2 = p.up * p.up;
   const long long n_work = static_cast<long long>(p.B) * p.tiles_y * p.tiles_x * p.n_ntiles * (p.up > 1 ? up2 : 1);
   if (static_cast<long long>(blockIdx.x) >= n_work) return;
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  __shared__ __align__(8) unsigned long long s_bar[8 + 8 + 1];  // full[8] empty[8] tmem_full
-  constexpr int kF = 0, kE = 8, kTF = 16;
-  __shared__ uint32_t s_tmem_base;
+  __shared__ __align__(8) unsigned long long s_full[8];
 
-  const int tid = threadIdx.x, wid = tid >> 5, lane = tid & 31;
-  if (tid == 128) {
-    for (int s = 0; s < C::STAGES; ++s) {
-      mbar_init(smem_u32(&s_bar[kF + s]), 1);  // the TMA lane's expect_tx arrival (rows + weights)
-      mbar_init(smem_u32(&s_bar[kE + s]), 1);  // tcgen05.commit
-    }
-    mbar_init(smem_u32(&s_bar[kTF]), 1);
+  const int tid = threadIdx.x, wg = tid >> 7, wtid = tid & 127;
+  if (tid == 0) {
+    for (int s = 0; s < S; ++s) mbar_init(smem_u32(&s_full[s]), 1);  // the TMA lane's expect_tx arrival (rows + weights)
     fence_mbar_init();
   }
-  if (wid == 4) {
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem_base)),
-                 "r"(static_cast<uint32_t>(C::TMEM_COLS))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem_base;
   const uint32_t ring = smem_u32(smem);
-  asm volatile("griddepcontrol.wait;" ::: "memory");  // the input image is the previous layer's output
-
   const int G = p.Cin / C::KC;
-  const int n_uses = (p.up > 1 ? 1 : p.taps) * G;
-  uint32_t ph = (wid == 4) ? 0u : 0xffffffffu;  // expected parity per stage (bit s), as in the sparse kernel
-  int item_it = 0;
-  for (long long w = blockIdx.x; w < n_work; w += gridDim.x, ++item_it) {
-    // decode: N tile fastest (neighbouring CTAs share the image tile in L2), then tap (transposed conv), x, y, batch
-    long long q = w;
-    const int nt = static_cast<int>(q % p.n_ntiles);
-    q /= p.n_ntiles;
-    int tap0 = 0;
-    if (p.up > 1) {
-      tap0 = static_cast<int>(q % up2);
-      q /= up2;
-    }
-    const int tx0 = static_cast<int>(q % p.tiles_x) * kTW;
-    q /= p.tiles_x;
-    const int ty0 = static_cast<int>(q % p.tiles_y) * kTH;
-    const int b = static_cast<int>(q / p.tiles_y);
-    const float *w_tile = packed_w + static_cast<size_t>(nt) * p.taps * p.Cin * (2 * N);
+  const int n_uses = (p.up > 1 ? 1 : p.taps) * G;  // steps per item
+  const long long n_items = (n_work - blockIdx.x + gridDim.x - 1) / gridDim.x;
+  const long long n_steps = n_items * n_uses;
 
-    if (wid < 4) {
-      // ---------------------------------------------------------------- epilogue
-      mbar_wait(smem_u32(&s_bar[kTF]), static_cast<uint32_t>(item_it & 1));
-      tc_fence_after();
-      const int m = tid;  // tile pixel of this thread = TMEM lane
-      const int iy = ty0 + m / kTW, ix = tx0 + m % kTW;
-      const bool live = iy < p.oH && ix < p.oW;
-      const int Y = iy * p.up + (p.up > 1 ? tap0 / p.up : 0), X = ix * p.up + (p.up > 1 ? tap0 % p.up : 0);
-      const size_t orow = (static_cast<size_t>(b) * p.out_H + Y) * p.out_W + X;
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(wid * 32) << 16);
-#pragma unroll 1
-      for (int c0 = 0; c0 < N; c0 += 16) {
-        uint32_t a[16];
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
-            "%15}, [%16];"
-            : "=r"(a[0]), "=r"(a[1]), "=r"(a[2]), "=r"(a[3]), "=r"(a[4]), "=r"(a[5]), "=r"(a[6]), "=r"(a[7]), "=r"(a[8]),
-              "=r"(a[9]), "=r"(a[10]), "=r"(a[11]), "=r"(a[12]), "=r"(a[13]), "=r"(a[14]), "=r"(a[15])
-            : "r"(taddr + static_cast<uint32_t>(c0)));
+  // thread 0: loads of global step q (item q / n_uses of this CTA) into slot q % S
+  auto issue = [&](long long q) {
+    const Item im = decode(blockIdx.x + (q / n_uses) * gridDim.x, p);
+    const int u = static_cast<int>(q % n_uses);
+    const int t = (p.up > 1 ? im.tap0 : u / G), g = u % G;
+    const int dy = p.up > 1 ? 0 : t / p.kw, dx = p.up > 1 ? 0 : t % p.kw;
+    const int x = im.tx0 * p.stride - p.pad + dx, y = im.ty0 * p.stride - p.pad + dy;  // may be negative: zero fill
+    const uint32_t slot = static_cast<uint32_t>(q % S);
+    const uint32_t st = ring + slot * C::STAGE, bar = smem_u32(&s_full[slot]);
+    const float *w_tile = packed_w + static_cast<size_t>(im.nt) * p.taps * p.Cin * (2 * N);
+    mbar_arrive_expect_tx(bar, static_cast<uint32_t>(C::STAGE));
+    tma_tile4d(st, &in_map, g * C::KC, x, y, im.b, bar);                       // hi half of the 32 channels
+    tma_tile4d(st + C::A_TILE, &in_map, p.Cin + g * C::KC, x, y, im.b, bar);   // lo half
+    bulk_g2s(st + C::A_STAGE, w_tile + (static_cast<size_t>(t) * p.Cin + g * C::KC) * (2 * N),
+             static_cast<uint32_t>(C::B_STAGE), bar);
+  };
+  long long next = 0;  // thread 0: next step to load
+  float acc[C::ACC], accx[C::ACC];  // hi x hi | cross terms
+  long long q = 0;
+  for (long long w = blockIdx.x; w < n_work; w += gridDim.x) {
+    const Item im = decode(w, p);
 #pragma unroll
-        for (int acc = 1; acc < 3; ++acc) {
-          uint32_t t[16];
-          asm volatile(
-              "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
-              "%15}, [%16];"
-              : "=r"(t[0]), "=r"(t[1]), "=r"(t[2]), "=r"(t[3]), "=r"(t[4]), "=r"(t[5]), "=r"(t[6]), "=r"(t[7]),
-                "=r"(t[8]), "=r"(t[9]), "=r"(t[10]), "=r"(t[11]), "=r"(t[12]), "=r"(t[13]), "=r"(t[14]), "=r"(t[15])
-              : "r"(taddr + static_cast<uint32_t>(acc * N + c0)));
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+    for (int i = 0; i < C::ACC; ++i) acc[i] = accx[i] = 0.f;
+    for (int u = 0; u < n_uses; ++u, ++q) {
+      __syncthreads();  // the wgmma of step q - 1 have retired in both warpgroups: its slot is free
+      if (tid == 0)
+        for (; next < n_steps && next <= q + S - 1; ++next) issue(next);
+      const uint32_t slot = static_cast<uint32_t>(q % S);
+      mbar_wait(smem_u32(&s_full[slot]), static_cast<uint32_t>((q / S) & 1));
+      const uint32_t a_hi = ring + slot * C::STAGE + static_cast<uint32_t>(wg * 64 * 128), a_lo = a_hi + C::A_TILE;
+      const uint32_t b_hi = ring + slot * C::STAGE + C::A_STAGE, b_lo = b_hi + N * 16;  // rows 0..N-1 = hi, N..2N-1 = lo
+      wg_fence();
 #pragma unroll
-          for (int j = 0; j < 16; ++j) a[j] = __float_as_uint(__uint_as_float(a[j]) + __uint_as_float(t[j]));
-        }
-        const int ch0 = nt * N + c0;  // first output channel of this chunk
-        if (live && ch0 < p.cout) {
-          float o[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            float v = __uint_as_float(a[j]);
-            if (ch0 + j < p.cout) {
-              if (scale) v = v * __ldg(scale + ch0 + j);
-              if (shift) v = v + __ldg(shift + ch0 + j);
-            }
-            if (p.relu) v = fmaxf(v, 0.f);
-            o[j] = v;
-          }
-          if (out_split) {  // channel counts of split-row layers are multiples of 16: whole chunks
-            float h[16], l[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) split_tf32(o[j], h[j], l[j]);
-            float *oh = out_split + orow * (2 * static_cast<size_t>(p.out_C)) + p.out_c0 + ch0;
-#pragma unroll
-            for (int j = 0; j < 16; j += 4) {
-              *reinterpret_cast<float4 *>(oh + j) = make_float4(h[j], h[j + 1], h[j + 2], h[j + 3]);
-              *reinterpret_cast<float4 *>(oh + p.out_C + j) = make_float4(l[j], l[j + 1], l[j + 2], l[j + 3]);
-            }
-          }
-          if (out_nchw) {  // fp32 planes [B, cout, out_H, out_W]: consecutive threads = consecutive x
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-              if (ch0 + j < p.cout)
-                out_nchw[((static_cast<size_t>(b) * p.cout + ch0 + j) * p.out_H + Y) * p.out_W + X] = o[j];
-          }
-        }
+      for (int j = 0; j < C::KC / 8; ++j) {
+        const uint32_t bo = static_cast<uint32_t>(2 * j) * (2 * N * 16);
+        const uint64_t dah = desc_sw128(a_hi + j * 32), dal = desc_sw128(a_lo + j * 32);
+        const uint64_t dbh = smem_desc(b_hi + bo, 2 * N * 16, 128), dbl = smem_desc(b_lo + bo, 2 * N * 16, 128);
+        wg::mma_tf32<N>(accx, dal, dbh, 1u);
+        wg::mma_tf32<N>(accx, dah, dbl, 1u);
+        wg::mma_tf32<N>(acc, dah, dbh, 1u);
       }
-      tc_fence_before();
-    } else if (wid == 4) {
-      // ---------------------------------------------------------------- MMA issuer (whole warp runs the stream)
-      int s = 0;
-      for (int u = 0; u < n_uses; ++u) {
-        mbar_wait(smem_u32(&s_bar[kF + s]), (ph >> s) & 1u);
-        ph ^= 1u << s;
-        tc_fence_after();
-        const uint32_t a_hi = ring + static_cast<uint32_t>(s * C::STAGE), a_lo = a_hi + C::A_TILE;
-        const uint32_t b_all = a_hi + C::A_STAGE;
+      wg_commit();
+      wg_wait<0>();
+    }
+    wg_fence_acc<C::ACC>(acc);
+    wg_fence_acc<C::ACC>(accx);
+
+    // ---------------------------------------------------------------- epilogue (accumulator fragment)
 #pragma unroll
-        for (int j = 0; j < C::KC / 8; ++j) {
-          const uint32_t bo = static_cast<uint32_t>(2 * j) * (2 * N * 16);
-          const uint64_t db = smem_desc(b_all + bo, 2 * N * 16, 128);  // rows 0..N-1 = hi, N..2N-1 = lo
-          const uint32_t first = (u | j) ? 1u : 0u;
-          mma_elect(tmem_base, desc_sw128(a_hi + j * 32), db, C::IDESC2, first);          // A_hi x [B_hi | B_lo]
-          mma_elect(tmem_base + 2 * N, desc_sw128(a_lo + j * 32), db, C::IDESC, first);   // A_lo x B_hi
+    for (int i = 0; i < C::ACC; i += 2) {
+      const int m = wg * 64 + frag_row(i, wtid), c = frag_col(i, wtid);  // tile pixel, N-tile column
+      const int iy = im.ty0 + m / kTW, ix = im.tx0 + m % kTW;
+      const int ch = im.nt * N + c;  // output channel
+      if (iy >= p.oH || ix >= p.oW || ch >= p.cout) continue;
+      const int Y = iy * p.up + (p.up > 1 ? im.tap0 / p.up : 0), X = ix * p.up + (p.up > 1 ? im.tap0 % p.up : 0);
+      const size_t orow = (static_cast<size_t>(im.b) * p.out_H + Y) * p.out_W + X;
+      float o[2];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        float v = accx[i + e] + acc[i + e];
+        if (ch + e < p.cout) {
+          if (scale) v = v * __ldg(scale + ch + e);
+          if (shift) v = v + __ldg(shift + ch + e);
         }
-        commit_elect(smem_u32(&s_bar[kE + s]));
-        if (u == n_uses - 1) commit_elect(smem_u32(&s_bar[kTF]));
-        s = (s + 1 == C::STAGES) ? 0 : s + 1;
+        if (p.relu) v = fmaxf(v, 0.f);
+        o[e] = v;
       }
-      tc_fence_before();
-    } else if (lane == 0) {
-      // ---------------------------------------------------------------- TMA: image tile (hi, lo) + weights per use
-      int s = 0;
-      const int t_begin = p.up > 1 ? tap0 : 0, t_end = p.up > 1 ? tap0 + 1 : p.taps;
-      for (int t = t_begin; t < t_end; ++t) {
-        const int dy = p.up > 1 ? 0 : t / p.kw, dx = p.up > 1 ? 0 : t % p.kw;
-        const int x = tx0 * p.stride - p.pad + dx, y = ty0 * p.stride - p.pad + dy;  // may be negative: zero fill
-        for (int g = 0; g < G; ++g) {
-          mbar_wait(smem_u32(&s_bar[kE + s]), (ph >> s) & 1u);
-          ph ^= 1u << s;
-          const uint32_t st = ring + static_cast<uint32_t>(s * C::STAGE), bar = smem_u32(&s_bar[kF + s]);
-          mbar_arrive_expect_tx(bar, static_cast<uint32_t>(C::STAGE));
-          tma_tile4d(st, &in_map, g * C::KC, x, y, b, bar);                       // hi half of the 32 channels
-          tma_tile4d(st + C::A_TILE, &in_map, p.Cin + g * C::KC, x, y, b, bar);   // lo half
-          bulk_g2s(st + C::A_STAGE, w_tile + (static_cast<size_t>(t) * p.Cin + g * C::KC) * (2 * N),
-                   static_cast<uint32_t>(C::B_STAGE), bar);
-          s = (s + 1 == C::STAGES) ? 0 : s + 1;
-        }
+      if (out_split) {  // channel counts of split-row layers are multiples of 16: whole pairs
+        float h[2], l[2];
+        split_tf32(o[0], h[0], l[0]);
+        split_tf32(o[1], h[1], l[1]);
+        float *oh = out_split + orow * (2 * static_cast<size_t>(p.out_C)) + p.out_c0 + ch;
+        *reinterpret_cast<float2 *>(oh) = make_float2(h[0], h[1]);
+        *reinterpret_cast<float2 *>(oh + p.out_C) = make_float2(l[0], l[1]);
+      }
+      if (out_nchw) {  // fp32 planes [B, cout, out_H, out_W]
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (ch + e < p.cout) out_nchw[((static_cast<size_t>(im.b) * p.cout + ch + e) * p.out_H + Y) * p.out_W + X] = o[e];
       }
     }
-    __syncthreads();  // item drained (epilogue has read TMEM) before the next item's first MMA overwrites it
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (wid == 4) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"(static_cast<uint32_t>(C::TMEM_COLS))
-                 : "memory");
   }
 }
 
@@ -332,7 +257,7 @@ int launch(const CUtensorMap &map, const Params &p, const float *packed, const f
   auto kern = dense_conv_kernel<N>;
   P3D_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   const long long work = static_cast<long long>(p.B) * p.tiles_y * p.tiles_x * p.n_ntiles * (p.up > 1 ? p.up * p.up : 1);
-  const long long slots = static_cast<long long>(kNumSMs) * C::MIN_CTAS;
+  const long long slots = static_cast<long long>(num_sms()) * C::MIN_CTAS;
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(static_cast<unsigned int>(work < slots ? work : slots));
   cfg.blockDim = dim3(kThreads);

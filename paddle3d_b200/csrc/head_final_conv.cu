@@ -4,7 +4,7 @@
 // per 32 input channels of one head; here a block stages a 16 x 8 pixel tile (+ halo) of one head's 64 input channels
 // in shared memory, channel-major, and every thread accumulates the <= 4 outputs of its pixel with exact fp32 FMAs in
 // (tap, channel) order.
-// Parity-green on a B200 (tests/test_gpu_dense.py::test_batched_head_matches_per_layer_head).  Two input formats: tf32
+// Checked by tests/test_gpu_dense.py::test_batched_head_matches_per_layer_head.  Two input formats: tf32
 // pixel split rows (p3d_head_final_conv) and fp16-pair pixel H16 rows (p3d_head_final_conv_h16).
 //
 //   input   pixel split rows [B*H*W][2][in_C]; group g reads channels [g*Cin, (g+1)*Cin) as hi + lo

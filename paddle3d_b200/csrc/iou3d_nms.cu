@@ -1,4 +1,4 @@
-// iou3d_nms ops for sm_100a: pairwise BEV overlap / IoU and sync-free rotated / axis-aligned NMS.
+// iou3d_nms ops for sm_90a: pairwise BEV overlap / IoU and sync-free rotated / axis-aligned NMS.
 // Replaces paddle3d/ops/iou3d_nms/iou3d_nms.cpp:44-204 + iou3d_nms_kernel.cu:275-482.
 #include "box_geom.cuh"
 #include "common.cuh"

@@ -3,7 +3,7 @@
 // no bias) + BatchNorm1D(eval) + ReLU, max over the M rows — one block per pillar, one thread per output channel, the
 // decorated rows staged in shared memory.  The reference runs this as ~15 elementwise / matmul / argmax launches over
 // the [N, M, F+5] and [N, M, C] intermediates; here only voxels [N, M, F] is read and [N, C] written.
-// Parity-green on a B200 (tests/test_gpu_voxelize.py::test_pillar_feature_net, 1e-4 vs the oracle restatement).
+// Checked by tests/test_gpu_voxelize.py::test_pillar_feature_net (1e-4 vs the oracle restatement).
 #include "common.cuh"
 #include "p3d_b200.h"
 

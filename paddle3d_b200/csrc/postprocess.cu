@@ -1,4 +1,4 @@
-// centerpoint_postprocess for sm_100a: all tasks batched in every launch, no host synchronisation.
+// centerpoint_postprocess for sm_90a: all tasks batched in every launch, no host synchronisation.
 //
 // Replaces paddle3d/ops/centerpoint_postprocess/postprocess.cu:104-280, which runs per task
 // 4 Paddle elementwise ops + decode_kernel + 2 masked_select (D2H sync) + argsort + nms_kernel +

@@ -1,4 +1,4 @@
-// Dense BEV canvas writer for sm_100a: PointPillarsScatter and sparse to_dense(+transpose), gather-formulated.
+// Dense BEV canvas writer for sm_90a: PointPillarsScatter and sparse to_dense(+transpose), gather-formulated.
 //
 // The reference does zeros + paddle.scatter + transpose (pillar_scatter.py:71-92) or
 // to_dense + transpose + reshape (sparse_resnet.py:202-206): three passes over the dense tensor.

@@ -1,4 +1,4 @@
-// Sparse 3-D convolution for sm_100a: rulebook build + output-stationary gather-GEMM.
+// Sparse 3-D convolution for sm_90a: rulebook build + output-stationary gather-GEMM.
 //
 // Replaces what SparseResNet3D asks of paddle.sparse.nn (sparse_resnet.py:31-60,84-111,125-206):
 // Paddle's phi kernels build a pair list per kernel offset and run K rounds of
@@ -16,7 +16,7 @@
 // (linear cell << 32 | row)), all counts kept on the device.
 //
 // This file holds the fp32 CUDA-core GEMM path (exact fp32 FMA accumulation, used for parity and
-// for the 5-channel input layer); the tcgen05 3xTF32 path lives in sparse_conv_tc.cu.
+// for the 5-channel input layer); the wgmma 3xTF32 path lives in sparse_conv_tc.cu.
 #include <cuda_fp16.h>
 
 #include "common.cuh"
@@ -455,7 +455,7 @@ __global__ void __launch_bounds__(128) small_cin_kernel(const float *__restrict_
 
 unsigned int persistent_grid(long long work_items) {
   const long long need = (work_items + 255) / 256;
-  const long long cap = static_cast<long long>(kNumSMs) * 8;  // 8 CTAs of 256 threads per SM = full occupancy
+  const long long cap = static_cast<long long>(num_sms()) * 8;  // 8 CTAs of 256 threads per SM = full occupancy
   return static_cast<unsigned int>(need < cap ? (need > 0 ? need : 1) : cap);
 }
 

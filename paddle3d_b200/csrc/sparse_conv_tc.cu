@@ -1,21 +1,20 @@
-// Sparse-conv gather-GEMM on Blackwell tensor cores: tcgen05.mma kind::tf32, accumulators in TMEM,
+// Sparse-conv gather-GEMM on Hopper tensor cores: wgmma kind tf32, fp32 accumulators in registers,
 // 3xTF32 split (a = hi + lo, b = hi + lo; D += a_hi*b_hi + a_hi*b_lo + a_lo*b_hi) for fp32-level accuracy.
 //
-// One CTA owns 128 consecutive output rows (UMMA M = 128, N = Cout, fp32 accumulate in Cout TMEM columns)
-// and walks the K dimension = (active taps) x (Cin in chunks of KC <= 32 channels) through a ring of
-// shared-memory stages:
+// One CTA (two warpgroups) owns 128 consecutive output rows — warpgroup g the rows 64g .. 64g+63, one m64nCout
+// accumulator — and walks the K dimension = (active taps) x (Cin in chunks of KC = 16 channels) through a ring of
+// shared-memory stages, STAGES - 1 uses ahead of the tensor cores:
 //
-//   warps 0-3  producers: thread r gathers row nbr[row0 + r][tap] of the input (KC floats, 16-byte
-//              loads), splits every value into tf32 hi / lo and stores both into the stage's A tiles in the
-//              canonical no-swizzle K-major core-matrix layout (8 rows x 16 B per core matrix) — a missing
-//              neighbour is a zero row.  Thread 0 also fires ONE cp.async.bulk per stage that drops the
-//              pre-packed weight slice [hi | lo] for (tap, chunk) into the B tiles (TMA engine, mbarrier
-//              complete_tx).  Generic-proxy stores are made visible to the tensor core with
-//              fence.proxy.async before the mbarrier arrive.
-//   warp 4     one elected lane issues 3 x KC/8 tcgen05.mma per stage and tcgen05.commit's the stage back to
-//              the producers; after the last stage it commits the accumulator to the epilogue barrier.
-//   warps 0-3  epilogue: tcgen05.ld 32 lanes x 16 columns at a time, fused BN scale/shift (+bias), residual,
-//              ReLU, 64 B per thread row stores.
+//   gather     thread r of the 128 rows (two threads per row, two 16-byte chunks each) loads row nbr[row0 + r][tap]
+//              of the input, splits every value into tf32 hi / lo and stores both into the stage's A tiles in the
+//              canonical no-swizzle K-major core-matrix layout (8 rows x 16 B per core matrix) — a missing neighbour is a
+//              zero row.  Thread 0 fires ONE cp.async.bulk per stage that drops the pre-packed weight slice [hi | lo] for
+//              (tap, chunk) into the B tiles (TMA engine, mbarrier complete_tx).  Generic-proxy stores are made visible
+//              to the tensor cores with fence.proxy.async before the CTA barrier that precedes the wgmma.
+//   mma        per 8-wide k-step 3 wgmma: hi x hi into one accumulator, lo x hi + hi x lo into a second one (the small
+//              cross terms keep their own rounding; the epilogue adds the two); the gather of use u + S - 1
+//              runs while the wgmma of use u execute, a stage is refilled once the wgmma that read it have retired.
+//   epilogue   from the accumulator fragment: fused BN scale/shift (+bias), residual, ReLU, 8-byte row stores.
 //
 // Taps that no row of the tile uses are skipped for the whole tile (block-uniform bitmask).
 // Weights are packed once per layer by p3d_sparse_conv_pack_weights into exactly the shared-memory image:
@@ -32,28 +31,22 @@ struct Cfg {
   static constexpr int CH = KC / 4;              // 16-byte k-chunks per stage
   static constexpr int A_TILE = KC * kM * 4;     // bytes, one of hi / lo
   static constexpr int B_TILE = KC * COUT * 4;   // bytes, one of hi / lo
-  static constexpr int A_STAGE = 2 * A_TILE;      // hi + lo
-  static constexpr int B_STAGE = 2 * B_TILE;      // hi + lo (one cp.async.bulk)
-  // two independent rings (<= 96 KB together: two CTAs per SM): SA slots of gathered rows, SB slots of weights.
-  // The weight ring is deeper so that the TMA latency never sits on the gather -> MMA critical path.
-  // Narrow layers (Cout <= 32) have 300-530 row tiles: three CTAs per SM (444 slots) instead of two keeps the
-  // 309-tile 32-channel layers in ONE wave and adds a third MMA-issuing warp per SM.
-  static constexpr int MIN_CTAS = (COUT <= 32) ? 3 : 2;
-  static constexpr int SA = (COUT <= 32) ? 3 : ((COUT <= 64) ? 4 : 3);
-  static constexpr int BUDGET = (COUT <= 32) ? 56 * 1024 : 96 * 1024;  // 3 x (56 K ring + 14 K map + 3 K) <= 228 KB per SM
-  static constexpr int SB_RAW = (BUDGET - SA * A_STAGE) / B_STAGE;
-  static constexpr int SB = SB_RAW > 8 ? 8 : SB_RAW;
-  static constexpr int RING_BYTES = SA * A_STAGE + SB * B_STAGE;
-  // Independent TMEM accumulators: back-to-back tcgen05.mma into ONE accumulator serialise on its dependency
-  // latency (~200 cycles each, measured), so the three 3xTF32 products go to separate column ranges and are summed
-  // in the epilogue.  Cout = 128 keeps two (256 columns) so that two CTAs still fit the 512 TMEM columns of an SM.
-  static constexpr int NACC = (COUT <= 64) ? 3 : 2;
-  static constexpr int TMEM_COLS = (NACC * COUT <= 32) ? 32 : (NACC * COUT <= 64) ? 64 : (NACC * COUT <= 128) ? 128
-                                   : (NACC * COUT <= 256) ? 256 : 512;
-  static constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | (static_cast<uint32_t>(COUT >> 3) << 17) |
-                                    (static_cast<uint32_t>(kM >> 4) << 24);
-  static_assert(CIN % 16 == 0 && COUT % 16 == 0 && COUT <= 256, "tensor-core path needs 16-channel multiples");
+  static constexpr int A_STAGE = 2 * A_TILE;     // hi + lo
+  static constexpr int B_STAGE = 2 * B_TILE;     // hi + lo (one cp.async.bulk)
+  static constexpr int STAGE = A_STAGE + B_STAGE;
+  static constexpr int MIN_CTAS = (COUT <= 64) ? 2 : 1;
+  static constexpr int BUDGET = (COUT <= 64) ? 96 * 1024 : 192 * 1024;
+  static constexpr int S_RAW = BUDGET / STAGE;
+  static constexpr int STAGES = S_RAW > 8 ? 8 : (S_RAW < 3 ? 3 : S_RAW);
+  static constexpr int ACC = COUT / 2;           // registers of one m64 x COUT accumulator per thread
+  static_assert(CIN % 16 == 0 && COUT % 16 == 0 && COUT <= 128, "tensor-core path needs 16-channel multiples");
+  static_assert(CH * kM * 4 == 2 * kThreads * 4, "two 16-byte chunks per thread and use");
 };
+
+__device__ __forceinline__ int nth_bit(uint32_t m, int k) {  // position of the k-th (0-based) set bit of m
+  for (int i = 0; i < k; ++i) m &= m - 1u;
+  return __ffs(m) - 1;
+}
 
 template <int CIN, int COUT>
 __global__ void __launch_bounds__(kThreads, Cfg<CIN, COUT>::MIN_CTAS)
@@ -63,6 +56,7 @@ __global__ void __launch_bounds__(kThreads, Cfg<CIN, COUT>::MIN_CTAS)
                               const float *__restrict__ shift, const float *__restrict__ residual, int relu,
                               float *__restrict__ out_base) {
   using C = Cfg<CIN, COUT>;
+  constexpr int S = C::STAGES;
   // Persistent CTAs: the grid is sized for the SMs (not for the row CAPACITY, which would launch thousands of empty
   // CTAs) and every CTA walks the work items  w = blockIdx.x, +gridDim.x, ...  with  w = tile * splits + split.
   // split-K over taps: split s owns the taps t == s (mod splits) and writes raw partial sums to slab s of `out_base`
@@ -73,50 +67,29 @@ __global__ void __launch_bounds__(kThreads, Cfg<CIN, COUT>::MIN_CTAS)
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t *a_base = smem;                                                  // SA x A_STAGE
-  uint8_t *b_base = smem + C::SA * C::A_STAGE;                             // SB x B_STAGE
-  int32_t *s_nbr = reinterpret_cast<int32_t *>(smem + C::RING_BYTES);      // [kM][K]
-  // barriers: a_full[4] a_empty[4] b_full[8] b_empty[8] tmem_full
-  __shared__ __align__(8) unsigned long long s_bar[4 + 4 + 8 + 8 + 1];
-  constexpr int kAF = 0, kAE = 4, kBF = 8, kBE = 16, kTF = 24;
-  __shared__ uint32_t s_tmem_base;
-  __shared__ uint32_t s_active;                                             // bit t: some row uses tap t (K <= 32)
+  int32_t *s_nbr = reinterpret_cast<int32_t *>(smem + S * C::STAGE);      // [kM][K]
+  __shared__ __align__(8) unsigned long long s_full[8];                  // weights of a stage landed
+  __shared__ uint32_t s_active;                                          // bit t: some row uses tap t (K <= 32)
 
-  const int tid = threadIdx.x, wid = tid >> 5, lane = tid & 31;
-  if (tid == kProducers) {  // first lane of the MMA warp
-    for (int s = 0; s < C::SA; ++s) {
-      mbar_init(smem_u32(&s_bar[kAF + s]), 32);        // the 32 lanes of the slot's producer warp
-      mbar_init(smem_u32(&s_bar[kAE + s]), 1);         // tcgen05.commit
-    }
-    for (int s = 0; s < C::SB; ++s) {
-      mbar_init(smem_u32(&s_bar[kBF + s]), 1);         // arrive.expect_tx + bulk-copy bytes
-      mbar_init(smem_u32(&s_bar[kBE + s]), 1);         // tcgen05.commit
-    }
-    mbar_init(smem_u32(&s_bar[kTF]), 1);
+  const int tid = threadIdx.x, lane = tid & 31, wg = tid >> 7, wtid = tid & 127;
+  if (tid == 0) {
+    for (int s = 0; s < S; ++s) mbar_init(smem_u32(&s_full[s]), 1);
     fence_mbar_init();
   }
-  if (wid == 4) {  // TMEM allocation is warp-collective
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem_base)),
-                 "r"(static_cast<uint32_t>(C::TMEM_COLS))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem_base;
+  const uint32_t ring = smem_u32(smem);
+  const int g_row = tid & (kM - 1), g_c0 = (tid >> 7) * 2;  // gather: row of the tile, first of two 16-byte chunks
 
-  int use_base = 0;  // pipeline uses consumed by earlier work items of this CTA: the ring phases keep running
-  int item_it = 0;
-  for (long long w = blockIdx.x; w < n_work; w += gridDim.x, ++item_it) {
+  uint32_t gu = 0;  // uses consumed by earlier work items of this CTA: the ring phases keep running
+  for (long long w = blockIdx.x; w < n_work; w += gridDim.x) {
     const long long tile = w / splits;
     const int split = static_cast<int>(w - tile * splits);
     const long long row0 = tile * kM;
     const int rows = static_cast<int>(min(static_cast<long long>(kM), n - row0));
     float *out = out_base + static_cast<size_t>(split) * static_cast<size_t>(n_cap) * COUT;
+    __syncthreads();  // previous item drained: s_nbr and s_active free
     if (tid == 0) s_active = 0u;
-    __syncthreads();  // previous item drained: epilogue finished reading TMEM, s_nbr free
+    __syncthreads();
     {
       uint32_t mine = 0u;
       for (int q = tid; q < kM * K; q += kThreads) {
@@ -134,182 +107,90 @@ __global__ void __launch_bounds__(kThreads, Cfg<CIN, COUT>::MIN_CTAS)
       for (int t = split; t < K; t += splits) tap_mask |= 1u << t;
     }
     const uint32_t active = s_active & tap_mask;
-    const int n_stage_uses = __popc(active) * C::G;
+    const int n_uses = __popc(active) * C::G;
 
-    if (wid < 4) {
-      // ---------------------------------------------------------------- producers
-      // Warp w (< SA) owns ring slot w: it gathers all 128 rows of its (tap, chunk) uses — lane l takes rows
-      // l, l+32, l+64, l+96, i.e. 4 x CH independent 16-byte loads in flight per lane — so SA stages' worth of L2
-      // gathers are in flight per CTA.  With one warp per slot a warp can never run a full mbarrier phase ahead of
-      // the tensor core, so the parity waits cannot alias.
-      const int r = tid;
-      int use = use_base;
-      for (int t = 0; t < K; ++t) {
-        if (!((active >> t) & 1u)) continue;
-        for (int g = 0; g < C::G; ++g, ++use) {
-          const int s = use % C::SA;
-          if (s != wid) continue;
-          const uint32_t ph = static_cast<uint32_t>((use / C::SA) & 1);
-          float4 v[4][C::CH];
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const int src = s_nbr[(lane + 32 * q) * K + t];
-            if (src >= 0) {
-              const float4 *p = reinterpret_cast<const float4 *>(in + static_cast<size_t>(src) * CIN + g * C::KC);
-#pragma unroll
-              for (int c = 0; c < C::CH; ++c) v[q][c] = __ldg(p + c);
-            } else {
-#pragma unroll
-              for (int c = 0; c < C::CH; ++c) v[q][c] = make_float4(0.f, 0.f, 0.f, 0.f);
-            }
-          }
-          mbar_wait(smem_u32(&s_bar[kAE + s]), ph ^ 1u);  // slot free (first pass returns at once)
-          uint8_t *st = a_base + s * C::A_STAGE;
-          // A-tile layout: k-chunk c at c*2048 (LBO), 8-row groups 128 B apart (SBO): the 32 lanes of one store
-          // instruction (32 consecutive rows, same chunk) cover 512 contiguous bytes — no bank conflicts.
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const int row = lane + 32 * q;
-            const uint32_t a_off = static_cast<uint32_t>((row >> 3) * 128 + (row & 7) * 16);
-#pragma unroll
-            for (int c = 0; c < C::CH; ++c) {
-              float4 h, l;
-              split_tf32(v[q][c].x, h.x, l.x);
-              split_tf32(v[q][c].y, h.y, l.y);
-              split_tf32(v[q][c].z, h.z, l.z);
-              split_tf32(v[q][c].w, h.w, l.w);
-              *reinterpret_cast<float4 *>(st + c * (kM * 16) + a_off) = h;
-              *reinterpret_cast<float4 *>(st + C::A_TILE + c * (kM * 16) + a_off) = l;
-            }
-          }
-          fence_proxy_async();
-          mbar_arrive(smem_u32(&s_bar[kAF + s]));
-        }
+    // gather use q (tap, chunk) of this item into its ring slot; thread 0 also posts the weight slice
+    auto issue = [&](int q) {
+      if (q >= n_uses) return;
+      const int t = nth_bit(active, q / C::G), g = q % C::G;
+      const uint32_t slot = (gu + static_cast<uint32_t>(q)) % S;
+      uint8_t *st = smem + slot * C::STAGE;
+      if (tid == 0) {
+        const uint32_t bar = smem_u32(&s_full[slot]);
+        mbar_arrive_expect_tx(bar, static_cast<uint32_t>(C::B_STAGE));
+        bulk_g2s(ring + slot * C::STAGE + C::A_STAGE, packed_w + (static_cast<size_t>(t) * C::G + g) * (2 * C::KC * COUT),
+                 static_cast<uint32_t>(C::B_STAGE), bar);
       }
-      // ---------------------------------------------------------------- epilogue
-      mbar_wait(smem_u32(&s_bar[kTF]), static_cast<uint32_t>(item_it & 1));
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(wid * 32) << 16);
-      const bool live = r < rows;
-      float *orow = out + (row0 + r) * COUT;
-      const float *rrow = residual ? residual + (row0 + r) * COUT : nullptr;
-#pragma unroll 1
-      for (int c0 = 0; c0 < COUT; c0 += 16) {
-        uint32_t a[16];
-        if (n_stage_uses > 0) {
-          asm volatile(
-              "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
-              "%15}, [%16];"
-              : "=r"(a[0]), "=r"(a[1]), "=r"(a[2]), "=r"(a[3]), "=r"(a[4]), "=r"(a[5]), "=r"(a[6]), "=r"(a[7]),
-                "=r"(a[8]), "=r"(a[9]), "=r"(a[10]), "=r"(a[11]), "=r"(a[12]), "=r"(a[13]), "=r"(a[14]), "=r"(a[15])
-              : "r"(taddr + static_cast<uint32_t>(c0)));
+      const int src = s_nbr[g_row * K + t];
+      float4 v[2];
 #pragma unroll
-          for (int acc = 1; acc < C::NACC; ++acc) {
-            uint32_t b[16];
-            asm volatile(
-                "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
-                "%15}, [%16];"
-                : "=r"(b[0]), "=r"(b[1]), "=r"(b[2]), "=r"(b[3]), "=r"(b[4]), "=r"(b[5]), "=r"(b[6]), "=r"(b[7]),
-                  "=r"(b[8]), "=r"(b[9]), "=r"(b[10]), "=r"(b[11]), "=r"(b[12]), "=r"(b[13]), "=r"(b[14]), "=r"(b[15])
-                : "r"(taddr + static_cast<uint32_t>(acc * COUT + c0)));
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      for (int c = 0; c < 2; ++c)
+        v[c] = src >= 0 ? __ldg(reinterpret_cast<const float4 *>(in + static_cast<size_t>(src) * CIN + g * C::KC) + g_c0 + c)
+                        : make_float4(0.f, 0.f, 0.f, 0.f);
+      // A-tile layout: k-chunk c at c*2048 (LBO), 8-row groups 128 B apart (SBO): the 32 lanes of one store
+      // instruction (32 consecutive rows, same chunk) cover 512 contiguous bytes — no bank conflicts.
+      const uint32_t a_off = static_cast<uint32_t>((g_row >> 3) * 128 + (g_row & 7) * 16);
 #pragma unroll
-            for (int j = 0; j < 16; ++j) a[j] = __float_as_uint(__uint_as_float(a[j]) + __uint_as_float(b[j]));
-          }
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        } else {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) a[j] = 0u;
-        }
-        if (live) {
-          float o[16], res[16];
-          if (rrow) {
-#pragma unroll
-            for (int j = 0; j < 16; j += 4) {
-              const float4 rv = __ldg(reinterpret_cast<const float4 *>(rrow + c0 + j));
-              res[j] = rv.x;
-              res[j + 1] = rv.y;
-              res[j + 2] = rv.z;
-              res[j + 3] = rv.w;
-            }
-          }
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            float v = __uint_as_float(a[j]);
-            if (scale) v = v * __ldg(scale + c0 + j);
-            if (shift) v = v + __ldg(shift + c0 + j);
-            if (rrow) v = v + res[j];
-            if (relu) v = fmaxf(v, 0.f);
-            o[j] = v;
-          }
-#pragma unroll
-          for (int j = 0; j < 16; j += 4)
-            *reinterpret_cast<float4 *>(orow + c0 + j) = make_float4(o[j], o[j + 1], o[j + 2], o[j + 3]);
-        }
+      for (int c = 0; c < 2; ++c) {
+        float4 h, l;
+        split_tf32(v[c].x, h.x, l.x);
+        split_tf32(v[c].y, h.y, l.y);
+        split_tf32(v[c].z, h.z, l.z);
+        split_tf32(v[c].w, h.w, l.w);
+        *reinterpret_cast<float4 *>(st + (g_c0 + c) * (kM * 16) + a_off) = h;
+        *reinterpret_cast<float4 *>(st + C::A_TILE + (g_c0 + c) * (kM * 16) + a_off) = l;
       }
-      tc_fence_before();
-    } else if (wid == 4) {
-      // ---------------------------------------------------------------- MMA issuer (warp 4)
-      if (n_stage_uses == 0) {
-        if (lane == 0) mbar_arrive(smem_u32(&s_bar[kTF]));
-      } else {
-        for (int u = 0; u < n_stage_uses; ++u) {
-          const int use = use_base + u;
-          const int sa = use % C::SA, sb = use % C::SB;
-          mbar_wait(smem_u32(&s_bar[kBF + sb]), static_cast<uint32_t>((use / C::SB) & 1));
-          mbar_wait(smem_u32(&s_bar[kAF + sa]), static_cast<uint32_t>((use / C::SA) & 1));
-          tc_fence_after();
-          if (lane == 0) {
-            const uint32_t a_hi = smem_u32(a_base + sa * C::A_STAGE), a_lo = a_hi + C::A_TILE;
-            const uint32_t b_hi = smem_u32(b_base + sb * C::B_STAGE), b_lo = b_hi + COUT * 16;  // lo rows follow the hi rows
+    };
+
+    float acc[C::ACC], accx[C::ACC];  // hi x hi | cross terms
 #pragma unroll
-            for (int j = 0; j < C::KC / 8; ++j) {
-              const uint32_t ao = static_cast<uint32_t>(2 * j) * (kM * 16), bo = static_cast<uint32_t>(2 * j) * (2 * COUT * 16);
-              const uint64_t dah = smem_desc(a_hi + ao, kM * 16, 128), dal = smem_desc(a_lo + ao, kM * 16, 128);
-              const uint64_t dbh = smem_desc(b_hi + bo, 2 * COUT * 16, 128), dbl = smem_desc(b_lo + bo, 2 * COUT * 16, 128);
-              const uint32_t first = (u | j) ? 1u : 0u;
-              umma_tf32(tmem_base, dal, dbh, C::IDESC, first);                               // acc 0
-              umma_tf32(tmem_base + (C::NACC == 3 ? COUT : 0), dah, dbl, C::IDESC, C::NACC == 3 ? first : 1u);  // acc 1 (or 0)
-              umma_tf32(tmem_base + (C::NACC - 1) * COUT, dah, dbh, C::IDESC, first);         // last acc
-            }
-            umma_commit(smem_u32(&s_bar[kAE + sa]));                             // gathered rows consumed
-            umma_commit(smem_u32(&s_bar[kBE + sb]));                             // weights consumed
-            if (u == n_stage_uses - 1) umma_commit(smem_u32(&s_bar[kTF]));      // accumulator ready
-          }
-          __syncwarp();
-        }
+    for (int i = 0; i < C::ACC; ++i) acc[i] = accx[i] = 0.f;
+    for (int q = 0; q < S - 1; ++q) issue(q);
+    for (int u = 0; u < n_uses; ++u) {
+      const uint32_t slot = (gu + static_cast<uint32_t>(u)) % S, par = ((gu + static_cast<uint32_t>(u)) / S) & 1u;
+      fence_proxy_async();  // this thread's generic-proxy stores of the A tiles -> wgmma (async proxy) reads
+      mbar_wait(smem_u32(&s_full[slot]), par);
+      __syncthreads();      // the whole stage is written; the wgmma of use u - 1 have retired in both warpgroups
+      const uint32_t a_hi = ring + slot * C::STAGE + static_cast<uint32_t>(wg * 8 * 128), a_lo = a_hi + C::A_TILE;
+      const uint32_t b_hi = ring + slot * C::STAGE + C::A_STAGE, b_lo = b_hi + COUT * 16;  // lo rows follow the hi rows
+      wg_fence();
+#pragma unroll
+      for (int j = 0; j < C::KC / 8; ++j) {
+        const uint32_t ao = static_cast<uint32_t>(2 * j) * (kM * 16), bo = static_cast<uint32_t>(2 * j) * (2 * COUT * 16);
+        const uint64_t dah = smem_desc(a_hi + ao, kM * 16, 128), dal = smem_desc(a_lo + ao, kM * 16, 128);
+        const uint64_t dbh = smem_desc(b_hi + bo, 2 * COUT * 16, 128), dbl = smem_desc(b_lo + bo, 2 * COUT * 16, 128);
+        wg::mma_tf32<COUT>(accx, dal, dbh, 1u);
+        wg::mma_tf32<COUT>(accx, dah, dbl, 1u);
+        wg::mma_tf32<COUT>(acc, dah, dbh, 1u);
       }
-      tc_fence_before();
-    } else {
-      // ---------------------------------------------------------------- weight TMA (warp 5, one lane)
-      if (lane == 0) {
-        int use = use_base;
-        for (int t = 0; t < K; ++t) {
-          if (!((active >> t) & 1u)) continue;
-          for (int g = 0; g < C::G; ++g, ++use) {
-            const int sb = use % C::SB;
-            mbar_wait(smem_u32(&s_bar[kBE + sb]), static_cast<uint32_t>((use / C::SB) & 1) ^ 1u);
-            mbar_arrive_expect_tx(smem_u32(&s_bar[kBF + sb]), static_cast<uint32_t>(C::B_STAGE));
-            bulk_g2s(smem_u32(b_base + sb * C::B_STAGE), packed_w + (static_cast<size_t>(t) * C::G + g) * (2 * C::KC * COUT),
-                     static_cast<uint32_t>(C::B_STAGE), smem_u32(&s_bar[kBF + sb]));
-          }
-        }
-      }
+      wg_commit();
+      issue(u + S - 1);  // the slot of use u - 1
+      wg_wait<0>();
     }
-    use_base += n_stage_uses;
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (wid == 4) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"(static_cast<uint32_t>(C::TMEM_COLS))
-                 : "memory");
+    wg_fence_acc<C::ACC>(acc);
+    wg_fence_acc<C::ACC>(accx);
+    gu += static_cast<uint32_t>(n_uses);
+
+    // ---------------------------------------------------------------- epilogue (accumulator fragment)
+#pragma unroll
+    for (int i = 0; i < C::ACC; i += 2) {
+      const int r = wg * 64 + frag_row(i, wtid), c = frag_col(i, wtid);
+      if (r >= rows) continue;
+      float2 v = make_float2(accx[i] + acc[i], accx[i + 1] + acc[i + 1]);
+      if (scale) v = make_float2(v.x * __ldg(scale + c), v.y * __ldg(scale + c + 1));
+      if (shift) v = make_float2(v.x + __ldg(shift + c), v.y + __ldg(shift + c + 1));
+      if (residual) {
+        const float2 rv = __ldg(reinterpret_cast<const float2 *>(residual + (row0 + r) * COUT + c));
+        v = make_float2(v.x + rv.x, v.y + rv.y);
+      }
+      if (relu) v = make_float2(fmaxf(v.x, 0.f), fmaxf(v.y, 0.f));
+      *reinterpret_cast<float2 *>(out + (row0 + r) * COUT + c) = v;
+    }
   }
 }
 
 // packed[tap][g][c][hl * Cout + n][j] = split(W[tap][g*KC + 4c + j][n]): per (tap, 16-channel chunk) a K-major
-// operand of 2*Cout rows (tf32 hi rows, then lo rows), so [B_hi | B_lo] is ONE UMMA operand with N = 2*Cout.
+// operand of 2*Cout rows (tf32 hi rows, then lo rows), so B_lo is the B_hi descriptor advanced by Cout rows.
 __global__ void __launch_bounds__(256) pack_weights_kernel(const float *__restrict__ w, int K, int Cin, int Cout,
                                                            float *__restrict__ packed) {
   const long long q = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -333,12 +214,12 @@ int launch(const float *in, const int32_t *nbr, const int32_t *n_out_dev, int64_
            const float *scale, const float *shift, const float *residual, int relu, float *out, cudaStream_t st,
            int splits = 1) {
   using C = Cfg<CIN, COUT>;
-  const size_t smem = static_cast<size_t>(C::RING_BYTES) + static_cast<size_t>(kM) * K * sizeof(int32_t) + 1024;
+  const size_t smem = static_cast<size_t>(C::STAGES) * C::STAGE + static_cast<size_t>(kM) * K * sizeof(int32_t) + 1024;
   if (smem > 227 * 1024) return P3D_ERR_UNSUPPORTED;
   auto kern = gather_gemm_tf32x3_kernel<CIN, COUT>;
   P3D_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   const long long work = ((n_cap + kM - 1) / kM) * splits;
-  const long long slots = static_cast<long long>(kNumSMs) * C::MIN_CTAS;
+  const long long slots = static_cast<long long>(num_sms()) * C::MIN_CTAS;
   kern<<<static_cast<unsigned int>(work < slots ? work : slots), kThreads, smem, st>>>(in, nbr, n_out_dev, n_cap, K, splits, packed, scale, shift, residual, relu,
                                                   out);
   P3D_LAUNCH_CHECK();
@@ -452,7 +333,7 @@ extern "C" int p3d_sparse_conv_gather_gemm_tf32x3_ws(const float *in, const int3
 #undef P3D_TC_CASE
   if (rc != P3D_OK || !split) return rc;
   const long long fin_blocks = (n_out_cap * (Cout / 4) + 255) / 256;
-  tc::rows_finalize_kernel<<<static_cast<unsigned int>(fin_blocks < kNumSMs * 8 ? fin_blocks : kNumSMs * 8), 256, 0, st>>>(conv_out, splits, n_out_dev, n_out_cap, Cout,
+  tc::rows_finalize_kernel<<<static_cast<unsigned int>(fin_blocks < num_sms() * 8 ? fin_blocks : num_sms() * 8), 256, 0, st>>>(conv_out, splits, n_out_dev, n_out_cap, Cout,
                                                                                 scale, shift, residual, relu, out);
   P3D_LAUNCH_CHECK();
   return P3D_OK;

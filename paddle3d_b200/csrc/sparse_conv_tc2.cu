@@ -1,22 +1,20 @@
-// Sparse-conv gather-GEMM on tcgen05, split-row version: activations travel between layers already split into their
+// Sparse-conv gather-GEMM on wgmma, split-row version: activations travel between layers already split into their
 // tf32 hi / lo halves (row layout [n][2][C]: hi row, then lo row), so the 3xTF32 split is paid ONCE per produced
 // element (in the producing layer's epilogue) instead of once per gathering neighbour (11-27x), and the gather
 // becomes a pure copy that cp.async (LDGSTS, 16 B, zero-fill for missing neighbours) drops straight into swizzled
-// UMMA operand tiles — no register staging, no ALU on the data in the producer loop.
+// wgmma operand tiles — no register staging, no ALU on the data in the gather.
 //
 //   grid        persistent: min(#work items at capacity, MIN_CTAS x SMs) CTAs, each walks the work items
 //               w = blockIdx.x, +gridDim.x, ... (w = tile * splits + split) of the DEVICE row count.
-//   warps 0..NPW-1  producers: per (tap, KC-channel chunk) "use", full-128-byte-line cp.async gathers (8 lanes per
-//               line, 4 rows per warp instruction) into SWIZZLE_128B (KC = 32) or SWIZZLE_64B (KC = 16) tiles;
-//               completion is signalled with cp.async.mbarrier.arrive.noinc.  Afterwards the same warps run the
-//               epilogue: tcgen05.ld, BN scale/shift (+bias), residual (= hi + lo of the split residual rows),
-//               ReLU, then plain fp32 rows, split rows for the next layer, or both.
-//   warp NPW    MMA issuer: 2 tcgen05.mma.kind::tf32 per 8-wide k-step, tcgen05.commit frees the stage.
-//   warp NPW+1  weight TMA: cp.async.bulk of the packed [hi | lo] slice of the use into the same stage.
-// The producer and MMA warps are bound by their own instruction latency (measured with tools/split_probe.py: the bare
-// barrier skeleton costs 550-690 cycles per use with 4 producer warps), so the row gather is spread over 8 warps
-// (or 4 CTAs per SM for the narrow layers) and the stage index restarts at 0 for every work item, which keeps the
-// operand addresses on the uniform datapath.
+//   CTA         two warpgroups; warpgroup g owns rows 64g .. 64g+63 of the 128-row tile (one m64nCout accumulator).
+//   gather      per (tap, KC-channel chunk) "use", full-128-byte-line cp.async gathers (8 threads per line, 32 rows
+//               per CTA instruction) into SWIZZLE_128B (KC = 32) or SWIZZLE_64B (KC = 16) tiles, STAGES - 1 uses ahead;
+//               thread 0 copies the packed [hi | lo] weight slice of the use with cp.async.bulk (mbarrier complete_tx).
+//               TMA = true (Cin >= 32): warp 0 gathers the rows with one 2-D TMA box (one 128-byte line) per row half
+//               instead; a missing neighbour (row -1) is out of bounds for the tensor map and arrives as zeros.
+//   mma         3 wgmma kind tf32 per 8-wide k-step: hi x hi into one accumulator, lo x hi + hi x lo into a second one.
+//   epilogue    BN scale/shift (+bias), residual (= hi + lo of the split residual rows), ReLU, then plain fp32 rows,
+//               split rows for the next layer, or both, from the accumulator fragment.
 #include <cuda.h>  // CUtensorMap (types only: the encoder is fetched with cudaGetDriverEntryPoint)
 
 #include "tc_common.cuh"
@@ -35,116 +33,42 @@ struct Cfg {
   static constexpr int A_STAGE = 2 * A_TILE;
   static constexpr int B_STAGE = 2 * KC * COUT * 4;      // [chunk][hi rows | lo rows][16 B]
   static constexpr int STAGE = A_STAGE + B_STAGE;        // ONE ring: rows and weights of a use share a slot
-  static constexpr bool NARROW = (CIN == 16 && COUT <= 32);
-  static constexpr int MIN_CTAS = NARROW ? 4 : (COUT <= 64 ? 2 : 1);
-  static constexpr int NPW = NARROW ? 4 : 8;             // producer (= epilogue) warps
-  static constexpr int THREADS = NPW * 32 + 64;
-  static constexpr int RPW = kM / NPW;                   // rows gathered by one producer warp
-  static constexpr int QN = RPW / 4;                     // warp instructions (4 rows each) per use and row half
-  static constexpr int BUDGET = NARROW ? 40 * 1024 : (COUT <= 64 ? 100 * 1024 : 192 * 1024);
+  static constexpr int MIN_CTAS = COUT <= 64 ? 2 : 1;
+  static constexpr int BUDGET = COUT <= 64 ? 96 * 1024 : 192 * 1024;
   static constexpr int S_RAW = BUDGET / STAGE;
-  static constexpr int STAGES = S_RAW > 8 ? 8 : (S_RAW < 2 ? 2 : S_RAW);
-  // Two MMAs per 8-wide k-step: [B_hi | B_lo] is one K-major operand of 2*Cout rows, so
-  //   acc[0 .. 2N)   += A_hi x [B_hi | B_lo]      (N' = 2*Cout)
-  //   acc[2N .. 3N)  += A_lo x B_hi               (N  = Cout)
-  // and the epilogue adds the three column ranges (fewer, wider instructions: each tcgen05.mma has a fixed issue
-  // cost that does not depend on its size).
-  static constexpr int TMEM_COLS = (3 * COUT <= 64) ? 64 : (3 * COUT <= 128) ? 128 : (3 * COUT <= 256) ? 256 : 512;
-  static constexpr uint32_t IDESC2 = (1u << 4) | (2u << 7) | (2u << 10) | (static_cast<uint32_t>((2 * COUT) >> 3) << 17) |
-                                     (static_cast<uint32_t>(kM >> 4) << 24);
-  static constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | (static_cast<uint32_t>(COUT >> 3) << 17) |
-                                    (static_cast<uint32_t>(kM >> 4) << 24);
+  static constexpr int STAGES = S_RAW > 8 ? 8 : (S_RAW < 3 ? 3 : S_RAW);
+  static constexpr int ACC = COUT / 2;                   // registers of one m64 x COUT accumulator per thread
   static_assert(CIN % 16 == 0 && COUT % 16 == 0 && COUT <= 128, "tensor-core path needs 16-channel multiples");
-  static_assert(MIN_CTAS * TMEM_COLS <= 512, "TMEM over-subscribed");
   static_assert(STAGE % 1024 == 0 || KC == 16, "SWIZZLE_128B tiles need 1024-byte alignment");
   static_assert(STAGE % 512 == 0, "SWIZZLE_64B tiles need 512-byte alignment");
 };
 
-// debug only (p3d_debug_set_flags): 1 skip weight copies, 2 skip row gathers, 4 skip MMAs, 8 skip fence.proxy.async,
-// 16 plain mbarrier arrive instead of tcgen05.commit
-__device__ int g_dbg_flags = 0;
-
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void *src, bool valid) {
-  const uint32_t sz = valid ? 16u : 0u;  // src-size 0 => 16 bytes of zeros
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(sz) : "memory");
-}
-__device__ __forceinline__ void cp_async_arrive_noinc(uint32_t bar) {
-  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
-}
-// K-major SWIZZLE_128B operand: rows of 128 bytes (32 tf32), 8-row atoms of 1024 bytes (SBO), the 16-byte chunk index
-// of a row XOR-ed with (row & 7).  Tile base 1024-byte aligned; a k-step advances the start address by 32 bytes.
-__device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((addr & 0x3ffffu) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;            // LBO: unused for swizzled K-major, canonical value 1
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;    // SBO
-  d |= 1ull << 46;                                // descriptor version 1
-  d |= 2ull << 61;                                // layout type SWIZZLE_128B
-  return d;
-}
-
-// K-major SWIZZLE_64B operand: rows of 64 bytes (16 tf32), 8-row atoms of 512 bytes (SBO), chunk ^= (row >> 1) & 3.
-__device__ __forceinline__ uint64_t smem_desc_sw64(uint32_t addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((addr & 0x3ffffu) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(512 >> 4) << 32;
-  d |= 1ull << 46;
-  d |= 4ull << 61;  // layout type SWIZZLE_64B
-  return d;
-}
-
-// Warp-uniform issue: every lane executes the instruction stream, one elected lane issues.
-__device__ __forceinline__ void umma_tf32_elect(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                                uint32_t accumulate) {
+// 2-D TMA box of the split rows' tensor map (one 128-byte line of one row) into a SWIZZLE_128B tile row
+__device__ __forceinline__ void tma_row(uint32_t dst, const CUtensorMap *map, int col, int row, uint32_t bar) {
   asm volatile(
-      "{\n\t.reg .pred p, e;\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "@e tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_elect(uint32_t bar) {
-  asm volatile(
-      "{\n\t.reg .pred e;\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(bar)
+      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(dst),
+      "l"(reinterpret_cast<uint64_t>(map)), "r"(col), "r"(row), "r"(bar)
       : "memory");
 }
 
-// TMA row gather (experimental, TMA = true, Cin >= 32): 4 rows x 128 bytes of the split rows per instruction, written
-// by the TMA engine in the SWIZZLE_128B pattern of the tensor map; a negative (missing neighbour) or out-of-range row
-// index is out of bounds for the map and arrives as zeros.
-__device__ __forceinline__ void tma_gather4(uint32_t dst, const CUtensorMap *map, int col, int r0, int r1, int r2, int r3,
-                                            uint32_t bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cta.global.tile::gather4.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, "
-      "%5, %6}], [%7];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(col), "r"(r0), "r"(r1), "r"(r2), "r"(r3), "r"(bar)
-      : "memory");
+__device__ __forceinline__ int nth_bit(uint32_t m, int k) {  // position of the k-th (0-based) set bit of m
+  for (int i = 0; i < k; ++i) m &= m - 1u;
+  return __ffs(m) - 1;
 }
 
 template <int CIN, int COUT, bool TMA>
-__global__ void __launch_bounds__(Cfg<CIN, COUT>::THREADS, Cfg<CIN, COUT>::MIN_CTAS)
+__global__ void __launch_bounds__(kThreads, Cfg<CIN, COUT>::MIN_CTAS)
     gather_gemm_split_kernel(const __grid_constant__ CUtensorMap in_map, const float *__restrict__ in_split,
                              const int32_t *__restrict__ nbr,
                              const int32_t *__restrict__ n_out_dev, long long n_cap, int K, int splits,
                              const float *__restrict__ packed_w, const float *__restrict__ scale,
                              const float *__restrict__ shift, const float *__restrict__ residual_split, int relu,
-                             float *__restrict__ out_f32, float *__restrict__ out_split, long long *__restrict__ dbg) {
-  // dbg (optional, CTA 0 only): per-use clock64 timeline, 8 slots per use (first 512 uses):
-  //   0 producer(warp0): slot free   1 producer: cp.async issued   2 TMA: slot free   3 TMA: issued
-  //   5 MMA: slot full               6 MMA: issued + committed
-  // and from dbg[4096], 4 slots per work item (first 64): item start, neighbour map in smem, accumulators complete,
-  // epilogue stored; dbg[4096 + 256 ..]: kernel entry, prologue done, exit.
+                             float *__restrict__ out_f32, float *__restrict__ out_split) {
   using C = Cfg<CIN, COUT>;
-  constexpr int kMmaWarp = C::NPW, kTmaWarp = C::NPW + 1;
-  // Programmatic dependent launch: let the next kernel of the stream start its prologue while this grid drains, and
-  // (below) do this kernel's own prologue - barriers, TMEM, neighbour map - before waiting for the previous grid.
-  // Nothing read before griddepcontrol.wait is written by the preceding conv layer (row count, neighbour map and
-  // packed weights come from the rulebook / init kernels, which never signal early).
+  constexpr int S = C::STAGES;
+  // Programmatic dependent launch: let the next kernel of the stream start its prologue while this grid drains.
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  asm volatile("griddepcontrol.wait;" ::: "memory");  // inputs of the previous layer are complete
   const long long n = n_out_dev ? min(static_cast<long long>(n_out_dev[0]), n_cap) : n_cap;
   // work items w = tile * splits + split; split s owns the taps t == s (mod splits) and, when splits > 1, writes raw
   // partial sums to slab s of out_f32 (the caller passes the scratch slabs and no epilogue operands).
@@ -154,43 +78,20 @@ __global__ void __launch_bounds__(Cfg<CIN, COUT>::THREADS, Cfg<CIN, COUT>::MIN_C
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   int32_t *s_nbr = reinterpret_cast<int32_t *>(smem + C::STAGES * C::STAGE);  // [kM][K]
-  __shared__ __align__(8) unsigned long long s_bar[8 + 8 + 2];  // full[8] empty[8] tmem_full nbr_loaded
-  constexpr int kF = 0, kE = 8, kTF = 16, kNB = 17;
-  __shared__ uint32_t s_tmem_base;
+  __shared__ __align__(8) unsigned long long s_bar[8 + 1];  // full[8] (weights, and the rows with TMA) nbr_loaded
+  constexpr int kF = 0, kNB = 8;
   __shared__ uint32_t s_active;
 
-  const int tid = threadIdx.x, wid = tid >> 5, lane = tid & 31;
-  const bool dbg0 = dbg && blockIdx.x == 0 && tid == 0;
-  if (dbg0) dbg[4096 + 256] = clock64();
-  if (tid == kMmaWarp * 32) {
-    for (int s = 0; s < C::STAGES; ++s) {
-      // cp.async completions of every producer thread + the weight copy's expect_tx arrival; with the TMA gather the
-      // one expect_tx arrival covers rows and weights
-      mbar_init(smem_u32(&s_bar[kF + s]), TMA ? 1 : C::NPW * 32 + 1);
-      mbar_init(smem_u32(&s_bar[kE + s]), 1);                // tcgen05.commit
-    }
-    mbar_init(smem_u32(&s_bar[kTF]), 1);
+  const int tid = threadIdx.x, lane = tid & 31, wg = tid >> 7, wtid = tid & 127;
+  if (tid == 0) {
+    for (int s = 0; s < S; ++s) mbar_init(smem_u32(&s_bar[kF + s]), 1);
     mbar_init(smem_u32(&s_bar[kNB]), 1);
     fence_mbar_init();
   }
-  if (wid == kMmaWarp) {
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem_base)),
-                 "r"(static_cast<uint32_t>(C::TMEM_COLS))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem_base;
   const uint32_t ring = smem_u32(smem);
-  if (dbg0) dbg[4096 + 257] = clock64();
 
-  // Every role walks the stages 0, 1, .. of each work item in the same order and keeps the parity it expects next
-  // on each stage's barrier in a bit mask (bit s): the stage index depends on loop counters only.
-  uint32_t ph = (wid == kMmaWarp) ? 0u : 0xffffffffu;  // full-barrier waits start at parity 0, empty-barrier waits at 1
-  int use_base = 0;                                    // uses of earlier items (debug timeline index only)
+  uint32_t gu = 0;  // uses of earlier work items: the ring phases keep running
   int item_it = 0;
   for (long long w = blockIdx.x; w < n_work; w += gridDim.x, ++item_it) {
     const long long tile = w / splits;
@@ -203,12 +104,11 @@ __global__ void __launch_bounds__(Cfg<CIN, COUT>::THREADS, Cfg<CIN, COUT>::MIN_C
     }
     const long long row0 = tile * kM;
     const int rows = static_cast<int>(min(static_cast<long long>(kM), n - row0));
+    __syncthreads();  // previous item fully drained (s_nbr free)
     if (tid == 0) s_active = 0u;
-    __syncthreads();  // previous item fully drained (epilogue done, s_nbr free)
-    if (dbg0 && item_it < 64) dbg[4096 + item_it * 4] = clock64();
     {
       // the tile's neighbour map is one contiguous block of the [n_cap, K] array: one bulk copy instead of a
-      // latency-bound load loop (measured ~10k cycles per work item); rows >= `rows` of the block are never used.
+      // latency-bound load loop; rows >= `rows` of the block are never used.
       const int avail = static_cast<int>(min(static_cast<long long>(kM), n_cap - row0));
       const uint32_t words = static_cast<uint32_t>(avail) * K, bulk_words = words & ~3u;
       if (tid == 0) {
@@ -217,267 +117,149 @@ __global__ void __launch_bounds__(Cfg<CIN, COUT>::THREADS, Cfg<CIN, COUT>::MIN_C
         if (bulk_words) bulk_g2s(smem_u32(s_nbr), nbr + row0 * K, bulk_words * 4, smem_u32(&s_bar[kNB]));
       }
       if (bulk_words + tid < words) s_nbr[bulk_words + tid] = __ldg(nbr + row0 * K + bulk_words + tid);
-      if (bulk_words != words) __syncthreads();  // (uniform) the up-to-3 tail words are plain stores
+      __syncthreads();  // s_active reset and the up-to-3 tail words are plain stores
       mbar_wait(smem_u32(&s_bar[kNB]), static_cast<uint32_t>(item_it & 1));
       uint32_t mine = 0u;
-      for (int q = tid; q < rows * K; q += C::THREADS)
+      for (int q = tid; q < rows * K; q += kThreads)
         if (s_nbr[q] >= 0) mine |= 1u << (q % K);
       mine = __reduce_or_sync(0xffffffffu, mine);
       if (lane == 0 && mine) atomicOr(&s_active, mine);
     }
     __syncthreads();
     const uint32_t active = s_active & tap_mask;
-    if (item_it == 0) asm volatile("griddepcontrol.wait;" ::: "memory");  // inputs of the previous layer are complete
-    if (dbg0 && item_it < 64) dbg[4096 + item_it * 4 + 1] = clock64();
     const int n_uses = __popc(active) * C::G;
-    const int flags = dbg ? g_dbg_flags : 0;  // only the debug entry point passes dbg
 
-    if (wid < C::NPW) {
-      // ---------------------------------------------------------------- producers (cp.async gathers)
-      // FULL-LINE gathers (measured 36-72 B/clk/SM vs 11-19 for 64-byte pieces, tools/gather_microbench.cu): 8 lanes
-      // fetch one 128-byte line, a warp instruction covers 4 rows and lands on 512 (KC = 32) or 2 x 256 (KC = 16)
-      // contiguous bytes of the swizzled tiles: no bank conflicts.
-      const int sub = lane >> 3;
-      int s = 0, u = 0;
-      for (int t = 0; t < (TMA ? 0 : K); ++t) {  // (the TMA variant has no producer loop: warp NPW + 1 gathers)
-        if (!((active >> t) & 1u)) continue;
-        int src[C::QN];
-#pragma unroll
-        for (int q = 0; q < C::QN; ++q) {
-          const int row = wid * C::RPW + q * 4 + sub;
-          src[q] = row < rows ? s_nbr[row * K + t] : -1;
-        }
-        for (int g = 0; g < C::G; ++g, ++u) {
-          mbar_wait(smem_u32(&s_bar[kE + s]), (ph >> s) & 1u);
-          ph ^= 1u << s;
-          if (dbg0 && use_base + u < 512) dbg[(use_base + u) * 8 + 0] = clock64();
-          const uint32_t st = ring + static_cast<uint32_t>(s * C::STAGE);
-          if (C::KC == 32) {
-            // SWIZZLE_128B tiles (row pitch 128 B, chunk ^= row & 7); the hi and the lo line of a row
-            const int ch = lane & 7;
-#pragma unroll
-            for (int q = 0; q < C::QN; ++q) {
-              const bool ok = src[q] >= 0;
-              const int row = wid * C::RPW + q * 4 + sub;
-              const float *p = in_split + (ok ? static_cast<size_t>(src[q]) * (2 * CIN) : 0) + g * 32 + ch * 4;
-              const uint32_t d = st + static_cast<uint32_t>(row * 128 + ((ch ^ (row & 7)) << 4));
-              if (flags & 2) continue;
-              cp_async16(d, p, ok);                    // hi
-              cp_async16(d + C::A_TILE, p + CIN, ok);  // lo
-            }
-          } else {
-            // 16-channel layers: a split row [hi 16 | lo 16] is ONE line (lanes 0-3 of a row fetch the hi chunks,
-            // 4-7 the lo chunks); SWIZZLE_64B tiles (row pitch 64 B, chunk ^= (row >> 1) & 3)
-            const int ch = lane & 3, part = (lane >> 2) & 1;
-#pragma unroll
-            for (int q = 0; q < C::QN; ++q) {
-              const bool ok = src[q] >= 0;
-              const int row = wid * C::RPW + q * 4 + sub;
-              const float *p = in_split + (ok ? static_cast<size_t>(src[q]) * (2 * CIN) : 0) + part * CIN + g * 16 + ch * 4;
-              const uint32_t d = st + static_cast<uint32_t>(part * C::A_TILE + row * 64 + ((ch ^ ((row >> 1) & 3)) << 4));
-              if (flags & 2) continue;
-              cp_async16(d, p, ok);
-            }
-          }
-          cp_async_arrive_noinc(smem_u32(&s_bar[kF + s]));
-          if (dbg0 && use_base + u < 512) dbg[(use_base + u) * 8 + 1] = clock64();
-          s = (s + 1 == C::STAGES) ? 0 : s + 1;
-        }
+    // gather use q (tap, chunk) of this item into its ring slot; thread 0 posts the weight slice (and the row bytes
+    // of the TMA gather) on the slot's barrier
+    auto issue = [&](int q) {
+      if (q >= n_uses) return;
+      const int t = nth_bit(active, q / C::G), g = q % C::G;
+      const uint32_t slot = (gu + static_cast<uint32_t>(q)) % S;
+      const uint32_t st = ring + slot * C::STAGE, bar = smem_u32(&s_bar[kF + slot]);
+      if (tid == 0) {
+        mbar_arrive_expect_tx(bar, static_cast<uint32_t>((TMA ? C::A_STAGE : 0) + C::B_STAGE));
+        bulk_g2s(st + C::A_STAGE, packed_w + (static_cast<size_t>(t) * CIN + g * C::KC) * (2 * COUT),
+                 static_cast<uint32_t>(C::B_STAGE), bar);
       }
-      // ---------------------------------------------------------------- epilogue
-      mbar_wait(smem_u32(&s_bar[kTF]), static_cast<uint32_t>(item_it & 1));
-      tc_fence_after();
-      if (dbg0 && item_it < 64) dbg[4096 + item_it * 4 + 2] = clock64();
-      // warp w reads TMEM lanes 32 * (w & 3) ..; with 8 epilogue warps the two warps of a lane quarter take
-      // alternate 16-column chunks
-      const int quarter = wid & 3;
-      const int r = quarter * 32 + lane;
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-      const bool live = r < rows;
-      const size_t orow = static_cast<size_t>(row0 + r);
-#pragma unroll 1
-      for (int c0 = (wid >> 2) * 16; c0 < COUT; c0 += 16 * (C::NPW / 4)) {
-        uint32_t a[16];
-        if (n_uses > 0) {
-          asm volatile(
-              "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
-              "%15}, [%16];"
-              : "=r"(a[0]), "=r"(a[1]), "=r"(a[2]), "=r"(a[3]), "=r"(a[4]), "=r"(a[5]), "=r"(a[6]), "=r"(a[7]),
-                "=r"(a[8]), "=r"(a[9]), "=r"(a[10]), "=r"(a[11]), "=r"(a[12]), "=r"(a[13]), "=r"(a[14]), "=r"(a[15])
-              : "r"(taddr + static_cast<uint32_t>(c0)));
-#pragma unroll
-          for (int acc = 1; acc < 3; ++acc) {
-            uint32_t b[16];
-            asm volatile(
-                "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
-                "%15}, [%16];"
-                : "=r"(b[0]), "=r"(b[1]), "=r"(b[2]), "=r"(b[3]), "=r"(b[4]), "=r"(b[5]), "=r"(b[6]), "=r"(b[7]),
-                  "=r"(b[8]), "=r"(b[9]), "=r"(b[10]), "=r"(b[11]), "=r"(b[12]), "=r"(b[13]), "=r"(b[14]), "=r"(b[15])
-                : "r"(taddr + static_cast<uint32_t>(acc * COUT + c0)));
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-            for (int j = 0; j < 16; ++j) a[j] = __float_as_uint(__uint_as_float(a[j]) + __uint_as_float(b[j]));
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) a[j] = 0u;
-        }
-        if (live) {
-          float o[16], res[16];
-          if (residual_split) {
-            const float4 *rh = reinterpret_cast<const float4 *>(residual_split + orow * (2 * COUT) + c0);
-            const float4 *rl = reinterpret_cast<const float4 *>(residual_split + orow * (2 * COUT) + COUT + c0);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const float4 h = __ldg(rh + j), l = __ldg(rl + j);
-              res[4 * j] = h.x + l.x;
-              res[4 * j + 1] = h.y + l.y;
-              res[4 * j + 2] = h.z + l.z;
-              res[4 * j + 3] = h.w + l.w;
-            }
-          }
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            float v = __uint_as_float(a[j]);
-            if (scale) v = v * __ldg(scale + c0 + j);
-            if (shift) v = v + __ldg(shift + c0 + j);
-            if (residual_split) v = v + res[j];
-            if (relu) v = fmaxf(v, 0.f);
-            o[j] = v;
-          }
-          if (out_rows) {
-#pragma unroll
-            for (int j = 0; j < 16; j += 4)
-              *reinterpret_cast<float4 *>(out_rows + orow * COUT + c0 + j) = make_float4(o[j], o[j + 1], o[j + 2], o[j + 3]);
-          }
-          if (out_split) {
-            float h[16], l[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) split_tf32(o[j], h[j], l[j]);
-#pragma unroll
-            for (int j = 0; j < 16; j += 4) {
-              *reinterpret_cast<float4 *>(out_split + orow * (2 * COUT) + c0 + j) = make_float4(h[j], h[j + 1], h[j + 2], h[j + 3]);
-              *reinterpret_cast<float4 *>(out_split + orow * (2 * COUT) + COUT + c0 + j) =
-                  make_float4(l[j], l[j + 1], l[j + 2], l[j + 3]);
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      if (dbg0 && item_it < 64) dbg[4096 + item_it * 4 + 3] = clock64();
-    } else if (wid == kMmaWarp) {
-      // ---------------------------------------------------------------- MMA issuer (whole warp runs the stream)
-      // the warp-reduction result lives in a uniform register: trip count, stage index and with them the operand
-      // descriptors stay on the uniform datapath (no per-MMA R2UR of descriptor words)
-      const int n_uses_u = __popc(__reduce_or_sync(0xffffffffu, active)) * C::G;
-      if (n_uses_u == 0) {
-        if (lane == 0) mbar_arrive(smem_u32(&s_bar[kTF]));
-      } else {
-        int s = 0;
-        for (int u = 0; u < n_uses_u; ++u) {
-          mbar_wait(smem_u32(&s_bar[kF + s]), (ph >> s) & 1u);
-          ph ^= 1u << s;
-          if (dbg && blockIdx.x == 0 && lane == 0 && use_base + u < 512) dbg[(use_base + u) * 8 + 5] = clock64();
-          if (!(flags & 8)) fence_proxy_async();  // cp.async (generic proxy) writes -> tensor-core (async proxy) reads
-          tc_fence_after();
-          const uint32_t a_hi = ring + static_cast<uint32_t>(s * C::STAGE), a_lo = a_hi + C::A_TILE;
-          const uint32_t b_all = a_hi + C::A_STAGE;
-#pragma unroll
-          for (int j = 0; j < C::KC / 8; ++j) {
-            // k-step j: 16-channel block j / 2, chunk pair (j & 1) inside it
-            const uint32_t bo = static_cast<uint32_t>(2 * j) * (2 * COUT * 16);
-            uint64_t dah, dal;
-            if (C::KC == 32) {  // SWIZZLE_128B tiles: k-step j starts 32 bytes further into the 128-byte rows
-              dah = smem_desc_sw128(a_hi + j * 32);
-              dal = smem_desc_sw128(a_lo + j * 32);
-            } else {            // SWIZZLE_64B tiles (16-channel layers)
-              dah = smem_desc_sw64(a_hi + j * 32);
-              dal = smem_desc_sw64(a_lo + j * 32);
-            }
-            const uint64_t db = smem_desc(b_all + bo, 2 * COUT * 16, 128);  // rows 0..N-1 = hi, N..2N-1 = lo
-            const uint32_t first = (u | j) ? 1u : 0u;
-            if (flags & 4) continue;
-            umma_tf32_elect(tmem_base, dah, db, C::IDESC2, first);             // A_hi x [B_hi | B_lo]
-            umma_tf32_elect(tmem_base + 2 * COUT, dal, db, C::IDESC, first);   // A_lo x B_hi
-          }
-          if (flags & 16) {
-            if (lane == 0) {
-              mbar_arrive(smem_u32(&s_bar[kE + s]));
-              if (u == n_uses_u - 1) mbar_arrive(smem_u32(&s_bar[kTF]));
-            }
-            __syncwarp();
-          } else {
-            umma_commit_elect(smem_u32(&s_bar[kE + s]));
-            if (u == n_uses_u - 1) umma_commit_elect(smem_u32(&s_bar[kTF]));
-          }
-          if (dbg && blockIdx.x == 0 && lane == 0 && use_base + u < 512) dbg[(use_base + u) * 8 + 6] = clock64();
-          s = (s + 1 == C::STAGES) ? 0 : s + 1;
-        }
-      }
-      tc_fence_before();
-    } else {
-      // ---------------------------------------------------------------- weight TMA (one lane)
       if (TMA) {
-        // whole warp: lane l gathers rows 4l .. 4l+3 of the tile (hi line and lo line of the 32-channel slice), lane 0
-        // also posts the byte count and copies the weights of the use
-        int s = 0, u = 0;
-        for (int t = 0; t < K; ++t) {
-          if (!((active >> t) & 1u)) continue;
-          int r[4];
+        if (tid < 32) {
+          __syncwarp();  // expect_tx is posted before any row can complete
 #pragma unroll
-          for (int q = 0; q < 4; ++q) r[q] = (lane * 4 + q) < rows ? s_nbr[(lane * 4 + q) * K + t] : -1;
-          for (int g = 0; g < C::G; ++g, ++u) {
-            mbar_wait(smem_u32(&s_bar[kE + s]), (ph >> s) & 1u);
-            ph ^= 1u << s;
-            const uint32_t st = ring + static_cast<uint32_t>(s * C::STAGE), bar = smem_u32(&s_bar[kF + s]);
-            if (lane == 0) {
-              if (dbg && blockIdx.x == 0 && use_base + u < 512) dbg[(use_base + u) * 8 + 2] = clock64();
-              mbar_arrive_expect_tx(bar, static_cast<uint32_t>(((flags & 2) ? 0 : C::A_STAGE) + ((flags & 1) ? 0 : C::B_STAGE)));
-              if (!(flags & 1))
-                bulk_g2s(st + C::A_STAGE, packed_w + (static_cast<size_t>(t) * CIN + g * C::KC) * (2 * COUT),
-                         static_cast<uint32_t>(C::B_STAGE), bar);
-            }
-            __syncwarp();
-            if (!(flags & 2)) {
-              tma_gather4(st + lane * 512, &in_map, g * 32, r[0], r[1], r[2], r[3], bar);                    // hi
-              tma_gather4(st + C::A_TILE + lane * 512, &in_map, CIN + g * 32, r[0], r[1], r[2], r[3], bar);  // lo
-            }
-            if (dbg && blockIdx.x == 0 && lane == 0 && use_base + u < 512) dbg[(use_base + u) * 8 + 3] = clock64();
-            s = (s + 1 == C::STAGES) ? 0 : s + 1;
+          for (int k = 0; k < 4; ++k) {
+            const int row = lane * 4 + k;
+            const int src = row < rows ? s_nbr[row * K + t] : -1;
+            tma_row(st + row * 128, &in_map, g * 32, src, bar);                   // hi
+            tma_row(st + C::A_TILE + row * 128, &in_map, CIN + g * 32, src, bar);  // lo
           }
         }
-      } else if (lane == 0) {
-        int s = 0, u = 0;
-        for (int t = 0; t < K; ++t) {
-          if (!((active >> t) & 1u)) continue;
-          for (int g = 0; g < C::G; ++g, ++u) {
-            mbar_wait(smem_u32(&s_bar[kE + s]), (ph >> s) & 1u);
-            ph ^= 1u << s;
-            if (dbg && blockIdx.x == 0 && use_base + u < 512) dbg[(use_base + u) * 8 + 2] = clock64();
-            if (flags & 1) {
-              mbar_arrive(smem_u32(&s_bar[kF + s]));
-            } else {
-              mbar_arrive_expect_tx(smem_u32(&s_bar[kF + s]), static_cast<uint32_t>(C::B_STAGE));
-              bulk_g2s(ring + static_cast<uint32_t>(s * C::STAGE + C::A_STAGE),
-                       packed_w + (static_cast<size_t>(t) * CIN + g * C::KC) * (2 * COUT), static_cast<uint32_t>(C::B_STAGE),
-                       smem_u32(&s_bar[kF + s]));
-            }
-            if (dbg && blockIdx.x == 0 && use_base + u < 512) dbg[(use_base + u) * 8 + 3] = clock64();
-            s = (s + 1 == C::STAGES) ? 0 : s + 1;
-          }
+        return;
+      }
+      const int sub = tid >> 3;  // 32 rows per CTA instruction
+      if (C::KC == 32) {
+        // SWIZZLE_128B tiles (row pitch 128 B, chunk ^= row & 7); the hi and the lo line of a row
+        const int ch = tid & 7;
+#pragma unroll
+        for (int q4 = 0; q4 < 4; ++q4) {
+          const int row = q4 * 32 + sub;
+          const int src = row < rows ? s_nbr[row * K + t] : -1;
+          const bool ok = src >= 0;
+          const float *p = in_split + (ok ? static_cast<size_t>(src) * (2 * CIN) : 0) + g * 32 + ch * 4;
+          const uint32_t d = st + static_cast<uint32_t>(row * 128 + ((ch ^ (row & 7)) << 4));
+          cp_async16(d, p, ok);                    // hi
+          cp_async16(d + C::A_TILE, p + CIN, ok);  // lo
         }
+      } else {
+        // 16-channel layers: a split row [hi 16 | lo 16] is ONE line (threads 0-3 of a row fetch the hi chunks,
+        // 4-7 the lo chunks); SWIZZLE_64B tiles (row pitch 64 B, chunk ^= (row >> 1) & 3)
+        const int ch = tid & 3, part = (tid >> 2) & 1;
+#pragma unroll
+        for (int q4 = 0; q4 < 4; ++q4) {
+          const int row = q4 * 32 + sub;
+          const int src = row < rows ? s_nbr[row * K + t] : -1;
+          const bool ok = src >= 0;
+          const float *p = in_split + (ok ? static_cast<size_t>(src) * (2 * CIN) : 0) + part * CIN + g * 16 + ch * 4;
+          const uint32_t d = st + static_cast<uint32_t>(part * C::A_TILE + row * 64 + ((ch ^ ((row >> 1) & 3)) << 4));
+          cp_async16(d, p, ok);
+        }
+      }
+    };
+
+    float acc[C::ACC], accx[C::ACC];  // hi x hi | cross terms
+#pragma unroll
+    for (int i = 0; i < C::ACC; ++i) acc[i] = accx[i] = 0.f;
+    for (int q = 0; q < S - 1; ++q) {
+      issue(q);
+      cp_async_commit();
+    }
+    for (int u = 0; u < n_uses; ++u) {
+      const uint32_t slot = (gu + static_cast<uint32_t>(u)) % S, par = ((gu + static_cast<uint32_t>(u)) / S) & 1u;
+      cp_async_wait<S - 2>();  // this thread's gathers of use u have landed
+      fence_proxy_async();     // cp.async (generic proxy) writes -> wgmma (async proxy) reads
+      mbar_wait(smem_u32(&s_bar[kF + slot]), par);
+      __syncthreads();         // whole stage present; the wgmma of use u - 1 have retired in both warpgroups
+      const uint32_t a_hi = ring + slot * C::STAGE, a_lo = a_hi + C::A_TILE;
+      const uint32_t b_hi = a_hi + C::A_STAGE, b_lo = b_hi + COUT * 16;  // rows 0..N-1 = hi, N..2N-1 = lo
+      const uint32_t a_wg = static_cast<uint32_t>(wg * 64 * (C::KC * 4));  // this warpgroup's 64 rows
+      wg_fence();
+#pragma unroll
+      for (int j = 0; j < C::KC / 8; ++j) {
+        // k-step j: 32 bytes further into the swizzled rows; B: 16-channel block j / 2, chunk pair (j & 1) inside it
+        const uint32_t bo = static_cast<uint32_t>(2 * j) * (2 * COUT * 16);
+        uint64_t dah, dal;
+        if (C::KC == 32) {
+          dah = desc_sw128(a_hi + a_wg + j * 32);
+          dal = desc_sw128(a_lo + a_wg + j * 32);
+        } else {
+          dah = desc_sw64(a_hi + a_wg + j * 32);
+          dal = desc_sw64(a_lo + a_wg + j * 32);
+        }
+        const uint64_t dbh = smem_desc(b_hi + bo, 2 * COUT * 16, 128), dbl = smem_desc(b_lo + bo, 2 * COUT * 16, 128);
+        wg::mma_tf32<COUT>(accx, dal, dbh, 1u);  // A_lo x B_hi
+        wg::mma_tf32<COUT>(accx, dah, dbl, 1u);  // A_hi x B_lo
+        wg::mma_tf32<COUT>(acc, dah, dbh, 1u);  // A_hi x B_hi
+      }
+      wg_commit();
+      issue(u + S - 1);  // the slot of use u - 1
+      cp_async_commit();
+      wg_wait<0>();
+    }
+    wg_fence_acc<C::ACC>(acc);
+    wg_fence_acc<C::ACC>(accx);
+    cp_async_wait<0>();
+    gu += static_cast<uint32_t>(n_uses);
+
+    // ---------------------------------------------------------------- epilogue (accumulator fragment)
+#pragma unroll
+    for (int i = 0; i < C::ACC; i += 2) {
+      const int r = wg * 64 + frag_row(i, wtid), c = frag_col(i, wtid);
+      if (r >= rows) continue;
+      const size_t orow = static_cast<size_t>(row0 + r);
+      float o[2] = {accx[i] + acc[i], accx[i + 1] + acc[i + 1]};
+      float res[2] = {0.f, 0.f};
+      if (residual_split) {
+        const float2 h = __ldg(reinterpret_cast<const float2 *>(residual_split + orow * (2 * COUT) + c));
+        const float2 l = __ldg(reinterpret_cast<const float2 *>(residual_split + orow * (2 * COUT) + COUT + c));
+        res[0] = h.x + l.x;
+        res[1] = h.y + l.y;
+      }
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        float v = o[e];
+        if (scale) v = v * __ldg(scale + c + e);
+        if (shift) v = v + __ldg(shift + c + e);
+        if (residual_split) v = v + res[e];
+        if (relu) v = fmaxf(v, 0.f);
+        o[e] = v;
+      }
+      if (out_rows) *reinterpret_cast<float2 *>(out_rows + orow * COUT + c) = make_float2(o[0], o[1]);
+      if (out_split) {
+        float h[2], l[2];
+        split_tf32(o[0], h[0], l[0]);
+        split_tf32(o[1], h[1], l[1]);
+        *reinterpret_cast<float2 *>(out_split + orow * (2 * COUT) + c) = make_float2(h[0], h[1]);
+        *reinterpret_cast<float2 *>(out_split + orow * (2 * COUT) + COUT + c) = make_float2(l[0], l[1]);
       }
     }
-    use_base += n_uses;
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (dbg0) dbg[4096 + 258] = clock64();
-  if (wid == kMmaWarp) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"(static_cast<uint32_t>(C::TMEM_COLS))
-                 : "memory");
   }
 }
 
@@ -507,8 +289,7 @@ inline int make_rows_map(const float *rows, int64_t n_rows, int C, CUtensorMap *
 template <int CIN, int COUT, bool TMA = false>
 int launch(const float *in_split, const int32_t *nbr, const int32_t *n_out_dev, int64_t n_cap, int K,
            const float *packed, const float *scale, const float *shift, const float *residual_split, int relu,
-           float *out_f32, float *out_split, cudaStream_t st, long long *dbg = nullptr, int splits = 1,
-           int64_t n_in_rows = 0) {
+           float *out_f32, float *out_split, cudaStream_t st, int splits = 1, int64_t n_in_rows = 0) {
   using C = Cfg<CIN, COUT>;
   CUtensorMap in_map = {};
   if (TMA) {
@@ -521,12 +302,12 @@ int launch(const float *in_split, const int32_t *nbr, const int32_t *n_out_dev, 
   auto kern = gather_gemm_split_kernel<CIN, COUT, TMA>;
   P3D_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   const long long work = ((n_cap + kM - 1) / kM) * splits;
-  const long long slots = static_cast<long long>(kNumSMs) * C::MIN_CTAS;
+  const long long slots = static_cast<long long>(num_sms()) * C::MIN_CTAS;
   const unsigned int grid = static_cast<unsigned int>(work < slots ? work : slots);
   static const bool pdl = !(getenv("P3D_PDL") && atoi(getenv("P3D_PDL")) == 0);  // tuning hook, default on
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(C::THREADS);
+  cfg.blockDim = dim3(kThreads);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
   cudaLaunchAttribute attr[1];
@@ -536,7 +317,7 @@ int launch(const float *in_split, const int32_t *nbr, const int32_t *n_out_dev, 
   cfg.numAttrs = pdl ? 1 : 0;
   const long long n_cap_ll = n_cap;
   P3D_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, in_map, in_split, nbr, n_out_dev, n_cap_ll, K, splits, packed, scale, shift,
-                                    residual_split, relu, out_f32, out_split, dbg));
+                                    residual_split, relu, out_f32, out_split));
   P3D_LAUNCH_CHECK();
   return P3D_OK;
 }
@@ -663,11 +444,11 @@ static int split_conv(const float *in_split, int64_t n_in_rows, bool tma, const 
 #define P3D_TC2_CASE(CI, CO)                                                                                           \
   if (!tma && Cin == CI && Cout == CO)                                                                                 \
     rc = tc2::launch<CI, CO>(in_split, nbr, n_out_dev, n_out_cap, K, packed_weight, k_scale, k_shift, k_res, k_relu,    \
-                             k_f32, k_split, st, nullptr, k_splits);
+                             k_f32, k_split, st, k_splits);
 #define P3D_TC2_TMA_CASE(CI, CO)                                                                                       \
   if (tma && Cin == CI && Cout == CO)                                                                                  \
     rc = tc2::launch<CI, CO, true>(in_split, nbr, n_out_dev, n_out_cap, K, packed_weight, k_scale, k_shift, k_res,      \
-                                   k_relu, k_f32, k_split, st, nullptr, k_splits, n_in_rows);
+                                   k_relu, k_f32, k_split, st, k_splits, n_in_rows);
   P3D_TC2_CASE(16, 16)
   P3D_TC2_CASE(16, 32)
   P3D_TC2_CASE(32, 32)
@@ -687,7 +468,7 @@ static int split_conv(const float *in_split, int64_t n_in_rows, bool tma, const 
   {
     static const bool pdl = !(getenv("P3D_PDL") && atoi(getenv("P3D_PDL")) == 0);
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(static_cast<unsigned int>(fin_blocks < kNumSMs * 8 ? fin_blocks : kNumSMs * 8));
+    cfg.gridDim = dim3(static_cast<unsigned int>(fin_blocks < num_sms() * 8 ? fin_blocks : num_sms() * 8));
     cfg.blockDim = dim3(256);
     cfg.stream = st;
     cudaLaunchAttribute attr[1];
@@ -731,29 +512,4 @@ extern "C" int p3d_sparse_conv_gather_gemm_split(const float *in_split, const in
                                                  int relu, float *out_f32, float *out_split, p3d_stream_t stream) {
   return p3d_sparse_conv_gather_gemm_split_ws(in_split, nbr, n_out_dev, n_out_cap, K, Cin, Cout, packed_weight, scale,
                                               shift, residual_split, relu, out_f32, out_split, nullptr, 0, stream);
-}
-
-// Debug aid (not part of the public header): the launch of p3d_sparse_conv_gather_gemm_split with a clock64 timeline of
-// CTA 0 written to dbg[4096 + 260] (layout in the kernel's header comment); tools/split_probe.py reads it.
-extern "C" int p3d_debug_split_launch(const float *in_split, const int32_t *nbr, const int32_t *n_out_dev,
-                                      int64_t n_out_cap, int K, int Cin, int Cout, const float *packed_weight,
-                                      float *out_f32, long long *dbg, int splits, p3d_stream_t stream) {
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-#define P3D_TC2_CASE(CI, CO)                                                                                          \
-  if (Cin == CI && Cout == CO)                                                                                        \
-    return tc2::launch<CI, CO>(in_split, nbr, n_out_dev, n_out_cap, K, packed_weight, nullptr, nullptr, nullptr, 0,   \
-                               out_f32, nullptr, st, dbg, splits);
-  P3D_TC2_CASE(16, 16)
-  P3D_TC2_CASE(16, 32)
-  P3D_TC2_CASE(32, 32)
-  P3D_TC2_CASE(32, 64)
-  P3D_TC2_CASE(64, 64)
-  P3D_TC2_CASE(64, 128)
-  P3D_TC2_CASE(128, 128)
-#undef P3D_TC2_CASE
-  return P3D_ERR_UNSUPPORTED;
-}
-
-extern "C" int p3d_debug_set_flags(int flags) {
-  return cudaMemcpyToSymbol(tc2::g_dbg_flags, &flags, sizeof(int)) == cudaSuccess ? 0 : -3;
 }

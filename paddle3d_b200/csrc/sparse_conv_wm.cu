@@ -1,9 +1,8 @@
 // Sparse-conv gather-GEMM for the NARROW layers (Cin, Cout <= 32) on fp16 hi/lo' pair rows: register gather + warp MMA.
 //
-// Why a second kernel next to sparse_conv_f16.cu (tcgen05): on the 16- and 32-channel levels the tcgen05 pipeline is
-// bound by what it costs to stage a gathered row in shared memory, not by the tensor pipe (profiles/r02_f16_sweep.md:
-// a missing neighbour costs a full cp.async slot, 55 % of the slots are missing neighbours, one full/empty mbarrier
-// round trip per 2-4 taps) - a level-0 layer takes 44 us for 0.38 GFLOP.  Here nothing is staged:
+// Why a second kernel next to sparse_conv_f16.cu (wgmma): on the 16- and 32-channel levels the staged pipeline is
+// bound by what it costs to stage a gathered row in shared memory, not by the tensor pipe (a missing neighbour costs a
+// full cp.async slot, and most slots of the narrow levels are missing neighbours).  Here nothing is staged:
 //
 //   * the product is computed TRANSPOSED, out^T[cout][row] = W^T[cout][k] x X^T[k][row] with mma.sync.m16n8k16: the
 //     weights are the A operand (16 output channels x 16 k), 8 gathered rows are the B operand.  A lane's B fragment
@@ -17,15 +16,15 @@
 //     compile-time slots ("groups" of up to D taps of one tile) that prefetches across tile boundaries; the neighbour
 //     indices of the next tile are staged with cp.async while the current one is computed;
 //   * work is cut stream-K style: the (tile, tap) units are divided into one equal contiguous range per warp of the grid
-//     (no wave quantisation: 2471 tiles on 2368 warps would otherwise take two rounds); a tile cut by a range boundary
+//     (no wave quantisation: a few more tiles than warps would otherwise take two rounds); a tile cut by a range boundary
 //     is summed by the LAST warp to finish it (ticket), pieces in warp order -> deterministic;
-//   * products exactly as the tcgen05 kernel: acc_m += hi x hi, acc_l += hi x lo' + lo' x hi (fp32 accumulators),
+//   * products exactly as the wgmma kernel: acc_m += hi x hi, acc_l += hi x lo' + lo' x hi (fp32 accumulators),
 //     out = acc_m + acc_l * 2^-11, then the same fused BN / bias / residual / ReLU epilogue (transposed back through a
 //     per-warp shared-memory tile so that rows are read and written 16 bytes at a time) and the same H16 / fp32 outputs:
 //     a drop-in for p3d_sparse_conv_f16 on these shapes.
 //
-// The tcgen05 pipe is irrelevant at these widths (N = 16/32): the bounds are the L2 gather (pairs x 4 Cin bytes), the
-// issue slots of the gather loop and, for 32 -> 32, the legacy HMMA rate - see DESIGN.md section 3 / 6.
+// The tensor pipe is irrelevant at these widths (N = 16/32): the bounds are the L2 gather (pairs x 4 Cin bytes), the
+// issue slots of the gather loop and, for 32 -> 32, the mma.sync rate.
 #include <cuda_fp16.h>
 #include <stdlib.h>
 
@@ -431,7 +430,7 @@ int launch(const Params &p, cudaStream_t st) {
   auto kern = conv_wm_kernel<CIN, COUT, D>;
   P3D_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   const long long blocks_needed = (p.n_cap + 16 * kWarps - 1) / (16 * kWarps);
-  long long grid = kNumSMs;
+  long long grid = num_sms();
   if (grid > blocks_needed) grid = blocks_needed;
   if (grid < 1) grid = 1;
   P3D_CUDA_CHECK(launch_pdl(kern, dim3(static_cast<unsigned int>(grid)), dim3(kWarps * 32), smem, st, p));
@@ -469,7 +468,7 @@ extern "C" size_t p3d_sparse_conv_wm_workspace_bytes(int64_t n_out_cap, int Cout
   if (n_out_cap <= 0 || Cout < 16) return 0;
   const size_t tiles = static_cast<size_t>((n_out_cap + 15) / 16);
   return align_up(tiles * sizeof(int32_t)) +
-         align_up(static_cast<size_t>(kNumSMs) * wm::kWarps * 2 * (Cout / 2) * 32 * sizeof(float));
+         align_up(static_cast<size_t>(num_sms()) * wm::kWarps * 2 * (Cout / 2) * 32 * sizeof(float));
 }
 
 extern "C" int p3d_sparse_conv_wm(const void *in_h16, const int32_t *nbr, const int32_t *n_out_dev, int64_t n_out_cap,
@@ -504,7 +503,7 @@ extern "C" int p3d_sparse_conv_wm(const void *in_h16, const int32_t *nbr, const 
   p.slabs = reinterpret_cast<float *>(static_cast<char *>(workspace) + align_up(static_cast<size_t>((n_out_cap + 15) / 16) * sizeof(int32_t)));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   static const int d_env = getenv("P3D_WM_D") ? atoi(getenv("P3D_WM_D")) : 0;  // tuning hook: ring depth
-  if (Cin == 16 && Cout == 16) {  // measured per level-0 layer: D = 3 25.5 us, D = 5 25.0 us, D = 9 27.0 us
+  if (Cin == 16 && Cout == 16) {
     if (d_env == 3) return wm::launch<16, 16, 3>(p, st);
     if (d_env == 9) return wm::launch<16, 16, 9>(p, st);
     return wm::launch<16, 16, 5>(p, st);
@@ -514,7 +513,7 @@ extern "C" int p3d_sparse_conv_wm(const void *in_h16, const int32_t *nbr, const 
     if (d_env == 9) return wm::launch<16, 32, 7>(p, st);
     return wm::launch<16, 32, 5>(p, st);
   }
-  if (Cin == 32 && Cout == 32) {  // measured: D = 3 33.4 us, D = 4 (8 bytes of spills) 35.4 us per level-1 layer
+  if (Cin == 32 && Cout == 32) {  // D = 4 spills 8 bytes
     if (d_env == 4) return wm::launch<32, 32, 4>(p, st);
     return wm::launch<32, 32, 3>(p, st);
   }

@@ -1,16 +1,16 @@
-// PTX helpers shared by the tcgen05 kernels (sm_100a): mbarrier, cp.async(.bulk), tcgen05.mma/commit/ld, UMMA
-// shared-memory descriptors (cute::UMMA::SmemDescriptor bit layout), tf32 hi/lo split.
+// PTX helpers shared by the tensor-core kernels (sm_90a): mbarrier, cp.async(.bulk), wgmma descriptors / fences,
+// the m64nN accumulator fragment, tf32 hi/lo split.
 #pragma once
 #include <stdlib.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace p3d {
 namespace tc {
 
-constexpr int kM = 128;
-constexpr int kProducers = 128;
-constexpr int kThreads = 192;  // 4 producer/epilogue warps + 1 MMA warp + 1 weight-TMA warp
+constexpr int kM = 128;       // rows of a tile: two warpgroups, 64 rows (one wgmma M) each
+constexpr int kThreads = 256;  // the two warpgroups; every thread gathers, issues wgmma and runs the epilogue
 
 __host__ __device__ constexpr int kc_of(int cin) { return cin < 16 ? cin : 16; }  // channels per pipeline stage
 
@@ -30,8 +30,7 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t byt
 #endif
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   // try_wait with a suspend-time hint: the thread sleeps in hardware until the phase completes (or ~20 us pass)
-  // instead of polling - with the short default limit the waiting warps executed ~70 % of all instructions of the
-  // sparse-conv kernels (ncu: 1400 warp instructions per pipeline use, issue slots 50 % busy).
+  // instead of polling, so waiting warps do not take issue slots from the ones doing the work.
   uint32_t done;
   int spins = 0;
   do {
@@ -47,38 +46,57 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
                "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
 
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void *src, bool valid) {
+  const uint32_t sz = valid ? 16u : 0u;  // src-size 0 => 16 bytes of zeros
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(sz) : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+// wgmma: fence before the first wgmma that touches freshly written accumulator registers, commit the issued wgmmas as
+// one group, wait until at most N groups of this warp are in flight.
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous wgmma
+template <int R>
+__device__ __forceinline__ void wg_fence_acc(float *d) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// K-major, no swizzle: core matrix = 8 rows x 16 B contiguous; LBO = distance between the two 16-byte
-// K-chunks of one MMA (K = 8 tf32), SBO = distance between 8-row groups (cute::UMMA::SmemDescriptor).
-__device__ __forceinline__ uint64_t smem_desc(uint32_t addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// wgmma shared-memory matrix descriptor: start address, leading / stride byte offsets, layout (0 no swizzle,
+// 1 SWIZZLE_128B, 2 SWIZZLE_64B, 3 SWIZZLE_32B).  K-major, no swizzle: core matrix = 8 rows x 16 B contiguous; LBO =
+// distance between the two 16-byte K-chunks of one k-step, SBO = distance between 8-row groups.  K-major swizzled: LBO
+// unused (1), SBO = 8 rows x row pitch; the swizzle is applied to the absolute shared-memory address, so a start
+// address advanced by k-steps (or by whole rows) reads what TMA / the XOR-ing producers wrote.
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t addr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout,
+                                              uint32_t base_offset = 0) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((addr & 0x3ffffu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3fffu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3fffu) << 32;
-  d |= 1ull << 46;  // descriptor version 1 (Blackwell)
-  return d;         // base_offset 0, lbo_mode 0, layout_type 0 = SWIZZLE_NONE
+  d |= static_cast<uint64_t>(base_offset & 7u) << 49;
+  d |= static_cast<uint64_t>(layout) << 62;
+  return d;
 }
+__device__ __forceinline__ uint64_t smem_desc(uint32_t addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  return gmma_desc(addr, lbo_bytes, sbo_bytes, 0);
+}
+__device__ __forceinline__ uint64_t desc_sw128(uint32_t addr, uint32_t sbo_bytes = 1024) { return gmma_desc(addr, 16, sbo_bytes, 1); }
+__device__ __forceinline__ uint64_t desc_sw64(uint32_t addr) { return gmma_desc(addr, 16, 512, 2); }
+
+// Position of accumulator element i of an m64nN fragment inside the warpgroup's 64 x N block (wgmma.cuh).
+__device__ __forceinline__ int frag_row(int i, int wg_tid) { return ((wg_tid >> 5) << 4) + ((wg_tid & 31) >> 2) + (((i >> 1) & 1) << 3); }
+__device__ __forceinline__ int frag_col(int i, int wg_tid) { return ((i >> 2) << 3) + ((wg_tid & 3) << 1) + (i & 1); }
 
 __device__ __forceinline__ void split_tf32(float x, float &hi, float &lo) {
   uint32_t h;

@@ -1,4 +1,4 @@
-// hard_voxelize for sm_100a — deterministic, CPU-semantics exact.
+// hard_voxelize for sm_90a — deterministic, CPU-semantics exact.
 //
 // Replaces the reference's 7-kernel + cumsum pipeline over three dense 332 MB grids
 // (paddle3d/ops/voxel/voxelize_op.cu:208-346) with a hash of the occupied cells only:
@@ -24,7 +24,7 @@
 //                      This is the HBM-roofline kernel: 4NF + 4VPF + 12V + 4V algorithmic bytes.
 //
 // All intermediate state (8*cap + 4*(N + cap + V*(2P + C + 1)) bytes, of which only the rows of live voxels are touched)
-// is L2-resident on B200.
+// is L2-resident on an H100 (50 MB L2).
 #include <limits.h>
 
 #include "common.cuh"
@@ -62,10 +62,9 @@ struct VoxWs {
 // Candidate slots per voxel: a voxel's first C points (in arrival order) are kept as they come, one atomicAdd each;
 // only voxels with more than C points fall back to the atomicMin cascade for the rest.
 inline int cand_slots(int P) {
-  // Measured (B200): recording arrivals costs one same-address atomicAdd per point of a voxel and the selection is
-  // quadratic in the voxel's population; it wins for the small P of the voxel models (C3, P = 10: K3 + K3b 13 us
-  // against 27 us for the all-cascade K3) and loses for pillar models (C2, P = 32, pillars of 200 points: 44 us
-  // against 36 us).  C = 0 selects the all-cascade path: K3 cascades every point into `ovf`, which K4 reads directly.
+  // Recording arrivals costs one same-address atomicAdd per point of a voxel and the selection is quadratic in the
+  // voxel's population; it pays off for the small P of the voxel models (C3, P = 10) and not for pillar models (C2,
+  // P = 32, pillars of 200 points).  C = 0 selects the all-cascade path: K3 cascades every point into `ovf`, which K4 reads directly.
   if (P > 16) return 0;
   int c = 4 * P > 32 ? 4 * P : 32;
   return (c + 3) & ~3;
@@ -284,8 +283,8 @@ __global__ void __launch_bounds__(256) vox_slots_kernel(const int32_t *__restric
   const int v = slot_vox[slot];
   if (v < 0) return;
   // One atomic per point: arrival number inside the voxel.  The first C arrivals are simply recorded (K3b orders them);
-  // measured on the C3 frame, where 38 % of the points sit in voxels of 11 .. 42 points, the earlier all-cascade version
-  // spent 27 us serialising ~c x P / 2 dependent same-line atomics per such voxel.
+  // on the C3 frame many points sit in voxels of 11 .. 42 points, where an all-cascade version serialises ~c x P / 2
+  // dependent same-line atomics per such voxel.
   if (C > 0) {
     const int a = atomicAdd(count + v, 1);
     if (a < C) {
@@ -316,7 +315,7 @@ __global__ void __launch_bounds__(256) vox_slots_kernel(const int32_t *__restric
   for (; s < P; ++s) {
     // plain (L1-cached, possibly stale) read: entries only shrink, so a stale "already smaller" is still true and the
     // atomic can be skipped at L1 latency; a stale "larger" merely costs the atomic, which returns the fresh value
-    // (with ld.cg here every level walked cost an L2 round trip: the P = 64 pillar config went from 348 to 477 us)
+    // (with ld.cg here every level walked would cost an L2 round trip)
     if (L[s] < cur) continue;
     const int old = atomicMin(&L[s], cur);
     if (old == kInf) break;     // landed in a free slot
@@ -478,7 +477,7 @@ int run_front(const float *points, int n, int F, const VoxGeom &g, int P, int V,
   const size_t n_t16 = static_cast<size_t>(w.cap) / 2;
   const size_t n_d16 = (static_cast<size_t>(w.nblocks) + 1 + 1) / 2;  // carve() pads to 256 B
   const size_t n_l16 = (static_cast<size_t>(V) * P + 3) / 4;
-  P3D_CUDA_CHECK(launch_pdl(vox_init_kernel, dim3(kNumSMs * 4), dim3(256), 0, st, reinterpret_cast<uint4 *>(w.table), n_t16,
+  P3D_CUDA_CHECK(launch_pdl(vox_init_kernel, dim3(num_sms() * 4), dim3(256), 0, st, reinterpret_cast<uint4 *>(w.table), n_t16,
                             reinterpret_cast<uint4 *>(w.desc), n_d16, reinterpret_cast<uint4 *>(w.ovf), n_l16,
                             reinterpret_cast<uint4 *>(w.count), (static_cast<size_t>(V) + 3) / 4));
   if (n > 0) {

@@ -3,7 +3,7 @@ SecondBackbone (backbones/second_backbone.py:72-120), SecondFPN (necks/second_fp
 and CenterHead (detection/centerpoint/center_head.py:43-220) — as a chain of `ops.dense_conv.dense_conv2d` launches
 with BatchNorm folded into the conv epilogue.  Same constructor vocabulary as the reference's yml
 (configs/centerpoint/centerpoint_voxels_0075voxel_nuscenes_10sweep.yml:127-162).  Default arithmetic: fp16 (hi, lo')
-pair operands on tcgen05 (csrc/dense_conv_f16.cu, `f16=True`); the round-1 tf32-pair kernels stay selectable
+pair operands on wgmma (csrc/dense_conv_f16.cu, `f16=True`); the tf32-pair kernels stay selectable
 (`f16=False`) for data outside fp16's range.  The 36 ConvModules of the heads run as ONE 64 -> 2304 convolution and
 the 36 output convs as one grouped CUDA-core launch (forward); forward_per_head keeps the layer-by-layer form for
 the parity tests."""

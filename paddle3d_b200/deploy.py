@@ -59,7 +59,7 @@ def write_results(path, box3d_lidar, label_preds, scores):
 
 
 class Predictor:
-    """`init_predictor` + `run` of the reference's deploy script over the B200 pipeline."""
+    """`init_predictor` + `run` of the reference's deploy script over this repository's CUDA pipeline."""
 
     def __init__(self, cfg=None, device="cuda:0", max_points=None, seed=0, precision=None, with_head=True, weights=None):
         import torch

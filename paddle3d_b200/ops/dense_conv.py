@@ -1,6 +1,6 @@
-"""SURVEY.md §8f-1: dense 2-D convolutions of the RPN / neck / CenterHead on tcgen05.  Default: the fp16-pair kernels of
-`csrc/dense_conv_f16.cu` (second half of this file; per-layer timings in profiles/r02_dense_bench*.jsonl).  The first
-half drives the round-1 tf32-pair kernels (`csrc/dense_conv_tc.cu`, images as "pixel split rows" [B*H*W, 2*C] fp32), kept
+"""SURVEY.md §8f-1: dense 2-D convolutions of the RPN / neck / CenterHead on wgmma.  Default: the fp16-pair kernels of
+`csrc/dense_conv_f16.cu` (second half of this file; per-layer timings: tools/dense_bench.py).  The first
+half drives the tf32-pair kernels (`csrc/dense_conv_tc.cu`, images as "pixel split rows" [B*H*W, 2*C] fp32), kept
 for models whose activations leave fp16's range.  Weights are given in Paddle's layouts (Conv2D [Cout, Cin, kH, kW],
 Conv2DTranspose [Cin, Cout, k, k])."""
 import torch
@@ -90,13 +90,13 @@ def n_tile_for_f16(cout, cin=None, kernel=None, stride=1, padding=0, up=1):
     """Output-channel tile.  P3D_DENSE_NTILE (tuning hook) forces 64 or 128 for the wide layers.  With P3D_DENSE_WS=1 a
     3x3 / stride 1 / pad 1 layer with few input and many output channels (the 64 -> 36 x 64 ConvModules of the CenterHead)
     takes 64 and the kernel keeps the N tile's whole weight image (9 * Cin * 256 bytes <= 144 KB) in shared memory
-    (weight-stationary); measured 5 % slower than the streaming N = 128 kernel, hence opt-in."""
+    (weight-stationary); not faster than the streaming N = 128 kernel, hence opt-in."""
     import os
     forced = os.environ.get("P3D_DENSE_NTILE")
     if forced and cout >= 128:
         return int(forced)
     if (cin is not None and kernel == 3 and stride == 1 and padding == 1 and up == 1 and cin <= 64 and cout >= 256
-            and os.environ.get("P3D_DENSE_WS", "0") != "0"):  # measured slower than N = 128 streaming: opt-in
+            and os.environ.get("P3D_DENSE_WS", "0") != "0"):  # opt-in
         return 64
     return 128 if cout >= 128 else 64
 

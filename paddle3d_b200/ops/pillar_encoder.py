@@ -1,4 +1,4 @@
-"""SURVEY.md §8a-5 / §8f-2 (parity-green on a B200): PillarFeatureNet (models/voxel_encoders/pillar_encoder.py:
+"""SURVEY.md §8a-5 / §8f-2 (tests/test_gpu_voxelize.py): PillarFeatureNet (models/voxel_encoders/pillar_encoder.py:
 115-210) with one PFNLayer as one launch over the `hard_voxelize` outputs."""
 import numpy as np
 import torch

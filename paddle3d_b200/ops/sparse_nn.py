@@ -9,7 +9,7 @@
 
 so the model file only changes its import line (`from paddle3d_b200.ops.sparse_nn import nn, ...`).
 
-Execution model (B200-first, not Paddle's): a convolution does not run when it is called.  It returns
+Execution model (GPU-first, not Paddle's): a convolution does not run when it is called.  It returns
 a tensor with a *pending* fused kernel; BatchNorm / add / ReLU applied to that tensor fold into the
 kernel's epilogue, and the single gather-GEMM launch happens when the values are needed (next conv,
 to_dense, .values()).  conv -> bn -> relu, and conv -> bn -> add -> relu, are one launch each.
@@ -26,18 +26,18 @@ from .._mem import ptr, require_cuda, stream, workspace
 from . import pillar_scatter as _ps
 
 # FP32         exact fp32 FMA on CUDA cores
-# TF32X3       tcgen05 3xTF32 on plain fp32 rows: the tf32 hi/lo split happens inside the gather loop
-# TF32X3_SPLIT tcgen05 3xTF32 on split-layout rows [n][2][C]: whole-line cp.async gathers, persistent tiles, split done
-#              once in the producing layer's epilogue (fastest measured, what the pipeline and the bench use)
-# TF32X3_TMA   experimental: TF32X3_SPLIT with the row gather of the Cin >= 32 layers done by TMA tile::gather4
-# F16X3        tcgen05 on fp16 hi/lo' pair rows (csrc/sparse_conv_f16.cu): same 22-bit products as TF32X3_SPLIT in half
+# TF32X3       wgmma 3xTF32 on plain fp32 rows: the tf32 hi/lo split happens inside the gather loop
+# TF32X3_SPLIT wgmma 3xTF32 on split-layout rows [n][2][C]: whole-line cp.async gathers, persistent tiles, split done
+#              once in the producing layer's epilogue
+# TF32X3_TMA   experimental: TF32X3_SPLIT with the row gather of the Cin >= 32 layers done by per-row TMA boxes
+# F16X3        wgmma on fp16 hi/lo' pair rows (csrc/sparse_conv_f16.cu): same 22-bit products as TF32X3_SPLIT in half
 #              the bytes, persistent + overlapped epilogue + device-chosen split-K; |activations| < 65504 (flagged)
 FP32, TF32X3, TF32X3_SPLIT, TF32X3_TMA, F16X3 = 0, 1, 2, 3, 4
 ROWS_F32, ROWS_SPLIT, ROWS_H16 = 0, 1, 2  # activation layouts: [n, C] fp32 | [n][2][C] tf32 hi/lo | fp16 hi/lo' pairs
 _default_precision = [FP32]
 F16_MAX_SPLITS = 4
 # F16X3 layers with (Cin, Cout) in {(16,16), (16,32), (32,32)} run on the register-gather warp-MMA kernel
-# (csrc/sparse_conv_wm.cu: same rows, same arithmetic, missing neighbours are free); P3D_SPARSE_WM=0 keeps them on tcgen05
+# (csrc/sparse_conv_wm.cu: same rows, same arithmetic, missing neighbours are free); P3D_SPARSE_WM=0 keeps them on wgmma
 NARROW_WM = [os.environ.get("P3D_SPARSE_WM", "1") != "0"]
 _status = {}
 
@@ -52,7 +52,7 @@ def status_tensor(device):
 
 
 def set_precision(p):
-    """FP32 = CUDA-core fp32 FMA; TF32X3 = tcgen05 tensor cores with 3xTF32 split accumulation."""
+    """FP32 = CUDA-core fp32 FMA; TF32X3 = wgmma tensor cores with 3xTF32 split accumulation."""
     _default_precision[0] = int(p)
 
 

@@ -1,4 +1,4 @@
-"""CenterPoint-voxel hot-path frame on one B200: the public API a user calls (bench.py `e2e`).
+"""CenterPoint-voxel hot-path frame on one GPU: the public API a user calls (bench.py `e2e`).
 
     voxelize (+ VoxelMean fused)  ->  SparseResNet3D (21 sparse convs)  ->  dense BEV [1,256,180,180]
     -> dense 2-D RPN + neck + CenterHead (with_head=True; otherwise resident synthetic head tensors)
@@ -284,8 +284,7 @@ class CenterPointSweep:
     CUDA graph and stream; frames are dealt round-robin.  A frame is a chain of ~70 kernels of very different shapes -
     persistent tensor-core kernels that fill the GPU, and latency-bound ones (voxel hashing, rulebooks, post-processing,
     the tails of every layer) that leave most SMs idle: with a second frame in flight those gaps are filled by the other
-    frame's kernels.  Measured on the C3 frame (tools/two_in_flight.py): 602 -> 713 frames/s with two lanes.  The latency
-    of one frame does not improve (use CenterPointHotPath.infer for that); results are those of the single-lane pipeline.
+    frame's kernels (tools/two_in_flight.py compares one and two lanes).  The latency of one frame does not improve (use CenterPointHotPath.infer for that); results are those of the single-lane pipeline.
     """
 
     def __init__(self, lanes=2, **kw):

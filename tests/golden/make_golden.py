@@ -1,5 +1,5 @@
-"""Generate the committed golden fixtures from the REFERENCE ITSELF (run in the build container only;
-/root/reference does not exist on the GPU box, the .npz files do).
+"""Generate the committed golden fixtures from the REFERENCE ITSELF (needs a Paddle3D source checkout named by
+$P3D_REFERENCE and oracle/_ref built from it; the tests only read the committed .npz files).
 
   voxelize_*.npz   outputs of the reference's own hard_voxelize_cpu (voxelize_op.cc:84-146, compiled
                    unmodified into oracle/_ref/libp3d_ref_cpu.so) AND of the reference's numba
@@ -23,7 +23,7 @@ sys.path.insert(0, ROOT)
 import oracle  # noqa: E402
 from paddle3d_b200 import synth  # noqa: E402
 
-REF = "/root/reference"
+REF = os.environ.get("P3D_REFERENCE", "")  # a Paddle3D source checkout
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 

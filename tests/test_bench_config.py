@@ -1,5 +1,4 @@
-"""CPU: both arms of bench.py print the identical `config` object for the same flags (the driver compares them), and the
-committed ncu captures the rooflines cite are readable."""
+"""CPU: both arms of bench.py print the identical `config` object for the same flags."""
 import os
 import sys
 
@@ -17,12 +16,3 @@ def test_config_dict_is_shared_by_both_arms():
     b = bench.make_config("0075", True, 4)
     assert a == b and a["frames_in_flight_per_gpu"] == 4 and "0.075 m" in a["workload"]
     assert bench.make_config("01", True)["workload"] != a["workload"]
-
-
-def test_committed_ncu_captures_feed_the_rooflines():
-    import bench
-    for name in ("r02_dense_ncu_metrics.csv", "r02_sparse_ncu_metrics.csv", "r02_voxelize_ncu_metrics.csv"):
-        assert bench.ncu_dram_bytes(name) and bench.ncu_dram_bytes(name) > 1e6, name
-    assert 40.0 < bench.ncu_tensor_active("r02_dense_ncu_metrics.csv") < 80.0
-    assert 10.0 < bench.ncu_tensor_active("r02_sparse_ncu_metrics.csv") < 60.0
-    assert bench.ncu_dram_bytes("no_such_capture.csv") is None

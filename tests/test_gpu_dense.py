@@ -103,7 +103,7 @@ def test_dense_conv_f16_vs_oracle(cuda, oracle_mod, cin, cout, k, stride, pad, u
 
 
 @pytest.mark.parametrize("cin,cout,h,w", [
-    (64, 320, 37, 19),    # 5 N tiles of 64 on 148 CTAs: every CTA's range is short, many start mid N tile
+    (64, 320, 37, 19),    # 5 N tiles of 64 on 132 CTAs: every CTA's range is short, many start mid N tile
     (32, 208, 50, 61),    # last N tile partly used; 52 pixel tiles x 4 N tiles: ranges cross N-tile boundaries (image swap)
     (64, 2304, 24, 16),   # the CenterHead shape: 36 N tiles
 ])

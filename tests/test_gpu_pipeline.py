@@ -134,8 +134,7 @@ def test_fused_pixel_h16_bev_matches_nchw_path(cuda):
     # Two sources of difference, both far inside the parity bar: the pair format of the last rows (2^-22 relative) and the
     # fp32 summation order of the stream-K pieces of the narrow layers, which follows the row order - and the strided
     # levels number their output sites with atomics, so two frames of the same cloud order their rows differently.
-    # (With all layers on the tcgen05 kernel, P3D_SPARSE_WM=0, the two tensors agree to 2^-20 relative / 1e-9 absolute.)
-    # Measured: 1.2e-5 relative on elements above 1 % of the maximum after the 21 layers; the bound is the parity bar.
+    # The bound is the parity bar.
     rel_check('fused pixel BEV vs NCHW BEV', bev_b, bev_a)
     # the dense head reads the pixel rows in (z, c) channel order through the permuted image of its first conv
     ha, hb = a.dense(a.bev_nchw()), b.dense.forward_h16(*b.out["bev_h16"])

@@ -12,7 +12,7 @@ from parity import rel_check
 
 pytestmark = pytest.mark.gpu
 
-# 0 fp32 CUDA cores, 1 tcgen05 on fp32 rows, 2 tcgen05 on tf32 split rows, 4 tcgen05 on fp16-pair rows (default);
+# 0 fp32 CUDA cores, 1 wgmma on fp32 rows, 2 wgmma on tf32 split rows, 4 wgmma on fp16-pair rows (default);
 # 3 = the slower TMA-gather variant of 2, kept for the record (P3D_EXPERIMENTAL=1)
 PRECISIONS = [0, 1, 2, 4] + ([3] if os.environ.get("P3D_EXPERIMENTAL") == "1" else [])
 
@@ -81,7 +81,7 @@ def test_single_conv(cuda, oracle_mod, precision, subm, ks, st, pd, cin, cout):
 ])
 def test_narrow_layers_on_both_kernels(cuda, oracle_mod, wm, subm, ks, st, pd, cin, cout, residual):
     """The 16/32-channel layers of the fp16-pair path: register-gather warp-MMA kernel (csrc/sparse_conv_wm.cu, default)
-    and the tcgen05 kernel (P3D_SPARSE_WM=0) against the oracle - conv + BN (+ residual) + ReLU, fp32 and H16 outputs,
+    and the wgmma kernel (P3D_SPARSE_WM=0) against the oracle - conv + BN (+ residual) + ReLU, fp32 and H16 outputs,
     a row count that is not a multiple of 16."""
     import torch
     from paddle3d_b200.ops import sparse_nn as sp

@@ -32,7 +32,7 @@ def test_iou_oracle_matches_reference_golden(oracle_mod):
 @pytest.mark.parametrize("cfg,seed", [(synth.C1, 3), (synth.C2, 4)])
 def test_voxelize_oracle_matches_reference_library(oracle_mod, cfg, seed):
     if oracle_mod.ref_lib("cpu") is None:
-        pytest.skip("oracle/_ref not built (no /root/reference here)")
+        pytest.skip("oracle/_ref not built (no Paddle3D checkout in $P3D_REFERENCE)")
     pts = synth.lidar_cloud(cfg, seed, num_points=min(cfg["num_points"], 20000))
     a = oracle_mod.hard_voxelize(pts, cfg["voxel_size"], cfg["point_cloud_range"], 5, 3000)
     b = oracle_mod.ref_hard_voxelize_cpu(pts, cfg["voxel_size"], cfg["point_cloud_range"], 5, 3000)

@@ -3,7 +3,7 @@
 
 Graph-replayed, one JSON line per distinct layer shape and kernel variant with its algorithmic TFLOP/s (2 * MACs of the
 convolution; the kernels execute 3 fp16 MMAs per product), then the whole head.  Needs a GPU:
-    python tools/dense_bench.py [--variants] [> profiles/...]
+    python tools/dense_bench.py [--variants] [> dense_layers.jsonl]
 """
 import argparse
 import json

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-kernel share of ONE frame from an `ncu --metrics gpu__time_duration.sum --csv` launch list of bench.py
 (cold-cache, serialised launch times: compare SHARES, not absolutes).  The frame = the launches between the last two
-`vox_init` kernels.    python tools/launch_shares.py gpurun_out/launches.csv [> profiles/..._shares.txt]"""
+`vox_init` kernels.    python tools/launch_shares.py launches.csv [> shares.txt]"""
 import collections
 import csv
 import re

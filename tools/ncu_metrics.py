@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Extract the per-launch metrics the rooflines cite from an .ncu-rep capture (ncu --set full) into a small CSV:
 duration, grid/block, registers, DRAM bytes read / written, L2 hit rate, tensor-pipe activity, issue activity.
-    python tools/ncu_metrics.py gpurun_out/x.ncu-rep > profiles/x_metrics.csv      (no GPU needed: ncu -i ... --page raw)
-The first two rows are header and units, as bench.py's ncu_dram_bytes() expects."""
+    python tools/ncu_metrics.py x.ncu-rep > x_metrics.csv      (no GPU needed: ncu -i ... --page raw)
+The first two rows are header and units (ncu's raw page)."""
 import csv
 import io
 import subprocess

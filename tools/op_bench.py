@@ -4,8 +4,8 @@
 launching stream after an L2 flush (a 256 MB write), so neither cached inputs nor host launch gaps distort it.  Output: one JSON line per op.
 
     python tools/op_bench.py [--iters 30] [--only voxelize,scatter,bev_pool,nms,postprocess]
-Run it under ncu for the committed captures (profiles/), e.g.
-    ncu --set full --clock-control none -k regex:'vox_write|scat_write|bev_fwd' -c 6 -o gpurun_out/ops python tools/op_bench.py --iters 2
+Under Nsight Compute, e.g.
+    ncu --set full --clock-control none -k regex:'vox_write|scat_write|bev_fwd' -c 6 -o ops python tools/op_bench.py --iters 2
 """
 import argparse
 import json
@@ -36,8 +36,7 @@ def timed(fn, iters, flush):
             fn()
         for _ in range(iters):
             # the flush is also what keeps the GPU busy while the host enqueues event + graph launch: with one 256 MB
-            # write (~45 us) the replay could arrive after the start event had fired, and every op measured >= ~57 us
-            # (round-2 finding); three writes give the host ~150 us of slack
+            # write the replay could arrive after the start event had fired; three writes give the host slack
             for _ in range(3):
                 flush.zero_()
             s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)

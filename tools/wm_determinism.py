@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Run the narrow-layer warp-MMA kernel twice on the level-0 / level-1 index sets of a C3 frame and compare bit for bit
-(stream-K fix-up order), and against the tcgen05 kernel (same arithmetic, different summation order)."""
+(stream-K fix-up order), and against the wgmma kernel (same arithmetic, different summation order)."""
 import os
 import sys
 
@@ -41,7 +41,7 @@ def main():
         same01 = torch.equal(outs[0], outs[1]) and torch.equal(outs[1], outs[2])
         nd = (outs[0] != outs[1]).sum().item() + (outs[1] != outs[2]).sum().item()
         d = (outs[0].float() - outs[3].float()).abs().max().item()
-        print("%d->%d rows %d: wm run-to-run bit-identical %s (%d halfs differ); wm vs tcgen05 max |diff| of the half words %.3g"
+        print("%d->%d rows %d: wm run-to-run bit-identical %s (%d halfs differ); wm vs wgmma max |diff| of the half words %.3g"
               % (cin, cout, outs[0].shape[0], same01, nd, d), flush=True)
 
 
