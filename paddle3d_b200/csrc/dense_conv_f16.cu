@@ -17,10 +17,12 @@
 //   * MT = 2 (N tile <= 64): two M tiles (8 x 32 pixels) share every weight block: half the weight traffic per flop.
 //
 //   work item   (batch, pixel tile, N tile[, tap of a k = s transposed conv]), N tile fastest
-//   step        (A unit, tap): HALO one A unit per 32-channel group serves 9 steps, TAP one A unit per step.  Thread 0
-//               keeps an activation ring (NA) and a weight ring (NB) ahead of the consumers across work items (TMA /
-//               cp.async.bulk, mbarrier complete_tx); warpgroup g computes rows 64g .. 64g+63 of every M tile and runs
-//               their epilogue from its registers.
+//   step        (A unit, tap): HALO one A unit per 32-channel group serves 9 steps, TAP one A unit per step.
+//   warp-specialized CTA of three warpgroups: warpgroup 0 is the producer - one thread keeps an activation ring (NA) and
+//               a weight ring (NB) filled ahead of the consumers across work items (TMA / cp.async.bulk onto "full"
+//               mbarriers, refilling a slot once its "empty" mbarrier says both consumers are done with it); consumer
+//               warpgroup c = 1, 2 computes rows 64(c-1) .. 64(c-1)+63 of every M tile with one wgmma group in flight
+//               behind the one being issued, and runs their epilogue from its registers while the producer loads on.
 #include <cuda.h>
 #include <cuda_fp16.h>
 
@@ -34,6 +36,10 @@ using namespace tc;
 
 constexpr int kTW = 8, kTH = 16;        // output tile of one M = 128 tile: 8 x 16 pixels
 constexpr int kMaxA = 6, kMaxB = 12;    // activation / weight ring depth limits
+constexpr int kDenseThreads = 384;      // producer warpgroup + two consumer warpgroups
+// register split of the warp-specialized kernel: 128 x 40 + 256 x 232 <= 64 K (the consumers hold 128 fp32 accumulators)
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;
+constexpr uint32_t kConsumerWarps = 8;  // arrivals that release a slot: one per consumer warp
 constexpr float kLoScale = 2048.0f, kLoInv = 1.0f / 2048.0f;
 
 struct Params {
@@ -132,7 +138,7 @@ __device__ __forceinline__ Item decode(long long w, const Params &p, int th) {
 }
 
 template <int N, int MT, bool HALO, int PITCH, bool WS = false>
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(kDenseThreads, 1)
     dense_conv_f16_kernel(const __grid_constant__ CUtensorMap in_map, const Params p) {
   using C = Cfg<N, MT, HALO, PITCH, WS>;
   constexpr int TH = kTH * MT;  // output tile height
@@ -150,100 +156,126 @@ __global__ void __launch_bounds__(kThreads, 1)
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  __shared__ __align__(8) unsigned long long s_bar[kMaxA + kMaxB + 1];  // activation full[NA] | weight full[NB] | image
-  constexpr int kAF = 0, kBF = kMaxA, kWF = kMaxA + kMaxB;
+  // full barriers: one producer arrive + the bytes of the load; empty barriers: one arrive per consumer warp once the
+  // wgmma that read the slot have retired.  Activation full[NA] | empty[NA] | weight full[NB] | empty[NB] | WS image
+  // full | empty.
+  __shared__ __align__(8) unsigned long long s_bar[2 * kMaxA + 2 * kMaxB + 2];
+  constexpr int kAF = 0, kAE = kMaxA, kBF = 2 * kMaxA, kBE = 2 * kMaxA + kMaxB, kWF = 2 * kMaxA + 2 * kMaxB, kWE = kWF + 1;
 
   const int tid = threadIdx.x, wg = tid >> 7, wtid = tid & 127;
   if (tid == 0) {
-    for (int s = 0; s < C::NA; ++s) mbar_init(smem_u32(&s_bar[kAF + s]), 1);
-    for (int s = 0; s < (WS ? 0 : C::NB); ++s) mbar_init(smem_u32(&s_bar[kBF + s]), 1);
+    for (int s = 0; s < C::NA; ++s) {
+      mbar_init(smem_u32(&s_bar[kAF + s]), 1);
+      mbar_init(smem_u32(&s_bar[kAE + s]), kConsumerWarps);
+    }
+    for (int s = 0; s < (WS ? 0 : C::NB); ++s) {
+      mbar_init(smem_u32(&s_bar[kBF + s]), 1);
+      mbar_init(smem_u32(&s_bar[kBE + s]), kConsumerWarps);
+    }
     mbar_init(smem_u32(&s_bar[kWF]), 1);
+    mbar_init(smem_u32(&s_bar[kWE]), kConsumerWarps);
     fence_mbar_init();
   }
+  __syncthreads();  // the only block-wide barrier: the mbarriers are initialised
   const uint32_t a_ring = smem_u32(smem);
   const uint32_t b_ring = a_ring + C::NA * C::A_BYTES;
   const int G = p.Cin / 32;
   // steps / activation units per item: HALO: one unit per group, 9 taps each; TAP: one unit per (tap, group)
   const int taps_item = p.up > 1 ? 1 : p.taps;
   const int units_item = HALO ? G : taps_item * G;
-  const int steps_item = units_item * C::SPU;
-  const long long n_units = n_items * units_item, n_steps = n_items * steps_item;
   auto item_w = [&](long long idx) { return w_first + idx * w_step; };
+  // Ring positions advance by one slot per fill / use; the phase bit flips when the slot index wraps.  The consumers wait
+  // for full[slot] to complete the phase of the current pass; the producer waits for empty[slot] to complete the phase
+  // of the previous pass (parity ph ^ 1: on the first pass that is the phase before the barrier's first, which counts as
+  // complete, so the first NA / NB fills do not wait).
 
-  // thread 0: activation buffer of global unit a / weight blocks of global step q
-  auto issue_a = [&](long long a) {
-    const Item im = decode<WS>(item_w(a / units_item), p, TH);
-    const int ua = static_cast<int>(a % units_item);
-    const int cg0 = p.grouped ? im.nt * G : 0;  // first 32-channel group of this item's input channels
-    const uint32_t slot = static_cast<uint32_t>(a % C::NA), bar = smem_u32(&s_bar[kAF + slot]);
-    mbar_arrive_expect_tx(bar, static_cast<uint32_t>(C::A_ROWS * 128));
-    if (HALO) {
-      tma_tile4d(a_ring + slot * C::A_BYTES, &in_map, (cg0 + ua) * 64, im.tx0 - 1, im.ty0 - 1, im.b, bar);
-    } else {
-      const int t = (p.up > 1 ? im.tap0 : ua / G), g = ua % G;
-      const int dy = p.up > 1 ? 0 : t / p.kw, dx = p.up > 1 ? 0 : t % p.kw;
-      const int x = im.tx0 * p.stride - p.pad + dx, y = im.ty0 * p.stride - p.pad + dy;  // may be negative: zero fill
-      tma_tile4d(a_ring + slot * C::A_BYTES, &in_map, (cg0 + g) * 64, x, y, im.b, bar);
+  if (wg == 0) {
+    // ------------------------------------------------------------------------------------------ producer
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
+    if (tid != 0) return;
+    uint32_t a_slot = 0, a_ph = 0, b_slot = 0, b_ph = 0;
+    int cur_nt = -1;  // WS: N tile whose weight image is resident
+    uint32_t img = 0; // WS: images loaded so far
+    for (long long idx = 0; idx < n_items; ++idx) {
+      const Item im = decode<WS>(item_w(idx), p, TH);
+      const int cg0 = p.grouped ? im.nt * G : 0;  // first 32-channel group of this item's input channels
+      const uint8_t *w_tile = p.packed_w + static_cast<size_t>(im.nt) * p.taps * (p.Cin / 16) * C::B_BLK;
+      if (WS && im.nt != cur_nt) {
+        // first item of a run on this N tile: replace the image once both consumers have retired every step of the
+        // previous run
+        if (img > 0) mbar_wait(smem_u32(&s_bar[kWE]), (img - 1) & 1u);
+        const uint32_t bar = smem_u32(&s_bar[kWF]);
+        mbar_arrive_expect_tx(bar, static_cast<uint32_t>(p.w_bytes));
+        for (int off = 0; off < p.w_bytes; off += 16384) {
+          const int bytes = p.w_bytes - off < 16384 ? p.w_bytes - off : 16384;
+          bulk_g2s(b_ring + static_cast<uint32_t>(off), w_tile + off, static_cast<uint32_t>(bytes), bar);
+        }
+        ++img;
+        cur_nt = im.nt;
+      }
+      // TAP units are (tap, group) with the group fastest; dy, dx follow the tap without dividing
+      int dy = 0, dx = 0;
+      for (int tu = 0; tu < (HALO ? 1 : taps_item); ++tu) {
+        const int tap = p.up > 1 ? im.tap0 : tu;
+        for (int g = 0; g < G; ++g) {
+          const uint32_t abar = smem_u32(&s_bar[kAF + a_slot]), a_dst = a_ring + a_slot * C::A_BYTES;
+          mbar_wait(smem_u32(&s_bar[kAE + a_slot]), a_ph ^ 1u);
+          mbar_arrive_expect_tx(abar, static_cast<uint32_t>(C::A_ROWS * 128));
+          if (HALO) {
+            tma_tile4d(a_dst, &in_map, (cg0 + g) * 64, im.tx0 - 1, im.ty0 - 1, im.b, abar);
+          } else {
+            const int x = im.tx0 * p.stride - p.pad + dx, y = im.ty0 * p.stride - p.pad + dy;  // may be negative: zero fill
+            tma_tile4d(a_dst, &in_map, (cg0 + g) * 64, x, y, im.b, abar);
+          }
+          if (++a_slot == C::NA) a_slot = 0, a_ph ^= 1u;
+          for (int t = 0; t < (WS ? 0 : C::SPU); ++t) {
+            const uint32_t bbar = smem_u32(&s_bar[kBF + b_slot]);
+            mbar_wait(smem_u32(&s_bar[kBE + b_slot]), b_ph ^ 1u);
+            mbar_arrive_expect_tx(bbar, static_cast<uint32_t>(C::B_BYTES));
+            bulk_g2s(b_ring + b_slot * C::B_BYTES, w_tile + (static_cast<size_t>(HALO ? t : tap) * (p.Cin / 16) + 2 * g) * C::B_BLK,
+                     static_cast<uint32_t>(C::B_BYTES), bbar);
+            if (++b_slot == C::NB) b_slot = 0, b_ph ^= 1u;
+          }
+        }
+        if (++dx == p.kw) dx = 0, ++dy;
+      }
     }
-  };
-  auto issue_b = [&](long long q) {
-    const Item im = decode<WS>(item_w(q / steps_item), p, TH);
-    const int u = static_cast<int>(q % steps_item);
-    int t, g;
-    if (HALO) {
-      g = u / 9;
-      t = u % 9;
-    } else {
-      t = p.up > 1 ? im.tap0 : u / G;
-      g = u % G;
-    }
-    const uint8_t *w_tile = p.packed_w + static_cast<size_t>(im.nt) * p.taps * (p.Cin / 16) * C::B_BLK;
-    const uint32_t slot = static_cast<uint32_t>(q % C::NB), bar = smem_u32(&s_bar[kBF + slot]);
-    mbar_arrive_expect_tx(bar, static_cast<uint32_t>(C::B_BYTES));
-    bulk_g2s(b_ring + slot * C::B_BYTES, w_tile + (static_cast<size_t>(t) * (p.Cin / 16) + 2 * g) * C::B_BLK,
-             static_cast<uint32_t>(C::B_BYTES), bar);
-  };
+    return;
+  }
 
+  // -------------------------------------------------------------------------------------------- consumers
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
+  const int cw = wg - 1;                 // rows 64 cw .. 64 cw + 63 of every M tile
+  const bool warp_leader = (tid & 31) == 0;
+  auto release = [&](int base, uint32_t slot) {
+    if (warp_leader) mbar_arrive(smem_u32(&s_bar[base + slot]));
+  };
   bool ovf = false;
-  long long next_a = 0, next_b = 0;  // thread 0: next unit / step to load
-  int cur_nt = -1;                   // WS: N tile whose weight image is resident
-  uint32_t img = 0;                  // WS: images loaded so far
-  long long q = 0;                   // global step
+  uint32_t a_slot = 0, a_ph = 0, b_slot = 0, b_ph = 0;
+  int cur_nt = -1;   // WS: N tile whose weight image is resident
+  uint32_t img = 0;  // WS: images used so far
   float acc[C::ACC];
   for (long long idx = 0; idx < n_items; ++idx) {
     const Item im = decode<WS>(item_w(idx), p, TH);
+    if (WS && im.nt != cur_nt) {
+      mbar_wait(smem_u32(&s_bar[kWF]), img & 1u);
+      ++img;
+      cur_nt = im.nt;
+    }
 #pragma unroll
     for (int i = 0; i < C::ACC; ++i) acc[i] = 0.f;
+    // slots of the step whose wgmma group is still in flight: weight slot, and the activation slot when that step was
+    // the last one of its unit (-1 otherwise)
+    uint32_t prev_b = 0;
+    int prev_a = -1;
+    bool pending = false;
     for (int ua = 0; ua < units_item; ++ua) {
-      for (int t = 0; t < C::SPU; ++t, ++q) {
-        __syncthreads();  // the wgmma of step q - 1 have retired in both warpgroups
-        if (WS && ua == 0 && t == 0 && im.nt != cur_nt) {
-          // first item of a run on this N tile: every step of the previous run has completed, replace the image
-          if (tid == 0) {
-            const uint32_t bar = smem_u32(&s_bar[kWF]);
-            mbar_arrive_expect_tx(bar, static_cast<uint32_t>(p.w_bytes));
-            const uint8_t *w_tile = p.packed_w + static_cast<size_t>(im.nt) * p.w_bytes;
-            for (int off = 0; off < p.w_bytes; off += 16384) {
-              const int bytes = p.w_bytes - off < 16384 ? p.w_bytes - off : 16384;
-              bulk_g2s(b_ring + static_cast<uint32_t>(off), w_tile + off, static_cast<uint32_t>(bytes), bar);
-            }
-          }
-          mbar_wait(smem_u32(&s_bar[kWF]), img & 1u);
-          ++img;
-          cur_nt = im.nt;
-        }
-        if (tid == 0) {
-          for (; next_a < n_units && (next_a - C::NA + 1) * C::SPU <= q; ++next_a) issue_a(next_a);
-          if (!WS)
-            for (; next_b < n_steps && next_b <= q + C::NB - 1; ++next_b) issue_b(next_b);
-        }
-        const long long ga = q / C::SPU;  // global unit of this step
-        const uint32_t sa = static_cast<uint32_t>(ga % C::NA), sb = static_cast<uint32_t>(q % C::NB);
-        mbar_wait(smem_u32(&s_bar[kAF + sa]), static_cast<uint32_t>((ga / C::NA) & 1));
-        if (!WS) mbar_wait(smem_u32(&s_bar[kBF + sb]), static_cast<uint32_t>((q / C::NB) & 1));
-        const uint32_t a_base = a_ring + sa * C::A_BYTES;
+      mbar_wait(smem_u32(&s_bar[kAF + a_slot]), a_ph);
+      const uint32_t a_base = a_ring + a_slot * C::A_BYTES;
+      for (int t = 0; t < C::SPU; ++t) {
+        if (!WS) mbar_wait(smem_u32(&s_bar[kBF + b_slot]), b_ph);
         const uint32_t b_base = WS ? b_ring + static_cast<uint32_t>((t * (p.Cin / 16) + 2 * ua) * C::B_BLK)
-                                   : b_ring + sb * C::B_BYTES;
+                                   : b_ring + b_slot * C::B_BYTES;
         wg_fence();
 #pragma unroll
         for (int kb = 0; kb < 2; ++kb) {
@@ -253,10 +285,10 @@ __global__ void __launch_bounds__(kThreads, 1)
           for (int mt = 0; mt < MT; ++mt) {
             uint32_t a0, sbo;
             if (HALO) {  // this warpgroup's 8 image rows of M tile mt, shifted by the tap
-              a0 = a_base + static_cast<uint32_t>(((mt * kTH + wg * 8 + t / 3) * PITCH + t % 3) * 128);
+              a0 = a_base + static_cast<uint32_t>(((mt * kTH + cw * 8 + t / 3) * PITCH + t % 3) * 128);
               sbo = PITCH * 128;
             } else {
-              a0 = a_base + static_cast<uint32_t>((mt * kM + wg * 64) * 128);
+              a0 = a_base + static_cast<uint32_t>((mt * kM + cw * 64) * 128);
               sbo = 1024;
             }
             const uint32_t ah = a0 + kb * 32, al = a0 + (2 + kb) * 32;
@@ -269,9 +301,23 @@ __global__ void __launch_bounds__(kThreads, 1)
           }
         }
         wg_commit();
-        wg_wait<0>();
+        wg_wait<1>();  // the previous step's group has retired: its slots go back to the producer
+        if (pending) {
+          if (!WS) release(kBE, prev_b);
+          if (prev_a >= 0) release(kAE, static_cast<uint32_t>(prev_a));
+        }
+        pending = true;
+        prev_b = b_slot;
+        prev_a = t == C::SPU - 1 ? static_cast<int>(a_slot) : -1;
+        if (!WS && ++b_slot == C::NB) b_slot = 0, b_ph ^= 1u;
       }
+      if (++a_slot == C::NA) a_slot = 0, a_ph ^= 1u;
     }
+    wg_wait<0>();
+    if (!WS) release(kBE, prev_b);
+    release(kAE, static_cast<uint32_t>(prev_a));  // the item's last step ends a unit
+    // WS: the last item of a run on this N tile has retired every step that reads the image
+    if (WS && (idx + 1 == n_items || decode<WS>(item_w(idx + 1), p, TH).nt != im.nt)) release(kWE, 0);
     wg_fence_acc<C::ACC>(acc);
 
     // ------------------------------------------------------------------------------------------ epilogue
@@ -280,7 +326,7 @@ __global__ void __launch_bounds__(kThreads, 1)
     for (int mt = 0; mt < MT; ++mt) {
 #pragma unroll
       for (int i = 0; i < H; i += 2) {
-        const int m = wg * 64 + frag_row(i, wtid), c = frag_col(i, wtid);  // pixel of the M tile, column of the N tile
+        const int m = cw * 64 + frag_row(i, wtid), c = frag_col(i, wtid);  // pixel of the M tile, column of the N tile
         const int iy = im.ty0 + mt * kTH + m / kTW, ix = im.tx0 + m % kTW;
         const int ch = im.nt * N + c;  // output channel
         if (iy >= p.oH || ix >= p.oW || (p.grouped ? c >= g_cnt : ch >= p.cout)) continue;
@@ -399,7 +445,7 @@ int launch(const CUtensorMap &map, const Params &p, cudaStream_t st) {
   cudaLaunchConfig_t cfg = {};
   const long long sms = num_sms();
   cfg.gridDim = dim3(static_cast<unsigned int>(work < sms ? work : sms));
-  cfg.blockDim = dim3(kThreads);
+  cfg.blockDim = dim3(kDenseThreads);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
   cudaLaunchAttribute attr[1];
@@ -650,14 +696,15 @@ static int dense_conv_f16(const void *in_h16, int B, int H, int W, int Cin, cons
   if (env_mode >= 0) mode = env_mode;
   if (env_mt >= 0) m_tiles = env_mt;
   const bool halo = (mode == 0 || mode == 2) && up == 1 && kh == 3 && kw == 3 && stride == 1 && pad == 1;
-  // two M tiles per item (half the weight traffic per flop) when that still leaves every SM an item
+  // one or two M tiles per item for the narrow N <= 64 layers (N = 128 keeps one: register budget): the persistent grid
+  // runs ceil(items / SMs) rounds of items MT M tiles long, so pick the MT with the fewer M-tile rounds; on a tie two M
+  // tiles, which share every weight block (half the weight traffic per flop)
   int mt = m_tiles;
   if (mt != 1 && mt != 2) {
-    const long long tx = (p.oW + dcf::kTW - 1) / dcf::kTW, ty2 = (p.oH + 2 * dcf::kTH - 1) / (2 * dcf::kTH);
-    const long long items2 = static_cast<long long>(B) * tx * ty2 * p.n_ntiles * (up > 1 ? up * up : 1);
-    // two M tiles for the narrow N = 64 layers (the second tile halves the weight traffic per flop and amortises the
-    // per-item prologue) when that still leaves every SM an item; N = 128 keeps one (register budget)
-    mt = (n_tile <= 64 && items2 >= (num_sms() * 9) / 10) ? 2 : 1;
+    const long long tx = (p.oW + dcf::kTW - 1) / dcf::kTW, sms = num_sms();
+    const long long per_row = static_cast<long long>(B) * tx * p.n_ntiles * (up > 1 ? up * up : 1);
+    const long long items1 = per_row * ((p.oH + dcf::kTH - 1) / dcf::kTH), items2 = per_row * ((p.oH + 2 * dcf::kTH - 1) / (2 * dcf::kTH));
+    mt = (n_tile <= 64 && 2 * ((items2 + sms - 1) / sms) <= (items1 + sms - 1) / sms) ? 2 : 1;
   }
   // weight-stationary variant: haloed 3x3, N tile 64, the N tile's weight image + 3 activation tiles fit in shared memory,
   // and every CTA has enough pixel tiles per weight image to amortise loading it (mode 2 forces it, P3D_DENSE_WS=0 disables)
