@@ -22,19 +22,23 @@ def _newer(src, dst, deps):
     return any(os.path.getmtime(p) > t for p in [src] + deps)
 
 
-def build(verbose=False, force=False):
-    os.makedirs(OBJ, exist_ok=True)
+def build(verbose=False, force=False, out_dir=None, extra_flags=()):
+    """out_dir / extra_flags: build a variant (e.g. -DP3D_DENSE_TRACE) into another directory; the in-tree library is
+    the default."""
+    obj_dir = os.path.join(out_dir, "_obj") if out_dir else OBJ
+    lib_path = os.path.join(out_dir, "libp3d_b200.so") if out_dir else LIB
+    os.makedirs(obj_dir, exist_ok=True)
     srcs = sorted(f for f in os.listdir(CSRC) if f.endswith(".cu"))
     hdrs = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".cuh")] + \
            [os.path.join(ROOT, "include", "p3d_b200.h")]
     jobs = []
     for s in srcs:
-        src, obj = os.path.join(CSRC, s), os.path.join(OBJ, s[:-3] + ".o")
+        src, obj = os.path.join(CSRC, s), os.path.join(obj_dir, s[:-3] + ".o")
         if force or _newer(src, obj, hdrs):
             jobs.append((src, obj))
 
     def cc(job):
-        cmd = [NVCC] + FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-c", job[0], "-o", job[1]]
+        cmd = [NVCC] + FLAGS + list(extra_flags) + (["-Xptxas", "-v"] if verbose else []) + ["-c", job[0], "-o", job[1]]
         r = subprocess.run(cmd, capture_output=True, text=True)
         return job[0], r.returncode, r.stdout + r.stderr
 
@@ -46,11 +50,11 @@ def build(verbose=False, force=False):
             failed |= rc != 0
     if failed:
         raise RuntimeError("nvcc failed")
-    objs = [os.path.join(OBJ, s[:-3] + ".o") for s in srcs]
-    if jobs or not os.path.exists(LIB):
-        cmd = [NVCC, "-shared"] + ARCH + ["-o", LIB] + objs
+    objs = [os.path.join(obj_dir, s[:-3] + ".o") for s in srcs]
+    if jobs or not os.path.exists(lib_path):
+        cmd = [NVCC, "-shared"] + ARCH + ["-o", lib_path] + objs
         subprocess.run(cmd, check=True)
-    return LIB
+    return lib_path
 
 
 if __name__ == "__main__":

@@ -22,7 +22,10 @@
 //               a weight ring (NB) filled ahead of the consumers across work items (TMA / cp.async.bulk onto "full"
 //               mbarriers, refilling a slot once its "empty" mbarrier says both consumers are done with it); consumer
 //               warpgroup c = 1, 2 computes rows 64(c-1) .. 64(c-1)+63 of every M tile with one wgmma group in flight
-//               behind the one being issued, and runs their epilogue from its registers while the producer loads on.
+//               behind the one being issued.  At the end of an item it parks hi + cross * 2^-11 in its fp32 staging
+//               tile and starts the next item; warps 1-3 of warpgroup 0 (the epilogue warps) apply scale / shift /
+//               ReLU, split and store from there, so the tensor pipe does not idle through the epilogue.  The
+//               weight-stationary variant (WS) keeps the epilogue in the consumers' registers.
 #include <cuda.h>
 #include <cuda_fp16.h>
 
@@ -37,9 +40,8 @@ using namespace tc;
 constexpr int kTW = 8, kTH = 16;        // output tile of one M = 128 tile: 8 x 16 pixels
 constexpr int kMaxA = 6, kMaxB = 12;    // activation / weight ring depth limits
 constexpr int kDenseThreads = 384;      // producer warpgroup + two consumer warpgroups
-// register split of the warp-specialized kernel: 128 x 40 + 256 x 232 <= 64 K (the consumers hold 128 fp32 accumulators)
-constexpr int kProducerRegs = 40, kConsumerRegs = 232;
 constexpr uint32_t kConsumerWarps = 8;  // arrivals that release a slot: one per consumer warp
+constexpr uint32_t kEpiThreads = 96;    // warps 1-3 of the producer warpgroup: the epilogue warps
 constexpr float kLoScale = 2048.0f, kLoInv = 1.0f / 2048.0f;
 
 struct Params {
@@ -77,14 +79,27 @@ struct Cfg {
   static constexpr int A_BYTES = ((A_ROWS * 128 + 1023) / 1024) * 1024;
   static constexpr int B_BYTES = 128 * N;                                    // weight blocks of one (tap, group): 2 k-blocks
   static constexpr int B_BLK = 64 * N;
+  // Staged epilogue (all but WS): a consumer warpgroup parks hi + cross * 2^-11 of its rows (MT x 64 rows x N columns,
+  // fp32) in its own staging tile and goes on with the next item; the epilogue warps apply scale / shift / ReLU, split
+  // and store.  Row pitch N + 8 floats: the 32 bytes of padding put the four rows of a half-warp's fragment stores on
+  // distinct banks.  WS keeps the epilogue in the consumers (its weight image leaves no room for the tiles).
+  static constexpr bool STAGE = !WS;
+  static constexpr int SP = N + 8;                                           // staging row pitch (floats)
+  static constexpr int STG_WG = MT * 64 * SP;                                // floats per consumer warpgroup
+  static constexpr int STG_BYTES = STAGE ? 2 * STG_WG * 4 : 0;
+  static constexpr int AVAIL = (227 - 6) * 1024 - STG_BYTES;  // 227 KB - alignment slack - static (barriers) - staging
   // TAP mode: every step needs a new activation buffer, so both rings get the same depth; HALO: 2 (WS: 3) buffers
-  static constexpr int NA_TAP_RAW = (227 - 6) * 1024 / (A_BYTES + B_BYTES);
+  static constexpr int NA_TAP_RAW = AVAIL / (A_BYTES + B_BYTES);
   static constexpr int NA = WS ? 3 : (HALO ? 2 : (NA_TAP_RAW > kMaxA ? kMaxA : NA_TAP_RAW));
-  static constexpr int BUDGET = (227 - 6) * 1024 - NA * A_BYTES;  // 227 KB - alignment slack - static (barriers)
+  static constexpr int BUDGET = AVAIL - NA * A_BYTES;
   static constexpr int NB_RAW = BUDGET / B_BYTES;
   static constexpr int NB = NB_RAW > kMaxB ? kMaxB : NB_RAW;                 // weight ring depth
   static constexpr int ACC = MT * N;                                         // fp32 registers per thread
   static constexpr int SPU = HALO ? 9 : 1;                                   // steps per activation buffer
+  // register split, 128 P + 256 C <= 384 x 168 (what a CTA of 384 threads holds at launch); the consumers hold up to 128
+  // fp32 accumulators.  The producer warpgroup needs more than 40 when its warps 1-3 run the epilogue.
+  static constexpr int P_REGS = STAGE ? 88 : 40, C_REGS = STAGE ? 208 : 232;
+  static_assert(128 * P_REGS + 256 * C_REGS <= kDenseThreads * 168, "register split");
   static_assert(N == 16 || N == 64 || N == 128, "N tile: 16 (grouped output convs), 64 or 128");
   static_assert(MT == 1 || MT == 2, "one or two M tiles");
   static_assert(MT * N <= 128, "accumulators: at most 128 registers per thread");
@@ -109,9 +124,64 @@ __device__ __forceinline__ void split_h16(float x, __half &hi, __half &lo, bool 
   lo = __float2half_rn((x - __half2float(hi)) * kLoScale);
 }
 
+// split_h16 of two values with paired conversions (round to nearest either way: the same bits)
+__device__ __forceinline__ void split_h16x2(float a, float b, __half2 &hi, __half2 &lo, bool &ovf) {
+  if (fabsf(a) > 65504.0f) {
+    ovf = true;
+    a = copysignf(65504.0f, a);
+  }
+  if (fabsf(b) > 65504.0f) {
+    ovf = true;
+    b = copysignf(65504.0f, b);
+  }
+  hi = __floats2half2_rn(a, b);
+  const float2 h = __half22float2(hi);
+  lo = __floats2half2_rn((a - h.x) * kLoScale, (b - h.y) * kLoScale);
+}
+
 struct Item {
   int nt, tap0, tx0, ty0, b;
 };
+
+// Trace build (-DP3D_DENSE_TRACE, tools/dense_bench.py --trace): each role sums clock64 intervals of where it waits and
+// adds them per CTA to g_dense_trace, which p3d_dense_trace_read copies out.  Without the macro every Trace member is
+// empty and the kernel compiles to the code it has without the calls.
+enum TraceField {
+  kTrItems, kTrCycles,                  // items of the CTA; cycles of consumer warpgroup 1 from start-up to its exit
+  kTrAFull, kTrBFull = kTrAFull + 2,    // per consumer warpgroup: waiting on activation / weight "full"
+  kTrMma = kTrBFull + 2,                // per consumer warpgroup: in wgmma.wait_group
+  kTrEpi = kTrMma + 2,                  // per consumer warpgroup: after the item's last wait_group until the next item
+                                        // (WS: the epilogue; otherwise writing the staging tile)
+  kTrStageFree = kTrEpi + 2,            // per consumer warpgroup: waiting for the epilogue warps to free its staging tile
+  kTrAEmpty = kTrStageFree + 2, kTrBEmpty,  // producer: waiting on activation / weight "empty"
+  kTrEwWait, kTrEwBusy,                 // epilogue warp 1: waiting on "staged"; scale / shift / ReLU / split and stores
+  kTrFields
+};
+#ifdef P3D_DENSE_TRACE
+constexpr int kTrMaxCtas = 1024;
+__device__ unsigned long long g_dense_trace[kTrMaxCtas][kTrFields];
+struct Trace {
+  unsigned long long sum[kTrFields] = {};
+  __device__ __forceinline__ long long now() const { return clock64(); }
+  __device__ __forceinline__ void add(int f, long long t0) { sum[f] += static_cast<unsigned long long>(clock64() - t0); }
+  __device__ __forceinline__ void count(int f, unsigned long long v) { sum[f] += v; }
+  // per-warpgroup fields are summed in the first of their pair and land in pair entry cw
+  __device__ void flush(int cw) const {
+#pragma unroll
+    for (int f = 0; f < kTrFields; ++f) {
+      const int dst = f >= kTrAFull && f < kTrAEmpty ? f + cw : f;
+      if (sum[f]) atomicAdd(&g_dense_trace[blockIdx.x % kTrMaxCtas][dst], sum[f]);
+    }
+  }
+};
+#else
+struct Trace {
+  __device__ __forceinline__ long long now() const { return 0; }
+  __device__ __forceinline__ void add(int, long long) {}
+  __device__ __forceinline__ void count(int, unsigned long long) {}
+  __device__ __forceinline__ void flush(int) const {}
+};
+#endif
 template <bool WS = false>
 __device__ __forceinline__ Item decode(long long w, const Params &p, int th) {
   Item it;
@@ -137,6 +207,91 @@ __device__ __forceinline__ Item decode(long long w, const Params &p, int th) {
   return it;
 }
 
+// Epilogue warps (warps 1-3 of the producer warpgroup, thread et = 0 .. 95).  For every item, and for consumer warpgroup
+// c = 0, 1 in turn: wait until c has staged its rows, apply scale / shift and ReLU with the expressions of the in-register
+// epilogue (hence the same bits), write the outputs, and hand the tile back.  Pixel H16 rows: a lane takes four channels
+// of one pixel, so eight lanes write one pixel's 32-channel group as 64 contiguous bytes of hi and 64 of lo'.  fp32 NCHW
+// planes: a lane takes one pixel of an 8-pixel tile row, so eight lanes write 32 contiguous bytes of a plane.
+template <int N, int MT>
+__device__ __forceinline__ void epilogue_warps(const Params &p, const float *stg, unsigned long long *staged,
+                                               unsigned long long *freed, long long n_items, long long w_first,
+                                               long long w_step, int th, int et) {
+  constexpr int SP = N + 8, ROWS = MT * 64;  // staging row pitch (floats) and rows per consumer warpgroup (Cfg)
+  const int ew = et >> 5, lane = et & 31;
+  bool ovf = false;
+  Trace tr;
+  for (long long idx = 0; idx < n_items; ++idx) {
+    const Item im = decode<false>(w_first + idx * w_step, p, th);
+    const int g_cnt = p.grouped ? __ldg(p.grp_cnt + im.nt) : 0, g_p0 = p.grouped ? __ldg(p.grp_plane0 + im.nt) : 0;
+    const int dy = p.up > 1 ? im.tap0 / p.up : 0, dx = p.up > 1 ? im.tap0 % p.up : 0;
+    for (int c = 0; c < 2; ++c) {
+      long long t0 = tr.now();
+      mbar_wait(smem_u32(staged + c), static_cast<uint32_t>(idx & 1));
+      tr.add(kTrEwWait, t0);
+      t0 = tr.now();
+      const float *st = stg + c * ROWS * SP;
+      // staging row r of consumer c is pixel c * 64 + r % 64 of M tile r / 64; false outside the output
+      auto pixel = [&](int r, int &Y, int &X) {
+        const int m = c * 64 + (r & 63), iy = im.ty0 + (r >> 6) * kTH + m / kTW, ix = im.tx0 + m % kTW;
+        Y = iy * p.up + dy;
+        X = ix * p.up + dx;
+        return iy < p.oH && ix < p.oW;
+      };
+      if (N >= 32 && p.out_h16) {
+        const int r4 = lane >> 3, c4 = (lane & 7) * 4;  // row of a 4-row quad, first of four columns
+        for (int q = 0; q < N / 32; ++q) {
+          const int col = q * 32 + c4, ch = im.nt * N + col, oc = p.out_c0 + ch;
+          // channel counts of H16 layers are multiples of 16: the four columns are valid together
+          if (ch >= p.cout) continue;
+          float sc[4], sh[4];
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            sc[e] = p.scale ? __ldg(p.scale + ch + e) : 1.0f;
+            sh[e] = p.shift ? __ldg(p.shift + ch + e) : 0.0f;
+          }
+#pragma unroll 2
+          for (int rq = ew; rq < ROWS / 4; rq += 3) {
+            const int r = rq * 4 + r4;
+            int Y, X;
+            if (!pixel(r, Y, X)) continue;
+            const float4 o4 = *reinterpret_cast<const float4 *>(st + r * SP + col);
+            float v[4] = {o4.x, o4.y, o4.z, o4.w};
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              v[e] = fmaf(v[e], sc[e], sh[e]);
+              if (p.relu) v[e] = fmaxf(v[e], 0.f);
+            }
+            __half2 h01, l01, h23, l23;
+            split_h16x2(v[0], v[1], h01, l01, ovf);
+            split_h16x2(v[2], v[3], h23, l23, ovf);
+            uint8_t *op = p.out_h16 + ((static_cast<size_t>(im.b) * p.out_H + Y) * p.out_W + X) * (4 * static_cast<size_t>(p.out_C)) +
+                          (oc / 32) * 128 + (oc % 32) * 2;
+            *reinterpret_cast<uint2 *>(op) = make_uint2(*reinterpret_cast<const uint32_t *>(&h01), *reinterpret_cast<const uint32_t *>(&h23));
+            *reinterpret_cast<uint2 *>(op + 64) = make_uint2(*reinterpret_cast<const uint32_t *>(&l01), *reinterpret_cast<const uint32_t *>(&l23));
+          }
+        }
+      }
+      if (p.out_nchw) {
+        const int px = lane & 7, cc = lane >> 3;  // pixel of an 8-pixel tile row, channel of a 4-channel quad
+        for (int u = ew; u < (ROWS / 8) * (N / 4); u += 3) {
+          const int r = (u % (ROWS / 8)) * 8 + px, col = (u / (ROWS / 8)) * 4 + cc, ch = im.nt * N + col;
+          int Y, X;
+          if ((p.grouped ? col >= g_cnt : ch >= p.cout) || !pixel(r, Y, X)) continue;
+          const float sc = p.scale ? __ldg(p.scale + ch) : 1.0f, sh = p.shift ? __ldg(p.shift + ch) : 0.0f;
+          float v = fmaf(st[r * SP + col], sc, sh);
+          if (p.relu) v = fmaxf(v, 0.f);
+          const int plane = p.grouped ? g_p0 + col : ch;
+          p.out_nchw[((static_cast<size_t>(im.b) * p.cout + plane) * p.out_H + Y) * p.out_W + X] = v;
+        }
+      }
+      mbar_arrive(smem_u32(freed + c));
+      tr.add(kTrEwBusy, t0);
+    }
+  }
+  if (ovf && p.status) atomicOr(p.status, 1);
+  if (et == 0) tr.flush(0);
+}
+
 template <int N, int MT, bool HALO, int PITCH, bool WS = false>
 __global__ void __launch_bounds__(kDenseThreads, 1)
     dense_conv_f16_kernel(const __grid_constant__ CUtensorMap in_map, const Params p) {
@@ -158,9 +313,11 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   // full barriers: one producer arrive + the bytes of the load; empty barriers: one arrive per consumer warp once the
   // wgmma that read the slot have retired.  Activation full[NA] | empty[NA] | weight full[NB] | empty[NB] | WS image
-  // full | empty.
-  __shared__ __align__(8) unsigned long long s_bar[2 * kMaxA + 2 * kMaxB + 2];
+  // full | empty | staging tile of consumer c staged[2] (one arrive per consumer thread) | free[2] (one arrive per
+  // epilogue thread).
+  __shared__ __align__(8) unsigned long long s_bar[2 * kMaxA + 2 * kMaxB + 6];
   constexpr int kAF = 0, kAE = kMaxA, kBF = 2 * kMaxA, kBE = 2 * kMaxA + kMaxB, kWF = 2 * kMaxA + 2 * kMaxB, kWE = kWF + 1;
+  constexpr int kSS = kWE + 1, kSF = kSS + 2;
 
   const int tid = threadIdx.x, wg = tid >> 7, wtid = tid & 127;
   if (tid == 0) {
@@ -174,11 +331,17 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
     }
     mbar_init(smem_u32(&s_bar[kWF]), 1);
     mbar_init(smem_u32(&s_bar[kWE]), kConsumerWarps);
+    for (int c = 0; c < 2; ++c) {
+      mbar_init(smem_u32(&s_bar[kSS + c]), 128);
+      mbar_init(smem_u32(&s_bar[kSF + c]), kEpiThreads);
+    }
     fence_mbar_init();
   }
   __syncthreads();  // the only block-wide barrier: the mbarriers are initialised
   const uint32_t a_ring = smem_u32(smem);
   const uint32_t b_ring = a_ring + C::NA * C::A_BYTES;
+  // staging tiles of the two consumer warpgroups, after the weight ring
+  float *const stg = reinterpret_cast<float *>(smem + C::NA * C::A_BYTES + C::NB * C::B_BYTES);
   const int G = p.Cin / 32;
   // steps / activation units per item: HALO: one unit per group, 9 taps each; TAP: one unit per (tap, group)
   const int taps_item = p.up > 1 ? 1 : p.taps;
@@ -190,12 +353,17 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
   // complete, so the first NA / NB fills do not wait).
 
   if (wg == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(C::P_REGS));
+    if (tid >= 32) {
+      if (C::STAGE) epilogue_warps<N, MT>(p, stg, s_bar + kSS, s_bar + kSF, n_items, w_first, w_step, TH, tid - 32);
+      return;
+    }
     // ------------------------------------------------------------------------------------------ producer
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
     if (tid != 0) return;
     uint32_t a_slot = 0, a_ph = 0, b_slot = 0, b_ph = 0;
     int cur_nt = -1;  // WS: N tile whose weight image is resident
     uint32_t img = 0; // WS: images loaded so far
+    Trace tr;
     for (long long idx = 0; idx < n_items; ++idx) {
       const Item im = decode<WS>(item_w(idx), p, TH);
       const int cg0 = p.grouped ? im.nt * G : 0;  // first 32-channel group of this item's input channels
@@ -219,7 +387,9 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
         const int tap = p.up > 1 ? im.tap0 : tu;
         for (int g = 0; g < G; ++g) {
           const uint32_t abar = smem_u32(&s_bar[kAF + a_slot]), a_dst = a_ring + a_slot * C::A_BYTES;
+          const long long t0 = tr.now();
           mbar_wait(smem_u32(&s_bar[kAE + a_slot]), a_ph ^ 1u);
+          tr.add(kTrAEmpty, t0);
           mbar_arrive_expect_tx(abar, static_cast<uint32_t>(C::A_ROWS * 128));
           if (HALO) {
             tma_tile4d(a_dst, &in_map, (cg0 + g) * 64, im.tx0 - 1, im.ty0 - 1, im.b, abar);
@@ -230,7 +400,9 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
           if (++a_slot == C::NA) a_slot = 0, a_ph ^= 1u;
           for (int t = 0; t < (WS ? 0 : C::SPU); ++t) {
             const uint32_t bbar = smem_u32(&s_bar[kBF + b_slot]);
+            const long long t1 = tr.now();
             mbar_wait(smem_u32(&s_bar[kBE + b_slot]), b_ph ^ 1u);
+            tr.add(kTrBEmpty, t1);
             mbar_arrive_expect_tx(bbar, static_cast<uint32_t>(C::B_BYTES));
             bulk_g2s(b_ring + b_slot * C::B_BYTES, w_tile + (static_cast<size_t>(HALO ? t : tap) * (p.Cin / 16) + 2 * g) * C::B_BLK,
                      static_cast<uint32_t>(C::B_BYTES), bbar);
@@ -240,11 +412,12 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
         if (++dx == p.kw) dx = 0, ++dy;
       }
     }
+    tr.flush(0);
     return;
   }
 
   // -------------------------------------------------------------------------------------------- consumers
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(C::C_REGS));
   const int cw = wg - 1;                 // rows 64 cw .. 64 cw + 63 of every M tile
   const bool warp_leader = (tid & 31) == 0;
   auto release = [&](int base, uint32_t slot) {
@@ -255,6 +428,8 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
   int cur_nt = -1;   // WS: N tile whose weight image is resident
   uint32_t img = 0;  // WS: images used so far
   float acc[C::ACC];
+  Trace tr;
+  const long long t_start = tr.now();
   for (long long idx = 0; idx < n_items; ++idx) {
     const Item im = decode<WS>(item_w(idx), p, TH);
     if (WS && im.nt != cur_nt) {
@@ -270,10 +445,14 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
     int prev_a = -1;
     bool pending = false;
     for (int ua = 0; ua < units_item; ++ua) {
+      long long t0 = tr.now();
       mbar_wait(smem_u32(&s_bar[kAF + a_slot]), a_ph);
+      tr.add(kTrAFull, t0);
       const uint32_t a_base = a_ring + a_slot * C::A_BYTES;
       for (int t = 0; t < C::SPU; ++t) {
+        t0 = tr.now();
         if (!WS) mbar_wait(smem_u32(&s_bar[kBF + b_slot]), b_ph);
+        tr.add(kTrBFull, t0);
         const uint32_t b_base = WS ? b_ring + static_cast<uint32_t>((t * (p.Cin / 16) + 2 * ua) * C::B_BLK)
                                    : b_ring + b_slot * C::B_BYTES;
         wg_fence();
@@ -301,7 +480,9 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
           }
         }
         wg_commit();
+        t0 = tr.now();
         wg_wait<1>();  // the previous step's group has retired: its slots go back to the producer
+        tr.add(kTrMma, t0);
         if (pending) {
           if (!WS) release(kBE, prev_b);
           if (prev_a >= 0) release(kAE, static_cast<uint32_t>(prev_a));
@@ -313,14 +494,39 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
       }
       if (++a_slot == C::NA) a_slot = 0, a_ph ^= 1u;
     }
+    long long t0 = tr.now();
     wg_wait<0>();
+    tr.add(kTrMma, t0);
+    t0 = tr.now();
     if (!WS) release(kBE, prev_b);
     release(kAE, static_cast<uint32_t>(prev_a));  // the item's last step ends a unit
     // WS: the last item of a run on this N tile has retired every step that reads the image
     if (WS && (idx + 1 == n_items || decode<WS>(item_w(idx + 1), p, TH).nt != im.nt)) release(kWE, 0);
     wg_fence_acc<C::ACC>(acc);
+    if constexpr (C::STAGE) {
+      // park hi + cross * 2^-11 in this warpgroup's staging tile (row mt * 64 + fragment row) once the epilogue warps
+      // have drained the previous item from it, and go on with the next item
+      tr.add(kTrEpi, t0);
+      t0 = tr.now();
+      if (idx > 0) mbar_wait(smem_u32(&s_bar[kSF + cw]), static_cast<uint32_t>((idx - 1) & 1));
+      tr.add(kTrStageFree, t0);
+      t0 = tr.now();
+      float *const st = stg + cw * C::STG_WG;
+#pragma unroll
+      for (int mt = 0; mt < MT; ++mt) {
+#pragma unroll
+        for (int i = 0; i < H; i += 2) {
+          const int r = mt * 64 + frag_row(i, wtid), c = frag_col(i, wtid);
+          *reinterpret_cast<float2 *>(st + r * C::SP + c) =
+              make_float2(fmaf(acc[mt * N + H + i], kLoInv, acc[mt * N + i]), fmaf(acc[mt * N + H + i + 1], kLoInv, acc[mt * N + i + 1]));
+        }
+      }
+      mbar_arrive(smem_u32(&s_bar[kSS + cw]));
+      tr.add(kTrEpi, t0);
+      continue;
+    }
 
-    // ------------------------------------------------------------------------------------------ epilogue
+    // ------------------------------------------------------------- epilogue in the registers (WS only)
     const int g_cnt = p.grouped ? __ldg(p.grp_cnt + im.nt) : 0, g_p0 = p.grouped ? __ldg(p.grp_plane0 + im.nt) : 0;
 #pragma unroll
     for (int mt = 0; mt < MT; ++mt) {
@@ -363,8 +569,14 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
         }
       }
     }
+    tr.add(kTrEpi, t0);
   }
   if (ovf && p.status) atomicOr(p.status, 1);
+  if (cw == 0) {
+    tr.count(kTrItems, static_cast<unsigned long long>(n_items));
+    tr.add(kTrCycles, t_start);
+  }
+  if (wtid == 0) tr.flush(cw);
 }
 
 // fp32 NCHW image -> pixel H16 rows (32 x 32 tile transpose through shared memory)
@@ -437,7 +649,7 @@ template <int N, int MT, bool HALO, int PITCH, bool WS = false>
 int launch(const CUtensorMap &map, const Params &p, cudaStream_t st) {
   using C = Cfg<N, MT, HALO, PITCH, WS>;
   const size_t smem = static_cast<size_t>(C::NA) * C::A_BYTES +
-                      (WS ? static_cast<size_t>(p.w_bytes) : static_cast<size_t>(C::NB) * C::B_BYTES) + 1024;
+                      (WS ? static_cast<size_t>(p.w_bytes) : static_cast<size_t>(C::NB) * C::B_BYTES) + C::STG_BYTES + 1024;
   if (smem > static_cast<size_t>(227 - 6) * 1024) return P3D_ERR_UNSUPPORTED;
   auto kern = dense_conv_f16_kernel<N, MT, HALO, PITCH, WS>;
   P3D_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
@@ -634,6 +846,23 @@ extern "C" int p3d_pixel_h16_to_nchw(const void *in_h16, int B, int C, int H, in
   return P3D_OK;
 }
 
+#ifdef P3D_DENSE_TRACE
+// Trace build only (not in p3d_b200.h): copies the per-CTA sums of dcf::TraceField ([max_ctas][fields] uint64) to the
+// host and zeroes them when reset != 0.  Returns the number of fields per CTA.
+extern "C" int p3d_dense_trace_read(unsigned long long *host, int max_ctas, int reset) {
+  const size_t n = static_cast<size_t>(max_ctas < dcf::kTrMaxCtas ? max_ctas : dcf::kTrMaxCtas) * dcf::kTrFields;
+  P3D_CUDA_CHECK(cudaDeviceSynchronize());
+  if (host) P3D_CUDA_CHECK(cudaMemcpyFromSymbol(host, dcf::g_dense_trace, n * sizeof(unsigned long long)));
+  if (reset) {
+    void *dev = nullptr;
+    P3D_CUDA_CHECK(cudaGetSymbolAddress(&dev, dcf::g_dense_trace));
+    P3D_CUDA_CHECK(cudaMemset(dev, 0, sizeof(dcf::g_dense_trace)));
+    P3D_CUDA_CHECK(cudaDeviceSynchronize());
+  }
+  return dcf::kTrFields;
+}
+#endif
+
 // packed weights: per N tile the image p3d_sparse_conv_f16_pack_weights makes of W[tap][Cin][n_tile] (zero-padded columns)
 extern "C" size_t p3d_dense_conv2d_f16_packed_weight_bytes(int taps, int Cin, int Cout, int n_tile) {
   if (taps < 1 || Cin < 32 || Cin % 32 || Cout < 1 || (n_tile != 16 && n_tile != 32 && n_tile != 64 && n_tile != 128)) return 0;
@@ -692,7 +921,7 @@ static int dense_conv_f16(const void *in_h16, int B, int H, int W, int Cin, cons
   // (tests/test_gpu_dense.py); P3D_DENSE_BO=1 sets it to the address bits 7-9 instead
   static const int env_bo = getenv("P3D_DENSE_BO") ? atoi(getenv("P3D_DENSE_BO")) : 0;
   p.base_offset_mode = env_bo;
-  const int pitch = env_pitch == 16 ? 16 : 10;
+  int pitch = env_pitch == 16 ? 16 : 10;
   if (env_mode >= 0) mode = env_mode;
   if (env_mt >= 0) m_tiles = env_mt;
   const bool halo = (mode == 0 || mode == 2) && up == 1 && kh == 3 && kw == 3 && stride == 1 && pad == 1;
@@ -721,6 +950,7 @@ static int dense_conv_f16(const void *in_h16, int B, int H, int W, int Cin, cons
   }
   if (mode == 2 && !ws) return P3D_ERR_UNSUPPORTED;
   if (ws || n_tile > 64) mt = 1;  // two M tiles of a 128-wide N tile would need 256 accumulator registers per thread
+  if (mt == 2) pitch = 10;        // two haloed M tiles at pitch 16 leave no room for the epilogue's staging tiles
   p.tiles_x = (p.oW + dcf::kTW - 1) / dcf::kTW;
   p.tiles_y = (p.oH + dcf::kTH * mt - 1) / (dcf::kTH * mt);
   CUtensorMap map;
@@ -732,7 +962,7 @@ static int dense_conv_f16(const void *in_h16, int B, int H, int W, int Cin, cons
 #define P3D_DCF(NT, M)                                                                          \
   if (n_tile == NT && mt == M) {                                                                \
     if (!halo) return dcf::launch<NT, M, false, 10>(map, p, st);                                \
-    if (pitch == 16) return dcf::launch<NT, M, true, 16>(map, p, st);                           \
+    if (M == 1 && pitch == 16) return dcf::launch<NT, 1, true, 16>(map, p, st);                 \
     return dcf::launch<NT, M, true, 10>(map, p, st);                                            \
   }
   P3D_DCF(16, 1)

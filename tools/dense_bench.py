@@ -4,11 +4,19 @@
 Graph-replayed, one JSON line per distinct layer shape and kernel variant with its algorithmic TFLOP/s (2 * MACs of the
 convolution; the kernels execute 3 fp16 MMAs per product), then the whole head.  Needs a GPU:
     python tools/dense_bench.py [--variants] [> dense_layers.jsonl]
+
+--trace builds the library with -DP3D_DENSE_TRACE into a temporary directory and prints, per layer, where the dense
+kernel's time goes, in SM cycles per work item (summed over the CTAs, divided by the items): the consumer warpgroups'
+waits on the activation / weight "full" barriers, in wgmma.wait_group, their epilogue (staging the accumulators) and
+their waits for a free staging tile; the producer thread's waits on "empty" barriers; the epilogue warps' waits on
+"staged" and their busy time.  Cycles are clock64 counts; the trace build is slower than the default one.
 """
 import argparse
+import ctypes
 import json
 import os
 import sys
+import tempfile
 
 import numpy as np
 import torch
@@ -38,21 +46,68 @@ def graph_time(fn, iters=10):
     return a.elapsed_time(b) / iters * 1e3  # us
 
 
+SHAPES = [  # (name, cin, cout, k, stride, pad, up, h, w) at the C3 BEV size 180 x 180
+    ("backbone0 256->128 s1", 256, 128, 3, 1, 1, 1, 180, 180), ("backbone0 128->128", 128, 128, 3, 1, 1, 1, 180, 180),
+    ("backbone1 128->256 s2", 128, 256, 3, 2, 1, 1, 180, 180), ("backbone1 256->256", 256, 256, 3, 1, 1, 1, 90, 90),
+    ("neck 1x1 128->256", 128, 256, 1, 1, 0, 1, 180, 180), ("neck deconv 256->256 x2", 256, 256, 2, 2, 0, 2, 90, 90),
+    ("shared 512->64", 512, 64, 3, 1, 1, 1, 180, 180), ("heads 64->2304 (36 batched)", 64, 2304, 3, 1, 1, 1, 180, 180),
+]
+# per-CTA fields of the trace build (dcf::TraceField in csrc/dense_conv_f16.cu)
+TRACE_FIELDS = ["items", "cycles", "a_full", "a_full_1", "b_full", "b_full_1", "mma_wait", "mma_wait_1", "epilogue",
+                "epilogue_1", "stage_free", "stage_free_1", "prod_a_empty", "prod_b_empty", "epi_warps_wait",
+                "epi_warps_busy"]
+
+
+def trace():
+    from paddle3d_b200 import _lib
+    from paddle3d_b200 import build as b
+    out = tempfile.mkdtemp(prefix="p3d_dense_trace_")
+    _lib.LIB_PATH = b.build(out_dir=out, extra_flags=["-DP3D_DENSE_TRACE"])
+    rd = _lib.lib().p3d_dense_trace_read
+    rd.restype, rd.argtypes = ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_int]
+    nf = rd(None, 0, 1)
+    assert nf == len(TRACE_FIELDS), "trace fields: library %d, tool %d" % (nf, len(TRACE_FIELDS))
+    dev = torch.device("cuda:0")
+    torch.cuda.set_device(dev)
+    rng = np.random.default_rng(0)
+    max_ctas = 1024
+    buf = np.zeros((max_ctas, nf), np.uint64)
+    for name, cin, cout, k, s, p, up, h, w in SHAPES:
+        conv = _Conv(cin, cout, k, s, p, bias=True, bn_eps=1e-3, up=up, f16=True).init(rng, dev)
+        x = (torch.randn((h * w, 2 * cin), device=dev) * 0.5).to(torch.float16)
+        conv(x, (1, h, w, cin))  # warm-up
+        reps = 5
+        rd(None, 0, 1)
+        for _ in range(reps):
+            conv(x, (1, h, w, cin))
+        _lib.check(0 if rd(buf.ctypes.data, max_ctas, 1) == nf else -1, "p3d_dense_trace_read")
+        tot = buf.sum(0).astype(np.float64)
+        items = tot[0]
+        per = {f: tot[i] / items for i, f in enumerate(TRACE_FIELDS) if i > 0}
+        row = {"layer": name, "items": int(items / reps), "ctas": int((buf[:, 0] > 0).sum()),
+               "cycles_per_item": round(per["cycles"])}
+        cons = ("a_full", "b_full", "mma_wait", "epilogue", "stage_free")
+        for f in cons:  # mean of the two consumer warpgroups
+            row[f] = round((per[f] + per[f + "_1"]) / 2)
+        row["other"] = row["cycles_per_item"] - sum(row[f] for f in cons)
+        for f in ("prod_a_empty", "prod_b_empty", "epi_warps_wait", "epi_warps_busy"):
+            row[f] = round(per[f])
+        print(json.dumps(row), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--variants", action="store_true", help="time every (mode, m_tiles) variant of each layer")
     ap.add_argument("--tf32", action="store_true", help="also time the round-1 tf32-pair kernels")
+    ap.add_argument("--trace", action="store_true", help="per-layer wait breakdown of the -DP3D_DENSE_TRACE build")
     args = ap.parse_args()
+    if args.trace:
+        return trace()
     dev = torch.device("cuda:0")
     torch.cuda.set_device(dev)
     rng = np.random.default_rng(0)
     H = W = 180
-    shapes = [  # (name, cin, cout, k, stride, pad, up, h, w)
-        ("backbone0 256->128 s1", 256, 128, 3, 1, 1, 1, H, W), ("backbone0 128->128", 128, 128, 3, 1, 1, 1, H, W),
-        ("backbone1 128->256 s2", 128, 256, 3, 2, 1, 1, H, W), ("backbone1 256->256", 256, 256, 3, 1, 1, 1, H // 2, W // 2),
-        ("neck 1x1 128->256", 128, 256, 1, 1, 0, 1, H, W), ("neck deconv 256->256 x2", 256, 256, 2, 2, 0, 2, H // 2, W // 2),
-        ("shared 512->64", 512, 64, 3, 1, 1, 1, H, W), ("heads 64->2304 (36 batched)", 64, 2304, 3, 1, 1, 1, H, W),
-    ]
+    shapes = SHAPES
     variants = [(0, 0)] + ([(0, 1), (0, 2), (1, 1), (1, 2)] if args.variants else [])
     for name, cin, cout, k, s, p, up, h, w in shapes:
         oh, ow = (h * up, w * up) if up > 1 else ((h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1)
