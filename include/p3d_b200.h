@@ -382,7 +382,7 @@ int p3d_dense_conv2d_f16(const void *in_h16, int B, int H, int W, int Cin, const
                          void *out_h16, int out_C, int out_c0, float *out_nchw, int mode, int m_tiles,
                          int32_t *status_dev, p3d_stream_t stream);
 
-/* EXPERIMENTAL (never run on a GPU yet), SURVEY.md 8f-2: PillarFeatureNet with one PFNLayer
+/* SURVEY.md 8f-2: PillarFeatureNet with one PFNLayer
  * (models/voxel_encoders/pillar_encoder.py:156-210, :81-106) fused into one launch: voxels [n, M, F] + counts + coors
  * [n, 4] (b, z, y, x) -> pillar features [n, C].  weight [F + 5, C] (paddle.nn.Linear layout, no bias); BatchNorm1D
  * folded by the caller: y = x * bn_scale[c] + bn_shift[c].  Rows >= *num_voxels_dev (if given) are left untouched. */
@@ -391,6 +391,29 @@ int p3d_pillar_feature_net(const float *voxels, const int32_t *num_points_per_vo
                            int out_channels, const float *weight, const float *bn_scale, const float *bn_shift,
                            const float *voxel_size_host, const float *point_cloud_range_host, float *out,
                            p3d_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * anchor_head_postprocess      SECOND v1.5 VoxelNet.predict (the path SSDHead.post_process -> rotate_nms_pcdet ports)
+ *                              for one class at batch 1, with no host synchronisation.
+ *   head [1, 10 R, H, W] fp32 planes: cls [R] | box [R x 7] | dir [R x 2]; channel a * K + k belongs to anchor
+ *   (y * W + x) * R + a.  anchors [A, 7] (x, y, z, w, l, h, theta), A = H * W * R;  anchor_corners [A, 4] int32
+ *   (x_min, y_min, x_max, y_max) clamped voxel indices of each anchor's near box (16-byte aligned).
+ *   coords [coords_cap, 4] (b, z, y, x) of the pillars, *num_coords_dev of them valid (null: all).
+ *   Anchors whose occupied-pillar count over the near box is <= anchor_area_threshold are dropped; then
+ *   sigmoid(cls) >= score_threshold, descending-score order with ties by ascending anchor index, the first
+ *   nms_pre_max_size, rotated NMS, the first nms_post_max_size kept, direction fix, centre range filter.
+ *   Outputs (device): boxes [nms_post_max_size, 7], scores, labels int64 (0), counts [2] int32 = (score-threshold
+ *   candidates, rows written).  Optional (null to skip): anchor_mask [A] uint8, and the decoded candidates in
+ *   score order before NMS: sorted_boxes [nms_pre_max_size, 7], sorted_scores [nms_pre_max_size].
+ * ------------------------------------------------------------------------------------------- */
+size_t p3d_anchor_head_postprocess_workspace_bytes(int num_anchors, int grid_nx, int grid_ny, int nms_pre_max_size);
+int p3d_anchor_head_postprocess(const float *head, int feat_h, int feat_w, int anchors_per_loc, const float *anchors,
+                                const int32_t *anchor_corners, const int32_t *coords, const int32_t *num_coords_dev,
+                                int coords_cap, int grid_nx, int grid_ny, int anchor_area_threshold, float score_threshold,
+                                float nms_iou_threshold, int nms_pre_max_size, int nms_post_max_size,
+                                const float *post_center_range_host, float *boxes, float *scores, int64_t *labels,
+                                int32_t *counts, uint8_t *anchor_mask, float *sorted_boxes, float *sorted_scores,
+                                void *workspace, size_t workspace_bytes, p3d_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -95,6 +95,9 @@ SIGNATURES = {
                                                      _vp, _sz, _vp]),
     "p3d_sparse_conv_gather_gemm": (_int, [_vp, _vp, _vp, _i64, _int, _int, _int, _vp, _vp, _vp, _vp, _int, _int,
                                            _vp, _vp]),
+    "p3d_anchor_head_postprocess_workspace_bytes": (_sz, [_int, _int, _int, _int]),
+    "p3d_anchor_head_postprocess": (_int, [_vp, _int, _int, _int, _vp, _vp, _vp, _vp, _int, _int, _int, _int, _f, _f,
+                                           _int, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
 }
 
 

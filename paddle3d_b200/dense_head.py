@@ -20,8 +20,11 @@ COMMON_HEADS = (("reg", 2), ("height", 1), ("dim", 3), ("rot", 2), ("vel", 2))  
 class _Conv:
     """Conv2D / Conv2DTranspose (+ BatchNorm2D eval) (+ ReLU) with seeded parameters."""
 
-    def __init__(self, cin, cout, k, stride=1, padding=0, bias=False, bn_eps=None, relu=True, up=1, f16=True):
+    def __init__(self, cin, cout, k, stride=1, padding=0, bias=False, bn_eps=None, relu=True, up=1, f16=True, transposed=False):
+        """transposed: a stride-1 Conv2DTranspose (weight [Cin, Cout, k, k]); with k = 1 it runs as a 1x1 conv whose packed
+        weight is the transpose (up > 1 implies a transposed conv)."""
         self.cin, self.cout, self.k, self.stride, self.padding, self.up = cin, cout, k, stride, padding, up
+        self.transposed = transposed or up > 1
         self.has_bias, self.bn_eps, self.relu = bias, bn_eps, relu
         self.f16 = f16 and cout >= 16  # the 1-3 channel output convs of the heads run on the CUDA cores (forward)
         self.n_tile = dc.n_tile_for_f16(cout, cin, k, stride, padding, up) if self.f16 else dc.n_tile_for(cout)
@@ -32,13 +35,14 @@ class _Conv:
         """Seeded parameters (numpy); with a device also the packed tensor-core image and the folded epilogue."""
         cin, cout, k = self.cin, self.cout, self.k
         bound = 1.0 / np.sqrt(cin * k * k)  # build_conv_layer "uniform" (second_backbone.py:43-48)
-        shape = (cin, cout, k, k) if self.up > 1 else (cout, cin, k, k)
+        shape = (cin, cout, k, k) if self.transposed else (cout, cin, k, k)
         w = rng.uniform(-bound, bound, size=shape).astype(np.float32)
         b = None
         if self.has_bias:
             b = (np.full(cout, bias_value, np.float32) if bias_value is not None
                  else rng.uniform(-bound, bound, size=cout).astype(np.float32))
-        p = dict(weight=w, bias=b, stride=self.stride, padding=self.padding, up=self.up, relu=self.relu, bn=None)
+        p = dict(weight=w, bias=b, stride=self.stride, padding=self.padding, up=self.up, relu=self.relu, bn=None,
+                 transposed=self.transposed)
         if self.bn_eps is not None:
             if randomize_bn:
                 g, bt = rng.uniform(0.5, 1.5, cout), rng.uniform(-0.2, 0.2, cout)
@@ -59,9 +63,9 @@ class _Conv:
         if device is None:
             return self
         if self.f16:
-            pack = dc.pack_deconv_weight_f16 if self.up > 1 else dc.pack_conv_weight_f16
+            pack = dc.pack_deconv_weight_f16 if self.transposed else dc.pack_conv_weight_f16
         else:
-            pack = dc.pack_deconv_weight if self.up > 1 else dc.pack_conv_weight
+            pack = dc.pack_deconv_weight if self.transposed else dc.pack_conv_weight
         self.dev = dict(
             packed=pack(torch.from_numpy(w).to(device), self.n_tile),
             scale=torch.from_numpy(s.astype(np.float32)).to(device) if p["bn"] is not None else None,
@@ -79,6 +83,62 @@ class _Conv:
                                d["scale"], d["shift"], self.relu, **kw)
 
 
+class SecondTrunk:
+    """SecondBackbone (second_backbone.py:72-120) + SecondFPN (second_fpn.py:99-160): strided 3x3 conv blocks, then one
+    deblock per block, all written into one channel-concat pixel image (`out_c0`).  BatchNorm eps 1e-3 throughout."""
+
+    def __init__(self, in_channels, out_channels, layer_nums, downsample_strides, fpn_out_channels, upsample_strides,
+                 use_conv_for_no_stride=True, f16=True):
+        self.f16 = f16
+
+        def conv(*a, **k):
+            return _Conv(*a, f16=f16, **k)
+        bn3 = 1e-3
+        self.blocks = []
+        cin = in_channels
+        for cout, n, s in zip(out_channels, layer_nums, downsample_strides):
+            blk = [conv(cin, cout, 3, s, 1, bn_eps=bn3)] + [conv(cout, cout, 3, 1, 1, bn_eps=bn3) for _ in range(n)]
+            self.blocks.append(blk)
+            cin = cout
+        self.deblocks = []
+        for ci, co, u in zip(out_channels, fpn_out_channels, upsample_strides):
+            # stride > 1 -> Conv2DTranspose k = s; stride 1 -> Conv2D k = 1 with use_conv_for_no_stride, else
+            # Conv2DTranspose k = 1 (second_fpn.py:118-139)
+            if u > 1:
+                self.deblocks.append(conv(ci, co, u, u, 0, bn_eps=bn3, up=u))
+            else:
+                self.deblocks.append(conv(ci, co, 1, 1, 0, bn_eps=bn3, transposed=not use_conv_for_no_stride))
+        self.fpn_channels = int(sum(fpn_out_channels))
+
+    def convs(self):
+        return [c for blk in self.blocks for c in blk] + list(self.deblocks)
+
+    def export_numpy(self):
+        return dict(blocks=[[c.np for c in blk] for blk in self.blocks], deblocks=[c.np for c in self.deblocks])
+
+    def __call__(self, x, shape, first=None):
+        """x: pixel rows [B*H*W, 2*C] (fp16 pairs or tf32 split) with shape = (B, H, W, C); first replaces the first conv.
+        Returns (concat image [B*oH*oW, 2*fpn_channels], (B, oH, oW, fpn_channels))."""
+        b = shape[0]
+        feats = []
+        for bi, blk in enumerate(self.blocks):
+            for ci, conv in enumerate(blk):
+                if bi == 0 and ci == 0 and first is not None:
+                    conv = first
+                x, _, (b_, oh, ow) = conv(x, shape)
+                shape = (b_, oh, ow, conv.cout)
+            feats.append((x, shape))
+        cat, c0, out_hw = None, 0, None
+        for (f, fshape), de in zip(feats, self.deblocks):
+            if cat is None:
+                out_hw = (fshape[1] * de.up, fshape[2] * de.up)
+                cat = torch.empty((fshape[0] * out_hw[0] * out_hw[1], 2 * self.fpn_channels),
+                                  dtype=torch.float16 if self.f16 else torch.float32, device=x.device)
+            de(f, fshape, out_split=cat, out_channels=self.fpn_channels, out_c0=c0)
+            c0 += de.cout
+        return cat, (b, out_hw[0], out_hw[1], self.fpn_channels)
+
+
 class DenseRPNHead:
     def __init__(self, in_channels=256, out_channels=(128, 256), layer_nums=(5, 5), downsample_strides=(1, 2),
                  fpn_out_channels=(256, 256), upsample_strides=(1, 2), tasks=(1, 2, 2, 1, 2, 2), share_conv_channel=64,
@@ -91,18 +151,10 @@ class DenseRPNHead:
 
         def conv(*a, **k):
             return _Conv(*a, f16=f16, **k)
-        bn3, bn5 = 1e-3, 1e-5
-        self.blocks = []
-        cin = in_channels
-        for cout, n, s in zip(out_channels, layer_nums, downsample_strides):
-            blk = [conv(cin, cout, 3, s, 1, bn_eps=bn3)] + [conv(cout, cout, 3, 1, 1, bn_eps=bn3) for _ in range(n)]
-            self.blocks.append(blk)
-            cin = cout
-        self.deblocks = []
-        for ci, co, u in zip(out_channels, fpn_out_channels, upsample_strides):
-            # use_conv_for_no_stride: stride 1 -> Conv2D k = 1; stride > 1 -> Conv2DTranspose k = s (second_fpn.py:118-139)
-            self.deblocks.append(conv(ci, co, 1, 1, 0, bn_eps=bn3) if u == 1 else conv(ci, co, u, u, 0, bn_eps=bn3, up=u))
-        self.fpn_channels = int(sum(fpn_out_channels))
+        bn5 = 1e-5
+        self.trunk = SecondTrunk(in_channels, out_channels, layer_nums, downsample_strides, fpn_out_channels,
+                                 upsample_strides, use_conv_for_no_stride=True, f16=f16)
+        self.blocks, self.deblocks, self.fpn_channels = self.trunk.blocks, self.trunk.deblocks, self.trunk.fpn_channels
         self.shared = conv(self.fpn_channels, share_conv_channel, 3, 1, 1, bias=True, bn_eps=bn5)
         self.heads = []  # per task: list of (name, ConvModule 64->64, final conv 64->classes)
         for ncls in self.tasks:
@@ -114,7 +166,7 @@ class DenseRPNHead:
         self._batched = None
 
     def all_convs(self):
-        out = [c for blk in self.blocks for c in blk] + list(self.deblocks) + [self.shared]
+        out = self.trunk.convs() + [self.shared]
         for hs in self.heads:
             for _, a, b in hs:
                 out += [a, b]
@@ -147,8 +199,8 @@ class DenseRPNHead:
         return self
 
     def export_numpy(self):
-        return dict(blocks=[[c.np for c in blk] for blk in self.blocks], deblocks=[c.np for c in self.deblocks],
-                    shared=self.shared.np, heads=[[(n, a.np, b.np) for n, a, b in hs] for hs in self.heads])
+        return dict(self.trunk.export_numpy(), shared=self.shared.np,
+                    heads=[[(n, a.np, b.np) for n, a, b in hs] for hs in self.heads])
 
     # ---- RPN + neck + shared conv: bev [B, C, H, W] fp32 -> (pixel rows of the shared feature map, its shape)
     def _trunk(self, bev, shape=None):
@@ -162,25 +214,8 @@ class DenseRPNHead:
             if not self.f16 or self._first_zc is None:
                 raise ValueError("pixel fp16-pair input needs the f16 head")
             x = bev
-            b = shape[0]
             first = self._first_zc  # channels arrive in (z, c) order
-        feats = []
-        for bi, blk in enumerate(self.blocks):
-            for ci, conv in enumerate(blk):
-                if bi == 0 and ci == 0 and first is not None:
-                    conv = first
-                x, _, (b_, oh, ow) = conv(x, shape)
-                shape = (b_, oh, ow, conv.cout)
-            feats.append((x, shape))
-        cat, c0, out_hw = None, 0, None
-        for (f, fshape), de in zip(feats, self.deblocks):
-            if cat is None:
-                out_hw = (fshape[1] * de.up, fshape[2] * de.up)
-                cat = torch.empty((fshape[0] * out_hw[0] * out_hw[1], 2 * self.fpn_channels),
-                                  dtype=torch.float16 if self.f16 else torch.float32, device=bev.device)
-            de(f, fshape, out_split=cat, out_channels=self.fpn_channels, out_c0=c0)
-            c0 += de.cout
-        H, W = out_hw
+        cat, (b, H, W, _) = self.trunk(x, shape, first=first)
         s, _, _ = self.shared(cat, (b, H, W, self.fpn_channels))
         return s, (b, H, W, self.shared.cout)
 

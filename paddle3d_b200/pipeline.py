@@ -40,96 +40,19 @@ def _count_graph_nodes(raw_graph):
     return out
 
 
-class CenterPointHotPath:
-    def __init__(self, cfg=None, device="cuda:0", precision=sp.FP32, seed=0, num_points=None, level_caps=None,
-                 head_seed=0, with_head=False, keep_bev=True, bn_gain=1.0):
-        self.cfg = dict(cfg or synth.C3)
-        self.device = torch.device(device)
-        self.n = int(num_points or self.cfg["num_points"])
-        self.F = self.cfg["point_dim"]
-        self.test_cfg = dict(synth.CENTERPOINT_TEST_CFG)
-        self.label_off = synth.label_offsets()
-        self.net = SparseResNet3D(self.F, self.cfg["voxel_size"], self.cfg["point_cloud_range"])
-        self.net.init_weight(seed=seed, device=self.device, bn_gain=bn_gain).set_precision(precision)
-        V = self.cfg["max_voxels"]
-        self.net.set_level_caps(level_caps or [3 * V, 3 * V, 2 * V, V])
-        h = synth.centerpoint_head_outputs(head_seed)
-        self.head_host = h
-        self.head = {k: [torch.from_numpy(x).to(self.device) for x in v] for k, v in h.items()}
-        # with_head: run the dense RPN / neck / CenterHead (dense_head.DenseRPNHead, SURVEY §8f-1) on the BEV tensor and
-        # feed ITS outputs to the postprocess instead of the resident synthetic head tensors (parity-green per layer and
-        # as a small network; this whole-frame composition has not been timed yet, hence off by default)
-        self.dense = None
-        if with_head:
-            from .dense_head import DenseRPNHead
-            self.dense = DenseRPNHead(in_channels=128 * 2).init_weight(seed=seed + 1, device=self.device, bn_gain=bn_gain)
-        # keep_bev=False (with the fp16-pair dense head): the sparse rows go straight into the pixel fp16-pair image the RPN
-        # reads; the reference's fp32 NCHW BEV tensor is then not materialised in the frame (bev_nchw() rebuilds it on demand)
-        self.keep_bev = keep_bev or self.dense is None or not self.dense.f16
-        self.points = torch.zeros((self.n, self.F), dtype=torch.float32, device=self.device)  # static input
-        self.graph = None
-        self.out = None
-        self.stream = torch.cuda.Stream(self.device)
-        rows = len(self.label_off) * self.test_cfg["nms_post_max_size"]
-        self.h_boxes = torch.empty((rows, 9), dtype=torch.float32).pin_memory()
+class CapturedFrame:
+    """Plumbing shared by the captured hot-path frames (CenterPointHotPath, pointpillars.PointPillarsHotPath): warm-up and
+    CUDA-graph capture of forward_device() on a side stream, the public infer() / infer_many() calls and their pinned
+    result slots.  A subclass sets self.device / self.points / self.stream / self.graph = self.out = None, calls
+    _alloc_host_outputs, and defines forward_device() (returning at least boxes / scores / labels / counts / status, with
+    counts[-1] the number of valid rows) and check_status()."""
+
+    def _alloc_host_outputs(self, rows, box_dims, n_counts, n_status):
+        self.h_boxes = torch.empty((rows, box_dims), dtype=torch.float32).pin_memory()
         self.h_scores = torch.empty((rows,), dtype=torch.float32).pin_memory()
         self.h_labels = torch.empty((rows,), dtype=torch.int64).pin_memory()
-        self.h_counts = torch.empty((len(self.label_off) + 1,), dtype=torch.int32).pin_memory()
-        self.h_status = torch.zeros((5,), dtype=torch.int32).pin_memory()
-
-    # ---- one frame, enqueued on the current stream, device in / device out
-    def forward_device(self):
-        cfg, tc = self.cfg, self.test_cfg
-        mean, coors, npv, nv = vox.voxelize_mean(self.points, cfg["voxel_size"], cfg["point_cloud_range"],
-                                                 cfg["max_points"], cfg["max_voxels"], 0)
-        bev, bev_h16 = None, None
-        if self.keep_bev:
-            bev = self.net(mean, coors, 1, num=nv)
-            h = self.dense(bev) if self.dense is not None else self.head
-        else:
-            bev_h16 = self.net(mean, coors, 1, num=nv, pixel_h16=True)
-            h = self.dense.forward_h16(*bev_h16)
-        # frame status word (ADVICE r1): [fp16-range overflow of the pair-row kernels, overflow flag of each strided level]
-        status = torch.stack([sp.status_tensor(self.device)[0]] + [c[1] for c in self.net.level_counters])
-        boxes, scores, labels, counts = cpp.centerpoint_postprocess_device(
-            h["hm"], h["reg"], h["height"], h["dim"], h["vel"], h["rot"], cfg["voxel_size"][:2],
-            cfg["point_cloud_range"], tc["post_center_limit_range"], self.label_off, tc["down_ratio"],
-            tc["score_threshold"], tc["nms_iou_threshold"], tc["nms_pre_max_size"], tc["nms_post_max_size"], True)
-        return dict(bev=bev, bev_h16=bev_h16, boxes=boxes, scores=scores, labels=labels, counts=counts, num_voxels=nv,
-                    coors=coors, mean=mean, status=status)
-
-    def bev_nchw(self):
-        """The dense BEV tensor [1, 256, H, W] fp32 of the last frame (rebuilt from the pixel fp16-pair image when the
-        frame did not materialise it)."""
-        if self.out["bev"] is not None:
-            self.stream.synchronize()
-            return self.out["bev"]
-        from .ops import dense_conv as dc
-        rows, shape = self.out["bev_h16"]
-        with torch.cuda.stream(self.stream):
-            out = dc.pixel_h16_to_nchw(rows, shape)
-            # pixel rows hold (z, c)-ordered channels (to_pixel_h16); the reference tensor is (c, z)-ordered
-            b, h, w, cd = shape
-            D = self.dense.bev_depth
-            out = out.view(b, D, cd // D, h, w).transpose(1, 2).reshape(b, cd, h, w).contiguous()
-        self.stream.synchronize()  # callers read it from other streams
-        return out
-
-    def calibrate_head(self, points_dev):
-        """Shift the heat-map biases of the (randomly initialised) dense head so that ~1.4 % of the BEV cells of this frame
-        score above the threshold, as SURVEY.md §8d specifies for the synthetic workload (see
-        DenseRPNHead.calibrate_heatmap_bias).  Call before capture()."""
-        if self.dense is None:
-            return self
-        cfg = self.cfg
-        with torch.cuda.stream(self.stream):
-            self.points.copy_(points_dev)
-            mean, coors, npv, nv = vox.voxelize_mean(self.points, cfg["voxel_size"], cfg["point_cloud_range"],
-                                                     cfg["max_points"], cfg["max_voxels"], 0)
-            bev = self.net(mean, coors, 1, num=nv)
-            self.dense.calibrate_heatmap_bias(bev, self.test_cfg["score_threshold"])
-        self.stream.synchronize()
-        return self
+        self.h_counts = torch.empty((n_counts,), dtype=torch.int32).pin_memory()
+        self.h_status = torch.zeros((n_status,), dtype=torch.int32).pin_memory()
 
     def capture(self, warmup=2, count_nodes=False):
         """Warm up (sizes the workspaces) on the side stream, then capture the frame into a CUDA graph.  count_nodes:
@@ -158,7 +81,7 @@ class CenterPointHotPath:
 
     # ---- public end-to-end call: host points in, host boxes out
     def infer(self, points_host):
-        """points_host: pinned [n, F] fp32 tensor.  Returns (boxes [K,9], scores [K], labels [K]) on the host."""
+        """points_host: pinned [n, F] fp32 tensor.  Returns (boxes [K, 9 or 7], scores [K], labels [K]) on the host."""
         with torch.cuda.stream(self.stream):
             self.points.copy_(points_host, non_blocking=True)
             if self.graph is not None:
@@ -175,18 +98,6 @@ class CenterPointHotPath:
         self.check_status(self.h_status)
         k = int(self.h_counts[-1])
         return self.h_boxes[:k], self.h_scores[:k], self.h_labels[:k]
-
-    @staticmethod
-    def check_status(status_host):
-        """Raise when the frame's device status word reports dropped work (never a silent wrong result)."""
-        st = [int(v) for v in status_host]
-        if st[0]:
-            raise RuntimeError("sparse backbone: an activation left fp16's range (|x| >= 65504) on the fp16-pair path; "
-                               "run this model with precision TF32X3_SPLIT")
-        for lvl, v in enumerate(st[1:]):
-            if v:
-                raise RuntimeError("sparse backbone: strided level %d overflowed its row capacity (set_level_caps); "
-                                   "output sites were dropped" % (lvl + 1))
 
     # ---- public end-to-end call for a sweep of frames: same per-frame work, copies overlapped with compute
     def prepare_sweep(self):
@@ -257,6 +168,108 @@ class CenterPointHotPath:
                self.h_status.numel() * 4)
         return h2d, d2h
 
+
+class CenterPointHotPath(CapturedFrame):
+    def __init__(self, cfg=None, device="cuda:0", precision=sp.FP32, seed=0, num_points=None, level_caps=None,
+                 head_seed=0, with_head=False, keep_bev=True, bn_gain=1.0):
+        self.cfg = dict(cfg or synth.C3)
+        self.device = torch.device(device)
+        self.n = int(num_points or self.cfg["num_points"])
+        self.F = self.cfg["point_dim"]
+        self.test_cfg = dict(synth.CENTERPOINT_TEST_CFG)
+        self.label_off = synth.label_offsets()
+        self.net = SparseResNet3D(self.F, self.cfg["voxel_size"], self.cfg["point_cloud_range"])
+        self.net.init_weight(seed=seed, device=self.device, bn_gain=bn_gain).set_precision(precision)
+        V = self.cfg["max_voxels"]
+        self.net.set_level_caps(level_caps or [3 * V, 3 * V, 2 * V, V])
+        h = synth.centerpoint_head_outputs(head_seed)
+        self.head_host = h
+        self.head = {k: [torch.from_numpy(x).to(self.device) for x in v] for k, v in h.items()}
+        # with_head: run the dense RPN / neck / CenterHead (dense_head.DenseRPNHead, SURVEY §8f-1) on the BEV tensor and
+        # feed ITS outputs to the postprocess instead of the resident synthetic head tensors (parity-green per layer and
+        # as a small network; this whole-frame composition has not been timed yet, hence off by default)
+        self.dense = None
+        if with_head:
+            from .dense_head import DenseRPNHead
+            self.dense = DenseRPNHead(in_channels=128 * 2).init_weight(seed=seed + 1, device=self.device, bn_gain=bn_gain)
+        # keep_bev=False (with the fp16-pair dense head): the sparse rows go straight into the pixel fp16-pair image the RPN
+        # reads; the reference's fp32 NCHW BEV tensor is then not materialised in the frame (bev_nchw() rebuilds it on demand)
+        self.keep_bev = keep_bev or self.dense is None or not self.dense.f16
+        self.points = torch.zeros((self.n, self.F), dtype=torch.float32, device=self.device)  # static input
+        self.graph = None
+        self.out = None
+        self.stream = torch.cuda.Stream(self.device)
+        self._alloc_host_outputs(len(self.label_off) * self.test_cfg["nms_post_max_size"], 9, len(self.label_off) + 1, 5)
+
+    # ---- one frame, enqueued on the current stream, device in / device out
+    def forward_device(self):
+        cfg, tc = self.cfg, self.test_cfg
+        mean, coors, npv, nv = vox.voxelize_mean(self.points, cfg["voxel_size"], cfg["point_cloud_range"],
+                                                 cfg["max_points"], cfg["max_voxels"], 0)
+        bev, bev_h16 = None, None
+        if self.keep_bev:
+            bev = self.net(mean, coors, 1, num=nv)
+            h = self.dense(bev) if self.dense is not None else self.head
+        else:
+            bev_h16 = self.net(mean, coors, 1, num=nv, pixel_h16=True)
+            h = self.dense.forward_h16(*bev_h16)
+        # frame status word (ADVICE r1): [fp16-range overflow of the pair-row kernels, overflow flag of each strided level]
+        status = torch.stack([sp.status_tensor(self.device)[0]] + [c[1] for c in self.net.level_counters])
+        boxes, scores, labels, counts = cpp.centerpoint_postprocess_device(
+            h["hm"], h["reg"], h["height"], h["dim"], h["vel"], h["rot"], cfg["voxel_size"][:2],
+            cfg["point_cloud_range"], tc["post_center_limit_range"], self.label_off, tc["down_ratio"],
+            tc["score_threshold"], tc["nms_iou_threshold"], tc["nms_pre_max_size"], tc["nms_post_max_size"], True)
+        return dict(bev=bev, bev_h16=bev_h16, boxes=boxes, scores=scores, labels=labels, counts=counts, num_voxels=nv,
+                    coors=coors, mean=mean, status=status)
+
+    def bev_nchw(self):
+        """The dense BEV tensor [1, 256, H, W] fp32 of the last frame (rebuilt from the pixel fp16-pair image when the
+        frame did not materialise it)."""
+        if self.out["bev"] is not None:
+            self.stream.synchronize()
+            return self.out["bev"]
+        from .ops import dense_conv as dc
+        rows, shape = self.out["bev_h16"]
+        with torch.cuda.stream(self.stream):
+            out = dc.pixel_h16_to_nchw(rows, shape)
+            # pixel rows hold (z, c)-ordered channels (to_pixel_h16); the reference tensor is (c, z)-ordered
+            b, h, w, cd = shape
+            D = self.dense.bev_depth
+            out = out.view(b, D, cd // D, h, w).transpose(1, 2).reshape(b, cd, h, w).contiguous()
+        self.stream.synchronize()  # callers read it from other streams
+        return out
+
+    def calibrate_head(self, points_dev):
+        """Shift the heat-map biases of the (randomly initialised) dense head so that ~1.4 % of the BEV cells of this frame
+        score above the threshold, as SURVEY.md §8d specifies for the synthetic workload (see
+        DenseRPNHead.calibrate_heatmap_bias).  Call before capture()."""
+        if self.dense is None:
+            return self
+        cfg = self.cfg
+        with torch.cuda.stream(self.stream):
+            self.points.copy_(points_dev)
+            mean, coors, npv, nv = vox.voxelize_mean(self.points, cfg["voxel_size"], cfg["point_cloud_range"],
+                                                     cfg["max_points"], cfg["max_voxels"], 0)
+            bev = self.net(mean, coors, 1, num=nv)
+            self.dense.calibrate_heatmap_bias(bev, self.test_cfg["score_threshold"])
+        self.stream.synchronize()
+        return self
+
+    @staticmethod
+    def check_status(status_host):
+        """Raise when the frame's device status word reports dropped work (never a silent wrong result)."""
+        st = [int(v) for v in status_host]
+        if st[0]:
+            raise RuntimeError("sparse backbone: an activation left fp16's range (|x| >= 65504) on the fp16-pair path; "
+                               "run this model with precision TF32X3_SPLIT")
+        for lvl, v in enumerate(st[1:]):
+            if v:
+                raise RuntimeError("sparse backbone: strided level %d overflowed its row capacity (set_level_caps); "
+                                   "output sites were dropped" % (lvl + 1))
+
+    def share_model(self, other):
+        self.net, self.dense = other.net, other.dense
+
     def export_weights_numpy(self):
         """Weights as plain numpy dicts for the CPU arm (oracle.cpu_reference.CpuFrame)."""
         def conv(l):
@@ -287,14 +300,16 @@ class CenterPointSweep:
     frame's kernels (tools/two_in_flight.py compares one and two lanes).  The latency of one frame does not improve (use CenterPointHotPath.infer for that); results are those of the single-lane pipeline.
     """
 
-    def __init__(self, lanes=2, **kw):
+    def __init__(self, lanes=2, frame_cls=None, **kw):
+        """frame_cls: the hot-path class of each lane (default CenterPointHotPath; pointpillars.PointPillarsHotPath)."""
         if lanes < 1:
             raise ValueError("lanes >= 1")
-        first = CenterPointHotPath(**kw)
+        frame_cls = frame_cls or CenterPointHotPath
+        first = frame_cls(**kw)
         self.lanes = [first]
         for _ in range(lanes - 1):
-            p = CenterPointHotPath(**kw)
-            p.net, p.dense = first.net, first.dense  # one model: calibration / weight loading happens once, on lane 0
+            p = frame_cls(**kw)
+            p.share_model(first)  # one model: calibration / weight loading happens once, on lane 0
             self.lanes.append(p)
         self.device = first.device
 

@@ -1,0 +1,241 @@
+"""PointPillars KITTI car inference (configs/pointpillars/pointpillars_xyres16_kitti_car.yml, the SECOND v1.5 `car.xyres_16`
+values) on one GPU, composed from this repository's kernels:
+
+    hard_voxelize -> PillarFeatureNet (one fused launch) -> pillar rows as fp16 pairs -> pixel fp16-pair image [496 x 432]
+    -> SecondBackbone + SecondFPN (dense_head.SecondTrunk) -> SSD head (cls | box | dir as ONE 384 -> 20 1x1 conv, fp32
+    planes) -> anchor_head_postprocess (csrc/anchor_postprocess.cu) -> boxes
+
+PointPillarsHotPath captures everything between the H2D copy of the points and the D2H copy of the boxes as one CUDA graph
+(pipeline.CapturedFrame).  Anchors are constant per model and built once on the host (create_anchors_3d_stride, SECOND's
+box_np_ops), as are the voxel-index corners of each anchor's near box (anchor_voxel_corners) the anchor mask reads."""
+import numpy as np
+import torch
+
+from . import synth
+from .dense_head import SecondTrunk, _Conv
+from .ops import anchor_postprocess as ahp
+from .ops import pillar_encoder as pe
+from .ops import sparse_nn as sp
+from .ops import voxelize as vox
+from .pipeline import CapturedFrame
+
+CONFIG = dict(
+    pfn_channels=64, pfn_bn_eps=1e-3,
+    backbone=dict(out_channels=(64, 128, 256), layer_nums=(3, 5, 5), downsample_strides=(2, 2, 2)),
+    fpn=dict(out_channels=(128, 128, 128), upsample_strides=(1, 2, 4), use_conv_for_no_stride=False),
+    anchors_per_loc=2, box_code_size=7, num_dir_bins=2,
+    anchor=dict(sizes=(1.6, 3.9, 1.56), strides=(0.32, 0.32, 0.0), offsets=(0.16, -39.52, -1.78), rotations=(0.0, 1.57)),
+    test=dict(anchor_area_threshold=1, nms_score_threshold=0.05, nms_iou_threshold=0.5, nms_pre_max_size=1000,
+              nms_post_max_size=300, post_center_limit_range=[0.0, -39.68, -5.0, 69.12, 39.68, 5.0]),
+)
+
+
+def grid_size(cfg):
+    """(nx, ny) of the pillar grid: 432 x 496 for synth.C2."""
+    pcr, vs = cfg["point_cloud_range"], cfg["voxel_size"]
+    return (int(round((pcr[3] - pcr[0]) / vs[0])), int(round((pcr[4] - pcr[1]) / vs[1])))
+
+
+def create_anchors_3d_stride(feature_size, sizes, anchor_strides, anchor_offsets, rotations, dtype=np.float32):
+    """SECOND box_np_ops.create_anchors_3d_stride: feature_size [D, H, W] -> [D, H, W, n_sizes, n_rot, 7] anchors
+    (x, y, z, w, l, h, theta), order (z, y, x, size, rot)."""
+    x_stride, y_stride, z_stride = anchor_strides
+    x_offset, y_offset, z_offset = anchor_offsets
+    z_centers = np.arange(feature_size[0], dtype=dtype) * z_stride + z_offset
+    y_centers = np.arange(feature_size[1], dtype=dtype) * y_stride + y_offset
+    x_centers = np.arange(feature_size[2], dtype=dtype) * x_stride + x_offset
+    sizes = np.reshape(np.array(sizes, dtype=dtype), [-1, 3])
+    rotations = np.array(rotations, dtype=dtype)
+    rets = list(np.meshgrid(x_centers, y_centers, z_centers, rotations, indexing="ij"))
+    tile_shape = [1] * 5
+    tile_shape[-2] = int(sizes.shape[0])
+    for i in range(len(rets)):
+        rets[i] = np.tile(rets[i][..., np.newaxis, :], tile_shape)[..., np.newaxis]
+    sizes = np.reshape(sizes, [1, 1, 1, -1, 1, 3])
+    tile_size_shape = list(rets[0].shape)
+    tile_size_shape[3] = 1
+    rets.insert(3, np.tile(sizes, tile_size_shape))
+    return np.transpose(np.concatenate(rets, axis=-1), [2, 1, 0, 3, 4, 5])
+
+
+def anchor_voxel_corners(anchors, voxel_size, point_cloud_range, grid):
+    """SECOND's anchor-mask geometry, computed once per model: rbbox2d_to_near_bbox (the axis-aligned box of (w, l), swapped
+    when |theta| folded into [0, pi) is nearer pi/2 than 0) and fused_get_anchors_area's floor / clamp to voxel indices.
+    anchors [A, 7] -> int32 [A, 4] (x_min, y_min, x_max, y_max)."""
+    rb = anchors[:, [0, 1, 3, 4, 6]]
+    rots = rb[:, -1]
+    folded = np.abs(rots - np.floor(rots / np.pi + 0.5) * np.pi)  # limit_period(rots, 0.5, pi)
+    cond = (folded > np.pi / 4)[:, np.newaxis]
+    centre_dims = np.where(cond, rb[:, [0, 1, 3, 2]], rb[:, :4])
+    near = np.concatenate([centre_dims[:, :2] - centre_dims[:, 2:] / 2, centre_dims[:, :2] + centre_dims[:, 2:] / 2], -1)
+    out = np.zeros(near.shape, dtype=np.int32)
+    out[:, 0] = np.floor((near[:, 0] - point_cloud_range[0]) / voxel_size[0])
+    out[:, 1] = np.floor((near[:, 1] - point_cloud_range[1]) / voxel_size[1])
+    out[:, 2] = np.floor((near[:, 2] - point_cloud_range[0]) / voxel_size[0])
+    out[:, 3] = np.floor((near[:, 3] - point_cloud_range[1]) / voxel_size[1])
+    out[:, [0, 2]] = np.clip(out[:, [0, 2]], 0, grid[0] - 1)
+    out[:, [1, 3]] = np.clip(out[:, [1, 3]], 0, grid[1] - 1)
+    return out
+
+
+class PointPillars:
+    """Seeded PointPillars model: PillarFeatureNet (one PFNLayer 9 -> 64, no bias, BatchNorm1D eps 1e-3), SecondTrunk and
+    the SSD head as one 384 -> 20 1x1 conv with bias (output channels: cls [2] | box [2 x 7] | dir [2 x 2], channel
+    a * K + k belonging to anchor (y * W + x) * 2 + a)."""
+
+    def __init__(self, cfg=None, model_cfg=None):
+        self.cfg = dict(cfg or synth.C2)
+        self.mc = model_cfg or CONFIG
+        mc = self.mc
+        self.grid = grid_size(self.cfg)
+        self.F = self.cfg["point_dim"]
+        self.C = mc["pfn_channels"]
+        self.trunk = SecondTrunk(self.C, mc["backbone"]["out_channels"], mc["backbone"]["layer_nums"],
+                                 mc["backbone"]["downsample_strides"], mc["fpn"]["out_channels"],
+                                 mc["fpn"]["upsample_strides"], mc["fpn"]["use_conv_for_no_stride"])
+        R = mc["anchors_per_loc"]
+        self.head_channels = R * (1 + mc["box_code_size"] + mc["num_dir_bins"])
+        self.head = _Conv(self.trunk.fpn_channels, self.head_channels, 1, bias=True, relu=False)
+        s = mc["backbone"]["downsample_strides"][0]  # the FPN output is at the first block's stride: 248 x 216
+        self.feat_hw = (self.grid[1] // s, self.grid[0] // s)
+        a = mc["anchor"]
+        self.anchors_np = create_anchors_3d_stride([1, self.feat_hw[0], self.feat_hw[1]], a["sizes"], a["strides"],
+                                                   a["offsets"], a["rotations"]).reshape(-1, 7)
+        self.corners_np = anchor_voxel_corners(self.anchors_np, self.cfg["voxel_size"], self.cfg["point_cloud_range"],
+                                               self.grid)
+        self.device = None
+
+    def init_weight(self, seed=0, device="cuda", bn_gain=1.0):
+        """device=None: numpy parameters only (enough for export_numpy / the CPU arm).  bn_gain multiplies every
+        BatchNorm gamma (the convention of dense_head.DenseRPNHead.init_weight)."""
+        rng = np.random.default_rng(seed)
+        C, F = self.C, self.F
+        self.pfn = dict(weight=synth.kaiming_uniform(rng, (F + 5, C), F + 5),
+                        gamma=np.full(C, bn_gain, np.float32), beta=np.zeros(C, np.float32),
+                        mean=np.zeros(C, np.float32), var=np.ones(C, np.float32), eps=self.mc["pfn_bn_eps"])
+        for c in self.trunk.convs():
+            c.init(rng, device, bn_gain=bn_gain)
+        self.head.init(rng, device)
+        self.device = None if device is None else torch.device(device)
+        if device is not None:
+            p = self.pfn
+            self.pfn_weight = torch.from_numpy(p["weight"]).to(device)
+            self.pfn_folded = pe.fold_bn(p["gamma"], p["beta"], p["mean"], p["var"], p["eps"], device)
+            self.anchors = torch.from_numpy(np.ascontiguousarray(self.anchors_np)).to(device)
+            self.corners = torch.from_numpy(np.ascontiguousarray(self.corners_np)).to(device)
+        return self
+
+    def export_numpy(self):
+        return dict(self.trunk.export_numpy(), pfn=self.pfn, head=self.head.np)
+
+    # ---- per frame, device in / device out
+    def encode(self, points):
+        """points [n, F] -> (pixel fp16-pair BEV image [ny * nx, 2 C], its shape (1, ny, nx, C), coors [V, 4], num [1])."""
+        cfg = self.cfg
+        voxels, co, npv, nv = vox.hard_voxelize(points, cfg["voxel_size"], cfg["point_cloud_range"], cfg["max_points"],
+                                                cfg["max_voxels"])
+        coors = torch.nn.functional.pad(co, (1, 0))  # (batch 0, z, y, x)
+        p = self.pfn
+        feats = pe.pillar_feature_net(voxels, npv, coors, self.pfn_weight, p["gamma"], p["beta"], p["mean"], p["var"],
+                                      p["eps"], cfg["voxel_size"], cfg["point_cloud_range"], num_voxels=nv,
+                                      folded=self.pfn_folded)
+        nx, ny = self.grid
+        rows = sp.sparse_coo_tensor(coors, feats, [1, 1, ny, nx, self.C], num=nv)
+        image, shape = rows.to_pixel_h16()
+        return image, shape, coors, nv
+
+    def dense(self, image, shape):
+        """Pixel fp16-pair BEV image -> SSD head planes [1, 20, H / 2, W / 2] fp32."""
+        cat, cshape = self.trunk(image, shape)
+        _, planes, _ = self.head(cat, cshape, want_nchw=True)
+        return planes
+
+    def postprocess(self, planes, coors, nv, anchor_mask=None, sorted_out=None):
+        t = self.mc["test"]
+        return ahp.anchor_head_postprocess_device(
+            planes, self.anchors, self.corners, coors, nv, self.grid, t["post_center_limit_range"],
+            t["anchor_area_threshold"], t["nms_score_threshold"], t["nms_iou_threshold"], t["nms_pre_max_size"],
+            t["nms_post_max_size"], anchor_mask=anchor_mask, sorted_out=sorted_out)
+
+    def calibrate_cls_bias(self, points, target_frac=0.02):
+        """Seeded weights leave the cls logits near the initial bias, so either almost none or most of the 107,136 anchors
+        would pass the 0.05 score threshold.  This shifts both cls biases so that `target_frac` of all anchors (2 %, about
+        2.1k) pass the anchor mask AND the threshold on this frame: more than nms_pre_max_size = 1000, so the top-k cut
+        runs.  Weights stay seeded and are exported unchanged to the CPU arm."""
+        image, shape, coors, nv = self.encode(points)
+        planes = self.dense(image, shape)
+        mask = torch.empty((self.anchors.shape[0],), dtype=torch.uint8, device=planes.device)
+        self.postprocess(planes, coors, nv, anchor_mask=mask)
+        R = self.mc["anchors_per_loc"]
+        logits = planes[0, :R].permute(1, 2, 0).reshape(-1)[mask.bool()].float().cpu().numpy()
+        k = int(round(target_frac * self.anchors.shape[0]))
+        thr = self.mc["test"]["nms_score_threshold"]
+        logit_thr = float(np.log(thr / (1.0 - thr)))
+        if len(logits) > k:
+            v = np.sort(logits)[::-1]
+            shift = logit_thr - 0.5 * (float(v[k - 1]) + float(v[k]))
+        else:
+            shift = logit_thr - float(logits.min()) + 1.0 if len(logits) else 0.0
+        b = self.head.np["bias"].copy()
+        b[:R] = (b[:R] + np.float32(shift)).astype(np.float32)
+        self.head.np["bias"] = b
+        self.head.dev["shift"].copy_(torch.from_numpy(b))
+        return self
+
+    def flops(self):
+        """Algorithmic flops (2 x MACs) of the dense part (backbone, FPN, head) at the model's grid."""
+        out = dict(backbone=0.0, fpn=0.0, head=0.0)
+        h, w = self.grid[1], self.grid[0]
+        sizes = []
+        for blk in self.trunk.blocks:
+            for c in blk:
+                h, w = (h + 2 * c.padding - c.k) // c.stride + 1, (w + 2 * c.padding - c.k) // c.stride + 1
+                out["backbone"] += 2.0 * h * w * c.cin * c.cout * c.k * c.k
+            sizes.append((h, w))
+        for (h, w), de in zip(sizes, self.trunk.deblocks):
+            out["fpn"] += 2.0 * (h * de.up) * (w * de.up) * de.cin * de.cout * (1 if de.up > 1 else de.k * de.k)
+        out["head"] = 2.0 * self.feat_hw[0] * self.feat_hw[1] * self.head.cin * self.head.cout
+        return out
+
+
+class PointPillarsHotPath(CapturedFrame):
+    """One PointPillars frame on one GPU: H2D -> [captured: hard_voxelize -> PFN -> pixel image -> trunk -> head conv ->
+    anchor postprocess] -> D2H of boxes [300, 7], scores, labels, counts (candidates, rows) and the status word."""
+
+    def __init__(self, cfg=None, device="cuda:0", seed=0, num_points=None, bn_gain=1.0):
+        self.cfg = dict(cfg or synth.C2)
+        self.device = torch.device(device)
+        self.n = int(num_points or self.cfg["num_points"])
+        self.F = self.cfg["point_dim"]
+        self.model = PointPillars(self.cfg).init_weight(seed=seed, device=self.device, bn_gain=bn_gain)
+        self.points = torch.zeros((self.n, self.F), dtype=torch.float32, device=self.device)
+        self.graph = None
+        self.out = None
+        self.stream = torch.cuda.Stream(self.device)
+        self._alloc_host_outputs(self.model.mc["test"]["nms_post_max_size"], 7, 2, 1)
+
+    def share_model(self, other):
+        self.model = other.model
+
+    def forward_device(self):
+        m = self.model
+        image, shape, coors, nv = m.encode(self.points)
+        planes = m.dense(image, shape)
+        boxes, scores, labels, counts = m.postprocess(planes, coors, nv)
+        status = sp.status_tensor(self.device).clone()
+        return dict(boxes=boxes, scores=scores, labels=labels, counts=counts, num_voxels=nv, coors=coors, planes=planes,
+                    status=status)
+
+    def calibrate_head(self, points_dev):
+        """See PointPillars.calibrate_cls_bias.  Call before capture()."""
+        with torch.cuda.stream(self.stream):
+            self.points.copy_(points_dev)
+            self.model.calibrate_cls_bias(self.points)
+        self.stream.synchronize()
+        return self
+
+    @staticmethod
+    def check_status(status_host):
+        """Raise when the frame's status word reports that an activation left fp16's range (never a silent wrong result)."""
+        if int(status_host[0]):
+            raise RuntimeError("PointPillars: an activation left fp16's range (|x| >= 65504) on the fp16-pair path")
