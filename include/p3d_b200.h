@@ -329,21 +329,18 @@ int p3d_dense_conv2d_split(const float *in_split, int B, int H, int W, int Cin, 
                            const float *shift, int relu, float *out_split, int out_C, int out_c0, float *out_nchw,
                            p3d_stream_t stream);
 
-/* EXPERIMENTAL (never run on a GPU yet): the grouped 3x3 output convs of CenterHead's SeparateHeads
- * (center_head.py:80-117) as one CUDA-core launch.  in_split: pixel split rows [B*H*W][2][in_C]; group g convolves
+/* The grouped 3x3 output convs of CenterHead's SeparateHeads (center_head.py:80-117) as one CUDA-core launch.  in_split: pixel split rows [B*H*W][2][in_C]; group g convolves
  * channels [g*Cin, (g+1)*Cin) with weight [groups][9][Cin][4] (outputs zero-padded to 4) + bias [groups][4] and
  * writes cnt[g] fp32 planes from plane0[g] of out_nchw [B, planes, H, W] (plane0 / cnt are HOST arrays). */
 int p3d_head_final_conv(const float *in_split, int B, int H, int W, int in_C, int Cin, int groups, const float *weight,
                         const float *bias, const int32_t *plane0_host, const int32_t *cnt_host, int planes,
                         float *out_nchw, p3d_stream_t stream);
-int p3d_head_final_conv_h16(const void *in_h16, int B, int H, int W, int in_C, int Cin, int groups, const float *weight,
-                            const float *bias, const int32_t *plane0_host, const int32_t *cnt_host, int planes,
-                            float *out_nchw, p3d_stream_t stream);
 
 /* fp16-pair dense convolution (csrc/dense_conv_f16.cu): same layer contract as p3d_dense_conv2d_split on pixel H16
  * rows [B*H*W][C / 32 groups][hi 32 | lo' 32] halfs.  3x3 / stride 1 / pad 1 layers load the haloed tile once per
  * 32-channel group and read the 9 taps through shifted wgmma descriptors; everything else loads one box per tap.
- * mode 0 = auto, 1 = force per-tap loads; m_tiles 0 = auto, 1 or 2 M tiles (8 x 16 pixels each) per work item. */
+ * mode 0 = auto, 1 = force per-tap loads (other values: P3D_ERR_INVALID_ARG); m_tiles 0 = auto, 1 or 2 M tiles
+ * (8 x 16 pixels each) per work item; n_tile 64 or 128. */
 int p3d_nchw_to_pixel_h16(const float *in, int B, int C, int H, int W, void *out_h16, int32_t *status_dev,
                           p3d_stream_t stream);
 int p3d_pixel_h16_to_nchw(const void *in_h16, int B, int C, int H, int W, float *out, p3d_stream_t stream);
@@ -363,17 +360,13 @@ int p3d_bev_pool_prepare(const float *coor, int B, int N, int D, int H, int W, c
                          int32_t *ranks_depth, int32_t *ranks_feat, int32_t *interval_starts, int32_t *interval_lengths,
                          int32_t *counts_dev, void *workspace, size_t workspace_bytes, p3d_stream_t stream);
 
-/* Grouped 3x3 output convs of the CenterHead (center_head.py:80-117) as one tensor-core launch: group g reads input
- * channels [g * Cin, (g + 1) * Cin) of the in_C-channel H16 image, uses weight tile g (pack with n_tile = 16, columns
- * >= cnt[g] zero), bias [groups][16], and writes cnt[g] fp32 planes from plane0[g] (device int32 arrays). */
-int p3d_grouped_head_conv_f16(const void *in_h16, int B, int H, int W, int in_C, int Cin, int groups,
-                              const void *packed_weight, const float *bias, const int32_t *plane0_dev,
-                              const int32_t *cnt_dev, int planes, float *out_nchw, int32_t *status_dev, p3d_stream_t stream);
-/* The same output convs with the 9 taps in the GEMM's N dimension (default for Cin = 32 / 64 / 128 and <= 3 output
- * channels per group; a wider conv is split into several groups over the same input slice): one [256 haloed pixels x Cin]
- * x [Cin x 27] GEMM per 14 x 14 output tile, then every pixel adds its 9 shifted partial sums.  Group g reads input
- * channels [cin0[g], cin0[g] + Cin) (cin0_dev null: g * Cin); packed_weight: per group
- * p3d_dense_conv2d_f16_pack_weights(taps 1, Cin, n_tile 32) of W2[c][tap * 3 + co]; bias [groups][4]. */
+/* Grouped 3x3 output convs of the CenterHead (center_head.py:80-117) as one tensor-core launch with the 9 taps in the
+ * GEMM's N dimension (<= 3 output channels per group; a wider conv is split into several groups over the same input
+ * slice): one [256 haloed pixels x Cin] x [Cin x 27] GEMM per 14 x 14 output tile, then every pixel adds its 9 shifted
+ * partial sums.  Group g reads input channels [cin0[g], cin0[g] + Cin) of the in_C-channel H16 image (cin0_dev null:
+ * g * Cin) and writes cnt[g] fp32 planes from plane0[g] (device int32 arrays); packed_weight: per group
+ * p3d_dense_conv2d_f16_pack_weights(taps 1, Cin, n_tile 32) of W2[c][tap * 3 + co]; bias [groups][4].
+ * Cin % 32 == 0 and Cin <= 320 (P3D_ERR_UNSUPPORTED above: the shared memory holds fewer than two activation tiles). */
 int p3d_head_out_conv_f16(const void *in_h16, int B, int H, int W, int in_C, int Cin, int groups, const void *packed_weight,
                           const float *bias, const int32_t *cin0_dev, const int32_t *plane0_dev, const int32_t *cnt_dev,
                           int planes, float *out_nchw, p3d_stream_t stream);

@@ -24,8 +24,7 @@
 //               warpgroup c = 1, 2 computes rows 64(c-1) .. 64(c-1)+63 of every M tile with one wgmma group in flight
 //               behind the one being issued.  At the end of an item it parks hi + cross * 2^-11 in its fp32 staging
 //               tile and starts the next item; warps 1-3 of warpgroup 0 (the epilogue warps) apply scale / shift /
-//               ReLU, split and store from there, so the tensor pipe does not idle through the epilogue.  The
-//               weight-stationary variant (WS) keeps the epilogue in the consumers' registers.
+//               ReLU, split and store from there, so the tensor pipe does not idle through the epilogue.
 #include <cuda.h>
 #include <cuda_fp16.h>
 
@@ -38,7 +37,9 @@ namespace dcf {
 using namespace tc;
 
 constexpr int kTW = 8, kTH = 16;        // output tile of one M = 128 tile: 8 x 16 pixels
+constexpr int kPitch = kTW + 2;         // pixels per row of the haloed tile in shared memory
 constexpr int kMaxA = 6, kMaxB = 12;    // activation / weight ring depth limits
+constexpr int kSmemBudget = (227 - 6) * 1024;  // 227 KB per CTA less alignment slack and the static barriers
 constexpr int kDenseThreads = 384;      // producer warpgroup + two consumer warpgroups
 constexpr uint32_t kConsumerWarps = 8;  // arrivals that release a slot: one per consumer warp
 constexpr uint32_t kEpiThreads = 96;    // warps 1-3 of the producer warpgroup: the epilogue warps
@@ -59,53 +60,38 @@ struct Params {
   uint8_t *out_h16;           // or null
   float *out_nchw;            // fp32 planes [B, cout, out_H, out_W] or null
   int32_t *status;            // bit 0: fp16 range overflow while writing out_h16
-  // grouped mode (the 36 output convs of the CenterHead as ONE launch): N tile nt reads input channels
-  // [nt * Cin, (nt + 1) * Cin) of an image with in_C channels, uses weight tile nt, and writes its first grp_cnt[nt]
-  // columns to the fp32 planes grp_plane0[nt] .. of out_nchw ([B, cout planes, out_H, out_W]); shift is [n_ntiles][N]
-  int grouped, in_C;
-  const int32_t *grp_plane0, *grp_cnt;
-  int base_offset_mode;       // 0 (default): base_offset field zero; 1: address bits 7-9 of the shifted start address
-  int w_bytes;                // weight-stationary kernel: bytes of one N tile's weight image (taps * Cin / 16 k-blocks)
 };
 
-// PITCH: pixels per row of the haloed tile in shared memory: 10 (tight: 8 + 2) or 16 (8-row groups stay 1024-byte aligned)
-// WS ("weight-stationary", HALO only): the whole weight image of an N tile (taps * Cin / 16 k-blocks, <= 144 KB) stays in
-// shared memory while the CTA walks a contiguous range of pixel tiles of that N tile; only the haloed activation tiles
-// stream.  For layers with few input and many output channels (the 64 -> 36 x 64 ConvModules of the CenterHead) this
-// replaces 43 B/clk of weight ingest per SM - the L2 -> SM limit - by 13 B/clk of activations.
-template <int N, int MT, bool HALO, int PITCH, bool WS = false>
+template <int N, int MT, bool HALO>
 struct Cfg {
-  static constexpr int A_ROWS = HALO ? PITCH * (kTH * MT + 2) : kM * MT;     // rows of 128 bytes per activation buffer
+  static constexpr int A_ROWS = HALO ? kPitch * (kTH * MT + 2) : kM * MT;    // rows of 128 bytes per activation buffer
   static constexpr int A_BYTES = ((A_ROWS * 128 + 1023) / 1024) * 1024;
   static constexpr int B_BYTES = 128 * N;                                    // weight blocks of one (tap, group): 2 k-blocks
   static constexpr int B_BLK = 64 * N;
-  // Staged epilogue (all but WS): a consumer warpgroup parks hi + cross * 2^-11 of its rows (MT x 64 rows x N columns,
-  // fp32) in its own staging tile and goes on with the next item; the epilogue warps apply scale / shift / ReLU, split
-  // and store.  Row pitch N + 8 floats: the 32 bytes of padding put the four rows of a half-warp's fragment stores on
-  // distinct banks.  WS keeps the epilogue in the consumers (its weight image leaves no room for the tiles).
-  static constexpr bool STAGE = !WS;
+  // Staged epilogue: a consumer warpgroup parks hi + cross * 2^-11 of its rows (MT x 64 rows x N columns, fp32) in its
+  // own staging tile and goes on with the next item; the epilogue warps apply scale / shift / ReLU, split and store.
+  // Row pitch N + 8 floats: the 32 bytes of padding put the four rows of a half-warp's fragment stores on distinct banks.
   static constexpr int SP = N + 8;                                           // staging row pitch (floats)
   static constexpr int STG_WG = MT * 64 * SP;                                // floats per consumer warpgroup
-  static constexpr int STG_BYTES = STAGE ? 2 * STG_WG * 4 : 0;
-  static constexpr int AVAIL = (227 - 6) * 1024 - STG_BYTES;  // 227 KB - alignment slack - static (barriers) - staging
-  // TAP mode: every step needs a new activation buffer, so both rings get the same depth; HALO: 2 (WS: 3) buffers
+  static constexpr int STG_BYTES = 2 * STG_WG * 4;
+  static constexpr int AVAIL = kSmemBudget - STG_BYTES;
+  // TAP mode: every step needs a new activation buffer, so both rings get the same depth; HALO: 2 buffers
   static constexpr int NA_TAP_RAW = AVAIL / (A_BYTES + B_BYTES);
-  static constexpr int NA = WS ? 3 : (HALO ? 2 : (NA_TAP_RAW > kMaxA ? kMaxA : NA_TAP_RAW));
+  static constexpr int NA = HALO ? 2 : (NA_TAP_RAW > kMaxA ? kMaxA : NA_TAP_RAW);
   static constexpr int BUDGET = AVAIL - NA * A_BYTES;
   static constexpr int NB_RAW = BUDGET / B_BYTES;
   static constexpr int NB = NB_RAW > kMaxB ? kMaxB : NB_RAW;                 // weight ring depth
   static constexpr int ACC = MT * N;                                         // fp32 registers per thread
   static constexpr int SPU = HALO ? 9 : 1;                                   // steps per activation buffer
   // register split, 128 P + 256 C <= 384 x 168 (what a CTA of 384 threads holds at launch); the consumers hold up to 128
-  // fp32 accumulators.  The producer warpgroup needs more than 40 when its warps 1-3 run the epilogue.
-  static constexpr int P_REGS = STAGE ? 88 : 40, C_REGS = STAGE ? 208 : 232;
+  // fp32 accumulators, the producer warpgroup's warps 1-3 run the epilogue.
+  static constexpr int P_REGS = 88, C_REGS = 208;
   static_assert(128 * P_REGS + 256 * C_REGS <= kDenseThreads * 168, "register split");
-  static_assert(N == 16 || N == 64 || N == 128, "N tile: 16 (grouped output convs), 64 or 128");
+  static_assert(N == 64 || N == 128, "N tile: 64 or 128");
   static_assert(MT == 1 || MT == 2, "one or two M tiles");
   static_assert(MT * N <= 128, "accumulators: at most 128 registers per thread");
-  static_assert(WS || NB >= 3, "weight ring too shallow");
+  static_assert(NB >= 3, "weight ring too shallow");
   static_assert(NA >= 2 && NA <= kMaxA, "activation ring depth");
-  static_assert(!WS || (HALO && MT == 1), "weight-stationary: haloed 3x3 tiles, one M tile");
 };
 
 __device__ __forceinline__ void tma_tile4d(uint32_t dst, const CUtensorMap *map, int c, int x, int y, int b, uint32_t bar) {
@@ -151,7 +137,7 @@ enum TraceField {
   kTrAFull, kTrBFull = kTrAFull + 2,    // per consumer warpgroup: waiting on activation / weight "full"
   kTrMma = kTrBFull + 2,                // per consumer warpgroup: in wgmma.wait_group
   kTrEpi = kTrMma + 2,                  // per consumer warpgroup: after the item's last wait_group until the next item
-                                        // (WS: the epilogue; otherwise writing the staging tile)
+                                        // (writing the staging tile), less kTrStageFree
   kTrStageFree = kTrEpi + 2,            // per consumer warpgroup: waiting for the epilogue warps to free its staging tile
   kTrAEmpty = kTrStageFree + 2, kTrBEmpty,  // producer: waiting on activation / weight "empty"
   kTrEwWait, kTrEwBusy,                 // epilogue warp 1: waiting on "staged"; scale / shift / ReLU / split and stores
@@ -182,18 +168,12 @@ struct Trace {
   __device__ __forceinline__ void flush(int) const {}
 };
 #endif
-template <bool WS = false>
-__device__ __forceinline__ Item decode(long long w, const Params &p, int th) {
+// item idx of this CTA: round robin over the grid, N tile fastest
+__device__ __forceinline__ Item decode(long long idx, const Params &p, int th) {
   Item it;
-  long long q = w;
-  if (WS) {  // N tile slowest: a CTA's contiguous item range stays on one N tile
-    const long long pix = static_cast<long long>(p.B) * p.tiles_y * p.tiles_x;
-    it.nt = static_cast<int>(q / pix);
-    q -= it.nt * pix;
-  } else {
-    it.nt = static_cast<int>(q % p.n_ntiles);
-    q /= p.n_ntiles;
-  }
+  long long q = blockIdx.x + idx * gridDim.x;
+  it.nt = static_cast<int>(q % p.n_ntiles);
+  q /= p.n_ntiles;
   it.tap0 = 0;
   if (p.up > 1) {
     const int up2 = p.up * p.up;
@@ -208,21 +188,19 @@ __device__ __forceinline__ Item decode(long long w, const Params &p, int th) {
 }
 
 // Epilogue warps (warps 1-3 of the producer warpgroup, thread et = 0 .. 95).  For every item, and for consumer warpgroup
-// c = 0, 1 in turn: wait until c has staged its rows, apply scale / shift and ReLU with the expressions of the in-register
-// epilogue (hence the same bits), write the outputs, and hand the tile back.  Pixel H16 rows: a lane takes four channels
-// of one pixel, so eight lanes write one pixel's 32-channel group as 64 contiguous bytes of hi and 64 of lo'.  fp32 NCHW
-// planes: a lane takes one pixel of an 8-pixel tile row, so eight lanes write 32 contiguous bytes of a plane.
+// c = 0, 1 in turn: wait until c has staged its rows, apply scale / shift and ReLU, write the outputs, and hand the tile
+// back.  Pixel H16 rows: a lane takes four channels of one pixel, so eight lanes write one pixel's 32-channel group as 64
+// contiguous bytes of hi and 64 of lo'.  fp32 NCHW planes: a lane takes one pixel of an 8-pixel tile row, so eight lanes
+// write 32 contiguous bytes of a plane.
 template <int N, int MT>
 __device__ __forceinline__ void epilogue_warps(const Params &p, const float *stg, unsigned long long *staged,
-                                               unsigned long long *freed, long long n_items, long long w_first,
-                                               long long w_step, int th, int et) {
+                                               unsigned long long *freed, long long n_items, int th, int et) {
   constexpr int SP = N + 8, ROWS = MT * 64;  // staging row pitch (floats) and rows per consumer warpgroup (Cfg)
   const int ew = et >> 5, lane = et & 31;
   bool ovf = false;
   Trace tr;
   for (long long idx = 0; idx < n_items; ++idx) {
-    const Item im = decode<false>(w_first + idx * w_step, p, th);
-    const int g_cnt = p.grouped ? __ldg(p.grp_cnt + im.nt) : 0, g_p0 = p.grouped ? __ldg(p.grp_plane0 + im.nt) : 0;
+    const Item im = decode(idx, p, th);
     const int dy = p.up > 1 ? im.tap0 / p.up : 0, dx = p.up > 1 ? im.tap0 % p.up : 0;
     for (int c = 0; c < 2; ++c) {
       long long t0 = tr.now();
@@ -237,7 +215,7 @@ __device__ __forceinline__ void epilogue_warps(const Params &p, const float *stg
         X = ix * p.up + dx;
         return iy < p.oH && ix < p.oW;
       };
-      if (N >= 32 && p.out_h16) {
+      if (p.out_h16) {
         const int r4 = lane >> 3, c4 = (lane & 7) * 4;  // row of a 4-row quad, first of four columns
         for (int q = 0; q < N / 32; ++q) {
           const int col = q * 32 + c4, ch = im.nt * N + col, oc = p.out_c0 + ch;
@@ -276,12 +254,11 @@ __device__ __forceinline__ void epilogue_warps(const Params &p, const float *stg
         for (int u = ew; u < (ROWS / 8) * (N / 4); u += 3) {
           const int r = (u % (ROWS / 8)) * 8 + px, col = (u / (ROWS / 8)) * 4 + cc, ch = im.nt * N + col;
           int Y, X;
-          if ((p.grouped ? col >= g_cnt : ch >= p.cout) || !pixel(r, Y, X)) continue;
+          if (ch >= p.cout || !pixel(r, Y, X)) continue;
           const float sc = p.scale ? __ldg(p.scale + ch) : 1.0f, sh = p.shift ? __ldg(p.shift + ch) : 0.0f;
           float v = fmaf(st[r * SP + col], sc, sh);
           if (p.relu) v = fmaxf(v, 0.f);
-          const int plane = p.grouped ? g_p0 + col : ch;
-          p.out_nchw[((static_cast<size_t>(im.b) * p.cout + plane) * p.out_H + Y) * p.out_W + X] = v;
+          p.out_nchw[((static_cast<size_t>(im.b) * p.cout + ch) * p.out_H + Y) * p.out_W + X] = v;
         }
       }
       mbar_arrive(smem_u32(freed + c));
@@ -292,10 +269,10 @@ __device__ __forceinline__ void epilogue_warps(const Params &p, const float *stg
   if (et == 0) tr.flush(0);
 }
 
-template <int N, int MT, bool HALO, int PITCH, bool WS = false>
+template <int N, int MT, bool HALO>
 __global__ void __launch_bounds__(kDenseThreads, 1)
     dense_conv_f16_kernel(const __grid_constant__ CUtensorMap in_map, const Params p) {
-  using C = Cfg<N, MT, HALO, PITCH, WS>;
+  using C = Cfg<N, MT, HALO>;
   constexpr int TH = kTH * MT;  // output tile height
   constexpr int H = N / 2;      // accumulator registers of the hi products of one M tile; the cross products follow
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -303,21 +280,15 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
   const int up2 = p.up * p.up;
   const long long n_total = static_cast<long long>(p.B) * p.tiles_y * p.tiles_x * p.n_ntiles * (p.up > 1 ? up2 : 1);
   if (static_cast<long long>(blockIdx.x) >= n_total) return;
-  // item sequence of this CTA: round robin (N tile fastest), or for WS a contiguous range (N tile slowest)
-  const long long w_first = WS ? (static_cast<long long>(blockIdx.x) * n_total) / gridDim.x : blockIdx.x;
-  const long long n_work = WS ? (static_cast<long long>(blockIdx.x + 1) * n_total) / gridDim.x : n_total;
-  const long long w_step = WS ? 1 : gridDim.x;
-  const long long n_items = (n_work - w_first + w_step - 1) / w_step;
+  const long long n_items = (n_total - blockIdx.x + gridDim.x - 1) / gridDim.x;  // round robin: see decode
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   // full barriers: one producer arrive + the bytes of the load; empty barriers: one arrive per consumer warp once the
-  // wgmma that read the slot have retired.  Activation full[NA] | empty[NA] | weight full[NB] | empty[NB] | WS image
-  // full | empty | staging tile of consumer c staged[2] (one arrive per consumer thread) | free[2] (one arrive per
-  // epilogue thread).
-  __shared__ __align__(8) unsigned long long s_bar[2 * kMaxA + 2 * kMaxB + 6];
-  constexpr int kAF = 0, kAE = kMaxA, kBF = 2 * kMaxA, kBE = 2 * kMaxA + kMaxB, kWF = 2 * kMaxA + 2 * kMaxB, kWE = kWF + 1;
-  constexpr int kSS = kWE + 1, kSF = kSS + 2;
+  // wgmma that read the slot have retired.  Activation full[NA] | empty[NA] | weight full[NB] | empty[NB] | staging
+  // tile of consumer c staged[2] (one arrive per consumer thread) | free[2] (one arrive per epilogue thread).
+  __shared__ __align__(8) unsigned long long s_bar[2 * kMaxA + 2 * kMaxB + 4];
+  constexpr int kAF = 0, kAE = kMaxA, kBF = 2 * kMaxA, kBE = 2 * kMaxA + kMaxB, kSS = 2 * kMaxA + 2 * kMaxB, kSF = kSS + 2;
 
   const int tid = threadIdx.x, wg = tid >> 7, wtid = tid & 127;
   if (tid == 0) {
@@ -325,12 +296,10 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
       mbar_init(smem_u32(&s_bar[kAF + s]), 1);
       mbar_init(smem_u32(&s_bar[kAE + s]), kConsumerWarps);
     }
-    for (int s = 0; s < (WS ? 0 : C::NB); ++s) {
+    for (int s = 0; s < C::NB; ++s) {
       mbar_init(smem_u32(&s_bar[kBF + s]), 1);
       mbar_init(smem_u32(&s_bar[kBE + s]), kConsumerWarps);
     }
-    mbar_init(smem_u32(&s_bar[kWF]), 1);
-    mbar_init(smem_u32(&s_bar[kWE]), kConsumerWarps);
     for (int c = 0; c < 2; ++c) {
       mbar_init(smem_u32(&s_bar[kSS + c]), 128);
       mbar_init(smem_u32(&s_bar[kSF + c]), kEpiThreads);
@@ -346,7 +315,6 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
   // steps / activation units per item: HALO: one unit per group, 9 taps each; TAP: one unit per (tap, group)
   const int taps_item = p.up > 1 ? 1 : p.taps;
   const int units_item = HALO ? G : taps_item * G;
-  auto item_w = [&](long long idx) { return w_first + idx * w_step; };
   // Ring positions advance by one slot per fill / use; the phase bit flips when the slot index wraps.  The consumers wait
   // for full[slot] to complete the phase of the current pass; the producer waits for empty[slot] to complete the phase
   // of the previous pass (parity ph ^ 1: on the first pass that is the phase before the barrier's first, which counts as
@@ -355,32 +323,16 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
   if (wg == 0) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(C::P_REGS));
     if (tid >= 32) {
-      if (C::STAGE) epilogue_warps<N, MT>(p, stg, s_bar + kSS, s_bar + kSF, n_items, w_first, w_step, TH, tid - 32);
+      epilogue_warps<N, MT>(p, stg, s_bar + kSS, s_bar + kSF, n_items, TH, tid - 32);
       return;
     }
     // ------------------------------------------------------------------------------------------ producer
     if (tid != 0) return;
     uint32_t a_slot = 0, a_ph = 0, b_slot = 0, b_ph = 0;
-    int cur_nt = -1;  // WS: N tile whose weight image is resident
-    uint32_t img = 0; // WS: images loaded so far
     Trace tr;
     for (long long idx = 0; idx < n_items; ++idx) {
-      const Item im = decode<WS>(item_w(idx), p, TH);
-      const int cg0 = p.grouped ? im.nt * G : 0;  // first 32-channel group of this item's input channels
+      const Item im = decode(idx, p, TH);
       const uint8_t *w_tile = p.packed_w + static_cast<size_t>(im.nt) * p.taps * (p.Cin / 16) * C::B_BLK;
-      if (WS && im.nt != cur_nt) {
-        // first item of a run on this N tile: replace the image once both consumers have retired every step of the
-        // previous run
-        if (img > 0) mbar_wait(smem_u32(&s_bar[kWE]), (img - 1) & 1u);
-        const uint32_t bar = smem_u32(&s_bar[kWF]);
-        mbar_arrive_expect_tx(bar, static_cast<uint32_t>(p.w_bytes));
-        for (int off = 0; off < p.w_bytes; off += 16384) {
-          const int bytes = p.w_bytes - off < 16384 ? p.w_bytes - off : 16384;
-          bulk_g2s(b_ring + static_cast<uint32_t>(off), w_tile + off, static_cast<uint32_t>(bytes), bar);
-        }
-        ++img;
-        cur_nt = im.nt;
-      }
       // TAP units are (tap, group) with the group fastest; dy, dx follow the tap without dividing
       int dy = 0, dx = 0;
       for (int tu = 0; tu < (HALO ? 1 : taps_item); ++tu) {
@@ -392,13 +344,13 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
           tr.add(kTrAEmpty, t0);
           mbar_arrive_expect_tx(abar, static_cast<uint32_t>(C::A_ROWS * 128));
           if (HALO) {
-            tma_tile4d(a_dst, &in_map, (cg0 + g) * 64, im.tx0 - 1, im.ty0 - 1, im.b, abar);
+            tma_tile4d(a_dst, &in_map, g * 64, im.tx0 - 1, im.ty0 - 1, im.b, abar);
           } else {
             const int x = im.tx0 * p.stride - p.pad + dx, y = im.ty0 * p.stride - p.pad + dy;  // may be negative: zero fill
-            tma_tile4d(a_dst, &in_map, (cg0 + g) * 64, x, y, im.b, abar);
+            tma_tile4d(a_dst, &in_map, g * 64, x, y, im.b, abar);
           }
           if (++a_slot == C::NA) a_slot = 0, a_ph ^= 1u;
-          for (int t = 0; t < (WS ? 0 : C::SPU); ++t) {
+          for (int t = 0; t < C::SPU; ++t) {
             const uint32_t bbar = smem_u32(&s_bar[kBF + b_slot]);
             const long long t1 = tr.now();
             mbar_wait(smem_u32(&s_bar[kBE + b_slot]), b_ph ^ 1u);
@@ -423,20 +375,11 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
   auto release = [&](int base, uint32_t slot) {
     if (warp_leader) mbar_arrive(smem_u32(&s_bar[base + slot]));
   };
-  bool ovf = false;
   uint32_t a_slot = 0, a_ph = 0, b_slot = 0, b_ph = 0;
-  int cur_nt = -1;   // WS: N tile whose weight image is resident
-  uint32_t img = 0;  // WS: images used so far
   float acc[C::ACC];
   Trace tr;
   const long long t_start = tr.now();
   for (long long idx = 0; idx < n_items; ++idx) {
-    const Item im = decode<WS>(item_w(idx), p, TH);
-    if (WS && im.nt != cur_nt) {
-      mbar_wait(smem_u32(&s_bar[kWF]), img & 1u);
-      ++img;
-      cur_nt = im.nt;
-    }
 #pragma unroll
     for (int i = 0; i < C::ACC; ++i) acc[i] = 0.f;
     // slots of the step whose wgmma group is still in flight: weight slot, and the activation slot when that step was
@@ -451,10 +394,9 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
       const uint32_t a_base = a_ring + a_slot * C::A_BYTES;
       for (int t = 0; t < C::SPU; ++t) {
         t0 = tr.now();
-        if (!WS) mbar_wait(smem_u32(&s_bar[kBF + b_slot]), b_ph);
+        mbar_wait(smem_u32(&s_bar[kBF + b_slot]), b_ph);
         tr.add(kTrBFull, t0);
-        const uint32_t b_base = WS ? b_ring + static_cast<uint32_t>((t * (p.Cin / 16) + 2 * ua) * C::B_BLK)
-                                   : b_ring + b_slot * C::B_BYTES;
+        const uint32_t b_base = b_ring + b_slot * C::B_BYTES;
         wg_fence();
 #pragma unroll
         for (int kb = 0; kb < 2; ++kb) {
@@ -464,15 +406,13 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
           for (int mt = 0; mt < MT; ++mt) {
             uint32_t a0, sbo;
             if (HALO) {  // this warpgroup's 8 image rows of M tile mt, shifted by the tap
-              a0 = a_base + static_cast<uint32_t>(((mt * kTH + cw * 8 + t / 3) * PITCH + t % 3) * 128);
-              sbo = PITCH * 128;
+              a0 = a_base + static_cast<uint32_t>(((mt * kTH + cw * 8 + t / 3) * kPitch + t % 3) * 128);
+              sbo = kPitch * 128;
             } else {
               a0 = a_base + static_cast<uint32_t>((mt * kM + cw * 64) * 128);
               sbo = 1024;
             }
-            const uint32_t ah = a0 + kb * 32, al = a0 + (2 + kb) * 32;
-            const uint32_t bo = p.base_offset_mode ? 1u : 0u;
-            const uint64_t dah = gmma_desc(ah, 16, sbo, 1, bo * ((ah >> 7) & 7u)), dal = gmma_desc(al, 16, sbo, 1, bo * ((al >> 7) & 7u));
+            const uint64_t dah = desc_sw128(a0 + kb * 32, sbo), dal = desc_sw128(a0 + (2 + kb) * 32, sbo);
             float *d = acc + mt * N;
             wg::mma_f16<N>(d, dah, dbh, 1u);      // A_hi x B_hi
             wg::mma_f16<N>(d + H, dah, dbl, 1u);  // A_hi x B_lo'
@@ -484,13 +424,13 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
         wg_wait<1>();  // the previous step's group has retired: its slots go back to the producer
         tr.add(kTrMma, t0);
         if (pending) {
-          if (!WS) release(kBE, prev_b);
+          release(kBE, prev_b);
           if (prev_a >= 0) release(kAE, static_cast<uint32_t>(prev_a));
         }
         pending = true;
         prev_b = b_slot;
         prev_a = t == C::SPU - 1 ? static_cast<int>(a_slot) : -1;
-        if (!WS && ++b_slot == C::NB) b_slot = 0, b_ph ^= 1u;
+        if (++b_slot == C::NB) b_slot = 0, b_ph ^= 1u;
       }
       if (++a_slot == C::NA) a_slot = 0, a_ph ^= 1u;
     }
@@ -498,80 +438,29 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
     wg_wait<0>();
     tr.add(kTrMma, t0);
     t0 = tr.now();
-    if (!WS) release(kBE, prev_b);
+    release(kBE, prev_b);
     release(kAE, static_cast<uint32_t>(prev_a));  // the item's last step ends a unit
-    // WS: the last item of a run on this N tile has retired every step that reads the image
-    if (WS && (idx + 1 == n_items || decode<WS>(item_w(idx + 1), p, TH).nt != im.nt)) release(kWE, 0);
     wg_fence_acc<C::ACC>(acc);
-    if constexpr (C::STAGE) {
-      // park hi + cross * 2^-11 in this warpgroup's staging tile (row mt * 64 + fragment row) once the epilogue warps
-      // have drained the previous item from it, and go on with the next item
-      tr.add(kTrEpi, t0);
-      t0 = tr.now();
-      if (idx > 0) mbar_wait(smem_u32(&s_bar[kSF + cw]), static_cast<uint32_t>((idx - 1) & 1));
-      tr.add(kTrStageFree, t0);
-      t0 = tr.now();
-      float *const st = stg + cw * C::STG_WG;
-#pragma unroll
-      for (int mt = 0; mt < MT; ++mt) {
-#pragma unroll
-        for (int i = 0; i < H; i += 2) {
-          const int r = mt * 64 + frag_row(i, wtid), c = frag_col(i, wtid);
-          *reinterpret_cast<float2 *>(st + r * C::SP + c) =
-              make_float2(fmaf(acc[mt * N + H + i], kLoInv, acc[mt * N + i]), fmaf(acc[mt * N + H + i + 1], kLoInv, acc[mt * N + i + 1]));
-        }
-      }
-      mbar_arrive(smem_u32(&s_bar[kSS + cw]));
-      tr.add(kTrEpi, t0);
-      continue;
-    }
-
-    // ------------------------------------------------------------- epilogue in the registers (WS only)
-    const int g_cnt = p.grouped ? __ldg(p.grp_cnt + im.nt) : 0, g_p0 = p.grouped ? __ldg(p.grp_plane0 + im.nt) : 0;
+    // park hi + cross * 2^-11 in this warpgroup's staging tile (row mt * 64 + fragment row) once the epilogue warps have
+    // drained the previous item from it, and go on with the next item
+    tr.add(kTrEpi, t0);
+    t0 = tr.now();
+    if (idx > 0) mbar_wait(smem_u32(&s_bar[kSF + cw]), static_cast<uint32_t>((idx - 1) & 1));
+    tr.add(kTrStageFree, t0);
+    t0 = tr.now();
+    float *const st = stg + cw * C::STG_WG;
 #pragma unroll
     for (int mt = 0; mt < MT; ++mt) {
 #pragma unroll
       for (int i = 0; i < H; i += 2) {
-        const int m = cw * 64 + frag_row(i, wtid), c = frag_col(i, wtid);  // pixel of the M tile, column of the N tile
-        const int iy = im.ty0 + mt * kTH + m / kTW, ix = im.tx0 + m % kTW;
-        const int ch = im.nt * N + c;  // output channel
-        if (iy >= p.oH || ix >= p.oW || (p.grouped ? c >= g_cnt : ch >= p.cout)) continue;
-        const int Y = iy * p.up + (p.up > 1 ? im.tap0 / p.up : 0), X = ix * p.up + (p.up > 1 ? im.tap0 % p.up : 0);
-        const size_t opix = (static_cast<size_t>(im.b) * p.out_H + Y) * p.out_W + X;
-        float v[2];
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const bool okc = p.grouped ? true : ch + e < p.cout;
-          const float sc = (p.scale && okc) ? __ldg(p.scale + ch + e) : 1.0f, sh = (p.shift && okc) ? __ldg(p.shift + ch + e) : 0.0f;
-          float o = fmaf(acc[mt * N + H + i + e], kLoInv, acc[mt * N + i + e]);
-          o = fmaf(o, sc, sh);
-          if (p.relu) o = fmaxf(o, 0.f);
-          v[e] = o;
-        }
-        if (p.out_h16) {  // channel counts of H16 layers are multiples of 16: whole pairs
-          __half h0, l0, h1, l1;
-          split_h16(v[0], h0, l0, ovf);
-          split_h16(v[1], h1, l1, ovf);
-          const int oc = p.out_c0 + ch;
-          uint8_t *op = p.out_h16 + opix * (4 * static_cast<size_t>(p.out_C)) + (oc / 32) * 128 + (oc % 32) * 2;
-          *reinterpret_cast<__half2 *>(op) = __halves2half2(h0, h1);
-          *reinterpret_cast<__half2 *>(op + 64) = __halves2half2(l0, l1);
-        }
-        if (p.out_nchw) {
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            if (p.grouped) {
-              if (c + e < g_cnt) p.out_nchw[((static_cast<size_t>(im.b) * p.cout + g_p0 + c + e) * p.out_H + Y) * p.out_W + X] = v[e];
-            } else if (ch + e < p.cout) {
-              p.out_nchw[((static_cast<size_t>(im.b) * p.cout + ch + e) * p.out_H + Y) * p.out_W + X] = v[e];
-            }
-          }
-        }
+        const int r = mt * 64 + frag_row(i, wtid), c = frag_col(i, wtid);
+        *reinterpret_cast<float2 *>(st + r * C::SP + c) =
+            make_float2(fmaf(acc[mt * N + H + i], kLoInv, acc[mt * N + i]), fmaf(acc[mt * N + H + i + 1], kLoInv, acc[mt * N + i + 1]));
       }
     }
+    mbar_arrive(smem_u32(&s_bar[kSS + cw]));
     tr.add(kTrEpi, t0);
   }
-  if (ovf && p.status) atomicOr(p.status, 1);
   if (cw == 0) {
     tr.count(kTrItems, static_cast<unsigned long long>(n_items));
     tr.add(kTrCycles, t_start);
@@ -645,13 +534,12 @@ inline int make_image_map(const void *img, int B, int H, int W, int Cin, int str
   return r == CUDA_SUCCESS ? P3D_OK : P3D_ERR_INVALID_ARG;
 }
 
-template <int N, int MT, bool HALO, int PITCH, bool WS = false>
+template <int N, int MT, bool HALO>
 int launch(const CUtensorMap &map, const Params &p, cudaStream_t st) {
-  using C = Cfg<N, MT, HALO, PITCH, WS>;
-  const size_t smem = static_cast<size_t>(C::NA) * C::A_BYTES +
-                      (WS ? static_cast<size_t>(p.w_bytes) : static_cast<size_t>(C::NB) * C::B_BYTES) + C::STG_BYTES + 1024;
-  if (smem > static_cast<size_t>(227 - 6) * 1024) return P3D_ERR_UNSUPPORTED;
-  auto kern = dense_conv_f16_kernel<N, MT, HALO, PITCH, WS>;
+  using C = Cfg<N, MT, HALO>;
+  const size_t smem = static_cast<size_t>(C::NA) * C::A_BYTES + static_cast<size_t>(C::NB) * C::B_BYTES + C::STG_BYTES + 1024;
+  if (smem > static_cast<size_t>(kSmemBudget)) return P3D_ERR_UNSUPPORTED;
+  auto kern = dense_conv_f16_kernel<N, MT, HALO>;
   P3D_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   const long long work = static_cast<long long>(p.B) * p.tiles_y * p.tiles_x * p.n_ntiles * (p.up > 1 ? p.up * p.up : 1);
   cudaLaunchConfig_t cfg = {};
@@ -673,7 +561,7 @@ int launch(const CUtensorMap &map, const Params &p, cudaStream_t st) {
 // ---------------------------------------------------------------------------------------------------------------------
 // CenterHead output convs with the 9 taps in the N dimension ("tap-as-N", center_head.py:80-117 SeparateHead finals).
 //
-// A 3x3 conv with <= 3 output channels is 9 * Cin/16 k-steps of N = 16 MMAs per 128 pixels in the generic kernel above.
+// A 3x3 conv with <= 3 output channels would be 9 * Cin/16 k-steps of N = 16 MMAs per 128 pixels as an ordinary conv.
 // Here one item is a 16 x 16-pixel haloed tile (256 rows = 2 M tiles) of one group's Cin channels and ONE GEMM
 //     P[pixel][tap * 3 + co] = sum_c  mid[pixel][c] * W[tap][c][co]            (N = 27 -> 32, K = Cin: 4 k-steps for 64)
 // the epilogue parks P in shared memory and every output pixel of the 14 x 14 interior adds its 9 shifted
@@ -870,14 +758,14 @@ extern "C" size_t p3d_dense_conv2d_f16_packed_weight_bytes(int taps, int Cin, in
   return align_up(tiles * taps * Cin * static_cast<size_t>(n_tile) * 4);
 }
 
-// mode: 0 auto (HALO for 3x3 stride 1 pad 1 convolutions - weight-stationary when it applies -, TAP otherwise), 1 force TAP,
-// 2 force the weight-stationary kernel (P3D_ERR_UNSUPPORTED when it does not apply); m_tiles: 0 auto, 1 or 2
-static int dense_conv_f16(const void *in_h16, int B, int H, int W, int Cin, const void *packed_weight, int Cout, int n_tile,
-                          int kh, int kw, int stride, int pad, int up, const float *scale, const float *shift, int relu,
-                          void *out_h16, int out_C, int out_c0, float *out_nchw, int mode, int m_tiles, int32_t *status_dev,
-                          p3d_stream_t stream, int groups, int in_C, const int32_t *grp_plane0, const int32_t *grp_cnt) {
-  if (!in_h16 || !packed_weight || (!out_h16 && !out_nchw) || B < 1 || H < 1 || W < 1 || Cout < 1) return P3D_ERR_INVALID_ARG;
-  if (Cin < 32 || Cin % 32 || (n_tile != 64 && n_tile != 128 && !(groups && n_tile == 16))) return P3D_ERR_UNSUPPORTED;
+// mode: 0 auto (HALO for 3x3 stride 1 pad 1 convolutions, TAP otherwise), 1 force TAP; m_tiles: 0 auto, 1 or 2
+extern "C" int p3d_dense_conv2d_f16(const void *in_h16, int B, int H, int W, int Cin, const void *packed_weight, int Cout,
+                                    int n_tile, int kh, int kw, int stride, int pad, int up, const float *scale,
+                                    const float *shift, int relu, void *out_h16, int out_C, int out_c0, float *out_nchw,
+                                    int mode, int m_tiles, int32_t *status_dev, p3d_stream_t stream) {
+  if (!in_h16 || !packed_weight || (!out_h16 && !out_nchw) || B < 1 || H < 1 || W < 1 || Cout < 1 || (mode != 0 && mode != 1))
+    return P3D_ERR_INVALID_ARG;
+  if (Cin < 32 || Cin % 32 || (n_tile != 64 && n_tile != 128)) return P3D_ERR_UNSUPPORTED;
   if (up < 1 || (up > 1 && (kh != up || kw != up || stride != up || pad != 0))) return P3D_ERR_UNSUPPORTED;
   if (up == 1 && (kh < 1 || kw < 1 || kh * kw > 32 || stride < 1 || stride > 2 || pad < 0)) return P3D_ERR_UNSUPPORTED;
   if (out_h16 && (Cout % 16 || out_C % 32 || out_c0 % 16 || out_c0 + Cout > out_C)) return P3D_ERR_INVALID_ARG;
@@ -899,12 +787,8 @@ static int dense_conv_f16(const void *in_h16, int B, int H, int W, int Cin, cons
   if (p.oH < 1 || p.oW < 1) return P3D_ERR_INVALID_ARG;
   p.out_H = up > 1 ? H * up : p.oH;
   p.out_W = up > 1 ? W * up : p.oW;
-  p.n_ntiles = groups ? groups : (Cout + n_tile - 1) / n_tile;
+  p.n_ntiles = (Cout + n_tile - 1) / n_tile;
   p.cout = Cout;
-  p.grouped = groups ? 1 : 0;
-  p.in_C = groups ? in_C : Cin;
-  p.grp_plane0 = grp_plane0;
-  p.grp_cnt = grp_cnt;
   p.out_C = out_C;
   p.out_c0 = out_c0;
   p.relu = relu;
@@ -914,17 +798,7 @@ static int dense_conv_f16(const void *in_h16, int B, int H, int W, int Cin, cons
   p.out_h16 = static_cast<uint8_t *>(out_h16);
   p.out_nchw = out_nchw;
   p.status = status_dev;
-  static const int env_mode = getenv("P3D_DENSE_MODE") ? atoi(getenv("P3D_DENSE_MODE")) : -1;  // tuning hooks
-  static const int env_mt = getenv("P3D_DENSE_MT") ? atoi(getenv("P3D_DENSE_MT")) : -1;
-  static const int env_pitch = getenv("P3D_DENSE_PITCH") ? atoi(getenv("P3D_DENSE_PITCH")) : 10;
-  // shifted tiles read correctly with base_offset = 0: the swizzle is a function of the absolute shared-memory address
-  // (tests/test_gpu_dense.py); P3D_DENSE_BO=1 sets it to the address bits 7-9 instead
-  static const int env_bo = getenv("P3D_DENSE_BO") ? atoi(getenv("P3D_DENSE_BO")) : 0;
-  p.base_offset_mode = env_bo;
-  int pitch = env_pitch == 16 ? 16 : 10;
-  if (env_mode >= 0) mode = env_mode;
-  if (env_mt >= 0) m_tiles = env_mt;
-  const bool halo = (mode == 0 || mode == 2) && up == 1 && kh == 3 && kw == 3 && stride == 1 && pad == 1;
+  const bool halo = mode == 0 && up == 1 && kh == 3 && kw == 3 && stride == 1 && pad == 1;
   // one or two M tiles per item for the narrow N <= 64 layers (N = 128 keeps one: register budget): the persistent grid
   // runs ceil(items / SMs) rounds of items MT M tiles long, so pick the MT with the fewer M-tile rounds; on a tie two M
   // tiles, which share every weight block (half the weight traffic per flop)
@@ -935,64 +809,17 @@ static int dense_conv_f16(const void *in_h16, int B, int H, int W, int Cin, cons
     const long long items1 = per_row * ((p.oH + dcf::kTH - 1) / dcf::kTH), items2 = per_row * ((p.oH + 2 * dcf::kTH - 1) / (2 * dcf::kTH));
     mt = (n_tile <= 64 && 2 * ((items2 + sms - 1) / sms) <= (items1 + sms - 1) / sms) ? 2 : 1;
   }
-  // weight-stationary variant: haloed 3x3, N tile 64, the N tile's weight image + 3 activation tiles fit in shared memory,
-  // and every CTA has enough pixel tiles per weight image to amortise loading it (mode 2 forces it, P3D_DENSE_WS=0 disables)
-  // The variant is OFF unless asked for (mode 2 or P3D_DENSE_WS=1): it was not faster than the streaming N = 128 kernel on
-  // the CenterHead's 64 -> 2304 layer.
-  static const int env_ws = getenv("P3D_DENSE_WS") ? atoi(getenv("P3D_DENSE_WS")) : 0;
-  p.w_bytes = p.taps * (Cin / 16) * 64 * n_tile;
-  bool ws = false;
-  if (halo && n_tile == 64 && !groups && pitch == 10 && (env_ws || mode == 2)) {
-    const size_t need = 3 * static_cast<size_t>(dcf::Cfg<64, 1, true, 10, true>::A_BYTES) + p.w_bytes + 1024;
-    const long long pix = static_cast<long long>(B) * ((p.oW + dcf::kTW - 1) / dcf::kTW) * ((p.oH + dcf::kTH - 1) / dcf::kTH);
-    const long long items = pix * p.n_ntiles;
-    ws = need <= static_cast<size_t>(227 - 6) * 1024 && (mode == 2 || items >= 8ll * num_sms());
-  }
-  if (mode == 2 && !ws) return P3D_ERR_UNSUPPORTED;
-  if (ws || n_tile > 64) mt = 1;  // two M tiles of a 128-wide N tile would need 256 accumulator registers per thread
-  if (mt == 2) pitch = 10;        // two haloed M tiles at pitch 16 leave no room for the epilogue's staging tiles
+  if (n_tile > 64) mt = 1;  // two M tiles of a 128-wide N tile would need 256 accumulator registers per thread
   p.tiles_x = (p.oW + dcf::kTW - 1) / dcf::kTW;
   p.tiles_y = (p.oH + dcf::kTH * mt - 1) / (dcf::kTH * mt);
   CUtensorMap map;
-  const int bx = halo ? pitch : dcf::kTW, by = halo ? dcf::kTH * mt + 2 : dcf::kTH * mt;
-  const int rc = dcf::make_image_map(in_h16, B, H, W, p.in_C, p.stride, bx, by, &map);
+  const int bx = halo ? dcf::kPitch : dcf::kTW, by = halo ? dcf::kTH * mt + 2 : dcf::kTH * mt;
+  const int rc = dcf::make_image_map(in_h16, B, H, W, Cin, p.stride, bx, by, &map);
   if (rc != P3D_OK) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (ws) return dcf::launch<64, 1, true, 10, true>(map, p, st);
-#define P3D_DCF(NT, M)                                                                          \
-  if (n_tile == NT && mt == M) {                                                                \
-    if (!halo) return dcf::launch<NT, M, false, 10>(map, p, st);                                \
-    if (M == 1 && pitch == 16) return dcf::launch<NT, 1, true, 16>(map, p, st);                 \
-    return dcf::launch<NT, M, true, 10>(map, p, st);                                            \
-  }
-  P3D_DCF(16, 1)
-  P3D_DCF(16, 2)
-  P3D_DCF(64, 1)
-  P3D_DCF(64, 2)
-  P3D_DCF(128, 1)
-#undef P3D_DCF
-  return P3D_ERR_UNSUPPORTED;
-}
-
-extern "C" int p3d_dense_conv2d_f16(const void *in_h16, int B, int H, int W, int Cin, const void *packed_weight, int Cout,
-                                    int n_tile, int kh, int kw, int stride, int pad, int up, const float *scale,
-                                    const float *shift, int relu, void *out_h16, int out_C, int out_c0, float *out_nchw,
-                                    int mode, int m_tiles, int32_t *status_dev, p3d_stream_t stream) {
-  return dense_conv_f16(in_h16, B, H, W, Cin, packed_weight, Cout, n_tile, kh, kw, stride, pad, up, scale, shift, relu, out_h16,
-                        out_C, out_c0, out_nchw, mode, m_tiles, status_dev, stream, 0, 0, nullptr, nullptr);
-}
-
-// Grouped 3x3 / stride 1 / pad 1 output convs (CenterHead SeparateHead finals, center_head.py:80-117) on the tensor cores:
-// group g convolves input channels [g * Cin, (g + 1) * Cin) of the in_C-channel image with its own W[9][Cin][16]
-// (columns >= cnt[g] zero) and writes cnt[g] fp32 planes from plane0[g] of out_nchw [B, planes, H, W].
-// packed_weight: `groups` weight tiles of p3d_dense_conv2d_f16_pack_weights(taps 9, Cin, n_tile 16); bias [groups][16].
-extern "C" int p3d_grouped_head_conv_f16(const void *in_h16, int B, int H, int W, int in_C, int Cin, int groups,
-                                         const void *packed_weight, const float *bias, const int32_t *plane0_dev,
-                                         const int32_t *cnt_dev, int planes, float *out_nchw, int32_t *status_dev,
-                                         p3d_stream_t stream) {
-  if (!plane0_dev || !cnt_dev || groups < 1 || groups * Cin > in_C || in_C % 32 || planes < 1) return P3D_ERR_INVALID_ARG;
-  return dense_conv_f16(in_h16, B, H, W, Cin, packed_weight, planes, 16, 3, 3, 1, 1, 1, nullptr, bias, 0, nullptr, 32, 0, out_nchw,
-                        0, 0, status_dev, stream, groups, in_C, plane0_dev, cnt_dev);
+  if (n_tile == 128) return halo ? dcf::launch<128, 1, true>(map, p, st) : dcf::launch<128, 1, false>(map, p, st);
+  if (mt == 2) return halo ? dcf::launch<64, 2, true>(map, p, st) : dcf::launch<64, 2, false>(map, p, st);
+  return halo ? dcf::launch<64, 1, true>(map, p, st) : dcf::launch<64, 1, false>(map, p, st);
 }
 
 // Output convs of the CenterHead, 9 taps in the GEMM's N dimension (dcf::out9 above): group g convolves input channels
@@ -1006,11 +833,16 @@ extern "C" int p3d_head_out_conv_f16(const void *in_h16, int B, int H, int W, in
   if (!in_h16 || !packed_weight || !bias || !plane0_dev || !cnt_dev || !out_nchw || B < 1 || H < 1 || W < 1 || groups < 1 ||
       planes < 1 || in_C % 32 || Cin > in_C)
     return P3D_ERR_INVALID_ARG;
-  if (Cin != 32 && Cin != 64 && Cin != 128) return P3D_ERR_UNSUPPORTED;
+  if (Cin < 32 || Cin % 32) return P3D_ERR_UNSUPPORTED;
   if ((reinterpret_cast<uintptr_t>(in_h16) & 15) || (reinterpret_cast<uintptr_t>(packed_weight) & 15) ||
       (reinterpret_cast<uintptr_t>(bias) & 15))
     return P3D_ERR_INVALID_ARG;
   namespace o9 = dcf::out9;
+  // activation ring: as many slots as the shared-memory budget leaves after the alignment slack, P and the weight ring
+  // (Cin = 32 / 64 / 128: 5 / 5 / 4 slots; fewer than two above Cin = 320)
+  const long long w_ring = static_cast<long long>(o9::kNW) * 2 * (Cin / 32) * o9::kWBlk;
+  const long long na = (dcf::kSmemBudget - 1024 - o9::kPBytes - w_ring) / o9::kABytes;
+  if (na < 2) return P3D_ERR_UNSUPPORTED;
   o9::Params p;
   p.B = B;
   p.H = H;
@@ -1020,7 +852,7 @@ extern "C" int p3d_head_out_conv_f16(const void *in_h16, int B, int H, int W, in
   p.tiles_y = (H + o9::kOT - 1) / o9::kOT;
   p.groups = groups;
   p.planes = planes;
-  p.NA = p.G <= 2 ? 5 : 4;
+  p.NA = static_cast<int>(na < o9::kMaxNA ? na : o9::kMaxNA);
   p.packed_w = static_cast<const uint8_t *>(packed_weight);
   p.bias = bias;
   p.cin0 = cin0_dev;
@@ -1030,7 +862,7 @@ extern "C" int p3d_head_out_conv_f16(const void *in_h16, int B, int H, int W, in
   CUtensorMap map;
   const int rc = dcf::make_image_map(in_h16, B, H, W, in_C, 1, o9::kHT, o9::kHT, &map);
   if (rc != P3D_OK) return rc;
-  const size_t smem = static_cast<size_t>(p.NA) * o9::kABytes + static_cast<size_t>(o9::kNW) * 2 * p.G * o9::kWBlk + o9::kPBytes + 1024;
+  const size_t smem = static_cast<size_t>(p.NA) * o9::kABytes + static_cast<size_t>(w_ring) + o9::kPBytes + 1024;
   auto kern = o9::head_out9_kernel;
   P3D_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   const long long work = static_cast<long long>(B) * p.tiles_y * p.tiles_x * groups;

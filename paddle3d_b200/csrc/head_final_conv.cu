@@ -4,14 +4,11 @@
 // per 32 input channels of one head; here a block stages a 16 x 8 pixel tile (+ halo) of one head's 64 input channels
 // in shared memory, channel-major, and every thread accumulates the <= 4 outputs of its pixel with exact fp32 FMAs in
 // (tap, channel) order.
-// Checked by tests/test_gpu_dense.py::test_batched_head_matches_per_layer_head.  Two input formats: tf32
-// pixel split rows (p3d_head_final_conv) and fp16-pair pixel H16 rows (p3d_head_final_conv_h16).
+// Checked by tests/test_gpu_dense.py::test_batched_head_matches_per_layer_head.
 //
 //   input   pixel split rows [B*H*W][2][in_C]; group g reads channels [g*Cin, (g+1)*Cin) as hi + lo
 //   weight  [groups][9][Cin][4] fp32 (outputs zero-padded to 4), bias [groups][4]
 //   output  fp32 planes [B][planes][H][W]; group g writes planes plane0[g] .. plane0[g] + cnt[g] - 1
-#include <cuda_fp16.h>
-
 #include "common.cuh"
 #include "p3d_b200.h"
 
@@ -29,7 +26,6 @@ struct FinalParams {
   int cnt[kMaxGroups];
 };
 
-template <bool H16>
 __global__ void __launch_bounds__(128) head_final_conv_kernel(const float *__restrict__ in_split, FinalParams p,
                                                               const float *__restrict__ weight,
                                                               const float *__restrict__ bias, float *__restrict__ out) {
@@ -51,14 +47,8 @@ __global__ void __launch_bounds__(128) head_final_conv_kernel(const float *__res
     float v = 0.f;
     if (y >= 0 && y < p.H && x >= 0 && x < p.W) {
       const size_t pix = (static_cast<size_t>(b) * p.H + y) * p.W + x;
-      if (H16) {  // pixel H16 rows: groups of 32 channels [hi 32 | lo' 32] halfs, x = hi + lo' * 2^-11
-        const int ch = g * p.Cin + c;
-        const __half *grp = reinterpret_cast<const __half *>(in_split) + pix * (2 * static_cast<size_t>(p.in_C)) + (ch / 32) * 64;
-        v = fmaf(__half2float(grp[32 + ch % 32]), 1.0f / 2048.0f, __half2float(grp[ch % 32]));
-      } else {
-        const float *row = in_split + pix * (2 * static_cast<size_t>(p.in_C));
-        v = __ldg(row + g * p.Cin + c) + __ldg(row + p.in_C + g * p.Cin + c);
-      }
+      const float *row = in_split + pix * (2 * static_cast<size_t>(p.in_C));
+      v = __ldg(row + g * p.Cin + c) + __ldg(row + p.in_C + g * p.Cin + c);
     }
     s_x[c * kPitch + px] = v;
   }
@@ -90,9 +80,9 @@ __global__ void __launch_bounds__(128) head_final_conv_kernel(const float *__res
 
 using namespace p3d;
 
-static int final_conv(const float *in_split, bool h16, int B, int H, int W, int in_C, int Cin, int groups,
-                      const float *weight, const float *bias, const int32_t *plane0_host, const int32_t *cnt_host, int planes,
-                      float *out_nchw, p3d_stream_t stream) {
+extern "C" int p3d_head_final_conv(const float *in_split, int B, int H, int W, int in_C, int Cin, int groups,
+                                   const float *weight, const float *bias, const int32_t *plane0_host,
+                                   const int32_t *cnt_host, int planes, float *out_nchw, p3d_stream_t stream) {
   if (!in_split || !weight || !bias || !plane0_host || !cnt_host || !out_nchw || B < 1 || H < 1 || W < 1)
     return P3D_ERR_INVALID_ARG;
   if (groups < 1 || groups > kMaxGroups || Cin < 4 || Cin % 4 || groups * Cin > in_C || planes < 1)
@@ -116,31 +106,10 @@ static int final_conv(const float *in_split, bool h16, int B, int H, int W, int 
   const size_t smem = (static_cast<size_t>(Cin) * kPitch + 9 * static_cast<size_t>(Cin) * 4) * sizeof(float);
   if (smem > 200 * 1024) return P3D_ERR_UNSUPPORTED;
   const long long blocks = static_cast<long long>(B) * p.tiles_y * p.tiles_x * groups;
-  if (h16) {
-    P3D_CUDA_CHECK(cudaFuncSetAttribute(head_final_conv_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        static_cast<int>(smem)));
-    head_final_conv_kernel<true><<<static_cast<unsigned int>(blocks), 128, smem, static_cast<cudaStream_t>(stream)>>>(
-        in_split, p, weight, bias, out_nchw);
-  } else {
-    P3D_CUDA_CHECK(cudaFuncSetAttribute(head_final_conv_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        static_cast<int>(smem)));
-    head_final_conv_kernel<false><<<static_cast<unsigned int>(blocks), 128, smem, static_cast<cudaStream_t>(stream)>>>(
-        in_split, p, weight, bias, out_nchw);
-  }
+  P3D_CUDA_CHECK(cudaFuncSetAttribute(head_final_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      static_cast<int>(smem)));
+  head_final_conv_kernel<<<static_cast<unsigned int>(blocks), 128, smem, static_cast<cudaStream_t>(stream)>>>(
+      in_split, p, weight, bias, out_nchw);
   P3D_LAUNCH_CHECK();
   return P3D_OK;
-}
-
-extern "C" int p3d_head_final_conv(const float *in_split, int B, int H, int W, int in_C, int Cin, int groups,
-                                   const float *weight, const float *bias, const int32_t *plane0_host,
-                                   const int32_t *cnt_host, int planes, float *out_nchw, p3d_stream_t stream) {
-  return final_conv(in_split, false, B, H, W, in_C, Cin, groups, weight, bias, plane0_host, cnt_host, planes, out_nchw, stream);
-}
-
-extern "C" int p3d_head_final_conv_h16(const void *in_h16, int B, int H, int W, int in_C, int Cin, int groups,
-                                       const float *weight, const float *bias, const int32_t *plane0_host,
-                                       const int32_t *cnt_host, int planes, float *out_nchw, p3d_stream_t stream) {
-  if (in_C % 32) return P3D_ERR_INVALID_ARG;
-  return final_conv(static_cast<const float *>(in_h16), true, B, H, W, in_C, Cin, groups, weight, bias, plane0_host, cnt_host,
-                    planes, out_nchw, stream);
 }

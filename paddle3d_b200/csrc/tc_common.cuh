@@ -81,13 +81,11 @@ __device__ __forceinline__ void wg_fence_acc(float *d) {
 // distance between the two 16-byte K-chunks of one k-step, SBO = distance between 8-row groups.  K-major swizzled: LBO
 // unused (1), SBO = 8 rows x row pitch; the swizzle is applied to the absolute shared-memory address, so a start
 // address advanced by k-steps (or by whole rows) reads what TMA / the XOR-ing producers wrote.
-__device__ __forceinline__ uint64_t gmma_desc(uint32_t addr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout,
-                                              uint32_t base_offset = 0) {
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t addr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((addr & 0x3ffffu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3fffu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3fffu) << 32;
-  d |= static_cast<uint64_t>(base_offset & 7u) << 49;
   d |= static_cast<uint64_t>(layout) << 62;
   return d;
 }

@@ -5,10 +5,8 @@ with BatchNorm folded into the conv epilogue.  Same constructor vocabulary as th
 (configs/centerpoint/centerpoint_voxels_0075voxel_nuscenes_10sweep.yml:127-162).  Default arithmetic: fp16 (hi, lo')
 pair operands on wgmma (csrc/dense_conv_f16.cu, `f16=True`); the tf32-pair kernels stay selectable
 (`f16=False`) for data outside fp16's range.  The 36 ConvModules of the heads run as ONE 64 -> 2304 convolution and
-the 36 output convs as one grouped CUDA-core launch (forward); forward_per_head keeps the layer-by-layer form for
-the parity tests."""
-import os
-
+the 36 output convs as one launch (forward: tap-as-N tensor-core kernel on the fp16-pair path, CUDA cores on the tf32
+one); forward_per_head keeps the layer-by-layer form for the parity tests."""
 import numpy as np
 import torch
 
@@ -27,7 +25,7 @@ class _Conv:
         self.transposed = transposed or up > 1
         self.has_bias, self.bn_eps, self.relu = bias, bn_eps, relu
         self.f16 = f16 and cout >= 16  # the 1-3 channel output convs of the heads run on the CUDA cores (forward)
-        self.n_tile = dc.n_tile_for_f16(cout, cin, k, stride, padding, up) if self.f16 else dc.n_tile_for(cout)
+        self.n_tile = dc.n_tile_for_f16(cout) if self.f16 else dc.n_tile_for(cout)
         self.np = None
         self.dev = None
 
@@ -148,6 +146,9 @@ class DenseRPNHead:
         self.num_classes = list(tasks)        # CenterHead.num_classes (center_head.py:64)
         self.with_velocity = with_velocity    # 'vel' in common_heads (center_head.py:77)
         self.f16 = f16
+        if f16 and (share_conv_channel % 32 or not 32 <= share_conv_channel <= 320):
+            raise ValueError("the fp16-pair head output convs need share_conv_channel a multiple of 32 and at most 320 "
+                             "(got %d); use f16=False" % share_conv_channel)
 
         def conv(*a, **k):
             return _Conv(*a, f16=f16, **k)
@@ -179,7 +180,7 @@ class DenseRPNHead:
         hm_finals = {id(b) for hs in self.heads for name, _, b in hs if name == "hm"}
         finals = {id(b) for hs in self.heads for _, _, b in hs}
         for c in self.all_convs():  # hm bias = -2.19 (center_head.py:113-117)
-            # the 1-3 channel output convs have no tensor-core image in f16 mode: they run grouped on the CUDA cores
+            # the 1-3 channel output convs have no per-conv image in f16 mode: they run in one tap-as-N launch
             dev = None if (self.f16 and id(c) in finals) else device
             c.init(rng, dev, randomize_bn, bias_value=-2.19 if id(c) in hm_finals else None, bn_gain=bn_gain)
         self._batched = None
@@ -220,21 +221,17 @@ class DenseRPNHead:
         return s, (b, H, W, self.shared.cout)
 
     def _final_convs(self, mid, shape, in_C, groups_params, planes_total, device):
-        """Grouped 64 -> {1..3} output convs in one launch: tensor cores on the fp16-pair path (p3d_grouped_head_conv_f16),
-        CUDA cores (p3d_head_final_conv) on the tf32 one."""
+        """Grouped 64 -> {1..3} output convs in one launch: tensor cores with the 9 taps in the GEMM's N dimension on the
+        fp16-pair path (p3d_head_out_conv_f16), CUDA cores (p3d_head_final_conv) on the tf32 one."""
         from ._lib import check, lib
         from ._mem import ptr, stream
         b, H, W, cin = shape
         gp = groups_params
         planes = torch.empty((b, planes_total, H, W), dtype=torch.float32, device=device)
-        if self.f16 and "packed9" in gp and not os.environ.get("P3D_HEAD_OUT_N16"):
+        if self.f16:
             check(lib().p3d_head_out_conv_f16(ptr(mid), b, H, W, in_C, cin, int(gp["cnt9"].numel()), ptr(gp["packed9"]),
                                               ptr(gp["bias9"]), ptr(gp["cin0_9"]), ptr(gp["plane0_9"]), ptr(gp["cnt9"]),
                                               planes_total, ptr(planes), stream(device)), "head_out_conv_f16")
-        elif self.f16:
-            check(lib().p3d_grouped_head_conv_f16(ptr(mid), b, H, W, in_C, cin, len(gp["cnt"]), ptr(gp["packed16"]),
-                                                  ptr(gp["bias16"]), ptr(gp["plane0_dev"]), ptr(gp["cnt_dev"]), planes_total,
-                                                  ptr(planes), ptr(dc._status(device)), stream(device)), "grouped_head_conv_f16")
         else:
             check(lib().p3d_head_final_conv(ptr(mid), b, H, W, in_C, cin, len(gp["cnt"]), ptr(gp["fw"]), ptr(gp["fb"]),
                                             gp["plane0"].ctypes.data, gp["cnt"].ctypes.data, planes_total, ptr(planes),
@@ -242,66 +239,54 @@ class DenseRPNHead:
         return planes
 
     def _group_params(self, finals, cin, device):
-        """Weights of a list of output convs [(name, _Conv)] in both grouped forms: [groups][9][Cin][4] fp32 for the
-        CUDA-core kernel, and per-group tensor-core tiles W[9][Cin][16] (fp16-pair k-blocks) + bias [groups][16]."""
+        """Weights of a list of output convs [(name, _Conv)] in the grouped form of _final_convs: on the fp16-pair path
+        per (virtual) group the tap-as-N weight image W2[c][tap * 3 + co] + bias [4]; on the tf32 one [groups][9][Cin][4]
+        fp32 + bias [groups][4] for the CUDA-core kernel."""
         groups = len(finals)
-        fw = np.zeros((groups, 9, cin, 4), np.float32)
-        fb = np.zeros((groups, 4), np.float32)
-        w16 = np.zeros((groups, 9, cin, 16), np.float32)
-        b16 = np.zeros((groups, 16), np.float32)
-        plane0, cnt, p0 = [], [], 0
-        for g, (_, f) in enumerate(finals):
-            k = f.cout
-            wt = f.np["weight"].transpose(2, 3, 1, 0).reshape(9, cin, k)  # [k, cin, 3, 3] -> [tap][cin][k]
-            fw[g, :, :, :k] = wt
-            w16[g, :, :, :k] = wt
-            fb[g, :k] = f.np["bias"]
-            b16[g, :k] = f.np["bias"]
+        wts, plane0, cnt, p0 = [], [], [], 0
+        for _, f in finals:
+            wts.append(f.np["weight"].transpose(2, 3, 1, 0).reshape(9, cin, f.cout))  # [k, cin, 3, 3] -> [tap][cin][k]
             plane0.append(p0)
-            cnt.append(k)
-            p0 += k
+            cnt.append(f.cout)
+            p0 += f.cout
         out = dict(plane0=np.asarray(plane0, np.int32), cnt=np.asarray(cnt, np.int32), planes=p0)
-        if self.f16:
-            from ._lib import check, lib
-            from ._mem import ptr, stream
-            L = lib()
-            blk = 9 * cin * 16 * 4
-            packed = torch.zeros((groups * blk,), dtype=torch.uint8, device=device)
-            for g in range(groups):
-                wt = torch.from_numpy(w16[g]).to(device)
-                check(L.p3d_dense_conv2d_f16_pack_weights(ptr(wt), 9, cin, 16, ptr(packed[g * blk:(g + 1) * blk]),
-                                                          ptr(dc._status(device)), stream(device)), "pack_weights")
-            out.update(packed16=packed, bias16=torch.from_numpy(b16).to(device),
-                       plane0_dev=torch.from_numpy(out["plane0"]).to(device), cnt_dev=torch.from_numpy(out["cnt"]).to(device))
-            if cin in (32, 64, 128):
-                # tap-as-N form (p3d_head_out_conv_f16): W2[c][tap * 3 + j]; a conv with more than 3 output channels
-                # becomes several virtual groups over the same input slice
-                w9, b9, cin0, pl0, cn = [], [], [], [], []
-                for g, (_, f) in enumerate(finals):
-                    for j0 in range(0, f.cout, 3):
-                        k = min(3, f.cout - j0)
-                        w27 = np.zeros((cin, 9, 3), np.float32)
-                        w27[:, :, :k] = w16[g][:, :, j0:j0 + k].transpose(1, 0, 2)  # [tap][c][j] -> [c][tap][j]
-                        w2 = np.zeros((cin, 32), np.float32)
-                        w2[:, :27] = w27.reshape(cin, 27)
-                        bb = np.zeros((4,), np.float32)
-                        bb[:k] = b16[g, j0:j0 + k]
-                        w9.append(w2)
-                        b9.append(bb)
-                        cin0.append(g * cin)
-                        pl0.append(int(plane0[g]) + j0)
-                        cn.append(k)
-                blk9 = cin * 32 * 4
-                packed9 = torch.zeros((len(w9) * blk9,), dtype=torch.uint8, device=device)
-                for v, w2 in enumerate(w9):
-                    wt = torch.from_numpy(w2).to(device)
-                    check(L.p3d_dense_conv2d_f16_pack_weights(ptr(wt), 1, cin, 32, ptr(packed9[v * blk9:(v + 1) * blk9]),
-                                                              ptr(dc._status(device)), stream(device)), "pack_weights")
-                i32 = lambda a: torch.from_numpy(np.asarray(a, np.int32)).to(device)  # noqa: E731
-                out.update(packed9=packed9, bias9=torch.from_numpy(np.stack(b9)).to(device), cin0_9=i32(cin0),
-                           plane0_9=i32(pl0), cnt9=i32(cn))
-        else:
+        if not self.f16:
+            fw = np.zeros((groups, 9, cin, 4), np.float32)
+            fb = np.zeros((groups, 4), np.float32)
+            for g, (_, f) in enumerate(finals):
+                fw[g, :, :, :f.cout] = wts[g]
+                fb[g, :f.cout] = f.np["bias"]
             out.update(fw=torch.from_numpy(fw).to(device), fb=torch.from_numpy(fb).to(device))
+            return out
+        from ._lib import check, lib
+        from ._mem import ptr, stream
+        L = lib()
+        # tap-as-N form (p3d_head_out_conv_f16): W2[c][tap * 3 + j]; a conv with more than 3 output channels becomes
+        # several virtual groups over the same input slice
+        w9, b9, cin0, pl0, cn = [], [], [], [], []
+        for g, (_, f) in enumerate(finals):
+            for j0 in range(0, f.cout, 3):
+                k = min(3, f.cout - j0)
+                w27 = np.zeros((cin, 9, 3), np.float32)
+                w27[:, :, :k] = wts[g][:, :, j0:j0 + k].transpose(1, 0, 2)  # [tap][c][j] -> [c][tap][j]
+                w2 = np.zeros((cin, 32), np.float32)
+                w2[:, :27] = w27.reshape(cin, 27)
+                bb = np.zeros((4,), np.float32)
+                bb[:k] = f.np["bias"][j0:j0 + k]
+                w9.append(w2)
+                b9.append(bb)
+                cin0.append(g * cin)
+                pl0.append(int(plane0[g]) + j0)
+                cn.append(k)
+        blk9 = cin * 32 * 4
+        packed9 = torch.zeros((len(w9) * blk9,), dtype=torch.uint8, device=device)
+        for v, w2 in enumerate(w9):
+            wt = torch.from_numpy(w2).to(device)
+            check(L.p3d_dense_conv2d_f16_pack_weights(ptr(wt), 1, cin, 32, ptr(packed9[v * blk9:(v + 1) * blk9]),
+                                                      ptr(dc._status(device)), stream(device)), "pack_weights")
+        i32 = lambda a: torch.from_numpy(np.asarray(a, np.int32)).to(device)  # noqa: E731
+        out.update(packed9=packed9, bias9=torch.from_numpy(np.stack(b9)).to(device), cin0_9=i32(cin0), plane0_9=i32(pl0),
+                   cnt9=i32(cn))
         return out
 
     def _batched_params(self, device):

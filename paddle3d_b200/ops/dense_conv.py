@@ -86,18 +86,12 @@ def dense_conv2d(x_split, shape, packed, cout, n_tile, kernel, stride=1, padding
 # ---------------------------------------------------------------------------------------------------------------------
 # fp16-pair ("H16") path (csrc/dense_conv_f16.cu): the default of DenseRPNHead.  Images are pixel H16 rows
 # [B*H*W, 2*C] float16 = per pixel, groups of 32 channels [hi 32 | lo' 32]; x = hi + lo' * 2^-11.
-def n_tile_for_f16(cout, cin=None, kernel=None, stride=1, padding=0, up=1):
-    """Output-channel tile.  P3D_DENSE_NTILE (tuning hook) forces 64 or 128 for the wide layers.  With P3D_DENSE_WS=1 a
-    3x3 / stride 1 / pad 1 layer with few input and many output channels (the 64 -> 36 x 64 ConvModules of the CenterHead)
-    takes 64 and the kernel keeps the N tile's whole weight image (9 * Cin * 256 bytes <= 144 KB) in shared memory
-    (weight-stationary); not faster than the streaming N = 128 kernel, hence opt-in."""
+def n_tile_for_f16(cout):
+    """Output-channel tile.  P3D_DENSE_NTILE (tuning hook) forces 64 or 128 for the wide layers."""
     import os
     forced = os.environ.get("P3D_DENSE_NTILE")
     if forced and cout >= 128:
         return int(forced)
-    if (cin is not None and kernel == 3 and stride == 1 and padding == 1 and up == 1 and cin <= 64 and cout >= 256
-            and os.environ.get("P3D_DENSE_WS", "0") != "0"):  # opt-in
-        return 64
     return 128 if cout >= 128 else 64
 
 

@@ -108,8 +108,11 @@ def test_invalid_arguments_of_the_conv_entry_points():
     assert L.p3d_dense_conv2d_split(p, 1, 8, 8, 64, p, 64, 64, 3, 3, 1, 1, 1, None, None, 0, p, 96, 64, None, None) == -1
     assert L.p3d_dense_conv2d_packed_weight_bytes(9, 64, 70, 16) == 5 * 9 * 64 * 32 * 4
     assert L.p3d_dense_conv2d_packed_weight_bytes(9, 48, 64, 64) == 0
+    # fp16-pair dense conv: mode 0 (auto) or 1 (per-tap loads) only
+    assert L.p3d_dense_conv2d_f16(p, 1, 8, 8, 64, p, 64, 64, 3, 3, 1, 1, 1, None, None, 0, p, 64, 0, None, 2, 0, None, None) == -1
     # grouped head output conv and the pillar encoder
     assert L.p3d_head_final_conv(p, 1, 8, 8, 128, 64, 3, p, p, p, p, 8, p, None) == -1     # 3 * 64 > 128 channels
+    assert L.p3d_head_out_conv_f16(p, 1, 8, 8, 352, 352, 1, p, p, None, p, p, 3, p, None) == -4  # < 2 activation slots
     assert L.p3d_pillar_feature_net(p, p, p, None, 10, 100, 4, 64, p, p, p, p, p, p, None) == -4  # > 64 points / pillar
     assert L.p3d_pillar_feature_net(p, p, p, None, 10, 32, 4, 64, None, p, p, p, p, p, None) == -1
 

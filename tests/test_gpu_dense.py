@@ -70,6 +70,8 @@ def test_dense_conv_vs_oracle(cuda, oracle_mod, cin, cout, k, stride, pad, up, h
     (64, 64, 2, 2, 0, 2, 9, 11),      # transposed conv k = s = 2
     (512, 64, 3, 1, 1, 1, 12, 18),    # the shared conv's channel count
     (64, 320, 3, 1, 1, 1, 37, 19),    # batched heads: three N tiles, the last one half used; two M tiles over 37 rows
+    (32, 208, 3, 1, 1, 1, 50, 61),    # last N tile partly used, many pixel tiles per N tile
+    (64, 2304, 3, 1, 1, 1, 24, 16),   # the CenterHead's batched ConvModules: 18 N tiles of 128
 ])
 def test_dense_conv_f16_vs_oracle(cuda, oracle_mod, cin, cout, k, stride, pad, up, h, w, mode, m_tiles):
     import torch
@@ -102,37 +104,6 @@ def test_dense_conv_f16_vs_oracle(cuda, oracle_mod, cin, cout, k, stride, pad, u
     rel_check("dense f16 nchw", o_nchw.cpu().numpy(), ref, floor=floor, small_atol=2e-6 if floor == 1e-2 else 1e-5)
 
 
-@pytest.mark.parametrize("cin,cout,h,w", [
-    (64, 320, 37, 19),    # 5 N tiles of 64 on 132 CTAs: every CTA's range is short, many start mid N tile
-    (32, 208, 50, 61),    # last N tile partly used; 52 pixel tiles x 4 N tiles: ranges cross N-tile boundaries (image swap)
-    (64, 2304, 24, 16),   # the CenterHead shape: 36 N tiles
-])
-def test_dense_conv_f16_weight_stationary(cuda, oracle_mod, cin, cout, h, w):
-    """mode 2 = the weight-stationary kernel (N tile's weight image resident in shared memory, contiguous item ranges
-    per CTA) against the oracle and against the streaming kernel (mode 0 with P3D_DENSE_WS unset picks it automatically
-    only for large layers; here it is forced)."""
-    import torch
-    from paddle3d_b200.ops import dense_conv as dc
-    rng = np.random.default_rng(cin * 7 + cout)
-    x = rng.normal(size=(2, cin, h, w)).astype(np.float32)
-    wt = (rng.normal(size=(cout, cin, 3, 3)) / np.sqrt(cin * 9)).astype(np.float32)
-    scale = rng.uniform(0.5, 1.5, cout).astype(np.float32)
-    shift = rng.normal(size=cout).astype(np.float32)
-    ref = oracle_mod.conv2d(x, wt, None, 1, 1).astype(np.float64)
-    ref = np.maximum(ref * scale.reshape(1, -1, 1, 1) + shift.reshape(1, -1, 1, 1), 0.0)
-    packed = dc.pack_conv_weight_f16(_t(cuda, wt), 64)
-    xs = dc.nchw_to_pixel_h16(_t(cuda, x))
-    oc = ((cout + 31) // 32) * 32
-    o_h16, _, (b, oh, ow) = dc.dense_conv2d_f16(xs, (2, h, w, cin), packed, cout, 64, 3, 1, 1, 1, _t(cuda, scale),
-                                               _t(cuda, shift), True, out_channels=oc, mode=2)
-    _, o_nchw, _ = dc.dense_conv2d_f16(xs, (2, h, w, cin), packed, cout, 64, 3, 1, 1, 1, _t(cuda, scale), _t(cuda, shift),
-                                       True, want_nchw=True, mode=2)
-    torch.cuda.synchronize()
-    got = dc.pixel_h16_to_nchw(o_h16, (b, oh, ow, oc)).cpu().numpy()[:, :cout]
-    rel_check("dense f16 ws %d->%d" % (cin, cout), got, ref)
-    rel_check("dense f16 ws nchw", o_nchw.cpu().numpy(), ref)
-
-
 def test_concat_offset_and_small_head(cuda, oracle_mod):
     import torch
     from oracle.cpu_reference import CpuDenseHead
@@ -157,8 +128,8 @@ def test_concat_offset_and_small_head(cuda, oracle_mod):
 
 
 def test_batched_head_matches_per_layer_head(cuda, oracle_mod):
-    """forward (one 64 -> 36*64 conv + one grouped CUDA-core launch for the output convs) against forward_per_head()
-    and the CPU reference, both kernel families."""
+    """forward (one 64 -> 36*64 conv + one launch for the output convs) against forward_per_head() and the CPU
+    reference, both kernel families."""
     import torch
     from oracle.cpu_reference import CpuDenseHead
     from paddle3d_b200.dense_head import DenseRPNHead
@@ -180,27 +151,28 @@ def test_batched_head_matches_per_layer_head(cuda, oracle_mod):
                 assert np.abs(y.cpu().numpy() - x.cpu().numpy()).max() <= tol, name
 
 
-def test_head_out_conv_tap_as_n(cuda, oracle_mod, monkeypatch):
+def test_head_out_conv_tap_as_n(cuda, oracle_mod):
     """p3d_head_out_conv_f16 (9 taps in the GEMM's N dimension, virtual groups for a 4-class heat map, image sides that are
-    not multiples of the 14-pixel tile, batch 2) against the N = 16 grouped kernel and the CPU reference."""
+    not multiples of the 14-pixel tile, batch 2) against the CPU reference, for head widths 64, 96 (an odd number of
+    32-channel groups) and 256 (two-slot activation ring)."""
     import torch
     from oracle.cpu_reference import CpuDenseHead
     from paddle3d_b200.dense_head import DenseRPNHead
-    net = DenseRPNHead(in_channels=64, out_channels=(32, 64), layer_nums=(1, 1), downsample_strides=(1, 2),
-                       fpn_out_channels=(64, 64), upsample_strides=(1, 2), tasks=(1, 4, 2), share_conv_channel=64, f16=True)
-    net.init_weight(seed=11, device=cuda, randomize_bn=True)
-    rng = np.random.default_rng(5)
-    bev = rng.normal(size=(2, 64, 30, 44)).astype(np.float32)
-    new = net.forward(_t(cuda, bev))
-    monkeypatch.setenv("P3D_HEAD_OUT_N16", "1")
-    old = net.forward(_t(cuda, bev))
-    torch.cuda.synchronize()
-    monkeypatch.delenv("P3D_HEAD_OUT_N16")
-    want = CpuDenseHead(net.export_numpy()).run(bev)
-    for name in want:
-        for x, y, w in zip(new[name], old[name], want[name]):
-            assert tuple(x.shape) == w.shape
-            tol = 1e-4 * max(1.0, np.abs(w).max())
-            assert np.abs(x.cpu().numpy() - y.cpu().numpy()).max() <= tol, name
-            assert np.abs(x.cpu().numpy() - w).max() <= tol, name
-            rel_check("head out conv %s" % name, x.cpu().numpy(), w, rtol=2e-4, floor=1e-1, small_atol=1e-4)
+    for share in (64, 96, 256):
+        tasks = (1, 4, 2) if share == 64 else (1, 4)  # the wide heads: few tasks keep the CPU reference fast
+        net = DenseRPNHead(in_channels=64, out_channels=(32, 64), layer_nums=(1, 1), downsample_strides=(1, 2),
+                           fpn_out_channels=(64, 64), upsample_strides=(1, 2), tasks=tasks, share_conv_channel=share,
+                           f16=True)
+        net.init_weight(seed=11, device=cuda, randomize_bn=True)
+        rng = np.random.default_rng(5)
+        bev = rng.normal(size=(2, 64, 30, 44)).astype(np.float32)
+        got = net.forward(_t(cuda, bev))
+        torch.cuda.synchronize()
+        want = CpuDenseHead(net.export_numpy()).run(bev)
+        for name in want:
+            for x, w in zip(got[name], want[name]):
+                assert tuple(x.shape) == w.shape
+                tol = 1e-4 * max(1.0, np.abs(w).max())
+                assert np.abs(x.cpu().numpy() - w).max() <= tol, "%s (share %d)" % (name, share)
+                rel_check("head out conv %s share %d" % (name, share), x.cpu().numpy(), w, rtol=2e-4, floor=1e-1,
+                          small_atol=1e-4)
