@@ -216,7 +216,7 @@ int p3d_sparse_conv_gather_gemm(const float *in, const int32_t *nbr, const int32
                                 p3d_stream_t stream);
 
 /* Tensor-core gather-GEMM with split-K over the kernel taps for the wide layers (Cout >= 64): layers with few
- * 128-row tiles are spread over 2 - 3 CTAs per tile; partial sums go to the caller's scratch slabs and are added in a
+ * 128-row tiles are spread over 2 CTAs per tile; partial sums go to the caller's scratch slabs and are added in a
  * fixed order by a finalize pass that also applies the epilogue (deterministic).  Same contract as
  * p3d_sparse_conv_gather_gemm(precision = P3D_CONV_TF32X3); with workspace == NULL it runs unsplit. */
 size_t p3d_sparse_conv_splitk_workspace_bytes(int64_t n_out_cap, int Cin, int Cout);
@@ -229,12 +229,13 @@ int p3d_sparse_conv_gather_gemm_tf32x3_ws(const float *in, const int32_t *nbr, c
  * Split-row activations for the tensor-core path.  A "split" row tensor stores every row as its tf32 hi half
  * followed by its tf32 lo half: [n][2][C] fp32 words (x ~= hi + lo, error <= 2^-22 |x|).  Keeping activations in
  * this form between sparse-conv layers moves the 3xTF32 split out of the gather loop (paid once per produced
- * element instead of once per gathering neighbour) and lets the kernel gather with cp.async.
+ * element instead of once per gathering neighbour) and lets the kernel gather with cp.async.  Both row layouts run on
+ * the same tensor-core kernel (csrc/sparse_conv_tc.cu) with the same arithmetic.
  *   p3d_rows_convert_layout: src_layout 0 = fp32 rows [n, C] -> split; 1 = split -> fp32 rows (hi + lo).
  *   p3d_sparse_conv_gather_gemm_split: same contract as p3d_sparse_conv_gather_gemm(precision = TF32X3) with
  *     in_split [n_in][2][Cin], residual_split [n_out][2][Cout] or NULL, packed weights
  *     (p3d_sparse_conv_pack_weights), and out_f32 [n_out, Cout] and / or out_split [n_out][2][Cout] (either may be
- *     NULL, not both).  Persistent grid sized to the device row count.
+ *     NULL, not both) and a 16-byte aligned nbr.  Persistent grid sized to the device row count.
  *   p3d_sparse_conv_gather_gemm_split_ws: the same with a scratch buffer of
  *     p3d_sparse_conv_splitk_workspace_bytes(n_out_cap, Cin, Cout) bytes; when present the wide layers run split-K over
  *     taps (partial sums in the scratch slabs, added in slab order by a finalize kernel: deterministic).
@@ -250,14 +251,6 @@ int p3d_sparse_conv_gather_gemm_split_ws(const float *in_split, const int32_t *n
                                          const float *scale, const float *shift, const float *residual_split, int relu,
                                          float *out_f32, float *out_split, void *workspace, size_t workspace_bytes,
                                          p3d_stream_t stream);
-/* EXPERIMENTAL (round-2 groundwork, not on the default path): the same layer with the row gather done by the TMA
- * engine (cp.async.bulk.tensor tile::gather4 through a tensor map over in_split [n_in_rows][2*Cin]) instead of
- * cp.async from 8 producer warps.  Cin >= 32 only (P3D_ERR_UNSUPPORTED otherwise). */
-int p3d_sparse_conv_gather_gemm_split_tma(const float *in_split, int64_t n_in_rows, const int32_t *nbr,
-                                          const int32_t *n_out_dev, int64_t n_out_cap, int K, int Cin, int Cout,
-                                          const float *packed_weight, const float *scale, const float *shift,
-                                          const float *residual_split, int relu, float *out_f32, float *out_split,
-                                          void *workspace, size_t workspace_bytes, p3d_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
  * fp16-pair ("H16") activations: the default tensor-core path of the sparse layers (csrc/sparse_conv_f16.cu).

@@ -57,8 +57,6 @@ SIGNATURES = {
                                                  _vp, _vp]),
     "p3d_sparse_conv_gather_gemm_split_ws": (_int, [_vp, _vp, _vp, _i64, _int, _int, _int, _vp, _vp, _vp, _vp, _int, _vp,
                                                     _vp, _vp, _sz, _vp]),
-    "p3d_sparse_conv_gather_gemm_split_tma": (_int, [_vp, _i64, _vp, _vp, _i64, _int, _int, _int, _vp, _vp, _vp, _vp, _int,
-                                                     _vp, _vp, _vp, _sz, _vp]),
     "p3d_sparse_conv_splitk_workspace_bytes": (_sz, [_i64, _int, _int]),
     "p3d_sparse_conv_small_cin_h16": (_int, [_vp, _vp, _vp, _i64, _int, _int, _int, _vp, _vp, _vp, _int, _vp, _vp, _vp, _vp]),
     "p3d_sparse_rows_to_pixel_h16": (_int, [_vp, _vp, _vp, _int, _int, _int, _int, _int, _int, _vp, _vp]),

@@ -6,7 +6,7 @@
 // significant bits; the power-of-two scale keeps lo' in fp16's normal range) in HALF the bytes: a split row is as large
 // as the plain fp32 row, a 32-channel slice of a row is one 128-byte line holding both halves, fp16 wgmma run at
 // twice the tf32 rate, and the weight image halves too.  Range: |x| < 65504 (flagged in `status` bit 0 otherwise);
-// the tf32 kernels (sparse_conv_tc2.cu) stay available for data outside that range.
+// the tf32-pair kernel (sparse_conv_tc.cu) stays available for data outside that range.
 //
 //   D[0, N)    += A_hi  x B_hi                      (N = Cout)
 //   D[N, 2N)   += A_hi  x B_lo' + A_lo' x B_hi      (both scaled by 2^11)         out = D[0,N) + D[N,2N) * 2^-11

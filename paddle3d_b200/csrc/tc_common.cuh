@@ -12,8 +12,6 @@ namespace tc {
 constexpr int kM = 128;       // rows of a tile: two warpgroups, 64 rows (one wgmma M) each
 constexpr int kThreads = 256;  // the two warpgroups; every thread gathers, issues wgmma and runs the epilogue
 
-__host__ __device__ constexpr int kc_of(int cin) { return cin < 16 ? cin : 16; }  // channels per pipeline stage
-
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -107,17 +105,6 @@ __device__ __forceinline__ void split_tf32(float x, float &hi, float &lo) {
   uint32_t l;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(l) : "f"(r));
   lo = __uint_as_float(l);
-}
-
-
-// split-K factor of the tensor-core sparse conv (taps spread over this many CTAs per 128-row tile)
-inline int splits_for(int Cout) {
-  // tuning hooks (not a public knob): P3D_SPLITS_128 / P3D_SPLITS_64 / P3D_SPLITS_32 override the defaults
-  static const int s128 = getenv("P3D_SPLITS_128") ? atoi(getenv("P3D_SPLITS_128")) : 2;
-  static const int s64 = getenv("P3D_SPLITS_64") ? atoi(getenv("P3D_SPLITS_64")) : 2;
-  static const int s32 = getenv("P3D_SPLITS_32") ? atoi(getenv("P3D_SPLITS_32")) : 1;
-  const int v = Cout >= 128 ? s128 : (Cout >= 64 ? s64 : s32);
-  return v < 1 ? 1 : (v > 8 ? 8 : v);
 }
 
 }  // namespace tc

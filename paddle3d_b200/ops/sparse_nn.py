@@ -26,13 +26,15 @@ from .._mem import ptr, require_cuda, stream, workspace
 from . import pillar_scatter as _ps
 
 # FP32         exact fp32 FMA on CUDA cores
-# TF32X3       wgmma 3xTF32 on plain fp32 rows: the tf32 hi/lo split happens inside the gather loop
-# TF32X3_SPLIT wgmma 3xTF32 on split-layout rows [n][2][C]: whole-line cp.async gathers, persistent tiles, split done
-#              once in the producing layer's epilogue
-# TF32X3_TMA   experimental: TF32X3_SPLIT with the row gather of the Cin >= 32 layers done by per-row TMA boxes
+# TF32X3       wgmma 3xTF32 on plain fp32 rows: the tf32 hi/lo split happens in the gather, once per gathering neighbour
+# TF32X3_SPLIT wgmma 3xTF32 on split-layout rows [n][2][C]: whole-line cp.async gathers, split done once in the
+#              producing layer's epilogue.  TF32X3 and TF32X3_SPLIT run the same kernel (csrc/sparse_conv_tc.cu); use
+#              TF32X3_SPLIT for activations outside fp16's range
 # F16X3        wgmma on fp16 hi/lo' pair rows (csrc/sparse_conv_f16.cu): same 22-bit products as TF32X3_SPLIT in half
 #              the bytes, persistent + overlapped epilogue + device-chosen split-K; |activations| < 65504 (flagged)
-FP32, TF32X3, TF32X3_SPLIT, TF32X3_TMA, F16X3 = 0, 1, 2, 3, 4
+FP32, TF32X3, TF32X3_SPLIT, F16X3 = 0, 1, 2, 4
+TF32X3_TMA = TF32X3_SPLIT  # the name `bench.py --precision tf32x3_tma` selects
+PRECISIONS = (FP32, TF32X3, TF32X3_SPLIT, F16X3)
 ROWS_F32, ROWS_SPLIT, ROWS_H16 = 0, 1, 2  # activation layouts: [n, C] fp32 | [n][2][C] tf32 hi/lo | fp16 hi/lo' pairs
 _default_precision = [FP32]
 F16_MAX_SPLITS = 4
@@ -51,9 +53,15 @@ def status_tensor(device):
     return t
 
 
+def _check_precision(p):
+    if p not in PRECISIONS:
+        raise ValueError("unknown sparse conv precision %r (expected one of %s)" % (p, PRECISIONS))
+    return p
+
+
 def set_precision(p):
-    """FP32 = CUDA-core fp32 FMA; TF32X3 = wgmma tensor cores with 3xTF32 split accumulation."""
-    _default_precision[0] = int(p)
+    """Default precision of the convs that do not set their own: FP32, TF32X3, TF32X3_SPLIT or F16X3."""
+    _default_precision[0] = _check_precision(int(p))
 
 
 def _triple(v):
@@ -277,25 +285,20 @@ def _run(p, t, want):
                                     ptr(p.scale), ptr(p.shift), ptr(res), int(p.relu), ptr(out_f32), ptr(out_h16),
                                     ptr(ws), wsb, F16_MAX_SPLITS, ptr(status_tensor(dev)), stream(dev)), "sparse_conv_f16")
         t._vals[ROWS_F32], t._vals[ROWS_H16] = out_f32, out_h16
-    elif p.precision in (TF32X3_SPLIT, TF32X3_TMA):
+    elif p.precision == TF32X3_SPLIT:
         xin = p.x.get(ROWS_SPLIT)
         res = p.residual.get(ROWS_SPLIT) if p.residual is not None else None
-        out_f32 = torch.empty((p.cap, p.cout), dtype=torch.float32, device=dev) if want == ROWS_F32 else None
+        # fp32 rows unless split rows are asked for: get() converts them to fp16-pair rows
+        out_f32 = torch.empty((p.cap, p.cout), dtype=torch.float32, device=dev) if want != ROWS_SPLIT else None
         out_split = torch.empty((p.cap, 2 * p.cout), dtype=torch.float32, device=dev) if want == ROWS_SPLIT else None
         if PROFILE is not None:
             s_ev.record(st)
         wsb = L.p3d_sparse_conv_splitk_workspace_bytes(p.cap, p.cin, p.cout)  # > 0 for the wide (split-K) layers
         ws = workspace(wsb, dev, "splitk") if wsb else None
-        if p.precision == TF32X3_TMA and p.cin >= 32:
-            check(L.p3d_sparse_conv_gather_gemm_split_tma(ptr(xin), xin.shape[0], ptr(p.nbr), ptr(p.num), p.cap, p.K,
-                                                          p.cin, p.cout, ptr(p.weight), ptr(p.scale), ptr(p.shift),
-                                                          ptr(res), int(p.relu), ptr(out_f32), ptr(out_split), ptr(ws),
-                                                          wsb, stream(dev)), "sparse_conv_gather_gemm_split_tma")
-        else:
-            check(L.p3d_sparse_conv_gather_gemm_split_ws(ptr(xin), ptr(p.nbr), ptr(p.num), p.cap, p.K, p.cin, p.cout,
-                                                         ptr(p.weight), ptr(p.scale), ptr(p.shift), ptr(res),
-                                                         int(p.relu), ptr(out_f32), ptr(out_split), ptr(ws), wsb,
-                                                         stream(dev)), "sparse_conv_gather_gemm_split_ws")
+        check(L.p3d_sparse_conv_gather_gemm_split_ws(ptr(xin), ptr(p.nbr), ptr(p.num), p.cap, p.K, p.cin, p.cout,
+                                                     ptr(p.weight), ptr(p.scale), ptr(p.shift), ptr(res), int(p.relu),
+                                                     ptr(out_f32), ptr(out_split), ptr(ws), wsb, stream(dev)),
+              "sparse_conv_gather_gemm_split_ws")
         t._vals[ROWS_F32], t._vals[ROWS_SPLIT] = out_f32, out_split
     elif (p.precision == FP32 and want == ROWS_H16 and p.residual is None and p.cin <= 8 and p.cout in (16, 32)
           and p.K * p.cin * p.cout * 4 <= 40 * 1024):
@@ -480,7 +483,7 @@ class _ConvBase(_Layer):
         p.weight, p.scale, p.shift, p.residual, p.relu = self.weight, None, self.bias, None, False
         p.ready = None
         p.wm = False
-        p.precision = self.precision if self.precision is not None else _default_precision[0]
+        p.precision = _check_precision(self.precision if self.precision is not None else _default_precision[0])
         if p.precision == F16X3:
             if not lib().p3d_sparse_conv_f16_packed_weight_bytes(K, self.in_channels, self.out_channels):
                 p.precision = FP32  # e.g. the 5-channel input layer stays on the exact fp32 path
@@ -489,7 +492,7 @@ class _ConvBase(_Layer):
                 p.weight = self._packed_weight(K, wm=True)
             else:
                 p.weight = self._packed_weight(K, f16=True)
-        elif p.precision in (TF32X3, TF32X3_SPLIT, TF32X3_TMA):
+        elif p.precision in (TF32X3, TF32X3_SPLIT):
             if not lib().p3d_sparse_conv_packed_weight_bytes(K, self.in_channels, self.out_channels) or K > 32:
                 p.precision = FP32  # e.g. the 5-channel input layer stays on the exact fp32 path
             else:

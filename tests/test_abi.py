@@ -76,7 +76,7 @@ def test_invalid_arguments_return_status_codes():
     assert L.p3d_nms(None, -1, 0.5, 0, None, None, None, 0, None) == -1
 
 
-def test_invalid_arguments_of_the_conv_entry_points():
+def test_conv_entry_points_reject_invalid_arguments():
     """Host-side validation of the sparse / dense conv entry points: every call below must be rejected before any
     CUDA call is made (no GPU here)."""
     import ctypes as C
@@ -88,7 +88,11 @@ def test_invalid_arguments_of_the_conv_entry_points():
     assert L.p3d_sparse_conv_gather_gemm_split_ws(p, p, None, 128, 0, 32, 32, p, None, None, None, 0, p, None, None, 0, None) == -1
     assert L.p3d_sparse_conv_gather_gemm_split_ws(p, p, None, 128, 27, 32, 32, p, None, None, None, 0, None, None, None, 0, None) == -1
     assert L.p3d_sparse_conv_gather_gemm_split_ws(odd, p, None, 128, 27, 32, 32, p, None, None, None, 0, p, None, None, 0, None) == -1
-    assert L.p3d_sparse_conv_gather_gemm_split_tma(p, 128, p, None, 128, 27, 16, 16, p, None, None, None, 0, p, None, None, 0, None) == -4
+    assert L.p3d_sparse_conv_gather_gemm_split_ws(p, p, None, 128, 27, 48, 48, p, None, None, None, 0, p, None, None, 0, None) == -4
+    # sparse fp32-row conv on the same kernel: K out of range, misaligned rows, unsupported channel counts
+    assert L.p3d_sparse_conv_gather_gemm_tf32x3_ws(p, p, None, 128, 0, 32, 32, p, None, None, None, 0, p, None, 0, None) == -1
+    assert L.p3d_sparse_conv_gather_gemm_tf32x3_ws(odd, p, None, 128, 27, 32, 32, p, None, None, None, 0, p, None, 0, None) == -1
+    assert L.p3d_sparse_conv_gather_gemm_tf32x3_ws(p, p, None, 128, 27, 48, 48, p, None, None, None, 0, p, None, 0, None) == -4
     assert L.p3d_sparse_conv_packed_weight_bytes(27, 5, 16) == 0 and L.p3d_sparse_conv_packed_weight_bytes(27, 16, 16) > 0
     assert L.p3d_rows_convert_layout(p, 2, None, 16, 16, p, None) == -1
     # narrow-layer warp-MMA conv: unsupported shape, missing output, misaligned neighbour map, missing / short workspace

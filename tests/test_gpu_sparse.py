@@ -2,8 +2,6 @@
 Tolerance: 1e-4 relative (fp32), BASELINE.json north_star.  PARITY UNPINNED by the reference (the
 arithmetic is PaddlePaddle's); the oracle restatement is itself checked against dense fp64 conv3d in
 tests/test_oracle.py."""
-import os
-
 import numpy as np
 import pytest
 
@@ -12,9 +10,8 @@ from parity import rel_check
 
 pytestmark = pytest.mark.gpu
 
-# 0 fp32 CUDA cores, 1 wgmma on fp32 rows, 2 wgmma on tf32 split rows, 4 wgmma on fp16-pair rows (default);
-# 3 = the slower TMA-gather variant of 2, kept for the record (P3D_EXPERIMENTAL=1)
-PRECISIONS = [0, 1, 2, 4] + ([3] if os.environ.get("P3D_EXPERIMENTAL") == "1" else [])
+# 0 fp32 CUDA cores, 1 wgmma on fp32 rows, 2 wgmma on tf32 split rows, 4 wgmma on fp16-pair rows (default)
+PRECISIONS = [0, 1, 2, 4]
 
 
 def _t(cuda, a):
@@ -72,6 +69,17 @@ def test_single_conv(cuda, oracle_mod, precision, subm, ks, st, pd, cin, cout):
     bev = y.to_dense_bev().cpu().numpy()
     want_bev = np.transpose(want, (0, 4, 1, 2, 3)).reshape(B, cout * osp[0], osp[1], osp[2])
     rel_check('single_conv bev', bev, want_bev)
+    if cout % 16:
+        return
+    # fp16-pair rows (what the pixel image of the dense RPN is built from) asked of a pending conv of this precision
+    from paddle3d_b200._lib import check, lib
+    from paddle3d_b200._mem import ptr, stream
+    h16 = sp.ReLU()(bn(conv(x))).get(sp.ROWS_H16)
+    back = torch.empty((y.index.cap, cout), dtype=torch.float32, device=cuda)
+    check(lib().p3d_rows_convert_h16(ptr(h16), 0, ptr(y.index.num), y.index.cap, cout, ptr(back), None, stream(cuda)),
+          "rows_convert_h16")
+    got16 = _dense(y.index.coords.cpu().numpy()[:n], back.cpu().numpy()[:n], B, y.index.spatial)
+    rel_check('single_conv p%d h16 rows' % precision, got16, want)
 
 
 @pytest.mark.parametrize("wm", [True, False])
@@ -129,6 +137,62 @@ def test_narrow_layers_on_both_kernels(cuda, oracle_mod, wm, subm, ks, st, pd, c
               "rows_convert_h16")
         got16 = _dense(y.index.coords.cpu().numpy()[:n], back.cpu().numpy()[:n], B, y.index.spatial)
         rel_check('narrow h16 rows wm=%d %d->%d' % (wm, cin, cout), got16, want)
+
+
+def test_tf32_abi_wide_layer_without_workspace(cuda, oracle_mod):
+    """p3d_sparse_conv_gather_gemm(precision = P3D_CONV_TF32X3) and p3d_sparse_conv_gather_gemm_split called directly
+    on a wide layer (64 -> 128, K = 27) without a workspace: the unsplit mode of the Cout >= 64 layers, which the Python
+    mirror never runs (it always passes one).  BN scale/shift, a residual and ReLU in each row layout, both outputs of
+    the split-row call; the fp32-row entry point also takes a neighbour map that is not 16-byte aligned."""
+    import torch
+    from paddle3d_b200._lib import check, lib
+    from paddle3d_b200._mem import ptr, stream
+    from paddle3d_b200.ops import sparse_nn as sp
+    L = lib()
+    rng = np.random.default_rng(64128)
+    B, D, H, W, cin, cout, K = 1, 11, 40, 37, 64, 128, 27
+    coords = _rand_sites(rng, B, D, H, W, 0.08)
+    n = len(coords)
+    feats = rng.normal(size=(n, cin)).astype(np.float32)
+    w = (rng.normal(size=(3, 3, 3, cin, cout)) / np.sqrt(K * cin)).astype(np.float32)
+    scale = rng.uniform(0.5, 1.5, cout).astype(np.float32)
+    shift = rng.uniform(-0.2, 0.2, cout).astype(np.float32)
+    res = rng.normal(size=(n, cout)).astype(np.float32)
+    x = sp.sparse_coo_tensor(_t(cuda, coords).t(), _t(cuda, feats), [B, D, H, W, cin])
+    nbr = x.index.subm_rulebook([3, 3, 3], None)
+    tw, ts, tsh, tin, tres = (_t(cuda, a) for a in (w, scale, shift, feats, res))
+    packed = torch.empty((L.p3d_sparse_conv_packed_weight_bytes(K, cin, cout) // 4,), dtype=torch.float32, device=cuda)
+    check(L.p3d_sparse_conv_pack_weights(ptr(tw), K, cin, cout, ptr(packed), stream(cuda)), "sparse_conv_pack_weights")
+
+    def convert(src, layout, C):  # layout 0: fp32 rows -> split rows; 1: split rows -> fp32 rows
+        dst = torch.empty((n, C * (2 if layout == 0 else 1)), dtype=torch.float32, device=cuda)
+        check(L.p3d_rows_convert_layout(ptr(src), layout, None, n, C, ptr(dst), stream(cuda)), "rows_convert_layout")
+        return dst
+
+    out = torch.empty((n, cout), dtype=torch.float32, device=cuda)
+    check(L.p3d_sparse_conv_gather_gemm(ptr(tin), ptr(nbr), None, n, K, cin, cout, ptr(packed), ptr(ts), ptr(tsh),
+                                        ptr(tres), 1, 1, ptr(out), stream(cuda)), "sparse_conv_gather_gemm")
+    nbr_buf = torch.empty((n * K + 1,), dtype=torch.int32, device=cuda)
+    nbr_odd = nbr_buf[1:].view(n, K)
+    nbr_odd.copy_(nbr)
+    assert nbr_odd.data_ptr() % 16 != 0
+    out_odd = torch.empty_like(out)
+    check(L.p3d_sparse_conv_gather_gemm(ptr(tin), ptr(nbr_odd), None, n, K, cin, cout, ptr(packed), ptr(ts), ptr(tsh),
+                                        ptr(tres), 1, 1, ptr(out_odd), stream(cuda)), "sparse_conv_gather_gemm")
+    in_split, res_split = convert(tin, 0, cin), convert(tres, 0, cout)
+    out_f32 = torch.empty((n, cout), dtype=torch.float32, device=cuda)
+    out_split = torch.empty((n, 2 * cout), dtype=torch.float32, device=cuda)
+    check(L.p3d_sparse_conv_gather_gemm_split(ptr(in_split), ptr(nbr), None, n, K, cin, cout, ptr(packed), ptr(ts),
+                                              ptr(tsh), ptr(res_split), 1, ptr(out_f32), ptr(out_split), stream(cuda)),
+          "sparse_conv_gather_gemm_split")
+    merged = convert(out_split, 1, cout)
+    oc, of, osp, _ = oracle_mod.sparse_conv3d(coords, feats, B, (D, H, W), w, 1, 1, True)
+    conv = _dense(oc, of, B, osp)[tuple(coords.T)]  # oracle rows in the order of the input sites
+    want = np.maximum(conv.astype(np.float64) * scale + shift + res, 0.0)
+    assert (want > 0).mean() > 0.3
+    for name, got in (("fp32 rows", out), ("split rows: fp32 output", out_f32), ("split rows: split output", merged)):
+        rel_check("tf32 abi 64->128 unsplit, %s" % name, got.cpu().numpy(), want)
+    assert torch.equal(out_odd, out)
 
 
 def test_strided_overflow_is_flagged(cuda):
