@@ -28,6 +28,7 @@
 #include <cuda.h>
 #include <cuda_fp16.h>
 
+#include "h16.cuh"
 #include "p3d_b200.h"
 #include "tc_common.cuh"
 
@@ -43,7 +44,6 @@ constexpr int kSmemBudget = (227 - 6) * 1024;  // 227 KB per CTA less alignment 
 constexpr int kDenseThreads = 384;      // producer warpgroup + two consumer warpgroups
 constexpr uint32_t kConsumerWarps = 8;  // arrivals that release a slot: one per consumer warp
 constexpr uint32_t kEpiThreads = 96;    // warps 1-3 of the producer warpgroup: the epilogue warps
-constexpr float kLoScale = 2048.0f, kLoInv = 1.0f / 2048.0f;
 
 struct Params {
   int B, H, W, Cin;           // input image (pixel H16 rows [B*H*W][4 * Cin bytes])
@@ -101,30 +101,6 @@ __device__ __forceinline__ void tma_tile4d(uint32_t dst, const CUtensorMap *map,
       "l"(reinterpret_cast<uint64_t>(map)), "r"(c), "r"(x), "r"(y), "r"(b), "r"(bar)
       : "memory");
 }
-__device__ __forceinline__ void split_h16(float x, __half &hi, __half &lo, bool &ovf) {
-  if (fabsf(x) > 65504.0f) {
-    ovf = true;
-    x = copysignf(65504.0f, x);
-  }
-  hi = __float2half_rn(x);
-  lo = __float2half_rn((x - __half2float(hi)) * kLoScale);
-}
-
-// split_h16 of two values with paired conversions (round to nearest either way: the same bits)
-__device__ __forceinline__ void split_h16x2(float a, float b, __half2 &hi, __half2 &lo, bool &ovf) {
-  if (fabsf(a) > 65504.0f) {
-    ovf = true;
-    a = copysignf(65504.0f, a);
-  }
-  if (fabsf(b) > 65504.0f) {
-    ovf = true;
-    b = copysignf(65504.0f, b);
-  }
-  hi = __floats2half2_rn(a, b);
-  const float2 h = __half22float2(hi);
-  lo = __floats2half2_rn((a - h.x) * kLoScale, (b - h.y) * kLoScale);
-}
-
 struct Item {
   int nt, tap0, tx0, ty0, b;
 };
@@ -505,7 +481,7 @@ __global__ void __launch_bounds__(256) pixel_h16_to_nchw_kernel(const __half *__
   const int c = static_cast<int>((q / HW) % C);
   const long long b = q / (HW * C);
   const __half *grp = in + (b * HW + px) * (2 * static_cast<long long>(C)) + (c / 32) * 64;
-  out[q] = fmaf(__half2float(grp[32 + c % 32]), kLoInv, __half2float(grp[c % 32]));
+  out[q] = merge_h16(grp[c % 32], grp[32 + c % 32]);
 }
 
 inline int make_image_map(const void *img, int B, int H, int W, int Cin, int stride, int box_x, int box_y, CUtensorMap *map) {

@@ -20,6 +20,7 @@
 #include <cuda_fp16.h>
 
 #include "common.cuh"
+#include "h16.cuh"
 
 namespace p3d {
 namespace {
@@ -429,17 +430,9 @@ __global__ void __launch_bounds__(128) small_cin_kernel(const float *__restrict_
     uint32_t hw[COUT / 2], lw[COUT / 2];
 #pragma unroll
     for (int c = 0; c < COUT; c += 2) {
-      float x0 = acc[c], x1 = acc[c + 1];
-      if (fabsf(x0) > 65504.f) {
-        ovf = true;
-        x0 = copysignf(65504.f, x0);
-      }
-      if (fabsf(x1) > 65504.f) {
-        ovf = true;
-        x1 = copysignf(65504.f, x1);
-      }
-      const __half h0 = __float2half_rn(x0), h1 = __float2half_rn(x1);
-      const __half l0 = __float2half_rn((x0 - __half2float(h0)) * 2048.0f), l1 = __float2half_rn((x1 - __half2float(h1)) * 2048.0f);
+      __half h0, l0, h1, l1;
+      split_h16(acc[c], h0, l0, ovf);
+      split_h16(acc[c + 1], h1, l1, ovf);
       const __half2 hh = __halves2half2(h0, h1), ll = __halves2half2(l0, l1);
       hw[c / 2] = *reinterpret_cast<const uint32_t *>(&hh);
       lw[c / 2] = *reinterpret_cast<const uint32_t *>(&ll);

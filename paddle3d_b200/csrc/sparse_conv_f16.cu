@@ -1,12 +1,11 @@
 // Sparse-conv gather-GEMM on wgmma, fp16 hi/lo split rows ("H16"), persistent, split-K / stream-K over taps.
 //
 // Why fp16 pairs instead of tf32 pairs: the kernel is bound by bytes moved into shared memory (LDGSTS issue rate for the
-// row gathers, L2->SM bandwidth for the weight slices), not by the tensor pipe.  x = hi + lo' * 2^-11 with
-// hi = fp16(x), lo' = fp16((x - hi) * 2^11) carries the same 22 mantissa bits as the tf32 pair (both formats have 11
-// significant bits; the power-of-two scale keeps lo' in fp16's normal range) in HALF the bytes: a split row is as large
-// as the plain fp32 row, a 32-channel slice of a row is one 128-byte line holding both halves, fp16 wgmma run at
-// twice the tf32 rate, and the weight image halves too.  Range: |x| < 65504 (flagged in `status` bit 0 otherwise);
-// the tf32-pair kernel (sparse_conv_tc.cu) stays available for data outside that range.
+// row gathers, L2->SM bandwidth for the weight slices), not by the tensor pipe.  The fp16 pair x = hi + lo' * 2^-11
+// (h16.cuh) carries the same 22 mantissa bits as the tf32 pair in HALF the bytes: a split row is as large as the plain
+// fp32 row, a 32-channel slice of a row is one 128-byte line holding both halves, fp16 wgmma run at twice the tf32 rate,
+// and the weight image halves too.  Range: |x| < 65504 (flagged in `status` bit 0 otherwise); the tf32-pair kernel
+// (sparse_conv_tc.cu) stays available for data outside that range.
 //
 //   D[0, N)    += A_hi  x B_hi                      (N = Cout)
 //   D[N, 2N)   += A_hi  x B_lo' + A_lo' x B_hi      (both scaled by 2^11)         out = D[0,N) + D[N,2N) * 2^-11
@@ -16,19 +15,21 @@
 // Shared-memory operand "sub-tile": 128 rows x 128 bytes, SWIZZLE_128B K-major (64 fp16 = 4 k-steps of 16):
 //   C >= 32: one (tap, 32-channel group): k-steps 0,1 = hi, 2,3 = lo'  -> one 128-byte line per gathered row
 //   C == 16: two taps: k-steps 0,1 = hi, lo' of tap a; 2,3 = hi, lo' of tap b -> two 64-byte half lines per row
-// A pipeline stage = NSUB sub-tiles + their weight blocks.
+// A pipeline stage = NSUB sub-tiles + their weight blocks (NSUB = 2 for Cin <= 32 and Cout <= 64, else 1).
 //
 // CTA = 1 per SM, two warpgroups (warpgroup g: rows 64g .. 64g+63 of the 128-row tile), persistent over work items (tile
 // of 128 output rows, tap split).  Every thread gathers rows with cp.async (zero-fill for missing neighbours) STAGES - 1
 // stages ahead of the tensor cores, thread 0 copies the weight blocks with cp.async.bulk (mbarrier complete_tx); after
 // the last stage the warpgroups run the epilogue (split-K fix-up, BN / bias / residual / ReLU, fp32 and / or H16 rows)
 // straight from their accumulator fragments.
-// Split-K over taps (few tiles on the deep levels): the split count is chosen ON THE DEVICE from the row count so
-// that the work items fill the grid; partial tiles go to scratch slabs and the LAST arriving CTA of a tile (ticket
-// counter) sums the slabs in index order (deterministic) and runs the fused epilogue - no finalize launch.
+// Split-K / stream-K over taps (few tiles on the deep levels): the decomposition (no split, 2-4 tap splits or stream-K)
+// is chosen ON THE DEVICE from the row count so that the work items fill the grid; partial tiles go to scratch slabs and
+// the LAST arriving CTA of a tile (ticket counter) sums the slabs in index order (deterministic) and runs the fused
+// epilogue - no finalize launch.  Launched with PDL (launch_pdl).
 #include <cuda.h>
 #include <cuda_fp16.h>
 
+#include "h16.cuh"
 #include "tc_common.cuh"
 
 namespace p3d {
@@ -39,13 +40,13 @@ using namespace tc;
 constexpr int kSub = 128 * 128;  // bytes of one A sub-tile
 constexpr int kMaxSplits = 4;
 constexpr int kMaxStages = 12;
-constexpr float kLoScale = 2048.0f, kLoInv = 1.0f / 2048.0f;
+constexpr int kSkFix = 6;  // cost of a stream-K tile's fix-up (slab writes, ticket, slab sums) in taps
 
-template <int CIN, int COUT, int NSUB_>
+template <int CIN, int COUT>
 struct Cfg {
   static constexpr int KC = (CIN >= 32) ? 32 : 16;
   static constexpr int G = CIN / KC;                         // sub-tiles per tap (CIN >= 32); CIN == 16: 2 taps / sub-tile
-  static constexpr int NSUB = NSUB_;                         // sub-tiles per stage
+  static constexpr int NSUB = (CIN <= 32 && COUT <= 64) ? 2 : 1;  // sub-tiles per stage: 4 (Cin 16) / 2 (Cin 32) taps
   static constexpr int B_SUB = 128 * COUT;                   // bytes of the weight blocks of one sub-tile (2 k-blocks)
   static constexpr int B_BLK = 64 * COUT;                    // one 16-channel k-block: [2 chunks][2*COUT rows][16 B]
   static constexpr int STAGE = NSUB * (kSub + B_SUB);
@@ -59,17 +60,6 @@ struct Cfg {
   static_assert(STAGE % 1024 == 0, "SWIZZLE_128B tiles need 1024-byte alignment");
   static_assert(STAGES >= 3, "ring too shallow");
 };
-
-// x -> (hi, lo') fp16 pair; sets ovf when |x| leaves fp16's range (value saturated)
-__device__ __forceinline__ void split_h16(float x, __half &hi, __half &lo, bool &ovf) {
-  if (fabsf(x) > 65504.0f) {
-    ovf = true;
-    x = copysignf(65504.0f, x);
-  }
-  hi = __float2half_rn(x);
-  lo = __float2half_rn((x - __half2float(hi)) * kLoScale);
-}
-__device__ __forceinline__ float merge_h16(__half hi, __half lo) { return fmaf(__half2float(lo), kLoInv, __half2float(hi)); }
 
 // Number of tap splits for `n_tiles` row tiles on `grid` persistent CTAs: minimise waves x (taps per item + fixed cost).
 __host__ __device__ inline int choose_splits(long long n_tiles, int grid, int K, int smax) {
@@ -100,13 +90,14 @@ __device__ __forceinline__ uint32_t split_taps(int split, int splits, int K) {
 // falls inside.  A tile cut by range boundaries has `pieces` partial sums (its CTAs are consecutive: piece = CTA - first
 // CTA), combined through the slabs / ticket like the splits.  No wave quantisation: e.g. 309 tiles on 132 CTAs cost 64 taps
 // per CTA instead of 3 x 27.  Ranges are never shorter than ceil((K - 1) / (kMaxSplits - 1)) units, so pieces <= kMaxSplits.
+// Stream-K needs slabs for kMaxSplits pieces and runs when its cost (taps per CTA + kSkFix) beats the split schedule's.
 struct Sched {
   int stream, splits, K;
   long long n_work;          // stream = 0: n_tiles * splits
   long long total, g_eff;    // stream = 1
   long long u0, u1;          // stream = 1: this CTA's unit range
 };
-__device__ __forceinline__ Sched make_sched(long long n_tiles, int K, int smax, int mode, int fix_taps) {
+__device__ __forceinline__ Sched make_sched(long long n_tiles, int K, int smax) {
   Sched sc;
   sc.K = K;
   sc.stream = 0;
@@ -116,15 +107,15 @@ __device__ __forceinline__ Sched make_sched(long long n_tiles, int K, int smax, 
   sc.total = n_tiles * K;
   sc.g_eff = 1;
   sc.u0 = sc.u1 = 0;
-  if (mode && smax >= 4 && sc.total > 0) {  // slabs for 4 pieces available
+  if (smax >= 4 && sc.total > 0) {  // slabs for 4 pieces available
     const int u_min = (K - 1 + 2) / 3 > 1 ? (K - 1 + 2) / 3 : 1;  // ceil((K - 1) / (kMaxSplits - 1)), kMaxSplits = 4
     long long g = sc.total / u_min;
     if (g > grid) g = grid;
     if (g < 1) g = 1;
     const long long waves = (sc.n_work + grid - 1) / grid;
     const long long cost_old = waves * ((K + sc.splits - 1) / sc.splits + 4 + (sc.splits > 1 ? 1 : 0));
-    const long long cost_stream = (sc.total + g - 1) / g + 4 + fix_taps;
-    if (mode == 2 || cost_stream < cost_old) {
+    const long long cost_stream = (sc.total + g - 1) / g + 4 + kSkFix;
+    if (cost_stream < cost_old) {
       sc.stream = 1;
       sc.g_eff = g;
       const long long c = blockIdx.x;
@@ -175,27 +166,23 @@ struct Params {
   float *slabs;             // split-K scratch [smax][tiles][128 rows][COUT] fp32 (smax > 1)
   int32_t *counters;        // split-K tickets [tiles], zero on entry, left zero
   int32_t *status;          // optional: bit 0 = fp16 range overflow while producing out_h16
-  const uint8_t *zero_row;  // 512 zero bytes in global memory (target of missing neighbours with flag 2)
-  int sk_mode, sk_fix;      // stream-K: 0 off, 1 when the cost model prefers it, 2 always; cost of a fix-up in taps
-  int flags;                // tuning / debug: 1 all neighbours missing, 2 missing neighbours read zero_row instead of a
-                            // zero-size copy, 4 all neighbours present (pseudo-random rows); 1 and 4 give wrong results
 };
 __device__ __forceinline__ int nth_bit(uint32_t m, int k) {  // position of the k-th (0-based) set bit of m
   for (int i = 0; i < k; ++i) m &= m - 1u;
   return __ffs(m) - 1;
 }
 
-template <int CIN, int COUT, int NSUB>
+template <int CIN, int COUT>
 __global__ void __launch_bounds__(kThreads, 1) conv_f16_kernel(const Params p) {
-  using C = Cfg<CIN, COUT, NSUB>;
-  constexpr int S = C::STAGES;
+  using C = Cfg<CIN, COUT>;
+  constexpr int S = C::STAGES, NSUB = C::NSUB;
   constexpr int H = COUT / 2;  // accumulator registers of the hi products; the cross products follow
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  asm volatile("griddepcontrol.wait;" ::: "memory");  // the input rows are the previous layer's output
+  pdl_trigger();
+  pdl_wait();  // the input rows are the previous layer's output
   const long long n = p.n_out_dev ? min(static_cast<long long>(p.n_out_dev[0]), p.n_cap) : p.n_cap;
   const long long n_tiles = (n + kM - 1) / kM;
   const int K = p.K;
-  const Sched sc = make_sched(n_tiles, K, p.smax, p.sk_mode, p.sk_fix);
+  const Sched sc = make_sched(n_tiles, K, p.smax);
   if (sc.stream ? (sc.u0 >= sc.u1) : (static_cast<long long>(blockIdx.x) >= sc.n_work)) return;
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -219,7 +206,6 @@ __global__ void __launch_bounds__(kThreads, 1) conv_f16_kernel(const Params p) {
   __syncthreads();
   const uint32_t ring = smem_u32(smem);
   const int sub4 = tid >> 3, ch = tid & 7;  // gather: 32 rows x 8 16-byte chunks per CTA instruction
-  const int flags = p.flags;
   constexpr int KCO = (COUT >= 32) ? 32 : 16;  // channels per H16 group of the output / residual rows
   const size_t tiles_cap = static_cast<size_t>((p.n_cap + kM - 1) / kM);
   bool ovf = false;
@@ -252,14 +238,6 @@ __global__ void __launch_bounds__(kThreads, 1) conv_f16_kernel(const Params p) {
       __syncthreads();
       mbar_wait(smem_u32(&s_bar[kNR]), static_cast<uint32_t>(it & 1));
     }
-    auto fetch = [&](int row, int t) -> int {
-      int idx = row < rows ? s_nbr[row * K + t] : -1;
-      if (flags & 5) {
-        if (flags & 1) idx = -1;
-        if ((flags & 4) && row < rows) idx = static_cast<int>(hash32(static_cast<uint32_t>(tile * kM + row) * 27u + t) % static_cast<uint32_t>(n));
-      }
-      return idx;
-    };
     // stage q of this item: sub-tiles q * NSUB .. (rows gathered by every thread, weight blocks by thread 0)
     auto issue = [&](int q) {
       if (q >= n_st) return;
@@ -288,13 +266,9 @@ __global__ void __launch_bounds__(kThreads, 1) conv_f16_kernel(const Params p) {
 #pragma unroll
             for (int q4 = 0; q4 < 4; ++q4) {
               const int row = q4 * 32 + sub4;
-              const int idx = fetch(row, t);
-              bool ok = idx >= 0;
-              const uint8_t *src = p.in + (ok ? static_cast<size_t>(idx) * 64 : 0) + (ch & 3) * 16;
-              if ((flags & 2) && !ok) {
-                src = p.zero_row + (ch & 3) * 16;
-                ok = true;
-              }
+              const int idx = row < rows ? s_nbr[row * K + t] : -1;
+              const bool ok = idx >= 0;
+              const uint8_t *src = p.in + static_cast<size_t>(max(idx, 0)) * 64 + (ch & 3) * 16;
               cp_async16(sb + static_cast<uint32_t>(row * 128 + ((ch ^ (row & 7)) << 4)), src, ok);
             }
           }
@@ -304,13 +278,9 @@ __global__ void __launch_bounds__(kThreads, 1) conv_f16_kernel(const Params p) {
 #pragma unroll
           for (int q4 = 0; q4 < 4; ++q4) {
             const int row = q4 * 32 + sub4;
-            const int idx = fetch(row, t);
-            bool ok = idx >= 0;
-            const uint8_t *src = p.in + (ok ? static_cast<size_t>(idx) * (4 * CIN) : 0) + g * 128 + ch * 16;
-            if ((flags & 2) && !ok) {
-              src = p.zero_row + ch * 16;
-              ok = true;
-            }
+            const int idx = row < rows ? s_nbr[row * K + t] : -1;
+            const bool ok = idx >= 0;
+            const uint8_t *src = p.in + static_cast<size_t>(max(idx, 0)) * (4 * CIN) + g * 128 + ch * 16;
             cp_async16(sb + static_cast<uint32_t>(row * 128 + ((ch ^ (row & 7)) << 4)), src, ok);
           }
         }
@@ -439,30 +409,17 @@ __global__ void __launch_bounds__(kThreads, 1) conv_f16_kernel(const Params p) {
   if (ovf && p.status) atomicOr(p.status, 1);
 }
 
-__device__ __align__(128) uint4 g_zero_row[32];  // 512 zero bytes: gather target of missing neighbours (flag 2)
-
-template <int CIN, int COUT, int NSUB>
+template <int CIN, int COUT>
 int launch(const Params &p, cudaStream_t st) {
-  using C = Cfg<CIN, COUT, NSUB>;
+  using C = Cfg<CIN, COUT>;
   const size_t smem = static_cast<size_t>(C::STAGES) * C::STAGE + static_cast<size_t>(kM) * p.K * sizeof(int32_t) + 1024;
   if (smem > 227 * 1024) return P3D_ERR_UNSUPPORTED;
-  auto kern = conv_f16_kernel<CIN, COUT, NSUB>;
+  auto kern = conv_f16_kernel<CIN, COUT>;
   P3D_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   const long long work = ((p.n_cap + kM - 1) / kM) * (p.smax > 1 ? p.smax : 1);
   const long long sms = num_sms();
   const unsigned int grid = static_cast<unsigned int>(work < sms ? work : sms);
-  static const bool pdl = !(getenv("P3D_PDL") && atoi(getenv("P3D_PDL")) == 0);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl ? 1 : 0;
-  P3D_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, p));
+  P3D_CUDA_CHECK(launch_pdl(kern, dim3(grid), dim3(kThreads), smem, st, p));
   P3D_LAUNCH_CHECK();
   return P3D_OK;
 }
@@ -481,9 +438,7 @@ __global__ void __launch_bounds__(256) pack_weights_kernel(const float *__restri
   __half hi, lo;
   bool ovf = false;
   split_h16(w[q], hi, lo, ovf);
-  const size_t base = kb * (32 * static_cast<size_t>(Cout)) * 1 + 0;  // halfs per k-block = 64 * Cout / 2
-  const size_t blk = kb * static_cast<size_t>(32 * Cout);
-  (void)base;
+  const size_t blk = kb * static_cast<size_t>(32 * Cout);  // halfs per k-block = 64 * Cout / 2
   packed[blk + (static_cast<size_t>(c) * (2 * Cout) + n) * 8 + j] = hi;
   packed[blk + (static_cast<size_t>(c) * (2 * Cout) + Cout + n) * 8 + j] = lo;
   if (ovf && status) atomicOr(status, 1);
@@ -601,13 +556,6 @@ extern "C" int p3d_sparse_conv_f16(const void *in_h16, const int32_t *nbr, const
   p.out_f32 = out_f32;
   p.out_h16 = static_cast<uint8_t *>(out_h16);
   p.status = status_dev;
-  static const int dflags = getenv("P3D_F16_FLAGS") ? atoi(getenv("P3D_F16_FLAGS")) : 0;  // tuning / debug, see Params::flags
-  p.flags = dflags;
-  {
-    void *z = nullptr;
-    P3D_CUDA_CHECK(cudaGetSymbolAddress(&z, f16::g_zero_row));
-    p.zero_row = static_cast<const uint8_t *>(z);
-  }
   // split-K is available up to the number of slabs the workspace holds
   int smax = max_splits;
   if (smax > f16::kMaxSplits) smax = f16::kMaxSplits;
@@ -621,31 +569,15 @@ extern "C" int p3d_sparse_conv_f16(const void *in_h16, const int32_t *nbr, const
     if (static_cast<size_t>(smax) > fit) smax = static_cast<int>(fit);
   }
   p.smax = smax < 1 ? 1 : smax;
-  // stream-K (contiguous (tile, tap) ranges per CTA instead of whole tiles) when the device-side cost model prefers it:
-  // P3D_F16_STREAMK = 0 off / 1 auto (default) / 2 always; P3D_F16_SKFIX = cost of a tile's fix-up in taps (default 6)
-  static const int sk_env = getenv("P3D_F16_STREAMK") ? atoi(getenv("P3D_F16_STREAMK")) : 1;
-  static const int skfix_env = getenv("P3D_F16_SKFIX") ? atoi(getenv("P3D_F16_SKFIX")) : 6;
-  p.sk_mode = sk_env;
-  p.sk_fix = skfix_env;
   p.counters = p.smax > 1 ? static_cast<int32_t *>(workspace) : nullptr;
   p.slabs = p.smax > 1 ? reinterpret_cast<float *>(static_cast<char *>(workspace) + tick) : nullptr;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // tuning hook: sub-tiles per pipeline stage (P3D_F16_NSUB = 1 / 2; default: 2 for Cin <= 32 - 4 resp. 2 taps per
-  // stage -, 1 above; Cout = 128 always 1)
-  static const int nsub_env = getenv("P3D_F16_NSUB") ? atoi(getenv("P3D_F16_NSUB")) : 0;
-  const int nsub = nsub_env ? nsub_env : (Cin <= 32 ? 2 : 1);
-#define P3D_F16_CASE(CI, CO)                                                \
-  if (Cin == CI && Cout == CO) {                                            \
-    if (nsub == 2 && CO <= 64) return f16::launch<CI, CO, (CO <= 64 ? 2 : 1)>(p, st); \
-    return f16::launch<CI, CO, 1>(p, st);                                   \
-  }
-  P3D_F16_CASE(16, 16)
-  P3D_F16_CASE(16, 32)
-  P3D_F16_CASE(32, 32)
-  P3D_F16_CASE(32, 64)
-  P3D_F16_CASE(64, 64)
-  P3D_F16_CASE(64, 128)
-  P3D_F16_CASE(128, 128)
-#undef P3D_F16_CASE
+  if (Cin == 16 && Cout == 16) return f16::launch<16, 16>(p, st);
+  if (Cin == 16 && Cout == 32) return f16::launch<16, 32>(p, st);
+  if (Cin == 32 && Cout == 32) return f16::launch<32, 32>(p, st);
+  if (Cin == 32 && Cout == 64) return f16::launch<32, 64>(p, st);
+  if (Cin == 64 && Cout == 64) return f16::launch<64, 64>(p, st);
+  if (Cin == 64 && Cout == 128) return f16::launch<64, 128>(p, st);
+  if (Cin == 128 && Cout == 128) return f16::launch<128, 128>(p, st);
   return P3D_ERR_UNSUPPORTED;
 }

@@ -26,14 +26,13 @@
 // The tensor pipe is irrelevant at these widths (N = 16/32): the bounds are the L2 gather (pairs x 4 Cin bytes), the
 // issue slots of the gather loop and, for 32 -> 32, the mma.sync rate.
 #include <cuda_fp16.h>
-#include <stdlib.h>
 
 #include "common.cuh"
+#include "h16.cuh"
 
 namespace p3d {
 namespace wm {
 
-constexpr float kLoScale = 2048.0f, kLoInv = 1.0f / 2048.0f;
 constexpr int kWarps = 16;  // warps per CTA of every instantiation, one CTA per SM
 
 struct Params {
@@ -58,16 +57,6 @@ __device__ __forceinline__ void mma16816(float (&c)[4], const uint4 &a, uint32_t
       : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
       : "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w), "r"(b0), "r"(b1));
 }
-
-__device__ __forceinline__ void split_h16(float x, __half &hi, __half &lo, bool &ovf) {
-  if (fabsf(x) > 65504.0f) {
-    ovf = true;
-    x = copysignf(65504.0f, x);
-  }
-  hi = __float2half_rn(x);
-  lo = __float2half_rn((x - __half2float(hi)) * kLoScale);
-}
-__device__ __forceinline__ float merge_h16(__half hi, __half lo) { return fmaf(__half2float(lo), kLoInv, __half2float(hi)); }
 
 // B-fragment words of one (tile, tap) unit for the two rows (g, g + 8) a lane serves: [row][half: hi, lo'][CIN / 8 words];
 // words 2s, 2s + 1 are (b0, b1) of k-step s
@@ -133,8 +122,9 @@ struct Group {
   bool valid, last;  // last group of this warp's tap range of the tile
 };
 
-template <int CIN, int COUT, int D>
+template <int CIN, int COUT>
 __global__ void __launch_bounds__(kWarps * 32, 1) conv_wm_kernel(const Params p) {
+  constexpr int D = (CIN == 16) ? 5 : 3;  // register-ring depth in taps; Cin = 32 spills at D = 4
   constexpr int KS = CIN / 16, MT = COUT / 16;
   constexpr int KCO = (COUT >= 32) ? 32 : 16;
   constexpr int SO = COUT + 4;          // row stride (floats) of the per-warp output tile: conflict-free both ways
@@ -421,13 +411,13 @@ __global__ void __launch_bounds__(256) pack_weights_wm_kernel(const float *__res
   if (ovf && status) atomicOr(status, 1);
 }
 
-template <int CIN, int COUT, int D>
+template <int CIN, int COUT>
 int launch(const Params &p, cudaStream_t st) {
   constexpr int KS = CIN / 16, MT = COUT / 16;
   const size_t smem = static_cast<size_t>(p.K) * KS * MT * 1024 + static_cast<size_t>(kWarps) * 2 * 16 * p.K * sizeof(int32_t) +
                       static_cast<size_t>(kWarps) * 16 * (COUT + 4) * sizeof(float);
   if (smem > 227 * 1024) return P3D_ERR_UNSUPPORTED;
-  auto kern = conv_wm_kernel<CIN, COUT, D>;
+  auto kern = conv_wm_kernel<CIN, COUT>;
   P3D_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   const long long blocks_needed = (p.n_cap + 16 * kWarps - 1) / (16 * kWarps);
   long long grid = num_sms();
@@ -502,20 +492,8 @@ extern "C" int p3d_sparse_conv_wm(const void *in_h16, const int32_t *nbr, const 
   p.tickets = static_cast<int32_t *>(workspace);
   p.slabs = reinterpret_cast<float *>(static_cast<char *>(workspace) + align_up(static_cast<size_t>((n_out_cap + 15) / 16) * sizeof(int32_t)));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  static const int d_env = getenv("P3D_WM_D") ? atoi(getenv("P3D_WM_D")) : 0;  // tuning hook: ring depth
-  if (Cin == 16 && Cout == 16) {
-    if (d_env == 3) return wm::launch<16, 16, 3>(p, st);
-    if (d_env == 9) return wm::launch<16, 16, 9>(p, st);
-    return wm::launch<16, 16, 5>(p, st);
-  }
-  if (Cin == 16 && Cout == 32) {
-    if (d_env == 3) return wm::launch<16, 32, 3>(p, st);
-    if (d_env == 9) return wm::launch<16, 32, 7>(p, st);
-    return wm::launch<16, 32, 5>(p, st);
-  }
-  if (Cin == 32 && Cout == 32) {  // D = 4 spills 8 bytes
-    if (d_env == 4) return wm::launch<32, 32, 4>(p, st);
-    return wm::launch<32, 32, 3>(p, st);
-  }
+  if (Cin == 16 && Cout == 16) return wm::launch<16, 16>(p, st);
+  if (Cin == 16 && Cout == 32) return wm::launch<16, 32>(p, st);
+  if (Cin == 32 && Cout == 32) return wm::launch<32, 32>(p, st);
   return P3D_ERR_UNSUPPORTED;
 }

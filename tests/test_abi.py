@@ -103,6 +103,14 @@ def test_conv_entry_points_reject_invalid_arguments():
     assert wm(p, p, None, 128, 27, 16, 16, p, None, None, None, 0, p, None, None, 0, None, None) == -2
     assert wm(p, p, None, 128, 27, 16, 16, p, None, None, None, 0, p, None, p, 16, None, None) == -2
     assert wm(p, p, None, 0, 27, 16, 16, p, None, None, None, 0, p, None, None, 0, None, None) == 0  # empty input: nothing to do
+    # fp16-pair wgmma conv: K out of range, missing output, misaligned rows, unsupported channel counts
+    f16 = L.p3d_sparse_conv_f16
+    assert f16(p, p, None, 128, 0, 32, 32, p, None, None, None, 0, p, None, None, 0, 4, None, None) == -1
+    assert f16(p, p, None, 128, 33, 32, 32, p, None, None, None, 0, p, None, None, 0, 4, None, None) == -1
+    assert f16(p, p, None, 128, 27, 32, 32, p, None, None, None, 0, None, None, None, 0, 4, None, None) == -1
+    assert f16(odd, p, None, 128, 27, 32, 32, p, None, None, None, 0, p, None, None, 0, 4, None, None) == -1
+    assert f16(p, p, None, 128, 27, 48, 48, p, None, None, None, 0, p, None, None, 0, 4, None, None) == -4
+    assert f16(p, p, None, 128, 27, 32, 48, p, None, None, None, 0, p, None, None, 0, 4, None, None) == -4
     # dense conv: channel counts, N tile, transposed-conv geometry, split-row output columns
     ok = dict(B=1, H=8, W=8)
     assert L.p3d_dense_conv2d_split(p, 1, 8, 8, 48, p, 64, 64, 3, 3, 1, 1, 1, None, None, 0, p, 64, 0, None, None) == -4

@@ -17,21 +17,15 @@ wrote (the slab region is NaN-filled before the launch) must be exactly the one 
 drift apart the test fails instead of quietly covering another path.  Lines starting with "REGIME" (pytest -s) list
 the decompositions each instantiation reached on the device."""
 import math
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 
 from parity import rel_check
 
-TESTS = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(TESTS)
-
 KM = 128              # rows per tile of the wgmma kernel (tc::kM)
 F16_MAX_SPLITS = 4    # f16::kMaxSplits
-SK_FIX = 6            # default cost of a stream-K fix-up in taps (P3D_F16_SKFIX)
+SK_FIX = 6            # cost of a stream-K fix-up in taps (f16::kSkFix)
 ALIGN = 256           # workspace region alignment (kAlign)
 WM_TILE, WM_WARPS = 16, 16
 LO = 2.0 ** -11       # weight of lo' in an fp16 pair
@@ -166,18 +160,18 @@ class Sched:
         return "no split" if self.splits == 1 else "%d splits" % self.splits
 
 
-def f16_sched(sms, n, n_cap, K, cout, max_splits, ws_bytes, mode=1, fix=SK_FIX):
+def f16_sched(sms, n, n_cap, K, cout, max_splits, ws_bytes):
     """f16::launch's grid and f16::make_sched / sched_item for device row count n (clamped to n_cap)."""
     smax = f16_smax(K, n_cap, cout, max_splits, ws_bytes)
     grid = min(_cdiv(n_cap, KM) * (smax if smax > 1 else 1), sms)
     n_tiles = _cdiv(min(n, n_cap), KM)
     splits = choose_splits(n_tiles, grid, K, smax)
     total = n_tiles * K
-    if mode and smax >= 4 and total > 0:
+    if smax >= 4 and total > 0:
         u_min = max((K + 1) // 3, 1)  # ceil((K - 1) / (kMaxSplits - 1))
         g = max(min(total // u_min, grid), 1)
         cost_old = _cdiv(n_tiles * splits, grid) * (_cdiv(K, splits) + 4 + (1 if splits > 1 else 0))
-        if mode == 2 or _cdiv(total, g) + 4 + fix < cost_old:
+        if _cdiv(total, g) + 4 + SK_FIX < cost_old:
             start = np.arange(n_tiles, dtype=np.int64) * K
             cf, cl = ((start + 1) * g - 1) // total, ((start + K) * g - 1) // total
             return Sched(True, 0, smax, grid, n_tiles, cl - cf + 1)
@@ -195,11 +189,11 @@ def f16_expected_blocks(sc, n_slabs, tiles_cap):
     return exp
 
 
-def f16_search(sms, K, n_cap, cout, max_splits, ws_bytes, mode=1):
+def f16_search(sms, K, n_cap, cout, max_splits, ws_bytes):
     """First tile count (<= the capacity's) of every decomposition the restatement can reach."""
     found = {}
     for t in range(1, _cdiv(n_cap, KM) + 1):
-        found.setdefault(f16_sched(sms, t * KM, n_cap, K, cout, max_splits, ws_bytes, mode).key, t)
+        found.setdefault(f16_sched(sms, t * KM, n_cap, K, cout, max_splits, ws_bytes).key, t)
     return found
 
 
@@ -309,7 +303,7 @@ def _verify(name, d, n, f32, h16, scale, shift, residual, relu, flagged=False):
 
 
 # ---------------------------------------------------------------------------------------------- wgmma kernel case
-def run_f16(d, label, n_dev, n_cap, max_splits=4, ws_kind="full", mode=1, residual=True, relu=True, affine=True,
+def run_f16(d, label, n_dev, n_cap, max_splits=4, ws_kind="full", residual=True, relu=True, affine=True,
             scale=None, expect=None):
     """One p3d_sparse_conv_f16 launch (fp32 and fp16-pair outputs at once) checked against the reference, the schedule
     restatement (slab fingerprint), the ticket words and a second launch on the same workspace."""
@@ -332,7 +326,7 @@ def run_f16(d, label, n_dev, n_cap, max_splits=4, ws_kind="full", mode=1, residu
         ws[:tick].zero_()  # tickets: zero on entry
         slabs = ws[tick:tick + n_slabs * slab].view(torch.float32).view(n_slabs, tiles_cap, KM * cout)
         slabs.fill_(float("nan"))
-    sc = f16_sched(sms, n_dev, n_cap, K, cout, max_splits, ws_bytes, mode)
+    sc = f16_sched(sms, n_dev, n_cap, K, cout, max_splits, ws_bytes)
     if expect is not None:
         assert sc.key == expect, "%s: restatement picks %s, the case was searched for %s" % (label, sc.key, expect)
     n = min(n_dev, n_cap)
@@ -488,39 +482,6 @@ def test_f16_every_schedule(cuda, cin, cout, K):
         n = rows(t_busy)
         dk = Data(cuda, cin, cout, K, F16_CAP, n, seed=cin + cout + K + 7, kind=kind)
         run_f16(dk, kind + " map", n, F16_CAP)
-        torch.cuda.empty_cache()
-
-
-@pytest.mark.gpu
-def test_f16_tiles_cut_into_four_pieces(cuda):
-    """Forced stream-K (P3D_F16_STREAMK=2, read once per process: a child interpreter) on every K = 27 instantiation at
-    a row count where the restatement cuts some tiles into four pieces - a combine the automatic cost model never picks."""
-    code = "import sys; sys.path[:0] = [%r, %r]; import test_gpu_sparse_schedule as m; m.four_piece_child()" % (ROOT, TESTS)
-    env = dict(os.environ, P3D_F16_STREAMK="2")
-    env.pop("P3D_F16_FLAGS", None)
-    args = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + ["-c", code]
-    r = subprocess.run(args, env=env, cwd=ROOT, capture_output=True, text=True, timeout=200)
-    sys.stdout.write(r.stdout)
-    assert r.returncode == 0, "forced stream-K child failed:\n%s\n%s" % (r.stdout[-4000:], r.stderr[-4000:])
-    assert r.stdout.count("four-piece ok") == sum(1 for s in F16_SHAPES if s[2] == 27)
-
-
-def four_piece_child():
-    import torch
-    from paddle3d_b200._lib import lib
-    dev = torch.device("cuda:0")
-    sms = _sms()
-    for cin, cout, K in F16_SHAPES:
-        if K != 27:
-            continue
-        ws_full = lib().p3d_sparse_conv_f16_workspace_bytes(F16_CAP, cout, F16_MAX_SPLITS)
-        found = f16_search(sms, K, F16_CAP, cout, F16_MAX_SPLITS, ws_full, mode=2)
-        assert "stream4" in found, found
-        n = found["stream4"] * KM - 37
-        d = Data(dev, cin, cout, K, F16_CAP, n, seed=cin * 7 + cout)
-        sc, _, _ = run_f16(d, "forced stream-K", n, F16_CAP, mode=2, expect="stream4")
-        print("four-piece ok %d->%d n=%d: %d of %d tiles in 4 pieces" % (cin, cout, n, int((sc.pieces == 4).sum()), sc.n_tiles))
-        del d
         torch.cuda.empty_cache()
 
 
