@@ -401,6 +401,34 @@ int p3d_anchor_head_postprocess(const float *head, int feat_h, int feat_w, int a
                                 int32_t *counts, uint8_t *anchor_mask, float *sorted_boxes, float *sorted_scores,
                                 void *workspace, size_t workspace_bytes, p3d_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * merge_sweeps      the multi-sweep input of the nuScenes 10-sweep CenterPoint model on the device: what
+ *                   LoadPointCloud.__call__ (paddle3d/transforms/reader.py:116-167) does on the host.
+ *   raw       [num_slots, slot_cap, raw_dim] fp32 raw file rows (16-byte aligned, slot_cap % 4 == 0)
+ *   desc      [num_entries] device frame descriptor, read by the kernel (one captured graph serves every frame):
+ *             entry 0 is the key sweep, then the earlier sweeps in merge order; an entry of 0 rows is empty.
+ *   use_dim_host[n_use_dim]  columns kept (n_use_dim == 0: all raw_dim columns); use_time_lag appends fp32(time_lag).
+ *   out       [cap, F] fp32, F = (n_use_dim ? n_use_dim : raw_dim) + use_time_lag, fully written: key rows, then the kept
+ *             rows of every sweep in input order (the reference's concatenation order), NaN rows from *n_out_dev on.
+ *   The key sweep keeps every row, lag 0, no transform.  A sweep drops a row when |c0| < r and |c1| < r (fp32, on the
+ *   selected columns 0 and 1); with has_transform its columns 0..2 become fp32(M[0..2] . (c0, c1, c2, 1)) computed in
+ *   fp64.  *n_out_dev = min(rows, cap); *status_dev: bit 0 = rows beyond cap were dropped, bit 1 = an entry with a slot
+ *   outside [0, num_slots) or rows outside [0, slot_cap] (read as empty).  (raw_dim + F) <= 12.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct p3d_sweep_desc {
+  int32_t slot;             /* slot of `raw` holding this sweep */
+  int32_t rows;             /* raw rows in that slot */
+  int32_t has_transform;    /* 0: the rows are already in the key frame */
+  float time_lag;           /* seconds, the lag column's value */
+  double ref_from_curr[12]; /* top three rows of the 4x4 transform into the key frame, row-major */
+} p3d_sweep_desc;
+
+size_t p3d_merge_sweeps_workspace_bytes(int num_entries, int64_t slot_cap);
+int p3d_merge_sweeps(const float *raw, int num_slots, int64_t slot_cap, int raw_dim, const p3d_sweep_desc *desc,
+                     int num_entries, const int32_t *use_dim_host, int n_use_dim, int use_time_lag,
+                     float sweep_remove_radius, float *out, int64_t cap, int32_t *n_out_dev, int32_t *status_dev,
+                     void *workspace, size_t workspace_bytes, p3d_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

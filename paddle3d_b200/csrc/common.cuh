@@ -76,6 +76,40 @@ inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, siz
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
 
+// Decoupled look-back across the tiles of a single-pass scan, 32 predecessors per round.  Called by all 32 lanes of one
+// warp of tile `bid` (tiles numbered in scan order, e.g. by an atomic ticket) with that tile's aggregate; returns the sum
+// of the aggregates of tiles [0, bid) in every lane and publishes the tile's inclusive prefix.  desc[b] =
+// (status << 32 | value): status 0 = not posted yet, 1 = tile aggregate, 2 = inclusive prefix; zero before the launch.
+__device__ __forceinline__ int lookback_exclusive_prefix(unsigned long long *desc, unsigned int bid, int aggregate) {
+  const int lane = threadIdx.x & 31;
+  int prefix = 0;
+  volatile unsigned long long *vd = desc;
+  if (bid == 0) {
+    if (lane == 0) vd[0] = (2ull << 32) | static_cast<uint32_t>(aggregate);
+    return 0;
+  }
+  if (lane == 0) vd[bid] = (1ull << 32) | static_cast<uint32_t>(aggregate);
+  int j = static_cast<int>(bid) - 1;  // lane l inspects tile j - l
+  while (true) {
+    const int b = j - lane;
+    const unsigned long long d = b >= 0 ? vd[b] : (2ull << 32);  // before tile 0: inclusive prefix 0
+    const uint32_t st = static_cast<uint32_t>(d >> 32);
+    const unsigned incl = __ballot_sync(0xffffffffu, st == 2);
+    const unsigned ready = __ballot_sync(0xffffffffu, st != 0);
+    const int last = incl ? __ffs(incl) - 1 : 31;                     // nearest inclusive prefix (or all 32)
+    const unsigned need = last == 31 ? 0xffffffffu : ((2u << last) - 1u);
+    if ((ready & need) != need) continue;                             // a needed predecessor has not posted yet
+    int val = lane <= last ? static_cast<int>(static_cast<uint32_t>(d)) : 0;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) val += __shfl_xor_sync(0xffffffffu, val, o);
+    prefix += val;
+    if (incl) break;
+    j -= 32;
+  }
+  if (lane == 0) vd[bid] = (2ull << 32) | static_cast<uint32_t>(prefix + aggregate);
+  return prefix;
+}
+
 __device__ __forceinline__ uint32_t hash32(uint32_t k) {
   k *= 0x9E3779B1u;  // Fibonacci hashing; callers take the top bits
   return k;

@@ -214,32 +214,7 @@ __global__ void __launch_bounds__(kScanBlock) vox_rank_kernel(const unsigned lon
     }
     if (lane < kScanBlock / 32) s_warp[lane] = winc - v;  // exclusive warp offsets
     const int aggregate = __shfl_sync(0xffffffffu, winc, 31);
-    // decoupled look-back, 32 predecessors per round (status 1 = block aggregate, 2 = inclusive prefix)
-    int prefix = 0;
-    volatile unsigned long long *vd = desc + 1;
-    if (bid == 0) {
-      if (lane == 0) vd[0] = (2ull << 32) | static_cast<uint32_t>(aggregate);
-    } else {
-      if (lane == 0) vd[bid] = (1ull << 32) | static_cast<uint32_t>(aggregate);
-      int j = static_cast<int>(bid) - 1;  // lane l inspects block j - l
-      while (true) {
-        const int b = j - lane;
-        const unsigned long long d = b >= 0 ? vd[b] : (2ull << 32);  // before block 0: inclusive prefix 0
-        const uint32_t st = static_cast<uint32_t>(d >> 32);
-        const unsigned incl = __ballot_sync(0xffffffffu, st == 2);
-        const unsigned ready = __ballot_sync(0xffffffffu, st != 0);
-        const int last = incl ? __ffs(incl) - 1 : 31;                     // nearest inclusive prefix (or all 32)
-        const unsigned need = last == 31 ? 0xffffffffu : ((2u << last) - 1u);
-        if ((ready & need) != need) continue;                             // a needed predecessor has not posted yet
-        int val = lane <= last ? static_cast<int>(static_cast<uint32_t>(d)) : 0;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) val += __shfl_xor_sync(0xffffffffu, val, o);
-        prefix += val;
-        if (incl) break;
-        j -= 32;
-      }
-      if (lane == 0) vd[bid] = (2ull << 32) | static_cast<uint32_t>(prefix + aggregate);
-    }
+    const int prefix = lookback_exclusive_prefix(desc + 1, bid, aggregate);
     if (lane == 0) {
       s_prefix = prefix;
       if (bid == gridDim.x - 1) {

@@ -61,7 +61,9 @@ def write_results(path, box3d_lidar, label_preds, scores):
 class Predictor:
     """`init_predictor` + `run` of the reference's deploy script over this repository's CUDA pipeline."""
 
-    def __init__(self, cfg=None, device="cuda:0", max_points=None, seed=0, precision=None, with_head=True, weights=None):
+    def __init__(self, cfg=None, device="cuda:0", max_points=None, seed=0, precision=None, with_head=True, weights=None,
+                 sweep_input=None):
+        """sweep_input: see CenterPointHotPath; the predictor then takes raw sweeps (run_sweeps) instead of points."""
         import torch
         from . import synth
         from .ops import sparse_nn as sp
@@ -69,7 +71,7 @@ class Predictor:
         self.torch = torch
         self.cfg = dict(cfg or synth.C3)
         self.pipe = CenterPointHotPath(self.cfg, device, precision=sp.F16X3 if precision is None else precision, seed=seed,
-                                       num_points=max_points, with_head=with_head)
+                                       num_points=max_points, with_head=with_head, sweep_input=sweep_input)
         self.host = torch.empty((self.pipe.n, self.pipe.F), dtype=torch.float32).pin_memory()
         self.captured = False
 
@@ -89,4 +91,14 @@ class Predictor:
             self.pipe.capture()
             self.captured = True
         boxes, scores, labels = self.pipe.infer(self.host)
+        return boxes.numpy().copy(), labels.numpy().copy(), scores.numpy().copy()
+
+    def run_sweeps(self, key, sweeps):
+        """Raw key sweep [n, raw_dim] + earlier sweeps [(cloud, ref_from_curr | None, time_lag)] -> (box3d_lidar,
+        label_preds, scores): the frame merges them on the GPU (LoadPointCloud, reader.py:116-167)."""
+        if not self.captured:
+            self.pipe.infer_sweeps(key, sweeps)  # eager first frame: loads the ring and descriptor the capture reads
+            self.pipe.capture()
+            self.captured = True
+        boxes, scores, labels = self.pipe.infer_sweeps(key, sweeps)
         return boxes.numpy().copy(), labels.numpy().copy(), scores.numpy().copy()

@@ -82,8 +82,12 @@ class CapturedFrame:
     # ---- public end-to-end call: host points in, host boxes out
     def infer(self, points_host):
         """points_host: pinned [n, F] fp32 tensor.  Returns (boxes [K, 9 or 7], scores [K], labels [K]) on the host."""
+        return self._infer(lambda: self.points.copy_(points_host, non_blocking=True))
+
+    def _infer(self, upload):
+        """One frame in latency mode: upload() enqueues the H2D copies of the inputs on the pipeline stream."""
         with torch.cuda.stream(self.stream):
-            self.points.copy_(points_host, non_blocking=True)
+            upload()
             if self.graph is not None:
                 self.graph.replay()
             else:
@@ -169,9 +173,44 @@ class CapturedFrame:
         return h2d, d2h
 
 
+def _stream_frames(lanes, ring, items):
+    """One frame per pushed sweep (cloud, global_from_lidar, timestamp) over the captured lanes sharing `ring`: frame j
+    runs on lane j % len(lanes), result slot (j // len(lanes)) & 1 (CenterPointSweep.plan); the H2D of sweep j + 1 runs
+    on the ring's copy stream while frame j computes.  Yields (boxes, scores, labels) per sweep, in order."""
+    import collections
+    L = len(lanes)
+    for p in lanes:
+        if p.graph is None or p.ring is not ring:
+            raise RuntimeError("infer_stream needs captured lanes with sweep input sharing one ring")
+        p.prepare_sweep()
+    ring.reset()
+    pending = collections.deque()
+    for i, (cloud, pose, t) in enumerate(items):
+        li, k = CenterPointSweep._lane_slot(i, L)
+        lane = lanes[li]
+        lane._submit_sweep(ring.push(cloud, pose, t), k)
+        pending.append((lane, k))
+        if len(pending) > L:
+            pl, pk = pending.popleft()
+            yield pl._result(pk)
+    while pending:
+        pl, pk = pending.popleft()
+        yield pl._result(pk)
+
+
+# sweep_input of CenterPointHotPath: ten nuScenes sweeps of 5 values per point, of which x, y, z, intensity are kept
+# and the time lag appended (the 5 columns deploy.preprocess gives the model), close points of earlier sweeps removed
+# within 1 m; slot_cap None = 2 x the mean rows per sweep of num_points
+SWEEP_INPUT = dict(max_sweeps=10, raw_dim=5, use_dim=4, use_time_lag=True, remove_radius=1.0, slot_cap=None)
+
+
 class CenterPointHotPath(CapturedFrame):
     def __init__(self, cfg=None, device="cuda:0", precision=sp.FP32, seed=0, num_points=None, level_caps=None,
-                 head_seed=0, with_head=False, keep_bev=True, bn_gain=1.0):
+                 head_seed=0, with_head=False, keep_bev=True, bn_gain=1.0, sweep_input=None, sweep_ring=None):
+        """sweep_input: None (the frame reads merged clouds from self.points) or a dict over SWEEP_INPUT's keys: the
+        frame then starts with the device merge (ops.sweep_merge) of raw sweeps held in a SweepRing into self.points
+        (num_points rows, NaN beyond the merged ones); see infer_sweeps / infer_stream.  sweep_ring: a ring shared
+        with other lanes (CenterPointSweep); default: an own ring of max_sweeps + 1 slots."""
         self.cfg = dict(cfg or synth.C3)
         self.device = torch.device(device)
         self.n = int(num_points or self.cfg["num_points"])
@@ -199,11 +238,98 @@ class CenterPointHotPath(CapturedFrame):
         self.graph = None
         self.out = None
         self.stream = torch.cuda.Stream(self.device)
-        self._alloc_host_outputs(len(self.label_off) * self.test_cfg["nms_post_max_size"], 9, len(self.label_off) + 1, 5)
+        self.sweep_input = self.ring = None
+        if sweep_input is not None:
+            self._init_sweep_input(dict(SWEEP_INPUT, **sweep_input), sweep_ring)
+        self._alloc_host_outputs(len(self.label_off) * self.test_cfg["nms_post_max_size"], 9, len(self.label_off) + 1,
+                                 5 if self.sweep_input is None else 6)
+
+    def _init_sweep_input(self, si, ring):
+        from . import sweep_ring
+        from .ops import sweep_merge as sm
+        si["use_dim"] = sm.columns(si["use_dim"], si["raw_dim"])
+        if len(si["use_dim"]) + bool(si["use_time_lag"]) != self.F:
+            raise ValueError("sweep_input gives %d columns per point, the model reads %d"
+                             % (len(si["use_dim"]) + bool(si["use_time_lag"]), self.F))
+        K = int(si["max_sweeps"])
+        if si["slot_cap"] is None:
+            si["slot_cap"] = -(-2 * self.n // K // 4) * 4
+        if ring is None:
+            ring = sweep_ring.SweepRing(K, si["raw_dim"], si["slot_cap"], K + 1, self.device)
+        if (ring.max_sweeps, ring.raw_dim, ring.slot_cap) != (K, si["raw_dim"], si["slot_cap"]):
+            raise ValueError("the sweep ring does not match sweep_input")
+        self.sweep_input, self.ring = si, ring
+        nb = K * sm.DESC_DTYPE.itemsize
+        self._sweep_desc = torch.zeros((nb,), dtype=torch.uint8, device=self.device)  # read by the captured merge
+        self._desc_host = [torch.zeros((nb,), dtype=torch.uint8).pin_memory() for _ in range(3)]
+        self._n_merged = torch.zeros((1,), dtype=torch.int32, device=self.device)
+        self._merge_status = torch.zeros((1,), dtype=torch.int32, device=self.device)
+
+    def _desc_view(self, k):
+        from .ops import sweep_merge as sm
+        return self._desc_host[k].numpy().view(sm.DESC_DTYPE)
+
+    def infer_sweeps(self, key, sweeps=()):
+        """One frame from raw arrays, latency mode: key [n, raw_dim] fp32, sweeps [(cloud, ref_from_curr | None,
+        time_lag)] in merge order, at most max_sweeps - 1 (io.merge_sweeps' arguments).  Returns what infer() returns
+        for the merged cloud.  Starts a new stream of the ring."""
+        si, ring = self.sweep_input, self.ring
+        if si is None:
+            raise RuntimeError("infer_sweeps needs a pipeline built with sweep_input")
+        if len(sweeps) + 1 > si["max_sweeps"]:
+            raise ValueError("%d sweeps exceed max_sweeps = %d" % (len(sweeps) + 1, si["max_sweeps"]))
+        from .ops import sweep_merge as sm
+        desc = self._desc_view(2)
+        self.stream.synchronize()  # the previous frame no longer reads the descriptor staging
+        desc[:] = np.zeros(1, sm.DESC_DTYPE)
+        ring.reset()
+        for e, (cloud, m, lag) in enumerate([(key, None, 0.0)] + list(sweeps)):
+            ring.load(e, cloud, self.stream)
+            sm.set_entry(desc[e], e, len(cloud), m, lag)
+
+        def upload():
+            self._sweep_desc.copy_(self._desc_host[2], non_blocking=True)
+        out = self._infer(upload)
+        ev = torch.cuda.Event()
+        ev.record(self.stream)
+        ring.mark_read(range(len(sweeps) + 1), ev)
+        return out
+
+    def infer_stream(self, items):
+        """items: iterable of (cloud [n, raw_dim] fp32, global_from_lidar 4x4, timestamp [s]), one per sensor sweep.
+        Yields one (boxes, scores, labels) per pushed sweep, in order: the frame keyed by that sweep with the
+        max_sweeps - 1 previous ones of the stream.  The H2D of the next sweep overlaps the current frame (as infer_many)."""
+        if self.graph is None:
+            raise RuntimeError("infer_stream needs a captured pipeline: call capture() first")
+        return _stream_frames([self], self.ring, items)
+
+    def _submit_sweep(self, j, k):
+        """Enqueue the frame keyed by ring sweep j into result slot k: descriptor H2D, graph replay, D2H of the results."""
+        read, pushed = self.ring.describe(j, self._desc_view(k))
+        st = self.stream
+        with torch.cuda.stream(st):
+            st.wait_event(pushed)
+            self._sweep_desc.copy_(self._desc_host[k], non_blocking=True)
+            self.graph.replay()
+            o, sl = self.out, self._slots[k]
+            for name in ("counts", "status", "boxes", "scores", "labels"):
+                sl[name].copy_(o[name], non_blocking=True)
+            self._done[k].record(st)
+        self.ring.mark_read(read, self._done[k])
+
+    def merged_rows(self):
+        """Rows of the last merged cloud (device scalar read back; sweep input only)."""
+        self.stream.synchronize()
+        return int(self._n_merged.item())
 
     # ---- one frame, enqueued on the current stream, device in / device out
     def forward_device(self):
         cfg, tc = self.cfg, self.test_cfg
+        si = self.sweep_input
+        if si is not None:
+            from .ops import sweep_merge as sm
+            sm.merge_into(self.ring.buf, self._sweep_desc, si["max_sweeps"], si["use_dim"], si["use_time_lag"],
+                          si["remove_radius"], self.points, self._n_merged, self._merge_status)
         mean, coors, npv, nv = vox.voxelize_mean(self.points, cfg["voxel_size"], cfg["point_cloud_range"],
                                                  cfg["max_points"], cfg["max_voxels"], 0)
         bev, bev_h16 = None, None
@@ -213,8 +339,10 @@ class CenterPointHotPath(CapturedFrame):
         else:
             bev_h16 = self.net(mean, coors, 1, num=nv, pixel_h16=True)
             h = self.dense.forward_h16(*bev_h16)
-        # frame status word (ADVICE r1): [fp16-range overflow of the pair-row kernels, overflow flag of each strided level]
-        status = torch.stack([sp.status_tensor(self.device)[0]] + [c[1] for c in self.net.level_counters])
+        # frame status word (ADVICE r1): [fp16-range overflow of the pair-row kernels, overflow flag of each strided level,
+        # with sweep input: the merge's status bits]
+        status = torch.stack([sp.status_tensor(self.device)[0]] + [c[1] for c in self.net.level_counters] +
+                             ([self._merge_status[0]] if si is not None else []))
         boxes, scores, labels, counts = cpp.centerpoint_postprocess_device(
             h["hm"], h["reg"], h["height"], h["dim"], h["vel"], h["rot"], cfg["voxel_size"][:2],
             cfg["point_cloud_range"], tc["post_center_limit_range"], self.label_off, tc["down_ratio"],
@@ -255,14 +383,20 @@ class CenterPointHotPath(CapturedFrame):
         self.stream.synchronize()
         return self
 
-    @staticmethod
-    def check_status(status_host):
+    def check_status(self, status_host):
         """Raise when the frame's device status word reports dropped work (never a silent wrong result)."""
         st = [int(v) for v in status_host]
+        n_levels = len(self.net.level_counters)
+        if len(st) > 1 + n_levels and st[1 + n_levels]:
+            from .ops import sweep_merge as sm
+            if st[1 + n_levels] & sm.BAD_ENTRY:
+                raise RuntimeError("sweep merge: a frame descriptor entry named a slot or row count outside the ring")
+            raise RuntimeError("sweep merge: the merged sweeps exceed the point capacity (num_points = %d); rows were "
+                               "dropped" % self.n)
         if st[0]:
             raise RuntimeError("sparse backbone: an activation left fp16's range (|x| >= 65504) on the fp16-pair path; "
                                "run this model with precision TF32X3_SPLIT")
-        for lvl, v in enumerate(st[1:]):
+        for lvl, v in enumerate(st[1:1 + n_levels]):
             if v:
                 raise RuntimeError("sparse backbone: strided level %d overflowed its row capacity (set_level_caps); "
                                    "output sites were dropped" % (lvl + 1))
@@ -306,6 +440,12 @@ class CenterPointSweep:
             raise ValueError("lanes >= 1")
         frame_cls = frame_cls or CenterPointHotPath
         first = frame_cls(**kw)
+        if kw.get("sweep_input") is not None and kw.get("sweep_ring") is None:
+            # one ring for all lanes, K + lanes slots: a slot is reused only after its last reader's result was read
+            from .sweep_ring import SweepRing
+            si = first.sweep_input
+            first.ring = SweepRing(si["max_sweeps"], si["raw_dim"], si["slot_cap"], si["max_sweeps"] + lanes, first.device)
+            kw = dict(kw, sweep_ring=first.ring)
         self.lanes = [first]
         for _ in range(lanes - 1):
             p = frame_cls(**kw)
@@ -362,6 +502,11 @@ class CenterPointSweep:
                 yield ("result",) + pending.popleft()
         while pending:
             yield ("result",) + pending.popleft()
+
+    def infer_stream(self, items):
+        """As CenterPointHotPath.infer_stream (one result per pushed sweep, in order), with the lanes sharing one sweep
+        ring and len(self) frames computing concurrently."""
+        return _stream_frames(self.lanes, self.lanes[0].ring, items)
 
     def infer_many(self, frames_host):
         """As CenterPointHotPath.infer_many (pinned host frames in, host results out, in order), with len(self) frames

@@ -94,6 +94,27 @@ def lidar_cloud(cfg, seed, num_points=None, sweeps=10, beams=32):
     return pts[:n].astype(np.float32)
 
 
+def sweep_sequence(n_sweeps, seed, points_per_sweep=29500, speed=10.0, yaw_rate=0.3, period=0.05):
+    """A raw multi-sweep LiDAR stream: [(cloud [n_i, 5] fp32 (x, y, z, intensity, ring) in the sensor frame,
+    global_from_lidar [4, 4] float64, timestamp [s])], one sweep every `period` (20 Hz) from an ego vehicle driving at
+    `speed` m/s while turning at `yaw_rate` rad/s.  Each sweep is one ring sweep of lidar_cloud (its scene drawn per
+    sweep); n_i = points_per_sweep +- 500, so ten merged sweeps stay within C3's 300k points."""
+    rng = np.random.default_rng(seed)
+    out = []
+    for s in range(n_sweeps):
+        n = int(points_per_sweep + rng.integers(-500, 501))
+        pts = lidar_cloud(dict(C3, point_dim=4), seed * 1000 + s, num_points=n, sweeps=1)
+        elev = np.degrees(np.arctan2(pts[:, 2], np.hypot(pts[:, 0], pts[:, 1])))
+        ring = np.clip(np.rint((elev + 30.67) / (41.34 / 31)), 0, 31).astype(np.float32)
+        t = 1000.0 + s * period
+        yaw = yaw_rate * s * period
+        x, y = speed * s * period * np.cos(yaw / 2), speed * s * period * np.sin(yaw / 2)
+        pose = np.array([[np.cos(yaw), -np.sin(yaw), 0.0, x], [np.sin(yaw), np.cos(yaw), 0.0, y], [0.0, 0.0, 1.0, 1.84],
+                         [0.0, 0.0, 0.0, 1.0]])
+        out.append((np.concatenate([pts, ring[:, None]], 1).astype(np.float32), pose, t))
+    return out
+
+
 def random_boxes(n, seed, extent=40.0, clustered=True):
     """[x,y,z,dx,dy,dz,heading] boxes; clustered centres so that rotated overlaps are common."""
     rng = np.random.default_rng(seed)
