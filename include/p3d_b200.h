@@ -166,23 +166,19 @@ int p3d_sparse_rulebook_conv(const int32_t *coords, const int32_t *n_in_dev, int
                              int32_t *nbr, void *workspace, size_t workspace_bytes, p3d_stream_t stream);
 
 /* Caller-owned coordinate tables (one per index set / resolution level): the same rulebooks with every level's
- * table built exactly once per frame.  p3d_sparse_table_build hashes an index set's coordinates;
- * p3d_sparse_rulebook_subm_t only looks neighbours up in it; p3d_sparse_rulebook_conv_t looks the inputs up in
- * table_in and leaves in table_out the table of the OUTPUT index set (a by-product of enumerating its sites), ready
- * for the next stage.  Tables are p3d_sparse_table_bytes(rows_cap) bytes, 16-byte aligned. */
+ * table built exactly once per frame (the two calls above run this path on tables carved out of their workspace).
+ * p3d_sparse_table_build hashes an index set's coordinates; p3d_sparse_rulebook_subm_t only looks neighbours up in it.
+ * Tables are p3d_sparse_table_bytes(rows_cap) bytes, 16-byte aligned. */
 size_t p3d_sparse_table_bytes(int64_t rows_cap);
 int p3d_sparse_table_build(const int32_t *coords, const int32_t *n_dev, int64_t n_cap, int batch,
                            const int *spatial_host, void *table, size_t table_bytes, p3d_stream_t stream);
 int p3d_sparse_rulebook_subm_t(const int32_t *coords, const int32_t *n_dev, int64_t n_cap, int batch,
                                const int *spatial_host, const int *ksize_host, const void *table, size_t table_bytes,
                                int32_t *nbr, p3d_stream_t stream);
-int p3d_sparse_rulebook_conv_t(const int32_t *coords, const int32_t *n_in_dev, int64_t n_in_cap, int batch,
-                               const int *spatial_host, const int *ksize_host, const int *stride_host,
-                               const int *pad_host, const void *table_in, size_t table_in_bytes, int32_t *out_coords,
-                               int32_t *n_out_dev, int64_t out_cap, void *table_out, size_t table_out_bytes,
-                               int32_t *nbr, p3d_stream_t stream);
 
-/* One resolution level in two launches: p3d_sparse_rulebook_conv_t plus, when nbr_subm is given, the SubM neighbour map
+/* One resolution level in two launches: the strided conv of p3d_sparse_rulebook_conv (out_coords, n_out_dev, nbr) with
+ * the inputs looked up in table_in; table_out is left holding the table of the OUTPUT index set (a by-product of
+ * enumerating its sites), ready for the next stage.  When nbr_subm is given, also the SubM neighbour map
  * [out_cap, prod(subm_ksize)] of the NEW level (odd kernel, "same" padding) looked up in table_out - what a following
  * p3d_sparse_rulebook_subm_t on the output index set would return. */
 int p3d_sparse_rulebook_level_t(const int32_t *coords, const int32_t *n_in_dev, int64_t n_in_cap, int batch,

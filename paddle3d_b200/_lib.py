@@ -45,8 +45,6 @@ SIGNATURES = {
     "p3d_sparse_table_bytes": (_sz, [_i64]),
     "p3d_sparse_table_build": (_int, [_vp, _vp, _i64, _int, _vp, _vp, _sz, _vp]),
     "p3d_sparse_rulebook_subm_t": (_int, [_vp, _vp, _i64, _int, _vp, _vp, _vp, _sz, _vp, _vp]),
-    "p3d_sparse_rulebook_conv_t": (_int, [_vp, _vp, _i64, _int, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _i64, _vp, _sz,
-                                          _vp, _vp]),
     "p3d_sparse_rulebook_level_t": (_int, [_vp, _vp, _i64, _int, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _i64, _vp, _sz,
                                            _vp, _vp, _vp, _vp]),
     "p3d_sparse_affine_act": (_int, [_vp, _vp, _i64, _int, _vp, _vp, _vp, _int, _vp, _vp]),

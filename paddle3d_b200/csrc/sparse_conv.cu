@@ -35,28 +35,6 @@ struct Dims {
   int oD, oH, oW;          // output spatial
 };
 
-struct RbWs {
-  unsigned long long *tab_in;   // [cap_in]
-  unsigned long long *tab_out;  // [cap_out]
-  uint32_t cap_in, shift_in, cap_out, shift_out;
-  size_t bytes;
-};
-
-RbWs carve_rb(void *p, int64_t n_in_cap, int64_t n_out_cap) {
-  RbWs w;
-  Carver c(p);
-  w.cap_in = next_pow2(static_cast<uint64_t>(n_in_cap > 512 ? n_in_cap : 512) * 2);
-  w.cap_out = next_pow2(static_cast<uint64_t>(n_out_cap > 512 ? n_out_cap : 512) * 2);
-  w.shift_in = 32;
-  for (uint32_t x = w.cap_in; x > 1; x >>= 1) --w.shift_in;
-  w.shift_out = 32;
-  for (uint32_t x = w.cap_out; x > 1; x >>= 1) --w.shift_out;
-  w.tab_in = c.take<unsigned long long>(w.cap_in);
-  w.tab_out = c.take<unsigned long long>(w.cap_out);
-  w.bytes = c.off;
-  return w;
-}
-
 __device__ __forceinline__ uint32_t lin(int b, int z, int y, int x, int D, int H, int W) {
   return ((static_cast<uint32_t>(b) * D + z) * H + y) * W + x;
 }
@@ -101,22 +79,22 @@ __global__ void __launch_bounds__(256) rb_insert_kernel(const int32_t *__restric
   }
 }
 
-// nbr[o][k] = row of the input at  o*stride - pad + k   (SubM: stride 1, pad k/2, o == i)
-__global__ void __launch_bounds__(256) rb_neighbors_kernel(const int32_t *__restrict__ out_coords,
+// SubM map: nbr[i][k] = row of the input at  coord(i) - pad + k   (pad k/2; the centre tap is row i itself)
+__global__ void __launch_bounds__(256) rb_neighbors_kernel(const int32_t *__restrict__ coords,
                                                            const int32_t *__restrict__ n_dev, long long n_cap, Dims d,
                                                            const unsigned long long *__restrict__ tab, uint32_t mask,
-                                                           uint32_t shift, int subm, int32_t *__restrict__ nbr) {
+                                                           uint32_t shift, int32_t *__restrict__ nbr) {
   const int K = d.kd * d.kh * d.kw;
   const long long n = n_dev ? min(static_cast<long long>(n_dev[0]), n_cap) : n_cap;
   const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
   // persistent grid-stride loop: the grid is sized for the SMs, not for the (much larger) capacity
   for (long long q = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; q < n * K; q += stride) {
     const int o = static_cast<int>(q / K), k = static_cast<int>(q - static_cast<long long>(o) * K);
-    const int4 c = *reinterpret_cast<const int4 *>(out_coords + static_cast<size_t>(o) * 4);
+    const int4 c = *reinterpret_cast<const int4 *>(coords + static_cast<size_t>(o) * 4);
     const int kz = k / (d.kh * d.kw), ky = (k / d.kw) % d.kh, kx = k % d.kw;
-    const int iz = c.y * d.sd - d.pd + kz, iy = c.z * d.sh - d.ph + ky, ix = c.w * d.sw - d.pw + kx;
+    const int iz = c.y - d.pd + kz, iy = c.z - d.ph + ky, ix = c.w - d.pw + kx;
     int r = -1;
-    if (subm && kz == d.kd / 2 && ky == d.kh / 2 && kx == d.kw / 2) {
+    if (kz == d.kd / 2 && ky == d.kh / 2 && kx == d.kw / 2) {
       r = o;
     } else if (iz >= 0 && iz < d.D && iy >= 0 && iy < d.H && ix >= 0 && ix < d.W) {
       r = lookup(tab, mask, shift, lin(c.x, iz, iy, ix, d.D, d.H, d.W));
@@ -196,10 +174,10 @@ __global__ void __launch_bounds__(256) rb_outputs_kernel(const int32_t *__restri
   }
 }
 
-// One launch per resolution level after rb_outputs: publishes the clamped output count / overflow flag (what
-// rb_finish_kernel did) and fills BOTH neighbour maps of the new index set: the strided conv's (rows of the input level,
-// through tab_in) and, when nbr_m is given, the 3-D SubM map of the level's residual blocks (rows of the output level,
-// through tab_out, which rb_outputs completed).  Query q < n * Ks: strided; else SubM.
+// One launch per resolution level after rb_outputs: publishes the clamped output count / overflow flag and fills BOTH
+// neighbour maps of the new index set: the strided conv's (rows of the input level, through tab_in) and, when nbr_m is
+// given, the 3-D SubM map of the level's residual blocks (rows of the output level, through tab_out, which rb_outputs
+// completed).  Query q < n * Ks: strided; else SubM.
 __global__ void __launch_bounds__(256) rb_level_neighbors_kernel(const int32_t *__restrict__ out_coords,
                                                                  int32_t *__restrict__ n_out_dev, long long out_cap, Dims ds,
                                                                  const unsigned long long *__restrict__ tab_in,
@@ -241,12 +219,6 @@ __global__ void __launch_bounds__(256) rb_level_neighbors_kernel(const int32_t *
       nbr_m[qm] = r;
     }
   }
-}
-
-__global__ void rb_finish_kernel(int32_t *n_out_dev, int out_cap) {
-  const int raw = n_out_dev[2];
-  n_out_dev[0] = raw < out_cap ? raw : out_cap;
-  n_out_dev[1] = (raw > out_cap || n_out_dev[3]) ? 1 : 0;
 }
 
 // ------------------------------------------------------------------ fp32 gather-GEMM
@@ -495,73 +467,6 @@ int make_dims(int batch, const int *sp, const int *ks, const int *st, const int 
 
 using namespace p3d;
 
-extern "C" size_t p3d_sparse_rulebook_workspace_bytes(int64_t n_in_cap, int64_t n_out_cap) {
-  if (n_in_cap < 0 || n_out_cap < 0 || n_in_cap > kMaxRows || n_out_cap > kMaxRows) return 0;
-  return carve_rb(nullptr, n_in_cap, n_out_cap).bytes;
-}
-
-extern "C" int p3d_sparse_rulebook_subm(const int32_t *coords, const int32_t *n_in_dev, int64_t n_in_cap, int batch,
-                                        const int *spatial_host, const int *ksize_host, int32_t *nbr,
-                                        void *workspace, size_t workspace_bytes, p3d_stream_t stream) {
-  Dims d;
-  int rc = make_dims(batch, spatial_host, ksize_host, nullptr, nullptr, 1, &d);
-  if (rc) return rc;
-  if (n_in_cap < 0 || n_in_cap > 0x7fffffff / 128 || !workspace || (n_in_cap && (!coords || !nbr)))
-    return P3D_ERR_INVALID_ARG;
-  if (reinterpret_cast<uintptr_t>(coords) & 15) return P3D_ERR_INVALID_ARG;
-  if (n_in_cap == 0) return P3D_OK;
-  RbWs w = carve_rb(workspace, n_in_cap, 0);
-  if (workspace_bytes < w.bytes) return P3D_ERR_WORKSPACE;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int K = d.kd * d.kh * d.kw;
-  P3D_CUDA_CHECK(cudaMemsetAsync(w.tab_in, 0xff, sizeof(unsigned long long) * w.cap_in, st));
-  rb_insert_kernel<<<div_up(n_in_cap, 256), 256, 0, st>>>(coords, n_in_dev, static_cast<int>(n_in_cap), d, w.tab_in,
-                                                         w.cap_in - 1, w.shift_in);
-  P3D_LAUNCH_CHECK();
-  rb_neighbors_kernel<<<persistent_grid(n_in_cap * K), 256, 0, st>>>(coords, n_in_dev, n_in_cap, d, w.tab_in,
-                                                                 w.cap_in - 1, w.shift_in, 1, nbr);
-  P3D_LAUNCH_CHECK();
-  return P3D_OK;
-}
-
-extern "C" int p3d_sparse_rulebook_conv(const int32_t *coords, const int32_t *n_in_dev, int64_t n_in_cap, int batch,
-                                        const int *spatial_host, const int *ksize_host, const int *stride_host,
-                                        const int *pad_host, int32_t *out_coords, int32_t *n_out_dev,
-                                        int64_t out_cap, int32_t *nbr, void *workspace, size_t workspace_bytes,
-                                        p3d_stream_t stream) {
-  Dims d;
-  int rc = make_dims(batch, spatial_host, ksize_host, stride_host, pad_host, 0, &d);
-  if (rc) return rc;
-  if (n_in_cap < 0 || out_cap < 1 || n_in_cap > 0x7fffffff / 128 || out_cap > 0x7fffffff / 128 || !workspace ||
-      !n_out_dev || !out_coords || !nbr || (n_in_cap && !coords))
-    return P3D_ERR_INVALID_ARG;
-  if ((reinterpret_cast<uintptr_t>(coords) & 15) || (reinterpret_cast<uintptr_t>(out_coords) & 15))
-    return P3D_ERR_INVALID_ARG;
-  if (static_cast<long long>(batch) * d.oD * d.oH * d.oW >= 0xffffffffll) return P3D_ERR_UNSUPPORTED;
-  RbWs w = carve_rb(workspace, n_in_cap, out_cap);
-  if (workspace_bytes < w.bytes) return P3D_ERR_WORKSPACE;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int K = d.kd * d.kh * d.kw;
-  P3D_CUDA_CHECK(cudaMemsetAsync(w.tab_in, 0xff, sizeof(unsigned long long) * w.cap_in, st));
-  P3D_CUDA_CHECK(cudaMemsetAsync(w.tab_out, 0xff, sizeof(unsigned long long) * w.cap_out, st));
-  P3D_CUDA_CHECK(cudaMemsetAsync(n_out_dev, 0, sizeof(int32_t) * 4, st));
-  if (n_in_cap > 0) {
-    rb_insert_kernel<<<div_up(n_in_cap, 256), 256, 0, st>>>(coords, n_in_dev, static_cast<int>(n_in_cap), d,
-                                                           w.tab_in, w.cap_in - 1, w.shift_in);
-    P3D_LAUNCH_CHECK();
-    rb_outputs_kernel<<<persistent_grid(n_in_cap * K), 256, 0, st>>>(coords, n_in_dev, n_in_cap, d, w.tab_out,
-                                                                 w.cap_out - 1, w.shift_out, out_coords, n_out_dev,
-                                                                 static_cast<int>(out_cap));
-    P3D_LAUNCH_CHECK();
-  }
-  rb_finish_kernel<<<1, 1, 0, st>>>(n_out_dev, static_cast<int>(out_cap));
-  P3D_LAUNCH_CHECK();
-  rb_neighbors_kernel<<<persistent_grid(out_cap * K), 256, 0, st>>>(out_coords, n_out_dev, out_cap, d, w.tab_in,
-                                                               w.cap_in - 1, w.shift_in, 0, nbr);
-  P3D_LAUNCH_CHECK();
-  return P3D_OK;
-}
-
 extern "C" int p3d_sparse_conv_gather_gemm_fp32(const float *in, const int32_t *nbr, const int32_t *n_out_dev,
                                                 int64_t n_out_cap, int K, int Cin, int Cout, const float *weight,
                                                 const float *scale, const float *shift, const float *residual,
@@ -623,10 +528,11 @@ extern "C" int p3d_sparse_affine_act(const float *x, const int32_t *n_dev, int64
   return P3D_OK;
 }
 
-// ------------------------------------------------------------------ coordinate tables owned by the caller
+// ------------------------------------------------------------------ coordinate tables
 // One table per index set (resolution level).  The level-0 table is built from the voxel coordinates; the table of a
 // strided conv's OUTPUT set is a by-product of enumerating its sites, and is what the next stage's SubM rulebook and
-// the next strided conv look coordinates up in — so every level's table is built exactly once per frame.
+// the next strided conv look coordinates up in — so every level's table is built exactly once per frame.  The
+// scratch-workspace entry points run the same code on tables carved out of their workspace.
 namespace {
 struct Tab {
   unsigned long long *p;
@@ -640,24 +546,47 @@ bool tab_of(void *mem, size_t bytes, int64_t rows_cap, Tab *t) {
   t->p = static_cast<unsigned long long *>(mem);
   return mem && bytes >= static_cast<size_t>(t->cap) * 8 && !(reinterpret_cast<uintptr_t>(mem) & 15);
 }
-}  // namespace
 
-extern "C" size_t p3d_sparse_table_bytes(int64_t rows_cap) {
-  if (rows_cap < 0 || rows_cap > kMaxRows) return 0;
+size_t tab_bytes(int64_t rows_cap) {
   return align_up(static_cast<size_t>(next_pow2(static_cast<uint64_t>(rows_cap > 512 ? rows_cap : 512) * 2)) * 8);
 }
 
-extern "C" int p3d_sparse_table_build(const int32_t *coords, const int32_t *n_dev, int64_t n_cap, int batch,
-                                      const int *spatial_host, void *table, size_t table_bytes, p3d_stream_t stream) {
-  const int one[3] = {1, 1, 1};
-  Dims d;
-  int rc = make_dims(batch, spatial_host, one, nullptr, nullptr, 1, &d);
+// The tables of p3d_sparse_rulebook_workspace_bytes(n_in_cap, n_out_cap): input set first, then output set.
+int carve_tables(void *ws, size_t ws_bytes, int64_t n_in_cap, int64_t n_out_cap, Tab *ti, Tab *to) {
+  const size_t in_bytes = tab_bytes(n_in_cap), out_bytes = tab_bytes(n_out_cap);
+  if (ws_bytes < in_bytes + out_bytes) return P3D_ERR_WORKSPACE;
+  char *p = static_cast<char *>(ws);
+  return tab_of(p, in_bytes, n_in_cap, ti) && tab_of(p + in_bytes, out_bytes, n_out_cap, to) ? P3D_OK
+                                                                                             : P3D_ERR_INVALID_ARG;
+}
+
+// Argument checks of the SubM / strided entry points; bad_buffers = the caller's own table or workspace check.
+int check_subm(const int32_t *coords, int64_t n_cap, int batch, const int *spatial_host, const int *ksize_host,
+               const int32_t *nbr, bool bad_buffers, Dims *d) {
+  int rc = make_dims(batch, spatial_host, ksize_host, nullptr, nullptr, 1, d);
   if (rc) return rc;
-  Tab t;
-  if (n_cap < 0 || n_cap > 0x7fffffff / 128 || !tab_of(table, table_bytes, n_cap, &t) || (n_cap && !coords) ||
+  if (n_cap < 0 || n_cap > 0x7fffffff / 128 || bad_buffers || (n_cap && (!coords || !nbr)) ||
       (reinterpret_cast<uintptr_t>(coords) & 15))
     return P3D_ERR_INVALID_ARG;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return P3D_OK;
+}
+
+int check_level(const int32_t *coords, int64_t n_in_cap, int batch, const int *spatial_host, const int *ksize_host,
+                const int *stride_host, const int *pad_host, const int32_t *out_coords, const int32_t *n_out_dev,
+                int64_t out_cap, const int32_t *nbr, bool bad_buffers, Dims *d) {
+  int rc = make_dims(batch, spatial_host, ksize_host, stride_host, pad_host, 0, d);
+  if (rc) return rc;
+  if (n_in_cap < 0 || out_cap < 1 || n_in_cap > 0x7fffffff / 128 || out_cap > 0x7fffffff / 128 || bad_buffers ||
+      !n_out_dev || !out_coords || !nbr || (n_in_cap && !coords))
+    return P3D_ERR_INVALID_ARG;
+  if ((reinterpret_cast<uintptr_t>(coords) & 15) || (reinterpret_cast<uintptr_t>(out_coords) & 15))
+    return P3D_ERR_INVALID_ARG;
+  if (static_cast<long long>(batch) * d->oD * d->oH * d->oW >= 0xffffffffll) return P3D_ERR_UNSUPPORTED;
+  return P3D_OK;
+}
+
+int build_table(const int32_t *coords, const int32_t *n_dev, int64_t n_cap, const Dims &d, const Tab &t,
+                cudaStream_t st) {
   P3D_CUDA_CHECK(cudaMemsetAsync(t.p, 0xff, static_cast<size_t>(t.cap) * 8, st));
   if (n_cap > 0) {
     rb_insert_kernel<<<div_up(n_cap, 256), 256, 0, st>>>(coords, n_dev, static_cast<int>(n_cap), d, t.p, t.cap - 1, t.shift);
@@ -666,50 +595,19 @@ extern "C" int p3d_sparse_table_build(const int32_t *coords, const int32_t *n_de
   return P3D_OK;
 }
 
-extern "C" int p3d_sparse_rulebook_subm_t(const int32_t *coords, const int32_t *n_dev, int64_t n_cap, int batch,
-                                          const int *spatial_host, const int *ksize_host, const void *table,
-                                          size_t table_bytes, int32_t *nbr, p3d_stream_t stream) {
-  Dims d;
-  int rc = make_dims(batch, spatial_host, ksize_host, nullptr, nullptr, 1, &d);
-  if (rc) return rc;
-  Tab t;
-  if (n_cap < 0 || n_cap > 0x7fffffff / 128 || !tab_of(const_cast<void *>(table), table_bytes, n_cap, &t) ||
-      (n_cap && (!coords || !nbr)) || (reinterpret_cast<uintptr_t>(coords) & 15))
-    return P3D_ERR_INVALID_ARG;
-  if (n_cap == 0) return P3D_OK;
+int subm_map(const int32_t *coords, const int32_t *n_dev, int64_t n_cap, const Dims &d, const Tab &t, int32_t *nbr,
+             cudaStream_t st) {
   const int K = d.kd * d.kh * d.kw;
-  rb_neighbors_kernel<<<persistent_grid(n_cap * K), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      coords, n_dev, n_cap, d, t.p, t.cap - 1, t.shift, 1, nbr);
+  rb_neighbors_kernel<<<persistent_grid(n_cap * K), 256, 0, st>>>(coords, n_dev, n_cap, d, t.p, t.cap - 1, t.shift, nbr);
   P3D_LAUNCH_CHECK();
   return P3D_OK;
 }
 
-// One resolution level: output sites + table of the strided conv, its neighbour map and (optionally) the SubM map of the
-// new level's blocks (kernel subm_ksize_host, odd sizes, "same" padding) in two launches.
-extern "C" int p3d_sparse_rulebook_level_t(const int32_t *coords, const int32_t *n_in_dev, int64_t n_in_cap, int batch,
-                                           const int *spatial_host, const int *ksize_host, const int *stride_host,
-                                           const int *pad_host, const void *table_in, size_t table_in_bytes,
-                                           int32_t *out_coords, int32_t *n_out_dev, int64_t out_cap, void *table_out,
-                                           size_t table_out_bytes, int32_t *nbr, const int *subm_ksize_host,
-                                           int32_t *nbr_subm, p3d_stream_t stream) {
-  Dims d;
-  int rc = make_dims(batch, spatial_host, ksize_host, stride_host, pad_host, 0, &d);
-  if (rc) return rc;
-  Tab ti, to;
-  if (n_in_cap < 0 || out_cap < 1 || n_in_cap > 0x7fffffff / 128 || out_cap > 0x7fffffff / 128 || !n_out_dev ||
-      !out_coords || !nbr || (n_in_cap && !coords) || !tab_of(const_cast<void *>(table_in), table_in_bytes, n_in_cap, &ti) ||
-      !tab_of(table_out, table_out_bytes, out_cap, &to) || (nbr_subm && !subm_ksize_host))
-    return P3D_ERR_INVALID_ARG;
-  if ((reinterpret_cast<uintptr_t>(coords) & 15) || (reinterpret_cast<uintptr_t>(out_coords) & 15))
-    return P3D_ERR_INVALID_ARG;
-  if (static_cast<long long>(batch) * d.oD * d.oH * d.oW >= 0xffffffffll) return P3D_ERR_UNSUPPORTED;
-  Dims dm = d;
-  if (nbr_subm) {
-    const int osp[3] = {d.oD, d.oH, d.oW};
-    rc = make_dims(batch, osp, subm_ksize_host, nullptr, nullptr, 1, &dm);
-    if (rc) return rc;
-  }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
+// One resolution level in two launches: output sites + table `to` of the strided conv d (inputs looked up in `ti`), its
+// neighbour map and, when nbr_subm is given, the SubM map dm of the new level.
+int level_maps(const int32_t *coords, const int32_t *n_in_dev, int64_t n_in_cap, const Dims &d, const Tab &ti,
+               int32_t *out_coords, int32_t *n_out_dev, int64_t out_cap, const Tab &to, int32_t *nbr, const Dims &dm,
+               int32_t *nbr_subm, cudaStream_t st) {
   const int K = d.kd * d.kh * d.kw, Km = nbr_subm ? dm.kd * dm.kh * dm.kw : 0;
   P3D_CUDA_CHECK(cudaMemsetAsync(to.p, 0xff, static_cast<size_t>(to.cap) * 8, st));
   P3D_CUDA_CHECK(cudaMemsetAsync(n_out_dev, 0, sizeof(int32_t) * 4, st));
@@ -724,13 +622,90 @@ extern "C" int p3d_sparse_rulebook_level_t(const int32_t *coords, const int32_t 
   P3D_LAUNCH_CHECK();
   return P3D_OK;
 }
+}  // namespace
 
-extern "C" int p3d_sparse_rulebook_conv_t(const int32_t *coords, const int32_t *n_in_dev, int64_t n_in_cap, int batch,
-                                          const int *spatial_host, const int *ksize_host, const int *stride_host,
-                                          const int *pad_host, const void *table_in, size_t table_in_bytes,
-                                          int32_t *out_coords, int32_t *n_out_dev, int64_t out_cap, void *table_out,
-                                          size_t table_out_bytes, int32_t *nbr, p3d_stream_t stream) {
-  return p3d_sparse_rulebook_level_t(coords, n_in_dev, n_in_cap, batch, spatial_host, ksize_host, stride_host, pad_host,
-                                     table_in, table_in_bytes, out_coords, n_out_dev, out_cap, table_out, table_out_bytes,
-                                     nbr, nullptr, nullptr, stream);
+extern "C" size_t p3d_sparse_table_bytes(int64_t rows_cap) {
+  if (rows_cap < 0 || rows_cap > kMaxRows) return 0;
+  return tab_bytes(rows_cap);
+}
+
+extern "C" int p3d_sparse_table_build(const int32_t *coords, const int32_t *n_dev, int64_t n_cap, int batch,
+                                      const int *spatial_host, void *table, size_t table_bytes, p3d_stream_t stream) {
+  const int one[3] = {1, 1, 1};
+  Dims d;
+  int rc = make_dims(batch, spatial_host, one, nullptr, nullptr, 1, &d);
+  if (rc) return rc;
+  Tab t;
+  if (n_cap < 0 || n_cap > 0x7fffffff / 128 || !tab_of(table, table_bytes, n_cap, &t) || (n_cap && !coords) ||
+      (reinterpret_cast<uintptr_t>(coords) & 15))
+    return P3D_ERR_INVALID_ARG;
+  return build_table(coords, n_dev, n_cap, d, t, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int p3d_sparse_rulebook_subm_t(const int32_t *coords, const int32_t *n_dev, int64_t n_cap, int batch,
+                                          const int *spatial_host, const int *ksize_host, const void *table,
+                                          size_t table_bytes, int32_t *nbr, p3d_stream_t stream) {
+  Dims d;
+  Tab t;
+  const bool bad = !tab_of(const_cast<void *>(table), table_bytes, n_cap, &t);
+  const int rc = check_subm(coords, n_cap, batch, spatial_host, ksize_host, nbr, bad, &d);
+  if (rc || n_cap == 0) return rc;
+  return subm_map(coords, n_dev, n_cap, d, t, nbr, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int p3d_sparse_rulebook_level_t(const int32_t *coords, const int32_t *n_in_dev, int64_t n_in_cap, int batch,
+                                           const int *spatial_host, const int *ksize_host, const int *stride_host,
+                                           const int *pad_host, const void *table_in, size_t table_in_bytes,
+                                           int32_t *out_coords, int32_t *n_out_dev, int64_t out_cap, void *table_out,
+                                           size_t table_out_bytes, int32_t *nbr, const int *subm_ksize_host,
+                                           int32_t *nbr_subm, p3d_stream_t stream) {
+  Dims d;
+  Tab ti, to;
+  const bool bad = !tab_of(const_cast<void *>(table_in), table_in_bytes, n_in_cap, &ti) ||
+                   !tab_of(table_out, table_out_bytes, out_cap, &to) || (nbr_subm && !subm_ksize_host);
+  int rc = check_level(coords, n_in_cap, batch, spatial_host, ksize_host, stride_host, pad_host, out_coords, n_out_dev,
+                       out_cap, nbr, bad, &d);
+  if (rc) return rc;
+  Dims dm = d;
+  if (nbr_subm) {
+    const int osp[3] = {d.oD, d.oH, d.oW};
+    rc = make_dims(batch, osp, subm_ksize_host, nullptr, nullptr, 1, &dm);
+    if (rc) return rc;
+  }
+  return level_maps(coords, n_in_dev, n_in_cap, d, ti, out_coords, n_out_dev, out_cap, to, nbr, dm, nbr_subm,
+                    static_cast<cudaStream_t>(stream));
+}
+
+// ------------------------------------------------------------------ scratch-workspace entry points (the Paddle ops)
+extern "C" size_t p3d_sparse_rulebook_workspace_bytes(int64_t n_in_cap, int64_t n_out_cap) {
+  if (n_in_cap < 0 || n_out_cap < 0 || n_in_cap > kMaxRows || n_out_cap > kMaxRows) return 0;
+  return tab_bytes(n_in_cap) + tab_bytes(n_out_cap);
+}
+
+extern "C" int p3d_sparse_rulebook_subm(const int32_t *coords, const int32_t *n_in_dev, int64_t n_in_cap, int batch,
+                                        const int *spatial_host, const int *ksize_host, int32_t *nbr,
+                                        void *workspace, size_t workspace_bytes, p3d_stream_t stream) {
+  Dims d;
+  Tab t, unused;
+  int rc = check_subm(coords, n_in_cap, batch, spatial_host, ksize_host, nbr, !workspace, &d);
+  if (rc || n_in_cap == 0) return rc;
+  if ((rc = carve_tables(workspace, workspace_bytes, n_in_cap, 0, &t, &unused))) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if ((rc = build_table(coords, n_in_dev, n_in_cap, d, t, st))) return rc;
+  return subm_map(coords, n_in_dev, n_in_cap, d, t, nbr, st);
+}
+
+extern "C" int p3d_sparse_rulebook_conv(const int32_t *coords, const int32_t *n_in_dev, int64_t n_in_cap, int batch,
+                                        const int *spatial_host, const int *ksize_host, const int *stride_host,
+                                        const int *pad_host, int32_t *out_coords, int32_t *n_out_dev,
+                                        int64_t out_cap, int32_t *nbr, void *workspace, size_t workspace_bytes,
+                                        p3d_stream_t stream) {
+  Dims d;
+  Tab ti, to;
+  int rc = check_level(coords, n_in_cap, batch, spatial_host, ksize_host, stride_host, pad_host, out_coords, n_out_dev,
+                       out_cap, nbr, !workspace, &d);
+  if (rc || (rc = carve_tables(workspace, workspace_bytes, n_in_cap, out_cap, &ti, &to))) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if ((rc = build_table(coords, n_in_dev, n_in_cap, d, ti, st))) return rc;
+  return level_maps(coords, n_in_dev, n_in_cap, d, ti, out_coords, n_out_dev, out_cap, to, nbr, d, nullptr, st);
 }

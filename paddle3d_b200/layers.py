@@ -11,8 +11,6 @@ torch CUDA tensors.  Data-dependent row counts stay on the device: the reference
 scalar (a D2H sync per sample, voxelize.py:43-45), here `num_voxels` travels with the tensors and
 callers that need exact shapes call `.trim()`.
 """
-import os
-
 import numpy as np
 import torch
 
@@ -147,8 +145,6 @@ class SparseResNet3D:
         self.extra_conv = [sp.Conv3D(128, 128, (3, 1, 1), (2, 1, 1), bias_attr=False),
                            sp.BatchNorm(128, epsilon=1e-3, momentum=0.01), sp.ReLU()]
         self.level_caps = None  # optional capacities of the 4 strided index sets
-        self.side_stream_rulebooks = os.environ.get("P3D_SIDE_STREAM", "0") != "0"  # off by default
-        self._side = {}
 
     def all_layers(self):
         out = list(self.conv_input[:2])
@@ -188,14 +184,6 @@ class SparseResNet3D:
     def forward_sparse(self, voxel_features, coors, batch_size, num=None):
         shape = [batch_size] + self.sparse_shape + [self.in_channels]
         x = sp.sparse_coo_tensor(coors, voxel_features, shape, num=num)
-        if self.side_stream_rulebooks:
-            # index sets and neighbour maps of all levels depend on the voxel coordinates only: build them on a side
-            # stream while the level-0 feature layers run (every consuming launch waits for its rulebook's event)
-            dev = x.index.coords.device
-            side = self._side.get(dev)
-            if side is None:
-                side = self._side[dev] = torch.cuda.Stream(device=dev)
-            sp.prepare_rulebooks(x.index, [l for l in self.all_layers() if not isinstance(l, sp.BatchNorm)], side)
         for l in self.conv_input:
             x = l(x)
         for b in self.blocks0:
@@ -212,10 +200,8 @@ class SparseResNet3D:
         return x, feats
 
     def join(self):
-        """Join the rulebook side stream into the current stream. Every conv launch already waits for the rulebook it
-        uses; this explicit join (after the lazily launched convs have been issued) is what stream capture needs."""
-        for dev, side in self._side.items():
-            torch.cuda.current_stream(dev).wait_stream(side)
+        """Does nothing: the network issues all its work on the caller's current stream, so there is no other stream to
+        join. Kept so that callers that join before stream capture keep working."""
 
     def forward(self, voxel_features, coors, batch_size, num=None, pixel_h16=False):
         """pixel_h16=False: the reference's dense BEV tensor [N, C*D, H, W] fp32.  True: the same tensor as pixel
@@ -224,9 +210,7 @@ class SparseResNet3D:
         # device counters [n_out, overflow, ...] of the 4 strided index sets: overflow != 0 means output sites were
         # dropped (capacity from set_level_caps too small) and the BEV tensor is incomplete; callers surface it
         self.level_counters = [t.index.counters for t in feats[1:]] + [out.index.counters]
-        dense = out.to_pixel_h16() if pixel_h16 else out.to_dense_bev()  # to_dense + transpose(0,4,1,2,3) + reshape
-        self.join()
-        return dense
+        return out.to_pixel_h16() if pixel_h16 else out.to_dense_bev()  # to_dense + transpose(0,4,1,2,3) + reshape
 
     __call__ = forward
 

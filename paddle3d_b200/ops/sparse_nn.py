@@ -68,6 +68,12 @@ def _triple(v):
     return [int(v)] * 3 if np.isscalar(v) else [int(x) for x in v]
 
 
+def _rulebook_key(key, ksize):
+    """Key of a SubM neighbour map in _IndexSet.subm_rulebooks: the layer's `key` (None: one map shared by the unkeyed
+    layers) and kernel size."""
+    return (key if key is not None else "_anon", tuple(ksize))
+
+
 class _IndexSet:
     """Active sites of one resolution level: coords [cap, 4] (b, z, y, x), device count, its coordinate hash table
     (built once: from the coordinates for the input level, as a by-product of the site enumeration for the output of a
@@ -77,7 +83,6 @@ class _IndexSet:
         self.coords, self.num, self.cap, self.batch, self.spatial = coords, num, cap, batch, list(spatial)
         self.subm_rulebooks = {}
         self.strided = {}      # id(Conv3D layer) -> (output _IndexSet, neighbour map), see _ConvBase.build_index
-        self.ready = {}        # rulebook key -> _Ready: built on another stream (prepare pass), wait before first use
         self._table = table
 
     def table(self):
@@ -90,7 +95,7 @@ class _IndexSet:
         return self._table
 
     def subm_rulebook(self, ksize, key):
-        k = (key, tuple(ksize)) if key is not None else ("_anon", tuple(ksize))
+        k = _rulebook_key(key, ksize)
         nbr = self.subm_rulebooks.get(k)
         if nbr is None:
             K = ksize[0] * ksize[1] * ksize[2]
@@ -102,20 +107,6 @@ class _IndexSet:
                                                    ptr(nbr), stream(dev)), "sparse_rulebook_subm_t")
             self.subm_rulebooks[k] = nbr
         return nbr
-
-
-class _Ready:
-    """Event recorded on the stream that built a rulebook; the consuming stream waits for it once."""
-
-    def __init__(self, stream_):
-        self.event = torch.cuda.Event()
-        self.event.record(stream_)
-        self.waited = False
-
-    def wait(self, stream_):
-        if not self.waited:
-            stream_.wait_event(self.event)
-            self.waited = True
 
 
 class SparseCooTensor:
@@ -217,33 +208,9 @@ def sparse_coo_tensor(indices, values, shape, stop_gradient=True, num=None):
     return SparseCooTensor(idx, values=values, channels=int(shape[4]))
 
 
-def prepare_rulebooks(index, conv_layers, side_stream):
-    """Build the index sets and neighbour maps of `conv_layers` (SubmConv3D / Conv3D, execution order, starting at
-    `index`) on `side_stream`: they depend on coordinates only, so they can run beside the first feature layers. Every
-    rulebook gets a _Ready event that the consuming launch waits for."""
-    dev = index.coords.device
-    main = torch.cuda.current_stream(dev)
-    side_stream.wait_stream(main)
-    with torch.cuda.stream(side_stream):
-        for l in conv_layers:
-            if l.subm:
-                k = (l.key if l.key is not None else "_anon", tuple(l.kernel_size))
-                key = ("subm",) + k
-                if key not in index.ready and k not in index.subm_rulebooks:
-                    index.subm_rulebook(l.kernel_size, l.key)
-                    index.ready[key] = _Ready(side_stream)
-            else:
-                key = ("conv", id(l))
-                fresh = id(l) not in index.strided
-                nxt, _ = l.build_index(index)
-                if fresh:
-                    index.ready[key] = _Ready(side_stream)
-                index = nxt
-
-
 class _Pending:
     __slots__ = ("x", "nbr", "num", "cap", "K", "cin", "cout", "weight", "scale", "shift", "residual", "relu", "precision",
-                 "ready", "wm")
+                 "wm")
 
 
 PROFILE = None  # set to a list to record (cin, cout, K, precision, nbr, num, start_event, end_event, kernel) per conv launch
@@ -255,8 +222,6 @@ def _run(p, t, want):
     L = lib()
     dev = p.nbr.device
     st = torch.cuda.current_stream(dev)
-    if p.ready is not None:
-        p.ready.wait(st)
     if PROFILE is not None:
         s_ev, e_ev = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     if p.precision == F16X3:
@@ -439,8 +404,7 @@ class _ConvBase(_Layer):
         return self
 
     def build_index(self, src):
-        """Strided conv: output site set + neighbour map of `src` under this layer's geometry (cached on `src`, so a
-        prepare pass can build it ahead of the feature path, on another stream)."""
+        """Strided conv: output site set + neighbour map of `src` under this layer's geometry (cached on `src`)."""
         hit = src.strided.get(id(self))
         if hit is not None:
             return hit
@@ -470,7 +434,7 @@ class _ConvBase(_Layer):
         index = _IndexSet(out_coords, n_out, cap, src.batch, osp, table=tab_out)
         index.counters = n_out
         if nbr_subm is not None:
-            index.subm_rulebooks[(fuse[1] if fuse[1] is not None else "_anon", sub_ks)] = nbr_subm
+            index.subm_rulebooks[_rulebook_key(fuse[1], sub_ks)] = nbr_subm
         src.strided[id(self)] = (index, nbr)
         return index, nbr
 
@@ -481,7 +445,6 @@ class _ConvBase(_Layer):
         p = _Pending()
         p.x, p.K, p.cin, p.cout = x, K, self.in_channels, self.out_channels
         p.weight, p.scale, p.shift, p.residual, p.relu = self.weight, None, self.bias, None, False
-        p.ready = None
         p.wm = False
         p.precision = _check_precision(self.precision if self.precision is not None else _default_precision[0])
         if p.precision == F16X3:
@@ -500,10 +463,8 @@ class _ConvBase(_Layer):
         if self.subm:
             index = x.index
             p.nbr = index.subm_rulebook(self.kernel_size, self.key)
-            p.ready = index.ready.get(("subm", self.key if self.key is not None else "_anon", tuple(self.kernel_size)))
         else:
             index, p.nbr = self.build_index(x.index)
-            p.ready = x.index.ready.get(("conv", id(self)))
         p.num, p.cap = index.num, index.cap
         return SparseCooTensor(index, channels=self.out_channels, pending=p)
 

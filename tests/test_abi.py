@@ -39,6 +39,10 @@ def test_status_strings_and_size_queries():
     assert L.p3d_scatter_dense_workspace_bytes(1, 1, 496, 432) >= 496 * 432 * 4
     assert L.p3d_centerpoint_postprocess_workspace_bytes(6, 180, 180, 1000, 83) > 0
     assert L.p3d_sparse_rulebook_workspace_bytes(160000, 640000) > 0
+    # the scratch-workspace rulebook calls hold one table per index set (512-row floor each)
+    for n_in, n_out in ((160000, 640000), (1000, 0), (0, 0)):
+        want = L.p3d_sparse_table_bytes(n_in) + L.p3d_sparse_table_bytes(n_out)
+        assert L.p3d_sparse_rulebook_workspace_bytes(n_in, n_out) == want
     # capacities whose hash table (2x rows, power of two) would not fit 2^31 entries are refused, not looped on (ADVICE r1)
     assert L.p3d_hard_voxelize_workspace_bytes(2 ** 31, 10, 10) == 0
     assert L.p3d_sparse_table_bytes(2 ** 31 + 5) == 0

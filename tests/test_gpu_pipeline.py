@@ -43,7 +43,7 @@ def test_frame_matches_cpu_oracle_frame(cuda, oracle_mod, precision):
     np.testing.assert_allclose(out["boxes"][:k].cpu().numpy(), ref["boxes"], rtol=1e-4, atol=1e-4)
 
 
-def test_graph_sweep_and_side_stream_agree_with_eager(cuda):
+def test_graph_and_sweep_agree_with_eager(cuda):
     import torch
     frames = _frames(4)
     pinned = [torch.from_numpy(f).pin_memory() for f in frames]
@@ -65,16 +65,6 @@ def test_graph_sweep_and_side_stream_agree_with_eager(cuda):
     for g, w in zip(got, want):
         assert torch.equal(g[0], w[0]) and torch.equal(g[1], w[1]) and torch.equal(g[2], w[2])
     assert len(list(graph.infer_many(iter(pinned[:1])))) == 1 and list(graph.infer_many(iter([]))) == []
-
-    side = _pipe(cuda, 2)  # rulebooks built on a side stream (optional mode): same bits
-    side.net.side_stream_rulebooks = True
-    for f, w in zip(pinned[:2], want):
-        b, s, l = side.infer(f)
-        assert torch.equal(b, w[0]) and torch.equal(side.out["bev"], w[3])
-    side.points.copy_(pinned[0])
-    side.capture()
-    b, s, l = side.infer(pinned[1])
-    assert torch.equal(b, want[1][0]) and torch.equal(side.out["bev"], want[1][3])
 
 
 def test_frame_with_dense_head(cuda, oracle_mod):

@@ -325,8 +325,9 @@ def test_hard_voxelizer_batch2(cuda, oracle_mod):
 
 
 def test_workspace_and_table_rulebook_apis_agree(cuda):
-    """The scratch-workspace rulebook entry point (p3d_sparse_rulebook_subm) and the caller-owned-table one
-    (p3d_sparse_table_build + p3d_sparse_rulebook_subm_t) must produce the same neighbour map."""
+    """The scratch-workspace rulebook entry points and the caller-owned-table ones must produce the same rulebooks:
+    p3d_sparse_rulebook_subm against p3d_sparse_table_build + p3d_sparse_rulebook_subm_t (same neighbour map), and
+    p3d_sparse_rulebook_conv against p3d_sparse_rulebook_level_t (the strided map)."""
     import torch
     from paddle3d_b200._lib import check, host_ints, lib
     from paddle3d_b200._mem import ptr, stream
@@ -351,6 +352,49 @@ def test_workspace_and_table_rulebook_apis_agree(cuda):
                 rows = np.nonzero(nb[:, k] >= 0)[0]
                 assert np.array_equal(coords[nb[rows, k]], coords[rows] + np.array([0, dz, dy, dx], np.int32))
                 k += 1
+
+    # Strided: site numbering comes from atomics, so the two are compared as sets: output coordinates, counters [0..2]
+    # and, for every output site, the input coordinate behind each tap.
+    def sites(out_coords, counters, nb):
+        m = int(counters[0])
+        src = np.concatenate([coords, np.full((1, 4), -1, np.int32)])[nb[:m]]  # row -1: no input
+        return {tuple(o): s.tobytes() for o, s in zip(out_coords[:m], src)}
+
+    full = None
+    # (kernel, stride, padding, rows counted on the device, out_cap): 3x3x3 stride 2; SparseResNet3D's extra conv; a
+    # device row count below the capacity; an out_cap too small for the sites (filled in from the first case)
+    for ks, st, pd, n_valid, out_cap in [(3, 2, 1, n, 4 * n), ((3, 1, 1), (2, 1, 1), 0, n, 4 * n),
+                                         (3, 2, 1, n // 2, 4 * n), (3, 2, 1, n, None)]:
+        small = out_cap is None
+        if small:
+            out_cap = len(full) // 2 + 1
+        num = torch.tensor([n_valid], dtype=torch.int32, device=cuda)
+        xs = sp.sparse_coo_tensor(x.index.coords.t(), x.values(), [2, 9, 33, 31, 16], num=num)
+        conv = sp.Conv3D(16, 16, ks, st, padding=pd, bias_attr=False)
+        conv.out_cap = out_cap
+        index, nbr_t = conv.build_index(xs.index)  # p3d_sparse_rulebook_level_t
+        K = nbr_t.shape[1]
+        out_coords = torch.empty((out_cap, 4), dtype=torch.int32, device=cuda)
+        n_out = torch.empty((4,), dtype=torch.int32, device=cuda)
+        nbr_w = torch.empty((out_cap, K), dtype=torch.int32, device=cuda)
+        ws = torch.empty((L.p3d_sparse_rulebook_workspace_bytes(n, out_cap),), dtype=torch.uint8, device=cuda)
+        check(L.p3d_sparse_rulebook_conv(ptr(xs.index.coords), ptr(num), n, 2, host_ints([9, 33, 31]),
+                                         host_ints(conv.kernel_size), host_ints(conv.stride), host_ints(conv.padding),
+                                         ptr(out_coords), ptr(n_out), out_cap, ptr(nbr_w), ptr(ws), ws.numel(),
+                                         stream(cuda)), "rulebook_conv")
+        cw, ct = n_out.cpu().numpy(), index.counters.cpu().numpy()
+        assert np.array_equal(cw[:3], ct[:3])
+        got = sites(out_coords.cpu().numpy(), cw, nbr_w.cpu().numpy())
+        want = sites(index.coords.cpu().numpy(), ct, nbr_t.cpu().numpy())
+        assert len(got) == len(want) == cw[0] > 0
+        if full is None:
+            full = want
+        if not small:
+            assert cw[1] == 0 and got == want
+            assert (nbr_w.cpu().numpy()[:cw[0]] < n_valid).all()  # rows past the device count are never used
+        else:  # overflow: each call keeps out_cap of the sites, which ones depends on the atomics
+            assert cw[0] == out_cap and cw[1] == 1 and cw[2] == len(full)
+            assert all(full.get(k) == v for k, v in got.items()) and all(full.get(k) == v for k, v in want.items())
 
 
 def test_level_rulebook_matches_separate_calls(cuda):
