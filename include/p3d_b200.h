@@ -376,22 +376,25 @@ int p3d_pillar_feature_net(const float *voxels, const int32_t *num_points_per_vo
 
 /* ---------------------------------------------------------------------------------------------
  * anchor_head_postprocess      SECOND v1.5 VoxelNet.predict (the path SSDHead.post_process -> rotate_nms_pcdet ports)
- *                              for one class at batch 1, with no host synchronisation.
- *   head [1, 10 R, H, W] fp32 planes: cls [R] | box [R x 7] | dir [R x 2]; channel a * K + k belongs to anchor
- *   (y * W + x) * R + a.  anchors [A, 7] (x, y, z, w, l, h, theta), A = H * W * R;  anchor_corners [A, 4] int32
- *   (x_min, y_min, x_max, y_max) clamped voxel indices of each anchor's near box (16-byte aligned).
+ *                              at batch 1 with sigmoid scores and class-agnostic NMS, with no host synchronisation.
+ *   head [1, R (C + 9), H, W] fp32 planes, C = num_classes: cls [R x C] | box [R x 7] | dir [R x 2]; channel a * K + k of
+ *   each group belongs to anchor (y * W + x) * R + a (K = C, 7, 2).  anchors [A, 7] (x, y, z, w, l, h, theta),
+ *   A = H * W * R;  anchor_corners [A, 4] int32 (x_min, y_min, x_max, y_max) clamped voxel indices of each anchor's
+ *   near box (16-byte aligned).
  *   coords [coords_cap, 4] (b, z, y, x) of the pillars, *num_coords_dev of them valid (null: all).
  *   Anchors whose occupied-pillar count over the near box is <= anchor_area_threshold are dropped; then
- *   sigmoid(cls) >= score_threshold, descending-score order with ties by ascending anchor index, the first
- *   nms_pre_max_size, rotated NMS, the first nms_post_max_size kept, direction fix, centre range filter.
- *   Outputs (device): boxes [nms_post_max_size, 7], scores, labels int64 (0), counts [2] int32 = (score-threshold
+ *   score = max over the classes of sigmoid(cls), label = the first class reaching it; score >= score_threshold,
+ *   descending-score order with ties by ascending anchor index, the first nms_pre_max_size, rotated NMS over all
+ *   classes together, the first nms_post_max_size kept, direction fix, centre range filter.  num_classes < 1: invalid.
+ *   Outputs (device): boxes [nms_post_max_size, 7], scores, labels int64, counts [2] int32 = (score-threshold
  *   candidates, rows written).  Optional (null to skip): anchor_mask [A] uint8, and the decoded candidates in
  *   score order before NMS: sorted_boxes [nms_pre_max_size, 7], sorted_scores [nms_pre_max_size].
  * ------------------------------------------------------------------------------------------- */
 size_t p3d_anchor_head_postprocess_workspace_bytes(int num_anchors, int grid_nx, int grid_ny, int nms_pre_max_size);
-int p3d_anchor_head_postprocess(const float *head, int feat_h, int feat_w, int anchors_per_loc, const float *anchors,
-                                const int32_t *anchor_corners, const int32_t *coords, const int32_t *num_coords_dev,
-                                int coords_cap, int grid_nx, int grid_ny, int anchor_area_threshold, float score_threshold,
+int p3d_anchor_head_postprocess(const float *head, int feat_h, int feat_w, int anchors_per_loc, int num_classes,
+                                const float *anchors, const int32_t *anchor_corners, const int32_t *coords,
+                                const int32_t *num_coords_dev, int coords_cap, int grid_nx, int grid_ny,
+                                int anchor_area_threshold, float score_threshold,
                                 float nms_iou_threshold, int nms_pre_max_size, int nms_post_max_size,
                                 const float *post_center_range_host, float *boxes, float *scores, int64_t *labels,
                                 int32_t *counts, uint8_t *anchor_mask, float *sorted_boxes, float *sorted_scores,

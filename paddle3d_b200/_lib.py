@@ -90,8 +90,8 @@ SIGNATURES = {
     "p3d_sparse_conv_gather_gemm": (_int, [_vp, _vp, _vp, _i64, _int, _int, _int, _vp, _vp, _vp, _vp, _int, _int,
                                            _vp, _vp]),
     "p3d_anchor_head_postprocess_workspace_bytes": (_sz, [_int, _int, _int, _int]),
-    "p3d_anchor_head_postprocess": (_int, [_vp, _int, _int, _int, _vp, _vp, _vp, _vp, _int, _int, _int, _int, _f, _f,
-                                           _int, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "p3d_anchor_head_postprocess": (_int, [_vp, _int, _int, _int, _int, _vp, _vp, _vp, _vp, _int, _int, _int, _int, _f,
+                                           _f, _int, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "p3d_merge_sweeps_workspace_bytes": (_sz, [_int, _i64]),
     "p3d_merge_sweeps": (_int, [_vp, _int, _i64, _int, _vp, _int, _vp, _int, _int, _f, _vp, _i64, _vp, _vp, _vp, _sz,
                                 _vp]),

@@ -1,4 +1,4 @@
-// Anchor (SSD) head postprocess for sm_90a: SECOND v1.5 VoxelNet.predict at batch 1, one class, no host synchronisation
+// Anchor (SSD) head postprocess for sm_90a: SECOND v1.5 VoxelNet.predict at batch 1, no host synchronisation
 // (every count stays on the device, buffers are sized by capacity), so a frame can be captured in a CUDA graph.
 //
 // The reference runs this in Python (SSDHead.post_process -> rotate_nms_pcdet): masked_select (D2H sync), argsort, the
@@ -6,11 +6,13 @@
 //   A1 ahp_occ        occupied-pillar count per BEV cell from the pillar coords (sparse_sum_for_anchors_mask)
 //   A2 ahp_col/row    2-D inclusive prefix sum of that map (cumsum(0).cumsum(1)), integers: exact in any order
 //   A3 ahp_score      per anchor: area = ID - IB - IC + IA on its four (host-precomputed) clamped voxel corners
-//                     (fused_get_anchors_area), keep area > thr; score = sigmoid(cls); candidate if score >= thr;
+//                     (fused_get_anchors_area), keep area > thr; score = max over the C classes of sigmoid(cls_c)
+//                     (encode_background_as_zeros, use_multi_class_nms off); candidate if score >= thr;
 //                     51-bit sort key (~score_bits << 20 | anchor) - descending score, ties by ascending anchor index
 //   A4 cub radix sort of the keys (non-candidates carry the all-ones key and sink to the end)
-//   A5 ahp_gather     first min(candidates, pre_max): second_box_decode, dir argmax, NMS box laid out as
-//                     rotate_nms_pcdet does: (x, y, z, l, w, h, -theta - pi/2) in fp32
+//   A5 ahp_gather     first min(candidates, pre_max): class label (recomputed, so no per-anchor label array),
+//                     second_box_decode, dir argmax, NMS box laid out as rotate_nms_pcdet does:
+//                     (x, y, z, l, w, h, -theta - pi/2) in fp32.  NMS is class-agnostic, as in the reference
 //   A6 rotated-IoU bit-matrix, one thread per pair (box_geom.cuh) + A7 on-device greedy pass (nms_reduce.cuh), stopping
 //                     at post_max kept boxes
 //   A8 ahp_emit       direction fix ((theta > 0) xor dir -> theta + pi), centre range filter, order-preserving compaction
@@ -32,7 +34,7 @@ constexpr float kHalfPi = 1.57079637f;               // fp32(pi / 2), as paddle 
 constexpr float kPi = 3.14159274f;                   // fp32(pi)
 
 struct AhpAttrs {
-  int A, HW, R, nx, ny, area_thr, pre_max, post_max, cbmax, coords_cap;
+  int A, HW, R, C, nx, ny, area_thr, pre_max, post_max, cbmax, coords_cap;
   float score_thr, iou_thr;
   float lo[3], hi[3];  // post_center_limit_range
 };
@@ -48,6 +50,7 @@ struct AhpWs {
   float *top_box;             // [pre_max, 7] decoded boxes in score order
   float *top_score;           // [pre_max]
   int32_t *top_dir;           // [pre_max]
+  int32_t *top_label;         // [pre_max]
   float *nms_box;             // [pre_max, 7]
   unsigned long long *mask;   // [pre_max, cbmax]
   int32_t *keep;              // [pre_max]
@@ -70,6 +73,7 @@ AhpWs carve(void *p, int A, int cells, int pre_max) {
   w.top_box = c.take<float>(static_cast<size_t>(pre_max) * 7);
   w.top_score = c.take<float>(pre_max);
   w.top_dir = c.take<int32_t>(pre_max);
+  w.top_label = c.take<int32_t>(pre_max);
   w.nms_box = c.take<float>(static_cast<size_t>(pre_max) * 7);
   w.mask = c.take<unsigned long long>(static_cast<size_t>(pre_max) * cbmax);
   w.keep = c.take<int32_t>(pre_max);
@@ -78,6 +82,22 @@ AhpWs carve(void *p, int A, int cells, int pre_max) {
 }
 
 __device__ __forceinline__ float sigmoid_f32(float x) { return __fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-x))); }
+
+// Score and label of one anchor: max over the C class planes of sigmoid(cls_c), label = the first class reaching it.
+// The comparison is on the fp32 sigmoid values (as the reference's max / argmax over sigmoid(cls)), not on the logits:
+// two logits may round to the same score, and then the lower class wins.  cls points at class 0 of the anchor's group.
+__device__ __forceinline__ float class_max(const float *__restrict__ cls, size_t HW, int C, int &label) {
+  float best = sigmoid_f32(cls[0]);
+  label = 0;
+  for (int c = 1; c < C; ++c) {
+    const float s = sigmoid_f32(cls[static_cast<size_t>(c) * HW]);
+    if (s > best) {
+      best = s;
+      label = c;
+    }
+  }
+  return best;
+}
 
 // coords [cap, 4] (b, z, y, x) of the pillars; one pillar per cell, the count is still a sum as in the reference
 __global__ void __launch_bounds__(256) ahp_occ_kernel(const int32_t *__restrict__ coords, const int32_t *__restrict__ n_dev,
@@ -138,7 +158,8 @@ __global__ void __launch_bounds__(256) ahp_score_kernel(const float *__restrict_
     if (mask_out) mask_out[i] = keep ? 1 : 0;
     if (keep) {
       const int cell = i / at.R, a = i - cell * at.R;
-      const float s = sigmoid_f32(head[static_cast<size_t>(a) * at.HW + cell]);
+      int label;
+      const float s = class_max(head + static_cast<size_t>(a) * at.C * at.HW + cell, at.HW, at.C, label);
       cand = s >= at.score_thr;
       key = (static_cast<unsigned long long>(0x7fffffffu - __float_as_uint(s)) << kIdxBits) | static_cast<unsigned>(i);
     }
@@ -159,7 +180,7 @@ __global__ void __launch_bounds__(128) ahp_gather_kernel(const float *__restrict
   const size_t HW = at.HW;
   const float *an = anchors + static_cast<size_t>(i) * 7;
   const float xa = an[0], ya = an[1], wa = an[3], la = an[4], ha = an[5], ra = an[6];
-  const float *bt = head + (static_cast<size_t>(at.R) + a * 7) * HW + cell;
+  const float *bt = head + (static_cast<size_t>(at.R) * at.C + a * 7) * HW + cell;
   const float xt = bt[0], yt = bt[HW], zt = bt[2 * HW], wt = bt[3 * HW], lt = bt[4 * HW], ht = bt[5 * HW], rt = bt[6 * HW];
   // second_box_decode (no smooth_dim, no angle vector)
   const float za = __fadd_rn(an[2], __fmul_rn(ha, 0.5f));
@@ -172,14 +193,16 @@ __global__ void __launch_bounds__(128) ahp_gather_kernel(const float *__restrict
   b[5] = __fmul_rn(expf(ht), ha);
   b[2] = __fsub_rn(__fadd_rn(__fmul_rn(zt, ha), za), __fmul_rn(b[5], 0.5f));
   b[6] = __fadd_rn(rt, ra);
-  const float *dt = head + (static_cast<size_t>(8) * at.R + a * 2) * HW + cell;
+  const float *dt = head + (static_cast<size_t>(at.C + 7) * at.R + a * 2) * HW + cell;
   const int dir = dt[HW] > dt[0] ? 1 : 0;  // argmax, ties to index 0
-  const float s = sigmoid_f32(head[static_cast<size_t>(a) * HW + cell]);
+  int label;
+  const float s = class_max(head + static_cast<size_t>(a) * at.C * HW + cell, HW, at.C, label);
   float *tb = w.top_box + static_cast<size_t>(r) * 7;
 #pragma unroll
   for (int k = 0; k < 7; ++k) tb[k] = b[k];
   w.top_score[r] = s;
   w.top_dir[r] = dir;
+  w.top_label[r] = label;
   float *nb = w.nms_box + static_cast<size_t>(r) * 7;  // rotate_nms_pcdet: columns (0, 1, 2, 4, 3, 5), -theta - pi/2
   nb[0] = b[0];
   nb[1] = b[1];
@@ -239,6 +262,7 @@ __global__ void __launch_bounds__(256) ahp_emit_kernel(AhpAttrs at, AhpWs w, flo
     bool ok = false;
     float b[7];
     float s = 0.f;
+    int label = 0;
     if (r < n) {
       const int j = w.keep[r];
       const float *tb = w.top_box + static_cast<size_t>(j) * 7;
@@ -246,6 +270,7 @@ __global__ void __launch_bounds__(256) ahp_emit_kernel(AhpAttrs at, AhpWs w, flo
       for (int k = 0; k < 7; ++k) b[k] = tb[k];
       if ((b[6] > 0.f) != (w.top_dir[j] != 0)) b[6] = __fadd_rn(b[6], kPi);
       s = w.top_score[j];
+      label = w.top_label[j];
       ok = b[0] >= at.lo[0] && b[1] >= at.lo[1] && b[2] >= at.lo[2] && b[0] <= at.hi[0] && b[1] <= at.hi[1] &&
            b[2] <= at.hi[2];
     }
@@ -262,7 +287,7 @@ __global__ void __launch_bounds__(256) ahp_emit_kernel(AhpAttrs at, AhpWs w, flo
 #pragma unroll
       for (int k = 0; k < 7; ++k) boxes[static_cast<size_t>(off) * 7 + k] = b[k];
       scores[off] = s;
-      labels[off] = 0;
+      labels[off] = label;
     }
     base += total;
     __syncthreads();
@@ -284,17 +309,19 @@ extern "C" size_t p3d_anchor_head_postprocess_workspace_bytes(int num_anchors, i
   return carve(nullptr, num_anchors, grid_nx * grid_ny, nms_pre_max_size).bytes;
 }
 
-extern "C" int p3d_anchor_head_postprocess(const float *head, int feat_h, int feat_w, int anchors_per_loc, const float *anchors,
-                                           const int32_t *anchor_corners, const int32_t *coords, const int32_t *num_coords_dev,
-                                           int coords_cap, int grid_nx, int grid_ny, int anchor_area_threshold,
-                                           float score_threshold, float nms_iou_threshold, int nms_pre_max_size,
+extern "C" int p3d_anchor_head_postprocess(const float *head, int feat_h, int feat_w, int anchors_per_loc, int num_classes,
+                                           const float *anchors, const int32_t *anchor_corners, const int32_t *coords,
+                                           const int32_t *num_coords_dev, int coords_cap, int grid_nx, int grid_ny,
+                                           int anchor_area_threshold, float score_threshold, float nms_iou_threshold,
+                                           int nms_pre_max_size,
                                            int nms_post_max_size, const float *post_center_range_host, float *boxes,
                                            float *scores, int64_t *labels, int32_t *counts, uint8_t *anchor_mask,
                                            float *sorted_boxes, float *sorted_scores, void *workspace,
                                            size_t workspace_bytes, p3d_stream_t stream) {
   if (!head || !anchors || !anchor_corners || !post_center_range_host || !boxes || !scores || !labels || !counts ||
-      !workspace || feat_h < 1 || feat_w < 1 || anchors_per_loc < 1 || coords_cap < 0 || (coords_cap && !coords) ||
-      grid_nx < 1 || grid_ny < 1 || nms_pre_max_size < 1 || nms_post_max_size < 1 || score_threshold < 0.f)
+      !workspace || feat_h < 1 || feat_w < 1 || anchors_per_loc < 1 || num_classes < 1 || coords_cap < 0 ||
+      (coords_cap && !coords) || grid_nx < 1 || grid_ny < 1 || nms_pre_max_size < 1 || nms_post_max_size < 1 ||
+      score_threshold < 0.f)
     return P3D_ERR_INVALID_ARG;
   if ((reinterpret_cast<uintptr_t>(anchor_corners) & 15) || (reinterpret_cast<uintptr_t>(coords) & 15))
     return P3D_ERR_INVALID_ARG;
@@ -308,6 +335,7 @@ extern "C" int p3d_anchor_head_postprocess(const float *head, int feat_h, int fe
   at.A = static_cast<int>(A);
   at.HW = feat_h * feat_w;
   at.R = anchors_per_loc;
+  at.C = num_classes;
   at.nx = grid_nx;
   at.ny = grid_ny;
   at.area_thr = anchor_area_threshold;

@@ -1,9 +1,12 @@
-"""PointPillars KITTI car inference (configs/pointpillars/pointpillars_xyres16_kitti_car.yml, the SECOND v1.5 `car.xyres_16`
-values) on one GPU, composed from this repository's kernels:
+"""PointPillars KITTI inference on one GPU: the car model (CONFIG with synth.C2:
+configs/pointpillars/pointpillars_xyres16_kitti_car.yml, the SECOND v1.5 `car.xyres_16` values) and the two-class
+cyclist / pedestrian model (CONFIG_PED_CYCLIST with synth.C2_PED_CYCLIST:
+pointpillars_xyres16_kitti_cyclist_pedestrian.yml, the SECOND v1.5 `ped_cycle/xyres_16` values), composed from this
+repository's kernels:
 
-    hard_voxelize -> PillarFeatureNet (one fused launch) -> pillar rows as fp16 pairs -> pixel fp16-pair image [496 x 432]
-    -> SecondBackbone + SecondFPN (dense_head.SecondTrunk) -> SSD head (cls | box | dir as ONE 384 -> 20 1x1 conv, fp32
-    planes) -> anchor_head_postprocess (csrc/anchor_postprocess.cu) -> boxes
+    hard_voxelize -> PillarFeatureNet (one fused launch) -> pillar rows as fp16 pairs -> pixel fp16-pair image
+    [496 x 432 car, 248 x 296 cyclist / pedestrian] -> SecondBackbone + SecondFPN (dense_head.SecondTrunk) -> SSD head
+    (cls | box | dir as ONE 1x1 conv, fp32 planes) -> anchor_head_postprocess (csrc/anchor_postprocess.cu) -> boxes
 
 PointPillarsHotPath captures everything between the H2D copy of the points and the D2H copy of the boxes as one CUDA graph
 (pipeline.CapturedFrame).  Anchors are constant per model and built once on the host (create_anchors_3d_stride, SECOND's
@@ -27,6 +30,21 @@ CONFIG = dict(
     anchor=dict(sizes=(1.6, 3.9, 1.56), strides=(0.32, 0.32, 0.0), offsets=(0.16, -39.52, -1.78), rotations=(0.0, 1.57)),
     test=dict(anchor_area_threshold=1, nms_score_threshold=0.05, nms_iou_threshold=0.5, nms_pre_max_size=1000,
               nms_post_max_size=300, post_center_limit_range=[0.0, -39.68, -5.0, 69.12, 39.68, 5.0]),
+)
+
+# SECOND v1.5 ped_cycle/xyres_16 (PARITY UNPINNED, like CONFIG): the first block keeps stride 1, so the head runs at the
+# full 248 x 296 grid.  One anchor generator per class, in label order (0 cyclist, 1 pedestrian); per location the
+# anchors are (class, rotation), R = 4, and the head has R * (2 + 7 + 2) = 44 channels.
+_PED_CYCLIST_ANCHOR = dict(strides=(0.16, 0.16, 0.0), offsets=(0.08, -19.76, -1.465), rotations=(0.0, 1.57))
+CONFIG_PED_CYCLIST = dict(
+    pfn_channels=64, pfn_bn_eps=1e-3,
+    backbone=dict(out_channels=(64, 128, 256), layer_nums=(3, 5, 5), downsample_strides=(1, 2, 2)),
+    fpn=dict(out_channels=(128, 128, 128), upsample_strides=(1, 2, 4), use_conv_for_no_stride=False),
+    num_classes=2, anchors_per_loc=4, box_code_size=7, num_dir_bins=2,
+    anchors=[dict(_PED_CYCLIST_ANCHOR, sizes=(0.6, 1.76, 1.73)),    # cyclist
+             dict(_PED_CYCLIST_ANCHOR, sizes=(0.6, 0.8, 1.73))],    # pedestrian
+    test=dict(anchor_area_threshold=1, nms_score_threshold=0.05, nms_iou_threshold=0.5, nms_pre_max_size=1000,
+              nms_post_max_size=300, post_center_limit_range=[0.0, -19.84, -2.5, 47.36, 19.84, 0.5]),
 )
 
 
@@ -80,8 +98,9 @@ def anchor_voxel_corners(anchors, voxel_size, point_cloud_range, grid):
 
 class PointPillars:
     """Seeded PointPillars model: PillarFeatureNet (one PFNLayer 9 -> 64, no bias, BatchNorm1D eps 1e-3), SecondTrunk and
-    the SSD head as one 384 -> 20 1x1 conv with bias (output channels: cls [2] | box [2 x 7] | dir [2 x 2], channel
-    a * K + k belonging to anchor (y * W + x) * 2 + a)."""
+    the SSD head as one 384 -> R (C + 9) 1x1 conv with bias, C classes and R anchors per location (output channels:
+    cls [R x C] | box [R x 7] | dir [R x 2], channel a * K + k of each group belonging to anchor (y * W + x) * R + a;
+    car: 384 -> 20)."""
 
     def __init__(self, cfg=None, model_cfg=None):
         self.cfg = dict(cfg or synth.C2)
@@ -93,14 +112,19 @@ class PointPillars:
         self.trunk = SecondTrunk(self.C, mc["backbone"]["out_channels"], mc["backbone"]["layer_nums"],
                                  mc["backbone"]["downsample_strides"], mc["fpn"]["out_channels"],
                                  mc["fpn"]["upsample_strides"], mc["fpn"]["use_conv_for_no_stride"])
-        R = mc["anchors_per_loc"]
-        self.head_channels = R * (1 + mc["box_code_size"] + mc["num_dir_bins"])
+        R, self.num_classes = mc["anchors_per_loc"], mc.get("num_classes", 1)
+        self.head_channels = R * (self.num_classes + mc["box_code_size"] + mc["num_dir_bins"])
         self.head = _Conv(self.trunk.fpn_channels, self.head_channels, 1, bias=True, relu=False)
-        s = mc["backbone"]["downsample_strides"][0]  # the FPN output is at the first block's stride: 248 x 216
+        s = mc["backbone"]["downsample_strides"][0]  # the FPN output is at the first block's stride: 248 x 216 (car)
         self.feat_hw = (self.grid[1] // s, self.grid[0] // s)
-        a = mc["anchor"]
-        self.anchors_np = create_anchors_3d_stride([1, self.feat_hw[0], self.feat_hw[1]], a["sizes"], a["strides"],
-                                                   a["offsets"], a["rotations"]).reshape(-1, 7)
+        # one generator per class, concatenated per location as SECOND's TargetAssigner.generate_anchors does:
+        # per location (class, rotation)
+        per_class = [create_anchors_3d_stride([1, self.feat_hw[0], self.feat_hw[1]], a["sizes"], a["strides"],
+                                              a["offsets"], a["rotations"])
+                     for a in (mc["anchors"] if "anchors" in mc else [mc["anchor"]])]
+        self.anchors_np = np.concatenate(per_class, axis=3).reshape(-1, 7)
+        if len(per_class) != self.num_classes or self.anchors_np.shape[0] != self.feat_hw[0] * self.feat_hw[1] * R:
+            raise ValueError("model config: one anchor generator per class, anchors_per_loc anchors per location")
         self.corners_np = anchor_voxel_corners(self.anchors_np, self.cfg["voxel_size"], self.cfg["point_cloud_range"],
                                                self.grid)
         self.device = None
@@ -145,7 +169,7 @@ class PointPillars:
         return image, shape, coors, nv
 
     def dense(self, image, shape):
-        """Pixel fp16-pair BEV image -> SSD head planes [1, 20, H / 2, W / 2] fp32."""
+        """Pixel fp16-pair BEV image -> SSD head planes [1, R (C + 9), H / s, W / s] fp32 (s: the first block's stride)."""
         cat, cshape = self.trunk(image, shape)
         _, planes, _ = self.head(cat, cshape, want_nchw=True)
         return planes
@@ -155,29 +179,32 @@ class PointPillars:
         return ahp.anchor_head_postprocess_device(
             planes, self.anchors, self.corners, coors, nv, self.grid, t["post_center_limit_range"],
             t["anchor_area_threshold"], t["nms_score_threshold"], t["nms_iou_threshold"], t["nms_pre_max_size"],
-            t["nms_post_max_size"], anchor_mask=anchor_mask, sorted_out=sorted_out)
+            t["nms_post_max_size"], anchor_mask=anchor_mask, sorted_out=sorted_out, num_classes=self.num_classes)
 
     def calibrate_cls_bias(self, points, target_frac=0.02):
-        """Seeded weights leave the cls logits near the initial bias, so either almost none or most of the 107,136 anchors
-        would pass the 0.05 score threshold.  This shifts both cls biases so that `target_frac` of all anchors (2 %, about
-        2.1k) pass the anchor mask AND the threshold on this frame: more than nms_pre_max_size = 1000, so the top-k cut
-        runs.  Weights stay seeded and are exported unchanged to the CPU arm."""
+        """Seeded weights leave the cls logits near the initial bias, so either almost none or most of the anchors (107,136
+        car) would pass the 0.05 score threshold.  This shifts the cls biases of each class so that `target_frac` / C of
+        all anchors pass the anchor mask AND the threshold in that class on this frame (at most 2 % together; about 2.1k
+        for the car): more than nms_pre_max_size = 1000, so the top-k cut runs, and every class has candidates, so every
+        label reaches the output.  Weights stay seeded and are exported unchanged to the CPU arm."""
         image, shape, coors, nv = self.encode(points)
         planes = self.dense(image, shape)
         mask = torch.empty((self.anchors.shape[0],), dtype=torch.uint8, device=planes.device)
         self.postprocess(planes, coors, nv, anchor_mask=mask)
-        R = self.mc["anchors_per_loc"]
-        logits = planes[0, :R].permute(1, 2, 0).reshape(-1)[mask.bool()].float().cpu().numpy()
-        k = int(round(target_frac * self.anchors.shape[0]))
+        R, C = self.mc["anchors_per_loc"], self.num_classes
+        cls = planes[0, :R * C].reshape(R, C, *planes.shape[2:])
+        k = int(round(target_frac * self.anchors.shape[0] / C))
         thr = self.mc["test"]["nms_score_threshold"]
         logit_thr = float(np.log(thr / (1.0 - thr)))
-        if len(logits) > k:
-            v = np.sort(logits)[::-1]
-            shift = logit_thr - 0.5 * (float(v[k - 1]) + float(v[k]))
-        else:
-            shift = logit_thr - float(logits.min()) + 1.0 if len(logits) else 0.0
         b = self.head.np["bias"].copy()
-        b[:R] = (b[:R] + np.float32(shift)).astype(np.float32)
+        for c in range(C):
+            logits = cls[:, c].permute(1, 2, 0).reshape(-1)[mask.bool()].float().cpu().numpy()
+            if len(logits) > k:
+                v = np.sort(logits)[::-1]
+                shift = logit_thr - 0.5 * (float(v[k - 1]) + float(v[k]))
+            else:
+                shift = logit_thr - float(logits.min()) + 1.0 if len(logits) else 0.0
+            b[c:R * C:C] = (b[c:R * C:C] + np.float32(shift)).astype(np.float32)  # cls channels a * C + c
         self.head.np["bias"] = b
         self.head.dev["shift"].copy_(torch.from_numpy(b))
         return self
@@ -202,12 +229,14 @@ class PointPillarsHotPath(CapturedFrame):
     """One PointPillars frame on one GPU: H2D -> [captured: hard_voxelize -> PFN -> pixel image -> trunk -> head conv ->
     anchor postprocess] -> D2H of boxes [300, 7], scores, labels, counts (candidates, rows) and the status word."""
 
-    def __init__(self, cfg=None, device="cuda:0", seed=0, num_points=None, bn_gain=1.0):
+    def __init__(self, cfg=None, device="cuda:0", seed=0, num_points=None, bn_gain=1.0, model_cfg=None):
+        """cfg: the point-cloud config (synth.C2 by default); model_cfg: the model config (CONFIG by default; synth.C2 with
+        CONFIG is the car model, synth.C2_PED_CYCLIST with CONFIG_PED_CYCLIST the cyclist / pedestrian one)."""
         self.cfg = dict(cfg or synth.C2)
         self.device = torch.device(device)
         self.n = int(num_points or self.cfg["num_points"])
         self.F = self.cfg["point_dim"]
-        self.model = PointPillars(self.cfg).init_weight(seed=seed, device=self.device, bn_gain=bn_gain)
+        self.model = PointPillars(self.cfg, model_cfg).init_weight(seed=seed, device=self.device, bn_gain=bn_gain)
         self.points = torch.zeros((self.n, self.F), dtype=torch.float32, device=self.device)
         self.graph = None
         self.out = None

@@ -18,6 +18,11 @@ C3 = dict(name="centerpoint_voxel_0075", num_points=300000, point_dim=5, voxel_s
 # 0.1 m variant named by BASELINE.json.metric: same 1440x1440x40 grid over a 144 m square
 C3_01 = dict(name="centerpoint_voxel_01", num_points=300000, point_dim=5, voxel_size=[0.1, 0.1, 0.2],
              point_cloud_range=[-72.0, -72.0, -5.0, 72.0, 72.0, 3.0], max_points=10, max_voxels=160000)
+# SECOND v1.5 ped_cycle/xyres_16, which configs/pointpillars/pointpillars_xyres16_kitti_cyclist_pedestrian.yml descends
+# from (PARITY UNPINNED: not checked against the yml): 0.16 m pillars over 47.36 x 39.68 m -> 296 x 248.  SECOND keeps
+# 100 points per pillar; the fused PFN kernel takes at most 64, so this uses C2's 32.
+C2_PED_CYCLIST = dict(name="pointpillars_kitti_ped_cyclist", num_points=20000, point_dim=4, voxel_size=[0.16, 0.16, 3.0],
+                      point_cloud_range=[0.0, -19.84, -2.5, 47.36, 19.84, 0.5], max_points=32, max_voxels=40000)
 C1 = dict(C2, name="c1_cpu", num_points=1000)
 # LiDAR branch of BEVFusion (configs/bevfusion/bevf_pp_2x8_1x_nusc.yaml:87-105): 0.25 m pillars on a 400 x 400 grid
 C4_LIDAR = dict(name="bevfusion_lidar_pillars", num_points=300000, point_dim=4, voxel_size=[0.25, 0.25, 8.0],

@@ -1,11 +1,14 @@
 #!/usr/bin/env python
 """tools/pointpillars_bench.py — PointPillars KITTI frames/s on an H100 (BASELINE config 2).
 
-  python tools/pointpillars_bench.py [--steps K] [--warmup W] [--in-flight L] [--no-cpu-baseline] [--dump-outputs DIR]
+  python tools/pointpillars_bench.py [--config car|ped_cyclist] [--steps K] [--warmup W] [--in-flight L]
+                                     [--no-cpu-baseline] [--dump-outputs DIR]
 
-A step = one 20k x 4-point synth.lidar_cloud(C2) frame through pointpillars.PointPillarsHotPath: hard_voxelize ->
-PillarFeatureNet -> pixel fp16-pair image [496 x 432] -> SecondBackbone + SecondFPN + SSD head conv (66.2 GFLOP) ->
-anchor_head_postprocess -> boxes.  Prints one JSON line.  The timing harness (CenterPointSweep lanes, e2e through
+A step = one 20k x 4-point synth.lidar_cloud frame through pointpillars.PointPillarsHotPath: hard_voxelize ->
+PillarFeatureNet -> pixel fp16-pair image -> SecondBackbone + SecondFPN + SSD head conv -> anchor_head_postprocess ->
+boxes.  --config car (default): synth.C2 with pointpillars.CONFIG, a 496 x 432 image, 66.2 GFLOP dense; ped_cyclist:
+synth.C2_PED_CYCLIST with pointpillars.CONFIG_PED_CYCLIST (two classes), a 248 x 296 image with a stride-1 first block.
+Prints one JSON line.  The timing harness (CenterPointSweep lanes, e2e through
 infer_many / infer, graph-timed stages) is bench.py's, imported from it, so both models are measured the same way.
 """
 import argparse
@@ -23,6 +26,9 @@ import numpy as np  # noqa: E402
 from bench import BN_GAIN, POOL, UNIT, frame_pool, graph_time_ms, measure, rel_errors  # noqa: E402
 
 PP_METRIC = "PointPillars KITTI frames/sec @20k pts, 0.16 m pillars, 496x432 BEV (pointpillars_xyres16_kitti_car)"
+PP_PED_CYCLIST_METRIC = ("PointPillars KITTI frames/sec @20k pts, 0.16 m pillars, 248x296 BEV "
+                         "(pointpillars_xyres16_kitti_cyclist_pedestrian)")
+CLASS_NAMES = {"car": ("car",), "ped_cyclist": ("cyclist", "pedestrian")}
 
 
 def gpu_identity(index=0):
@@ -38,10 +44,10 @@ def gpu_identity(index=0):
 
 def pp_frame_check(got, cpu, gpu_candidates, tc, tol=1e-3):
     """GPU frame vs CPU arm on the same points.  Boxes are paired by centre; a pair matches when every box value and the
-    score agree within `tol` (relative, absolute below 1).  Every CPU box without a match is listed with its score and
-    the likely cause, so a difference is explained rather than hidden by a wider tolerance."""
-    gb, gs = got[0].numpy(), got[1].numpy()
-    cb, cs = cpu["boxes"], cpu["scores"]
+    score agree within `tol` (relative, absolute below 1) and the labels are equal.  Every CPU box without a match is
+    listed with its score and the likely cause, so a difference is explained rather than hidden by a wider tolerance."""
+    gb, gs, gl = got[0].numpy(), got[1].numpy(), got[2].numpy()
+    cb, cs, cl = cpu["boxes"], cpu["scores"], cpu["labels"]
     chk = {"pillars_gpu": None, "pillars_cpu": int(cpu["num_voxels"]), "boxes_gpu": int(len(gb)), "boxes_cpu": int(len(cb)),
            "candidates_gpu": int(gpu_candidates), "candidates_cpu": int(cpu["candidates"]), "tolerance": tol}
     used, worst_box, worst_score, unmatched = set(), 0.0, 0.0, []
@@ -50,12 +56,13 @@ def pp_frame_check(got, cpu, gpu_candidates, tc, tol=1e-3):
         if j >= 0 and j not in used:
             eb = float((np.abs(gb[j] - cb[i]) / np.maximum(1.0, np.abs(cb[i]))).max())
             es = float(abs(gs[j] - cs[i]) / max(1.0, abs(cs[i])))
-            if eb <= tol and es <= tol:
+            if eb <= tol and es <= tol and gl[j] == cl[i]:
                 used.add(j)
                 worst_box, worst_score = max(worst_box, eb), max(worst_score, es)
                 continue
         thr = tc["nms_score_threshold"]
-        cause = ("score within %g of the threshold" % tol if abs(cs[i] - thr) <= tol else
+        cause = ("label differs (GPU %d, CPU %d)" % (gl[j], cl[i]) if j >= 0 and j not in used and gl[j] != cl[i] else
+                 "score within %g of the threshold" % tol if abs(cs[i] - thr) <= tol else
                  "candidate count over nms_pre_max_size: top-k boundary" if cpu["candidates"] > tc["nms_pre_max_size"]
                  and i >= len(cb) - 5 else "NMS decision of a box pair at the IoU threshold (or a neighbour of one)")
         unmatched.append({"cpu_row": i, "score": float(cs[i]), "box": [float(v) for v in cb[i]], "cause": cause})
@@ -65,8 +72,8 @@ def pp_frame_check(got, cpu, gpu_candidates, tc, tol=1e-3):
 
 
 def run(args):
-    """PointPillars KITTI-shape inference (BASELINE config 2): synth.C2 frames (20k x 4 points) through
-    pointpillars.PointPillarsHotPath.  `value` = frames/s with --in-flight frames resident in HBM (CUDA-graph replay);
+    """PointPillars KITTI-shape inference (BASELINE config 2): synth.C2 (or synth.C2_PED_CYCLIST) frames (20k x 4 points)
+    through pointpillars.PointPillarsHotPath.  `value` = frames/s with --in-flight frames resident in HBM (CUDA-graph replay);
     e2e = pinned host points in, host boxes out (pipelined and one frame at a time); eager per-stage device times; the
     graph-timed dense stage (backbone + FPN + head) with its algorithmic TFLOP/s; the anchor postprocess alone; the CPU
     arm; a check of the GPU frame against the CPU arm on frame 0."""
@@ -76,14 +83,16 @@ def run(args):
     from paddle3d_b200.ops import sparse_nn as sp
     from paddle3d_b200.ops import voxelize as vox
     from paddle3d_b200.pipeline import CenterPointSweep
-    from paddle3d_b200.pointpillars import PointPillarsHotPath
+    from paddle3d_b200.pointpillars import CONFIG, CONFIG_PED_CYCLIST, PointPillarsHotPath
     if not torch.cuda.is_available():
         raise SystemExit("pointpillars_bench.py needs a CUDA device (no CPU fallback exists)")
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
-    cfg = synth.C2
+    car = args.config == "car"
+    cfg, model_cfg = (synth.C2, CONFIG) if car else (synth.C2_PED_CYCLIST, CONFIG_PED_CYCLIST)
     lanes = max(1, args.in_flight)
-    sweep = CenterPointSweep(lanes, frame_cls=PointPillarsHotPath, cfg=cfg, device=dev, seed=0, bn_gain=BN_GAIN)
+    sweep = CenterPointSweep(lanes, frame_cls=PointPillarsHotPath, cfg=cfg, device=dev, seed=0, bn_gain=BN_GAIN,
+                             model_cfg=model_cfg)
     pipe = sweep.lanes[0]
     m = pipe.model
     frames = frame_pool(cfg, POOL)
@@ -139,9 +148,10 @@ def run(args):
                   "peak_source": "MEASURED_PEAKS.json bf16_tflops" if pk else
                   "H100 SXM data sheet 989 TFLOP/s dense fp16/bf16 at 700 W (not measured)",
                   "note": "algorithmic flops (2 x MACs); the kernel executes 3 fp16 MMAs per product (fp16-pair operands)"}
-    line = {"metric": PP_METRIC, "model": "pointpillars", "value": res["value"], "unit": UNIT, "n_gpus": 1,
-            "steps": args.steps, "warmup": args.warmup, "ms_per_step": res["ms_per_step"], "higher_is_better": True,
-            "frames_in_flight": lanes, "data": "synthetic (synth.lidar_cloud, config C2)",
+    line = {"metric": PP_METRIC if car else PP_PED_CYCLIST_METRIC, "model": "pointpillars", "value": res["value"],
+            "unit": UNIT, "n_gpus": 1, "steps": args.steps, "warmup": args.warmup, "ms_per_step": res["ms_per_step"],
+            "higher_is_better": True, "frames_in_flight": lanes,
+            "data": "synthetic (synth.lidar_cloud, config %s)" % ("C2" if car else "C2_PED_CYCLIST"),
             "dtype": "f16x3 (fp16 hi/lo' pairs, f32 accumulation) dense; fp32 encoder and postprocess",
             "gpu": ident, "clocks": res["clocks"],
             "e2e": {"value": res["e2e_value"], "sync_value": res["e2e_sync_value"], "unit": UNIT,
@@ -150,10 +160,17 @@ def run(args):
             "gpu_launches_per_step": pipe.graph_nodes["kernel"] if pipe.graph_nodes else None,
             "stage_ms_eager": stage, "dense": dense_roof, "anchor_postprocess_ms": ms_post,
             "num_pillars_frame0": int(nv.item())}
+    names = CLASS_NAMES[args.config]
+    if len(names) > 1:
+        labels0 = pipe.infer(host_frames[0])[2].numpy()
+        line["boxes_per_class_frame0"] = {n: int((labels0 == c).sum()) for c, n in enumerate(names)}
     if not args.no_cpu_baseline:
         import oracle
         from oracle.pointpillars import CpuPointPillars
-        cpu = CpuPointPillars(cfg, m.export_numpy(), m.anchors_np, m.corners_np, m.grid, m.mc["test"])
+        from oracle.pointpillars_multiclass import CpuPointPillarsMulticlass
+        cpu = (CpuPointPillars(cfg, m.export_numpy(), m.anchors_np, m.corners_np, m.grid, m.mc["test"]) if car else
+               CpuPointPillarsMulticlass(cfg, m.export_numpy(), m.anchors_np, m.corners_np, m.grid, m.mc["test"],
+                                         m.num_classes))
         t0 = time.perf_counter()
         r = cpu.run(frames[0])
         cpu_s = time.perf_counter() - t0
@@ -165,12 +182,16 @@ def run(args):
         chk = pp_frame_check(got, r, int(pipe.h_counts[0]), m.mc["test"])
         chk["pillars_gpu"] = int(pipe.out["num_voxels"][0].item())
         chk["head_planes"] = rel_errors(pipe.out["planes"].cpu().numpy(), r["planes"])
+        if len(names) > 1:
+            chk["boxes_per_class_cpu"] = {n: int((r["labels"] == c).sum()) for c, n in enumerate(names)}
         line["frame0_check"] = chk
     print(json.dumps(line))
 
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--config", choices=sorted(CLASS_NAMES), default="car",
+                    help="car: pointpillars_xyres16_kitti_car; ped_cyclist: the two-class cyclist / pedestrian model")
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--in-flight", type=int, default=4, help="frames computing concurrently (CenterPointSweep lanes)")
