@@ -373,6 +373,17 @@ int p3d_pillar_feature_net(const float *voxels, const int32_t *num_points_per_vo
                            int out_channels, const float *weight, const float *bn_scale, const float *bn_shift,
                            const float *voxel_size_host, const float *point_cloud_range_host, float *out,
                            p3d_stream_t stream);
+/* PillarFeatureNet with two PFNLayers (feat_channels [2 mid, out], as CenterPoint-pillars uses it), fused into one launch:
+ * the decoration and padding of p3d_pillar_feature_net, then Linear(F + 5 -> mid) + BN + ReLU per row (weight1
+ * [F + 5, mid]), x_max = max over the M rows, Linear over concat([x, x_max]) (weight2 [2 mid, out]: rows 0..mid-1 multiply
+ * x, rows mid..2 mid-1 x_max) + BN + ReLU, max over the rows -> [n, out].  Padding rows take part in both maxima.  Both
+ * BatchNorm1D folded by the caller.  fp32 FMAs throughout.  mid <= 64 and M <= 64, F <= 8 (P3D_ERR_UNSUPPORTED above). */
+int p3d_pillar_feature_net2(const float *voxels, const int32_t *num_points_per_voxel, const int32_t *coors,
+                            const int32_t *num_voxels_dev, int64_t n_cap, int max_points, int num_point_dim,
+                            int mid_channels, const float *weight1, const float *bn_scale1, const float *bn_shift1,
+                            int out_channels, const float *weight2, const float *bn_scale2, const float *bn_shift2,
+                            const float *voxel_size_host, const float *point_cloud_range_host, float *out,
+                            p3d_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
  * anchor_head_postprocess      SECOND v1.5 VoxelNet.predict (the path SSDHead.post_process -> rotate_nms_pcdet ports)

@@ -101,9 +101,12 @@ class SecondTrunk:
         self.deblocks = []
         for ci, co, u in zip(out_channels, fpn_out_channels, upsample_strides):
             # stride > 1 -> Conv2DTranspose k = s; stride 1 -> Conv2D k = 1 with use_conv_for_no_stride, else
-            # Conv2DTranspose k = 1 (second_fpn.py:118-139)
+            # Conv2DTranspose k = 1; stride < 1 -> Conv2D k = stride = round(1 / s) (second_fpn.py:118-139)
             if u > 1:
                 self.deblocks.append(conv(ci, co, u, u, 0, bn_eps=bn3, up=u))
+            elif u < 1:
+                k = int(round(1 / u))
+                self.deblocks.append(conv(ci, co, k, k, 0, bn_eps=bn3))
             else:
                 self.deblocks.append(conv(ci, co, 1, 1, 0, bn_eps=bn3, transposed=not use_conv_for_no_stride))
         self.fpn_channels = int(sum(fpn_out_channels))
@@ -126,15 +129,25 @@ class SecondTrunk:
                 x, _, (b_, oh, ow) = conv(x, shape)
                 shape = (b_, oh, ow, conv.cout)
             feats.append((x, shape))
-        cat, c0, out_hw = None, 0, None
+        out_hws = {self.deblock_out_hw(de, fshape[1], fshape[2]) for (_, fshape), de in zip(feats, self.deblocks)}
+        if len(out_hws) != 1:
+            raise ValueError("the FPN deblocks give feature maps of different sizes %s; the concat needs one size"
+                             % sorted(out_hws))
+        out_hw = out_hws.pop()
+        cat = torch.empty((b * out_hw[0] * out_hw[1], 2 * self.fpn_channels),
+                          dtype=torch.float16 if self.f16 else torch.float32, device=x.device)
+        c0 = 0
         for (f, fshape), de in zip(feats, self.deblocks):
-            if cat is None:
-                out_hw = (fshape[1] * de.up, fshape[2] * de.up)
-                cat = torch.empty((fshape[0] * out_hw[0] * out_hw[1], 2 * self.fpn_channels),
-                                  dtype=torch.float16 if self.f16 else torch.float32, device=x.device)
             de(f, fshape, out_split=cat, out_channels=self.fpn_channels, out_c0=c0)
             c0 += de.cout
         return cat, (b, out_hw[0], out_hw[1], self.fpn_channels)
+
+    @staticmethod
+    def deblock_out_hw(de, h, w):
+        """Output (H, W) of a deblock on an h x w feature map: x up for a transposed conv, the conv geometry otherwise."""
+        if de.up > 1:
+            return h * de.up, w * de.up
+        return (h + 2 * de.padding - de.k) // de.stride + 1, (w + 2 * de.padding - de.k) // de.stride + 1
 
 
 class DenseRPNHead:
@@ -185,7 +198,8 @@ class DenseRPNHead:
             c.init(rng, dev, randomize_bn, bias_value=-2.19 if id(c) in hm_finals else None, bn_gain=bn_gain)
         self._batched = None
         self._first_zc = None
-        if self.f16 and device is not None and self.in_channels % self.bev_depth == 0:
+        # bev_depth 1 (pillars): the (z, c) order is the (c, z) order, the first conv reads the pixel rows as it is
+        if self.f16 and device is not None and self.bev_depth > 1 and self.in_channels % self.bev_depth == 0:
             # second image of the first conv for BEV tensors that arrive as pixel fp16-pair rows straight from the sparse
             # rows (SparseCooTensor.to_pixel_h16): there a pixel's channels are ordered (z, c) = z * C + c, while the
             # reference's to_dense + transpose + reshape (sparse_resnet.py:202-206) orders them (c, z) = c * D + z.  The
@@ -212,10 +226,10 @@ class DenseRPNHead:
             x = dc.nchw_to_pixel_h16(bev) if self.f16 else dc.nchw_to_pixel_split(bev)
             shape = (b, h, w, c)
         else:
-            if not self.f16 or self._first_zc is None:
+            if not self.f16 or (self.bev_depth > 1 and self._first_zc is None):
                 raise ValueError("pixel fp16-pair input needs the f16 head")
             x = bev
-            first = self._first_zc  # channels arrive in (z, c) order
+            first = self._first_zc  # channels arrive in (z, c) order (None with bev_depth 1: the trunk's own first conv)
         cat, (b, H, W, _) = self.trunk(x, shape, first=first)
         s, _, _ = self.shared(cat, (b, H, W, self.fpn_channels))
         return s, (b, H, W, self.shared.cout)
@@ -313,13 +327,14 @@ class DenseRPNHead:
         self._batched.update(self._group_params(finals, cin, device))
         return self._batched
 
-    def calibrate_heatmap_bias(self, bev, score_threshold=0.1, target_frac=0.014):
+    def calibrate_heatmap_bias(self, bev, score_threshold=0.1, target_frac=0.014, shape=None):
         """Seeded random weights give heat maps that hover around the initial bias (sigmoid(-2.19) = 0.1: half of all cells
         would pass a 0.1 score threshold, 16k candidates per task).  A trained CenterPoint fires on a few hundred cells per
         task; SURVEY.md §8d specifies ~1.4 % of cells above the threshold for the synthetic workload.  This shifts the bias of
         every task's heat-map conv so that `target_frac` of the cells of `bev`'s frame score above `score_threshold`
-        (weights stay seeded and are exported unchanged to the CPU arm)."""
-        out = self.forward(bev)
+        (weights stay seeded and are exported unchanged to the CPU arm).  bev: as forward() takes it (with `shape`, pixel
+        fp16-pair rows)."""
+        out = self.forward(bev, shape)
         logit_thr = float(np.log(score_threshold / (1.0 - score_threshold)))
         for t, hs in enumerate(self.heads):
             hm = out["hm"][t].float().amax(dim=1).flatten()

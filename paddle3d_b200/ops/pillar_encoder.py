@@ -1,5 +1,5 @@
 """SURVEY.md §8a-5 / §8f-2 (tests/test_gpu_voxelize.py): PillarFeatureNet (models/voxel_encoders/pillar_encoder.py:
-115-210) with one PFNLayer as one launch over the `hard_voxelize` outputs."""
+115-210) with one PFNLayer (PointPillars) or two (CenterPoint-pillars) as one launch over the `hard_voxelize` outputs."""
 import numpy as np
 import torch
 
@@ -33,4 +33,30 @@ def pillar_feature_net(voxels, num_points_per_voxel, coors, weight, bn_gamma, bn
     check(lib().p3d_pillar_feature_net(ptr(voxels), ptr(npv), ptr(coors), nump, n, m, f, c, ptr(weight), ptr(scale),
                                        ptr(shift), host_floats(voxel_size), host_floats(point_cloud_range), ptr(out),
                                        stream(dev)), "pillar_feature_net")
+    return out
+
+
+def pillar_feature_net2(voxels, num_points_per_voxel, coors, layers, voxel_size, point_cloud_range, num_voxels=None,
+                        folded=None):
+    """PillarFeatureNet with two PFNLayers (CenterPoint-pillars, feat_channels [64, 64]) as one launch.  layers: two dicts
+    of weight / gamma / beta / mean / var / eps, weight [F + 5, mid] then [2 mid, out] on the device.  folded: the two
+    (scale, shift) pairs of fold_bn, to keep host->device copies out of the per-frame path.  Returns [n, out]."""
+    voxels = require_cuda(voxels, "voxels", torch.float32)
+    npv = require_cuda(num_points_per_voxel, "num_points_per_voxel", torch.int32)
+    coors = require_cuda(coors, "coors", torch.int32)
+    w1 = require_cuda(layers[0]["weight"], "layers[0].weight", torch.float32)
+    w2 = require_cuda(layers[1]["weight"], "layers[1].weight", torch.float32)
+    n, m, f = voxels.shape
+    mid, c = w1.shape[1], w2.shape[1]
+    if w1.shape[0] != f + 5 or w2.shape[0] != 2 * mid:
+        raise ValueError("weights must be [F + 5, mid] and [2 mid, out]")
+    dev = voxels.device
+    if folded is None:
+        folded = [fold_bn(l["gamma"], l["beta"], l["mean"], l["var"], l["eps"], dev) for l in layers]
+    (s1, t1), (s2, t2) = folded
+    out = torch.zeros((n, c), dtype=torch.float32, device=dev)
+    nump = ptr(require_cuda(num_voxels, "num_voxels", torch.int32)) if num_voxels is not None else ptr(None)
+    check(lib().p3d_pillar_feature_net2(ptr(voxels), ptr(npv), ptr(coors), nump, n, m, f, mid, ptr(w1), ptr(s1), ptr(t1),
+                                        c, ptr(w2), ptr(s2), ptr(t2), host_floats(voxel_size),
+                                        host_floats(point_cloud_range), ptr(out), stream(dev)), "pillar_feature_net2")
     return out

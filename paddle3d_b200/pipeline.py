@@ -41,11 +41,13 @@ def _count_graph_nodes(raw_graph):
 
 
 class CapturedFrame:
-    """Plumbing shared by the captured hot-path frames (CenterPointHotPath, pointpillars.PointPillarsHotPath): warm-up and
-    CUDA-graph capture of forward_device() on a side stream, the public infer() / infer_many() calls and their pinned
-    result slots.  A subclass sets self.device / self.points / self.stream / self.graph = self.out = None, calls
-    _alloc_host_outputs, and defines forward_device() (returning at least boxes / scores / labels / counts / status, with
-    counts[-1] the number of valid rows) and check_status()."""
+    """Plumbing shared by the captured hot-path frames (CenterPointHotPath, pointpillars.PointPillarsHotPath,
+    centerpoint_pillars.CenterPointPillarsHotPath): warm-up and CUDA-graph capture of forward_device() on a side stream,
+    the public infer() / infer_many() calls and their pinned result slots, and the sweep input (infer_sweeps /
+    infer_stream).  A subclass sets self.device / self.points / self.stream / self.graph = self.out = None (and
+    self.sweep_input = self.ring = None, or calls _init_sweep_input and starts forward_device() with _merge_sweeps()),
+    calls _alloc_host_outputs, and defines forward_device() (returning at least boxes / scores / labels / counts / status,
+    with counts[-1] the number of valid rows) and check_status()."""
 
     def _alloc_host_outputs(self, rows, box_dims, n_counts, n_status):
         self.h_boxes = torch.empty((rows, box_dims), dtype=torch.float32).pin_memory()
@@ -166,84 +168,7 @@ class CapturedFrame:
         if i >= 0:
             yield self._result(i & 1)
 
-    def bytes_per_frame(self):
-        h2d = self.n * self.F * 4
-        d2h = (self.h_boxes.numel() * 4 + self.h_scores.numel() * 4 + self.h_labels.numel() * 8 + self.h_counts.numel() * 4 +
-               self.h_status.numel() * 4)
-        return h2d, d2h
-
-
-def _stream_frames(lanes, ring, items):
-    """One frame per pushed sweep (cloud, global_from_lidar, timestamp) over the captured lanes sharing `ring`: frame j
-    runs on lane j % len(lanes), result slot (j // len(lanes)) & 1 (CenterPointSweep.plan); the H2D of sweep j + 1 runs
-    on the ring's copy stream while frame j computes.  Yields (boxes, scores, labels) per sweep, in order."""
-    import collections
-    L = len(lanes)
-    for p in lanes:
-        if p.graph is None or p.ring is not ring:
-            raise RuntimeError("infer_stream needs captured lanes with sweep input sharing one ring")
-        p.prepare_sweep()
-    ring.reset()
-    pending = collections.deque()
-    for i, (cloud, pose, t) in enumerate(items):
-        li, k = CenterPointSweep._lane_slot(i, L)
-        lane = lanes[li]
-        lane._submit_sweep(ring.push(cloud, pose, t), k)
-        pending.append((lane, k))
-        if len(pending) > L:
-            pl, pk = pending.popleft()
-            yield pl._result(pk)
-    while pending:
-        pl, pk = pending.popleft()
-        yield pl._result(pk)
-
-
-# sweep_input of CenterPointHotPath: ten nuScenes sweeps of 5 values per point, of which x, y, z, intensity are kept
-# and the time lag appended (the 5 columns deploy.preprocess gives the model), close points of earlier sweeps removed
-# within 1 m; slot_cap None = 2 x the mean rows per sweep of num_points
-SWEEP_INPUT = dict(max_sweeps=10, raw_dim=5, use_dim=4, use_time_lag=True, remove_radius=1.0, slot_cap=None)
-
-
-class CenterPointHotPath(CapturedFrame):
-    def __init__(self, cfg=None, device="cuda:0", precision=sp.FP32, seed=0, num_points=None, level_caps=None,
-                 head_seed=0, with_head=False, keep_bev=True, bn_gain=1.0, sweep_input=None, sweep_ring=None):
-        """sweep_input: None (the frame reads merged clouds from self.points) or a dict over SWEEP_INPUT's keys: the
-        frame then starts with the device merge (ops.sweep_merge) of raw sweeps held in a SweepRing into self.points
-        (num_points rows, NaN beyond the merged ones); see infer_sweeps / infer_stream.  sweep_ring: a ring shared
-        with other lanes (CenterPointSweep); default: an own ring of max_sweeps + 1 slots."""
-        self.cfg = dict(cfg or synth.C3)
-        self.device = torch.device(device)
-        self.n = int(num_points or self.cfg["num_points"])
-        self.F = self.cfg["point_dim"]
-        self.test_cfg = dict(synth.CENTERPOINT_TEST_CFG)
-        self.label_off = synth.label_offsets()
-        self.net = SparseResNet3D(self.F, self.cfg["voxel_size"], self.cfg["point_cloud_range"])
-        self.net.init_weight(seed=seed, device=self.device, bn_gain=bn_gain).set_precision(precision)
-        V = self.cfg["max_voxels"]
-        self.net.set_level_caps(level_caps or [3 * V, 3 * V, 2 * V, V])
-        h = synth.centerpoint_head_outputs(head_seed)
-        self.head_host = h
-        self.head = {k: [torch.from_numpy(x).to(self.device) for x in v] for k, v in h.items()}
-        # with_head: run the dense RPN / neck / CenterHead (dense_head.DenseRPNHead, SURVEY §8f-1) on the BEV tensor and
-        # feed ITS outputs to the postprocess instead of the resident synthetic head tensors (parity-green per layer and
-        # as a small network; this whole-frame composition has not been timed yet, hence off by default)
-        self.dense = None
-        if with_head:
-            from .dense_head import DenseRPNHead
-            self.dense = DenseRPNHead(in_channels=128 * 2).init_weight(seed=seed + 1, device=self.device, bn_gain=bn_gain)
-        # keep_bev=False (with the fp16-pair dense head): the sparse rows go straight into the pixel fp16-pair image the RPN
-        # reads; the reference's fp32 NCHW BEV tensor is then not materialised in the frame (bev_nchw() rebuilds it on demand)
-        self.keep_bev = keep_bev or self.dense is None or not self.dense.f16
-        self.points = torch.zeros((self.n, self.F), dtype=torch.float32, device=self.device)  # static input
-        self.graph = None
-        self.out = None
-        self.stream = torch.cuda.Stream(self.device)
-        self.sweep_input = self.ring = None
-        if sweep_input is not None:
-            self._init_sweep_input(dict(SWEEP_INPUT, **sweep_input), sweep_ring)
-        self._alloc_host_outputs(len(self.label_off) * self.test_cfg["nms_post_max_size"], 9, len(self.label_off) + 1,
-                                 5 if self.sweep_input is None else 6)
-
+    # ---- sweep input (sweep_input=...): raw sweeps in a SweepRing, merged on the device inside the captured frame
     def _init_sweep_input(self, si, ring):
         from . import sweep_ring
         from .ops import sweep_merge as sm
@@ -322,14 +247,106 @@ class CenterPointHotPath(CapturedFrame):
         self.stream.synchronize()
         return int(self._n_merged.item())
 
+    def _merge_sweeps(self):
+        """Enqueue the device merge (ops.sweep_merge) of the frame's sweeps in the ring into self.points."""
+        from .ops import sweep_merge as sm
+        si = self.sweep_input
+        sm.merge_into(self.ring.buf, self._sweep_desc, si["max_sweeps"], si["use_dim"], si["use_time_lag"],
+                      si["remove_radius"], self.points, self._n_merged, self._merge_status)
+
+    def _check_merge_status(self, v):
+        """Raise when the merge's status bits report a bad descriptor entry or dropped rows."""
+        if v:
+            from .ops import sweep_merge as sm
+            if v & sm.BAD_ENTRY:
+                raise RuntimeError("sweep merge: a frame descriptor entry named a slot or row count outside the ring")
+            raise RuntimeError("sweep merge: the merged sweeps exceed the point capacity (num_points = %d); rows were "
+                               "dropped" % self.n)
+
+    def bytes_per_frame(self):
+        h2d = self.n * self.F * 4
+        d2h = (self.h_boxes.numel() * 4 + self.h_scores.numel() * 4 + self.h_labels.numel() * 8 + self.h_counts.numel() * 4 +
+               self.h_status.numel() * 4)
+        return h2d, d2h
+
+
+def _stream_frames(lanes, ring, items):
+    """One frame per pushed sweep (cloud, global_from_lidar, timestamp) over the captured lanes sharing `ring`: frame j
+    runs on lane j % len(lanes), result slot (j // len(lanes)) & 1 (CenterPointSweep.plan); the H2D of sweep j + 1 runs
+    on the ring's copy stream while frame j computes.  Yields (boxes, scores, labels) per sweep, in order."""
+    import collections
+    L = len(lanes)
+    for p in lanes:
+        if p.graph is None or p.ring is not ring:
+            raise RuntimeError("infer_stream needs captured lanes with sweep input sharing one ring")
+        p.prepare_sweep()
+    ring.reset()
+    pending = collections.deque()
+    for i, (cloud, pose, t) in enumerate(items):
+        li, k = CenterPointSweep._lane_slot(i, L)
+        lane = lanes[li]
+        lane._submit_sweep(ring.push(cloud, pose, t), k)
+        pending.append((lane, k))
+        if len(pending) > L:
+            pl, pk = pending.popleft()
+            yield pl._result(pk)
+    while pending:
+        pl, pk = pending.popleft()
+        yield pl._result(pk)
+
+
+# sweep_input of CenterPointHotPath: ten nuScenes sweeps of 5 values per point, of which x, y, z, intensity are kept
+# and the time lag appended (the 5 columns deploy.preprocess gives the model), close points of earlier sweeps removed
+# within 1 m; slot_cap None = 2 x the mean rows per sweep of num_points
+SWEEP_INPUT = dict(max_sweeps=10, raw_dim=5, use_dim=4, use_time_lag=True, remove_radius=1.0, slot_cap=None)
+
+
+class CenterPointHotPath(CapturedFrame):
+    def __init__(self, cfg=None, device="cuda:0", precision=sp.FP32, seed=0, num_points=None, level_caps=None,
+                 head_seed=0, with_head=False, keep_bev=True, bn_gain=1.0, sweep_input=None, sweep_ring=None):
+        """sweep_input: None (the frame reads merged clouds from self.points) or a dict over SWEEP_INPUT's keys: the
+        frame then starts with the device merge (ops.sweep_merge) of raw sweeps held in a SweepRing into self.points
+        (num_points rows, NaN beyond the merged ones); see infer_sweeps / infer_stream.  sweep_ring: a ring shared
+        with other lanes (CenterPointSweep); default: an own ring of max_sweeps + 1 slots."""
+        self.cfg = dict(cfg or synth.C3)
+        self.device = torch.device(device)
+        self.n = int(num_points or self.cfg["num_points"])
+        self.F = self.cfg["point_dim"]
+        self.test_cfg = dict(synth.CENTERPOINT_TEST_CFG)
+        self.label_off = synth.label_offsets()
+        self.net = SparseResNet3D(self.F, self.cfg["voxel_size"], self.cfg["point_cloud_range"])
+        self.net.init_weight(seed=seed, device=self.device, bn_gain=bn_gain).set_precision(precision)
+        V = self.cfg["max_voxels"]
+        self.net.set_level_caps(level_caps or [3 * V, 3 * V, 2 * V, V])
+        h = synth.centerpoint_head_outputs(head_seed)
+        self.head_host = h
+        self.head = {k: [torch.from_numpy(x).to(self.device) for x in v] for k, v in h.items()}
+        # with_head: run the dense RPN / neck / CenterHead (dense_head.DenseRPNHead, SURVEY §8f-1) on the BEV tensor and
+        # feed ITS outputs to the postprocess instead of the resident synthetic head tensors (parity-green per layer and
+        # as a small network; this whole-frame composition has not been timed yet, hence off by default)
+        self.dense = None
+        if with_head:
+            from .dense_head import DenseRPNHead
+            self.dense = DenseRPNHead(in_channels=128 * 2).init_weight(seed=seed + 1, device=self.device, bn_gain=bn_gain)
+        # keep_bev=False (with the fp16-pair dense head): the sparse rows go straight into the pixel fp16-pair image the RPN
+        # reads; the reference's fp32 NCHW BEV tensor is then not materialised in the frame (bev_nchw() rebuilds it on demand)
+        self.keep_bev = keep_bev or self.dense is None or not self.dense.f16
+        self.points = torch.zeros((self.n, self.F), dtype=torch.float32, device=self.device)  # static input
+        self.graph = None
+        self.out = None
+        self.stream = torch.cuda.Stream(self.device)
+        self.sweep_input = self.ring = None
+        if sweep_input is not None:
+            self._init_sweep_input(dict(SWEEP_INPUT, **sweep_input), sweep_ring)
+        self._alloc_host_outputs(len(self.label_off) * self.test_cfg["nms_post_max_size"], 9, len(self.label_off) + 1,
+                                 5 if self.sweep_input is None else 6)
+
     # ---- one frame, enqueued on the current stream, device in / device out
     def forward_device(self):
         cfg, tc = self.cfg, self.test_cfg
         si = self.sweep_input
         if si is not None:
-            from .ops import sweep_merge as sm
-            sm.merge_into(self.ring.buf, self._sweep_desc, si["max_sweeps"], si["use_dim"], si["use_time_lag"],
-                          si["remove_radius"], self.points, self._n_merged, self._merge_status)
+            self._merge_sweeps()
         mean, coors, npv, nv = vox.voxelize_mean(self.points, cfg["voxel_size"], cfg["point_cloud_range"],
                                                  cfg["max_points"], cfg["max_voxels"], 0)
         bev, bev_h16 = None, None
@@ -387,12 +404,8 @@ class CenterPointHotPath(CapturedFrame):
         """Raise when the frame's device status word reports dropped work (never a silent wrong result)."""
         st = [int(v) for v in status_host]
         n_levels = len(self.net.level_counters)
-        if len(st) > 1 + n_levels and st[1 + n_levels]:
-            from .ops import sweep_merge as sm
-            if st[1 + n_levels] & sm.BAD_ENTRY:
-                raise RuntimeError("sweep merge: a frame descriptor entry named a slot or row count outside the ring")
-            raise RuntimeError("sweep merge: the merged sweeps exceed the point capacity (num_points = %d); rows were "
-                               "dropped" % self.n)
+        if len(st) > 1 + n_levels:
+            self._check_merge_status(st[1 + n_levels])
         if st[0]:
             raise RuntimeError("sparse backbone: an activation left fp16's range (|x| >= 65504) on the fp16-pair path; "
                                "run this model with precision TF32X3_SPLIT")
