@@ -341,13 +341,52 @@ int p3d_dense_conv2d_f16_pack_weights(const float *weight_tci, int taps, int Cin
  *   (paddle3d/models/transformers/bevdet_transformer.py:230-274): frustum points coor [B, N, D, H, W, 3] fp32 ->
  *   ranks_bev / ranks_depth / ranks_feat sorted by ranks_bev (ties: ascending point index = stable argsort),
  *   interval_starts / interval_lengths; all outputs int32 [B*N*D*H*W] (capacity), counts_dev = {n_kept, n_intervals}.
- *   Entries beyond the counts are zero.  grid_size_host = (X, Y, Z) cells, lower bound / interval per axis (x, y, z).
+ *   Entries beyond the counts are zero, except interval_starts (left unwritten).  grid_size_host = (X, Y, Z) cells,
+ *   lower bound / interval per axis (x, y, z).
  * ------------------------------------------------------------------------------------------- */
 size_t p3d_bev_pool_prepare_workspace_bytes(int64_t num_points);
 int p3d_bev_pool_prepare(const float *coor, int B, int N, int D, int H, int W, const float *grid_lower_bound_host,
                          const float *grid_interval_host, const int32_t *grid_size_host, int32_t *ranks_bev,
                          int32_t *ranks_depth, int32_t *ranks_feat, int32_t *interval_starts, int32_t *interval_lengths,
                          int32_t *counts_dev, void *workspace, size_t workspace_bytes, p3d_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * LSS view transform (LSSViewTransformer, bevdet_transformer.py:147-316, PARITY UNPINNED: no checkout was read; the
+ * restatement follows BEVDet's get_lidar_coor(sensor2ego, ego2global, cam2imgs, post_rots, post_trans, bda) with a 3x3
+ * bda).  One camera descriptor per (b, n), row-major, computed on the host in fp64 and rounded to fp32 once.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct p3d_lss_camera {
+  float inv_post_rot[9]; /* inv(post_rots) */
+  float post_trans[3];
+  float combine[9];      /* sensor2ego[:3, :3] . inv(cam2imgs) */
+  float trans[3];        /* sensor2ego[:3, 3] */
+} p3d_lss_camera;
+
+/* get_lidar_coor fused with voxel_pooling_prepare_v2: the outputs, their capacity B*N*D*H*W, the tie order and the
+ * workspace (p3d_bev_pool_prepare_workspace_bytes(B*N*D*H*W)) are those of p3d_bev_pool_prepare, but the frustum points
+ * are computed in registers instead of read from a coor tensor.  cams [B*N] and bda [B, 9] are device buffers (refresh
+ * them with a copy before each launch and one captured graph serves every calibration); axis_depth [D], axis_x [W],
+ * axis_y [H] fp32 are create_frustum's arange(*depth), linspace(0, W_in - 1, W), linspace(0, H_in - 1, H).
+ * coor (nullable): the ego points as [B, N, D, H, W, 3] fp32, what get_lidar_coor returns. */
+int p3d_lss_prepare(const p3d_lss_camera *cams, const float *bda, const float *axis_depth, const float *axis_x,
+                    const float *axis_y, int B, int N, int D, int H, int W, const float *grid_lower_bound_host,
+                    const float *grid_interval_host, const int32_t *grid_size_host, float *coor, int32_t *ranks_bev,
+                    int32_t *ranks_depth, int32_t *ranks_feat, int32_t *interval_starts, int32_t *interval_lengths,
+                    int32_t *counts_dev, void *workspace, size_t workspace_bytes, p3d_stream_t stream);
+/* Depth softmax + feature permute of view_transform, one launch: logits [BN, D, H, W] -> depth [BN, D, H, W] =
+ * softmax over D (max subtracted, expf, sum in ascending d, one division); tran_feat [BN, C, H, W] -> feat [BN, H, W, C].
+ * D <= 382 and C <= 370 (P3D_ERR_UNSUPPORTED above). */
+int p3d_lss_depth_feat(const float *logits, const float *tran_feat, int BN, int D, int H, int W, int C, float *depth,
+                       float *feat, p3d_stream_t stream);
+/* bev_pool_v2 with the interval count on the device (counts_dev[1], as p3d_bev_pool_prepare / p3d_lss_prepare write it;
+ * capacity = length of the rank arrays), so that it can be captured once for every calibration.  Bit-identical to
+ * p3d_bev_pool_v2 (same kernel).  out is zero-filled here: planar 0 -> [B, Z, Y, X, c], planar 1 -> [B, Z * c, Y, X]
+ * with channel z * c + ch (view_transform's collapse_z layout).  c % 4 == 0, c <= 256, feat / out 16-byte aligned
+ * (P3D_ERR_UNSUPPORTED otherwise). */
+int p3d_bev_pool_v2_dev(const float *depth, const float *feat, const int32_t *ranks_depth, const int32_t *ranks_feat,
+                        const int32_t *ranks_bev, const int32_t *interval_lengths, const int32_t *interval_starts,
+                        const int32_t *counts_dev, int64_t capacity, int c, int B, int Z, int Y, int X, int planar,
+                        float *out, p3d_stream_t stream);
 
 /* Grouped 3x3 output convs of the CenterHead (center_head.py:80-117) as one tensor-core launch with the 9 taps in the
  * GEMM's N dimension (<= 3 output channels per group; a wider conv is split into several groups over the same input

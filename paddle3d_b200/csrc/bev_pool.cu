@@ -74,7 +74,11 @@ __global__ void __launch_bounds__(256) bev_fwd_kernel(int cv, int n_intervals, c
 // float4 channel groups (C <= 256), and the feature rows of the next 8 points are in flight while the current ones are
 // accumulated.  Per channel the fp32 FMA chain runs over the points in index order, exactly as bev_pool_cuda.cu:24-43:
 // results stay bit-identical to the reference kernel.
-template <int G>
+// DEV: the interval count is read from counts_dev[1] (the grid covers an upper bound; warps at or past the count exit), so
+// one captured graph serves every calibration.  PLANAR: the output is [B, Z * C, Y, X] with channel z * C + c, the layout
+// view_transform returns (torch.cat(bev.unbind(dim=2), 1) of the [B, C, Z, Y, X] pool), instead of [B, Z, Y, X, C];
+// yx = Y * X.  The accumulation is the same in every instantiation.
+template <int G, bool DEV = false, bool PLANAR = false>
 __global__ void __launch_bounds__(256) bev_fwd_warp_kernel(int cv, int n_intervals, const float *__restrict__ depth,
                                                            const float *__restrict__ feat,
                                                            const int *__restrict__ ranks_depth,
@@ -82,10 +86,11 @@ __global__ void __launch_bounds__(256) bev_fwd_warp_kernel(int cv, int n_interva
                                                            const int *__restrict__ ranks_bev,
                                                            const int *__restrict__ interval_starts,
                                                            const int *__restrict__ interval_lengths,
-                                                           float *__restrict__ out) {
+                                                           float *__restrict__ out, const int *__restrict__ counts_dev = nullptr,
+                                                           int yx = 0) {
   const int k = static_cast<int>((static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5);
   const int lane = threadIdx.x & 31;
-  if (k >= n_intervals) return;
+  if (k >= (DEV ? __ldg(counts_dev + 1) : n_intervals)) return;
   const int s = interval_starts[k], len = interval_lengths[k];
   const int c = cv * 4;
   bool own[G];
@@ -147,6 +152,20 @@ __global__ void __launch_bounds__(256) bev_fwd_warp_kernel(int cv, int n_interva
     d_cur = d_nxt;
     rf_nxt = rf_nn;
     rd_nxt = rd_nn;
+  }
+  if (PLANAR) {
+    const int rb = __ldg(ranks_bev + s);  // b * Z*Y*X + z * Y*X + (y * X + x): plane (b * Z + z) * C + c
+    float *o = out + static_cast<size_t>(rb / yx) * c * yx + rb % yx;
+#pragma unroll
+    for (int g = 0; g < G; ++g)
+      if (own[g]) {
+        const size_t ch = 4 * (lane + 32 * g);
+        o[ch * yx] = acc[g].x;
+        o[(ch + 1) * yx] = acc[g].y;
+        o[(ch + 2) * yx] = acc[g].z;
+        o[(ch + 3) * yx] = acc[g].w;
+      }
+    return;
   }
   float4 *o = reinterpret_cast<float4 *>(out + static_cast<size_t>(__ldg(ranks_bev + s)) * c);
 #pragma unroll
@@ -220,6 +239,38 @@ extern "C" int p3d_bev_pool_v2(const float *depth, const float *feat, const int3
     bev_fwd_kernel<1><<<div_up(static_cast<long long>(n_intervals) * c, 256), 256, 0, st>>>(
         c, n_intervals, depth, feat, ranks_depth, ranks_feat, ranks_bev, interval_starts, interval_lengths, out);
   }
+  P3D_LAUNCH_CHECK();
+  return P3D_OK;
+}
+
+extern "C" int p3d_bev_pool_v2_dev(const float *depth, const float *feat, const int32_t *ranks_depth,
+                                   const int32_t *ranks_feat, const int32_t *ranks_bev, const int32_t *interval_lengths,
+                                   const int32_t *interval_starts, const int32_t *counts_dev, int64_t capacity, int c, int B,
+                                   int Z, int Y, int X, int planar, float *out, p3d_stream_t stream) {
+  if (!depth || !feat || !ranks_depth || !ranks_feat || !ranks_bev || !interval_lengths || !interval_starts || !counts_dev ||
+      !out || capacity < 0 || c < 1 || B < 1 || Z < 1 || Y < 1 || X < 1 || (planar != 0 && planar != 1))
+    return P3D_ERR_INVALID_ARG;
+  const long long cells = static_cast<long long>(B) * Z * Y * X;
+  if (c % 4 || c > 256 || (reinterpret_cast<uintptr_t>(feat) & 15) || (reinterpret_cast<uintptr_t>(out) & 15) ||
+      capacity > 0x7fffffffll || cells >= 0xffffffffll || static_cast<long long>(Y) * X > 0x7fffffffll)
+    return P3D_ERR_UNSUPPORTED;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  P3D_CUDA_CHECK(cudaMemsetAsync(out, 0, static_cast<size_t>(cells) * c * sizeof(float), st));
+  // every interval is a distinct cell: the count is bounded by the cells as well as by the rank capacity
+  const long long bound = capacity < cells ? capacity : cells;
+  if (bound == 0) return P3D_OK;
+  const int cv = c / 4, yx = Y * X;
+  const unsigned int blocks = div_up(bound * 32, 256);
+  const int n = static_cast<int>(bound);
+#define P3D_BEV_DEV(G, P)                                                                                                  \
+  bev_fwd_warp_kernel<G, true, P><<<blocks, 256, 0, st>>>(cv, n, depth, feat, ranks_depth, ranks_feat, ranks_bev,         \
+                                                          interval_starts, interval_lengths, out, counts_dev, yx)
+  if (cv <= 32) {
+    if (planar) P3D_BEV_DEV(1, true); else P3D_BEV_DEV(1, false);
+  } else {
+    if (planar) P3D_BEV_DEV(2, true); else P3D_BEV_DEV(2, false);
+  }
+#undef P3D_BEV_DEV
   P3D_LAUNCH_CHECK();
   return P3D_OK;
 }

@@ -1,4 +1,5 @@
 """`paddle3d.ops.bev_pool_v2` mirror — op `bev_pool_v2` (paddle3d/ops/bev_pool_v2/bev_pool.cc:111-118)."""
+import numpy as np
 import torch
 
 from .._lib import check, lib
@@ -53,3 +54,98 @@ def trim(prepared):
     if k == 0 or m == 0:
         return None, None, None, None, None
     return rb[:k], rd[:k], rf[:k], st[:m], ln[:m]
+
+
+# ---------------------------------------------------------------------------------------------- LSS view transform
+CAM_FLOATS = 24  # struct p3d_lss_camera: inv_post_rot[9], post_trans[3], combine[9], trans[3]
+
+
+def pack_cameras(sensor2ego, cam2imgs, post_rots, post_trans, bda):
+    """Host camera descriptor of p3d_lss_prepare: fp32 [B*N*24 + B*9] = the p3d_lss_camera entries of every (b, n), then
+    bda [B, 3, 3] row-major.  sensor2ego [B, N, 4, 4], cam2imgs / post_rots [B, N, 3, 3], post_trans [B, N, 3], bda
+    [B, 3, 3] (numpy or CPU tensors); the inverses and combine = sensor2ego[:3, :3] . inv(cam2imgs) are taken in fp64 and
+    every entry is rounded to fp32 once."""
+    s2e = _f64(sensor2ego)
+    B, N = s2e.shape[:2]
+    cams = np.empty((B, N, CAM_FLOATS), np.float64)
+    cams[..., 0:9] = np.linalg.inv(_f64(post_rots)).reshape(B, N, 9)
+    cams[..., 9:12] = _f64(post_trans).reshape(B, N, 3)
+    cams[..., 12:21] = (s2e[..., :3, :3] @ np.linalg.inv(_f64(cam2imgs))).reshape(B, N, 9)
+    cams[..., 21:24] = s2e[..., :3, 3]
+    return np.concatenate([cams.reshape(-1), _f64(bda).reshape(B * 9)]).astype(np.float32)
+
+
+def unpack_cameras(desc, B, N):
+    """Inverse of pack_cameras: dict of fp32 inv_post_rots / combine [B, N, 3, 3], post_trans / trans [B, N, 3],
+    bda [B, 3, 3]."""
+    desc = np.asarray(desc, np.float32)
+    cams = desc[:B * N * CAM_FLOATS].reshape(B, N, CAM_FLOATS)
+    return dict(inv_post_rots=cams[..., 0:9].reshape(B, N, 3, 3), post_trans=cams[..., 9:12],
+                combine=cams[..., 12:21].reshape(B, N, 3, 3), trans=cams[..., 21:24],
+                bda=desc[B * N * CAM_FLOATS:].reshape(B, 3, 3))
+
+
+def _f64(a):
+    return np.asarray(a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else a, np.float64)
+
+
+def lss_prepare(desc, axis_depth, axis_x, axis_y, B, N, grid_lower_bound, grid_interval, grid_size, with_coor=False):
+    """get_lidar_coor + voxel_pooling_prepare_v2 in one pass (p3d_lss_prepare), no host sync.  desc: device fp32 buffer
+    from pack_cameras; axis_*: device fp32 frustum axes [D] / [W] / [H].  Returns (ranks_bev, ranks_depth, ranks_feat,
+    interval_starts, interval_lengths, counts) as voxel_pooling_prepare_v2 does, plus coor [B, N, D, H, W, 3] with_coor."""
+    from .._lib import host_floats, host_ints
+    from .._mem import workspace
+    desc = require_cuda(desc, "desc", torch.float32)
+    ad = require_cuda(axis_depth, "axis_depth", torch.float32)
+    ax = require_cuda(axis_x, "axis_x", torch.float32)
+    ay = require_cuda(axis_y, "axis_y", torch.float32)
+    D, H, W = ad.numel(), ay.numel(), ax.numel()
+    if desc.numel() != B * N * CAM_FLOATS + B * 9:
+        raise ValueError("lss_prepare: descriptor has %d floats, want %d" % (desc.numel(), B * N * CAM_FLOATS + B * 9))
+    n = B * N * D * H * W
+    dev = desc.device
+    outs = [torch.empty((n,), dtype=torch.int32, device=dev) for _ in range(5)]
+    counts = torch.empty((2,), dtype=torch.int32, device=dev)
+    coor = torch.empty((B, N, D, H, W, 3), dtype=torch.float32, device=dev) if with_coor else None
+    L = lib()
+    wsb = L.p3d_bev_pool_prepare_workspace_bytes(n)
+    ws = workspace(wsb, dev, "bev_pool_prepare")
+    bda = desc[B * N * CAM_FLOATS:]
+    check(L.p3d_lss_prepare(ptr(desc), ptr(bda), ptr(ad), ptr(ax), ptr(ay), B, N, D, H, W, host_floats(grid_lower_bound),
+                            host_floats(grid_interval), host_ints(grid_size), ptr(coor), ptr(outs[0]), ptr(outs[1]),
+                            ptr(outs[2]), ptr(outs[3]), ptr(outs[4]), ptr(counts), ptr(ws), wsb, stream(dev)), "lss_prepare")
+    res = (outs[0], outs[1], outs[2], outs[3], outs[4], counts)
+    return res + (coor,) if with_coor else res
+
+
+def lss_depth_feat(logits, tran_feat, depth=None, feat=None):
+    """Depth softmax + permute (p3d_lss_depth_feat): logits [BN, D, H, W], tran_feat [BN, C, H, W] fp32 ->
+    (depth [BN, D, H, W] = softmax over D, feat [BN, H, W, C]); depth / feat: optional preallocated outputs."""
+    logits = require_cuda(logits, "logits", torch.float32)
+    tran_feat = require_cuda(tran_feat, "tran_feat", torch.float32)
+    BN, D, H, W = logits.shape
+    C = tran_feat.shape[1]
+    if tuple(tran_feat.shape) != (BN, C, H, W):
+        raise ValueError("lss_depth_feat: tran_feat %s does not match logits %s" % (tuple(tran_feat.shape), tuple(logits.shape)))
+    depth = torch.empty_like(logits) if depth is None else depth
+    feat = torch.empty((BN, H, W, C), dtype=torch.float32, device=logits.device) if feat is None else feat
+    check(lib().p3d_lss_depth_feat(ptr(logits), ptr(tran_feat), BN, D, H, W, C, ptr(depth), ptr(feat), stream(logits.device)),
+          "lss_depth_feat")
+    return depth, feat
+
+
+def bev_pool_v2_dev(depth, feat, prepared, bev_feat_shape, planar=False, out=None):
+    """bev_pool_v2 with the interval count read on the device (p3d_bev_pool_v2_dev): `prepared` as voxel_pooling_prepare_v2
+    / lss_prepare return it (untrimmed); bev_feat_shape (B, Z, Y, X, C).  planar=False -> [B, Z, Y, X, C];
+    planar=True -> [B, Z * C, Y, X] (view_transform's layout, channel z * C + c)."""
+    depth = require_cuda(depth, "depth", torch.float32)
+    feat = require_cuda(feat, "feat", torch.float32)
+    rb, rd, rf, st, ln, counts = prepared[:6]
+    B, Z, Y, X, C = [int(s) for s in bev_feat_shape]
+    if out is None:
+        shape = (B, Z * C, Y, X) if planar else (B, Z, Y, X, C)
+        out = torch.empty(shape, dtype=torch.float32, device=feat.device)
+    check(lib().p3d_bev_pool_v2_dev(ptr(depth), ptr(feat), ptr(rd), ptr(rf), ptr(rb), ptr(ln), ptr(st), ptr(counts),
+                                    rb.numel(), C, B, Z, Y, X, int(bool(planar)), ptr(out), stream(feat.device)),
+          "bev_pool_v2_dev")
+    return out

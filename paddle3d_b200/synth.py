@@ -226,3 +226,63 @@ def bev_pool_inputs(seed, n_cams=6, D=118, H=16, W=44, C=80, grid=(128, 128, 1),
 def kaiming_uniform(rng, shape, fan_in):
     bound = math.sqrt(6.0 / fan_in) / math.sqrt(1 + 5.0)  # a = sqrt(5), as reset_parameters does
     return rng.uniform(-bound, bound, size=shape).astype(np.float32)
+
+
+# LSSViewTransformer grids (BEVDet-R50's 0.8 m grid and BASELINE config 4's 0.5 m grid; D = 118 depth bins of 0.5 m)
+LSS_BEVDET = dict(x=[-51.2, 51.2, 0.8], y=[-51.2, 51.2, 0.8], z=[-5.0, 3.0, 8.0], depth=[1.0, 60.0, 0.5])
+LSS_C4 = dict(LSS_BEVDET, x=[-50.0, 50.0, 0.5], y=[-50.0, 50.0, 0.5])
+LSS_INPUT_SIZE, LSS_DOWNSAMPLE, LSS_CHANNELS = (256, 704), 16, 80
+
+
+def _rot(axis, a):
+    c, s = np.cos(a), np.sin(a)
+    i, j = [(1, 2), (2, 0), (0, 1)][axis]
+    m = np.eye(3)
+    m[i, i], m[i, j], m[j, i], m[j, j] = c, -s, s, c
+    return m
+
+
+def camera_rig(seed, B=1, n_cams=6, bda=True):
+    """Camera matrices of a nuScenes-like rig in the form BEVDet's LSSViewTransformer.get_lidar_coor takes them, float32:
+    sensor2ego / ego2global [B, N, 4, 4], cam2imgs / post_rots [B, N, 3, 3], post_trans [B, N, 3], bda [B, 3, 3].
+    Pinhole intrinsics at the 1600 x 900 scale (fx = fy = 1266, seeded principal point near the centre); cameras at
+    60-degree yaw steps (z forward, x right, y down) with a seeded pitch / roll of up to 2 degrees and seeded mounting
+    offsets; image augmentation = resize by 0.44 to 704 x 396 and a crop of the bottom 256 rows; bda = a seeded flip +
+    rotation of up to 22.5 degrees (bda=True) or the identity."""
+    rng = np.random.default_rng(seed)
+    N = n_cams
+    s2e = np.zeros((B, N, 4, 4))
+    e2g = np.zeros((B, N, 4, 4))
+    k = np.zeros((B, N, 3, 3))
+    prot = np.zeros((B, N, 3, 3))
+    ptr = np.zeros((B, N, 3))
+    bd = np.zeros((B, 3, 3))
+    # camera axes in the ego frame (x forward, y left, z up): x_cam = right, y_cam = down, z_cam = forward
+    base = np.array([[0.0, 0.0, 1.0], [-1.0, 0.0, 0.0], [0.0, -1.0, 0.0]])
+    for b in range(B):
+        for n in range(N):
+            yaw = n * np.pi / 3 + rng.uniform(-0.02, 0.02)
+            r = _rot(2, yaw) @ _rot(1, rng.uniform(-0.035, 0.035)) @ _rot(0, rng.uniform(-0.035, 0.035)) @ base
+            s2e[b, n, :3, :3] = r
+            s2e[b, n, :3, 3] = [1.0 * np.cos(yaw) + rng.uniform(-0.1, 0.1), 0.5 * np.sin(yaw) + rng.uniform(-0.1, 0.1),
+                                1.5 + rng.uniform(-0.05, 0.05)]
+            s2e[b, n, 3, 3] = 1.0
+            e2g[b, n] = np.eye(4)
+            e2g[b, n, :3, :3] = _rot(2, 0.3 * b + 0.1)
+            e2g[b, n, :3, 3] = [600.0 + b, 1600.0, 0.0]
+            k[b, n] = [[1266.0, 0.0, 800.0 + rng.uniform(-20, 20)], [0.0, 1266.0, 450.0 + rng.uniform(-10, 10)], [0, 0, 1]]
+            prot[b, n] = np.diag([0.44, 0.44, 1.0])
+            ptr[b, n] = [0.0, -(900 * 0.44 - 256), 0.0]
+        if bda:
+            flip = np.diag([-1.0 if rng.uniform() < 0.5 else 1.0, -1.0 if rng.uniform() < 0.5 else 1.0, 1.0])
+            bd[b] = flip @ _rot(2, rng.uniform(-np.pi / 8, np.pi / 8))
+        else:
+            bd[b] = np.eye(3)
+    f = np.float32
+    return dict(sensor2ego=s2e.astype(f), ego2global=e2g.astype(f), cam2imgs=k.astype(f), post_rots=prot.astype(f),
+                post_trans=ptr.astype(f), bda=bd.astype(f))
+
+
+def lss_mats(rig):
+    """(sensor2ego, cam2imgs, post_rots, post_trans, bda) of a camera_rig, the order LSSHotPath takes them in."""
+    return rig["sensor2ego"], rig["cam2imgs"], rig["post_rots"], rig["post_trans"], rig["bda"]

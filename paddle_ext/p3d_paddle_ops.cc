@@ -594,3 +594,84 @@ PD_BUILD_OP(p3d_bev_pool_prepare)
     .SetKernelFn(PD_KERNEL(p3d_bev_pool_prepare_op))
     .SetInferShapeFn(PD_INFER_SHAPE(PrepInferShape))
     .SetInferDtypeFn(PD_INFER_DTYPE(PrepInferDtype));
+
+// LSSViewTransformer.get_lidar_coor fused with voxel_pooling_prepare_v2: CAMS [B*N*24 + B*9] fp32 (the p3d_lss_camera
+// entries, then bda [B, 3, 3]) and the frustum axes DEPTH [D], XS [W], YS [H] -> the outputs of p3d_bev_pool_prepare plus
+// COOR: [B, N, D, H, W, 3] with with_coor (get_lidar_coor), otherwise an empty [0] tensor and no coordinate is written.
+std::vector<paddle::Tensor> p3d_lss_prepare_op(const paddle::Tensor &cams, const paddle::Tensor &axis_d,
+                                               const paddle::Tensor &axis_x, const paddle::Tensor &axis_y, int B, int N,
+                                               const std::vector<float> &lower, const std::vector<float> &interval,
+                                               const std::vector<int> &grid_size, bool with_coor) {
+  P3D_CHECK_GPU(cams);
+  const int D = axis_d.shape()[0], W = axis_x.shape()[0], H = axis_y.shape()[0];
+  const int64_t n = static_cast<int64_t>(B) * N * D * H * W;
+  std::vector<paddle::Tensor> out;
+  for (int i = 0; i < 5; ++i) out.push_back(paddle::empty({n}, paddle::DataType::INT32, paddle::GPUPlace()));
+  out.push_back(paddle::empty({2}, paddle::DataType::INT32, paddle::GPUPlace()));
+  if (with_coor)
+    out.push_back(paddle::empty({B, N, D, H, W, 3}, paddle::DataType::FLOAT32, paddle::GPUPlace()));
+  else
+    out.push_back(paddle::empty({0}, paddle::DataType::FLOAT32, paddle::GPUPlace()));
+  const size_t ws_bytes = p3d_bev_pool_prepare_workspace_bytes(n);
+  auto ws = workspace(ws_bytes);
+  const float *c = cams.data<float>();
+  P3D_CALL(p3d_lss_prepare(reinterpret_cast<const p3d_lss_camera *>(c), c + static_cast<int64_t>(B) * N * 24,
+                           axis_d.data<float>(), axis_x.data<float>(), axis_y.data<float>(), B, N, D, H, W, lower.data(),
+                           interval.data(), grid_size.data(), with_coor ? out[6].data<float>() : nullptr, out[0].data<int>(), out[1].data<int>(),
+                           out[2].data<int>(), out[3].data<int>(), out[4].data<int>(), out[5].data<int>(), ws.data<uint8_t>(),
+                           ws_bytes, cams.stream()));
+  return out;
+}
+std::vector<std::vector<int64_t>> LssPrepInferShape(std::vector<int64_t> c, std::vector<int64_t> d, std::vector<int64_t> x,
+                                                    std::vector<int64_t> y, int B, int N, const std::vector<float> &lower,
+                                                    const std::vector<float> &interval, const std::vector<int> &grid_size,
+                                                    bool with_coor) {
+  const int64_t n = static_cast<int64_t>(B) * N * d[0] * y[0] * x[0];
+  const std::vector<int64_t> coor = with_coor ? std::vector<int64_t>{B, N, d[0], y[0], x[0], 3} : std::vector<int64_t>{0};
+  return {{n}, {n}, {n}, {n}, {n}, {2}, coor};
+}
+std::vector<paddle::DataType> LssPrepInferDtype(paddle::DataType c, paddle::DataType d, paddle::DataType x, paddle::DataType y) {
+  return {paddle::DataType::INT32, paddle::DataType::INT32, paddle::DataType::INT32, paddle::DataType::INT32,
+          paddle::DataType::INT32, paddle::DataType::INT32, paddle::DataType::FLOAT32};
+}
+PD_BUILD_OP(p3d_lss_prepare)
+    .Inputs({"CAMS", "DEPTH", "XS", "YS"})
+    .Outputs({"RANKS_BEV", "RANKS_DEPTH", "RANKS_FEAT", "INTERVAL_STARTS", "INTERVAL_LENGTHS", "COUNTS", "COOR"})
+    .Attrs({"B: int", "N: int", "grid_lower_bound: std::vector<float>", "grid_interval: std::vector<float>",
+            "grid_size: std::vector<int>", "with_coor: bool"})
+    .SetKernelFn(PD_KERNEL(p3d_lss_prepare_op))
+    .SetInferShapeFn(PD_INFER_SHAPE(LssPrepInferShape))
+    .SetInferDtypeFn(PD_INFER_DTYPE(LssPrepInferDtype));
+
+// bev_pool_v2 with the interval count on the device (COUNTS from p3d_bev_pool_prepare / p3d_lss_prepare) into
+// view_transform's [B, Z * C, Y, X] layout; bzyx = (B, Z, Y, X).
+std::vector<paddle::Tensor> p3d_bev_pool_v2_dev_op(const paddle::Tensor &depth, const paddle::Tensor &feat,
+                                                   const paddle::Tensor &ranks_depth, const paddle::Tensor &ranks_feat,
+                                                   const paddle::Tensor &ranks_bev, const paddle::Tensor &interval_lengths,
+                                                   const paddle::Tensor &interval_starts, const paddle::Tensor &counts,
+                                                   const std::vector<int> &bzyx) {
+  P3D_CHECK_GPU(feat);
+  const int c = feat.shape()[feat.shape().size() - 1];
+  auto out = paddle::empty({bzyx[0], bzyx[1] * c, bzyx[2], bzyx[3]}, paddle::DataType::FLOAT32, paddle::GPUPlace());
+  P3D_CALL(p3d_bev_pool_v2_dev(depth.data<float>(), feat.data<float>(), ranks_depth.data<int>(), ranks_feat.data<int>(),
+                               ranks_bev.data<int>(), interval_lengths.data<int>(), interval_starts.data<int>(),
+                               counts.data<int>(), ranks_bev.shape()[0], c, bzyx[0], bzyx[1], bzyx[2], bzyx[3], 1,
+                               out.data<float>(), feat.stream()));
+  return {out};
+}
+std::vector<std::vector<int64_t>> PoolDevInferShape(std::vector<int64_t> d, std::vector<int64_t> f, std::vector<int64_t> a,
+                                                    std::vector<int64_t> b, std::vector<int64_t> e, std::vector<int64_t> g,
+                                                    std::vector<int64_t> h, std::vector<int64_t> k, const std::vector<int> &bzyx) {
+  return {{bzyx[0], bzyx[1] * f.back(), bzyx[2], bzyx[3]}};
+}
+std::vector<paddle::DataType> PoolDevInferDtype(paddle::DataType d, paddle::DataType f, paddle::DataType a, paddle::DataType b,
+                                                paddle::DataType e, paddle::DataType g, paddle::DataType h, paddle::DataType k) {
+  return {paddle::DataType::FLOAT32};
+}
+PD_BUILD_OP(p3d_bev_pool_v2_dev)
+    .Inputs({"DEPTH", "FEAT", "RANKS_DEPTH", "RANKS_FEAT", "RANKS_BEV", "INTERVAL_LENGTHS", "INTERVAL_STARTS", "COUNTS"})
+    .Outputs({"OUT"})
+    .Attrs({"bzyx: std::vector<int>"})
+    .SetKernelFn(PD_KERNEL(p3d_bev_pool_v2_dev_op))
+    .SetInferShapeFn(PD_INFER_SHAPE(PoolDevInferShape))
+    .SetInferDtypeFn(PD_INFER_DTYPE(PoolDevInferDtype));
