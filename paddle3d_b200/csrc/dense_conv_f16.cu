@@ -22,9 +22,11 @@
 //               a weight ring (NB) filled ahead of the consumers across work items (TMA / cp.async.bulk onto "full"
 //               mbarriers, refilling a slot once its "empty" mbarrier says both consumers are done with it); consumer
 //               warpgroup c = 1, 2 computes rows 64(c-1) .. 64(c-1)+63 of every M tile with one wgmma group in flight
-//               behind the one being issued.  At the end of an item it parks hi + cross * 2^-11 in its fp32 staging
-//               tile and starts the next item; warps 1-3 of warpgroup 0 (the epilogue warps) apply scale / shift /
-//               ReLU, split and store from there, so the tensor pipe does not idle through the epilogue.
+//               behind the one being issued.  At the end of an item it hands its rows to warps 1-3 of warpgroup 0 (the
+//               epilogue warps) through its staging tile and starts the next item, so the tensor pipe does not idle
+//               through the stores.  A launch that writes only the pixel H16 image stages finished fp16-pair rows
+//               (scale / shift / ReLU and the split done by the consumers) that one epilogue thread stores with TMA;
+//               a launch with fp32 planes stages hi + cross * 2^-11 in fp32 and the epilogue warps do the rest.
 #include <cuda.h>
 #include <cuda_fp16.h>
 
@@ -74,6 +76,10 @@ struct Cfg {
   static constexpr int SP = N + 8;                                           // staging row pitch (floats)
   static constexpr int STG_WG = MT * 64 * SP;                                // floats per consumer warpgroup
   static constexpr int STG_BYTES = 2 * STG_WG * 4;
+  // Without fp32 planes the same tile holds the fp16-pair rows instead: one 8 KB TMA block per (M tile, 32-channel group)
+  // and after them two buffers of the item's N scale and N shift values
+  static constexpr int PAIR_BLK = 64 * 128, PAIR_BYTES = MT * (N / 32) * PAIR_BLK;
+  static_assert(PAIR_BYTES + 2 * 2 * N * 4 <= STG_WG * 4 && STG_WG * 4 % 1024 == 0, "pair tile inside the staging tile");
   static constexpr int AVAIL = kSmemBudget - STG_BYTES;
   // TAP mode: every step needs a new activation buffer, so both rings get the same depth; HALO: 2 buffers
   static constexpr int NA_TAP_RAW = AVAIL / (A_BYTES + B_BYTES);
@@ -101,6 +107,31 @@ __device__ __forceinline__ void tma_tile4d(uint32_t dst, const CUtensorMap *map,
       "l"(reinterpret_cast<uint64_t>(map)), "r"(c), "r"(x), "r"(y), "r"(b), "r"(bar)
       : "memory");
 }
+// TMA tensor stores shared -> global into the issuing thread's bulk async-group
+__device__ __forceinline__ void tma_store4d(const CUtensorMap *map, uint32_t src, int c, int x, int y, int b) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(map)),
+               "r"(src), "r"(c), "r"(x), "r"(y), "r"(b)
+               : "memory");
+}
+__device__ __forceinline__ void tma_store5d(const CUtensorMap *map, uint32_t src, int c, int d1, int d2, int d3, int d4) {
+  asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(map)),
+               "r"(src), "r"(c), "r"(d1), "r"(d2), "r"(d3), "r"(d4)
+               : "memory");
+}
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v));
+}
+__device__ __forceinline__ float2 ld_shared_f2(uint32_t addr) {
+  float2 v;
+  asm("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr));  // ordered by its address only
+  return v;
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// .read: the shared-memory sources of the committed stores may be overwritten; without: the writes are done
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 struct Item {
   int nt, tap0, tx0, ty0, b;
 };
@@ -116,7 +147,9 @@ enum TraceField {
                                         // (writing the staging tile), less kTrStageFree
   kTrStageFree = kTrEpi + 2,            // per consumer warpgroup: waiting for the epilogue warps to free its staging tile
   kTrAEmpty = kTrStageFree + 2, kTrBEmpty,  // producer: waiting on activation / weight "empty"
-  kTrEwWait, kTrEwBusy,                 // epilogue warp 1: waiting on "staged"; scale / shift / ReLU / split and stores
+  kTrEwWait, kTrEwBusy,                 // epilogue thread 0: waiting on "staged"; from "staged" to "freed" (fp32
+                                        // staging: scale / shift / ReLU / split and stores; pair tile: the TMA stores
+                                        // until their shared-memory reads are done)
   kTrFields
 };
 #ifdef P3D_DENSE_TRACE
@@ -245,9 +278,77 @@ __device__ __forceinline__ void epilogue_warps(const Params &p, const float *stg
   if (et == 0) tr.flush(0);
 }
 
+// Pair-tile epilogue (launches without fp32 planes).  The consumers have applied scale / shift / ReLU and the split and
+// staged fp16-pair rows in the layout a SWIZZLE_128B TMA box lands in: one 8 KB block per (M tile, 32-channel group) of
+// 64 rows x 128 bytes, row = pixel y * 8 + x of the warpgroup's 8 x 8 pixels, 16-byte chunk XOR-ed with row & 7.  Thread
+// et = 0 stores every block whose 32 channels the layer owns with TMA (a transposed conv: one box per input-pixel row,
+// rows below the image skipped so that a ragged tile does not spill into the next batch image) and hands the tile back
+// once the stores have read it.  A box over a group the layer owns in part (out_c0 % 32 == 16, or the last group of a
+// partly used N tile) would overwrite the neighbour's channels: all 96 threads copy the owned 32-byte hi and lo' halves
+// of such blocks with ordinary stores.
+template <int N, int MT>
+__device__ __forceinline__ void epilogue_pairs(const Params &p, const CUtensorMap *out_map, const uint8_t *tiles, int tile_bytes,
+                                               unsigned long long *staged, unsigned long long *freed, long long n_items,
+                                               int th, int et) {
+  constexpr int NQ = N / 32, BLK = 64 * 128;
+  const bool lead = et == 0;
+  const bool whole = p.out_c0 % 32 == 0;  // output groups line up with the N tile's 32-channel groups
+  Trace tr;
+  for (long long idx = 0; idx < n_items; ++idx) {
+    const Item im = decode(idx, p, th);
+    const int dy = p.up > 1 ? im.tap0 / p.up : 0, dx = p.up > 1 ? im.tap0 % p.up : 0;
+    for (int c = 0; c < 2; ++c) {
+      long long t0 = tr.now();
+      mbar_wait(smem_u32(staged + c), static_cast<uint32_t>(idx & 1));
+      tr.add(kTrEwWait, t0);
+      t0 = tr.now();
+      for (int blk = 0; blk < MT * NQ; ++blk) {
+        const int ch0 = im.nt * N + (blk % NQ) * 32, iy0 = im.ty0 + (blk / NQ) * kTH + c * 8;
+        if (ch0 >= p.cout) continue;
+        const uint8_t *src = tiles + c * tile_bytes + blk * BLK;
+        if (whole && ch0 + 32 <= p.cout) {
+          if (!lead) continue;
+          const int hc = 2 * (p.out_c0 + ch0);  // first half of the group in a pixel row
+          if (p.up == 1) {
+            tma_store4d(out_map, smem_u32(src), hc, im.tx0, iy0, im.b);
+          } else {
+            for (int y = 0; y < 8 && iy0 + y < p.oH; ++y)
+              tma_store5d(out_map, smem_u32(src + y * 1024), hc, dx, im.tx0, dy, im.b * p.oH + iy0 + y);
+          }
+          continue;
+        }
+        for (int u = et; u < 128; u += kEpiThreads) {  // (row, 16-channel half)
+          const int r = u >> 1, h = u & 1, iy = iy0 + (r >> 3), ix = im.tx0 + (r & 7);
+          if (ch0 + 16 * h >= p.cout || iy >= p.oH || ix >= p.oW) continue;
+          const int oc = p.out_c0 + ch0 + 16 * h, Y = iy * p.up + dy, X = ix * p.up + dx;
+          uint8_t *op = p.out_h16 + ((static_cast<size_t>(im.b) * p.out_H + Y) * p.out_W + X) * (4 * static_cast<size_t>(p.out_C)) +
+                        (oc / 32) * 128 + (oc % 32) * 2;
+          const uint8_t *row = src + r * 128;
+#pragma unroll
+          for (int k = 0; k < 2; ++k) {
+            *reinterpret_cast<uint4 *>(op + 16 * k) = *reinterpret_cast<const uint4 *>(row + (((2 * h + k) ^ (r & 7)) << 4));
+            *reinterpret_cast<uint4 *>(op + 64 + 16 * k) = *reinterpret_cast<const uint4 *>(row + (((4 + 2 * h + k) ^ (r & 7)) << 4));
+          }
+        }
+      }
+      if (lead) {
+        bulk_commit();
+        bulk_wait_read();
+      }
+      mbar_arrive(smem_u32(freed + c));
+      tr.add(kTrEwBusy, t0);
+    }
+  }
+  if (lead) {
+    bulk_wait_all();  // the image is written before this grid counts as complete for the next layer
+    tr.flush(0);
+  }
+}
+
 template <int N, int MT, bool HALO>
 __global__ void __launch_bounds__(kDenseThreads, 1)
-    dense_conv_f16_kernel(const __grid_constant__ CUtensorMap in_map, const Params p) {
+    dense_conv_f16_kernel(const __grid_constant__ CUtensorMap in_map, const __grid_constant__ CUtensorMap out_map,
+                          const Params p) {
   using C = Cfg<N, MT, HALO>;
   constexpr int TH = kTH * MT;  // output tile height
   constexpr int H = N / 2;      // accumulator registers of the hi products of one M tile; the cross products follow
@@ -287,6 +388,7 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
   const uint32_t b_ring = a_ring + C::NA * C::A_BYTES;
   // staging tiles of the two consumer warpgroups, after the weight ring
   float *const stg = reinterpret_cast<float *>(smem + C::NA * C::A_BYTES + C::NB * C::B_BYTES);
+  const bool pairs = p.out_nchw == nullptr;  // stage fp16-pair rows for TMA stores (epilogue_pairs)
   const int G = p.Cin / 32;
   // steps / activation units per item: HALO: one unit per group, 9 taps each; TAP: one unit per (tap, group)
   const int taps_item = p.up > 1 ? 1 : p.taps;
@@ -299,7 +401,11 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
   if (wg == 0) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(C::P_REGS));
     if (tid >= 32) {
-      epilogue_warps<N, MT>(p, stg, s_bar + kSS, s_bar + kSF, n_items, TH, tid - 32);
+      if (pairs)
+        epilogue_pairs<N, MT>(p, &out_map, reinterpret_cast<const uint8_t *>(stg), C::STG_WG * 4, s_bar + kSS, s_bar + kSF,
+                              n_items, TH, tid - 32);
+      else
+        epilogue_warps<N, MT>(p, stg, s_bar + kSS, s_bar + kSF, n_items, TH, tid - 32);
       return;
     }
     // ------------------------------------------------------------------------------------------ producer
@@ -353,11 +459,23 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
   };
   uint32_t a_slot = 0, a_ph = 0, b_slot = 0, b_ph = 0;
   float acc[C::ACC];
+  bool ovf = false;  // fp16 range overflow of the pair tile (status bit 0)
   Trace tr;
   const long long t_start = tr.now();
   for (long long idx = 0; idx < n_items; ++idx) {
 #pragma unroll
     for (int i = 0; i < C::ACC; ++i) acc[i] = 0.f;
+    const Item im = decode(idx, p, TH);
+    // pair tile: the item's scale / shift columns are staged in shared memory while the K loop runs, in one of two
+    // buffers (item parity) after the warpgroup's pair blocks; its epilogue reads them after a warpgroup barrier
+    const uint32_t ss = smem_u32(stg) + cw * C::STG_WG * 4 + C::PAIR_BYTES + static_cast<uint32_t>(idx & 1) * 2 * N * 4;
+    if (pairs) {
+      for (int c = wtid; c < 2 * N; c += 128) {
+        const int ch = im.nt * N + c % N;
+        const float *src = c < N ? p.scale : p.shift;
+        st_shared_u32(ss + c * 4, __float_as_uint(ch < p.cout && src ? __ldg(src + ch) : (c < N ? 1.0f : 0.0f)));
+      }
+    }
     // slots of the step whose wgmma group is still in flight: weight slot, and the activation slot when that step was
     // the last one of its unit (-1 otherwise)
     uint32_t prev_b = 0;
@@ -417,26 +535,75 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
     release(kBE, prev_b);
     release(kAE, static_cast<uint32_t>(prev_a));  // the item's last step ends a unit
     wg_fence_acc<C::ACC>(acc);
-    // park hi + cross * 2^-11 in this warpgroup's staging tile (row mt * 64 + fragment row) once the epilogue warps have
-    // drained the previous item from it, and go on with the next item
+    // fill this warpgroup's staging tile once the epilogue warps have drained the previous item from it, and go on with
+    // the next item
     tr.add(kTrEpi, t0);
     t0 = tr.now();
     if (idx > 0) mbar_wait(smem_u32(&s_bar[kSF + cw]), static_cast<uint32_t>((idx - 1) & 1));
     tr.add(kTrStageFree, t0);
     t0 = tr.now();
-    float *const st = stg + cw * C::STG_WG;
+    if (pairs) {
+      // fp16-pair rows, the operations of epilogue_warps in its order: per 8-column group j, lanes 4q .. 4q + 3 write
+      // the hi and the lo' 16-byte chunks of fragment row q (mod 8), which the swizzle puts on distinct banks
+      const int lane = wtid & 31, key = lane >> 2;  // fragment row & 7
+      // shared address of fragment row q, column pair (lane & 3) of chunk jj's hi / lo' halves; the (M tile, group)
+      // block and the row half h are immediate offsets
+      const uint32_t row = smem_u32(stg) + cw * C::STG_WG * 4 + ((wtid >> 5) * 16 + key) * 128 + (lane & 3) * 4;
+      uint32_t a_hi[4], a_lo[4];
 #pragma unroll
-    for (int mt = 0; mt < MT; ++mt) {
+      for (int jj = 0; jj < 4; ++jj) a_hi[jj] = row + ((jj ^ key) << 4), a_lo[jj] = row + (((4 + jj) ^ key) << 4);
+      // the scale / shift columns are staged once the warpgroup passes its barrier; the barrier's zero output makes the
+      // reads depend on it
+      uint32_t after_bar;
+      asm volatile("bar.sync %1, 128;\n\tmov.u32 %0, 0;" : "=r"(after_bar) : "r"(1 + cw) : "memory");
+      const uint32_t sc_col = ss + after_bar + (lane & 3) * 8;
+      bool o[MT][2] = {};
 #pragma unroll
-      for (int i = 0; i < H; i += 2) {
-        const int r = mt * 64 + frag_row(i, wtid), c = frag_col(i, wtid);
-        *reinterpret_cast<float2 *>(st + r * C::SP + c) =
-            make_float2(fmaf(acc[mt * N + H + i], kLoInv, acc[mt * N + i]), fmaf(acc[mt * N + H + i + 1], kLoInv, acc[mt * N + i + 1]));
+      for (int j = 0; j < N / 8; ++j) {
+        // columns past cout: scale 1, shift 0, value 0, no overflow
+        const float2 sc = ld_shared_f2(sc_col + j * 32), sh = ld_shared_f2(sc_col + (N + j * 8) * 4);
+        const float sc0 = sc.x, sc1 = sc.y, sh0 = sh.x, sh1 = sh.y;
+#pragma unroll
+        for (int mt = 0; mt < MT; ++mt) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int i = j * 4 + h * 2;
+            float v0 = fmaf(acc[mt * N + H + i], kLoInv, acc[mt * N + i]);
+            float v1 = fmaf(acc[mt * N + H + i + 1], kLoInv, acc[mt * N + i + 1]);
+            v0 = fmaf(v0, sc0, sh0);
+            v1 = fmaf(v1, sc1, sh1);
+            if (p.relu) v0 = fmaxf(v0, 0.f), v1 = fmaxf(v1, 0.f);
+            __half2 hi, lo;
+            split_h16x2(v0, v1, hi, lo, o[mt][h]);
+            const uint32_t off = (mt * (N / 32) + j / 4) * C::PAIR_BLK + h * 8 * 128;
+            st_shared_u32(a_hi[j & 3] + off, *reinterpret_cast<const uint32_t *>(&hi));
+            st_shared_u32(a_lo[j & 3] + off, *reinterpret_cast<const uint32_t *>(&lo));
+          }
+        }
+      }
+      // only values that reach the image count (fragment row q + 8 h: pixel row iy + h, column ix)
+      const int iy = im.ty0 + cw * 8 + (wtid >> 5) * 2, ix = im.tx0 + key;
+#pragma unroll
+      for (int mt = 0; mt < MT; ++mt)
+        ovf |= ix < p.oW && ((o[mt][0] && iy + mt * kTH < p.oH) || (o[mt][1] && iy + mt * kTH + 1 < p.oH));
+      fence_proxy_async();  // the TMA stores read the tile through the async proxy
+    } else {
+      // hi + cross * 2^-11 in fp32, row mt * 64 + fragment row
+      float *const st = stg + cw * C::STG_WG;
+#pragma unroll
+      for (int mt = 0; mt < MT; ++mt) {
+#pragma unroll
+        for (int i = 0; i < H; i += 2) {
+          const int r = mt * 64 + frag_row(i, wtid), c = frag_col(i, wtid);
+          *reinterpret_cast<float2 *>(st + r * C::SP + c) =
+              make_float2(fmaf(acc[mt * N + H + i], kLoInv, acc[mt * N + i]), fmaf(acc[mt * N + H + i + 1], kLoInv, acc[mt * N + i + 1]));
+        }
       }
     }
     mbar_arrive(smem_u32(&s_bar[kSS + cw]));
     tr.add(kTrEpi, t0);
   }
+  if (ovf && p.status) atomicOr(p.status, 1);
   if (cw == 0) {
     tr.count(kTrItems, static_cast<unsigned long long>(n_items));
     tr.add(kTrCycles, t_start);
@@ -484,19 +651,24 @@ __global__ void __launch_bounds__(256) pixel_h16_to_nchw_kernel(const __half *__
   out[q] = merge_h16(grp[c % 32], grp[32 + c % 32]);
 }
 
-inline int make_image_map(const void *img, int B, int H, int W, int Cin, int stride, int box_x, int box_y, CUtensorMap *map) {
-  // Cin = channels per pixel of the image in memory
-  using Encode = CUresult (*)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
-                              const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
-                              CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+using Encode = CUresult (*)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
+                            const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
+                            CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+inline Encode tensor_map_encoder() {  // cuTensorMapEncodeTiled from the driver, or null
   static Encode encode = nullptr;
   if (!encode) {
     void *fn = nullptr;
     cudaDriverEntryPointQueryResult qr;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qr) != cudaSuccess || !fn)
-      return P3D_ERR_UNSUPPORTED;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qr) != cudaSuccess || !fn) return nullptr;
     encode = reinterpret_cast<Encode>(fn);
   }
+  return encode;
+}
+
+inline int make_image_map(const void *img, int B, int H, int W, int Cin, int stride, int box_x, int box_y, CUtensorMap *map) {
+  // Cin = channels per pixel of the image in memory
+  const Encode encode = tensor_map_encoder();
+  if (!encode) return P3D_ERR_UNSUPPORTED;
   const cuuint64_t row = static_cast<cuuint64_t>(4) * Cin;  // bytes per pixel
   const cuuint64_t gdim[4] = {static_cast<cuuint64_t>(2 * Cin), static_cast<cuuint64_t>(W), static_cast<cuuint64_t>(H),
                               static_cast<cuuint64_t>(B)};
@@ -510,8 +682,36 @@ inline int make_image_map(const void *img, int B, int H, int W, int Cin, int str
   return r == CUDA_SUCCESS ? P3D_OK : P3D_ERR_INVALID_ARG;
 }
 
+// Store map of the pair-tile epilogue over the out_C-channel output image.  Convolution: {2 out_C halfs, out_W, out_H, B}
+// with an 8 x 8-pixel box of one 32-channel group.  Transposed conv (kernel = stride = up, input H x W): the output
+// pixel (iy up + dy, ix up + dx) as {2 out_C halfs, up (dx), W (ix), up (dy), B H (iy)} with a box of one tap's 8 pixels
+// of an input row.  Boxes past the right and bottom edges are clipped.
+inline int make_out_map(void *img, int B, int H, int W, int out_C, int up, CUtensorMap *map) {
+  const Encode encode = tensor_map_encoder();
+  if (!encode) return P3D_ERR_UNSUPPORTED;
+  const cuuint64_t row = static_cast<cuuint64_t>(4) * out_C;  // bytes per output pixel
+  CUresult r;
+  if (up == 1) {
+    const cuuint64_t gdim[4] = {static_cast<cuuint64_t>(2 * out_C), static_cast<cuuint64_t>(W), static_cast<cuuint64_t>(H),
+                                static_cast<cuuint64_t>(B)};
+    const cuuint64_t gstride[3] = {row, row * W, row * W * H};
+    const cuuint32_t box[4] = {64u, static_cast<cuuint32_t>(kTW), 8u, 1u}, estride[4] = {1u, 1u, 1u, 1u};
+    r = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, img, gdim, gstride, box, estride, CU_TENSOR_MAP_INTERLEAVE_NONE,
+               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  } else {
+    const cuuint64_t u = static_cast<cuuint64_t>(up), ow = u * W;
+    const cuuint64_t gdim[5] = {static_cast<cuuint64_t>(2 * out_C), u, static_cast<cuuint64_t>(W), u,
+                                static_cast<cuuint64_t>(B) * H};
+    const cuuint64_t gstride[4] = {row, row * u, row * ow, row * ow * u};
+    const cuuint32_t box[5] = {64u, 1u, static_cast<cuuint32_t>(kTW), 1u, 1u}, estride[5] = {1u, 1u, 1u, 1u, 1u};
+    r = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, img, gdim, gstride, box, estride, CU_TENSOR_MAP_INTERLEAVE_NONE,
+               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  }
+  return r == CUDA_SUCCESS ? P3D_OK : P3D_ERR_INVALID_ARG;
+}
+
 template <int N, int MT, bool HALO>
-int launch(const CUtensorMap &map, const Params &p, cudaStream_t st) {
+int launch(const CUtensorMap &map, const CUtensorMap &out_map, const Params &p, cudaStream_t st) {
   using C = Cfg<N, MT, HALO>;
   const size_t smem = static_cast<size_t>(C::NA) * C::A_BYTES + static_cast<size_t>(C::NB) * C::B_BYTES + C::STG_BYTES + 1024;
   if (smem > static_cast<size_t>(kSmemBudget)) return P3D_ERR_UNSUPPORTED;
@@ -529,7 +729,7 @@ int launch(const CUtensorMap &map, const Params &p, cudaStream_t st) {
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  P3D_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, map, p));
+  P3D_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, map, out_map, p));
   P3D_LAUNCH_CHECK();
   return P3D_OK;
 }
@@ -790,12 +990,14 @@ extern "C" int p3d_dense_conv2d_f16(const void *in_h16, int B, int H, int W, int
   p.tiles_y = (p.oH + dcf::kTH * mt - 1) / (dcf::kTH * mt);
   CUtensorMap map;
   const int bx = halo ? dcf::kPitch : dcf::kTW, by = halo ? dcf::kTH * mt + 2 : dcf::kTH * mt;
-  const int rc = dcf::make_image_map(in_h16, B, H, W, Cin, p.stride, bx, by, &map);
+  int rc = dcf::make_image_map(in_h16, B, H, W, Cin, p.stride, bx, by, &map);
   if (rc != P3D_OK) return rc;
+  CUtensorMap omap = {};  // read only by the pair-tile epilogue of launches without fp32 planes
+  if (!out_nchw && (rc = dcf::make_out_map(out_h16, B, p.oH, p.oW, out_C, up, &omap)) != P3D_OK) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (n_tile == 128) return halo ? dcf::launch<128, 1, true>(map, p, st) : dcf::launch<128, 1, false>(map, p, st);
-  if (mt == 2) return halo ? dcf::launch<64, 2, true>(map, p, st) : dcf::launch<64, 2, false>(map, p, st);
-  return halo ? dcf::launch<64, 1, true>(map, p, st) : dcf::launch<64, 1, false>(map, p, st);
+  if (n_tile == 128) return halo ? dcf::launch<128, 1, true>(map, omap, p, st) : dcf::launch<128, 1, false>(map, omap, p, st);
+  if (mt == 2) return halo ? dcf::launch<64, 2, true>(map, omap, p, st) : dcf::launch<64, 2, false>(map, omap, p, st);
+  return halo ? dcf::launch<64, 1, true>(map, omap, p, st) : dcf::launch<64, 1, false>(map, omap, p, st);
 }
 
 // Output convs of the CenterHead, 9 taps in the GEMM's N dimension (dcf::out9 above): group g convolves input channels

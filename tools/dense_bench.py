@@ -8,8 +8,10 @@ convolution; the kernels execute 3 fp16 MMAs per product), then the whole head. 
 --trace builds the library with -DP3D_DENSE_TRACE into a temporary directory and prints, per layer, where the dense
 kernel's time goes, in SM cycles per work item (summed over the CTAs, divided by the items): the consumer warpgroups'
 waits on the activation / weight "full" barriers, in wgmma.wait_group, their epilogue (staging the accumulators) and
-their waits for a free staging tile; the producer thread's waits on "empty" barriers; the epilogue warps' waits on
-"staged" and their busy time.  Cycles are clock64 counts; the trace build is slower than the default one.
+their waits for a free staging tile; the producer thread's waits on "empty" barriers; epilogue thread 0's waits on
+"staged" and its time from "staged" to "freed" (these layers write only the pixel H16 image: the TMA stores of the
+consumers' fp16-pair tile until they have read it).  Cycles are clock64 counts; the trace build is slower than the
+default one.
 """
 import argparse
 import ctypes
