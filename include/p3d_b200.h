@@ -398,6 +398,22 @@ int p3d_bev_pool_v2_dev(const float *depth, const float *feat, const int32_t *ra
 int p3d_head_out_conv_f16(const void *in_h16, int B, int H, int W, int in_C, int Cin, int groups, const void *packed_weight,
                           const float *bias, const int32_t *cin0_dev, const int32_t *plane0_dev, const int32_t *cnt_dev,
                           int planes, float *out_nchw, p3d_stream_t stream);
+/* The CenterHead's batched ConvModule conv fused with the GEMM of its output convs (the path DenseRPNHead.forward takes
+ * when every output conv has <= 3 channels): a 3x3, pad 1 conv of Cout / 64 heads of 64 channels (packed_weight with
+ * n_tile 128, scale / shift, ReLU) whose fp16-pair outputs stay in shared memory, where each head's tap-as-N GEMM
+ * P[pixel][tap * 3 + co] = sum_c mid[pixel][c] W2[c][tap * 3 + co] runs on them.  packed_w2: per head
+ * p3d_dense_conv2d_f16_pack_weights(taps 1, Cin 64, n_tile 32) of W2 (8 KB, heads in Cout order).  Writes p_out
+ * [B][Cout / 64][H][W][28] fp32 (columns 0..26 used, 27 zero); status bit 0 as p3d_dense_conv2d_f16.  P is
+ * bit-identical to what p3d_head_out_conv_f16 computes from the heads' pixel H16 image.  Cin % 32 == 0 and
+ * Cout % 128 == 0 (P3D_ERR_UNSUPPORTED otherwise). */
+int p3d_head_conv_p_f16(const void *in_h16, int B, int H, int W, int Cin, const void *packed_weight, int Cout,
+                        const float *scale, const float *shift, const void *packed_w2, float *p_out, int32_t *status_dev,
+                        p3d_stream_t stream);
+/* The output convs from P of p3d_head_conv_p_f16 (groups = Cout / 64): out_nchw[b][plane0[g] + co] = bias[g][co] + the
+ * sum of P over the 9 taps, for co < cnt[g] <= 3 (device int32 arrays); bias [groups][4].  Bit-identical to
+ * p3d_head_out_conv_f16 on the same heads. */
+int p3d_head_tap_sum(const float *p_in, int B, int H, int W, int groups, const float *bias, const int32_t *plane0_dev,
+                     const int32_t *cnt_dev, int planes, float *out_nchw, p3d_stream_t stream);
 int p3d_dense_conv2d_f16(const void *in_h16, int B, int H, int W, int Cin, const void *packed_weight, int Cout, int n_tile,
                          int kh, int kw, int stride, int pad, int up, const float *scale, const float *shift, int relu,
                          void *out_h16, int out_C, int out_c0, float *out_nchw, int mode, int m_tiles,

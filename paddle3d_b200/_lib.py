@@ -87,6 +87,8 @@ SIGNATURES = {
     "p3d_lss_depth_feat": (_int, [_vp, _vp, _int, _int, _int, _int, _int, _vp, _vp, _vp]),
     "p3d_bev_pool_v2_dev": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _int, _int, _int, _int, _int, _int, _vp, _vp]),
     "p3d_head_out_conv_f16": (_int, [_vp, _int, _int, _int, _int, _int, _int, _vp, _vp, _vp, _vp, _vp, _int, _vp, _vp]),
+    "p3d_head_conv_p_f16": (_int, [_vp, _int, _int, _int, _int, _vp, _int, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "p3d_head_tap_sum": (_int, [_vp, _int, _int, _int, _int, _vp, _vp, _vp, _int, _vp, _vp]),
     "p3d_dense_conv2d_f16": (_int, [_vp, _int, _int, _int, _int, _vp, _int, _int, _int, _int, _int, _int, _int, _vp, _vp,
                                     _int, _vp, _int, _int, _vp, _int, _int, _vp, _vp]),
     "p3d_dense_conv2d_split": (_int, [_vp, _int, _int, _int, _int, _vp, _int, _int, _int, _int, _int, _int, _int, _vp, _vp,

@@ -30,6 +30,8 @@
 #include <cuda.h>
 #include <cuda_fp16.h>
 
+#include <type_traits>
+
 #include "h16.cuh"
 #include "p3d_b200.h"
 #include "tc_common.cuh"
@@ -63,6 +65,18 @@ struct Params {
   float *out_nchw;            // fp32 planes [B, cout, out_H, out_W] or null
   int32_t *status;            // bit 0: fp16 range overflow while writing out_h16
 };
+// Parameters of the FUSE_P kernel (a separate type keeps the other instantiations' parameter block as it is): per N tile
+// the two 64-channel heads' tap-as-N weight images (out9 layout, 2 x kP2Bytes)
+struct ParamsP : Params {
+  const uint8_t *packed_w2;
+};
+template <bool FUSE_P>
+using KParams = std::conditional_t<FUSE_P, ParamsP, Params>;
+
+// FUSE_P: the tap-as-N GEMM of the output convs (out9 below) on a staged pair tile.  A 64-channel head's W2 image is
+// p3d_dense_conv2d_f16_pack_weights(taps 1, Cin 64, n_tile 32): 4 k-blocks of 2 KB; P rows have kPPitch fp32 columns
+// (the 27 used ones and a zero column that keeps a pixel's row 16-byte aligned).
+constexpr int kP2Blk = 64 * 32, kP2Bytes = 4 * kP2Blk, kPPitch = 28;
 
 template <int N, int MT, bool HALO>
 struct Cfg {
@@ -285,8 +299,9 @@ __device__ __forceinline__ void epilogue_warps(const Params &p, const float *stg
 // rows below the image skipped so that a ragged tile does not spill into the next batch image) and hands the tile back
 // once the stores have read it.  A box over a group the layer owns in part (out_c0 % 32 == 16, or the last group of a
 // partly used N tile) would overwrite the neighbour's channels: all 96 threads copy the owned 32-byte hi and lo' halves
-// of such blocks with ordinary stores.
-template <int N, int MT>
+// of such blocks with ordinary stores.  FUSE_P: the consumers have staged the item's two P groups instead ([group][64
+// rows][kPPitch] fp32), which thread 0 stores as one box of the P buffer (make_p_map).
+template <int N, int MT, bool FUSE_P>
 __device__ __forceinline__ void epilogue_pairs(const Params &p, const CUtensorMap *out_map, const uint8_t *tiles, int tile_bytes,
                                                unsigned long long *staged, unsigned long long *freed, long long n_items,
                                                int th, int et) {
@@ -302,32 +317,36 @@ __device__ __forceinline__ void epilogue_pairs(const Params &p, const CUtensorMa
       mbar_wait(smem_u32(staged + c), static_cast<uint32_t>(idx & 1));
       tr.add(kTrEwWait, t0);
       t0 = tr.now();
-      for (int blk = 0; blk < MT * NQ; ++blk) {
-        const int ch0 = im.nt * N + (blk % NQ) * 32, iy0 = im.ty0 + (blk / NQ) * kTH + c * 8;
-        if (ch0 >= p.cout) continue;
-        const uint8_t *src = tiles + c * tile_bytes + blk * BLK;
-        if (whole && ch0 + 32 <= p.cout) {
-          if (!lead) continue;
-          const int hc = 2 * (p.out_c0 + ch0);  // first half of the group in a pixel row
-          if (p.up == 1) {
-            tma_store4d(out_map, smem_u32(src), hc, im.tx0, iy0, im.b);
-          } else {
-            for (int y = 0; y < 8 && iy0 + y < p.oH; ++y)
-              tma_store5d(out_map, smem_u32(src + y * 1024), hc, dx, im.tx0, dy, im.b * p.oH + iy0 + y);
+      if constexpr (FUSE_P) {  // P groups 2 nt, 2 nt + 1 of batch image b: 2 n_ntiles groups per image
+        if (lead) tma_store4d(out_map, smem_u32(tiles + c * tile_bytes), 0, im.tx0, im.ty0 + c * 8, (im.b * p.n_ntiles + im.nt) * 2);
+      } else {
+        for (int blk = 0; blk < MT * NQ; ++blk) {
+          const int ch0 = im.nt * N + (blk % NQ) * 32, iy0 = im.ty0 + (blk / NQ) * kTH + c * 8;
+          if (ch0 >= p.cout) continue;
+          const uint8_t *src = tiles + c * tile_bytes + blk * BLK;
+          if (whole && ch0 + 32 <= p.cout) {
+            if (!lead) continue;
+            const int hc = 2 * (p.out_c0 + ch0);  // first half of the group in a pixel row
+            if (p.up == 1) {
+              tma_store4d(out_map, smem_u32(src), hc, im.tx0, iy0, im.b);
+            } else {
+              for (int y = 0; y < 8 && iy0 + y < p.oH; ++y)
+                tma_store5d(out_map, smem_u32(src + y * 1024), hc, dx, im.tx0, dy, im.b * p.oH + iy0 + y);
+            }
+            continue;
           }
-          continue;
-        }
-        for (int u = et; u < 128; u += kEpiThreads) {  // (row, 16-channel half)
-          const int r = u >> 1, h = u & 1, iy = iy0 + (r >> 3), ix = im.tx0 + (r & 7);
-          if (ch0 + 16 * h >= p.cout || iy >= p.oH || ix >= p.oW) continue;
-          const int oc = p.out_c0 + ch0 + 16 * h, Y = iy * p.up + dy, X = ix * p.up + dx;
-          uint8_t *op = p.out_h16 + ((static_cast<size_t>(im.b) * p.out_H + Y) * p.out_W + X) * (4 * static_cast<size_t>(p.out_C)) +
-                        (oc / 32) * 128 + (oc % 32) * 2;
-          const uint8_t *row = src + r * 128;
-#pragma unroll
-          for (int k = 0; k < 2; ++k) {
-            *reinterpret_cast<uint4 *>(op + 16 * k) = *reinterpret_cast<const uint4 *>(row + (((2 * h + k) ^ (r & 7)) << 4));
-            *reinterpret_cast<uint4 *>(op + 64 + 16 * k) = *reinterpret_cast<const uint4 *>(row + (((4 + 2 * h + k) ^ (r & 7)) << 4));
+          for (int u = et; u < 128; u += kEpiThreads) {  // (row, 16-channel half)
+            const int r = u >> 1, h = u & 1, iy = iy0 + (r >> 3), ix = im.tx0 + (r & 7);
+            if (ch0 + 16 * h >= p.cout || iy >= p.oH || ix >= p.oW) continue;
+            const int oc = p.out_c0 + ch0 + 16 * h, Y = iy * p.up + dy, X = ix * p.up + dx;
+            uint8_t *op = p.out_h16 + ((static_cast<size_t>(im.b) * p.out_H + Y) * p.out_W + X) * (4 * static_cast<size_t>(p.out_C)) +
+                          (oc / 32) * 128 + (oc % 32) * 2;
+            const uint8_t *row = src + r * 128;
+  #pragma unroll
+            for (int k = 0; k < 2; ++k) {
+              *reinterpret_cast<uint4 *>(op + 16 * k) = *reinterpret_cast<const uint4 *>(row + (((2 * h + k) ^ (r & 7)) << 4));
+              *reinterpret_cast<uint4 *>(op + 64 + 16 * k) = *reinterpret_cast<const uint4 *>(row + (((4 + 2 * h + k) ^ (r & 7)) << 4));
+            }
           }
         }
       }
@@ -345,11 +364,20 @@ __device__ __forceinline__ void epilogue_pairs(const Params &p, const CUtensorMa
   }
 }
 
-template <int N, int MT, bool HALO>
+// FUSE_P (N = 128, MT = 1, HALO; the CenterHead's batched ConvModule conv): after the pair split the consumers also run
+// the tap-as-N GEMM of the next layer, P[pixel][tap * 3 + co] = sum_c mid[pixel][c] W2[c][tap * 3 + co], on the staged
+// pair rows of each of the N tile's two 64-channel heads (A: pair blocks 2j, 2j + 1; B: one extra weight-ring fill per
+// item holding both heads' W2 images), and stage P over the retired pair blocks for the epilogue thread: the output
+// convs' input image is never written.  The wgmma order is head_out9_kernel's, so P is bit-identical to what out9
+// computes from the image read back, and p3d_head_tap_sum finishes the convs.
+template <int N, int MT, bool HALO, bool FUSE_P = false>
 __global__ void __launch_bounds__(kDenseThreads, 1)
     dense_conv_f16_kernel(const __grid_constant__ CUtensorMap in_map, const __grid_constant__ CUtensorMap out_map,
-                          const Params p) {
+                          const KParams<FUSE_P> p) {
   using C = Cfg<N, MT, HALO>;
+  static_assert(!FUSE_P || (N == 128 && MT == 1 && HALO && 2 * kP2Bytes == C::B_BYTES &&
+                            2 * 64 * kPPitch * 4 <= C::PAIR_BYTES),
+                "fused P: two 64-channel heads' W2 images fill one weight slot; P fits over the pair blocks");
   constexpr int TH = kTH * MT;  // output tile height
   constexpr int H = N / 2;      // accumulator registers of the hi products of one M tile; the cross products follow
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -402,7 +430,7 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(C::P_REGS));
     if (tid >= 32) {
       if (pairs)
-        epilogue_pairs<N, MT>(p, &out_map, reinterpret_cast<const uint8_t *>(stg), C::STG_WG * 4, s_bar + kSS, s_bar + kSF,
+        epilogue_pairs<N, MT, FUSE_P>(p, &out_map, reinterpret_cast<const uint8_t *>(stg), C::STG_WG * 4, s_bar + kSS, s_bar + kSF,
                               n_items, TH, tid - 32);
       else
         epilogue_warps<N, MT>(p, stg, s_bar + kSS, s_bar + kSF, n_items, TH, tid - 32);
@@ -444,6 +472,16 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
           }
         }
         if (++dx == p.kw) dx = 0, ++dy;
+      }
+      if constexpr (FUSE_P) {  // the item's W2 images, used after its last step
+        const uint32_t bbar = smem_u32(&s_bar[kBF + b_slot]);
+        const long long t1 = tr.now();
+        mbar_wait(smem_u32(&s_bar[kBE + b_slot]), b_ph ^ 1u);
+        tr.add(kTrBEmpty, t1);
+        mbar_arrive_expect_tx(bbar, static_cast<uint32_t>(C::B_BYTES));
+        bulk_g2s(b_ring + b_slot * C::B_BYTES, p.packed_w2 + static_cast<size_t>(im.nt) * C::B_BYTES,
+                 static_cast<uint32_t>(C::B_BYTES), bbar);
+        if (++b_slot == C::NB) b_slot = 0, b_ph ^= 1u;
       }
     }
     tr.flush(0);
@@ -586,7 +624,54 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
 #pragma unroll
       for (int mt = 0; mt < MT; ++mt)
         ovf |= ix < p.oW && ((o[mt][0] && iy + mt * kTH < p.oH) || (o[mt][1] && iy + mt * kTH + 1 < p.oH));
-      fence_proxy_async();  // the TMA stores read the tile through the async proxy
+      fence_proxy_async();  // the TMA stores (FUSE_P: the wgmma) read the tile through the async proxy
+      if constexpr (FUSE_P) {
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");  // the warpgroup's pair rows are all staged
+        const long long t1 = tr.now();
+        mbar_wait(smem_u32(&s_bar[kBF + b_slot]), b_ph);
+        tr.add(kTrBFull, t1);
+        const uint32_t w2 = b_ring + b_slot * C::B_BYTES, tile = smem_u32(stg) + cw * C::STG_WG * 4;
+        float pacc[64];  // per head j: hi products [32 j, 32 j + 16), cross products [32 j + 16, 32 j + 32)
+#pragma unroll
+        for (int i = 0; i < 64; ++i) pacc[i] = 0.f;
+        wg_fence();
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+#pragma unroll
+          for (int k = 0; k < 2; ++k) {  // 32-channel group of the head, then k-step: head_out9_kernel's order
+#pragma unroll
+            for (int kb = 0; kb < 2; ++kb) {
+              const uint32_t bk = w2 + static_cast<uint32_t>(j * kP2Bytes + (k * 2 + kb) * kP2Blk);
+              const uint64_t dbh = smem_desc(bk, 2 * 32 * 16, 128), dbl = smem_desc(bk + 32 * 16, 2 * 32 * 16, 128);
+              const uint32_t a0 = tile + static_cast<uint32_t>((2 * j + k) * C::PAIR_BLK);
+              const uint64_t dah = desc_sw128(a0 + kb * 32), dal = desc_sw128(a0 + (2 + kb) * 32);
+              wg::mma_f16<32>(pacc + 32 * j, dah, dbh, 1u);
+              wg::mma_f16<32>(pacc + 32 * j + 16, dah, dbl, 1u);
+              wg::mma_f16<32>(pacc + 32 * j + 16, dal, dbh, 1u);
+            }
+          }
+        }
+        wg_commit();
+        wg_wait<0>();
+        release(kBE, b_slot);
+        if (++b_slot == C::NB) b_slot = 0, b_ph ^= 1u;
+        wg_fence_acc<64>(pacc);
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");  // every warp's wgmma have read the pair rows
+        // P[group j][row][col] = hi + cross * 2^-11 over the retired pair blocks, columns 0 .. kPPitch - 1 (27 is 0)
+        float *const pt = stg + cw * C::STG_WG;
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+#pragma unroll
+          for (int i = 0; i < 16; i += 2) {
+            const int r = frag_row(i, wtid), c = frag_col(i, wtid);
+            if (c < kPPitch)
+              *reinterpret_cast<float2 *>(pt + (j * 64 + r) * kPPitch + c) =
+                  make_float2(fmaf(pacc[32 * j + 16 + i], kLoInv, pacc[32 * j + i]),
+                              fmaf(pacc[32 * j + 17 + i], kLoInv, pacc[32 * j + 1 + i]));
+          }
+        }
+        fence_proxy_async();
+      }
     } else {
       // hi + cross * 2^-11 in fp32, row mt * 64 + fragment row
       float *const st = stg + cw * C::STG_WG;
@@ -710,12 +795,27 @@ inline int make_out_map(void *img, int B, int H, int W, int out_C, int up, CUten
   return r == CUDA_SUCCESS ? P3D_OK : P3D_ERR_INVALID_ARG;
 }
 
-template <int N, int MT, bool HALO>
-int launch(const CUtensorMap &map, const CUtensorMap &out_map, const Params &p, cudaStream_t st) {
+// Store map of the FUSE_P epilogue over the P buffer [B * p_groups][H][W][kPPitch] fp32: one box is an item's two
+// groups of one consumer warpgroup's 8 x 8 pixels; boxes past the right and bottom edges are clipped.
+inline int make_p_map(float *pbuf, int B, int H, int W, int p_groups, CUtensorMap *map) {
+  const Encode encode = tensor_map_encoder();
+  if (!encode) return P3D_ERR_UNSUPPORTED;
+  const cuuint64_t px = static_cast<cuuint64_t>(4) * kPPitch;  // bytes per pixel of a group
+  const cuuint64_t gdim[4] = {static_cast<cuuint64_t>(kPPitch), static_cast<cuuint64_t>(W), static_cast<cuuint64_t>(H),
+                              static_cast<cuuint64_t>(B) * p_groups};
+  const cuuint64_t gstride[3] = {px, px * W, px * W * H};
+  const cuuint32_t box[4] = {static_cast<cuuint32_t>(kPPitch), static_cast<cuuint32_t>(kTW), 8u, 2u}, estride[4] = {1u, 1u, 1u, 1u};
+  const CUresult r = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, pbuf, gdim, gstride, box, estride, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                            CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? P3D_OK : P3D_ERR_INVALID_ARG;
+}
+
+template <int N, int MT, bool HALO, bool FUSE_P = false>
+int launch(const CUtensorMap &map, const CUtensorMap &out_map, const KParams<FUSE_P> &p, cudaStream_t st) {
   using C = Cfg<N, MT, HALO>;
   const size_t smem = static_cast<size_t>(C::NA) * C::A_BYTES + static_cast<size_t>(C::NB) * C::B_BYTES + C::STG_BYTES + 1024;
   if (smem > static_cast<size_t>(kSmemBudget)) return P3D_ERR_UNSUPPORTED;
-  auto kern = dense_conv_f16_kernel<N, MT, HALO>;
+  auto kern = dense_conv_f16_kernel<N, MT, HALO, FUSE_P>;
   P3D_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   const long long work = static_cast<long long>(p.B) * p.tiles_y * p.tiles_x * p.n_ntiles * (p.up > 1 ? p.up * p.up : 1);
   cudaLaunchConfig_t cfg = {};
@@ -884,6 +984,60 @@ __global__ void __launch_bounds__(kThreads, 1) head_out9_kernel(const __grid_con
   }
 }
 }  // namespace out9
+
+// Spatial half of the fused output convs (FUSE_P): out[b][plane0 + co][y][x] = bias + sum_tap P[y + dy][x + dx][tap * 3
+// + co], taps in out9's order with +0 for neighbours outside the image (what out9 adds there from its zero-filled
+// halo), so the planes are bit-identical to out9's.  A block stages the 10 x 34 haloed pixels of one 8 x 32 output tile
+// of one P group with coalesced 16-byte loads (row pitch 27 floats: the per-pixel reads of a warp hit distinct banks);
+// one thread per output pixel, so a warp stores 32 consecutive floats of a plane row.
+namespace tapsum {
+constexpr int kTX = 32, kTY = 8, kThreads = kTX * kTY, kSX = kTX + 2, kSY = kTY + 2, kSP = 27;
+
+struct Params {
+  int B, H, W, groups, planes, tiles_x, tiles_y;
+  const float *p;               // [B * groups][H][W][kPPitch]
+  const float *bias;            // [groups][4]
+  const int32_t *plane0, *cnt;  // [groups]
+  float *out;                   // [B, planes, H, W]
+};
+
+__global__ void __launch_bounds__(kThreads) head_tap_sum_kernel(const Params p) {
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  __shared__ float s_p[kSY * kSX * kSP];
+  long long q = blockIdx.x;
+  const int tx0 = static_cast<int>(q % p.tiles_x) * kTX;
+  q /= p.tiles_x;
+  const int ty0 = static_cast<int>(q % p.tiles_y) * kTY;
+  q /= p.tiles_y;
+  const int g = static_cast<int>(q % p.groups), b = static_cast<int>(q / p.groups);
+  const float *src = p.p + static_cast<size_t>(b * p.groups + g) * p.H * p.W * kPPitch;
+  constexpr int V = kPPitch / 4;  // float4 per pixel
+  for (int u = threadIdx.x; u < kSY * kSX * V; u += kThreads) {
+    const int pix = u / V, v = u - pix * V, sy = pix / kSX, sx = pix - sy * kSX, Y = ty0 - 1 + sy, X = tx0 - 1 + sx;
+    float4 f = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (Y >= 0 && Y < p.H && X >= 0 && X < p.W)
+      f = __ldg(reinterpret_cast<const float4 *>(src + (static_cast<size_t>(Y) * p.W + X) * kPPitch) + v);
+    float *d = s_p + pix * kSP + v * 4;
+    d[0] = f.x;
+    d[1] = f.y;
+    d[2] = f.z;
+    if (v < V - 1) d[3] = f.w;  // column 27 is not used
+  }
+  __syncthreads();
+  const int lx = threadIdx.x % kTX, ly = threadIdx.x / kTX, X = tx0 + lx, Y = ty0 + ly;
+  if (X >= p.W || Y >= p.H) return;
+  const int cnt = __ldg(p.cnt + g), p0 = __ldg(p.plane0 + g);
+  const size_t plane = static_cast<size_t>(p.H) * p.W;
+  float *op = p.out + (static_cast<size_t>(b) * p.planes + p0) * plane + static_cast<size_t>(Y) * p.W + X;
+  for (int co = 0; co < cnt; ++co) {
+    float s = __ldg(p.bias + g * 4 + co);
+#pragma unroll
+    for (int t = 0; t < 9; ++t) s += s_p[((ly + t / 3) * kSX + lx + t % 3) * kSP + t * 3 + co];
+    op[co * plane] = s;
+  }
+}
+}  // namespace tapsum
 
 }  // namespace dcf
 }  // namespace p3d
@@ -1056,6 +1210,76 @@ extern "C" int p3d_head_out_conv_f16(const void *in_h16, int B, int H, int W, in
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   P3D_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, map, p));
+  P3D_LAUNCH_CHECK();
+  return P3D_OK;
+}
+
+// CenterHead ConvModule conv (3x3, pad 1, scale / shift, ReLU) of Cout / 64 heads fused with the GEMM of their output
+// convs (dcf::dense_conv_f16_kernel<128, 1, true, true>): writes P [B][Cout / 64][H][W][28] fp32 instead of the heads'
+// pixel H16 image; p3d_head_tap_sum makes the planes.
+extern "C" int p3d_head_conv_p_f16(const void *in_h16, int B, int H, int W, int Cin, const void *packed_weight, int Cout,
+                                   const float *scale, const float *shift, const void *packed_w2, float *p_out,
+                                   int32_t *status_dev, p3d_stream_t stream) {
+  if (!in_h16 || !packed_weight || !packed_w2 || !p_out || B < 1 || H < 1 || W < 1 || Cout < 1) return P3D_ERR_INVALID_ARG;
+  if (Cin < 32 || Cin % 32 || Cout % 128) return P3D_ERR_UNSUPPORTED;
+  if ((reinterpret_cast<uintptr_t>(in_h16) & 15) || (reinterpret_cast<uintptr_t>(packed_weight) & 15) ||
+      (reinterpret_cast<uintptr_t>(packed_w2) & 15) || (reinterpret_cast<uintptr_t>(p_out) & 15))
+    return P3D_ERR_INVALID_ARG;
+  dcf::ParamsP p = {};
+  p.B = B;
+  p.H = p.oH = p.out_H = H;
+  p.W = p.oW = p.out_W = W;
+  p.Cin = Cin;
+  p.taps = 9;
+  p.kw = 3;
+  p.stride = p.pad = p.up = 1;
+  p.n_ntiles = Cout / 128;
+  p.cout = Cout;
+  p.relu = 1;
+  p.packed_w = static_cast<const uint8_t *>(packed_weight);
+  p.scale = scale;
+  p.shift = shift;
+  p.status = status_dev;
+  p.packed_w2 = static_cast<const uint8_t *>(packed_w2);
+  p.tiles_x = (W + dcf::kTW - 1) / dcf::kTW;
+  p.tiles_y = (H + dcf::kTH - 1) / dcf::kTH;
+  CUtensorMap map, pmap;
+  int rc = dcf::make_image_map(in_h16, B, H, W, Cin, 1, dcf::kPitch, dcf::kTH + 2, &map);
+  if (rc != P3D_OK || (rc = dcf::make_p_map(p_out, B, H, W, Cout / 64, &pmap)) != P3D_OK) return rc;
+  return dcf::launch<128, 1, true, true>(map, pmap, p, static_cast<cudaStream_t>(stream));
+}
+
+// Output convs of p3d_head_conv_p_f16's heads from P: group g writes cnt[g] <= 3 planes from plane0[g] of out_nchw
+// [B, planes, H, W] (device int32 arrays); bias [groups][4].
+extern "C" int p3d_head_tap_sum(const float *p_in, int B, int H, int W, int groups, const float *bias, const int32_t *plane0_dev,
+                                const int32_t *cnt_dev, int planes, float *out_nchw, p3d_stream_t stream) {
+  if (!p_in || !bias || !plane0_dev || !cnt_dev || !out_nchw || B < 1 || H < 1 || W < 1 || groups < 1 || planes < 1 ||
+      (reinterpret_cast<uintptr_t>(p_in) & 15))
+    return P3D_ERR_INVALID_ARG;
+  namespace ts = dcf::tapsum;
+  ts::Params p;
+  p.B = B;
+  p.H = H;
+  p.W = W;
+  p.groups = groups;
+  p.planes = planes;
+  p.tiles_x = (W + ts::kTX - 1) / ts::kTX;
+  p.tiles_y = (H + ts::kTY - 1) / ts::kTY;
+  p.p = p_in;
+  p.bias = bias;
+  p.plane0 = plane0_dev;
+  p.cnt = cnt_dev;
+  p.out = out_nchw;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(static_cast<unsigned int>(static_cast<long long>(B) * groups * p.tiles_y * p.tiles_x));
+  cfg.blockDim = dim3(ts::kThreads);
+  cfg.stream = static_cast<cudaStream_t>(stream);
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  P3D_CUDA_CHECK(cudaLaunchKernelEx(&cfg, ts::head_tap_sum_kernel, p));
   P3D_LAUNCH_CHECK();
   return P3D_OK;
 }

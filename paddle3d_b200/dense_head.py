@@ -349,14 +349,50 @@ class DenseRPNHead:
         """Same as forward() for a BEV given as pixel fp16-pair rows (SparseResNet3D.forward(pixel_h16=True))."""
         return self.forward(rows, shape)
 
+    def fused_heads(self, bp):
+        """Whether forward fuses the output convs' tap-as-N GEMM into the batched ConvModule conv (p3d_head_conv_p_f16,
+        then p3d_head_tap_sum): fp16-pair path, 64-channel heads on the 128-wide N tile (two heads per tile), and every
+        output conv <= 3 channels, so that each head is one tap-as-N group.  Otherwise the heads' image is written and
+        read back by p3d_head_out_conv_f16."""
+        big = bp["big"]
+        return (self.f16 and self.shared.cout == 64 and big.n_tile == 128 and big.cout % 128 == 0
+                and all(int(k) <= 3 for k in bp["cnt"]))
+
+    def _heads_conv_p(self, s, shape, bp, device):
+        """Fused path, first launch: the batched ConvModule conv and the output convs' per-pixel GEMM -> P
+        [B, heads, H, W, 28] fp32 (the heads' 64-channel image is never written)."""
+        from ._lib import check, lib
+        from ._mem import ptr, stream
+        b, H, W, cin = shape
+        big = bp["big"]
+        d = big.dev
+        p = torch.empty((b, big.cout // 64, H, W, 28), dtype=torch.float32, device=device)
+        check(lib().p3d_head_conv_p_f16(ptr(s), b, H, W, cin, ptr(d["packed"]), big.cout, ptr(d["scale"]), ptr(d["shift"]),
+                                        ptr(bp["packed9"]), ptr(p), ptr(dc._status(device)), stream(device)), "head_conv_p_f16")
+        return p
+
+    def _tap_sum(self, p, bp, device):
+        """Fused path, second launch: P -> the output convs' fp32 planes [B, planes, H, W]."""
+        from ._lib import check, lib
+        from ._mem import ptr, stream
+        b, groups, H, W, _ = p.shape
+        planes = torch.empty((b, bp["planes"], H, W), dtype=torch.float32, device=device)
+        check(lib().p3d_head_tap_sum(ptr(p), b, H, W, groups, ptr(bp["bias9"]), ptr(bp["plane0_9"]), ptr(bp["cnt9"]),
+                                     bp["planes"], ptr(planes), stream(device)), "head_tap_sum")
+        return planes
+
     def forward(self, bev, shape=None):
         """bev [B, C, H, W] fp32 -> dict name -> list (per task) of [B, k, H, W] fp32 tensors.  The 36 ConvModules run as
-        one 64 -> 2304 convolution, the 36 output convs as one grouped launch."""
+        one 64 -> 2304 convolution, the 36 output convs as one grouped launch (fused_heads: the conv also runs the
+        output convs' GEMM, and one launch sums its taps)."""
         s, shape = self._trunk(bev, shape)
         bp = self._batched_params(bev.device)
         big = bp["big"]
-        mid, _, _ = big(s, shape)  # [B*H*W] pixel rows of 36 * 64 channels
-        planes = self._final_convs(mid, shape, big.cout, bp, bp["planes"], bev.device)
+        if self.fused_heads(bp):
+            planes = self._tap_sum(self._heads_conv_p(s, shape, bp, bev.device), bp, bev.device)
+        else:
+            mid, _, _ = big(s, shape)  # [B*H*W] pixel rows of 36 * 64 channels
+            planes = self._final_convs(mid, shape, big.cout, bp, bp["planes"], bev.device)
         out = {}
         for name, p0, k in zip(bp["names"], bp["plane0"], bp["cnt"]):
             out.setdefault(name, []).append(planes[:, int(p0):int(p0) + int(k)])

@@ -136,9 +136,15 @@ def main():
     s, shape = net._trunk(bev)
     bp = net._batched_params(dev)
     mid, _, _ = bp["big"](s, shape)
+    pbuf = net._heads_conv_p(s, shape, bp, dev)
+    # heads_big_conv_us + final_convs_us: the unfused heads (image written, read back by p3d_head_out_conv_f16);
+    # fused_conv_us + tap_sum_us: what forward runs when net.fused_heads(bp)
     print(json.dumps({"trunk_us": round(graph_time(lambda: net._trunk(bev), 3), 1),
                       "heads_big_conv_us": round(graph_time(lambda: bp["big"](s, shape), 3), 1),
                       "final_convs_us": round(graph_time(lambda: net._final_convs(mid, shape, bp["big"].cout, bp, bp["planes"], dev), 3), 1),
+                      "fused_conv_us": round(graph_time(lambda: net._heads_conv_p(s, shape, bp, dev), 3), 1),
+                      "tap_sum_us": round(graph_time(lambda: net._tap_sum(pbuf, bp, dev), 3), 1),
+                      "fused_heads": net.fused_heads(bp),
                       "nchw_to_h16_us": round(graph_time(lambda: dc.nchw_to_pixel_h16(bev), 3), 1)}), flush=True)
     if args.tf32:
         net32 = DenseRPNHead(in_channels=256, f16=False).init_weight(seed=1, device=dev)
