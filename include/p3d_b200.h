@@ -418,6 +418,31 @@ int p3d_dense_conv2d_f16(const void *in_h16, int B, int H, int W, int Cin, const
                          int kh, int kw, int stride, int pad, int up, const float *scale, const float *shift, int relu,
                          void *out_h16, int out_C, int out_c0, float *out_nchw, int mode, int m_tiles,
                          int32_t *status_dev, p3d_stream_t stream);
+/* p3d_dense_conv2d_f16 with a residual (ResNet BasicBlock's conv2 + identity): channels [0, Cout) of the pixel H16 image
+ * res_h16 [B, oH, oW, res_C] are added after scale / shift and before ReLU, v = fma(acc, scale, shift) + (hi + lo' 2^-11).
+ * res_h16 16-byte aligned and res_C >= Cout (P3D_ERR_INVALID_ARG otherwise); up == 1, H16 output only (out_nchw null),
+ * out_c0 % 32 == 0 and res_C % 32 == 0 (P3D_ERR_UNSUPPORTED otherwise). */
+int p3d_dense_conv2d_f16_residual(const void *in_h16, int B, int H, int W, int Cin, const void *packed_weight, int Cout,
+                                  int n_tile, int kh, int kw, int stride, int pad, int up, const float *scale,
+                                  const float *shift, int relu, void *out_h16, int out_C, int out_c0, float *out_nchw,
+                                  const void *res_h16, int res_C, int mode, int m_tiles, int32_t *status_dev,
+                                  p3d_stream_t stream);
+/* Bilinear upsampling (align_corners=True, integer scale s >= 1) of pixel H16 rows in_h16 [B, h, w, C] into channels
+ * [out_c0, out_c0 + C) of out_h16 [B, s h, s w, out_C]: Paddle's bilinear_interp_v2 on the merged pair values in fp32
+ * (ratio = (in - 1) / (out - 1), h2l (w2l a + w1l b) + h1l (w2l c + w1l d), no contraction), split again; s == 1 copies
+ * the pairs.  Status bit 0: an output left fp16's range.  C % 32 == 0 (whole input rows of 32-channel groups),
+ * out_c0 % 16 == 0, out_C % 32 == 0,
+ * out_c0 + C <= out_C, 16-byte aligned images (P3D_ERR_INVALID_ARG otherwise). */
+int p3d_upsample_bilinear_h16(const void *in_h16, int B, int h, int w, int C, int scale, void *out_h16, int out_C, int out_c0,
+                              int32_t *status_dev, p3d_stream_t stream);
+/* p3d_bev_pool_v2_dev into pixel H16 rows: out_h16 [B, Y, X, out_C] with channel z * c + ch of cell (y, x) (the layout of
+ * the planar output, one pixel per row), same accumulation, then split into (hi, lo'); status bit 0 on fp16 overflow.
+ * out_h16 is zero-filled here (empty cells and channels >= Z * c).  out_C % 32 == 0 and out_C >= Z * c
+ * (P3D_ERR_INVALID_ARG otherwise); c % 4 == 0, c <= 256, feat / out_h16 16-byte aligned (P3D_ERR_UNSUPPORTED). */
+int p3d_bev_pool_v2_dev_h16(const float *depth, const float *feat, const int32_t *ranks_depth, const int32_t *ranks_feat,
+                            const int32_t *ranks_bev, const int32_t *interval_lengths, const int32_t *interval_starts,
+                            const int32_t *counts_dev, int64_t capacity, int c, int B, int Z, int Y, int X, void *out_h16,
+                            int out_C, int32_t *status_dev, p3d_stream_t stream);
 
 /* SURVEY.md 8f-2: PillarFeatureNet with one PFNLayer
  * (models/voxel_encoders/pillar_encoder.py:156-210, :81-106) fused into one launch: voxels [n, M, F] + counts + coors

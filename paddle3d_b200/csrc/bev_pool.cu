@@ -12,6 +12,7 @@
 #include <stdlib.h>
 
 #include "common.cuh"
+#include "h16.cuh"
 
 namespace p3d {
 namespace {
@@ -77,8 +78,10 @@ __global__ void __launch_bounds__(256) bev_fwd_kernel(int cv, int n_intervals, c
 // DEV: the interval count is read from counts_dev[1] (the grid covers an upper bound; warps at or past the count exit), so
 // one captured graph serves every calibration.  PLANAR: the output is [B, Z * C, Y, X] with channel z * C + c, the layout
 // view_transform returns (torch.cat(bev.unbind(dim=2), 1) of the [B, C, Z, Y, X] pool), instead of [B, Z, Y, X, C];
-// yx = Y * X.  The accumulation is the same in every instantiation.
-template <int G, bool DEV = false, bool PLANAR = false>
+// yx = Y * X.  PIX: the output is pixel H16 rows [B, Y, X, row_c] (the image the dense fp16-pair convs read), channel
+// z * C + c of the planar layout at row b * Y*X + y * X + x, split into (hi, lo'); Z = cells along z.  The accumulation is
+// the same in every instantiation.
+template <int G, bool DEV = false, bool PLANAR = false, bool PIX = false>
 __global__ void __launch_bounds__(256) bev_fwd_warp_kernel(int cv, int n_intervals, const float *__restrict__ depth,
                                                            const float *__restrict__ feat,
                                                            const int *__restrict__ ranks_depth,
@@ -87,7 +90,7 @@ __global__ void __launch_bounds__(256) bev_fwd_warp_kernel(int cv, int n_interva
                                                            const int *__restrict__ interval_starts,
                                                            const int *__restrict__ interval_lengths,
                                                            float *__restrict__ out, const int *__restrict__ counts_dev = nullptr,
-                                                           int yx = 0) {
+                                                           int yx = 0, int Z = 1, int row_c = 0, int32_t *status = nullptr) {
   const int k = static_cast<int>((static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5);
   const int lane = threadIdx.x & 31;
   if (k >= (DEV ? __ldg(counts_dev + 1) : n_intervals)) return;
@@ -152,6 +155,26 @@ __global__ void __launch_bounds__(256) bev_fwd_warp_kernel(int cv, int n_interva
     d_cur = d_nxt;
     rf_nxt = rf_nn;
     rd_nxt = rd_nn;
+  }
+  if (PIX) {
+    // rank b * Z*Y*X + z * Y*X + (y * X + x): row b * Y*X + y * X + x, channels z * C + 4 (lane + 32 g) .. + 3, whose hi
+    // halves are 8 bytes at (ch / 32) * 128 + (ch % 32) * 2 of the row and the lo' halves 64 bytes further
+    const int rb = __ldg(ranks_bev + s), bz = rb / yx;
+    uint8_t *row = reinterpret_cast<uint8_t *>(out) + (static_cast<size_t>(bz / Z) * yx + rb % yx) * (4 * static_cast<size_t>(row_c));
+    bool ovf = false;
+#pragma unroll
+    for (int g = 0; g < G; ++g)
+      if (own[g]) {
+        const int ch = (bz % Z) * c + 4 * (lane + 32 * g);
+        __half2 h01, l01, h23, l23;
+        split_h16x2(acc[g].x, acc[g].y, h01, l01, ovf);
+        split_h16x2(acc[g].z, acc[g].w, h23, l23, ovf);
+        uint8_t *o = row + (ch >> 5) * 128 + (ch & 31) * 2;
+        *reinterpret_cast<uint2 *>(o) = make_uint2(*reinterpret_cast<const uint32_t *>(&h01), *reinterpret_cast<const uint32_t *>(&h23));
+        *reinterpret_cast<uint2 *>(o + 64) = make_uint2(*reinterpret_cast<const uint32_t *>(&l01), *reinterpret_cast<const uint32_t *>(&l23));
+      }
+    if (ovf && status) atomicOr(status, 1);
+    return;
   }
   if (PLANAR) {
     const int rb = __ldg(ranks_bev + s);  // b * Z*Y*X + z * Y*X + (y * X + x): plane (b * Z + z) * C + c
@@ -271,6 +294,36 @@ extern "C" int p3d_bev_pool_v2_dev(const float *depth, const float *feat, const 
     if (planar) P3D_BEV_DEV(2, true); else P3D_BEV_DEV(2, false);
   }
 #undef P3D_BEV_DEV
+  P3D_LAUNCH_CHECK();
+  return P3D_OK;
+}
+
+extern "C" int p3d_bev_pool_v2_dev_h16(const float *depth, const float *feat, const int32_t *ranks_depth,
+                                       const int32_t *ranks_feat, const int32_t *ranks_bev, const int32_t *interval_lengths,
+                                       const int32_t *interval_starts, const int32_t *counts_dev, int64_t capacity, int c,
+                                       int B, int Z, int Y, int X, void *out_h16, int out_C, int32_t *status_dev,
+                                       p3d_stream_t stream) {
+  if (!depth || !feat || !ranks_depth || !ranks_feat || !ranks_bev || !interval_lengths || !interval_starts || !counts_dev ||
+      !out_h16 || capacity < 0 || c < 1 || B < 1 || Z < 1 || Y < 1 || X < 1 || out_C < 32 || out_C % 32 ||
+      static_cast<long long>(Z) * c > out_C)
+    return P3D_ERR_INVALID_ARG;
+  const long long cells = static_cast<long long>(B) * Z * Y * X;
+  if (c % 4 || c > 256 || (reinterpret_cast<uintptr_t>(feat) & 15) || (reinterpret_cast<uintptr_t>(out_h16) & 15) ||
+      capacity > 0x7fffffffll || cells >= 0xffffffffll || static_cast<long long>(Y) * X > 0x7fffffffll)
+    return P3D_ERR_UNSUPPORTED;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  // empty cells and the channels from Z * c up to out_C stay zero
+  P3D_CUDA_CHECK(cudaMemsetAsync(out_h16, 0, static_cast<size_t>(B) * Y * X * out_C * 4, st));
+  const long long bound = capacity < cells ? capacity : cells;
+  if (bound == 0) return P3D_OK;
+  const int cv = c / 4, yx = Y * X;
+  const unsigned int blocks = div_up(bound * 32, 256);
+  const int n = static_cast<int>(bound);
+  // one instantiation for every c: G = 2 keeps 8 feature rows in flight per lane, which fits the registers without
+  // spilling (G = 1's 16 do not once the split is added); lanes past c / 4 only take part in the shuffles
+  bev_fwd_warp_kernel<2, true, false, true><<<blocks, 256, 0, st>>>(cv, n, depth, feat, ranks_depth, ranks_feat, ranks_bev,
+                                                                   interval_starts, interval_lengths, static_cast<float *>(out_h16),
+                                                                   counts_dev, yx, Z, out_C, status_dev);
   P3D_LAUNCH_CHECK();
   return P3D_OK;
 }

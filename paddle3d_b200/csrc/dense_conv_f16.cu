@@ -70,8 +70,14 @@ struct Params {
 struct ParamsP : Params {
   const uint8_t *packed_w2;
 };
-template <bool FUSE_P>
-using KParams = std::conditional_t<FUSE_P, ParamsP, Params>;
+// Parameters of residual launches (RES): the pixel H16 image [B, out_H, out_W, res_C] whose channels [0, cout) are added
+// after scale / shift and before ReLU
+struct ParamsR : Params {
+  const uint8_t *res_h16;
+  int res_C;
+};
+template <bool FUSE_P, bool RES = false>
+using KParams = std::conditional_t<FUSE_P, ParamsP, std::conditional_t<RES, ParamsR, Params>>;
 
 // FUSE_P: the tap-as-N GEMM of the output convs (out9 below) on a staged pair tile.  A 64-channel head's W2 image is
 // p3d_dense_conv2d_f16_pack_weights(taps 1, Cin 64, n_tile 32): 4 k-blocks of 2 KB; P rows have kPPitch fp32 columns
@@ -370,11 +376,15 @@ __device__ __forceinline__ void epilogue_pairs(const Params &p, const CUtensorMa
 // item holding both heads' W2 images), and stage P over the retired pair blocks for the epilogue thread: the output
 // convs' input image is never written.  The wgmma order is head_out9_kernel's, so P is bit-identical to what out9
 // computes from the image read back, and p3d_head_tap_sum finishes the convs.
-template <int N, int MT, bool HALO, bool FUSE_P = false>
+// RES (pair tile, up == 1): each consumer thread adds the residual of its own fragment elements, read from global memory
+// (the hi and lo' halves of two adjacent channels: 4 + 4 bytes), before ReLU; the residual-free instantiations compile
+// to the code they have without it.
+template <int N, int MT, bool HALO, bool FUSE_P = false, bool RES = false>
 __global__ void __launch_bounds__(kDenseThreads, 1)
     dense_conv_f16_kernel(const __grid_constant__ CUtensorMap in_map, const __grid_constant__ CUtensorMap out_map,
-                          const KParams<FUSE_P> p) {
+                          const KParams<FUSE_P, RES> p) {
   using C = Cfg<N, MT, HALO>;
+  static_assert(!(FUSE_P && RES), "a residual launch writes the pixel H16 image");
   static_assert(!FUSE_P || (N == 128 && MT == 1 && HALO && 2 * kP2Bytes == C::B_BYTES &&
                             2 * 64 * kPPitch * 4 <= C::PAIR_BYTES),
                 "fused P: two 64-channel heads' W2 images fill one weight slot; P fits over the pair blocks");
@@ -595,6 +605,24 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
       uint32_t after_bar;
       asm volatile("bar.sync %1, 128;\n\tmov.u32 %0, 0;" : "=r"(after_bar) : "r"(1 + cw) : "memory");
       const uint32_t sc_col = ss + after_bar + (lane & 3) * 8;
+      // RES: fragment row q + 8 h of M tile mt is pixel (iy + mt * kTH + h, ix); column pair (lane & 3) of 8-column group
+      // j is channel nt * N + 8 j + 2 (lane & 3), at byte (channel / 32) * 128 + (channel % 32) * 2 of a residual row
+      // (+ 64 for lo').  r_off: byte offset of that pixel's first column pair in the residual image (< 2^31, checked by
+      // the host), -1 outside the output; r_rem: channels of the N tile below cout
+      int r_off[MT][2], r_rem = 0;
+      if constexpr (RES) {
+        const int r_iy = im.ty0 + cw * 8 + (wtid >> 5) * 2, r_ix = im.tx0 + key;
+#pragma unroll
+        for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int Y = r_iy + mt * kTH + h;
+            r_off[mt][h] = r_ix < p.oW && Y < p.oH
+                               ? ((im.b * p.out_H + Y) * p.out_W + r_ix) * 4 * p.res_C + (im.nt * N / 32) * 128 + (lane & 3) * 4
+                               : -1;
+          }
+        r_rem = p.cout - im.nt * N;
+      }
       bool o[MT][2] = {};
 #pragma unroll
       for (int j = 0; j < N / 8; ++j) {
@@ -610,6 +638,18 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
             float v1 = fmaf(acc[mt * N + H + i + 1], kLoInv, acc[mt * N + i + 1]);
             v0 = fmaf(v0, sc0, sh0);
             v1 = fmaf(v1, sc1, sh1);
+            if constexpr (RES) {
+              // pixels outside the output and channels past cout are not stored: no residual read there
+              if (r_off[mt][h] >= 0 && j * 8 < r_rem) {
+                const uint8_t *rp = p.res_h16 + r_off[mt][h] + (j / 4) * 128 + (j & 3) * 16;
+                const uint32_t rh = __ldg(reinterpret_cast<const unsigned int *>(rp));
+                const uint32_t rl = __ldg(reinterpret_cast<const unsigned int *>(rp + 64));
+                const float2 fh = __half22float2(*reinterpret_cast<const __half2 *>(&rh));
+                const float2 fl = __half22float2(*reinterpret_cast<const __half2 *>(&rl));
+                v0 += fmaf(fl.x, kLoInv, fh.x);
+                v1 += fmaf(fl.y, kLoInv, fh.y);
+              }
+            }
             if (p.relu) v0 = fmaxf(v0, 0.f), v1 = fmaxf(v1, 0.f);
             __half2 hi, lo;
             split_h16x2(v0, v1, hi, lo, o[mt][h]);
@@ -810,12 +850,12 @@ inline int make_p_map(float *pbuf, int B, int H, int W, int p_groups, CUtensorMa
   return r == CUDA_SUCCESS ? P3D_OK : P3D_ERR_INVALID_ARG;
 }
 
-template <int N, int MT, bool HALO, bool FUSE_P = false>
-int launch(const CUtensorMap &map, const CUtensorMap &out_map, const KParams<FUSE_P> &p, cudaStream_t st) {
+template <int N, int MT, bool HALO, bool FUSE_P = false, bool RES = false>
+int launch(const CUtensorMap &map, const CUtensorMap &out_map, const KParams<FUSE_P, RES> &p, cudaStream_t st) {
   using C = Cfg<N, MT, HALO>;
   const size_t smem = static_cast<size_t>(C::NA) * C::A_BYTES + static_cast<size_t>(C::NB) * C::B_BYTES + C::STG_BYTES + 1024;
   if (smem > static_cast<size_t>(kSmemBudget)) return P3D_ERR_UNSUPPORTED;
-  auto kern = dense_conv_f16_kernel<N, MT, HALO, FUSE_P>;
+  auto kern = dense_conv_f16_kernel<N, MT, HALO, FUSE_P, RES>;
   P3D_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   const long long work = static_cast<long long>(p.B) * p.tiles_y * p.tiles_x * p.n_ntiles * (p.up > 1 ? p.up * p.up : 1);
   cudaLaunchConfig_t cfg = {};
@@ -1088,11 +1128,14 @@ extern "C" size_t p3d_dense_conv2d_f16_packed_weight_bytes(int taps, int Cin, in
   return align_up(tiles * taps * Cin * static_cast<size_t>(n_tile) * 4);
 }
 
-// mode: 0 auto (HALO for 3x3 stride 1 pad 1 convolutions, TAP otherwise), 1 force TAP; m_tiles: 0 auto, 1 or 2
-extern "C" int p3d_dense_conv2d_f16(const void *in_h16, int B, int H, int W, int Cin, const void *packed_weight, int Cout,
-                                    int n_tile, int kh, int kw, int stride, int pad, int up, const float *scale,
-                                    const float *shift, int relu, void *out_h16, int out_C, int out_c0, float *out_nchw,
-                                    int mode, int m_tiles, int32_t *status_dev, p3d_stream_t stream) {
+namespace {
+// mode: 0 auto (HALO for 3x3 stride 1 pad 1 convolutions, TAP otherwise), 1 force TAP; m_tiles: 0 auto, 1 or 2.  RES:
+// res_h16 / res_C as p3d_dense_conv2d_f16_residual takes them (checked by the caller)
+template <bool RES>
+int dense_conv2d_f16(const void *in_h16, int B, int H, int W, int Cin, const void *packed_weight, int Cout, int n_tile, int kh,
+                     int kw, int stride, int pad, int up, const float *scale, const float *shift, int relu, void *out_h16,
+                     int out_C, int out_c0, float *out_nchw, const void *res_h16, int res_C, int mode, int m_tiles,
+                     int32_t *status_dev, p3d_stream_t stream) {
   if (!in_h16 || !packed_weight || (!out_h16 && !out_nchw) || B < 1 || H < 1 || W < 1 || Cout < 1 || (mode != 0 && mode != 1))
     return P3D_ERR_INVALID_ARG;
   if (Cin < 32 || Cin % 32 || (n_tile != 64 && n_tile != 128)) return P3D_ERR_UNSUPPORTED;
@@ -1102,7 +1145,11 @@ extern "C" int p3d_dense_conv2d_f16(const void *in_h16, int B, int H, int W, int
   if ((reinterpret_cast<uintptr_t>(in_h16) & 15) || (reinterpret_cast<uintptr_t>(packed_weight) & 15) ||
       (reinterpret_cast<uintptr_t>(out_h16) & 15))
     return P3D_ERR_INVALID_ARG;
-  dcf::Params p;
+  dcf::KParams<false, RES> p;
+  if constexpr (RES) {
+    p.res_h16 = static_cast<const uint8_t *>(res_h16);
+    p.res_C = res_C;
+  }
   p.B = B;
   p.H = H;
   p.W = W;
@@ -1149,9 +1196,36 @@ extern "C" int p3d_dense_conv2d_f16(const void *in_h16, int B, int H, int W, int
   CUtensorMap omap = {};  // read only by the pair-tile epilogue of launches without fp32 planes
   if (!out_nchw && (rc = dcf::make_out_map(out_h16, B, p.oH, p.oW, out_C, up, &omap)) != P3D_OK) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (n_tile == 128) return halo ? dcf::launch<128, 1, true>(map, omap, p, st) : dcf::launch<128, 1, false>(map, omap, p, st);
-  if (mt == 2) return halo ? dcf::launch<64, 2, true>(map, omap, p, st) : dcf::launch<64, 2, false>(map, omap, p, st);
-  return halo ? dcf::launch<64, 1, true>(map, omap, p, st) : dcf::launch<64, 1, false>(map, omap, p, st);
+  if (n_tile == 128)
+    return halo ? dcf::launch<128, 1, true, false, RES>(map, omap, p, st) : dcf::launch<128, 1, false, false, RES>(map, omap, p, st);
+  if (mt == 2)
+    return halo ? dcf::launch<64, 2, true, false, RES>(map, omap, p, st) : dcf::launch<64, 2, false, false, RES>(map, omap, p, st);
+  return halo ? dcf::launch<64, 1, true, false, RES>(map, omap, p, st) : dcf::launch<64, 1, false, false, RES>(map, omap, p, st);
+}
+}  // namespace
+
+extern "C" int p3d_dense_conv2d_f16(const void *in_h16, int B, int H, int W, int Cin, const void *packed_weight, int Cout,
+                                    int n_tile, int kh, int kw, int stride, int pad, int up, const float *scale,
+                                    const float *shift, int relu, void *out_h16, int out_C, int out_c0, float *out_nchw,
+                                    int mode, int m_tiles, int32_t *status_dev, p3d_stream_t stream) {
+  return dense_conv2d_f16<false>(in_h16, B, H, W, Cin, packed_weight, Cout, n_tile, kh, kw, stride, pad, up, scale, shift, relu,
+                                 out_h16, out_C, out_c0, out_nchw, nullptr, 0, mode, m_tiles, status_dev, stream);
+}
+
+// p3d_dense_conv2d_f16 with a residual added before ReLU (ResNet BasicBlock conv2): pixel H16 res_h16 [B, oH, oW, res_C]
+extern "C" int p3d_dense_conv2d_f16_residual(const void *in_h16, int B, int H, int W, int Cin, const void *packed_weight,
+                                             int Cout, int n_tile, int kh, int kw, int stride, int pad, int up,
+                                             const float *scale, const float *shift, int relu, void *out_h16, int out_C,
+                                             int out_c0, float *out_nchw, const void *res_h16, int res_C, int mode,
+                                             int m_tiles, int32_t *status_dev, p3d_stream_t stream) {
+  if (!res_h16 || (reinterpret_cast<uintptr_t>(res_h16) & 15)) return P3D_ERR_INVALID_ARG;
+  if (up != 1 || out_nchw || !out_h16 || out_c0 % 32 || res_C % 32) return P3D_ERR_UNSUPPORTED;
+  if (res_C < Cout) return P3D_ERR_INVALID_ARG;
+  // the kernel addresses the residual with 32-bit byte offsets
+  const long long oh = (H + 2 * pad - kh) / (stride > 0 ? stride : 1) + 1, ow = (W + 2 * pad - kw) / (stride > 0 ? stride : 1) + 1;
+  if (static_cast<long long>(B) * oh * ow * 4 * res_C > 0x7fffffffll) return P3D_ERR_UNSUPPORTED;
+  return dense_conv2d_f16<true>(in_h16, B, H, W, Cin, packed_weight, Cout, n_tile, kh, kw, stride, pad, up, scale, shift, relu,
+                                out_h16, out_C, out_c0, out_nchw, res_h16, res_C, mode, m_tiles, status_dev, stream);
 }
 
 // Output convs of the CenterHead, 9 taps in the GEMM's N dimension (dcf::out9 above): group g convolves input channels

@@ -18,10 +18,13 @@ COMMON_HEADS = (("reg", 2), ("height", 1), ("dim", 3), ("rot", 2), ("vel", 2))  
 class _Conv:
     """Conv2D / Conv2DTranspose (+ BatchNorm2D eval) (+ ReLU) with seeded parameters."""
 
-    def __init__(self, cin, cout, k, stride=1, padding=0, bias=False, bn_eps=None, relu=True, up=1, f16=True, transposed=False):
+    def __init__(self, cin, cout, k, stride=1, padding=0, bias=False, bn_eps=None, relu=True, up=1, f16=True, transposed=False,
+                 cin_pad=None):
         """transposed: a stride-1 Conv2DTranspose (weight [Cin, Cout, k, k]); with k = 1 it runs as a 1x1 conv whose packed
-        weight is the transpose (up > 1 implies a transposed conv)."""
+        weight is the transpose (up > 1 implies a transposed conv).  cin_pad: the packed weight is zero-padded on Cin to
+        this many channels (an input image whose rows carry zero padding channels); the exported weight keeps cin."""
         self.cin, self.cout, self.k, self.stride, self.padding, self.up = cin, cout, k, stride, padding, up
+        self.cin_pad = cin_pad
         self.transposed = transposed or up > 1
         self.has_bias, self.bn_eps, self.relu = bias, bn_eps, relu
         self.f16 = f16 and cout >= 16  # the 1-3 channel output convs of the heads run on the CUDA cores (forward)
@@ -64,8 +67,13 @@ class _Conv:
             pack = dc.pack_deconv_weight_f16 if self.transposed else dc.pack_conv_weight_f16
         else:
             pack = dc.pack_deconv_weight if self.transposed else dc.pack_conv_weight
+        wd = w
+        if self.cin_pad and self.cin_pad > cin:
+            ax = 0 if self.transposed else 1
+            wd = np.zeros(shape[:ax] + (self.cin_pad,) + shape[ax + 1:], np.float32)
+            wd[(slice(None),) * ax + (slice(0, cin),)] = w
         self.dev = dict(
-            packed=pack(torch.from_numpy(w).to(device), self.n_tile),
+            packed=pack(torch.from_numpy(wd).to(device), self.n_tile),
             scale=torch.from_numpy(s.astype(np.float32)).to(device) if p["bn"] is not None else None,
             shift=torch.from_numpy(t.astype(np.float32)).to(device) if (p["bn"] is not None or b is not None) else None)
         return self
@@ -153,7 +161,12 @@ class SecondTrunk:
 class DenseRPNHead:
     def __init__(self, in_channels=256, out_channels=(128, 256), layer_nums=(5, 5), downsample_strides=(1, 2),
                  fpn_out_channels=(256, 256), upsample_strides=(1, 2), tasks=(1, 2, 2, 1, 2, 2), share_conv_channel=64,
-                 f16=True, with_velocity=True, bev_depth=2):
+                 f16=True, with_velocity=True, bev_depth=2, trunk=None):
+        """trunk: the network between the BEV image and the shared conv (None: SecondBackbone + SecondFPN from the
+        arguments above); another object with SecondTrunk's __call__(x, shape, first=None) / fpn_channels / convs() /
+        export_numpy() contract, on pixel fp16-pair rows with bev_depth 1 (bevdet.BEVDetEncoder)."""
+        if trunk is not None and (not f16 or bev_depth > 1):
+            raise ValueError("a custom trunk runs on the fp16-pair path with bev_depth 1")
         self.tasks = list(tasks)
         self.in_channels, self.bev_depth = in_channels, bev_depth
         self.num_classes = list(tasks)        # CenterHead.num_classes (center_head.py:64)
@@ -166,9 +179,13 @@ class DenseRPNHead:
         def conv(*a, **k):
             return _Conv(*a, f16=f16, **k)
         bn5 = 1e-5
-        self.trunk = SecondTrunk(in_channels, out_channels, layer_nums, downsample_strides, fpn_out_channels,
-                                 upsample_strides, use_conv_for_no_stride=True, f16=f16)
-        self.blocks, self.deblocks, self.fpn_channels = self.trunk.blocks, self.trunk.deblocks, self.trunk.fpn_channels
+        if trunk is None:
+            trunk = SecondTrunk(in_channels, out_channels, layer_nums, downsample_strides, fpn_out_channels,
+                                upsample_strides, use_conv_for_no_stride=True, f16=f16)
+            self.blocks, self.deblocks = trunk.blocks, trunk.deblocks
+        else:
+            self.blocks = self.deblocks = None
+        self.trunk, self.fpn_channels = trunk, trunk.fpn_channels
         self.shared = conv(self.fpn_channels, share_conv_channel, 3, 1, 1, bias=True, bn_eps=bn5)
         self.heads = []  # per task: list of (name, ConvModule 64->64, final conv 64->classes)
         for ncls in self.tasks:

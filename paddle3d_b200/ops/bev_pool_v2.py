@@ -149,3 +149,21 @@ def bev_pool_v2_dev(depth, feat, prepared, bev_feat_shape, planar=False, out=Non
                                     rb.numel(), C, B, Z, Y, X, int(bool(planar)), ptr(out), stream(feat.device)),
           "bev_pool_v2_dev")
     return out
+
+
+def bev_pool_v2_dev_h16(depth, feat, prepared, bev_feat_shape, out_channels=None, out=None):
+    """bev_pool_v2_dev straight into pixel fp16-pair rows (p3d_bev_pool_v2_dev_h16): [B*Y*X, 2*out_channels] float16,
+    channel z * C + c of a cell's row (the planar layout's channel order); out_channels defaults to Z * C rounded up to a
+    multiple of 32, the padding channels are zero."""
+    from .sparse_nn import status_tensor
+    depth = require_cuda(depth, "depth", torch.float32)
+    feat = require_cuda(feat, "feat", torch.float32)
+    rb, rd, rf, st, ln, counts = prepared[:6]
+    B, Z, Y, X, C = [int(s) for s in bev_feat_shape]
+    oc = int(out_channels or (Z * C + 31) // 32 * 32)
+    if out is None:
+        out = torch.empty((B * Y * X, 2 * oc), dtype=torch.float16, device=feat.device)
+    check(lib().p3d_bev_pool_v2_dev_h16(ptr(depth), ptr(feat), ptr(rd), ptr(rf), ptr(rb), ptr(ln), ptr(st), ptr(counts),
+                                        rb.numel(), C, B, Z, Y, X, ptr(out), oc, ptr(status_tensor(feat.device)),
+                                        stream(feat.device)), "bev_pool_v2_dev_h16")
+    return out

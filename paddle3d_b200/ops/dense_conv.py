@@ -149,10 +149,13 @@ def pack_deconv_weight_f16(weight, n_tile):
 
 
 def dense_conv2d_f16(x_h16, shape, packed, cout, n_tile, kernel, stride=1, padding=0, up=1, scale=None, shift=None,
-                     relu=False, out_h16=None, out_channels=None, out_c0=0, want_nchw=False, mode=0, m_tiles=0):
+                     relu=False, out_h16=None, out_channels=None, out_c0=0, want_nchw=False, mode=0, m_tiles=0,
+                     residual=None, res_channels=None):
     """x_h16 [B*H*W, 2*Cin] float16 pixel H16 rows; shape = (B, H, W, Cin).  Returns (out_h16 or None, out_nchw or None,
     (B, oH, oW)).  out_h16: an existing [B*oH*oW, 2*out_channels] buffer to write channels [out_c0, out_c0 + cout) of
-    (channel concat), or None to allocate one; want_nchw adds fp32 planes.  mode 1 forces per-tap loads."""
+    (channel concat), or None to allocate one; want_nchw adds fp32 planes.  mode 1 forces per-tap loads.  residual: pixel
+    H16 rows [B*oH*oW, 2*res_channels] (default cout channels) whose channels [0, cout) are added before ReLU
+    (p3d_dense_conv2d_f16_residual: H16 output only)."""
     x_h16 = require_cuda(x_h16, "x_h16", torch.float16)
     b, h, w, cin = [int(v) for v in shape]
     if up > 1:
@@ -168,7 +171,33 @@ def dense_conv2d_f16(x_h16, shape, packed, cout, n_tile, kernel, stride=1, paddi
     if out_h16 is None and not want_nchw:
         out_h16 = torch.empty((b * oh * ow, 2 * oc), dtype=torch.float16, device=dev)
     out_nchw = torch.empty((b, cout, oh, ow), dtype=torch.float32, device=dev) if want_nchw else None
+    if residual is not None:
+        residual = require_cuda(residual, "residual", torch.float16)
+        rc = int(res_channels or cout)
+        if tuple(residual.shape) != (b * oh * ow, 2 * rc):
+            raise ValueError("residual rows %s, want (%d, %d)" % (tuple(residual.shape), b * oh * ow, 2 * rc))
+        check(lib().p3d_dense_conv2d_f16_residual(
+            ptr(x_h16), b, h, w, cin, ptr(packed), int(cout), int(n_tile), kh, kw, st, pd, int(up), ptr(scale), ptr(shift),
+            int(relu), ptr(out_h16), oc, int(out_c0), ptr(out_nchw), ptr(residual), rc, int(mode), int(m_tiles),
+            ptr(_status(dev)), stream(dev)), "dense_conv2d_f16_residual")
+        return out_h16, out_nchw, (b, oh, ow)
     check(lib().p3d_dense_conv2d_f16(ptr(x_h16), b, h, w, cin, ptr(packed), int(cout), int(n_tile), kh, kw, st, pd, int(up),
                                      ptr(scale), ptr(shift), int(relu), ptr(out_h16), oc, int(out_c0), ptr(out_nchw),
                                      int(mode), int(m_tiles), ptr(_status(dev)), stream(dev)), "dense_conv2d_f16")
     return out_h16, out_nchw, (b, oh, ow)
+
+
+def upsample_bilinear_h16(x_h16, shape, scale, out_h16=None, out_channels=None, out_c0=0):
+    """nn.Upsample(scale_factor=scale, mode='bilinear', align_corners=True) on pixel H16 rows x_h16 [B*h*w, 2*C], shape =
+    (B, h, w, C) (p3d_upsample_bilinear_h16; scale 1 copies).  Writes channels [out_c0, out_c0 + C) of out_h16 [B*sh*sw,
+    2*out_channels] (None: a new C-channel image).  Returns (out_h16, (B, s h, s w))."""
+    x_h16 = require_cuda(x_h16, "x_h16", torch.float16)
+    b, h, w, c = [int(v) for v in shape]
+    s = int(scale)
+    oc = int(out_channels or c)
+    dev = x_h16.device
+    if out_h16 is None:
+        out_h16 = torch.empty((b * h * s * w * s, 2 * oc), dtype=torch.float16, device=dev)
+    check(lib().p3d_upsample_bilinear_h16(ptr(x_h16), b, h, w, c, s, ptr(out_h16), oc, int(out_c0), ptr(_status(dev)),
+                                          stream(dev)), "upsample_bilinear_h16")
+    return out_h16, (b, h * s, w * s)

@@ -675,3 +675,106 @@ PD_BUILD_OP(p3d_bev_pool_v2_dev)
     .SetKernelFn(PD_KERNEL(p3d_bev_pool_v2_dev_op))
     .SetInferShapeFn(PD_INFER_SHAPE(PoolDevInferShape))
     .SetInferDtypeFn(PD_INFER_DTYPE(PoolDevInferDtype));
+
+// p3d_dense_conv2d_f16 with a residual added before ReLU (CustomResNet BasicBlock: relu(bn2(conv2(.)) + identity)):
+// RESIDUAL [B*oH*oW, 2*res_channels] FLOAT16 pixel rows, channels [0, cout) added; H16 output, stride-1 or -2 conv.
+std::vector<paddle::Tensor> p3d_dense_conv2d_f16_residual_op(const paddle::Tensor &image, const paddle::Tensor &weight,
+                                                             const paddle::Tensor &scale, const paddle::Tensor &shift,
+                                                             const paddle::Tensor &residual, const paddle::Tensor &status,
+                                                             const std::vector<int> &bhwc, const int cout, const int n_tile,
+                                                             const int kernel, const int stride, const int pad, const int relu,
+                                                             const int out_channels, const int out_c0, const int res_channels) {
+  P3D_CHECK_GPU(image);
+  const int B = bhwc[0], H = bhwc[1], W = bhwc[2], Cin = bhwc[3];
+  const int oH = (H + 2 * pad - kernel) / stride + 1, oW = (W + 2 * pad - kernel) / stride + 1;
+  auto out = paddle::empty({static_cast<int64_t>(B) * oH * oW, 2 * out_channels}, paddle::DataType::FLOAT16, paddle::GPUPlace());
+  P3D_CALL(p3d_dense_conv2d_f16_residual(image.data(), B, H, W, Cin, weight.data(), cout, n_tile, kernel, kernel, stride, pad, 1,
+                                         scale.data<float>(), shift.data<float>(), relu, out.data(), out_channels, out_c0, nullptr,
+                                         residual.data(), res_channels, 0, 0, const_cast<int *>(status.data<int>()),
+                                         image.stream()));
+  return {out};
+}
+std::vector<std::vector<int64_t>> DcF16ResInferShape(std::vector<int64_t> im, std::vector<int64_t> w, std::vector<int64_t> sc,
+                                                     std::vector<int64_t> sh, std::vector<int64_t> res, std::vector<int64_t> st,
+                                                     const std::vector<int> &bhwc, const int &cout, const int &n_tile,
+                                                     const int &kernel, const int &stride, const int &pad, const int &relu,
+                                                     const int &out_channels, const int &out_c0, const int &res_channels) {
+  const int64_t oH = (bhwc[1] + 2 * pad - kernel) / stride + 1, oW = (bhwc[2] + 2 * pad - kernel) / stride + 1;
+  return {{bhwc[0] * oH * oW, 2 * static_cast<int64_t>(out_channels)}};
+}
+std::vector<paddle::DataType> DcF16ResInferDtype(paddle::DataType im, paddle::DataType w, paddle::DataType sc,
+                                                 paddle::DataType sh, paddle::DataType res, paddle::DataType st) {
+  return {paddle::DataType::FLOAT16};
+}
+PD_BUILD_OP(p3d_dense_conv2d_f16_residual)
+    .Inputs({"IMAGE", "WEIGHT", "SCALE", "SHIFT", "RESIDUAL", "STATUS"})
+    .Outputs({"OUT"})
+    .Attrs({"bhwc: std::vector<int>", "cout: int", "n_tile: int", "kernel: int", "stride: int", "pad: int", "relu: int",
+            "out_channels: int", "out_c0: int", "res_channels: int"})
+    .SetKernelFn(PD_KERNEL(p3d_dense_conv2d_f16_residual_op))
+    .SetInferShapeFn(PD_INFER_SHAPE(DcF16ResInferShape))
+    .SetInferDtypeFn(PD_INFER_DTYPE(DcF16ResInferDtype));
+
+// nn.Upsample(scale_factor, mode='bilinear', align_corners=True) of FPN_LSS on pixel fp16-pair rows: IMAGE [B*h*w, 2*C]
+// FLOAT16 -> [B*sh*sw, 2*out_channels] with channels [out_c0, out_c0 + C) written (the rest of a new tensor is left as
+// allocated: callers that concatenate write the other channels).
+std::vector<paddle::Tensor> p3d_upsample_bilinear_h16_op(const paddle::Tensor &image, const paddle::Tensor &status,
+                                                         const std::vector<int> &bhwc, const int scale, const int out_channels,
+                                                         const int out_c0) {
+  P3D_CHECK_GPU(image);
+  const int B = bhwc[0], h = bhwc[1], w = bhwc[2], C = bhwc[3];
+  auto out = paddle::empty({static_cast<int64_t>(B) * h * scale * w * scale, 2 * out_channels}, paddle::DataType::FLOAT16,
+                           paddle::GPUPlace());
+  P3D_CALL(p3d_upsample_bilinear_h16(image.data(), B, h, w, C, scale, out.data(), out_channels, out_c0,
+                                     const_cast<int *>(status.data<int>()), image.stream()));
+  return {out};
+}
+std::vector<std::vector<int64_t>> UpH16InferShape(std::vector<int64_t> im, std::vector<int64_t> st, const std::vector<int> &bhwc,
+                                                  const int &scale, const int &out_channels, const int &out_c0) {
+  return {{static_cast<int64_t>(bhwc[0]) * bhwc[1] * scale * bhwc[2] * scale, 2 * static_cast<int64_t>(out_channels)}};
+}
+std::vector<paddle::DataType> UpH16InferDtype(paddle::DataType im, paddle::DataType st) { return {paddle::DataType::FLOAT16}; }
+PD_BUILD_OP(p3d_upsample_bilinear_h16)
+    .Inputs({"IMAGE", "STATUS"})
+    .Outputs({"OUT"})
+    .Attrs({"bhwc: std::vector<int>", "scale: int", "out_channels: int", "out_c0: int"})
+    .SetKernelFn(PD_KERNEL(p3d_upsample_bilinear_h16_op))
+    .SetInferShapeFn(PD_INFER_SHAPE(UpH16InferShape))
+    .SetInferDtypeFn(PD_INFER_DTYPE(UpH16InferDtype));
+
+// bev_pool_v2 with the interval count on the device straight into pixel fp16-pair rows [B*Y*X, 2*out_channels] FLOAT16
+// (channel z * C + c of a cell; empty cells and channels >= Z * C zero), the first dense conv's input; bzyx = (B, Z, Y, X).
+std::vector<paddle::Tensor> p3d_bev_pool_v2_dev_h16_op(const paddle::Tensor &depth, const paddle::Tensor &feat,
+                                                       const paddle::Tensor &ranks_depth, const paddle::Tensor &ranks_feat,
+                                                       const paddle::Tensor &ranks_bev, const paddle::Tensor &interval_lengths,
+                                                       const paddle::Tensor &interval_starts, const paddle::Tensor &counts,
+                                                       const paddle::Tensor &status, const std::vector<int> &bzyx,
+                                                       const int out_channels) {
+  P3D_CHECK_GPU(feat);
+  const int c = feat.shape()[feat.shape().size() - 1];
+  auto out = paddle::empty({static_cast<int64_t>(bzyx[0]) * bzyx[2] * bzyx[3], 2 * out_channels}, paddle::DataType::FLOAT16,
+                           paddle::GPUPlace());
+  P3D_CALL(p3d_bev_pool_v2_dev_h16(depth.data<float>(), feat.data<float>(), ranks_depth.data<int>(), ranks_feat.data<int>(),
+                                   ranks_bev.data<int>(), interval_lengths.data<int>(), interval_starts.data<int>(),
+                                   counts.data<int>(), ranks_bev.shape()[0], c, bzyx[0], bzyx[1], bzyx[2], bzyx[3], out.data(),
+                                   out_channels, const_cast<int *>(status.data<int>()), feat.stream()));
+  return {out};
+}
+std::vector<std::vector<int64_t>> PoolH16InferShape(std::vector<int64_t> d, std::vector<int64_t> f, std::vector<int64_t> a,
+                                                    std::vector<int64_t> b, std::vector<int64_t> e, std::vector<int64_t> g,
+                                                    std::vector<int64_t> h, std::vector<int64_t> k, std::vector<int64_t> st,
+                                                    const std::vector<int> &bzyx, const int &out_channels) {
+  return {{static_cast<int64_t>(bzyx[0]) * bzyx[2] * bzyx[3], 2 * static_cast<int64_t>(out_channels)}};
+}
+std::vector<paddle::DataType> PoolH16InferDtype(paddle::DataType d, paddle::DataType f, paddle::DataType a, paddle::DataType b,
+                                                paddle::DataType e, paddle::DataType g, paddle::DataType h, paddle::DataType k,
+                                                paddle::DataType st) {
+  return {paddle::DataType::FLOAT16};
+}
+PD_BUILD_OP(p3d_bev_pool_v2_dev_h16)
+    .Inputs({"DEPTH", "FEAT", "RANKS_DEPTH", "RANKS_FEAT", "RANKS_BEV", "INTERVAL_LENGTHS", "INTERVAL_STARTS", "COUNTS", "STATUS"})
+    .Outputs({"OUT"})
+    .Attrs({"bzyx: std::vector<int>", "out_channels: int"})
+    .SetKernelFn(PD_KERNEL(p3d_bev_pool_v2_dev_h16_op))
+    .SetInferShapeFn(PD_INFER_SHAPE(PoolH16InferShape))
+    .SetInferDtypeFn(PD_INFER_DTYPE(PoolH16InferDtype));
