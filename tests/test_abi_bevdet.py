@@ -38,6 +38,31 @@ def test_residual_conv_argument_checks():
     assert f(p, 1, 8, 8, 64, p, 64, 64, 3, 3, 1, 1, 1, None, None, 1, p, 64, 0, None, p, 64, 2, 0, None, None) == -1
 
 
+def test_residual_offset_guard():
+    """The kernel addresses the residual with 32-bit byte offsets: a residual image of B * oH * oW * 4 * res_C bytes past
+    0x7fffffff is refused (P3D_ERR_UNSUPPORTED), one at or below it is not, and the count is on the output's size
+    (stride 2 halves each side).  Every call passes mode 2, which the conv's own argument checks refuse
+    (P3D_ERR_INVALID_ARG) after the guard and before any tensor map or launch: -4 is the guard, -1 a call past it."""
+    L = _lib()
+    buf = ctypes.create_string_buffer(256)
+    p = ctypes.addressof(buf) + (-ctypes.addressof(buf)) % 16
+
+    def call(B, H, W, stride, res_c):
+        return L.p3d_dense_conv2d_f16_residual(p, B, H, W, 64, p, 64, 64, 3, 3, stride, 1, 1, None, None, 1, p, 64, 0, None,
+                                               p, res_c, 2, 0, None, None)
+    limit = 0x7fffffff
+    assert 2 * 2048 * 2048 * 4 * 64 == limit + 1
+    assert call(2, 2048, 2048, 1, 64) == -4       # 2^23 pixels x 256 bytes
+    assert call(1, 1, 2 ** 23, 1, 64) == -4       # the same bytes in one pixel row
+    assert (2 ** 23 - 1) * 4 * 64 == limit + 1 - 256
+    assert call(1, 1, 2 ** 23 - 1, 1, 64) == -1   # one pixel fewer: past the guard
+    assert call(1, 4096, 4096, 2, 128) == -4      # 2048 x 2048 outputs x 512 bytes
+    assert call(1, 4096, 4096, 2, 64) == -1       # 2^32 bytes counted on the input, 2^30 on the output
+    assert 5592406 * 4 * 96 - limit == 257 and limit - 5592405 * 4 * 96 == 127
+    assert call(1, 1, 5592406, 1, 96) == -4       # one pixel row of 5592406 x 384 bytes
+    assert call(1, 1, 5592405, 1, 96) == -1
+
+
 def test_upsample_and_pixel_pool_argument_checks():
     L = _lib()
     buf = ctypes.create_string_buffer(256)
