@@ -443,6 +443,15 @@ int p3d_bev_pool_v2_dev_h16(const float *depth, const float *feat, const int32_t
                             const int32_t *ranks_bev, const int32_t *interval_lengths, const int32_t *interval_starts,
                             const int32_t *counts_dev, int64_t capacity, int c, int B, int Z, int Y, int X, void *out_h16,
                             int out_C, int32_t *status_dev, p3d_stream_t stream);
+/* BEVDet4D's shift_feature on pixel H16 rows: channels [0, C) of in_h16 [B, h, w, in_C] resampled at the grid of the
+ * affine tf_dev [B, 6] (device fp32, row-major rows 0 and 1 of the 3x3 BEV-pixel transform: g = tf (x, y, 1)),
+ * normalised by / (w - 1) * 2 - 1 and sampled as grid_sample(bilinear, padding_mode='zeros', align_corners=True), in fp32
+ * without contraction; written to channels [out_c0, out_c0 + C) of out_h16 [B, h, w, out_C].  Taps outside the image
+ * (non-finite coordinates included) contribute 0 and are not read.  in_h16 may be out_h16 when the channel ranges are
+ * disjoint.  Status bit 0: an output left fp16's range.  C % 16 == 0, C <= in_C, in_C % 32 == 0, out_C % 32 == 0,
+ * out_c0 % 16 == 0, out_c0 + C <= out_C, h, w >= 2, 16-byte aligned images (P3D_ERR_INVALID_ARG otherwise). */
+int p3d_bev_shift_h16(const void *in_h16, int B, int h, int w, int in_C, int C, const float *tf_dev, void *out_h16, int out_C,
+                      int out_c0, int32_t *status_dev, p3d_stream_t stream);
 
 /* SURVEY.md 8f-2: PillarFeatureNet with one PFNLayer
  * (models/voxel_encoders/pillar_encoder.py:156-210, :81-106) fused into one launch: voxels [n, M, F] + counts + coors

@@ -96,6 +96,7 @@ SIGNATURES = {
     "p3d_upsample_bilinear_h16": (_int, [_vp, _int, _int, _int, _int, _int, _vp, _int, _int, _vp, _vp]),
     "p3d_bev_pool_v2_dev_h16": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _int, _int, _int, _int, _int, _vp, _int,
                                        _vp, _vp]),
+    "p3d_bev_shift_h16": (_int, [_vp, _int, _int, _int, _int, _int, _vp, _vp, _int, _int, _vp, _vp]),
     "p3d_dense_conv2d_split": (_int, [_vp, _int, _int, _int, _int, _vp, _int, _int, _int, _int, _int, _int, _int, _vp, _vp,
                                       _int, _vp, _int, _int, _vp, _vp]),
     "p3d_sparse_conv_gather_gemm_tf32x3_ws": (_int, [_vp, _vp, _vp, _i64, _int, _int, _int, _vp, _vp, _vp, _vp, _int, _vp,

@@ -44,24 +44,33 @@ class BEVDetEncoder:
     in_pad: channels of the input image rows (the pool image's, in_channels rounded up to 32); the first stage's weights
     are zero-padded on Cin to it once, when they are packed."""
 
-    def __init__(self, in_channels, num_channels, strides, blocks, fpn_out, scale_factor, input_feature_index,
-                 extra_upsample, bn_eps=1e-5, in_pad=None):
+    def __init__(self, in_channels, num_channels, strides, blocks, fpn_out, scale_factor=None, input_feature_index=None,
+                 extra_upsample=None, bn_eps=1e-5, in_pad=None, row_pad=None):
+        """fpn_out None: CustomResNet alone (BEVDet4D's pre_process net).  row_pad: channels of the rows every conv writes
+        (None: its Cout); every conv's weights are zero-padded on Cin to the rows it reads, whose padding channels the
+        caller keeps zero (pre_process writes 80 channels into 96-channel rows)."""
         self.in_channels, self.in_pad = in_channels, in_pad or round32(in_channels)
+        self.row_pad = row_pad
         self.scale_factor, self.extra_upsample = scale_factor, extra_upsample
-        self.index = tuple(input_feature_index)
         self.stages = []
-        cin = in_channels
-        for si, (cout, s) in enumerate(zip(num_channels, strides)):
-            pad = self.in_pad if si == 0 else None
+        cin, rows = in_channels, self.in_pad
+        for cout, s in zip(num_channels, strides):
+            out_rows = row_pad or cout
+            pad = rows if rows != cin else None
+            rpad = out_rows if out_rows != cout else None
             stage = [dict(conv1=_Conv(cin, cout, 3, s, 1, bn_eps=bn_eps, cin_pad=pad),
-                          conv2=_Conv(cout, cout, 3, 1, 1, bn_eps=bn_eps),  # ReLU after the residual
+                          conv2=_Conv(cout, cout, 3, 1, 1, bn_eps=bn_eps, cin_pad=rpad),  # ReLU after the residual
                           down=_Conv(cin, cout, 3, s, 1, bias=True, relu=False, cin_pad=pad))]
             for _ in range(blocks - 1):
-                stage.append(dict(conv1=_Conv(cout, cout, 3, 1, 1, bn_eps=bn_eps), conv2=_Conv(cout, cout, 3, 1, 1, bn_eps=bn_eps),
-                                  down=None))
+                stage.append(dict(conv1=_Conv(cout, cout, 3, 1, 1, bn_eps=bn_eps, cin_pad=rpad),
+                                  conv2=_Conv(cout, cout, 3, 1, 1, bn_eps=bn_eps, cin_pad=rpad), down=None))
             self.stages.append(stage)
-            cin = cout
+            cin, rows = cout, out_rows
         self.stage_channels = tuple(num_channels)
+        self.fpn, self.fpn_channels, self.index, self.cat_channels = [], None, None, None
+        if fpn_out is None:
+            return
+        self.index = tuple(input_feature_index)
         self.cat_channels = num_channels[self.index[0]] + num_channels[self.index[1]]
         mid = fpn_out * (2 if extra_upsample else 1)
         self.fpn = [_Conv(self.cat_channels, mid, 3, 1, 1, bn_eps=bn_eps), _Conv(mid, mid, 3, 1, 1, bn_eps=bn_eps),
@@ -81,27 +90,33 @@ class BEVDetEncoder:
                     fpn=[c.np for c in self.fpn], fpn_index=self.index, scale_factor=self.scale_factor,
                     extra_upsample=self.extra_upsample)
 
-    @staticmethod
-    def _block(blk, x, shape):
+    def _block(self, blk, x, shape, bufs=None, out=None):
+        """One BasicBlock.  bufs: dict conv name -> preallocated output rows (None / missing: allocated); out = (rows,
+        channels, c0): conv2 writes channels [c0, c0 + Cout) of those rows instead."""
         b = shape[0]
-        t, _, (_, oh, ow) = blk["conv1"](x, shape)
+        bufs = bufs or {}
         cout = blk["conv1"].cout
-        idn = x if blk["down"] is None else blk["down"](x, shape)[0]
-        y, _, _ = blk["conv2"](t, (b, oh, ow, cout), residual=idn, res_channels=cout)
-        return y, (b, oh, ow, cout)
+        rows = self.row_pad or cout
+        t, _, (_, oh, ow) = blk["conv1"](x, shape, out_h16=bufs.get("conv1"), out_channels=rows)
+        idn = x if blk["down"] is None else blk["down"](x, shape, out_h16=bufs.get("down"), out_channels=rows)[0]
+        o, oc, c0 = out or (bufs.get("conv2"), rows, 0)
+        y, _, _ = blk["conv2"](t, (b, oh, ow, rows), residual=idn, res_channels=rows, out_h16=o, out_channels=oc, out_c0=c0)
+        return y, (b, oh, ow, rows)
 
-    def backbone(self, x, shape):
-        """CustomResNet: the pixel image of every stage's output, [(rows, (B, H, W, C))]."""
+    def backbone(self, x, shape, bufs=None, out=None):
+        """CustomResNet: the pixel image of every stage's output, [(rows, (B, H, W, C))].  bufs: per stage, per block, the
+        _block buffers; out: where the last conv writes (_block)."""
         feats = []
-        for stage in self.stages:
-            for blk in stage:
-                x, shape = self._block(blk, x, shape)
+        for si, stage in enumerate(self.stages):
+            for bi, blk in enumerate(stage):
+                last = si == len(self.stages) - 1 and bi == len(stage) - 1
+                x, shape = self._block(blk, x, shape, bufs[si][bi] if bufs else None, out if last else None)
             feats.append((x, shape))
         return feats
 
     def __call__(self, x, shape, first=None):
         """x: pixel fp16-pair rows [B*H*W, 2*in_pad], shape = (B, H, W, in_pad).  Returns (FPN_LSS output rows, shape)."""
-        if first is not None or int(shape[3]) != self.in_pad:
+        if first is not None or int(shape[3]) != self.in_pad or not self.fpn:
             raise ValueError("BEVDetEncoder takes the %d-channel pool image" % self.in_pad)
         feats = self.backbone(x, shape)
         (x0, s0), (x2, s2) = feats[self.index[0]], feats[self.index[1]]
@@ -133,8 +148,10 @@ class BEVDet:
         X, Y, Z = self.vt.grid
         self.pool_C = round32(Z * mc["channels"])
         b, f, h = mc["backbone"], mc["fpn"], mc["head"]
-        self.encoder = BEVDetEncoder(Z * mc["channels"], b["num_channels"], b["strides"], b["blocks"], f["out_channels"],
-                                     f["scale_factor"], f["input_feature_index"], f["extra_upsample"], b["bn_eps"], self.pool_C)
+        enc_in = b.get("in_channels", Z * mc["channels"])  # BEVDet4D: the 160-channel concat
+        self.encoder = BEVDetEncoder(enc_in, b["num_channels"], b["strides"], b["blocks"], f["out_channels"],
+                                     f["scale_factor"], f["input_feature_index"], f["extra_upsample"], b["bn_eps"],
+                                     round32(enc_in))
         if self.encoder.cat_channels != f["in_channels"]:
             raise ValueError("FPN_LSS in_channels %d, the concat has %d" % (f["in_channels"], self.encoder.cat_channels))
         self.head = DenseRPNHead(in_channels=f["out_channels"], tasks=h["tasks"], share_conv_channel=h["share_conv_channel"],
@@ -142,6 +159,7 @@ class BEVDet:
         self.test_cfg = dict(mc["test"])
         self.label_off = synth.label_offsets(list(h["tasks"]))
         self.image_shape = (1, Y, X, self.pool_C)
+        self.enc_shape = (1, Y, X, self.encoder.in_pad)  # the encoder's input rows (BEVDet: the pool image)
 
     def init_weight(self, seed=0, bn_gain=1.0, device=None):
         """Seeded weights (dense_head.DenseRPNHead.init_weight); device=False: numpy parameters only."""
@@ -163,11 +181,11 @@ class BEVDet:
         return self.pool(depth, feat, prepared)
 
     def encode(self, image):
-        return self.encoder(image, self.image_shape)
+        return self.encoder(image, self.enc_shape)
 
     def dense(self, image):
-        """Pool image -> dict name -> per-task [1, k, 128, 128] fp32 head planes."""
-        return self.head.forward_h16(image, self.image_shape)
+        """Encoder input (BEVDet: the pool image) -> dict name -> per-task [1, k, 128, 128] fp32 head planes."""
+        return self.head.forward_h16(image, self.enc_shape)
 
     def postprocess(self, h):
         tc = self.test_cfg
@@ -184,7 +202,7 @@ class BEVDet:
         """DenseRPNHead.calibrate_heatmap_bias on this frame: ~1.4 % of the cells above the score threshold, as the LiDAR
         frames do.  Weights stay seeded and are exported unchanged to the CPU arm."""
         img = self.image(mats, logits, tran_feat)
-        self.head.calibrate_heatmap_bias(img, self.test_cfg["score_threshold"], target_frac, shape=self.image_shape)
+        self.head.calibrate_heatmap_bias(img, self.test_cfg["score_threshold"], target_frac, shape=self.enc_shape)
         return self
 
     def flops(self):
@@ -252,6 +270,7 @@ class BEVDetHotPath:
         self.h_counts = torch.zeros((len(model.label_off) + 1,), dtype=torch.int32).pin_memory()
         self.h_status = torch.zeros((1,), dtype=torch.int32).pin_memory()
         self.graphs, self.graph_nodes, self.prepared, self.last, self.out = {}, None, None, None, None
+        self.outs = {}  # graph name -> the device outputs its capture left (self.out of the graph last launched)
         self.done = torch.cuda.Event()
 
     def share_model(self, other):
@@ -264,10 +283,14 @@ class BEVDetHotPath:
         self.prepared = self.model.vt._prepare(self.desc, 1, self.model.N)
 
     def _frame(self):
-        m = self.model
         bp.lss_depth_feat(self.logits, self.tran_feat, self.depth, self.feat)
-        m.pool(self.depth, self.feat, self.prepared, out=self.image)
-        h = m.dense(self.image)
+        self.model.pool(self.depth, self.feat, self.prepared, out=self.image)
+        self._dense(self.image)
+
+    def _dense(self, x):
+        """Encoder -> head -> postprocess from the encoder's input rows x, then the D2H copies."""
+        m = self.model
+        h = m.dense(x)
         boxes, scores, labels, counts = m.postprocess(h)
         self.out = dict(boxes=boxes, scores=scores, labels=labels, counts=counts, head=h)
         self.h_boxes.copy_(boxes, non_blocking=True)
@@ -280,10 +303,14 @@ class BEVDetHotPath:
         self._ranks()
         self._frame()
 
+    def _parts(self):
+        """Graph name -> the stages it captures."""
+        return {"ranks": self._ranks, "frame": self._frame} if self.model.vt.accelerate else {"frame": self._full}
+
     def capture(self, count_nodes=False):
         """Warm up eagerly (sizes the workspaces), then capture the frame graph (accelerate: the rank graph and the rest).
         count_nodes: node counts by type of the graphs in self.graph_nodes."""
-        parts = {"ranks": self._ranks, "frame": self._frame} if self.model.vt.accelerate else {"frame": self._full}
+        parts = self._parts()
         with torch.cuda.stream(self.stream):
             self._full()
             self.stream.synchronize()
@@ -292,6 +319,7 @@ class BEVDetHotPath:
                 with torch.cuda.graph(g, stream=self.stream):
                     fn()
                 self.graphs[name] = g
+                self.outs[name] = self.out
                 if count_nodes:
                     nodes = _count_graph_nodes(g.raw_cuda_graph())
                     self.graph_nodes = nodes if self.graph_nodes is None else {k: self.graph_nodes[k] + nodes[k] for k in nodes}
@@ -303,8 +331,15 @@ class BEVDetHotPath:
         """Enqueue one frame on self.stream.  mats = (sensor2ego, cam2imgs, post_rots, post_trans, bda) of one sample on
         the host; logits [N, D, H, W] / tran_feat [N, C, H, W]: device tensors copied into the frame's inputs (None:
         already written there)."""
+        self._launch(mats, logits, tran_feat, "frame")
+
+    def _launch(self, mats, logits, tran_feat, frame, host_inputs=None):
+        """launch() replaying the graph named frame (with accelerate: after the rank graph when the cameras changed);
+        host_inputs: called once the previous frame is done, to write further pinned inputs the graph uploads."""
         packed = bp.pack_cameras(*mats)
         self.done.synchronize()  # the previous frame's H2D has read h_desc and its D2H has landed
+        if host_inputs is not None:
+            host_inputs()
         self.stream.wait_stream(torch.cuda.current_stream(self.device))  # inputs written on the caller's stream
         with torch.cuda.stream(self.stream):
             if logits is not None:
@@ -313,13 +348,12 @@ class BEVDetHotPath:
                 self.tran_feat.copy_(tran_feat, non_blocking=True)
             if not self.model.vt.accelerate:
                 self.h_desc.copy_(torch.from_numpy(packed))
-                self.graphs["frame"].replay()
-            else:
-                if self.last is None or not np.array_equal(self.last, packed):
-                    self.h_desc.copy_(torch.from_numpy(packed))
-                    self.graphs["ranks"].replay()
-                    self.last = packed
-                self.graphs["frame"].replay()
+            elif self.last is None or not np.array_equal(self.last, packed):
+                self.h_desc.copy_(torch.from_numpy(packed))
+                self.graphs["ranks"].replay()
+                self.last = packed
+            self.graphs[frame].replay()
+            self.out = self.outs[frame]
             self.done.record(self.stream)
 
     def result(self):
@@ -338,3 +372,190 @@ class BEVDetHotPath:
         """Raise when an activation left fp16's range on the fp16-pair path (never a silent wrong result)."""
         if int(status_host[0]):
             raise RuntimeError("BEVDet: an activation left fp16's range (|x| >= 65504) on the fp16-pair path")
+
+
+# ---------------------------------------------------------------------------------------------------------- BEVDet4D
+# PARITY UNPINNED, as CONFIG: BEVDet4D (bevdet4d-r50 configs; Paddle3D's bevdet4d.py descends from it) in sequential mode
+# with one adjacent frame (multi_adj_frame_id_cfg = (1, 2, 1)): pre_process_net = CustomResNet(numC_input=80,
+# num_layer=[2], num_channels=[80], stride=[1]) and the encoder's numC_input = 80 * (num_adj + 1).
+CONFIG_4D = dict(CONFIG, backbone=dict(CONFIG["backbone"], in_channels=160),
+                 pre_process=dict(num_channels=(80,), strides=(1,), blocks=2), num_adj=1)
+
+
+def _copy_rows(dst, src, width):
+    """cudaMemcpy2DAsync of the first `width` bytes of every row of src into the rows of dst on the current stream (one
+    memcpy node of a captured graph).  The runtime is torch's own (dlopen of its soname returns the loaded library)."""
+    import ctypes as C
+    rt = C.CDLL("libcudart.so.12")
+    rt.cudaMemcpy2DAsync.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int,
+                                     C.c_void_p]
+    rows = src.shape[0]
+    if dst.shape[0] != rows or width > dst.stride(0) * dst.element_size() or width > src.stride(0) * src.element_size():
+        raise ValueError("_copy_rows: %d bytes of %s rows into %s rows" % (width, tuple(src.shape), tuple(dst.shape)))
+    rc = rt.cudaMemcpy2DAsync(dst.data_ptr(), dst.stride(0) * dst.element_size(), src.data_ptr(),
+                              src.stride(0) * src.element_size(), width, rows, 3,  # cudaMemcpyDeviceToDevice
+                              torch.cuda.current_stream(src.device).cuda_stream)
+    if rc != 0:
+        raise RuntimeError("cudaMemcpy2DAsync failed (cudaError %d)" % rc)
+
+
+class BEVDet4D(BEVDet):
+    """Seeded BEVDet4D (CONFIG_4D) in sequential mode (extract_img_feat_sequential): the view transform and pre_process
+    give this frame's bev_feat; the previous frame's bev_feat (feat_prev) is shifted into the current ego frame
+    (shift_feature: a bilinear grid_sample by the ego motion between the two frames' camera 0) and concatenated after it,
+    and the 160-channel concat runs BEVDet's encoder, head and postprocess.  Batch 1.
+
+    Layout on pixel fp16-pair rows: pre_process reads the 96-channel pool image and writes 80 channels into 96-channel
+    rows (channels 80..95 of its intermediate images are never written: callers allocate them zero-filled); its last conv
+    writes channels [0, 80) of the concat [Y*X, 2*160], the shift channels [80, 160).  bev_feat / feat_prev: the first 96
+    channels of the concat's rows ([Y*X, 2*96]; channels 80..95 are not read)."""
+
+    def __init__(self, model_cfg=None, accelerate=False, device="cuda"):
+        mc = model_cfg or CONFIG_4D
+        if mc.get("num_adj", 1) != 1:
+            raise ValueError("BEVDet4D runs one adjacent frame (num_adj = 1), got num_adj = %r" % mc.get("num_adj"))
+        super().__init__(mc, accelerate, device)
+        pp, b = mc["pre_process"], mc["backbone"]
+        X, Y, Z = self.vt.grid
+        self.pre_process = BEVDetEncoder(Z * mc["channels"], pp["num_channels"], pp["strides"], pp["blocks"], None,
+                                         bn_eps=b["bn_eps"], in_pad=self.pool_C, row_pad=self.pool_C)
+        self.bev_C = pp["num_channels"][-1]
+        self.hist_C = self.pool_C
+        if (any(s != 1 for s in pp["strides"]) or self.bev_C > self.hist_C or self.bev_C % 16
+                or self.encoder.in_channels != 2 * self.bev_C or self.encoder.in_pad != 2 * self.bev_C):
+            raise ValueError("BEVDet4D: the encoder takes cat([bev_feat, shifted feat_prev]) of %d + %d channels"
+                             % (self.bev_C, self.bev_C))
+
+    def init_weight(self, seed=0, bn_gain=1.0, device=None):
+        super().init_weight(seed=seed, bn_gain=bn_gain, device=device)
+        rng = np.random.default_rng([seed, 4])
+        dev = None if device is False else (device or self.device)
+        for c in self.pre_process.convs():
+            c.init(rng, dev, bn_gain=bn_gain)
+        return self
+
+    def export_numpy(self):
+        return dict(super().export_numpy(), pre_process=self.pre_process.export_numpy()["backbone"])
+
+    # ---- stages, device in / device out
+    def pre_buffers(self):
+        """Zero-filled intermediate images of pre_process ([Y*X, 2*96] each; their padding channels stay zero)."""
+        _, Y, X, pc = self.image_shape
+        z = lambda: torch.zeros((Y * X, 2 * pc), dtype=torch.float16, device=self.device)  # noqa: E731
+        bufs = []
+        for si, stage in enumerate(self.pre_process.stages):
+            bufs.append([])
+            for bi, blk in enumerate(stage):
+                last = si == len(self.pre_process.stages) - 1 and bi == len(stage) - 1
+                d = dict(conv1=z())
+                if blk["down"] is not None:
+                    d["down"] = z()
+                if not last:
+                    d["conv2"] = z()
+                bufs[-1].append(d)
+        return bufs
+
+    def pre(self, image, concat, bufs):
+        """pre_process of the pool image into channels [0, 80) of the concat rows."""
+        self.pre_process.backbone(image, self.image_shape, bufs, out=(concat, self.encoder.in_pad, 0))
+
+    def shift_desc(self, mats, prev_sensor2keyego=None):
+        """pack_shift of this frame: mats as forward takes them (mats[0] = the current sensor2keyego); prev None: the
+        start of a sequence (the frame is its own adjacent frame)."""
+        lower, interval, _ = self.vt.grid_args()
+        prev = mats[0] if prev_sensor2keyego is None else prev_sensor2keyego
+        return bp.pack_shift(mats[0], prev, mats[4], lower, interval)
+
+    def shift(self, feat_prev, tf, concat):
+        """shift_feature of feat_prev (the history rows, or None: the concat's own bev_feat) into channels [80, 160)."""
+        _, Y, X, ec = self.enc_shape
+        src, in_c = (concat, ec) if feat_prev is None else (feat_prev, self.hist_C)
+        bp.bev_shift_h16(src, (1, Y, X, in_c), tf, self.bev_C, out_h16=concat, out_channels=ec, out_c0=self.bev_C)
+
+    def encoder_input(self, mats, prev_sensor2keyego, logits, tran_feat, feat_prev=None):
+        """Eager: the concat rows [Y*X, 2*160] of a frame (feat_prev None: the start of a sequence)."""
+        _, Y, X, ec = self.enc_shape
+        concat = torch.empty((Y * X, 2 * ec), dtype=torch.float16, device=self.device)
+        self.pre(self.image(mats, logits, tran_feat), concat, self.pre_buffers())
+        tf = torch.from_numpy(self.shift_desc(mats, None if feat_prev is None else prev_sensor2keyego)).to(self.device)
+        self.shift(feat_prev, tf, concat)
+        return concat
+
+    def forward(self, mats, prev_sensor2keyego, logits, tran_feat, feat_prev=None):
+        """Eager frame: ((boxes, scores, labels, counts) as BEVDet.forward, bev_feat [Y*X, 2*96]: the next frame's
+        feat_prev).  mats = (sensor2keyego, cam2imgs, post_rots, post_trans, bda) of this frame; prev_sensor2keyego [1, N, 4,
+        4]: the previous frame's cameras in this frame's ego (ops.bev_pool_v2.sensor2keyegos); feat_prev None starts a
+        sequence (bev_feat is its own adjacent frame and prev_sensor2keyego is not used)."""
+        concat = self.encoder_input(mats, prev_sensor2keyego, logits, tran_feat, feat_prev)
+        bev_feat = concat[:, :2 * self.hist_C].contiguous()
+        return self.postprocess(self.dense(concat)), bev_feat
+
+    def calibrate_heatmap_bias(self, mats, logits, tran_feat, target_frac=0.014):
+        """BEVDet.calibrate_heatmap_bias on the start frame of a sequence with these inputs."""
+        x = self.encoder_input(mats, None, logits, tran_feat)
+        self.head.calibrate_heatmap_bias(x, self.test_cfg["score_threshold"], target_frac, shape=self.enc_shape)
+        return self
+
+    def flops(self):
+        """BEVDet.flops (the encoder's first stage at 160 input channels) plus pre_process (five 3x3 convs 80 -> 80 at the
+        pool image's size; the Cin padding 80 -> 96 is not counted)."""
+        out = super().flops()
+        _, H, W, _ = self.image_shape
+        out["pre_process"] = sum(2.0 * H * W * c.cin * c.cout * c.k * c.k for c in self.pre_process.convs())
+        out["total"] += out["pre_process"]
+        return out
+
+
+class BEVDet4DHotPath(BEVDetHotPath):
+    """One BEVDet4D frame as one captured CUDA graph, BEVDetHotPath's frame with the temporal stages: camera descriptor
+    H2D -> ranks -> softmax / permute -> memset + pool -> shift descriptor H2D -> pre_process into the concat -> shift
+    (the lane's history -> concat channels [80, 160)) -> a 2-D memcpy of the concat's first 96 channels into the history
+    -> encoder -> head -> postprocess -> D2H.  The shift reads the old history before the copy replaces it.  Two frame
+    graphs over the same buffers: "continue" shifts the history, "start" (the first frame of a sequence) shifts the
+    concat's own bev_feat at the transform of prev = curr.  accelerate: the rank graph, then one of the two; the shift
+    descriptor is uploaded in the frame graph, so the ranks are still recomputed only when the cameras change.  Each lane
+    owns its history: lanes in flight run independent sequences."""
+
+    def __init__(self, model, device="cuda", stream=None):
+        super().__init__(model, device, stream)
+        _, Y, X, ec = model.enc_shape
+        self.concat = torch.empty((Y * X, 2 * ec), dtype=torch.float16, device=self.device)
+        self.history = torch.zeros((Y * X, 2 * model.hist_C), dtype=torch.float16, device=self.device)
+        self.pre_bufs = model.pre_buffers()  # zero-filled once, outside the graphs
+        self.h_shift = torch.zeros((bp.SHIFT_FLOATS,), dtype=torch.float32).pin_memory()
+        self.tf = torch.zeros((bp.SHIFT_FLOATS,), dtype=torch.float32, device=self.device)
+        self.started = False
+
+    def _frame(self, start=False):
+        m = self.model
+        bp.lss_depth_feat(self.logits, self.tran_feat, self.depth, self.feat)
+        m.pool(self.depth, self.feat, self.prepared, out=self.image)
+        self.tf.copy_(self.h_shift, non_blocking=True)
+        m.pre(self.image, self.concat, self.pre_bufs)
+        m.shift(None if start else self.history, self.tf, self.concat)
+        _copy_rows(self.history, self.concat, self.history.stride(0) * self.history.element_size())
+        self._dense(self.concat)
+
+    def _parts(self):
+        if self.model.vt.accelerate:
+            return {"ranks": self._ranks, "start": lambda: self._frame(True), "continue": self._frame}
+        return {"start": lambda: (self._ranks(), self._frame(True)), "continue": self._full}
+
+    def launch(self, mats, prev_sensor2keyego=None, logits=None, tran_feat=None, new_sequence=False):
+        """Enqueue one frame of this lane's sequence.  mats = (sensor2keyego, cam2imgs, post_rots, post_trans, bda);
+        prev_sensor2keyego [1, N, 4, 4]: the previous frame's cameras in this frame's ego (ops.bev_pool_v2.sensor2keyegos);
+        new_sequence: this frame starts a sequence (prev_sensor2keyego is not used).  A lane's first frame must start one."""
+        if not (new_sequence or self.started):
+            raise ValueError("BEVDet4DHotPath: the first frame of a lane must start a sequence (new_sequence=True)")
+        tf = self.model.shift_desc(mats, None if new_sequence else prev_sensor2keyego)
+        self._launch(mats, logits, tran_feat, "start" if new_sequence else "continue",
+                     host_inputs=lambda: self.h_shift.copy_(torch.from_numpy(tf.reshape(-1))))
+        self.started = True
+
+    def infer(self, mats, prev_sensor2keyego=None, logits=None, tran_feat=None, new_sequence=False):
+        self.launch(mats, prev_sensor2keyego, logits, tran_feat, new_sequence)
+        return self.result()
+
+    def check_status(self, status_host):
+        if int(status_host[0]):
+            raise RuntimeError("BEVDet4D: an activation left fp16's range (|x| >= 65504) on the fp16-pair path")

@@ -5,6 +5,8 @@
 #pragma once
 #include <cuda_fp16.h>
 
+#include <cstdint>
+
 namespace p3d {
 
 constexpr float kLoScale = 2048.0f, kLoInv = 1.0f / 2048.0f;
@@ -35,5 +37,18 @@ __device__ __forceinline__ void split_h16x2(float a, float b, __half2 &hi, __hal
 }
 
 __device__ __forceinline__ float merge_h16(__half hi, __half lo) { return fmaf(__half2float(lo), kLoInv, __half2float(hi)); }
+
+// channels 8 q .. 8 q + 7 of a pixel row, merged to fp32: hi at (q / 4) * 128 + (q % 4) * 16, lo' 64 bytes further
+__device__ __forceinline__ void load8(const uint8_t *px, int q, float v[8]) {
+  const uint8_t *g = px + (q >> 2) * 128 + (q & 3) * 16;
+  const uint4 hi = __ldg(reinterpret_cast<const uint4 *>(g)), lo = __ldg(reinterpret_cast<const uint4 *>(g + 64));
+  const __half2 *h2 = reinterpret_cast<const __half2 *>(&hi), *l2 = reinterpret_cast<const __half2 *>(&lo);
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const float2 fh = __half22float2(h2[k]), fl = __half22float2(l2[k]);
+    v[2 * k] = fmaf(fl.x, kLoInv, fh.x);
+    v[2 * k + 1] = fmaf(fl.y, kLoInv, fh.y);
+  }
+}
 
 }  // namespace p3d

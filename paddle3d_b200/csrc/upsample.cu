@@ -22,19 +22,6 @@ struct UpParams {
   int32_t *status;
 };
 
-__device__ __forceinline__ void load8(const uint8_t *px, int q, float v[8]) {
-  // channels 8 q .. 8 q + 7 of a pixel row: hi at (q / 4) * 128 + (q % 4) * 16, lo' 64 bytes further
-  const uint8_t *g = px + (q >> 2) * 128 + (q & 3) * 16;
-  const uint4 hi = __ldg(reinterpret_cast<const uint4 *>(g)), lo = __ldg(reinterpret_cast<const uint4 *>(g + 64));
-  const __half2 *h2 = reinterpret_cast<const __half2 *>(&hi), *l2 = reinterpret_cast<const __half2 *>(&lo);
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    const float2 fh = __half22float2(h2[k]), fl = __half22float2(l2[k]);
-    v[2 * k] = fmaf(fl.x, kLoInv, fh.x);
-    v[2 * k + 1] = fmaf(fl.y, kLoInv, fh.y);
-  }
-}
-
 __global__ void __launch_bounds__(256) upsample_bilinear_h16_kernel(const UpParams p) {
   const int qn = p.C / 8;
   const long long total = static_cast<long long>(p.B) * p.H * p.W * qn;

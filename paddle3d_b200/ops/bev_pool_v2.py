@@ -89,6 +89,62 @@ def _f64(a):
     return np.asarray(a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else a, np.float64)
 
 
+# ------------------------------------------------------------------------------------- BEVDet4D's temporal alignment
+SHIFT_FLOATS = 6  # rows 0 and 1 of the 3x3 BEV-pixel transform tf, row-major
+
+
+def sensor2keyegos(sensor2ego, ego2global, key_ego2global):
+    """BEVDet's data pipeline: the cameras of a frame in the key (current) frame's ego frame, fp64
+    inv(keyego2global) . ego2global . sensor2ego.  sensor2ego / ego2global [B, N, 4, 4] of the frame; key_ego2global
+    [B, N, 4, 4] of the current frame, whose camera 0 defines the key ego (the current frame gives its own sensor2ego)."""
+    key = _f64(key_ego2global)[:, 0:1]
+    return np.linalg.inv(key) @ _f64(ego2global) @ _f64(sensor2ego)
+
+
+def shift_matrix(sensor2keyego_curr, sensor2keyego_prev, bda, grid_lower_bound, grid_interval):
+    """BEVDet4D.gen_grid's tf [B, 3, 3] in fp64: bda4 = [[bda, 0], [0, 1]], c02l0 = bda4 . curr[:, 0], c12l0 = bda4 . prev[:, 0],
+    l02l1 = (c02l0 . inv(c12l0)) restricted to (x, y, w), tf = inv(feat2bev) . l02l1 . feat2bev with feat2bev the BEV pixel
+    index -> metres map (grid_interval, grid_lower_bound)."""
+    curr, prev, bda = _f64(sensor2keyego_curr), _f64(sensor2keyego_prev), _f64(bda)
+    B = curr.shape[0]
+    bda4 = np.zeros((B, 4, 4))
+    bda4[:, :3, :3] = bda
+    bda4[:, 3, 3] = 1.0
+    c02l0 = bda4 @ curr[:, 0]
+    c12l0 = bda4 @ prev[:, 0]
+    l02l1 = (c02l0 @ np.linalg.inv(c12l0))[:, [0, 1, 3]][:, :, [0, 1, 3]]
+    f2b = np.array([[grid_interval[0], 0.0, grid_lower_bound[0]], [0.0, grid_interval[1], grid_lower_bound[1]],
+                    [0.0, 0.0, 1.0]], np.float64)
+    return np.linalg.inv(f2b) @ l02l1 @ f2b
+
+
+def pack_shift(sensor2keyego_curr, sensor2keyego_prev, bda, grid_lower_bound, grid_interval):
+    """Device descriptor of p3d_bev_shift_h16: fp32 [B, 6] = rows 0 and 1 of shift_matrix, computed in fp64 and rounded
+    once (pack_cameras' policy).  sensor2keyego_* [B, N, 4, 4] (camera 0 is used), bda [B, 3, 3]."""
+    tf = shift_matrix(sensor2keyego_curr, sensor2keyego_prev, bda, grid_lower_bound, grid_interval)
+    return np.ascontiguousarray(tf[:, :2].reshape(-1, SHIFT_FLOATS)).astype(np.float32)
+
+
+def bev_shift_h16(x_h16, shape, tf, C, out_h16=None, out_channels=None, out_c0=0):
+    """BEVDet4D.shift_feature on pixel fp16-pair rows (p3d_bev_shift_h16): channels [0, C) of x_h16 [B*h*w, 2*in_C],
+    shape = (B, h, w, in_C), sampled at tf's grid (device fp32 [B, 6] from pack_shift) into channels [out_c0, out_c0 + C)
+    of out_h16 [B*h*w, 2*out_channels] (None: a new C-channel image; x_h16 itself when the channel ranges are disjoint).
+    Returns out_h16."""
+    from .sparse_nn import status_tensor
+    x_h16 = require_cuda(x_h16, "x_h16", torch.float16)
+    tf = require_cuda(tf, "tf", torch.float32)
+    b, h, w, in_c = [int(v) for v in shape]
+    if tf.numel() != b * SHIFT_FLOATS:
+        raise ValueError("bev_shift_h16: tf has %d floats, want %d" % (tf.numel(), b * SHIFT_FLOATS))
+    oc = int(out_channels or C)
+    dev = x_h16.device
+    if out_h16 is None:
+        out_h16 = torch.empty((b * h * w, 2 * oc), dtype=torch.float16, device=dev)
+    check(lib().p3d_bev_shift_h16(ptr(x_h16), b, h, w, in_c, int(C), ptr(tf), ptr(out_h16), oc, int(out_c0),
+                                  ptr(status_tensor(dev)), stream(dev)), "bev_shift_h16")
+    return out_h16
+
+
 def lss_prepare(desc, axis_depth, axis_x, axis_y, B, N, grid_lower_bound, grid_interval, grid_size, with_coor=False):
     """get_lidar_coor + voxel_pooling_prepare_v2 in one pass (p3d_lss_prepare), no host sync.  desc: device fp32 buffer
     from pack_cameras; axis_*: device fp32 frustum axes [D] / [W] / [H].  Returns (ranks_bev, ranks_depth, ranks_feat,

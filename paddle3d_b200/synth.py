@@ -283,6 +283,18 @@ def camera_rig(seed, B=1, n_cams=6, bda=True):
                 post_trans=ptr.astype(f), bda=bd.astype(f))
 
 
+def ego_poses(n_frames, speed=10.0, yaw_rate=0.3, period=0.5, origin=(600.0, 1600.0)):
+    """global_from_ego [n_frames, 4, 4] float64 of an ego vehicle driving at `speed` m/s while turning at `yaw_rate` rad/s,
+    one pose every `period` s (sweep_sequence's motion; 0.5 s = nuScenes' 2 Hz key frames), starting at `origin`."""
+    out = np.zeros((n_frames, 4, 4))
+    for s in range(n_frames):
+        yaw = yaw_rate * s * period
+        x, y = speed * s * period * np.cos(yaw / 2), speed * s * period * np.sin(yaw / 2)
+        out[s] = [[np.cos(yaw), -np.sin(yaw), 0.0, origin[0] + x], [np.sin(yaw), np.cos(yaw), 0.0, origin[1] + y],
+                  [0.0, 0.0, 1.0, 0.0], [0.0, 0.0, 0.0, 1.0]]
+    return out
+
+
 def lss_mats(rig):
     """(sensor2ego, cam2imgs, post_rots, post_trans, bda) of a camera_rig, the order LSSHotPath takes them in."""
     return rig["sensor2ego"], rig["cam2imgs"], rig["post_rots"], rig["post_trans"], rig["bda"]

@@ -778,3 +778,33 @@ PD_BUILD_OP(p3d_bev_pool_v2_dev_h16)
     .SetKernelFn(PD_KERNEL(p3d_bev_pool_v2_dev_h16_op))
     .SetInferShapeFn(PD_INFER_SHAPE(PoolH16InferShape))
     .SetInferDtypeFn(PD_INFER_DTYPE(PoolH16InferDtype));
+
+// BEVDet4D's shift_feature on pixel fp16-pair rows: channels [0, C) of IMAGE [B*h*w, 2*in_C] FLOAT16 resampled by the
+// per-sample affine TF [B, 6] FLOAT32 (ops.bev_pool_v2.pack_shift) into channels [out_c0, out_c0 + C) of a new
+// [B*h*w, 2*out_channels] (the rest of the tensor is left as allocated: the concat's other channels come from
+// pre_process).  bhwc = (B, h, w, in_C).
+std::vector<paddle::Tensor> p3d_bev_shift_h16_op(const paddle::Tensor &image, const paddle::Tensor &tf,
+                                                 const paddle::Tensor &status, const std::vector<int> &bhwc, const int C,
+                                                 const int out_channels, const int out_c0) {
+  P3D_CHECK_GPU(image);
+  const int B = bhwc[0], h = bhwc[1], w = bhwc[2], in_C = bhwc[3];
+  auto out = paddle::empty({static_cast<int64_t>(B) * h * w, 2 * out_channels}, paddle::DataType::FLOAT16, paddle::GPUPlace());
+  P3D_CALL(p3d_bev_shift_h16(image.data(), B, h, w, in_C, C, tf.data<float>(), out.data(), out_channels, out_c0,
+                             const_cast<int *>(status.data<int>()), image.stream()));
+  return {out};
+}
+std::vector<std::vector<int64_t>> ShiftH16InferShape(std::vector<int64_t> im, std::vector<int64_t> tf, std::vector<int64_t> st,
+                                                     const std::vector<int> &bhwc, const int &C, const int &out_channels,
+                                                     const int &out_c0) {
+  return {{static_cast<int64_t>(bhwc[0]) * bhwc[1] * bhwc[2], 2 * static_cast<int64_t>(out_channels)}};
+}
+std::vector<paddle::DataType> ShiftH16InferDtype(paddle::DataType im, paddle::DataType tf, paddle::DataType st) {
+  return {paddle::DataType::FLOAT16};
+}
+PD_BUILD_OP(p3d_bev_shift_h16)
+    .Inputs({"IMAGE", "TF", "STATUS"})
+    .Outputs({"OUT"})
+    .Attrs({"bhwc: std::vector<int>", "C: int", "out_channels: int", "out_c0: int"})
+    .SetKernelFn(PD_KERNEL(p3d_bev_shift_h16_op))
+    .SetInferShapeFn(PD_INFER_SHAPE(ShiftH16InferShape))
+    .SetInferDtypeFn(PD_INFER_DTYPE(ShiftH16InferDtype));
