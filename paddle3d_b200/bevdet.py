@@ -13,13 +13,13 @@ import numpy as np
 import torch
 
 from . import synth
-from .dense_head import COMMON_HEADS, DenseRPNHead, _Conv
-from .lss import LSSViewTransformer
+from .dense_head import DenseRPNHead, _Conv
+from .frame import ResultSlot, ResultSlotOwner, copy_rows
+from .lss import CameraFrame, LSSViewTransformer
 from .ops import bev_pool_v2 as bp
 from .ops import centerpoint_postprocess as cpp
 from .ops import dense_conv as dc
 from .ops import sparse_nn as sp
-from .pipeline import _count_graph_nodes
 
 # PARITY UNPINNED (see the module docstring)
 CONFIG = dict(
@@ -189,10 +189,7 @@ class BEVDet:
 
     def postprocess(self, h):
         tc = self.test_cfg
-        return cpp.centerpoint_postprocess_device(
-            h["hm"], h["reg"], h["height"], h["dim"], h["vel"], h["rot"], tc["voxel_size"], tc["point_cloud_range"],
-            tc["post_center_limit_range"], self.label_off, tc["down_ratio"], tc["score_threshold"],
-            tc["nms_iou_threshold"], tc["nms_pre_max_size"], tc["nms_post_max_size"], True)
+        return cpp.centerpoint_postprocess_heads(h, tc["voxel_size"], tc["point_cloud_range"], tc, self.label_off)
 
     def forward(self, mats, logits, tran_feat):
         """Eager frame: (boxes, scores, labels, counts) on the device, worst-case sized (counts[-1] rows valid)."""
@@ -208,7 +205,7 @@ class BEVDet:
     def flops(self):
         """Algorithmic flops (2 x MACs) of the dense part: backbone (CustomResNet with its identity convs), FPN_LSS and
         the head (shared conv, the 36 ConvModules, the output convs).  The Cin padding 80 -> 96 is not counted."""
-        out = dict(backbone=0.0, fpn=0.0, head_shared=0.0, head_convmodules=0.0, head_output=0.0)
+        out = dict(backbone=0.0, fpn=0.0)
         _, H, W, _ = self.image_shape
         h, w = H, W
         for stage in self.encoder.stages:
@@ -225,144 +222,53 @@ class BEVDet:
         f0, f1, f2, f3 = enc.fpn
         for c, hh in ((f0, h0), (f1, h0), (f2, h1), (f3, h1)):
             out["fpn"] += 2.0 * hh * hh * c.cin * c.cout * c.k * c.k
-        px = h1 * h1
-        sh = self.head.shared
-        out["head_shared"] = 2.0 * px * sh.cin * sh.cout * sh.k * sh.k
-        for hs in self.head.heads:
-            for _, a, f in hs:
-                out["head_convmodules"] += 2.0 * px * a.cin * a.cout * a.k * a.k
-                out["head_output"] += 2.0 * px * f.cin * f.cout * f.k * f.k
-        out["head"] = out["head_shared"] + out["head_convmodules"] + out["head_output"]
+        out.update(self.head.head_flops(h1, h1))
         out["total"] = out["backbone"] + out["fpn"] + out["head"]
         return out
 
     def head_planes(self):
-        return sum(sum(c for _, c in COMMON_HEADS) + n for n in self.head.tasks)
+        return self.head.head_planes()
 
 
-class BEVDetHotPath:
-    """One BEVDet frame as one captured CUDA graph on its own stream: camera descriptor H2D -> p3d_lss_prepare -> depth
-    softmax / permute -> memset + pool into the pixel image -> encoder -> head -> postprocess -> one D2H of boxes [6 x 83,
-    9], scores, labels, counts and the status word.  Any calibration replays the same graph.  accelerate (the model's
-    view transformer built with accelerate=True): two graphs, ranks (replayed only when the camera matrices differ from
-    the last ones) and the rest.  Several lanes may share one model (share_model), each with its own buffers and stream.
-    The status word is the device's fp16-pair overflow flag (ops.sparse_nn.status_tensor), which stays set once raised."""
+class BEVDetHotPath(ResultSlotOwner, CameraFrame):
+    """One BEVDet frame as one captured CUDA graph on its own stream (CameraFrame): camera descriptor H2D ->
+    p3d_lss_prepare -> depth softmax / permute -> memset + pool into the pixel image -> encoder -> head -> postprocess ->
+    one D2H of boxes [6 x 83, 9], scores, labels, counts and the status word.  Any calibration replays the same graph.
+    accelerate (the model's view transformer built with accelerate=True): two graphs, ranks (replayed only when the camera
+    matrices differ from the last ones) and the rest.  Several lanes may share one model (share_model), each with its own
+    buffers and stream.  The status word is the device's fp16-pair overflow flag (ops.sparse_nn.status_tensor), which
+    stays set once raised."""
 
     def __init__(self, model, device="cuda", stream=None):
+        super().__init__(model.vt, 1, model.N, device, stream)
         self.model = model
-        self.device = torch.device(device)
-        self.stream = stream or torch.cuda.Stream(self.device)
-        vt, N = model.vt, model.N
-        nd = N * bp.CAM_FLOATS + 9
-        self.h_desc = torch.zeros((nd,), dtype=torch.float32).pin_memory()
-        self.desc = torch.zeros((nd,), dtype=torch.float32, device=self.device)
-        D, H, W, C = vt.D, vt.H, vt.W, vt.out_channels
-        self.logits = torch.zeros((N, D, H, W), dtype=torch.float32, device=self.device)
-        self.tran_feat = torch.zeros((N, C, H, W), dtype=torch.float32, device=self.device)
-        self.depth = torch.empty_like(self.logits)
-        self.feat = torch.empty((N, H, W, C), dtype=torch.float32, device=self.device)
         _, Y, X, pc = model.image_shape
         self.image = torch.empty((Y * X, 2 * pc), dtype=torch.float16, device=self.device)
-        rows = len(model.label_off) * model.test_cfg["nms_post_max_size"]
-        self.h_boxes = torch.zeros((rows, 9), dtype=torch.float32).pin_memory()
-        self.h_scores = torch.zeros((rows,), dtype=torch.float32).pin_memory()
-        self.h_labels = torch.zeros((rows,), dtype=torch.int64).pin_memory()
-        self.h_counts = torch.zeros((len(model.label_off) + 1,), dtype=torch.int32).pin_memory()
-        self.h_status = torch.zeros((1,), dtype=torch.int32).pin_memory()
-        self.graphs, self.graph_nodes, self.prepared, self.last, self.out = {}, None, None, None, None
-        self.outs = {}  # graph name -> the device outputs its capture left (self.out of the graph last launched)
-        self.done = torch.cuda.Event()
+        self.slot = ResultSlot(len(model.label_off) * model.test_cfg["nms_post_max_size"], 9, len(model.label_off) + 1, 1)
 
     def share_model(self, other):
-        self.model = other.model
+        self.model, self.vt = other.model, other.vt
         return self
 
     # ---- stages, as they are captured
-    def _ranks(self):
-        self.desc.copy_(self.h_desc, non_blocking=True)
-        self.prepared = self.model.vt._prepare(self.desc, 1, self.model.N)
-
     def _frame(self):
         bp.lss_depth_feat(self.logits, self.tran_feat, self.depth, self.feat)
         self.model.pool(self.depth, self.feat, self.prepared, out=self.image)
-        self._dense(self.image)
+        return self._dense(self.image)
 
     def _dense(self, x):
         """Encoder -> head -> postprocess from the encoder's input rows x, then the D2H copies."""
         m = self.model
         h = m.dense(x)
         boxes, scores, labels, counts = m.postprocess(h)
-        self.out = dict(boxes=boxes, scores=scores, labels=labels, counts=counts, head=h)
-        self.h_boxes.copy_(boxes, non_blocking=True)
-        self.h_scores.copy_(scores, non_blocking=True)
-        self.h_labels.copy_(labels, non_blocking=True)
-        self.h_counts.copy_(counts, non_blocking=True)
-        self.h_status.copy_(sp.status_tensor(self.device), non_blocking=True)
-
-    def _full(self):
-        self._ranks()
-        self._frame()
-
-    def _parts(self):
-        """Graph name -> the stages it captures."""
-        return {"ranks": self._ranks, "frame": self._frame} if self.model.vt.accelerate else {"frame": self._full}
-
-    def capture(self, count_nodes=False):
-        """Warm up eagerly (sizes the workspaces), then capture the frame graph (accelerate: the rank graph and the rest).
-        count_nodes: node counts by type of the graphs in self.graph_nodes."""
-        parts = self._parts()
-        with torch.cuda.stream(self.stream):
-            self._full()
-            self.stream.synchronize()
-            for name, fn in parts.items():
-                g = torch.cuda.CUDAGraph(keep_graph=True) if count_nodes else torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g, stream=self.stream):
-                    fn()
-                self.graphs[name] = g
-                self.outs[name] = self.out
-                if count_nodes:
-                    nodes = _count_graph_nodes(g.raw_cuda_graph())
-                    self.graph_nodes = nodes if self.graph_nodes is None else {k: self.graph_nodes[k] + nodes[k] for k in nodes}
-        self.stream.synchronize()
-        self.last = None
-        return self
-
-    def launch(self, mats, logits=None, tran_feat=None):
-        """Enqueue one frame on self.stream.  mats = (sensor2ego, cam2imgs, post_rots, post_trans, bda) of one sample on
-        the host; logits [N, D, H, W] / tran_feat [N, C, H, W]: device tensors copied into the frame's inputs (None:
-        already written there)."""
-        self._launch(mats, logits, tran_feat, "frame")
-
-    def _launch(self, mats, logits, tran_feat, frame, host_inputs=None):
-        """launch() replaying the graph named frame (with accelerate: after the rank graph when the cameras changed);
-        host_inputs: called once the previous frame is done, to write further pinned inputs the graph uploads."""
-        packed = bp.pack_cameras(*mats)
-        self.done.synchronize()  # the previous frame's H2D has read h_desc and its D2H has landed
-        if host_inputs is not None:
-            host_inputs()
-        self.stream.wait_stream(torch.cuda.current_stream(self.device))  # inputs written on the caller's stream
-        with torch.cuda.stream(self.stream):
-            if logits is not None:
-                self.logits.copy_(logits, non_blocking=True)
-            if tran_feat is not None:
-                self.tran_feat.copy_(tran_feat, non_blocking=True)
-            if not self.model.vt.accelerate:
-                self.h_desc.copy_(torch.from_numpy(packed))
-            elif self.last is None or not np.array_equal(self.last, packed):
-                self.h_desc.copy_(torch.from_numpy(packed))
-                self.graphs["ranks"].replay()
-                self.last = packed
-            self.graphs[frame].replay()
-            self.out = self.outs[frame]
-            self.done.record(self.stream)
+        out = dict(boxes=boxes, scores=scores, labels=labels, counts=counts, status=sp.status_tensor(self.device), head=h)
+        self.slot.copy_from(out)
+        return out
 
     def result(self):
         """Wait for the last launched frame: (boxes [K, 9], scores [K], labels [K]) host tensors owned by the lane (valid
         until its next launch); raises from check_status."""
-        self.done.synchronize()
-        self.check_status(self.h_status)
-        k = int(self.h_counts[-1])
-        return self.h_boxes[:k], self.h_scores[:k], self.h_labels[:k]
+        return self.slot.read(self.check_status, self.done)
 
     def infer(self, mats, logits=None, tran_feat=None):
         self.launch(mats, logits, tran_feat)
@@ -380,23 +286,6 @@ class BEVDetHotPath:
 # num_layer=[2], num_channels=[80], stride=[1]) and the encoder's numC_input = 80 * (num_adj + 1).
 CONFIG_4D = dict(CONFIG, backbone=dict(CONFIG["backbone"], in_channels=160),
                  pre_process=dict(num_channels=(80,), strides=(1,), blocks=2), num_adj=1)
-
-
-def _copy_rows(dst, src, width):
-    """cudaMemcpy2DAsync of the first `width` bytes of every row of src into the rows of dst on the current stream (one
-    memcpy node of a captured graph).  The runtime is torch's own (dlopen of its soname returns the loaded library)."""
-    import ctypes as C
-    rt = C.CDLL("libcudart.so.12")
-    rt.cudaMemcpy2DAsync.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int,
-                                     C.c_void_p]
-    rows = src.shape[0]
-    if dst.shape[0] != rows or width > dst.stride(0) * dst.element_size() or width > src.stride(0) * src.element_size():
-        raise ValueError("_copy_rows: %d bytes of %s rows into %s rows" % (width, tuple(src.shape), tuple(dst.shape)))
-    rc = rt.cudaMemcpy2DAsync(dst.data_ptr(), dst.stride(0) * dst.element_size(), src.data_ptr(),
-                              src.stride(0) * src.element_size(), width, rows, 3,  # cudaMemcpyDeviceToDevice
-                              torch.cuda.current_stream(src.device).cuda_stream)
-    if rc != 0:
-        raise RuntimeError("cudaMemcpy2DAsync failed (cudaError %d)" % rc)
 
 
 class BEVDet4D(BEVDet):
@@ -533,13 +422,13 @@ class BEVDet4DHotPath(BEVDetHotPath):
         self.tf.copy_(self.h_shift, non_blocking=True)
         m.pre(self.image, self.concat, self.pre_bufs)
         m.shift(None if start else self.history, self.tf, self.concat)
-        _copy_rows(self.history, self.concat, self.history.stride(0) * self.history.element_size())
-        self._dense(self.concat)
+        copy_rows(self.history, self.concat, self.history.stride(0) * self.history.element_size())
+        return self._dense(self.concat)
 
     def _parts(self):
-        if self.model.vt.accelerate:
+        if self.vt.accelerate:
             return {"ranks": self._ranks, "start": lambda: self._frame(True), "continue": self._frame}
-        return {"start": lambda: (self._ranks(), self._frame(True)), "continue": self._full}
+        return {"start": lambda: self._full(True), "continue": self._full}
 
     def launch(self, mats, prev_sensor2keyego=None, logits=None, tran_feat=None, new_sequence=False):
         """Enqueue one frame of this lane's sequence.  mats = (sensor2keyego, cam2imgs, post_rots, post_trans, bda);

@@ -7,7 +7,7 @@ synth.CP_PILLARS with CONFIG), composed from this repository's kernels:
     -> centerpoint_postprocess_device -> boxes
 
 CenterPointPillarsHotPath captures everything between the H2D copy of the points and the D2H copy of the boxes as one
-CUDA graph (pipeline.CapturedFrame), optionally starting with the device merge of raw sweeps (sweep_input).
+CUDA graph (frame.CapturedFrame), optionally starting with the device merge of raw sweeps (sweep_input).
 
 PARITY UNPINNED: the model values (CONFIG, synth.CP_PILLARS, synth.CENTERPOINT_PILLARS_TEST_CFG) are recalled from
 Paddle3D's yml and det3d's nusc_centerpoint_pp_02voxel_two_pfn_10sweep, which it descends from; they were not checked
@@ -16,12 +16,13 @@ import numpy as np
 import torch
 
 from . import synth
-from .dense_head import COMMON_HEADS, DenseRPNHead, SecondTrunk
+from .dense_head import DenseRPNHead, SecondTrunk
+from .frame import CapturedFrame, ResultSlot
 from .ops import centerpoint_postprocess as cpp
 from .ops import pillar_encoder as pe
 from .ops import sparse_nn as sp
 from .ops import voxelize as vox
-from .pipeline import SWEEP_INPUT, CapturedFrame
+from .pointpillars import grid_size
 
 # PARITY UNPINNED (see the module docstring)
 CONFIG = dict(
@@ -31,12 +32,6 @@ CONFIG = dict(
     head=dict(tasks=tuple(synth.CENTERPOINT_TASKS), share_conv_channel=64),
     test=synth.CENTERPOINT_PILLARS_TEST_CFG,
 )
-
-
-def grid_size(cfg):
-    """(nx, ny) of the pillar grid: 512 x 512 for synth.CP_PILLARS."""
-    pcr, vs = cfg["point_cloud_range"], cfg["voxel_size"]
-    return (int(round((pcr[3] - pcr[0]) / vs[0])), int(round((pcr[4] - pcr[1]) / vs[1])))
 
 
 class CenterPointPillars:
@@ -115,11 +110,8 @@ class CenterPointPillars:
         return self.head.forward_h16(image, shape)
 
     def postprocess(self, h):
-        cfg, tc = self.cfg, self.test_cfg
-        return cpp.centerpoint_postprocess_device(
-            h["hm"], h["reg"], h["height"], h["dim"], h["vel"], h["rot"], cfg["voxel_size"][:2], cfg["point_cloud_range"],
-            tc["post_center_limit_range"], self.label_off, tc["down_ratio"], tc["score_threshold"],
-            tc["nms_iou_threshold"], tc["nms_pre_max_size"], tc["nms_post_max_size"], True)
+        return cpp.centerpoint_postprocess_heads(h, self.cfg["voxel_size"][:2], self.cfg["point_cloud_range"],
+                                                 self.test_cfg, self.label_off)
 
     def calibrate_heatmap_bias(self, points, target_frac=0.014):
         """DenseRPNHead.calibrate_heatmap_bias on this frame's pixel image: ~1.4 % of the cells above the score
@@ -129,13 +121,12 @@ class CenterPointPillars:
         return self
 
     def head_planes(self):
-        """Output planes of the CenterHead: per task 2 + 1 + 3 + 2 + 2 + classes (70 for the six nuScenes tasks)."""
-        return sum(sum(c for _, c in COMMON_HEADS) + n for n in self.head.tasks)
+        return self.head.head_planes()
 
     def flops(self):
         """Algorithmic flops (2 x MACs) of the dense part at the model's grid: backbone, FPN and head (shared conv, the 36
         ConvModules, the output convs)."""
-        out = dict(backbone=0.0, fpn=0.0, head_shared=0.0, head_convmodules=0.0, head_output=0.0)
+        out = dict(backbone=0.0, fpn=0.0)
         h, w = self.grid[1], self.grid[0]
         for blk in self.head.blocks:
             for c in blk:
@@ -144,14 +135,7 @@ class CenterPointPillars:
         for (h, w), de in zip(self.feat_hw, self.head.deblocks):
             oh, ow = SecondTrunk.deblock_out_hw(de, h, w)
             out["fpn"] += 2.0 * oh * ow * de.cin * de.cout * (1 if de.up > 1 else de.k * de.k)
-        px = self.cat_hw[0] * self.cat_hw[1]
-        sh = self.head.shared
-        out["head_shared"] = 2.0 * px * sh.cin * sh.cout * sh.k * sh.k
-        for hs in self.head.heads:
-            for _, a, f in hs:
-                out["head_convmodules"] += 2.0 * px * a.cin * a.cout * a.k * a.k
-                out["head_output"] += 2.0 * px * f.cin * f.cout * f.k * f.k
-        out["head"] = out["head_shared"] + out["head_convmodules"] + out["head_output"]
+        out.update(self.head.head_flops(*self.cat_hw))
         return out
 
 
@@ -164,24 +148,11 @@ class CenterPointPillarsHotPath(CapturedFrame):
                  sweep_input=None, sweep_ring=None):
         """cfg: the point-cloud config (synth.CP_PILLARS by default); sweep_input / sweep_ring: as
         pipeline.CenterPointHotPath (the merged columns are x, y, z, intensity and the time lag: F = 5)."""
-        self.cfg = dict(cfg or synth.CP_PILLARS)
-        self.device = torch.device(device)
-        self.n = int(num_points or self.cfg["num_points"])
-        self.F = self.cfg["point_dim"]
-        self.model = CenterPointPillars(self.cfg, model_cfg).init_weight(seed=seed, device=self.device, bn_gain=bn_gain)
-        self.points = torch.zeros((self.n, self.F), dtype=torch.float32, device=self.device)
-        self.graph = None
-        self.out = None
-        self.stream = torch.cuda.Stream(self.device)
-        self.sweep_input = self.ring = None
-        if sweep_input is not None:
-            self._init_sweep_input(dict(SWEEP_INPUT, **sweep_input), sweep_ring)
-        m = self.model
-        self._alloc_host_outputs(len(m.label_off) * m.test_cfg["nms_post_max_size"], 9, len(m.label_off) + 1,
-                                 1 if self.sweep_input is None else 2)
-
-    def share_model(self, other):
-        self.model = other.model
+        super().__init__(cfg or synth.CP_PILLARS, device, num_points, sweep_input, sweep_ring)
+        m = self.model = CenterPointPillars(self.cfg, model_cfg).init_weight(seed=seed, device=self.device,
+                                                                             bn_gain=bn_gain)
+        self.slot = ResultSlot(len(m.label_off) * m.test_cfg["nms_post_max_size"], 9, len(m.label_off) + 1,
+                               1 if self.sweep_input is None else 2)
 
     def forward_device(self):
         m = self.model
@@ -195,13 +166,8 @@ class CenterPointPillarsHotPath(CapturedFrame):
         return dict(boxes=boxes, scores=scores, labels=labels, counts=counts, num_voxels=nv, coors=coors, head=h,
                     status=status)
 
-    def calibrate_head(self, points_dev):
-        """See CenterPointPillars.calibrate_heatmap_bias.  Call before capture()."""
-        with torch.cuda.stream(self.stream):
-            self.points.copy_(points_dev)
-            self.model.calibrate_heatmap_bias(self.points)
-        self.stream.synchronize()
-        return self
+    def _calibrate(self):
+        self.model.calibrate_heatmap_bias(self.points)
 
     def check_status(self, status_host):
         """Raise when the frame's status word reports dropped rows or an activation outside fp16's range (never a silent

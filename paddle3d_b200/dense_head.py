@@ -203,6 +203,23 @@ class DenseRPNHead:
                 out += [a, b]
         return out
 
+    def head_planes(self):
+        """Output planes of the CenterHead: per task 2 + 1 + 3 + 2 + 2 + classes (70 for the six nuScenes tasks)."""
+        return sum(sum(c for _, c in COMMON_HEADS) + n for n in self.tasks)
+
+    def head_flops(self, h, w):
+        """Algorithmic flops (2 x MACs) of the CenterHead on an h x w map: the shared conv, the ConvModules and the output
+        convs, and their sum "head"."""
+        px = h * w
+        sh = self.shared
+        out = dict(head_shared=2.0 * px * sh.cin * sh.cout * sh.k * sh.k, head_convmodules=0.0, head_output=0.0)
+        for hs in self.heads:
+            for _, a, f in hs:
+                out["head_convmodules"] += 2.0 * px * a.cin * a.cout * a.k * a.k
+                out["head_output"] += 2.0 * px * f.cin * f.cout * f.k * f.k
+        out["head"] = out["head_shared"] + out["head_convmodules"] + out["head_output"]
+        return out
+
     def init_weight(self, seed=0, device="cuda", randomize_bn=False, bn_gain=1.0):
         """device=None: numpy parameters only (enough for export_numpy / the CPU arm).  bn_gain multiplies every BatchNorm
         gamma (sqrt(6) keeps the activations O(1) through the stack, see sparse_nn.BatchNorm.init_parameters)."""

@@ -9,8 +9,8 @@ output on, and LSSHotPath, the same forward as one CUDA graph that serves every 
 import numpy as np
 import torch
 
+from .frame import GraphFrame
 from .ops import bev_pool_v2 as bp
-from .pipeline import _count_graph_nodes
 
 
 class LSSViewTransformer:
@@ -102,70 +102,57 @@ def _mats(input):
     return input[1], input[3], input[4], input[5], input[6]
 
 
-class LSSHotPath:
-    """LSSViewTransformer.forward for B samples of N cameras as one captured CUDA graph on its own stream.  The camera
-    descriptor is a device buffer refreshed by an H2D copy at the head of the graph, so any calibration replays the same
-    graph.  launch() enqueues a frame; infer() waits for it and returns the BEV tensor with counts = (n_kept, n_intervals),
-    copied back in one D2H.  accelerate=True: two graphs, ranks (replayed only when the camera matrices differ from the
-    last ones) and pool (softmax / permute + memset + pool)."""
+class CameraFrame(GraphFrame):
+    """A frame of B samples of N cameras from the depth net's output (logits, tran_feat: device inputs) as captured CUDA
+    graphs on its own stream.  The camera descriptor is a device buffer refreshed by an H2D copy at the head of the rank
+    stage, so any calibration replays the same graphs.  The frame graph is the rank stage and _frame(); with
+    vt.accelerate, a graph "ranks" (replayed only when the camera matrices differ from the last ones) and the graph
+    "frame" of the rest.  A subclass defines _frame()."""
 
     def __init__(self, vt, B, N, device="cuda", stream=None):
+        super().__init__(device, stream)
         self.vt, self.B, self.N = vt, B, N
-        self.device = torch.device(device)
-        self.stream = stream or torch.cuda.Stream(self.device)
         nd = B * N * bp.CAM_FLOATS + B * 9
         self.h_desc = torch.zeros((nd,), dtype=torch.float32).pin_memory()
-        self.h_counts = torch.zeros((2,), dtype=torch.int32).pin_memory()
         self.desc = torch.zeros((nd,), dtype=torch.float32, device=self.device)
         D, H, W, C = vt.D, vt.H, vt.W, vt.out_channels
         self.logits = torch.zeros((B * N, D, H, W), dtype=torch.float32, device=self.device)
         self.tran_feat = torch.zeros((B * N, C, H, W), dtype=torch.float32, device=self.device)
         self.depth = torch.empty_like(self.logits)
         self.feat = torch.empty((B * N, H, W, C), dtype=torch.float32, device=self.device)
-        X, Y, Z = vt.grid
-        self.bev = torch.empty((B, Z * C, Y, X), dtype=torch.float32, device=self.device)
-        self.graphs, self.graph_nodes, self.prepared, self.last = {}, None, None, None
+        self.prepared, self.last = None, None
         self.done = torch.cuda.Event()
 
     # ---- stages, as they are captured
     def _ranks(self):
         self.desc.copy_(self.h_desc, non_blocking=True)
         self.prepared = self.vt._prepare(self.desc, self.B, self.N)
-        self.h_counts.copy_(self.prepared[5], non_blocking=True)
 
-    def _pool(self):
-        bp.lss_depth_feat(self.logits, self.tran_feat, self.depth, self.feat)
-        bp.bev_pool_v2_dev(self.depth, self.feat, self.prepared, self.vt.bev_feat_shape(self.B), planar=True, out=self.bev)
-
-    def _full(self):
+    def _full(self, *args):
         self._ranks()
-        self._pool()
+        return self._frame(*args)
 
-    def capture(self, count_nodes=False):
-        """Warm up eagerly (sizes the workspaces), then capture the frame graph (or, with vt.accelerate, the rank and pool
-        graphs).  count_nodes: node counts by type of the frame graph in self.graph_nodes."""
-        parts = {"ranks": self._ranks, "pool": self._pool} if self.vt.accelerate else {"frame": self._full}
-        with torch.cuda.stream(self.stream):
-            self._full()
-            self.stream.synchronize()
-            for name, fn in parts.items():
-                g = torch.cuda.CUDAGraph(keep_graph=True) if count_nodes else torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g, stream=self.stream):
-                    fn()
-                self.graphs[name] = g
-                if count_nodes:
-                    nodes = _count_graph_nodes(g.raw_cuda_graph())
-                    self.graph_nodes = nodes if self.graph_nodes is None else {
-                        k: self.graph_nodes[k] + nodes[k] for k in nodes}
-        self.stream.synchronize()
+    def _parts(self):
+        return {"ranks": self._ranks, "frame": self._frame} if self.vt.accelerate else {"frame": self._full}
+
+    def capture(self, warmup=1, count_nodes=False):
+        """Warm up eagerly (sizes the workspaces), then capture the graphs.  count_nodes: node counts by type of the
+        graphs in self.graph_nodes."""
         self.last = None
-        return self
+        return super().capture(warmup, count_nodes)
 
     def launch(self, mats, logits=None, tran_feat=None):
         """Enqueue one frame on self.stream.  mats = (sensor2ego, cam2imgs, post_rots, post_trans, bda) on the host;
         logits / tran_feat: device tensors copied into the frame's inputs (None: already written there)."""
+        self._launch(mats, logits, tran_feat, "frame")
+
+    def _launch(self, mats, logits, tran_feat, frame, host_inputs=None):
+        """launch() replaying the graph named frame (with accelerate: after the rank graph when the cameras changed);
+        host_inputs: called once the previous frame is done, to write further pinned inputs the graph uploads."""
         packed = bp.pack_cameras(*mats)
-        self.done.synchronize()  # the previous frame's H2D has read h_desc
+        self.done.synchronize()  # the previous frame's H2D has read h_desc and its D2H has landed
+        if host_inputs is not None:
+            host_inputs()
         self.stream.wait_stream(torch.cuda.current_stream(self.device))  # inputs written on the caller's stream
         with torch.cuda.stream(self.stream):
             if logits is not None:
@@ -174,14 +161,34 @@ class LSSHotPath:
                 self.tran_feat.copy_(tran_feat, non_blocking=True)
             if not self.vt.accelerate:
                 self.h_desc.copy_(torch.from_numpy(packed))
-                self.graphs["frame"].replay()
-            else:
-                if self.last is None or not np.array_equal(self.last, packed):
-                    self.h_desc.copy_(torch.from_numpy(packed))
-                    self.graphs["ranks"].replay()
-                    self.last = packed
-                self.graphs["pool"].replay()
+            elif self.last is None or not np.array_equal(self.last, packed):
+                self.h_desc.copy_(torch.from_numpy(packed))
+                self.graphs["ranks"].replay()
+                self.last = packed
+            self.graphs[frame].replay()
+            self.out = self.outs[frame]
             self.done.record(self.stream)
+
+
+class LSSHotPath(CameraFrame):
+    """LSSViewTransformer.forward for B samples of N cameras as one captured CUDA graph (CameraFrame): descriptor H2D,
+    ranks, softmax / permute, memset + pool.  launch() enqueues a frame; infer() waits for it and returns the BEV tensor
+    with counts = (n_kept, n_intervals), copied back in one D2H inside the rank stage."""
+
+    def __init__(self, vt, B, N, device="cuda", stream=None):
+        super().__init__(vt, B, N, device, stream)
+        self.h_counts = torch.zeros((2,), dtype=torch.int32).pin_memory()
+        X, Y, Z = vt.grid
+        self.bev = torch.empty((B, Z * vt.out_channels, Y, X), dtype=torch.float32, device=self.device)
+
+    # ---- stages, as they are captured
+    def _ranks(self):
+        super()._ranks()
+        self.h_counts.copy_(self.prepared[5], non_blocking=True)
+
+    def _frame(self):
+        bp.lss_depth_feat(self.logits, self.tran_feat, self.depth, self.feat)
+        bp.bev_pool_v2_dev(self.depth, self.feat, self.prepared, self.vt.bev_feat_shape(self.B), planar=True, out=self.bev)
 
     def infer(self, mats, logits=None, tran_feat=None):
         """One frame, waited for: returns (bev [B, C * Z, Y, X] device tensor owned by the frame, counts (n_kept,

@@ -45,6 +45,16 @@ def centerpoint_postprocess_device(hm, reg, height, dim, vel, rot, voxel_size, p
     return bboxes, scores, labels, counts
 
 
+def centerpoint_postprocess_heads(h, voxel_size, point_cloud_range, test_cfg, label_offsets):
+    """centerpoint_postprocess_device (with velocity) of a CenterHead output h = dict name -> [tensor per task], with the
+    range limit, down ratio, threshold and NMS settings of test_cfg and the tasks' label offsets."""
+    tc = test_cfg
+    return centerpoint_postprocess_device(
+        h["hm"], h["reg"], h["height"], h["dim"], h["vel"], h["rot"], voxel_size, point_cloud_range,
+        tc["post_center_limit_range"], label_offsets, tc["down_ratio"], tc["score_threshold"], tc["nms_iou_threshold"],
+        tc["nms_pre_max_size"], tc["nms_post_max_size"], True)
+
+
 def centerpoint_postprocess(hm, reg, height, dim, vel, rot, voxel_size, point_cloud_range, post_center_range,
                             num_classes, down_ratio, score_threshold, nms_iou_threshold, nms_pre_max_size,
                             nms_post_max_size, with_velocity):

@@ -9,7 +9,7 @@ repository's kernels:
     (cls | box | dir as ONE 1x1 conv, fp32 planes) -> anchor_head_postprocess (csrc/anchor_postprocess.cu) -> boxes
 
 PointPillarsHotPath captures everything between the H2D copy of the points and the D2H copy of the boxes as one CUDA graph
-(pipeline.CapturedFrame).  Anchors are constant per model and built once on the host (create_anchors_3d_stride, SECOND's
+(frame.CapturedFrame).  Anchors are constant per model and built once on the host (create_anchors_3d_stride, SECOND's
 box_np_ops), as are the voxel-index corners of each anchor's near box (anchor_voxel_corners) the anchor mask reads."""
 import numpy as np
 import torch
@@ -20,7 +20,7 @@ from .ops import anchor_postprocess as ahp
 from .ops import pillar_encoder as pe
 from .ops import sparse_nn as sp
 from .ops import voxelize as vox
-from .pipeline import CapturedFrame
+from .frame import CapturedFrame, ResultSlot
 
 CONFIG = dict(
     pfn_channels=64, pfn_bn_eps=1e-3,
@@ -232,19 +232,9 @@ class PointPillarsHotPath(CapturedFrame):
     def __init__(self, cfg=None, device="cuda:0", seed=0, num_points=None, bn_gain=1.0, model_cfg=None):
         """cfg: the point-cloud config (synth.C2 by default); model_cfg: the model config (CONFIG by default; synth.C2 with
         CONFIG is the car model, synth.C2_PED_CYCLIST with CONFIG_PED_CYCLIST the cyclist / pedestrian one)."""
-        self.cfg = dict(cfg or synth.C2)
-        self.device = torch.device(device)
-        self.n = int(num_points or self.cfg["num_points"])
-        self.F = self.cfg["point_dim"]
+        super().__init__(cfg or synth.C2, device, num_points)
         self.model = PointPillars(self.cfg, model_cfg).init_weight(seed=seed, device=self.device, bn_gain=bn_gain)
-        self.points = torch.zeros((self.n, self.F), dtype=torch.float32, device=self.device)
-        self.graph = None
-        self.out = None
-        self.stream = torch.cuda.Stream(self.device)
-        self._alloc_host_outputs(self.model.mc["test"]["nms_post_max_size"], 7, 2, 1)
-
-    def share_model(self, other):
-        self.model = other.model
+        self.slot = ResultSlot(self.model.mc["test"]["nms_post_max_size"], 7, 2, 1)
 
     def forward_device(self):
         m = self.model
@@ -255,13 +245,8 @@ class PointPillarsHotPath(CapturedFrame):
         return dict(boxes=boxes, scores=scores, labels=labels, counts=counts, num_voxels=nv, coors=coors, planes=planes,
                     status=status)
 
-    def calibrate_head(self, points_dev):
-        """See PointPillars.calibrate_cls_bias.  Call before capture()."""
-        with torch.cuda.stream(self.stream):
-            self.points.copy_(points_dev)
-            self.model.calibrate_cls_bias(self.points)
-        self.stream.synchronize()
-        return self
+    def _calibrate(self):
+        self.model.calibrate_cls_bias(self.points)
 
     @staticmethod
     def check_status(status_host):

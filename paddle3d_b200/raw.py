@@ -36,6 +36,8 @@ def cudart():
         _rt.cudaMalloc.argtypes = [C.POINTER(C.c_void_p), C.c_size_t]
         _rt.cudaFree.argtypes = [C.c_void_p]
         _rt.cudaMemcpyAsync.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p]
+        _rt.cudaMemcpy2DAsync.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t,
+                                          C.c_int, C.c_void_p]
         _rt.cudaMemsetAsync.argtypes = [C.c_void_p, C.c_int, C.c_size_t, C.c_void_p]
         _rt.cudaStreamCreate.argtypes = [C.POINTER(C.c_void_p)]
         _rt.cudaStreamDestroy.argtypes = [C.c_void_p]

@@ -162,7 +162,8 @@ def main():
 def temporal(args):
     import torch
     from paddle3d_b200 import synth
-    from paddle3d_b200.bevdet import BEVDet, BEVDet4D, BEVDet4DHotPath, BEVDetHotPath, _copy_rows
+    from paddle3d_b200.bevdet import BEVDet, BEVDet4D, BEVDet4DHotPath, BEVDetHotPath
+    from paddle3d_b200.frame import copy_rows
     from paddle3d_b200.ops import bev_pool_v2 as bp
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
@@ -248,7 +249,7 @@ def temporal(args):
         st.synchronize()
     t = {"pre_process (5 convs 80 -> 80, residual epilogue)": graph_time_ms(lambda: m4.pre(img, concat, bufs), st, 10),
          "shift (p3d_bev_shift_h16)": graph_time_ms(lambda: m4.shift(history, tf, concat), st, 50),
-         "history copy (2-D memcpy)": graph_time_ms(lambda: _copy_rows(history, concat, 384), st, 50),
+         "history copy (2-D memcpy)": graph_time_ms(lambda: copy_rows(history, concat, 384), st, 50),
          "encoder (CustomResNet(160) + FPN_LSS)": graph_time_ms(lambda: m4.encode(concat), st, 10)}
     line["stages_ms"] = t
     shift_bytes = 2 * 4 * m4.bev_C * Y * X

@@ -126,7 +126,7 @@ def config4_graph(args, dev, cam):
     from paddle3d_b200.lss import LSSHotPath
     from paddle3d_b200.ops import bev_pool_v2 as bp
     from paddle3d_b200.ops import pillar_encoder, pillar_scatter, voxelize
-    from paddle3d_b200.pipeline import _count_graph_nodes
+    from paddle3d_b200.frame import count_graph_nodes
     vt, mats, logits, tran = cam
     frame = LSSHotPath(vt, 1, 6, device=dev)
     frame.logits.copy_(logits)
@@ -165,7 +165,7 @@ def config4_graph(args, dev, cam):
         g = torch.cuda.CUDAGraph(keep_graph=True)
         with torch.cuda.graph(g, stream=main):
             both()
-        nodes = _count_graph_nodes(g.raw_cuda_graph())
+        nodes = count_graph_nodes(g)
         for _ in range(args.warmup):
             g.replay()
         main.synchronize()

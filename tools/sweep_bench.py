@@ -55,27 +55,18 @@ def host_merge_frames(seq, K, si, cap, pool):
 
 def reupload_stream(sweep, ring, seq, K):
     """Mode (ii): every frame uploads all of its sweeps again (K pushes), then merges them on the device."""
-    import collections
-    lanes = sweep.lanes
-    L = len(lanes)
-    for p in lanes:
+    from paddle3d_b200.frame import run_in_flight
+    for p in sweep.lanes:
         p.prepare_sweep()
     ring.reset()
-    pending = collections.deque()
-    for j in range(len(seq)):
+
+    def submit(lane, j, _, k):
         ids = list(range(max(0, j - K + 1), j + 1))  # oldest first: the key is the last push
         for s in ids:
             last = ring.push(*seq[s])
-        li, k = sweep._lane_slot(j, L)
         ring.first = last - len(ids) + 1  # the frame reads exactly this frame's uploads
-        lanes[li]._submit_sweep(last, k)
-        pending.append((lanes[li], k))
-        if len(pending) > L:
-            pl, pk = pending.popleft()
-            yield pl._result(pk)
-    while pending:
-        pl, pk = pending.popleft()
-        yield pl._result(pk)
+        lane._submit_sweep(last, k)
+    yield from run_in_flight(sweep.lanes, range(len(seq)), submit)
 
 
 def timed(results):
