@@ -342,7 +342,8 @@ int p3d_dense_conv2d_f16_pack_weights(const float *weight_tci, int taps, int Cin
  *   ranks_bev / ranks_depth / ranks_feat sorted by ranks_bev (ties: ascending point index = stable argsort),
  *   interval_starts / interval_lengths; all outputs int32 [B*N*D*H*W] (capacity), counts_dev = {n_kept, n_intervals}.
  *   Entries beyond the counts are zero, except interval_starts (left unwritten).  grid_size_host = (X, Y, Z) cells,
- *   lower bound / interval per axis (x, y, z).
+ *   lower bound / interval per axis (x, y, z).  B * X * Y * Z <= 2^31, so that every rank (at most cells - 1) is an
+ *   int32, and B * N * D * H * W <= 2^31 - 1 (P3D_ERR_UNSUPPORTED otherwise).
  * ------------------------------------------------------------------------------------------- */
 size_t p3d_bev_pool_prepare_workspace_bytes(int64_t num_points);
 int p3d_bev_pool_prepare(const float *coor, int B, int N, int D, int H, int W, const float *grid_lower_bound_host,
@@ -363,8 +364,8 @@ typedef struct p3d_lss_camera {
 } p3d_lss_camera;
 
 /* get_lidar_coor fused with voxel_pooling_prepare_v2: the outputs, their capacity B*N*D*H*W, the tie order and the
- * workspace (p3d_bev_pool_prepare_workspace_bytes(B*N*D*H*W)) are those of p3d_bev_pool_prepare, but the frustum points
- * are computed in registers instead of read from a coor tensor.  cams [B*N] and bda [B, 9] are device buffers (refresh
+ * workspace (p3d_bev_pool_prepare_workspace_bytes(B*N*D*H*W)) and the size limits (B*X*Y*Z <= 2^31) are those of
+ * p3d_bev_pool_prepare, but the frustum points are computed in registers instead of read from a coor tensor.  cams [B*N] and bda [B, 9] are device buffers (refresh
  * them with a copy before each launch and one captured graph serves every calibration); axis_depth [D], axis_x [W],
  * axis_y [H] fp32 are create_frustum's arange(*depth), linspace(0, W_in - 1, W), linspace(0, H_in - 1, H).
  * coor (nullable): the ego points as [B, N, D, H, W, 3] fp32, what get_lidar_coor returns. */
@@ -381,8 +382,8 @@ int p3d_lss_depth_feat(const float *logits, const float *tran_feat, int BN, int 
 /* bev_pool_v2 with the interval count on the device (counts_dev[1], as p3d_bev_pool_prepare / p3d_lss_prepare write it;
  * capacity = length of the rank arrays), so that it can be captured once for every calibration.  Bit-identical to
  * p3d_bev_pool_v2 (same kernel).  out is zero-filled here: planar 0 -> [B, Z, Y, X, c], planar 1 -> [B, Z * c, Y, X]
- * with channel z * c + ch (view_transform's collapse_z layout).  c % 4 == 0, c <= 256, feat / out 16-byte aligned
- * (P3D_ERR_UNSUPPORTED otherwise). */
+ * with channel z * c + ch (view_transform's collapse_z layout).  c % 4 == 0, c <= 256, feat / out 16-byte aligned,
+ * B * Z * Y * X <= 2^31 (the int32 ranks' range) (P3D_ERR_UNSUPPORTED otherwise). */
 int p3d_bev_pool_v2_dev(const float *depth, const float *feat, const int32_t *ranks_depth, const int32_t *ranks_feat,
                         const int32_t *ranks_bev, const int32_t *interval_lengths, const int32_t *interval_starts,
                         const int32_t *counts_dev, int64_t capacity, int c, int B, int Z, int Y, int X, int planar,
@@ -438,7 +439,8 @@ int p3d_upsample_bilinear_h16(const void *in_h16, int B, int h, int w, int C, in
 /* p3d_bev_pool_v2_dev into pixel H16 rows: out_h16 [B, Y, X, out_C] with channel z * c + ch of cell (y, x) (the layout of
  * the planar output, one pixel per row), same accumulation, then split into (hi, lo'); status bit 0 on fp16 overflow.
  * out_h16 is zero-filled here (empty cells and channels >= Z * c).  out_C % 32 == 0 and out_C >= Z * c
- * (P3D_ERR_INVALID_ARG otherwise); c % 4 == 0, c <= 256, feat / out_h16 16-byte aligned (P3D_ERR_UNSUPPORTED). */
+ * (P3D_ERR_INVALID_ARG otherwise); c % 4 == 0, c <= 256, feat / out_h16 16-byte aligned, B * Z * Y * X <= 2^31 (the int32
+ * ranks' range) (P3D_ERR_UNSUPPORTED). */
 int p3d_bev_pool_v2_dev_h16(const float *depth, const float *feat, const int32_t *ranks_depth, const int32_t *ranks_feat,
                             const int32_t *ranks_bev, const int32_t *interval_lengths, const int32_t *interval_starts,
                             const int32_t *counts_dev, int64_t capacity, int c, int B, int Z, int Y, int X, void *out_h16,

@@ -273,9 +273,9 @@ extern "C" int p3d_bev_pool_v2_dev(const float *depth, const float *feat, const 
   if (!depth || !feat || !ranks_depth || !ranks_feat || !ranks_bev || !interval_lengths || !interval_starts || !counts_dev ||
       !out || capacity < 0 || c < 1 || B < 1 || Z < 1 || Y < 1 || X < 1 || (planar != 0 && planar != 1))
     return P3D_ERR_INVALID_ARG;
-  const long long cells = static_cast<long long>(B) * Z * Y * X;
+  const long long cells = static_cast<long long>(B) * Z * Y * X;  // <= 2^31: every rank, at most cells - 1, is an int32
   if (c % 4 || c > 256 || (reinterpret_cast<uintptr_t>(feat) & 15) || (reinterpret_cast<uintptr_t>(out) & 15) ||
-      capacity > 0x7fffffffll || cells >= 0xffffffffll || static_cast<long long>(Y) * X > 0x7fffffffll)
+      capacity > 0x7fffffffll || cells > 0x80000000ll || static_cast<long long>(Y) * X > 0x7fffffffll)
     return P3D_ERR_UNSUPPORTED;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   P3D_CUDA_CHECK(cudaMemsetAsync(out, 0, static_cast<size_t>(cells) * c * sizeof(float), st));
@@ -309,7 +309,7 @@ extern "C" int p3d_bev_pool_v2_dev_h16(const float *depth, const float *feat, co
     return P3D_ERR_INVALID_ARG;
   const long long cells = static_cast<long long>(B) * Z * Y * X;
   if (c % 4 || c > 256 || (reinterpret_cast<uintptr_t>(feat) & 15) || (reinterpret_cast<uintptr_t>(out_h16) & 15) ||
-      capacity > 0x7fffffffll || cells >= 0xffffffffll || static_cast<long long>(Y) * X > 0x7fffffffll)
+      capacity > 0x7fffffffll || cells > 0x80000000ll || static_cast<long long>(Y) * X > 0x7fffffffll)
     return P3D_ERR_UNSUPPORTED;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   // empty cells and the channels from Z * c up to out_C stay zero

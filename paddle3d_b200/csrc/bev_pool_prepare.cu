@@ -187,7 +187,8 @@ int prep_setup(int B, int N, int D, int H, int W, const float *lower, const floa
   if (!lower || !interval || !grid_size || !workspace || B < 1 || N < 1 || D < 1 || H < 1 || W < 1) return P3D_ERR_INVALID_ARG;
   const long long n = static_cast<long long>(B) * N * D * H * W;
   const long long cells = static_cast<long long>(B) * grid_size[0] * grid_size[1] * grid_size[2];
-  if (n > 0x7fffffffll || cells < 1 || cells >= 0xffffffffll || grid_size[0] < 1 || grid_size[1] < 1 || grid_size[2] < 1)
+  // ranks are int32: the largest, cells - 1, must fit (a larger key would be stored as a negative rank)
+  if (n > 0x7fffffffll || cells < 1 || cells > 0x80000000ll || grid_size[0] < 1 || grid_size[1] < 1 || grid_size[2] < 1)
     return P3D_ERR_UNSUPPORTED;
   if (reinterpret_cast<uintptr_t>(workspace) & 255) return P3D_ERR_INVALID_ARG;
   for (int a = 0; a < 3; ++a) {

@@ -111,19 +111,26 @@ def test_lss_entry_points_reject_invalid_arguments():
     lo, iv = _lib.host_floats([-51.2, -51.2, -5]), _lib.host_floats([0.8, 0.8, 8])
     gs = _lib.host_ints([128, 128, 1])
 
-    def prep(cams=p, bda=p, ad=p, ax=p, ay=p, B=1, N=6, D=118, H=16, W=44, lo=lo, iv=iv, gs=gs, outs=(p,) * 6, ws=p):
-        return L.p3d_lss_prepare(cams, bda, ad, ax, ay, B, N, D, H, W, lo, iv, gs, None, *outs, ws, 1 << 30, None)
+    def prep(cams=p, bda=p, ad=p, ax=p, ay=p, B=1, N=6, D=118, H=16, W=44, lo=lo, iv=iv, gs=gs, outs=(p,) * 6, ws=p,
+             wsb=1 << 30):
+        return L.p3d_lss_prepare(cams, bda, ad, ax, ay, B, N, D, H, W, lo, iv, gs, None, *outs, ws, wsb, None)
     for kw in (dict(cams=None), dict(bda=None), dict(ad=None), dict(ax=None), dict(ay=None), dict(lo=None), dict(gs=None),
                dict(outs=(p,) * 5 + (None,)), dict(outs=(None,) + (p,) * 5), dict(ws=None), dict(B=0), dict(N=-1), dict(D=0),
                dict(H=0), dict(W=0)):
         assert prep(**kw) == -1, kw
     assert prep(B=2, N=6, D=4096, H=512, W=512) == -4                        # B*N*D*H*W > 2^31 - 1
-    assert prep(B=1 << 12, N=1, D=1, H=1, W=1, gs=_lib.host_ints([1024, 1024, 1024])) == -4  # B * cells >= 2^32
+    # ranks are int32: B * X * Y * Z <= 2^31 cells.  Exactly 2^31 gets past the guard to the workspace check (1 byte:
+    # P3D_ERR_WORKSPACE, before any launch); one more column is refused.
+    g31, g31x = _lib.host_ints([1024, 1024, 1024]), _lib.host_ints([1025, 1024, 1024])
+    assert prep(B=2, N=1, D=1, H=1, W=1, gs=g31, wsb=1) == -2
+    assert prep(B=2, N=1, D=1, H=1, W=1, gs=g31x, wsb=1) == -4
     assert prep(gs=_lib.host_ints([128, 0, 1])) == -4
     assert prep(ws=C.c_void_p(260)) == -1                                    # workspace not 256-byte aligned
     # the existing coordinate entry point keeps its checks
     assert L.p3d_bev_pool_prepare(None, 1, 6, 118, 16, 44, lo, iv, gs, p, p, p, p, p, p, p, 1 << 30, None) == -1
     assert L.p3d_bev_pool_prepare(p, 2, 6, 4096, 512, 512, lo, iv, gs, p, p, p, p, p, p, p, 1 << 30, None) == -4
+    assert L.p3d_bev_pool_prepare(p, 2, 1, 1, 1, 1, lo, iv, g31, p, p, p, p, p, p, p, 1, None) == -2
+    assert L.p3d_bev_pool_prepare(p, 2, 1, 1, 1, 1, lo, iv, g31x, p, p, p, p, p, p, p, 1, None) == -4
     # depth softmax + permute
     df = L.p3d_lss_depth_feat
     assert df(None, p, 6, 118, 16, 44, 80, p, p, None) == -1
@@ -144,5 +151,8 @@ def test_lss_entry_points_reject_invalid_arguments():
     assert pool(cap=-1) == -1 and pool(c=0) == -1 and pool(Y=0) == -1 and pool(planar=2) == -1
     assert pool(c=7) == -4 and pool(c=260) == -4                            # warp kernel: c % 4 == 0, c <= 256
     assert pool(out=C.c_void_p(260)) == -4                                  # float4 stores need 16-byte alignment
-    assert pool(B=1 << 12, Z=1024, Y=1024, X=1) == -4                       # B * cells >= 2^32
+    assert pool(B=2, Z=1024, Y=1024, X=1025) == -4                          # B * cells > 2^31: a rank past int32
     assert pool(cap=1 << 31) == -4
+    # the pixel-row form has the same cell limit (c = 4 so that Z * c fits out_C)
+    ph = L.p3d_bev_pool_v2_dev_h16
+    assert ph(*(p,) * 8, 1000, 4, 2, 1024, 1024, 1025, p, 4096, p, None) == -4
