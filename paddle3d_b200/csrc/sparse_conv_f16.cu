@@ -25,7 +25,8 @@
 // Split-K / stream-K over taps (few tiles on the deep levels): the decomposition (no split, 2-4 tap splits or stream-K)
 // is chosen ON THE DEVICE from the row count so that the work items fill the grid; partial tiles go to scratch slabs and
 // the LAST arriving CTA of a tile (ticket counter) sums the slabs in index order (deterministic) and runs the fused
-// epilogue - no finalize launch.  Launched with PDL (launch_pdl).
+// epilogue - no finalize launch.  Nothing else runs on the SM during an epilogue, so its global loads (slabs, residual
+// rows) are issued a fragment at a time, not one dependent round trip per pair.  Launched with PDL (launch_pdl).
 #include <cuda.h>
 #include <cuda_fp16.h>
 
@@ -178,21 +179,14 @@ __global__ void __launch_bounds__(kThreads, 1) conv_f16_kernel(const Params p) {
   constexpr int S = C::STAGES, NSUB = C::NSUB;
   constexpr int H = COUT / 2;  // accumulator registers of the hi products; the cross products follow
   pdl_trigger();
-  pdl_wait();  // the input rows are the previous layer's output
-  const long long n = p.n_out_dev ? min(static_cast<long long>(p.n_out_dev[0]), p.n_cap) : p.n_cap;
-  const long long n_tiles = (n + kM - 1) / kM;
-  const int K = p.K;
-  const Sched sc = make_sched(n_tiles, K, p.smax);
-  if (sc.stream ? (sc.u0 >= sc.u1) : (static_cast<long long>(blockIdx.x) >= sc.n_work)) return;
-
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  int32_t *s_nbr = reinterpret_cast<int32_t *>(smem + S * C::STAGE);  // [kM * K]
   __shared__ __align__(8) unsigned long long s_bar[kMaxStages + 1];    // full[S] (weight bytes) | neighbour map landed
   constexpr int kF = 0, kNR = kMaxStages;
   __shared__ int s_last;
   __shared__ float s_scale[COUT], s_shift[COUT];
 
+  // barrier init and the BN constants read nothing the previous kernel wrote: they overlap its tail
   const int tid = threadIdx.x, wg = tid >> 7, wtid = tid & 127;
   if (tid < COUT) {
     s_scale[tid] = p.scale ? __ldg(p.scale + tid) : 1.0f;
@@ -204,6 +198,13 @@ __global__ void __launch_bounds__(kThreads, 1) conv_f16_kernel(const Params p) {
     fence_mbar_init();
   }
   __syncthreads();
+  pdl_wait();  // the row count and the input rows are earlier kernels' output
+  const long long n = p.n_out_dev ? min(static_cast<long long>(p.n_out_dev[0]), p.n_cap) : p.n_cap;
+  const long long n_tiles = (n + kM - 1) / kM;
+  const int K = p.K;
+  const Sched sc = make_sched(n_tiles, K, p.smax);
+  if (sc.stream ? (sc.u0 >= sc.u1) : (static_cast<long long>(blockIdx.x) >= sc.n_work)) return;
+  int32_t *s_nbr = reinterpret_cast<int32_t *>(smem + S * C::STAGE);  // [kM * K]
   const uint32_t ring = smem_u32(smem);
   const int sub4 = tid >> 3, ch = tid & 7;  // gather: 32 rows x 8 16-byte chunks per CTA instruction
   constexpr int KCO = (COUT >= 32) ? 32 : 16;  // channels per H16 group of the output / residual rows
@@ -356,23 +357,40 @@ __global__ void __launch_bounds__(kThreads, 1) conv_f16_kernel(const Params p) {
       finish = s_last != 0;
       if (finish) {
         __threadfence();
-        // slabs in index order (deterministic)
+        // slabs in index order (deterministic); slab outermost, so that a slab's loads are all in flight together
+        // instead of one round trip per fragment pair
 #pragma unroll
-        for (int i = 0; i < H; i += 2) {
-          const int r = wg * 64 + frag_row(i, wtid), c = frag_col(i, wtid);
-          float2 v = make_float2(0.f, 0.f);
-          for (int sp = 0; sp < pieces; ++sp) {
-            const float2 t2 = __ldcg(reinterpret_cast<const float2 *>(
-                p.slabs + ((static_cast<size_t>(sp) * tiles_cap + static_cast<size_t>(tile)) * kM + r) * COUT + c));
-            v.x += t2.x;
-            v.y += t2.y;
+        for (int i = 0; i < H; ++i) acc[i] = 0.f;
+        for (int sp = 0; sp < pieces; ++sp) {
+          const float *slab = p.slabs + ((static_cast<size_t>(sp) * tiles_cap + static_cast<size_t>(tile)) * kM) * COUT;
+          float2 t2[H / 2];
+#pragma unroll
+          for (int i = 0; i < H; i += 2) {
+            const int r = wg * 64 + frag_row(i, wtid), c = frag_col(i, wtid);
+            t2[i / 2] = __ldcg(reinterpret_cast<const float2 *>(slab + r * COUT + c));
           }
-          acc[i] = v.x;
-          acc[i + 1] = v.y;
+#pragma unroll
+          for (int i = 0; i < H; i += 2) {
+            acc[i] += t2[i / 2].x;
+            acc[i + 1] += t2[i / 2].y;
+          }
         }
       }
     }
     if (finish) {
+      // the residual pairs of the whole fragment are loaded before the first output store (the compiler cannot move a
+      // load above a store that may alias it): one round trip instead of one per fragment pair
+      __half2 rhi[H / 2], rlo[H / 2];
+      if (p.residual) {
+#pragma unroll
+        for (int i = 0; i < H; i += 2) {
+          const int r = wg * 64 + frag_row(i, wtid), c = frag_col(i, wtid);
+          if (r >= rows) continue;
+          const uint8_t *rp = p.residual + static_cast<size_t>(row0 + r) * (4 * COUT) + (c / KCO) * (4 * KCO) + (c % KCO) * 2;
+          rhi[i / 2] = *reinterpret_cast<const __half2 *>(rp);
+          rlo[i / 2] = *reinterpret_cast<const __half2 *>(rp + 2 * KCO);
+        }
+      }
 #pragma unroll
       for (int i = 0; i < H; i += 2) {
         const int r = wg * 64 + frag_row(i, wtid), c = frag_col(i, wtid);
@@ -382,8 +400,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_f16_kernel(const Params p) {
         float v[2] = {acc[i], acc[i + 1]};
         float res[2] = {0.f, 0.f};
         if (p.residual) {
-          const uint8_t *rp = p.residual + orow * (4 * COUT) + goff;
-          const __half2 hh = *reinterpret_cast<const __half2 *>(rp), ll = *reinterpret_cast<const __half2 *>(rp + 2 * KCO);
+          const __half2 hh = rhi[i / 2], ll = rlo[i / 2];
           res[0] = merge_h16(__low2half(hh), __low2half(ll));
           res[1] = merge_h16(__high2half(hh), __high2half(ll));
         }
