@@ -140,7 +140,46 @@ int p3d_centerpoint_postprocess(int num_tasks, const float *const *hm, const int
                                 size_t workspace_bytes, p3d_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
- * Sparse 3-D convolution      replaces the paddle.sparse.nn layer calls made by SparseResNet3D /
+ * bevdet_postprocess      BEVDet's own box decode, CenterHead.get_bboxes (CenterPointBBoxCoder.decode,
+ *                         get_task_detections with scale-NMS, circle_nms), batch size 1.  PARITY UNPINNED: the rules
+ *                         below are recalled from BEVDet's head, not checked against a checkout of it.
+ *   hm/reg/height/dim/vel/rot, hm_channels_host[T]: as centerpoint_postprocess.  Per task t with C_t classes:
+ *   1. every (class c, cell i) with score = sigmoid(hm[c, i]) > score_threshold is a candidate (not the cell's arg-max);
+ *   2. the max_num best of them, by descending score; equal scores order by ascending c * H*W + i (torch.topk leaves
+ *      ties undefined; this is the order defined here);
+ *   3. x = (xs + reg0) * out_size_factor * voxel_size[0] + point_cloud_range[0], y likewise, z = height,
+ *      dims = exp(dim), rot = atan2f(rot0, rot1), velocity copied (fp32, each operation rounded on its own);
+ *   4. kept iff the DECODED (x, y, z) lies in post_center_range, both ends inclusive;
+ *   5. suppression over the first pre_max_size survivors in score order; a box is suppressed by a kept box ahead of it
+ *      nms_type_host[t] == P3D_BEVDET_NMS_ROTATE: when the rotated BEV IoU of (x, y, z, dx*f, dy*f, dz, rot) exceeds
+ *        nms_thr_host[t], f = rescale_host[class] (one factor per class, the tasks' classes concatenated; no w/l swap);
+ *      nms_type_host[t] == P3D_BEVDET_NMS_CIRCLE: when the squared centre distance (fp32) is <= min_radius_host[t];
+ *      the first post_max_size kept boxes survive;
+ *   6. rows are (x, y, z - dz/2, dx, dy, dz, rot, vx, vy): bottom centre, dims unscaled (the reference multiplies by f
+ *      and divides again: at most one ulp from the value written here), label = c + label_offset_host[t].
+ *   Outputs (device), sized for the worst case: bboxes [T * post_max_size, 9], scores, labels int64,
+ *   counts [T + 1] int32: rows per task, then the total.  An empty task contributes no row.
+ *   Non-finite inputs: a NaN logit is no candidate and +inf scores 1, so every score is finite; a candidate whose
+ *   decoded centre is NaN or infinite fails the range test, and one whose dims, rot or velocity are NaN or infinite
+ *   is dropped with it (the reference has no such rule: it would carry the value into its NMS).  Every row is finite.
+ *   Limits (P3D_ERR_UNSUPPORTED): T <= 16, at most 64 classes over all tasks, max_num <= 393216.
+ * ------------------------------------------------------------------------------------------- */
+#define P3D_BEVDET_NMS_ROTATE 0
+#define P3D_BEVDET_NMS_CIRCLE 1
+size_t p3d_bevdet_postprocess_workspace_bytes(int num_tasks, const int32_t *hm_channels_host, int feat_h, int feat_w,
+                                              int max_num);
+int p3d_bevdet_postprocess(int num_tasks, const float *const *hm, const int32_t *hm_channels_host,
+                           const float *const *reg, const float *const *height, const float *const *dim,
+                           const float *const *vel, const float *const *rot, int feat_h, int feat_w,
+                           const float *voxel_size_host, const float *point_cloud_range_host,
+                           const float *post_center_range_host, int out_size_factor, float score_threshold,
+                           int max_num, int pre_max_size, int post_max_size, const int32_t *nms_type_host,
+                           const float *nms_thr_host, const float *min_radius_host, const float *rescale_host,
+                           const int32_t *label_offset_host, float *bboxes, float *scores, int64_t *labels,
+                           int32_t *counts, void *workspace, size_t workspace_bytes, p3d_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Sparse 3-D convolution     replaces the paddle.sparse.nn layer calls made by SparseResNet3D /
  *   SparseNet3D (paddle3d/models/middle_encoders/sparse_resnet.py:31-60,84-111,125-206;
  *   sparsenet.py:38-52,75-155): SubmConv3D / Conv3D (+ BatchNorm(eval) + residual add + ReLU fused).
  *

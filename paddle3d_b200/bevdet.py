@@ -5,10 +5,13 @@ against either file):
     camera descriptor H2D -> p3d_lss_prepare -> depth softmax / permute -> bev_pool straight into the pixel fp16-pair image
     [128 x 128 x 96] (channels 80..95 zero) -> CustomResNet (BasicBlocks, residual added in the conv epilogue) -> FPN_LSS
     (bilinear x4 / x2 with align_corners on the pair rows) -> CenterHead (dense_head.DenseRPNHead with this encoder as its
-    trunk) -> centerpoint_postprocess_device -> boxes
+    trunk) -> centerpoint_postprocess_device or bevdet_postprocess_device -> boxes
 
-BEVDetHotPath captures all of it, from the descriptor upload to the D2H copy of the boxes, as one CUDA graph.  The
-postprocess is the custom op Paddle3D's predict_by_custom_op calls (rotated NMS per task), not BEVDet's scale-NMS."""
+BEVDetHotPath captures all of it, from the descriptor upload to the D2H copy of the boxes, as one CUDA graph.  Which
+decode runs follows from the model's test config, as in the reference's configs: one without nms_type (CONFIG) runs the
+custom op Paddle3D's predict_by_custom_op calls (arg-max class per cell, one rotated NMS threshold, 83 boxes per task,
+gravity centre); one with nms_type (CONFIG_BEVDET_NMS) runs BEVDet's own get_bboxes (ops.bevdet_postprocess: top-K over
+class x cell, per-class scale-NMS or circle NMS, bottom centre, up to post_max_size boxes per task)."""
 import numpy as np
 import torch
 
@@ -17,6 +20,7 @@ from .dense_head import DenseRPNHead, _Conv
 from .frame import ResultSlot, ResultSlotOwner, copy_rows
 from .lss import CameraFrame, LSSViewTransformer
 from .ops import bev_pool_v2 as bp
+from .ops import bevdet_postprocess as bdp
 from .ops import centerpoint_postprocess as cpp
 from .ops import dense_conv as dc
 from .ops import sparse_nn as sp
@@ -31,6 +35,19 @@ CONFIG = dict(
     # voxel size 0.1 x down_ratio 8 = the 0.8 m cells of the BEV grid
     test=dict(synth.CENTERPOINT_TEST_CFG, voxel_size=(0.1, 0.1), point_cloud_range=[-51.2, -51.2, -5.0, 51.2, 51.2, 3.0]),
 )
+
+# PARITY UNPINNED: BEVDet's own test config, recalled from bevdet-r50 (tasks: car | truck, construction vehicle | bus,
+# trailer | barrier | motorcycle, bicycle | pedestrian, traffic cone).  nms_rescale_factor is per task a scalar or one
+# factor per class; max_per_img is carried for completeness: get_bboxes never reads it.
+TEST_CFG_BEVDET = dict(
+    max_num=500, score_threshold=0.1, out_size_factor=8, pre_max_size=1000, post_max_size=500, max_per_img=500,
+    post_center_limit_range=[-61.2, -61.2, -10.0, 61.2, 61.2, 10.0],
+    nms_type=["rotate", "rotate", "rotate", "circle", "rotate", "rotate"],
+    nms_thr=[0.2, 0.2, 0.2, 0.2, 0.2, 0.5],
+    nms_rescale_factor=[1.0, [0.7, 0.7], [0.4, 0.55], 1.1, [1.0, 1.0], [4.5, 9.0]],
+    min_radius=[4, 12, 10, 1, 0.85, 0.175],
+    voxel_size=(0.1, 0.1), point_cloud_range=[-51.2, -51.2, -5.0, 51.2, 51.2, 3.0])
+CONFIG_BEVDET_NMS = dict(CONFIG, test=TEST_CFG_BEVDET)
 
 
 def round32(c):
@@ -187,8 +204,15 @@ class BEVDet:
         """Encoder input (BEVDet: the pool image) -> dict name -> per-task [1, k, 128, 128] fp32 head planes."""
         return self.head.forward_h16(image, self.enc_shape)
 
+    def result_rows(self):
+        """Rows of the worst-case-sized outputs of postprocess."""
+        tc = self.test_cfg
+        return len(self.label_off) * tc["post_max_size" if "nms_type" in tc else "nms_post_max_size"]
+
     def postprocess(self, h):
         tc = self.test_cfg
+        if "nms_type" in tc:  # BEVDet's get_bboxes; without it the Paddle custom op's rules
+            return bdp.bevdet_postprocess_heads(h, tc, self.label_off)
         return cpp.centerpoint_postprocess_heads(h, tc["voxel_size"], tc["point_cloud_range"], tc, self.label_off)
 
     def forward(self, mats, logits, tran_feat):
@@ -233,7 +257,7 @@ class BEVDet:
 class BEVDetHotPath(ResultSlotOwner, CameraFrame):
     """One BEVDet frame as one captured CUDA graph on its own stream (CameraFrame): camera descriptor H2D ->
     p3d_lss_prepare -> depth softmax / permute -> memset + pool into the pixel image -> encoder -> head -> postprocess ->
-    one D2H of boxes [6 x 83, 9], scores, labels, counts and the status word.  Any calibration replays the same graph.
+    one D2H of boxes [6 x 83, 9] ([6 x 500, 9] with BEVDet's own decode), scores, labels, counts and the status word.  Any calibration replays the same graph.
     accelerate (the model's view transformer built with accelerate=True): two graphs, ranks (replayed only when the camera
     matrices differ from the last ones) and the rest.  Several lanes may share one model (share_model), each with its own
     buffers and stream.  The status word is the device's fp16-pair overflow flag (ops.sparse_nn.status_tensor), which
@@ -244,7 +268,7 @@ class BEVDetHotPath(ResultSlotOwner, CameraFrame):
         self.model = model
         _, Y, X, pc = model.image_shape
         self.image = torch.empty((Y * X, 2 * pc), dtype=torch.float16, device=self.device)
-        self.slot = ResultSlot(len(model.label_off) * model.test_cfg["nms_post_max_size"], 9, len(model.label_off) + 1, 1)
+        self.slot = ResultSlot(model.result_rows(), 9, len(model.label_off) + 1, 1)
 
     def share_model(self, other):
         self.model, self.vt = other.model, other.vt
@@ -286,6 +310,7 @@ class BEVDetHotPath(ResultSlotOwner, CameraFrame):
 # num_layer=[2], num_channels=[80], stride=[1]) and the encoder's numC_input = 80 * (num_adj + 1).
 CONFIG_4D = dict(CONFIG, backbone=dict(CONFIG["backbone"], in_channels=160),
                  pre_process=dict(num_channels=(80,), strides=(1,), blocks=2), num_adj=1)
+CONFIG_4D_BEVDET_NMS = dict(CONFIG_4D, test=TEST_CFG_BEVDET)
 
 
 class BEVDet4D(BEVDet):

@@ -808,3 +808,69 @@ PD_BUILD_OP(p3d_bev_shift_h16)
     .SetKernelFn(PD_KERNEL(p3d_bev_shift_h16_op))
     .SetInferShapeFn(PD_INFER_SHAPE(ShiftH16InferShape))
     .SetInferDtypeFn(PD_INFER_DTYPE(ShiftH16InferDtype));
+
+// ---------------------------------------------------------------- p3d_bevdet_postprocess  (BEVDet's CenterHead.get_bboxes, Python in the reference)
+// nms_type: 0 rotate / 1 circle per task; nms_rescale_factor: one factor per class, the tasks' classes concatenated.
+std::vector<paddle::Tensor> p3d_bevdet_postprocess_op(
+    const std::vector<paddle::Tensor> &hm, const std::vector<paddle::Tensor> &reg,
+    const std::vector<paddle::Tensor> &height, const std::vector<paddle::Tensor> &dim,
+    const std::vector<paddle::Tensor> &vel, const std::vector<paddle::Tensor> &rot, const std::vector<float> &voxel_size,
+    const std::vector<float> &point_cloud_range, const std::vector<float> &post_center_range,
+    const std::vector<int> &label_offsets, const int out_size_factor, const float score_threshold, const int max_num,
+    const int pre_max_size, const int post_max_size, const std::vector<int> &nms_type, const std::vector<float> &nms_thr,
+    const std::vector<float> &min_radius, const std::vector<float> &nms_rescale_factor) {
+  P3D_CHECK_GPU(hm[0]);
+  PD_CHECK(hm[0].shape()[0] == 1, "hm[0] batch size must be 1.");
+  const int T = static_cast<int>(hm.size());
+  const int H = static_cast<int>(hm[0].shape()[2]), W = static_cast<int>(hm[0].shape()[3]);
+  std::vector<const float *> p[6];
+  std::vector<int32_t> hm_c(T);
+  const std::vector<paddle::Tensor> *lists[6] = {&hm, &reg, &height, &dim, &vel, &rot};
+  size_t classes = 0;
+  for (int k = 0; k < 6; ++k) {
+    PD_CHECK(static_cast<int>(lists[k]->size()) == T, "one tensor per task in every input list.");
+    for (int t = 0; t < T; ++t) p[k].push_back((*lists[k])[t].data<float>());
+  }
+  for (int t = 0; t < T; ++t) classes += hm_c[t] = static_cast<int32_t>(hm[t].shape()[1]);
+  PD_CHECK(static_cast<int>(label_offsets.size()) >= T && static_cast<int>(nms_type.size()) == T &&
+               static_cast<int>(nms_thr.size()) == T && static_cast<int>(min_radius.size()) == T,
+           "label_offsets, nms_type, nms_thr and min_radius have one entry per task.");
+  PD_CHECK(nms_rescale_factor.size() == classes, "nms_rescale_factor has one entry per class.");
+  const int rows = T * (post_max_size > 1 ? post_max_size : 1);
+  auto bboxes = paddle::empty({rows, 9}, paddle::DataType::FLOAT32, paddle::GPUPlace());
+  auto scores = paddle::empty({rows}, paddle::DataType::FLOAT32, paddle::GPUPlace());
+  auto labels = paddle::empty({rows}, paddle::DataType::INT64, paddle::GPUPlace());
+  auto counts = paddle::empty({T + 1}, paddle::DataType::INT32, paddle::GPUPlace());
+  const size_t ws_bytes = p3d_bevdet_postprocess_workspace_bytes(T, hm_c.data(), H, W, max_num);
+  auto ws = workspace(ws_bytes);
+  P3D_CALL(p3d_bevdet_postprocess(T, p[0].data(), hm_c.data(), p[1].data(), p[2].data(), p[3].data(), p[4].data(),
+                                  p[5].data(), H, W, voxel_size.data(), point_cloud_range.data(), post_center_range.data(),
+                                  out_size_factor, score_threshold, max_num, pre_max_size, post_max_size, nms_type.data(),
+                                  nms_thr.data(), min_radius.data(), nms_rescale_factor.data(), label_offsets.data(),
+                                  bboxes.data<float>(), scores.data<float>(), labels.data<int64_t>(), counts.data<int>(),
+                                  ws.data<uint8_t>(), ws_bytes, hm[0].stream()));
+  // data-dependent shape {-1, 9}: one scalar read gives K, then slice
+  const int k = counts.copy_to(paddle::CPUPlace(), true).data<int>()[T];
+  return {paddle::experimental::slice(bboxes, {0}, {0}, {k}, {}, {}), paddle::experimental::slice(scores, {0}, {0}, {k}, {}, {}),
+          paddle::experimental::slice(labels, {0}, {0}, {k}, {}, {})};
+}
+
+std::vector<std::vector<int64_t>> BevdetPostProcessInferShape(
+    const std::vector<std::vector<int64_t>> &hm_shape, const std::vector<std::vector<int64_t>> &reg_shape,
+    const std::vector<std::vector<int64_t>> &height_shape, const std::vector<std::vector<int64_t>> &dim_shape,
+    const std::vector<std::vector<int64_t>> &vel_shape, const std::vector<std::vector<int64_t>> &rot_shape) {
+  return {{-1, 9}, {-1}, {-1}};
+}
+
+PD_BUILD_OP(p3d_bevdet_postprocess)
+    .Inputs({paddle::Vec("HM"), paddle::Vec("REG"), paddle::Vec("HEIGHT"), paddle::Vec("DIM"), paddle::Vec("VEL"),
+             paddle::Vec("ROT")})
+    .Outputs({"BBOXES", "SCORES", "LABELS"})
+    .SetKernelFn(PD_KERNEL(p3d_bevdet_postprocess_op))
+    .Attrs({"voxel_size: std::vector<float>", "point_cloud_range: std::vector<float>",
+            "post_center_range: std::vector<float>", "label_offsets: std::vector<int>", "out_size_factor: int",
+            "score_threshold: float", "max_num: int", "pre_max_size: int", "post_max_size: int",
+            "nms_type: std::vector<int>", "nms_thr: std::vector<float>", "min_radius: std::vector<float>",
+            "nms_rescale_factor: std::vector<float>"})
+    .SetInferShapeFn(PD_INFER_SHAPE(BevdetPostProcessInferShape))
+    .SetInferDtypeFn(PD_INFER_DTYPE(PostProcessInferDtype));

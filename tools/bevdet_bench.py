@@ -3,6 +3,7 @@
 
   python tools/bevdet_bench.py [--steps K] [--warmup W] [--in-flight L] [--no-cpu-check] [--dump-outputs DIR]
   python tools/bevdet_bench.py --temporal [--steps K] [--warmup W] [--in-flight L] [--rounds R] [--no-cpu-check]
+  python tools/bevdet_bench.py --bevdet-nms [--temporal] [--steps K] [--warmup W] [--in-flight L] [--rounds R]
 
 A frame = six cameras of 16 x 44 features (D = 118, C = 80) -> LSS view transform into the 128 x 128 x 96 pixel fp16-pair
 image -> CustomResNet + FPN_LSS -> CenterHead (6 tasks) -> centerpoint postprocess -> one D2H.  Reports frames/s with
@@ -18,6 +19,12 @@ Reports frames/s in flight and one at a time for full frames and accelerate=True
 with the single-frame BEVDet on the same inputs (median of the rounds); the shift graph-timed with its algorithmic bytes
 and GB/s; pre_process and the encoder graph-timed with TFLOP/s; the node counts of the start and continue graphs; the
 card; and a frame-0 check against the CPU arm (bevdet4d_oracle.CpuBEVDet4D, test infrastructure under tests/).
+
+--bevdet-nms: the frames with BEVDet's own box decode (bevdet.CONFIG_BEVDET_NMS, with --temporal CONFIG_4D_BEVDET_NMS:
+top-K over class x cell, per-class scale-NMS / circle NMS) next to the same weights with the default decode
+(centerpoint_postprocess), measured in rounds that alternate the two on the same inputs (median of the rounds): frames/s
+in flight and one at a time, both decodes graph-timed on the same head planes in us, the node counts of both frame
+graphs, the boxes of frame 0 under each, and the card.
 """
 import argparse
 import json
@@ -57,11 +64,15 @@ def main():
     ap.add_argument("--dump-outputs", metavar="DIR", default=None,
                     help="write the boxes / scores / labels of frame 0 to DIR/*.npy")
     ap.add_argument("--temporal", action="store_true", help="BEVDet4D sequential frames, alternated with BEVDet")
-    ap.add_argument("--rounds", type=int, default=3, help="--temporal: alternating measurement rounds")
+    ap.add_argument("--rounds", type=int, default=3, help="--temporal / --bevdet-nms: alternating measurement rounds")
+    ap.add_argument("--bevdet-nms", action="store_true",
+                    help="BEVDet's own box decode (scale-NMS / circle NMS), alternated with the default decode")
     args = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("bevdet_bench.py needs a CUDA device (no CPU fallback exists)")
+    if args.bevdet_nms:
+        return bevdet_nms(args)
     if args.temporal:
         return temporal(args)
     from paddle3d_b200 import synth
@@ -283,6 +294,94 @@ def temporal(args):
                                     "paired_frac": paired / max(1, len(cpu["boxes"])), "cpu_oracle_s": s,
                                     "kind": "fp64-accumulating numpy + OpenMP oracle, not a tuned CPU implementation"}
     line["value"] = line["bevdet4d_full"]["fps_in_flight"]
+    print(json.dumps(line))
+
+
+def bevdet_nms(args):
+    import torch
+    from paddle3d_b200 import bevdet as bd
+    from paddle3d_b200 import synth
+    from paddle3d_b200.ops import bev_pool_v2 as bp
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    four = args.temporal
+    model_cls, hot_cls = (bd.BEVDet4D, bd.BEVDet4DHotPath) if four else (bd.BEVDet, bd.BEVDetHotPath)
+    cfgs = {"default_decode": bd.CONFIG_4D if four else bd.CONFIG,
+            "bevdet_nms": bd.CONFIG_4D_BEVDET_NMS if four else bd.CONFIG_BEVDET_NMS}
+    models = {}
+    for name, cfg in cfgs.items():  # one set of weights under both test configs
+        m = model_cls(cfg, device=dev)
+        if models:
+            first = models["default_decode"]
+            m.encoder, m.head = first.encoder, first.head
+            if four:
+                m.pre_process = first.pre_process
+        else:
+            m.init_weight(seed=args.seed, bn_gain=BN_GAIN)
+        models[name] = m
+    m0 = models["default_decode"]
+    rigs = [synth.camera_rig(s) for s in range(4)]
+    mats = [synth.lss_mats(r) for r in rigs]
+    poses = [np.broadcast_to(p, (1, m0.N, 4, 4)) for p in synth.ego_poses(2)]
+    prev = [bp.sensor2keyegos(r["sensor2ego"], poses[0], poses[1]) for r in rigs]
+    rng = np.random.default_rng(args.seed)
+    vt = m0.vt
+    logits = torch.from_numpy(rng.normal(0, 2, (m0.N, vt.D, vt.H, vt.W)).astype(np.float32)).to(dev)
+    tran = torch.from_numpy(rng.normal(0, 1, (m0.N, vt.out_channels, vt.H, vt.W)).astype(np.float32)).to(dev)
+    m0.calibrate_heatmap_bias(mats[0], logits, tran)
+    line = {"metric": "%s frames/s with BEVDet's own box decode (scale-NMS / circle NMS) next to the default decode, from "
+                      "the depth net's output" % ("BEVDet4D sequential" if four else "BEVDet"),
+            "unit": "frames/s", "gpu": gpu_identity(0), "steps": args.steps, "warmup": args.warmup}
+    lanes_n = max(1, args.in_flight)
+    runs = {}
+    for name, m in models.items():
+        lanes = [hot_cls(m, device=dev).capture(count_nodes=(i == 0)) for i in range(lanes_n)]
+        for ln in lanes:  # inputs written once: the timed frames replay on resident depth-net outputs
+            ln.logits.copy_(logits)
+            ln.tran_feat.copy_(tran)
+        runs[name] = lanes
+    torch.cuda.synchronize()
+    frames = {}
+
+    def launch(name, lane_i, lane):
+        k = frames.get((name, lane_i), 0)
+        frames[(name, lane_i)] = k + 1
+        r = (lane_i + k) % 4  # a new calibration every frame
+        if four:
+            lane.launch(mats[lane_i % 4], prev[lane_i % 4], new_sequence=k == 0)
+        else:
+            lane.launch(mats[r])
+
+    def one_at_a_time(name, lane):
+        launch(name, 0, lane)
+        lane.result()
+    rates = {n: {"fps_in_flight": [], "fps_one_at_a_time": []} for n in runs}
+    for name, lanes in runs.items():
+        for i in range(args.warmup):
+            launch(name, i % lanes_n, lanes[i % lanes_n])
+    torch.cuda.synchronize()
+    for _ in range(max(1, args.rounds)):  # alternate the decodes so that clocks and temperature drift hit both
+        for name, lanes in runs.items():
+            rates[name]["fps_in_flight"].append(
+                _rate(lambda i: launch(name, i % lanes_n, lanes[i % lanes_n]), torch.cuda.synchronize, args.steps))
+            rates[name]["fps_one_at_a_time"].append(
+                _rate(lambda i: one_at_a_time(name, lanes[0]), torch.cuda.synchronize, args.steps))
+    # both decodes graph-timed on the same head planes (frame 0)
+    st = torch.cuda.Stream(dev)
+    with torch.cuda.stream(st):
+        x = m0.encoder_input(mats[0], None, logits, tran) if four else m0.image(mats[0], logits, tran)
+        h = m0.dense(x)
+        st.synchronize()
+    for name, lanes in runs.items():
+        for ln in lanes:
+            ln.result()  # raises on an fp16-range overflow
+        m = models[name]
+        r = {k: float(np.median(v)) for k, v in rates[name].items()}
+        got = lanes[0].infer(mats[0], None, new_sequence=True) if four else lanes[0].infer(mats[0])
+        r.update(rounds=rates[name], lanes=lanes_n, graph_nodes=lanes[0].graph_nodes, boxes_frame0=int(len(got[0])),
+                 result_rows=m.result_rows(), decode_us=1e3 * graph_time_ms(lambda: m.postprocess(h), st, 50))
+        line[name] = r
+    line["value"] = line["bevdet_nms"]["fps_in_flight"]
     print(json.dumps(line))
 
 
