@@ -418,6 +418,12 @@ int p3d_lss_prepare(const p3d_lss_camera *cams, const float *bda, const float *a
  * D <= 382 and C <= 370 (P3D_ERR_UNSUPPORTED above). */
 int p3d_lss_depth_feat(const float *logits, const float *tran_feat, int BN, int D, int H, int W, int C, float *depth,
                        float *feat, p3d_stream_t stream);
+/* p3d_lss_depth_feat from the depth net's pixel H16 rows rows_h16 [BN, H, W, in_C] (channels [0, D) the logits, [D, D + C)
+ * the features; each value merged as hi + lo' 2^-11): writes what p3d_lss_depth_feat writes for those merged values,
+ * bit for bit (same softmax operations in the same order).  in_C % 32 == 0, D + C <= in_C, rows_h16 16-byte aligned
+ * (P3D_ERR_INVALID_ARG otherwise); D <= 370, BN <= 65535, BN * H * W * 4 * in_C bytes < 2^31 (P3D_ERR_UNSUPPORTED above). */
+int p3d_lss_depth_feat_h16(const void *rows_h16, int BN, int H, int W, int in_C, int D, int C, float *depth, float *feat,
+                           p3d_stream_t stream);
 /* bev_pool_v2 with the interval count on the device (counts_dev[1], as p3d_bev_pool_prepare / p3d_lss_prepare write it;
  * capacity = length of the rank arrays), so that it can be captured once for every calibration.  Bit-identical to
  * p3d_bev_pool_v2 (same kernel).  out is zero-filled here: planar 0 -> [B, Z, Y, X, c], planar 1 -> [B, Z * c, Y, X]
@@ -475,6 +481,24 @@ int p3d_dense_conv2d_f16_residual(const void *in_h16, int B, int H, int W, int C
  * out_c0 + C <= out_C, 16-byte aligned images (P3D_ERR_INVALID_ARG otherwise). */
 int p3d_upsample_bilinear_h16(const void *in_h16, int B, int h, int w, int C, int scale, void *out_h16, int out_C, int out_c0,
                               int32_t *status_dev, p3d_stream_t stream);
+/* Nearest upsampling (F.interpolate(mode='nearest') to scale x the size, source pixel = output pixel / scale) of pixel
+ * H16 rows in_h16 [B, h, w, C] into channels [out_c0, out_c0 + C) of out_h16 [B, scale h, scale w, out_C]: the pairs are
+ * copied (exact, no status).  CustomFPN's top-down step writes it as the residual rows of the lateral conv.  Argument
+ * contract of p3d_upsample_bilinear_h16 (P3D_ERR_INVALID_ARG otherwise). */
+int p3d_upsample_nearest_h16(const void *in_h16, int B, int h, int w, int C, int scale, void *out_h16, int out_C, int out_c0,
+                             p3d_stream_t stream);
+/* ResNet stem (mmdet ResNet, style 'pytorch'): MaxPool2d(3, 2, 1)(ReLU(conv7x7(in, stride 2, pad 3) * scale[c] +
+ * shift[c])) of fp32 NCHW images in [B, 3, H, W], 3 -> 64 channels, into pixel H16 rows out_h16 [B, pH, pW, 64] with
+ * cH = (H - 1) / 2 + 1, pH = (cH - 1) / 2 + 1 (the same for W).  Conv on warp MMA with both operands as fp16 pairs
+ * (hi.hi + hi.lo' + lo'.hi, fp32 accumulation), BatchNorm (eval) folded into scale / shift [64] by the caller; the pool
+ * takes the max in fp32 and the result is split once.  Status bit 0: an input, weight or output left fp16's range.
+ * packed_weight: p3d_resnet_stem_packed_weight_bytes() bytes written by p3d_resnet_stem_pack_weights from W [64][3][7][7]
+ * fp32 (paddle.nn.Conv2D layout).  Null pointers, B, H, W < 1, packed_weight / out_h16 not 16-byte aligned:
+ * P3D_ERR_INVALID_ARG; B > 65535 or B * 3 * H * W >= 2^31: P3D_ERR_UNSUPPORTED. */
+size_t p3d_resnet_stem_packed_weight_bytes(void);
+int p3d_resnet_stem_pack_weights(const float *weight, void *packed, int32_t *status_dev, p3d_stream_t stream);
+int p3d_resnet_stem_h16(const float *in, int B, int H, int W, const void *packed_weight, const float *scale, const float *shift,
+                        void *out_h16, int32_t *status_dev, p3d_stream_t stream);
 /* p3d_bev_pool_v2_dev into pixel H16 rows: out_h16 [B, Y, X, out_C] with channel z * c + ch of cell (y, x) (the layout of
  * the planar output, one pixel per row), same accumulation, then split into (hi, lo'); status bit 0 on fp16 overflow.
  * out_h16 is zero-filled here (empty cells and channels >= Z * c).  out_C % 32 == 0 and out_C >= Z * c

@@ -97,6 +97,11 @@ SIGNATURES = {
     "p3d_dense_conv2d_f16_residual": (_int, [_vp, _int, _int, _int, _int, _vp, _int, _int, _int, _int, _int, _int, _int, _vp,
                                              _vp, _int, _vp, _int, _int, _vp, _vp, _int, _int, _int, _vp, _vp]),
     "p3d_upsample_bilinear_h16": (_int, [_vp, _int, _int, _int, _int, _int, _vp, _int, _int, _vp, _vp]),
+    "p3d_upsample_nearest_h16": (_int, [_vp, _int, _int, _int, _int, _int, _vp, _int, _int, _vp]),
+    "p3d_resnet_stem_packed_weight_bytes": (_sz, []),
+    "p3d_resnet_stem_pack_weights": (_int, [_vp, _vp, _vp, _vp]),
+    "p3d_resnet_stem_h16": (_int, [_vp, _int, _int, _int, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "p3d_lss_depth_feat_h16": (_int, [_vp, _int, _int, _int, _int, _int, _int, _vp, _vp, _vp]),
     "p3d_bev_pool_v2_dev_h16": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _int, _int, _int, _int, _int, _vp, _int,
                                        _vp, _vp]),
     "p3d_bev_shift_h16": (_int, [_vp, _int, _int, _int, _int, _int, _vp, _vp, _int, _int, _vp, _vp]),

@@ -11,7 +11,11 @@ BEVDetHotPath captures all of it, from the descriptor upload to the D2H copy of 
 decode runs follows from the model's test config, as in the reference's configs: one without nms_type (CONFIG) runs the
 custom op Paddle3D's predict_by_custom_op calls (arg-max class per cell, one rotated NMS threshold, 83 boxes per task,
 gravity centre); one with nms_type (CONFIG_BEVDET_NMS) runs BEVDet's own get_bboxes (ops.bevdet_postprocess: top-K over
-class x cell, per-class scale-NMS or circle NMS, bottom centre, up to post_max_size boxes per task)."""
+class x cell, per-class scale-NMS or circle NMS, bottom centre, up to post_max_size boxes per task).
+
+BEVDetFromImages / BEVDetImageHotPath (CONFIG_IMG) put BEVDet's image half in front of it: six normalised camera images ->
+ResNet-50 (p3d_resnet_stem_h16, then Bottlenecks on the dense fp16-pair conv) -> CustomFPN -> depth net ->
+p3d_lss_depth_feat_h16 -> the frame above, one captured graph."""
 import numpy as np
 import torch
 
@@ -302,6 +306,286 @@ class BEVDetHotPath(ResultSlotOwner, CameraFrame):
         """Raise when an activation left fp16's range on the fp16-pair path (never a silent wrong result)."""
         if int(status_host[0]):
             raise RuntimeError("BEVDet: an activation left fp16's range (|x| >= 65504) on the fp16-pair path")
+
+
+# ------------------------------------------------------------------------------------------------ BEVDet from images
+# PARITY UNPINNED, as CONFIG: BEVDet-R50's image half, recalled from bevdet-r50 (not checked against it or Paddle3D's
+# configs/bevdet): img_backbone = mmdet ResNet(depth=50, num_stages=4, out_indices=(2, 3), style='pytorch') with BN (eval,
+# eps 1e-5); img_neck = CustomFPN(in_channels=[1024, 2048], out_channels=512, num_outs=1, start_level=0, out_ids=[0]);
+# the view transformer's depth_net = Conv2d(512, D + C, 1).  Stages: (planes, blocks, stride).
+IMG_BACKBONE = dict(depth=50, stages=((64, 3, 1), (128, 4, 2), (256, 6, 2), (512, 3, 2)), out_indices=(2, 3), bn_eps=1e-5)
+IMG_NECK = dict(in_channels=(1024, 2048), out_channels=512)
+DEPTH_NET = dict(in_channels=512)
+CONFIG_IMG = dict(CONFIG, img_backbone=IMG_BACKBONE, img_neck=IMG_NECK, depth_net=DEPTH_NET)
+CONFIG_IMG_BEVDET_NMS = dict(CONFIG_IMG, test=TEST_CFG_BEVDET)
+
+
+def round16(c):
+    return (int(c) + 15) // 16 * 16
+
+
+class BEVDetImageEncoder:
+    """BEVDet's image encoder on pixel fp16-pair rows: ResNet-50 (stem: p3d_resnet_stem_h16, conv 7x7 s2 + BN + ReLU +
+    MaxPool 3x3 s2 in one kernel; Bottlenecks relu(bn3(conv3(relu(bn2(conv2(relu(bn1(conv1(x))))))) + identity), the
+    stride on the 3x3 conv, a 1x1 stride-s conv + BN as the identity of each stage's first block, the add in conv3's
+    epilogue), CustomFPN on stages 2 and 3 (1x1 lateral convs with bias; lateral1 nearest-upsampled x2 into the residual
+    rows of lateral0's conv, so the top-down add happens in its epilogue; a 3x3 conv with bias) and the depth net (1x1
+    conv 512 -> D + C with bias, computed as round16(D + C) channels into round32 rows, the extra ones zero).
+
+    Seeded weights (init_weight) stay inside fp16's range: _Conv's uniform init scales a signal's mean square by ~1/3
+    and ReLU halves it, so the BN gains are sqrt(6) after a ReLU-ed conv (STEM_GAIN, MID_GAIN), sqrt(3) on the downsample
+    identity (DOWN_GAIN), and RES_GAIN on each Bottleneck's last BN (zero_init_residual in spirit: the residual stream of
+    the 16 blocks grows slowly).  Per-stage max |x| of the seeded model (seed 0) on synth.camera_images at 256 x 704, six
+    cameras (fp64): stem 12.5, layer1 12.9, layer2 11.4, layer3 7.6, layer4 6.2, CustomFPN 1.6, depth net 1.1."""
+
+    STEM_GAIN = MID_GAIN = 6.0 ** 0.5
+    DOWN_GAIN = 3.0 ** 0.5
+    RES_GAIN = 0.5
+
+    def __init__(self, backbone, neck, depth_net, D, C):
+        eps = backbone["bn_eps"]
+        self.D, self.C = int(D), int(C)
+        self.stem = _Conv(3, 64, 7, 2, 3, bn_eps=eps)  # runs on p3d_resnet_stem_h16, not the dense conv
+        self.stages, cin = [], 64
+        for planes, blocks, stride in backbone["stages"]:
+            stage = []
+            for bi in range(blocks):
+                s = stride if bi == 0 else 1
+                stage.append(dict(conv1=_Conv(cin, planes, 1, 1, 0, bn_eps=eps),
+                                  conv2=_Conv(planes, planes, 3, s, 1, bn_eps=eps),
+                                  conv3=_Conv(planes, 4 * planes, 1, 1, 0, bn_eps=eps),  # ReLU after the residual
+                                  down=_Conv(cin, 4 * planes, 1, s, 0, bn_eps=eps, relu=False) if bi == 0 else None))
+                cin = 4 * planes
+            self.stages.append(stage)
+        self.out_indices = tuple(backbone["out_indices"])
+        c0, c1 = neck["in_channels"]
+        if (c0, c1) != tuple(4 * self.stages[i][0]["conv1"].cout for i in self.out_indices):
+            raise ValueError("CustomFPN in_channels %s do not match the ResNet's stages %s" % ((c0, c1), self.out_indices))
+        oc = neck["out_channels"]
+        self.lateral = [_Conv(c0, oc, 1, 1, 0, bias=True, relu=False), _Conv(c1, oc, 1, 1, 0, bias=True, relu=False)]
+        self.fpn_conv = _Conv(oc, oc, 3, 1, 1, bias=True, relu=False)
+        if depth_net["in_channels"] != oc:
+            raise ValueError("depth_net in_channels %d, the neck gives %d" % (depth_net["in_channels"], oc))
+        self.out_C = round32(self.D + self.C)  # the depth net's rows
+        self.depth_net = _Conv(oc, self.D + self.C, 1, 1, 0, bias=True, relu=False, cout_pad=round16(self.D + self.C))
+        self.stem_dev = None
+
+    def convs(self):
+        """Every conv in parameter order (the stem first)."""
+        out = [self.stem]
+        for stage in self.stages:
+            for blk in stage:
+                out += [blk["conv1"], blk["conv2"], blk["conv3"]] + ([blk["down"]] if blk["down"] is not None else [])
+        return out + self.lateral + [self.fpn_conv, self.depth_net]
+
+    def init_weight(self, seed=0, device=None):
+        """Seeded parameters (numpy; with a device also the packed device images).  Gains: see the class docstring."""
+        rng = np.random.default_rng([seed, 6])
+        self.stem.init(rng, None, bn_gain=self.STEM_GAIN)
+        for stage in self.stages:
+            for blk in stage:
+                blk["conv1"].init(rng, device, bn_gain=self.MID_GAIN)
+                blk["conv2"].init(rng, device, bn_gain=self.MID_GAIN)
+                blk["conv3"].init(rng, device, bn_gain=self.RES_GAIN)
+                if blk["down"] is not None:
+                    blk["down"].init(rng, device, bn_gain=self.DOWN_GAIN)
+        for c in self.lateral + [self.fpn_conv, self.depth_net]:
+            c.init(rng, device)
+        if device is not None:
+            p = self.stem.np
+            bn = p["bn"]
+            sc = bn["gamma"].astype(np.float64) / np.sqrt(bn["var"].astype(np.float64) + bn["eps"])
+            sh = -bn["mean"].astype(np.float64) * sc + bn["beta"]
+            self.stem_dev = dict(packed=dc.pack_stem_weight(torch.from_numpy(p["weight"]).to(device)),
+                                 scale=torch.from_numpy(sc.astype(np.float32)).to(device),
+                                 shift=torch.from_numpy(sh.astype(np.float32)).to(device))
+        return self
+
+    def export_numpy(self):
+        return dict(stem=self.stem.np,
+                    stages=[[{k: (c.np if c is not None else None) for k, c in blk.items()} for blk in stage]
+                            for stage in self.stages],
+                    out_indices=self.out_indices, lateral=[c.np for c in self.lateral], fpn_conv=self.fpn_conv.np,
+                    depth_net=self.depth_net.np, D=self.D, C=self.C)
+
+    # ---- device stages (pixel fp16-pair rows in and out)
+    def stem_forward(self, imgs):
+        d = self.stem_dev
+        return dc.resnet_stem_h16(imgs, d["packed"], d["scale"], d["shift"])
+
+    @staticmethod
+    def bottleneck(blk, x, shape):
+        """One Bottleneck: (rows, (B, oH, oW, 4 planes))."""
+        b = shape[0]
+        t, _, _ = blk["conv1"](x, shape)
+        t, _, (_, oh, ow) = blk["conv2"](t, (b, shape[1], shape[2], blk["conv1"].cout))
+        c3 = blk["conv3"]
+        idn = x if blk["down"] is None else blk["down"](x, shape)[0]
+        y, _, _ = c3(t, (b, oh, ow, blk["conv2"].cout), residual=idn, res_channels=c3.cout)
+        return y, (b, oh, ow, c3.cout)
+
+    def stage_forward(self, si, x, shape):
+        for blk in self.stages[si]:
+            x, shape = self.bottleneck(blk, x, shape)
+        return x, shape
+
+    def backbone(self, imgs):
+        """The pixel rows of every stage's output after the stem, [(rows, (B, H, W, C))]."""
+        x, shape = self.stem_forward(imgs)
+        feats = []
+        for si in range(len(self.stages)):
+            x, shape = self.stage_forward(si, x, shape)
+            feats.append((x, shape))
+        return feats
+
+    def neck(self, feats):
+        """CustomFPN: (rows, shape) of its 512-channel output."""
+        (x0, s0), (x1, s1) = feats[self.out_indices[0]], feats[self.out_indices[1]]
+        l0c, l1c = self.lateral
+        oc = l0c.cout
+        l1, _, _ = l1c(x1, s1)
+        up, (b, h, w) = dc.upsample_nearest_h16(l1, (s1[0], s1[1], s1[2], oc), s0[1] // s1[1])
+        if (h, w) != tuple(s0[1:3]):
+            raise ValueError("CustomFPN: lateral1 %s does not upsample to lateral0 %s" % ((h, w), tuple(s0[1:3])))
+        l0, _, _ = l0c(x0, s0, residual=up, res_channels=oc)
+        y, _, _ = self.fpn_conv(l0, (b, h, w, oc))
+        return y, (b, h, w, oc)
+
+    def head(self, y, shape):
+        """The depth net: rows [B*H*W, 2*out_C] (channels [0, D) logits, [D, D + C) tran_feat, the rest zero)."""
+        b, h, w, _ = shape
+        out = torch.zeros((b * h * w, 2 * self.out_C), dtype=torch.float16, device=y.device) \
+            if self.out_C > self.depth_net.cout_pad else None
+        d, _, _ = self.depth_net(y, shape, out_h16=out, out_channels=self.out_C)
+        return d, (b, h, w, self.out_C)
+
+    def __call__(self, imgs):
+        """imgs [N, 3, H, W] fp32 (normalised) -> the depth net's pixel rows and their shape (N, H / 16, W / 16, out_C)."""
+        return self.head(*self.neck(self.backbone(imgs)))
+
+    def flops(self, H, W, n):
+        """Algorithmic flops (2 x MACs) of n images at H x W: stem, layers, neck, depth net (D + C outputs, unpadded)."""
+        ch, cw = (H - 1) // 2 + 1, (W - 1) // 2 + 1
+        out = dict(img_stem=2.0 * n * ch * cw * 3 * 49 * 64)
+        h, w = dc.stem_shape(H, W)
+        layers, sizes = 0.0, []
+        for stage in self.stages:
+            for blk in stage:
+                s = blk["conv2"].stride
+                oh, ow = (h - 1) // s + 1, (w - 1) // s + 1
+                layers += 2.0 * n * (h * w * blk["conv1"].cin * blk["conv1"].cout
+                                     + oh * ow * 9 * blk["conv2"].cin * blk["conv2"].cout
+                                     + oh * ow * blk["conv3"].cin * blk["conv3"].cout)
+                if blk["down"] is not None:
+                    layers += 2.0 * n * oh * ow * blk["down"].cin * blk["down"].cout
+                h, w = oh, ow
+            sizes.append((h, w))
+        out["img_layers"] = layers
+        out["img_backbone"] = out["img_stem"] + layers
+        (h0, w0), (h1, w1) = sizes[self.out_indices[0]], sizes[self.out_indices[1]]
+        l0, l1, f = self.lateral[0], self.lateral[1], self.fpn_conv
+        out["img_neck"] = 2.0 * n * (h0 * w0 * l0.cin * l0.cout + h1 * w1 * l1.cin * l1.cout + h0 * w0 * 9 * f.cin * f.cout)
+        out["depth_net"] = 2.0 * n * h0 * w0 * self.depth_net.cin * self.depth_net.cout
+        return out
+
+
+class BEVDetFromImages(BEVDet):
+    """BEVDet (CONFIG_IMG) from six normalised camera images: BEVDetImageEncoder, p3d_lss_depth_feat_h16 on its rows, then
+    BEVDet's view transform, encoder, head and postprocess.  Batch 1.  input_size must be a multiple of 32 (so that the
+    ResNet's stride-16 stage is input_size // 16 and CustomFPN's x2 upsampling is exact)."""
+
+    def __init__(self, model_cfg=None, accelerate=False, device="cuda"):
+        mc = model_cfg or CONFIG_IMG
+        H_in, W_in = mc["input_size"]
+        if H_in % 32 or W_in % 32:
+            raise ValueError("BEVDetFromImages: input_size %s is not a multiple of 32" % (tuple(mc["input_size"]),))
+        if mc["downsample"] != 16:
+            raise ValueError("BEVDetFromImages: the depth net runs on the ResNet's stride-16 stage (downsample 16), got %r"
+                             % mc["downsample"])
+        super().__init__(mc, accelerate, device)
+        self.input_size = (int(H_in), int(W_in))
+        self.image_encoder = BEVDetImageEncoder(mc["img_backbone"], mc["img_neck"], mc["depth_net"], self.vt.D,
+                                                mc["channels"])
+
+    def init_weight(self, seed=0, bn_gain=1.0, device=None):
+        super().init_weight(seed=seed, bn_gain=bn_gain, device=device)
+        self.image_encoder.init_weight(seed, device=None if device is False else (device or self.device))
+        return self
+
+    def export_numpy(self):
+        return dict(super().export_numpy(), image_encoder=self.image_encoder.export_numpy())
+
+    def stage_shapes(self):
+        """(C, H, W) of the stem and of every ResNet stage's output, then of the depth net's rows."""
+        H, W = self.input_size
+        h, w = dc.stem_shape(H, W)
+        out = [(64, h, w)]
+        for stage in self.image_encoder.stages:
+            s = stage[0]["conv2"].stride
+            h, w = (h - 1) // s + 1, (w - 1) // s + 1
+            out.append((stage[0]["conv3"].cout, h, w))
+        return out + [(self.image_encoder.out_C, self.vt.H, self.vt.W)]
+
+    def depth_feat(self, rows, shape, depth=None, feat=None):
+        return bp.lss_depth_feat_h16(rows, shape, self.vt.D, self.vt.out_channels, depth, feat)
+
+    def image_from_images(self, mats, imgs):
+        """Eager image encoder + view transform into the pool image."""
+        prepared = self.vt.ranks(mats, 1, self.N)
+        depth, feat = self.depth_feat(*self.image_encoder(imgs))
+        return self.pool(depth, feat, prepared)
+
+    def forward_images(self, mats, imgs):
+        """Eager frame from imgs [N, 3, H, W] fp32 on the device: (boxes, scores, labels, counts) as BEVDet.forward."""
+        return self.postprocess(self.dense(self.image_from_images(mats, imgs)))
+
+    def calibrate_heatmap_bias(self, mats, imgs, target_frac=0.014):
+        """BEVDet.calibrate_heatmap_bias on the frame of these images."""
+        img = self.image_from_images(mats, imgs)
+        self.head.calibrate_heatmap_bias(img, self.test_cfg["score_threshold"], target_frac, shape=self.enc_shape)
+        return self
+
+    def flops(self):
+        """BEVDet.flops (BEV side, its keys unchanged) plus img_backbone (img_stem + img_layers), img_neck, depth_net and
+        img_total; frame_total = total + img_total."""
+        out = super().flops()
+        img = self.image_encoder.flops(self.input_size[0], self.input_size[1], self.N)
+        img["img_total"] = img["img_backbone"] + img["img_neck"] + img["depth_net"]
+        out.update(img)
+        out["frame_total"] = out["total"] + img["img_total"]
+        return out
+
+
+class BEVDetImageHotPath(BEVDetHotPath):
+    """BEVDetHotPath from camera images: one captured CUDA graph from the camera descriptor to the D2H of the boxes, the
+    frame being image encoder -> p3d_lss_depth_feat_h16 into the frame's depth / feat -> memset + pool -> encoder -> head
+    -> postprocess.  launch(mats, imgs) copies imgs [N, 3, H, W] (a device tensor) into the lane's input buffer on its
+    stream first, as CameraFrame.launch copies logits.  Lanes, share_model and accelerate as in BEVDetHotPath."""
+
+    def __init__(self, model, device="cuda", stream=None):
+        super().__init__(model, device, stream)
+        H, W = model.input_size
+        self.imgs = torch.zeros((model.N, 3, H, W), dtype=torch.float32, device=self.device)
+
+    def _frame(self):
+        m = self.model
+        rows, shape = m.image_encoder(self.imgs)
+        m.depth_feat(rows, shape, self.depth, self.feat)
+        m.pool(self.depth, self.feat, self.prepared, out=self.image)
+        return self._dense(self.image)
+
+    def launch(self, mats, imgs=None):
+        """Enqueue one frame: mats = (sensor2ego, cam2imgs, post_rots, post_trans, bda) on the host; imgs: a device tensor
+        copied into the frame's input (None: already written there)."""
+        if imgs is not None:
+            self.stream.wait_stream(torch.cuda.current_stream(self.device))
+            with torch.cuda.stream(self.stream):  # after the lane's previous frame, which read the buffer
+                self.imgs.copy_(imgs, non_blocking=True)
+        self._launch(mats, None, None, "frame")
+
+    def infer(self, mats, imgs=None):
+        self.launch(mats, imgs)
+        return self.result()
 
 
 # ---------------------------------------------------------------------------------------------------------- BEVDet4D

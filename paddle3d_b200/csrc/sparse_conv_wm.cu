@@ -29,9 +29,12 @@
 
 #include "common.cuh"
 #include "h16.cuh"
+#include "tc_common.cuh"
 
 namespace p3d {
 namespace wm {
+
+using tc::mma16816;
 
 constexpr int kWarps = 16;  // warps per CTA of every instantiation, one CTA per SM
 
@@ -51,12 +54,6 @@ struct Params {
   float *slabs;              // stream-K partial tiles [warps of the grid][2][COUT / 2][32 lanes]
   int32_t *tickets;          // [tiles] arrival counters of split tiles, zero on entry, left zero
 };
-
-__device__ __forceinline__ void mma16816(float (&c)[4], const uint4 &a, uint32_t b0, uint32_t b1) {
-  asm("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
-      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-      : "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w), "r"(b0), "r"(b1));
-}
 
 // B-fragment words of one (tile, tap) unit for the two rows (g, g + 8) a lane serves: [row][half: hi, lo'][CIN / 8 words];
 // words 2s, 2s + 1 are (b0, b1) of k-step s

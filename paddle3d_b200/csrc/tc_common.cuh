@@ -1,5 +1,5 @@
 // PTX helpers shared by the tensor-core kernels (sm_90a): mbarrier, cp.async(.bulk), wgmma descriptors / fences,
-// the m64nN accumulator fragment, tf32 hi/lo split.
+// the m64nN accumulator fragment, the warp mma.sync m16n8k16, tf32 hi/lo split.
 #pragma once
 #include <stdlib.h>
 
@@ -96,6 +96,14 @@ __device__ __forceinline__ uint64_t desc_sw64(uint32_t addr) { return gmma_desc(
 // Position of accumulator element i of an m64nN fragment inside the warpgroup's 64 x N block (wgmma.cuh).
 __device__ __forceinline__ int frag_row(int i, int wg_tid) { return ((wg_tid >> 5) << 4) + ((wg_tid & 31) >> 2) + (((i >> 1) & 1) << 3); }
 __device__ __forceinline__ int frag_col(int i, int wg_tid) { return ((i >> 2) << 3) + ((wg_tid & 3) << 1) + (i & 1); }
+
+// warp MMA D = A B + D, m16n8k16, fp16 inputs, fp32 accumulators: a = the row-major A fragment (a0a1, a2a3, a4a5, a6a7),
+// (b0, b1) the column-major B fragment
+__device__ __forceinline__ void mma16816(float (&c)[4], const uint4 &a, uint32_t b0, uint32_t b1) {
+  asm("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+      : "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w), "r"(b0), "r"(b1));
+}
 
 __device__ __forceinline__ void split_tf32(float x, float &hi, float &lo) {
   uint32_t h;

@@ -6,6 +6,7 @@
 // four source pixels are merged to fp32, interpolated in Paddle's expression with every product and sum rounded on its
 // own (__fmul_rn / __fadd_rn: no FMA contraction, so a numpy fp32 restatement matches bit for bit) and split again.
 // Scale 1 copies the pairs (FPN_LSS places x0 into the concat with it).  HBM-bound: 4 C h w + 4 C H W bytes.
+// Nearest upsampling (CustomFPN's top-down step) copies the pairs of the source pixel, with the same output contract.
 #include <cuda_fp16.h>
 
 #include "common.cuh"
@@ -71,6 +72,27 @@ __global__ void __launch_bounds__(256) upsample_bilinear_h16_kernel(const UpPara
   if (ovf && p.status) atomicOr(p.status, 1);
 }
 
+// Nearest upsampling by an integer factor (F.interpolate(mode='nearest') to s x the size: source index = dst / s), the
+// top-down step of CustomFPN: one thread per (output pixel, 8 channels) copies the 16 bytes of hi and of lo' (exact).
+__global__ void __launch_bounds__(256) upsample_nearest_h16_kernel(const UpParams p) {
+  const int qn = p.C / 8;
+  const long long total = static_cast<long long>(p.B) * p.H * p.W * qn;
+  const long long t = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (t >= total) return;
+  const int q = static_cast<int>(t % qn);
+  long long r = t / qn;
+  const int X = static_cast<int>(r % p.W);
+  r /= p.W;
+  const int Y = static_cast<int>(r % p.H);
+  const int b = static_cast<int>(r / p.H);
+  const size_t in_row = 4 * static_cast<size_t>(p.C), out_row = 4 * static_cast<size_t>(p.out_C);
+  const int oc = p.out_c0 + 8 * q;
+  uint8_t *o = p.out + ((static_cast<size_t>(b) * p.H + Y) * p.W + X) * out_row + (oc >> 5) * 128 + (oc & 31) * 2;
+  const uint8_t *g = p.in + ((static_cast<size_t>(b) * p.h + Y / p.s) * p.w + X / p.s) * in_row + (q >> 2) * 128 + (q & 3) * 16;
+  *reinterpret_cast<uint4 *>(o) = __ldg(reinterpret_cast<const uint4 *>(g));
+  *reinterpret_cast<uint4 *>(o + 64) = __ldg(reinterpret_cast<const uint4 *>(g + 64));
+}
+
 }  // namespace
 }  // namespace p3d
 
@@ -99,6 +121,29 @@ extern "C" int p3d_upsample_bilinear_h16(const void *in_h16, int B, int h, int w
   p.status = status_dev;
   const long long total = static_cast<long long>(B) * p.H * p.W * (C / 8);
   upsample_bilinear_h16_kernel<<<div_up(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  P3D_LAUNCH_CHECK();
+  return P3D_OK;
+}
+
+extern "C" int p3d_upsample_nearest_h16(const void *in_h16, int B, int h, int w, int C, int scale, void *out_h16, int out_C,
+                                        int out_c0, p3d_stream_t stream) {
+  if (!in_h16 || !out_h16 || B < 1 || h < 1 || w < 1 || scale < 1 || C < 32 || C % 32 || out_c0 < 0 || out_c0 % 16 ||
+      out_C % 32 || out_c0 + C > out_C || (reinterpret_cast<uintptr_t>(in_h16) & 15) || (reinterpret_cast<uintptr_t>(out_h16) & 15))
+    return P3D_ERR_INVALID_ARG;
+  UpParams p = {};
+  p.in = static_cast<const uint8_t *>(in_h16);
+  p.out = static_cast<uint8_t *>(out_h16);
+  p.B = B;
+  p.h = h;
+  p.w = w;
+  p.C = C;
+  p.H = h * scale;
+  p.W = w * scale;
+  p.out_C = out_C;
+  p.out_c0 = out_c0;
+  p.s = scale;
+  const long long total = static_cast<long long>(B) * p.H * p.W * (C / 8);
+  upsample_nearest_h16_kernel<<<div_up(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(p);
   P3D_LAUNCH_CHECK();
   return P3D_OK;
 }

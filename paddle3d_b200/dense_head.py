@@ -19,12 +19,14 @@ class _Conv:
     """Conv2D / Conv2DTranspose (+ BatchNorm2D eval) (+ ReLU) with seeded parameters."""
 
     def __init__(self, cin, cout, k, stride=1, padding=0, bias=False, bn_eps=None, relu=True, up=1, f16=True, transposed=False,
-                 cin_pad=None):
+                 cin_pad=None, cout_pad=None):
         """transposed: a stride-1 Conv2DTranspose (weight [Cin, Cout, k, k]); with k = 1 it runs as a 1x1 conv whose packed
         weight is the transpose (up > 1 implies a transposed conv).  cin_pad: the packed weight is zero-padded on Cin to
-        this many channels (an input image whose rows carry zero padding channels); the exported weight keeps cin."""
+        this many channels (an input image whose rows carry zero padding channels); the exported weight keeps cin.
+        cout_pad: the device conv computes this many output channels, the ones past cout with zero weights, bias and
+        shift (an fp16-pair output needs Cout % 16 == 0); the exported parameters keep cout."""
         self.cin, self.cout, self.k, self.stride, self.padding, self.up = cin, cout, k, stride, padding, up
-        self.cin_pad = cin_pad
+        self.cin_pad, self.cout_pad = cin_pad, cout_pad
         self.transposed = transposed or up > 1
         self.has_bias, self.bn_eps, self.relu = bias, bn_eps, relu
         self.f16 = f16 and cout >= 16  # the 1-3 channel output convs of the heads run on the CUDA cores (forward)
@@ -72,6 +74,13 @@ class _Conv:
             ax = 0 if self.transposed else 1
             wd = np.zeros(shape[:ax] + (self.cin_pad,) + shape[ax + 1:], np.float32)
             wd[(slice(None),) * ax + (slice(0, cin),)] = w
+        if self.cout_pad and self.cout_pad > cout:
+            if self.transposed:
+                raise ValueError("cout_pad: Conv2D weights only")
+            wp = np.zeros((self.cout_pad,) + wd.shape[1:], np.float32)
+            wp[:cout] = wd
+            wd = wp
+            s, t = np.concatenate([s, np.ones(self.cout_pad - cout)]), np.concatenate([t, np.zeros(self.cout_pad - cout)])
         self.dev = dict(
             packed=pack(torch.from_numpy(wd).to(device), self.n_tile),
             scale=torch.from_numpy(s.astype(np.float32)).to(device) if p["bn"] is not None else None,
@@ -83,8 +92,8 @@ class _Conv:
         if self.f16:
             if "out_split" in kw:
                 kw["out_h16"] = kw.pop("out_split")
-            return dc.dense_conv2d_f16(x_split, shape, d["packed"], self.cout, self.n_tile, self.k, self.stride, self.padding,
-                                       self.up, d["scale"], d["shift"], self.relu, **kw)
+            return dc.dense_conv2d_f16(x_split, shape, d["packed"], self.cout_pad or self.cout, self.n_tile, self.k, self.stride,
+                                       self.padding, self.up, d["scale"], d["shift"], self.relu, **kw)
         return dc.dense_conv2d(x_split, shape, d["packed"], self.cout, self.n_tile, self.k, self.stride, self.padding, self.up,
                                d["scale"], d["shift"], self.relu, **kw)
 

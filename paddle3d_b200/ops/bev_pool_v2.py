@@ -190,6 +190,21 @@ def lss_depth_feat(logits, tran_feat, depth=None, feat=None):
     return depth, feat
 
 
+def lss_depth_feat_h16(rows, shape, D, C, depth=None, feat=None):
+    """lss_depth_feat from the depth net's pixel H16 rows [BN*H*W, 2*in_C], shape = (BN, H, W, in_C): channels [0, D) are
+    the logits, [D, D + C) the features (p3d_lss_depth_feat_h16) -> (depth [BN, D, H, W], feat [BN, H, W, C]); depth /
+    feat: optional preallocated outputs."""
+    rows = require_cuda(rows, "rows", torch.float16)
+    BN, H, W, in_C = [int(v) for v in shape]
+    if tuple(rows.shape) != (BN * H * W, 2 * in_C):
+        raise ValueError("lss_depth_feat_h16: rows %s, want (%d, %d)" % (tuple(rows.shape), BN * H * W, 2 * in_C))
+    depth = torch.empty((BN, D, H, W), dtype=torch.float32, device=rows.device) if depth is None else depth
+    feat = torch.empty((BN, H, W, C), dtype=torch.float32, device=rows.device) if feat is None else feat
+    check(lib().p3d_lss_depth_feat_h16(ptr(rows), BN, H, W, in_C, int(D), int(C), ptr(depth), ptr(feat), stream(rows.device)),
+          "lss_depth_feat_h16")
+    return depth, feat
+
+
 def bev_pool_v2_dev(depth, feat, prepared, bev_feat_shape, planar=False, out=None):
     """bev_pool_v2 with the interval count read on the device (p3d_bev_pool_v2_dev): `prepared` as voxel_pooling_prepare_v2
     / lss_prepare return it (untrimmed); bev_feat_shape (B, Z, Y, X, C).  planar=False -> [B, Z, Y, X, C];

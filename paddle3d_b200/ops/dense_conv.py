@@ -201,3 +201,52 @@ def upsample_bilinear_h16(x_h16, shape, scale, out_h16=None, out_channels=None, 
     check(lib().p3d_upsample_bilinear_h16(ptr(x_h16), b, h, w, c, s, ptr(out_h16), oc, int(out_c0), ptr(_status(dev)),
                                           stream(dev)), "upsample_bilinear_h16")
     return out_h16, (b, h * s, w * s)
+
+
+def upsample_nearest_h16(x_h16, shape, scale, out_h16=None, out_channels=None, out_c0=0):
+    """F.interpolate(mode='nearest') to scale x the size on pixel H16 rows x_h16 [B*h*w, 2*C], shape = (B, h, w, C)
+    (p3d_upsample_nearest_h16: the pairs are copied).  Writes channels [out_c0, out_c0 + C) of out_h16 [B*sh*sw,
+    2*out_channels] (None: a new C-channel image).  Returns (out_h16, (B, s h, s w))."""
+    x_h16 = require_cuda(x_h16, "x_h16", torch.float16)
+    b, h, w, c = [int(v) for v in shape]
+    s = int(scale)
+    oc = int(out_channels or c)
+    dev = x_h16.device
+    if out_h16 is None:
+        out_h16 = torch.empty((b * h * s * w * s, 2 * oc), dtype=torch.float16, device=dev)
+    check(lib().p3d_upsample_nearest_h16(ptr(x_h16), b, h, w, c, s, ptr(out_h16), oc, int(out_c0), stream(dev)),
+          "upsample_nearest_h16")
+    return out_h16, (b, h * s, w * s)
+
+
+def pack_stem_weight(weight):
+    """ResNet stem weight [64, 3, 7, 7] fp32 -> the mma fragment image p3d_resnet_stem_h16 reads."""
+    weight = require_cuda(weight, "weight", torch.float32).contiguous()
+    if tuple(weight.shape) != (64, 3, 7, 7):
+        raise ValueError("resnet stem weight %s, want (64, 3, 7, 7)" % (tuple(weight.shape),))
+    L = lib()
+    packed = torch.empty((L.p3d_resnet_stem_packed_weight_bytes(),), dtype=torch.uint8, device=weight.device)
+    check(L.p3d_resnet_stem_pack_weights(ptr(weight), ptr(packed), ptr(_status(weight.device)), stream(weight.device)),
+          "resnet_stem_pack_weights")
+    return packed
+
+
+def stem_shape(h, w):
+    """(pH, pW) of the stem's output: conv 7x7 s2 p3, then MaxPool2d(3, 2, 1)."""
+    ch, cw = (h - 1) // 2 + 1, (w - 1) // 2 + 1
+    return (ch - 1) // 2 + 1, (cw - 1) // 2 + 1
+
+
+def resnet_stem_h16(x, packed, scale, shift, out_h16=None):
+    """MaxPool2d(3, 2, 1)(ReLU(BN(conv7x7 s2 p3))) of fp32 images x [B, 3, H, W] (p3d_resnet_stem_h16) -> (pixel H16 rows
+    [B*pH*pW, 2*64], (B, pH, pW, 64)).  packed: pack_stem_weight; scale / shift [64]: the folded BatchNorm."""
+    x = require_cuda(x, "x", torch.float32)
+    b, c, h, w = x.shape
+    if c != 3:
+        raise ValueError("resnet_stem_h16 takes 3-channel images, got %d" % c)
+    ph, pw = stem_shape(h, w)
+    if out_h16 is None:
+        out_h16 = torch.empty((b * ph * pw, 128), dtype=torch.float16, device=x.device)
+    check(lib().p3d_resnet_stem_h16(ptr(x), b, h, w, ptr(packed), ptr(scale), ptr(shift), ptr(out_h16),
+                                    ptr(_status(x.device)), stream(x.device)), "resnet_stem_h16")
+    return out_h16, (b, ph, pw, 64)

@@ -295,6 +295,31 @@ def ego_poses(n_frames, speed=10.0, yaw_rate=0.3, period=0.5, origin=(600.0, 160
     return out
 
 
+def camera_images(seed, n_cams=6, H=256, W=704, cell=16):
+    """Seeded normalised camera images [n_cams, 3, H, W] float32, what BEVDet's data pipeline hands the image backbone
+    (img_inputs[0] after mean / std normalisation): spatially smooth (white noise on a grid of `cell`-pixel cells,
+    interpolated bilinearly, plus 10 % pixel noise), each channel scaled to zero mean and unit variance, so that the convs
+    see image-like structure rather than white noise."""
+    rng = np.random.default_rng([seed, 11])
+    gh, gw = H // cell + 2, W // cell + 2
+    coarse = rng.normal(size=(n_cams, 3, gh, gw))
+
+    def axis(n, g):
+        src = (np.arange(n) + 0.5) / cell
+        i = np.minimum(np.floor(src).astype(np.int64), g - 2)
+        return i, (src - i)[:, None] if n == H else (src - i)[None, :]
+    yi, ly = axis(H, gh)
+    xi, lx = axis(W, gw)
+    a = coarse[:, :, yi][:, :, :, xi]
+    b = coarse[:, :, yi][:, :, :, xi + 1]
+    c = coarse[:, :, yi + 1][:, :, :, xi]
+    d = coarse[:, :, yi + 1][:, :, :, xi + 1]
+    img = (a * (1 - lx) + b * lx) * (1 - ly) + (c * (1 - lx) + d * lx) * ly
+    img = img + 0.1 * rng.normal(size=img.shape)
+    img = (img - img.mean(axis=(2, 3), keepdims=True)) / img.std(axis=(2, 3), keepdims=True)
+    return img.astype(np.float32)
+
+
 def lss_mats(rig):
     """(sensor2ego, cam2imgs, post_rots, post_trans, bda) of a camera_rig, the order LSSHotPath takes them in."""
     return rig["sensor2ego"], rig["cam2imgs"], rig["post_rots"], rig["post_trans"], rig["bda"]
