@@ -499,6 +499,23 @@ size_t p3d_resnet_stem_packed_weight_bytes(void);
 int p3d_resnet_stem_pack_weights(const float *weight, void *packed, int32_t *status_dev, p3d_stream_t stream);
 int p3d_resnet_stem_h16(const float *in, int B, int H, int W, const void *packed_weight, const float *scale, const float *shift,
                         void *out_h16, int32_t *status_dev, p3d_stream_t stream);
+/* BEVDet's test-time image pipeline (PrepareImageInputs.img_transform + mmlabNormalize) of decoded uint8 RGB frames,
+ * bit-identical to the host's PIL.Image.resize((rW, rH)) (BICUBIC, 8 bits per channel: fixed-point coefficients with 22
+ * fraction bits, horizontal pass rounded and clamped to uint8, then the vertical pass), PIL crop (crop_x, crop_y,
+ * crop_x + fW, crop_y + fH) of the resized image (0 outside it) and mmcv.imnormalize: out[n][c][y][x] =
+ * fp32(fp64(fp32(v - mean_host[c])) * std_inv_host[c]) with v = the cropped pixel's channel (swap_rb ? 2 - c : c).
+ *   frames [N][band_rows][W0][3] uint8: rows [y0, y0 + band_rows) of each H0 x W0 source frame.
+ *   kh [rW][kh_size], xbounds [rW][2] = (xmin, n): resized column x = sum over t < n of kh[x][t] * source column xmin + t;
+ *   kv [rH][kv_size], ybounds [rH][2] the same for the rows, ymin relative to y0 (ops/image_prep.resize_coeffs; device
+ *   int32).  Taps outside the band read 0.  mean_host [3] fp32, std_inv_host [3] fp64: host arrays, copied at the call.
+ *   out [N][3][fH][fW] fp32, 16-byte aligned, written in full and nothing else.  No allocation, no host synchronisation.
+ * Null pointers, a size < 1, band_rows > H0, |crop| > 2^28, out not 16-byte aligned, or kh_size / kv_size other than
+ * Pillow's 2 * ceil(2 * max(in / out, 1)) + 1 for W0 -> rW / H0 -> rH: P3D_ERR_INVALID_ARG.  A reduction by more than 8
+ * on either axis (more than 33 taps), N > 65535 or N * 3 * fH * fW >= 2^31: P3D_ERR_UNSUPPORTED. */
+int p3d_image_prep_u8(const uint8_t *frames, int N, int band_rows, int H0, int W0, const int32_t *kh, const int32_t *xbounds,
+                      int kh_size, int rW, const int32_t *kv, const int32_t *ybounds, int kv_size, int rH, int crop_x,
+                      int crop_y, int fH, int fW, const float *mean_host, const double *std_inv_host, int swap_rb,
+                      float *out, p3d_stream_t stream);
 /* p3d_bev_pool_v2_dev into pixel H16 rows: out_h16 [B, Y, X, out_C] with channel z * c + ch of cell (y, x) (the layout of
  * the planar output, one pixel per row), same accumulation, then split into (hi, lo'); status bit 0 on fp16 overflow.
  * out_h16 is zero-filled here (empty cells and channels >= Z * c).  out_C % 32 == 0 and out_C >= Z * c

@@ -102,6 +102,8 @@ SIGNATURES = {
     "p3d_resnet_stem_pack_weights": (_int, [_vp, _vp, _vp, _vp]),
     "p3d_resnet_stem_h16": (_int, [_vp, _int, _int, _int, _vp, _vp, _vp, _vp, _vp, _vp]),
     "p3d_lss_depth_feat_h16": (_int, [_vp, _int, _int, _int, _int, _int, _int, _vp, _vp, _vp]),
+    "p3d_image_prep_u8": (_int, [_vp, _int, _int, _int, _int, _vp, _vp, _int, _int, _vp, _vp, _int, _int, _int, _int, _int,
+                                 _int, _vp, _vp, _int, _vp, _vp]),
     "p3d_bev_pool_v2_dev_h16": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _int, _int, _int, _int, _int, _vp, _int,
                                        _vp, _vp]),
     "p3d_bev_shift_h16": (_int, [_vp, _int, _int, _int, _int, _int, _vp, _vp, _int, _int, _vp, _vp]),

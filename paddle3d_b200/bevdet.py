@@ -15,11 +15,14 @@ class x cell, per-class scale-NMS or circle NMS, bottom centre, up to post_max_s
 
 BEVDetFromImages / BEVDetImageHotPath (CONFIG_IMG) put BEVDet's image half in front of it: six normalised camera images ->
 ResNet-50 (p3d_resnet_stem_h16, then Bottlenecks on the dense fp16-pair conv) -> CustomFPN -> depth net ->
-p3d_lss_depth_feat_h16 -> the frame above, one captured graph."""
+p3d_lss_depth_feat_h16 -> the frame above, one captured graph.
+
+BEVDetFrameHotPath (DATA_CONFIG) starts that graph one step earlier, from six decoded uint8 camera frames: the test
+pipeline's resize, crop and normalisation (ops.image_prep, bit-identical to Pillow + OpenCV on the host) -> the images."""
 import numpy as np
 import torch
 
-from . import synth
+from . import raw, synth
 from .dense_head import DenseRPNHead, _Conv
 from .frame import ResultSlot, ResultSlotOwner, copy_rows
 from .lss import CameraFrame, LSSViewTransformer
@@ -27,6 +30,7 @@ from .ops import bev_pool_v2 as bp
 from .ops import bevdet_postprocess as bdp
 from .ops import centerpoint_postprocess as cpp
 from .ops import dense_conv as dc
+from .ops import image_prep as ip
 from .ops import sparse_nn as sp
 
 # PARITY UNPINNED (see the module docstring)
@@ -319,6 +323,13 @@ DEPTH_NET = dict(in_channels=512)
 CONFIG_IMG = dict(CONFIG, img_backbone=IMG_BACKBONE, img_neck=IMG_NECK, depth_net=DEPTH_NET)
 CONFIG_IMG_BEVDET_NMS = dict(CONFIG_IMG, test=TEST_CFG_BEVDET)
 
+# PARITY UNPINNED, as CONFIG: bevdet-r50's data_config as its test pipeline reads it (PrepareImageInputs with
+# train=False: resize to input_size's width, crop the bottom rows, no flip or rotation) and mmlabNormalize's mean / std
+# (float32 arrays there, to_rgb=True), recalled, not checked against the reference.  A model config without data_config
+# takes this one at its own input_size.
+DATA_CONFIG = dict(src_size=(900, 1600), input_size=(256, 704), crop_h=(0.0, 0.0), resize_test=0.0,
+                   mean=(123.675, 116.28, 103.53), std=(58.395, 57.12, 57.375), to_rgb=True)
+
 
 def round16(c):
     return (int(c) + 15) // 16 * 16
@@ -506,11 +517,40 @@ class BEVDetFromImages(BEVDet):
         self.input_size = (int(H_in), int(W_in))
         self.image_encoder = BEVDetImageEncoder(mc["img_backbone"], mc["img_neck"], mc["depth_net"], self.vt.D,
                                                 mc["channels"])
+        self.data_config = dict(mc.get("data_config", dict(DATA_CONFIG, input_size=self.input_size)))
+        self.augmentation = ip.test_augmentation(self.data_config)
+        x0, y0, x1, y1 = self.augmentation["crop"]
+        if (y1 - y0, x1 - x0) != self.input_size:
+            raise ValueError("BEVDetFromImages: data_config crops %s images, the model takes %s"
+                             % ((y1 - y0, x1 - x0), self.input_size))
+        self.prep_plan = None
 
     def init_weight(self, seed=0, bn_gain=1.0, device=None):
+        """Seeded weights; with a device also the image prep plan of data_config (ops.image_prep.ImagePrepPlan)."""
         super().init_weight(seed=seed, bn_gain=bn_gain, device=device)
         self.image_encoder.init_weight(seed, device=None if device is False else (device or self.device))
+        if device is not False:
+            self.prep_plan = ip.ImagePrepPlan.from_data_config(self.data_config, device or self.device)
         return self
+
+    def test_mats(self, sensor2ego, cam2imgs, bda):
+        """(sensor2ego, cam2imgs, post_rots, post_trans, bda) of camera frames run through data_config's test
+        augmentation: post_rots / post_trans [B, N, 3, 3] / [B, N, 3] float32 from it."""
+        b, n = np.shape(sensor2ego)[:2]
+        a = self.augmentation
+        return (sensor2ego, cam2imgs, np.broadcast_to(a["post_rot"], (b, n, 3, 3)).copy(),
+                np.broadcast_to(a["post_tran"], (b, n, 3)).copy(), bda)
+
+    def images_from_frames(self, frames):
+        """frames [N, H0, W0, 3] uint8 on the device (decoded RGB) -> the normalised images [N, 3, H, W] fp32."""
+        if self.prep_plan is None:
+            raise RuntimeError("BEVDetFromImages: call init_weight with a device first (it builds the image prep plan)")
+        return ip.image_prep_u8(frames, self.prep_plan)
+
+    def forward_frames(self, sensor2ego, cam2imgs, bda, frames):
+        """Eager frame from decoded camera frames [N, H0, W0, 3] uint8 on the device: (boxes, scores, labels, counts) as
+        forward_images on images_from_frames(frames) with test_mats."""
+        return self.forward_images(self.test_mats(sensor2ego, cam2imgs, bda), self.images_from_frames(frames))
 
     def export_numpy(self):
         return dict(super().export_numpy(), image_encoder=self.image_encoder.export_numpy())
@@ -585,6 +625,66 @@ class BEVDetImageHotPath(BEVDetHotPath):
 
     def infer(self, mats, imgs=None):
         self.launch(mats, imgs)
+        return self.result()
+
+
+class BEVDetFrameHotPath(BEVDetImageHotPath):
+    """BEVDetImageHotPath from decoded camera frames: the captured frame starts with p3d_image_prep_u8 (the model's
+    data_config test pipeline: Pillow BICUBIC resize, crop, mmcv.imnormalize, bit-identical to the host's) from the
+    lane's uint8 band buffer into the images, then runs BEVDetImageHotPath's frame.  launch_frames copies only the source
+    rows the crop needs (the plan's band) of every camera, as one 2-D copy on the lane's stream before the replay.  Lanes,
+    share_model and accelerate as in BEVDetImageHotPath; the model needs init_weight with a device (its prep plan)."""
+
+    def __init__(self, model, device="cuda", stream=None):
+        if getattr(model, "prep_plan", None) is None:
+            raise ValueError("BEVDetFrameHotPath: the model has no image prep plan (init_weight with a device builds it)")
+        super().__init__(model, device, stream)
+        plan = model.prep_plan
+        self.band = torch.zeros((model.N, plan.band_rows, plan.src_size[1], 3), dtype=torch.uint8, device=self.device)
+
+    def _frame(self):
+        ip.image_prep_u8(self.band, self.model.prep_plan, out=self.imgs)
+        return super()._frame()
+
+    def launch_frames(self, sensor2ego, cam2imgs, bda, frames):
+        """Enqueue one frame from decoded camera frames [N, H0, W0, 3] uint8 (contiguous; on this device, or in pinned
+        host memory, which must stay unchanged until the frame's result is read); the camera matrices as test_mats
+        takes them.  Pageable host memory raises ValueError (its copy would not be asynchronous)."""
+        plan = self.model.prep_plan
+        (H0, W0), N = plan.src_size, self.model.N
+        if not isinstance(frames, torch.Tensor) or frames.dtype != torch.uint8 or tuple(frames.shape) != (N, H0, W0, 3) \
+                or not frames.is_contiguous():
+            raise ValueError("BEVDetFrameHotPath: frames must be a contiguous uint8 tensor [%d, %d, %d, 3], got %s %s"
+                             % (N, H0, W0, getattr(frames, "dtype", type(frames)), tuple(getattr(frames, "shape", ()))))
+        if frames.is_cuda:
+            if frames.device != self.device:
+                raise ValueError("BEVDetFrameHotPath: frames on %s, the lane runs on %s" % (frames.device, self.device))
+        elif not frames.is_pinned():
+            raise ValueError("BEVDetFrameHotPath: frames in pageable host memory; pass a device tensor or pinned host "
+                             "memory (tensor.pin_memory())")
+        mats = self.model.test_mats(sensor2ego, cam2imgs, bda)
+        self.stream.wait_stream(torch.cuda.current_stream(self.device))
+        with torch.cuda.stream(self.stream):  # after the lane's previous frame, which read the band
+            self.copy_band(frames)
+            if frames.is_cuda:
+                frames.record_stream(self.stream)
+        self._launch(mats, None, None, "frame")
+
+    def copy_band(self, frames):
+        """Enqueue the copy of the band rows of frames [N, H0, W0, 3] (checked by launch_frames) into the lane's band
+        buffer on the current stream: one cudaMemcpy2DAsync, a camera per row."""
+        plan = self.model.prep_plan
+        H0, W0 = plan.src_size
+        row = W0 * 3
+        width = plan.band_rows * row
+        rc = raw.cudart().cudaMemcpy2DAsync(self.band.data_ptr(), width, frames.data_ptr() + plan.band[0] * row, H0 * row,
+                                            width, frames.shape[0], 4,  # cudaMemcpyDefault
+                                            torch.cuda.current_stream(self.device).cuda_stream)
+        if rc != 0:
+            raise RuntimeError("cudaMemcpy2DAsync failed (cudaError %d)" % rc)
+
+    def infer_frames(self, sensor2ego, cam2imgs, bda, frames):
+        self.launch_frames(sensor2ego, cam2imgs, bda, frames)
         return self.result()
 
 

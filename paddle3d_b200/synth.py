@@ -320,6 +320,30 @@ def camera_images(seed, n_cams=6, H=256, W=704, cell=16):
     return img.astype(np.float32)
 
 
+def camera_frames(seed, n_cams=6, H=900, W=1600):
+    """Seeded decoded camera frames [n_cams, H, W, 3] uint8 (HWC RGB, what np.array(Image.open(path)) gives for a nuScenes
+    image): smooth structure (noise on a 48-pixel grid, interpolated bilinearly), a dozen hard-edged rectangles, pixel
+    noise, and a contrast that saturates part of every frame at 0 and at 255, so that resampling meets edges and both
+    clamps."""
+    rng = np.random.default_rng([seed, 13])
+    cell = 48
+    gh, gw = H // cell + 2, W // cell + 2
+    coarse = rng.normal(size=(n_cams, gh, gw, 3)).astype(np.float32)
+    ys, xs = (np.arange(H, dtype=np.float32) + 0.5) / cell, (np.arange(W, dtype=np.float32) + 0.5) / cell
+    yi, xi = np.minimum(ys.astype(np.int64), gh - 2), np.minimum(xs.astype(np.int64), gw - 2)
+    ly, lx = (ys - yi)[None, :, None, None], (xs - xi)[None, None, :, None]
+    top = coarse[:, yi][:, :, xi] * (1 - lx) + coarse[:, yi][:, :, xi + 1] * lx
+    bot = coarse[:, yi + 1][:, :, xi] * (1 - lx) + coarse[:, yi + 1][:, :, xi + 1] * lx
+    img = 128.0 + 110.0 * (top * (1 - ly) + bot * ly)
+    for n in range(n_cams):
+        for _ in range(12):
+            h, w = int(rng.integers(8, H // 3)), int(rng.integers(8, W // 3))
+            y, x = int(rng.integers(0, H - h)), int(rng.integers(0, W - w))
+            img[n, y:y + h, x:x + w] = rng.uniform(-40, 300, 3).astype(np.float32)
+    img += rng.normal(0, 6, img.shape).astype(np.float32)
+    return np.ascontiguousarray(np.clip(np.rint(img), 0, 255).astype(np.uint8))
+
+
 def lss_mats(rig):
     """(sensor2ego, cam2imgs, post_rots, post_trans, bda) of a camera_rig, the order LSSHotPath takes them in."""
     return rig["sensor2ego"], rig["cam2imgs"], rig["post_rots"], rig["post_trans"], rig["bda"]

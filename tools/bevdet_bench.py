@@ -27,6 +27,13 @@ alternate the two (median of the rounds): frames/s in flight and one at a time; 
 depth net + lss_depth_feat_h16 with their GFLOP and TFLOP/s; the stem's algorithmic bytes and GB/s; the node counts of
 both frame graphs; the card; and a frame-0 check against the CPU arm (bevdet_images_oracle.CpuBEVDetImages, tests/).
 
+--raw-images: BEVDet from six decoded 900 x 1600 uint8 camera frames (bevdet.BEVDetFrameHotPath: the test pipeline's
+resize, crop and normalisation in p3d_image_prep_u8 at the head of the captured frame) fed from pinned host memory, the
+band's H2D included, next to BEVDetImageHotPath on resident fp32 images, in rounds that alternate the two (median of the
+rounds): frames/s in flight and one at a time; the host baseline (Pillow + OpenCV prep of the six cameras, one thread,
+timed on this host); the graph-timed prep kernel with its algorithmic bytes and GB/s; the band's H2D bytes and time; the
+node counts of both frame graphs; the card; and a frame-0 check that the device images equal the host pipeline's.
+
 --bevdet-nms: the frames with BEVDet's own box decode (bevdet.CONFIG_BEVDET_NMS, with --temporal CONFIG_4D_BEVDET_NMS:
 top-K over class x cell, per-class scale-NMS / circle NMS) next to the same weights with the default decode
 (centerpoint_postprocess), measured in rounds that alternate the two on the same inputs (median of the rounds): frames/s
@@ -77,10 +84,15 @@ def main():
     ap.add_argument("--images", action="store_true",
                     help="BEVDet from six camera images (ResNet-50 + CustomFPN + depth net in the frame), alternated with "
                          "the frame from the depth net's output")
+    ap.add_argument("--raw-images", action="store_true",
+                    help="BEVDet from six decoded uint8 camera frames (image prep in the frame), alternated with the frame "
+                         "from normalised images")
     args = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("bevdet_bench.py needs a CUDA device (no CPU fallback exists)")
+    if args.raw_images:
+        return raw_images(args)
     if args.images:
         return images(args)
     if args.bevdet_nms:
@@ -445,6 +457,107 @@ def images(args):
                                     "cpu_oracle_s": s,
                                     "kind": "fp64-accumulating numpy + OpenMP oracle, not a tuned CPU implementation"}
     line["value"] = line["images"]["fps_in_flight"]
+    print(json.dumps(line))
+
+
+def raw_images(args):
+    import cv2
+    import torch
+    from paddle3d_b200 import bevdet as bd
+    from paddle3d_b200 import synth
+    from paddle3d_b200.ops import image_prep as ip
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from image_prep_oracle import pipeline_pil_cv2
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    m = bd.BEVDetFromImages(device=dev).init_weight(seed=args.seed, bn_gain=BN_GAIN)
+    plan, dcfg, aug = m.prep_plan, m.data_config, m.augmentation
+    rigs = [synth.camera_rig(s) for s in range(4)]
+    cams = [(r["sensor2ego"], r["cam2imgs"], r["bda"]) for r in rigs]
+    mats = [m.test_mats(*c) for c in cams]
+    frames_np = [synth.camera_frames(args.seed + i) for i in range(2)]
+    frames_host = [torch.from_numpy(f).pin_memory() for f in frames_np]
+    imgs = ip.image_prep_u8(frames_host[0].to(dev), plan)
+    m.calibrate_heatmap_bias(mats[0], imgs)
+    line = {"metric": "BEVDet frames/s from six decoded 900 x 1600 uint8 camera frames in pinned host memory (band H2D -> "
+                      "resize / crop / normalise -> ResNet-50 + CustomFPN + depth net -> LSS -> BEV encoder -> CenterHead "
+                      "-> boxes)", "unit": "frames/s", "gpu": gpu_identity(0), "steps": args.steps,
+            "warmup": args.warmup}
+    lanes_n = max(1, args.in_flight)
+    runs = {"frames": [bd.BEVDetFrameHotPath(m, device=dev).capture(count_nodes=(i == 0)) for i in range(lanes_n)],
+            "images": [bd.BEVDetImageHotPath(m, device=dev).capture(count_nodes=(i == 0)) for i in range(lanes_n)]}
+    for ln in runs["images"]:  # resident fp32 images: the timed frames replay on them
+        ln.imgs.copy_(imgs)
+    torch.cuda.synchronize()
+    count = {}
+
+    def launch(name, lane):
+        k = count.get(name, 0)
+        count[name] = k + 1
+        if name == "frames":  # a new calibration and new frames every frame
+            lane.launch_frames(*cams[k % 4], frames_host[k % 2])
+        else:
+            lane.launch(mats[k % 4])
+
+    def one(name, lane):
+        launch(name, lane)
+        lane.result()
+    rates = {n: {"fps_in_flight": [], "fps_one_at_a_time": []} for n in runs}
+    for name, lanes in runs.items():
+        for i in range(args.warmup):
+            launch(name, lanes[i % lanes_n])
+    torch.cuda.synchronize()
+    for _ in range(max(1, args.rounds)):  # alternate the frames so that clocks and temperature drift hit both
+        for name, lanes in runs.items():
+            rates[name]["fps_in_flight"].append(
+                _rate(lambda i: launch(name, lanes[i % lanes_n]), torch.cuda.synchronize, args.steps))
+            rates[name]["fps_one_at_a_time"].append(
+                _rate(lambda i: one(name, lanes[0]), torch.cuda.synchronize, args.steps))
+    for name, lanes in runs.items():
+        for ln in lanes:
+            ln.result()  # raises on an fp16-range overflow
+        r = {k: float(np.median(v)) for k, v in rates[name].items()}
+        r.update(rounds=rates[name], lanes=lanes_n, graph_nodes=lanes[0].graph_nodes)
+        line[name] = r
+    hot = runs["frames"][0]
+    got = [t.clone().numpy() for t in hot.infer_frames(*cams[0], frames_host[0])]
+    line["boxes_frame0"] = int(len(got[0]))
+    # host baseline: Pillow resize + crop and mmcv.imnormalize's OpenCV steps of the six cameras, one thread
+    cv2.setNumThreads(1)
+    reps = 5
+    host_imgs = pipeline_pil_cv2(frames_np[0], aug["resize_dims"], aug["crop"], dcfg["mean"], dcfg["std"], dcfg["to_rgb"])
+    t0 = time.perf_counter()
+    for i in range(reps):
+        pipeline_pil_cv2(frames_np[i % 2], aug["resize_dims"], aug["crop"], dcfg["mean"], dcfg["std"], dcfg["to_rgb"])
+    host_s = (time.perf_counter() - t0) / reps
+    line["host_prep"] = {"s_per_frame": host_s, "frames_per_s": 1.0 / host_s, "cpus": os.cpu_count(),
+                         "kind": "PIL.Image.resize + crop and cv2 cvtColor / subtract / multiply of six 900 x 1600 frames, "
+                                 "one thread, no H2D"}
+    dev_imgs = hot.imgs.cpu().numpy()
+    line["images_equal_host_pipeline_frame0"] = bool(np.array_equal(dev_imgs.view(np.int32), host_imgs.view(np.int32)))
+    # the prep kernel, graph-timed, and the band's H2D
+    st = torch.cuda.Stream(dev)
+    band, out = hot.band, torch.empty_like(hot.imgs)
+    prep_ms = graph_time_ms(lambda: ip.image_prep_u8(band, plan, out=out), st, 50)
+    n = m.N
+    nbytes = plan.band_bytes(n) + plan.out_bytes(n)
+    line["prep_kernel"] = {"us": prep_ms * 1e3, "algorithmic_bytes": nbytes, "GB_per_s": nbytes / (prep_ms * 1e-3) / 1e9,
+                           "band_rows": plan.band_rows,
+                           "note": "the band of six cameras read once (uint8) + the fp32 images written once"}
+    with torch.cuda.stream(st):
+        hot.copy_band(frames_host[0])
+        st.synchronize()
+        s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        s.record(st)
+        for _ in range(20):
+            hot.copy_band(frames_host[0])
+        e.record(st)
+    e.synchronize()
+    h2d_ms = s.elapsed_time(e) / 20
+    line["band_h2d"] = {"bytes_per_frame": plan.band_bytes(n), "ms": h2d_ms,
+                        "GB_per_s": plan.band_bytes(n) / (h2d_ms * 1e-3) / 1e9,
+                        "full_fp32_images_bytes": plan.out_bytes(n)}
+    line["value"] = line["frames"]["fps_in_flight"]
     print(json.dumps(line))
 
 
