@@ -10,7 +10,7 @@ Reference: the conv in float64 on the device (one fp64 GEMM per tap), with X the
 image (hi + lo' 2^-11, built here from fp32 and checked bit-equal to p3d_nchw_to_pixel_h16) and W the fp32 weight (so
 the weight split error is part of what is checked), then scale / shift / ReLU in the epilogue's order.  The bar is the
 one of test_gpu_dense.py (tests/parity.py's definition, evaluated on the device): 1e-4 true relative error above a
-floor of 1e-2 x max (5e-2 x max for sums of 2304 terms or more, see `bar`), 2e-6 (1e-5) x max below it, per batch
+floor of 1e-2 x max (5e-2 x max for sums of 2048 terms or more, see `bar`), 2e-6 (1e-5) x max below it, per batch
 image.  Every
 case also shows that the bar REJECTS two wrong answers computed from the reference: the hi x hi products alone, and the
 result without one tap (1x1 and transposed convs: without one 32-channel input group).
@@ -296,20 +296,24 @@ def epilogue(acc, scale, shift, relu):
 
 
 def bar(terms):
-    """(floor, small_atol) of test_gpu_dense.py's two bars for sums of `terms` products, with sums of exactly 2304 terms
-    (the 3x3 256-channel layers) on the 5e-2 floor.  At full size the wgmma fp32 accumulation noise is flat in absolute
-    terms (H100, 256 -> 128 at 180 x 180: std 2.6e-7 x max, worst 3.4e-6 x max, the same for the haloed and the per-tap
-    loads and the same against the exact pair products without lo' x lo'), so its relative error grows as the element
-    shrinks: 1.1e-4 between 1e-2 and 2e-2 x max, 6e-5 up to 5e-2, 2.5e-5 up to 1e-1 (1152 terms: 6.3e-5 / 3.0e-5 /
-    1.5e-5).  The same bar holds up to 7200 terms (BEVDet's encoder layers at full size in every decomposition of
+    """(floor, small_atol) of test_gpu_dense.py's two bars for sums of `terms` products, with sums of 2048 terms or more
+    (the 3x3 256-channel layers, the 1x1 2048-channel ones) on the 5e-2 floor.  At full size the wgmma fp32 accumulation
+    noise is flat in absolute terms (H100, 256 -> 128 at 180 x 180: std 2.6e-7 x max, worst 3.4e-6 x max, the same for
+    the haloed and the per-tap loads and the same against the exact pair products without lo' x lo'), so its relative
+    error grows as the element shrinks: 1.1e-4 between 1e-2 and 2e-2 x max, 6e-5 up to 5e-2, 2.5e-5 up to 1e-1 (1152
+    terms: 6.3e-5 / 3.0e-5 / 1.5e-5).  The same bar holds up to 7200 terms (BEVDet's encoder layers at full size in every decomposition of
     test_gpu_dense_residual.py::test_bevdet_layer_every_decomposition, whose "BAR" lines print these figures, on an
     H100 80GB HBM3 at a 700 W power limit): std of the error 5.2e-7 / 7.0e-7 / 7.5e-7 x max for 4608 / 5760 / 7200
     terms, at most 3.0e-6 / 3.6e-6 / 4.9e-6 x max on the elements below 5e-2 x max, and relative error above 5e-2 x max
     at most 5.6e-5 / 7.3e-5 / 7.0e-5.  The fused CenterHead's planes (a 9 Cin-term conv, its fp16-pair rounding and a
     576-term output conv) stay on the 576-term bar, same card: relative error above 1e-2 x max at most 7.2e-5 and at
-    most 1.2e-6 x max below it (test_gpu_head_fused_schedule.py's "BAR" lines).  A lost tap or cross product would show
-    a constant relative error instead, which the guards check."""
-    return (1e-2, 2e-6) if terms < 2304 else (5e-2, 1e-5)
+    most 1.2e-6 x max below it (test_gpu_head_fused_schedule.py's "BAR" lines).  The 1x1 convs over 2048 channels of
+    BEVDet's image encoder (test_gpu_image_encoder_schedule.py, six cameras at 256 x 704, same card) do not hold the
+    1e-2 floor: std 1.5e-7 / 2.1e-7 x max (stage-3 conv1 / lateral1), at most 1.3e-6 / 1.2e-6 x max below 5e-2 x max,
+    so 1.15e-4 / 1.2e-4 relative at the 1e-2 floor, and relative error above 5e-2 x max at most 2.8e-5 / 2.7e-5, the
+    same bits in every decomposition; 1024 terms: std 5.5e-8 to 8.3e-8 x max, at most 9.1e-7 x max below 5e-2 x max.
+    A lost tap or cross product would show a constant relative error instead, which the guards check."""
+    return (1e-2, 2e-6) if terms < 2048 else (5e-2, 1e-5)
 
 
 def rel_check_dev(name, got, want, terms, rtol=1e-4):
