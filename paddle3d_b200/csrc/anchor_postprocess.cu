@@ -7,7 +7,8 @@
 //   A2 ahp_col/row    2-D inclusive prefix sum of that map (cumsum(0).cumsum(1)), integers: exact in any order
 //   A3 ahp_score      per anchor: area = ID - IB - IC + IA on its four (host-precomputed) clamped voxel corners
 //                     (fused_get_anchors_area), keep area > thr; score = max over the C classes of sigmoid(cls_c)
-//                     (encode_background_as_zeros, use_multi_class_nms off); candidate if score >= thr;
+//                     (encode_background_as_zeros, use_multi_class_nms off; NaN if any class is NaN); candidate if
+//                     score >= thr;
 //                     51-bit sort key (~score_bits << 20 | anchor) - descending score, ties by ascending anchor index
 //   A4 cub radix sort of the keys (non-candidates carry the all-ones key and sink to the end)
 //   A5 ahp_gather     first min(candidates, pre_max): class label (recomputed, so no per-anchor label array),
@@ -85,13 +86,15 @@ __device__ __forceinline__ float sigmoid_f32(float x) { return __fdiv_rn(1.0f, _
 
 // Score and label of one anchor: max over the C class planes of sigmoid(cls_c), label = the first class reaching it.
 // The comparison is on the fp32 sigmoid values (as the reference's max / argmax over sigmoid(cls)), not on the logits:
-// two logits may round to the same score, and then the lower class wins.  cls points at class 0 of the anchor's group.
+// two logits may round to the same score, and then the lower class wins.  A NaN logit in any class makes the score NaN
+// (labelled with the first NaN class), as the reference's max propagates it, so the anchor is never a candidate.
+// cls points at class 0 of the anchor's group.
 __device__ __forceinline__ float class_max(const float *__restrict__ cls, size_t HW, int C, int &label) {
   float best = sigmoid_f32(cls[0]);
   label = 0;
-  for (int c = 1; c < C; ++c) {
+  for (int c = 1; c < C && best == best; ++c) {
     const float s = sigmoid_f32(cls[static_cast<size_t>(c) * HW]);
-    if (s > best) {
+    if (s > best || s != s) {
       best = s;
       label = c;
     }

@@ -78,6 +78,10 @@ def test_invalid_arguments_return_status_codes():
     rc = L.p3d_hard_voxelize(None, 0, 4, tiny, big, 4, 16, None, None, None, None, None, 0, None)
     assert rc == -4
     assert L.p3d_nms(None, -1, 0.5, 0, None, None, None, 0, None) == -1
+    # 17 tasks is more than the postprocess batches: unsupported, decided before any pointer is read; 0 tasks is invalid
+    for tasks, rc in ((17, -4), (0, -1)):
+        assert L.p3d_centerpoint_postprocess(tasks, *[None] * 7, 180, 180, *[None] * 4, 8, 0.1, 0.2, 1000, 83, 1,
+                                             *[None] * 5, 0, None) == rc
 
 
 def test_conv_entry_points_reject_invalid_arguments():
