@@ -18,13 +18,19 @@ ResNet-50 (p3d_resnet_stem_h16, then Bottlenecks on the dense fp16-pair conv) ->
 p3d_lss_depth_feat_h16 -> the frame above, one captured graph.
 
 BEVDetFrameHotPath (DATA_CONFIG) starts that graph one step earlier, from six decoded uint8 camera frames: the test
-pipeline's resize, crop and normalisation (ops.image_prep, bit-identical to Pillow + OpenCV on the host) -> the images."""
+pipeline's resize, crop and normalisation (ops.image_prep, bit-identical to Pillow + OpenCV on the host) -> the images.
+
+BEVDet4DFromImages / BEVDet4DImageHotPath / BEVDet4DFrameHotPath (CONFIG_4D_IMG) do the same for BEVDet4D: the image
+encoder (and the image prep) at the head of both temporal graphs; BEVDet4DFrameHotPath.infer_stream runs a drive from
+frames and ego poses (drive_mats)."""
+import itertools
+
 import numpy as np
 import torch
 
 from . import raw, synth
 from .dense_head import DenseRPNHead, _Conv
-from .frame import ResultSlot, ResultSlotOwner, copy_rows
+from .frame import ResultSlot, ResultSlotOwner, copy_rows, in_flight
 from .lss import CameraFrame, LSSViewTransformer
 from .ops import bev_pool_v2 as bp
 from .ops import bevdet_postprocess as bdp
@@ -283,8 +289,13 @@ class BEVDetHotPath(ResultSlotOwner, CameraFrame):
         return self
 
     # ---- stages, as they are captured
-    def _frame(self):
+    def _depth_feat(self):
+        """The frame's first stage: fill self.depth / self.feat (here from the depth net's output in self.logits /
+        self.tran_feat; ImageInput and FrameInput override it)."""
         bp.lss_depth_feat(self.logits, self.tran_feat, self.depth, self.feat)
+
+    def _frame(self):
+        self._depth_feat()
         self.model.pool(self.depth, self.feat, self.prepared, out=self.image)
         return self._dense(self.image)
 
@@ -596,7 +607,90 @@ class BEVDetFromImages(BEVDet):
         return out
 
 
-class BEVDetImageHotPath(BEVDetHotPath):
+class ImageInput:
+    """Mixin of a camera lane (BEVDetHotPath or a subclass) whose depth / feat come from camera images: the lane's
+    _depth_feat stage is image encoder -> p3d_lss_depth_feat_h16 on the images in self.imgs [N, 3, H, W] fp32."""
+
+    def _init_images(self):
+        H, W = self.model.input_size
+        self.imgs = torch.zeros((self.model.N, 3, H, W), dtype=torch.float32, device=self.device)
+
+    def _depth_feat(self):
+        m = self.model
+        rows, shape = m.image_encoder(self.imgs)
+        m.depth_feat(rows, shape, self.depth, self.feat)
+
+    def _put_images(self, imgs):
+        """Enqueue the copy of imgs (a device tensor; None: nothing) into the lane's images on its stream."""
+        if imgs is not None:
+            self.stream.wait_stream(torch.cuda.current_stream(self.device))
+            with torch.cuda.stream(self.stream):  # after the lane's previous frame, which read the buffer
+                self.imgs.copy_(imgs, non_blocking=True)
+
+
+class FrameInput(ImageInput):
+    """ImageInput from decoded camera frames: the lane's _depth_feat stage starts with p3d_image_prep_u8 (the model's
+    data_config test pipeline) from the lane's uint8 band buffer self.band into the images.  Only the source rows the
+    crop needs (the plan's band) of every camera are copied, as one 2-D copy on the lane's stream before the replay."""
+
+    @classmethod
+    def check_plan(cls, model):
+        """Raise ValueError when the model has no image prep plan (called before the lane allocates anything)."""
+        if getattr(model, "prep_plan", None) is None:
+            raise ValueError("%s: the model has no image prep plan (init_weight with a device builds it)" % cls.__name__)
+
+    def _init_band(self):
+        plan = self.model.prep_plan
+        self.band = torch.zeros((self.model.N, plan.band_rows, plan.src_size[1], 3), dtype=torch.uint8,
+                                device=self.device)
+
+    def _depth_feat(self):
+        ip.image_prep_u8(self.band, self.model.prep_plan, out=self.imgs)
+        super()._depth_feat()
+
+    def check_frames(self, frames):
+        """Raise ValueError unless frames is a contiguous uint8 [N, H0, W0, 3] tensor on the lane's device or in pinned
+        host memory (a copy from pageable memory would not be asynchronous)."""
+        name = type(self).__name__
+        plan = self.model.prep_plan
+        (H0, W0), N = plan.src_size, self.model.N
+        if not isinstance(frames, torch.Tensor) or frames.dtype != torch.uint8 or tuple(frames.shape) != (N, H0, W0, 3) \
+                or not frames.is_contiguous():
+            raise ValueError("%s: frames must be a contiguous uint8 tensor [%d, %d, %d, 3], got %s %s"
+                             % (name, N, H0, W0, getattr(frames, "dtype", type(frames)),
+                                tuple(getattr(frames, "shape", ()))))
+        if frames.is_cuda:
+            if frames.device != self.device:
+                raise ValueError("%s: frames on %s, the lane runs on %s" % (name, frames.device, self.device))
+        elif not frames.is_pinned():
+            raise ValueError("%s: frames in pageable host memory; pass a device tensor or pinned host memory "
+                             "(tensor.pin_memory())" % name)
+
+    def _put_frames(self, frames):
+        """Enqueue the copy of the band of frames (checked by check_frames) into the lane's band buffer on its stream."""
+        self.stream.wait_stream(torch.cuda.current_stream(self.device))
+        with torch.cuda.stream(self.stream):  # after the lane's previous frame, which read the band
+            self.copy_band(frames)
+            if frames.is_cuda:
+                frames.record_stream(self.stream)
+
+    def copy_band(self, frames, out=None):
+        """Enqueue the copy of the band rows of frames [N, H0, W0, 3] (checked by check_frames) into out (a band-shaped
+        uint8 device tensor; None: the lane's band buffer) on the current stream: one cudaMemcpy2DAsync, a camera per
+        row."""
+        plan = self.model.prep_plan
+        H0, W0 = plan.src_size
+        row = W0 * 3
+        width = plan.band_rows * row
+        dst = self.band if out is None else out
+        rc = raw.cudart().cudaMemcpy2DAsync(dst.data_ptr(), width, frames.data_ptr() + plan.band[0] * row, H0 * row,
+                                            width, frames.shape[0], 4,  # cudaMemcpyDefault
+                                            torch.cuda.current_stream(self.device).cuda_stream)
+        if rc != 0:
+            raise RuntimeError("cudaMemcpy2DAsync failed (cudaError %d)" % rc)
+
+
+class BEVDetImageHotPath(ImageInput, BEVDetHotPath):
     """BEVDetHotPath from camera images: one captured CUDA graph from the camera descriptor to the D2H of the boxes, the
     frame being image encoder -> p3d_lss_depth_feat_h16 into the frame's depth / feat -> memset + pool -> encoder -> head
     -> postprocess.  launch(mats, imgs) copies imgs [N, 3, H, W] (a device tensor) into the lane's input buffer on its
@@ -604,23 +698,12 @@ class BEVDetImageHotPath(BEVDetHotPath):
 
     def __init__(self, model, device="cuda", stream=None):
         super().__init__(model, device, stream)
-        H, W = model.input_size
-        self.imgs = torch.zeros((model.N, 3, H, W), dtype=torch.float32, device=self.device)
-
-    def _frame(self):
-        m = self.model
-        rows, shape = m.image_encoder(self.imgs)
-        m.depth_feat(rows, shape, self.depth, self.feat)
-        m.pool(self.depth, self.feat, self.prepared, out=self.image)
-        return self._dense(self.image)
+        self._init_images()
 
     def launch(self, mats, imgs=None):
         """Enqueue one frame: mats = (sensor2ego, cam2imgs, post_rots, post_trans, bda) on the host; imgs: a device tensor
         copied into the frame's input (None: already written there)."""
-        if imgs is not None:
-            self.stream.wait_stream(torch.cuda.current_stream(self.device))
-            with torch.cuda.stream(self.stream):  # after the lane's previous frame, which read the buffer
-                self.imgs.copy_(imgs, non_blocking=True)
+        self._put_images(imgs)
         self._launch(mats, None, None, "frame")
 
     def infer(self, mats, imgs=None):
@@ -628,60 +711,25 @@ class BEVDetImageHotPath(BEVDetHotPath):
         return self.result()
 
 
-class BEVDetFrameHotPath(BEVDetImageHotPath):
+class BEVDetFrameHotPath(FrameInput, BEVDetImageHotPath):
     """BEVDetImageHotPath from decoded camera frames: the captured frame starts with p3d_image_prep_u8 (the model's
     data_config test pipeline: Pillow BICUBIC resize, crop, mmcv.imnormalize, bit-identical to the host's) from the
-    lane's uint8 band buffer into the images, then runs BEVDetImageHotPath's frame.  launch_frames copies only the source
-    rows the crop needs (the plan's band) of every camera, as one 2-D copy on the lane's stream before the replay.  Lanes,
-    share_model and accelerate as in BEVDetImageHotPath; the model needs init_weight with a device (its prep plan)."""
+    lane's uint8 band buffer into the images, then runs BEVDetImageHotPath's frame (FrameInput).  Lanes, share_model and
+    accelerate as in BEVDetImageHotPath; the model needs init_weight with a device (its prep plan)."""
 
     def __init__(self, model, device="cuda", stream=None):
-        if getattr(model, "prep_plan", None) is None:
-            raise ValueError("BEVDetFrameHotPath: the model has no image prep plan (init_weight with a device builds it)")
+        self.check_plan(model)
         super().__init__(model, device, stream)
-        plan = model.prep_plan
-        self.band = torch.zeros((model.N, plan.band_rows, plan.src_size[1], 3), dtype=torch.uint8, device=self.device)
-
-    def _frame(self):
-        ip.image_prep_u8(self.band, self.model.prep_plan, out=self.imgs)
-        return super()._frame()
+        self._init_band()
 
     def launch_frames(self, sensor2ego, cam2imgs, bda, frames):
         """Enqueue one frame from decoded camera frames [N, H0, W0, 3] uint8 (contiguous; on this device, or in pinned
         host memory, which must stay unchanged until the frame's result is read); the camera matrices as test_mats
         takes them.  Pageable host memory raises ValueError (its copy would not be asynchronous)."""
-        plan = self.model.prep_plan
-        (H0, W0), N = plan.src_size, self.model.N
-        if not isinstance(frames, torch.Tensor) or frames.dtype != torch.uint8 or tuple(frames.shape) != (N, H0, W0, 3) \
-                or not frames.is_contiguous():
-            raise ValueError("BEVDetFrameHotPath: frames must be a contiguous uint8 tensor [%d, %d, %d, 3], got %s %s"
-                             % (N, H0, W0, getattr(frames, "dtype", type(frames)), tuple(getattr(frames, "shape", ()))))
-        if frames.is_cuda:
-            if frames.device != self.device:
-                raise ValueError("BEVDetFrameHotPath: frames on %s, the lane runs on %s" % (frames.device, self.device))
-        elif not frames.is_pinned():
-            raise ValueError("BEVDetFrameHotPath: frames in pageable host memory; pass a device tensor or pinned host "
-                             "memory (tensor.pin_memory())")
+        self.check_frames(frames)
         mats = self.model.test_mats(sensor2ego, cam2imgs, bda)
-        self.stream.wait_stream(torch.cuda.current_stream(self.device))
-        with torch.cuda.stream(self.stream):  # after the lane's previous frame, which read the band
-            self.copy_band(frames)
-            if frames.is_cuda:
-                frames.record_stream(self.stream)
+        self._put_frames(frames)
         self._launch(mats, None, None, "frame")
-
-    def copy_band(self, frames):
-        """Enqueue the copy of the band rows of frames [N, H0, W0, 3] (checked by launch_frames) into the lane's band
-        buffer on the current stream: one cudaMemcpy2DAsync, a camera per row."""
-        plan = self.model.prep_plan
-        H0, W0 = plan.src_size
-        row = W0 * 3
-        width = plan.band_rows * row
-        rc = raw.cudart().cudaMemcpy2DAsync(self.band.data_ptr(), width, frames.data_ptr() + plan.band[0] * row, H0 * row,
-                                            width, frames.shape[0], 4,  # cudaMemcpyDefault
-                                            torch.cuda.current_stream(self.device).cuda_stream)
-        if rc != 0:
-            raise RuntimeError("cudaMemcpy2DAsync failed (cudaError %d)" % rc)
 
     def infer_frames(self, sensor2ego, cam2imgs, bda, frames):
         self.launch_frames(sensor2ego, cam2imgs, bda, frames)
@@ -770,27 +818,34 @@ class BEVDet4D(BEVDet):
         src, in_c = (concat, ec) if feat_prev is None else (feat_prev, self.hist_C)
         bp.bev_shift_h16(src, (1, Y, X, in_c), tf, self.bev_C, out_h16=concat, out_channels=ec, out_c0=self.bev_C)
 
-    def encoder_input(self, mats, prev_sensor2keyego, logits, tran_feat, feat_prev=None):
-        """Eager: the concat rows [Y*X, 2*160] of a frame (feat_prev None: the start of a sequence)."""
+    def concat_of(self, image, mats, prev_sensor2keyego, feat_prev=None):
+        """Eager: the concat rows [Y*X, 2*160] of a frame from its pool image (feat_prev None: the start of a sequence)."""
         _, Y, X, ec = self.enc_shape
         concat = torch.empty((Y * X, 2 * ec), dtype=torch.float16, device=self.device)
-        self.pre(self.image(mats, logits, tran_feat), concat, self.pre_buffers())
+        self.pre(image, concat, self.pre_buffers())
         tf = torch.from_numpy(self.shift_desc(mats, None if feat_prev is None else prev_sensor2keyego)).to(self.device)
         self.shift(feat_prev, tf, concat)
         return concat
+
+    def forward_concat(self, concat):
+        """Eager: (boxes, scores, labels, counts) of the concat rows and bev_feat [Y*X, 2*96], their first 96 channels."""
+        bev_feat = concat[:, :2 * self.hist_C].contiguous()
+        return self.postprocess(self.dense(concat)), bev_feat
+
+    def encoder_input(self, mats, prev_sensor2keyego, logits, tran_feat, feat_prev=None):
+        """Eager: the concat rows [Y*X, 2*160] of a frame (feat_prev None: the start of a sequence)."""
+        return self.concat_of(self.image(mats, logits, tran_feat), mats, prev_sensor2keyego, feat_prev)
 
     def forward(self, mats, prev_sensor2keyego, logits, tran_feat, feat_prev=None):
         """Eager frame: ((boxes, scores, labels, counts) as BEVDet.forward, bev_feat [Y*X, 2*96]: the next frame's
         feat_prev).  mats = (sensor2keyego, cam2imgs, post_rots, post_trans, bda) of this frame; prev_sensor2keyego [1, N, 4,
         4]: the previous frame's cameras in this frame's ego (ops.bev_pool_v2.sensor2keyegos); feat_prev None starts a
         sequence (bev_feat is its own adjacent frame and prev_sensor2keyego is not used)."""
-        concat = self.encoder_input(mats, prev_sensor2keyego, logits, tran_feat, feat_prev)
-        bev_feat = concat[:, :2 * self.hist_C].contiguous()
-        return self.postprocess(self.dense(concat)), bev_feat
+        return self.forward_concat(BEVDet4D.encoder_input(self, mats, prev_sensor2keyego, logits, tran_feat, feat_prev))
 
     def calibrate_heatmap_bias(self, mats, logits, tran_feat, target_frac=0.014):
         """BEVDet.calibrate_heatmap_bias on the start frame of a sequence with these inputs."""
-        x = self.encoder_input(mats, None, logits, tran_feat)
+        x = BEVDet4D.encoder_input(self, mats, None, logits, tran_feat)
         self.head.calibrate_heatmap_bias(x, self.test_cfg["score_threshold"], target_frac, shape=self.enc_shape)
         return self
 
@@ -826,7 +881,7 @@ class BEVDet4DHotPath(BEVDetHotPath):
 
     def _frame(self, start=False):
         m = self.model
-        bp.lss_depth_feat(self.logits, self.tran_feat, self.depth, self.feat)
+        self._depth_feat()
         m.pool(self.depth, self.feat, self.prepared, out=self.image)
         self.tf.copy_(self.h_shift, non_blocking=True)
         m.pre(self.image, self.concat, self.pre_bufs)
@@ -843,12 +898,16 @@ class BEVDet4DHotPath(BEVDetHotPath):
         """Enqueue one frame of this lane's sequence.  mats = (sensor2keyego, cam2imgs, post_rots, post_trans, bda);
         prev_sensor2keyego [1, N, 4, 4]: the previous frame's cameras in this frame's ego (ops.bev_pool_v2.sensor2keyegos);
         new_sequence: this frame starts a sequence (prev_sensor2keyego is not used).  A lane's first frame must start one."""
-        if not (new_sequence or self.started):
-            raise ValueError("BEVDet4DHotPath: the first frame of a lane must start a sequence (new_sequence=True)")
+        self.check_sequence(new_sequence)
         tf = self.model.shift_desc(mats, None if new_sequence else prev_sensor2keyego)
         self._launch(mats, logits, tran_feat, "start" if new_sequence else "continue",
                      host_inputs=lambda: self.h_shift.copy_(torch.from_numpy(tf.reshape(-1))))
         self.started = True
+
+    def check_sequence(self, new_sequence):
+        """Raise ValueError when a frame would continue a sequence this lane never started."""
+        if not (new_sequence or self.started):
+            raise ValueError("%s: the first frame of a lane must start a sequence (new_sequence=True)" % type(self).__name__)
 
     def infer(self, mats, prev_sensor2keyego=None, logits=None, tran_feat=None, new_sequence=False):
         self.launch(mats, prev_sensor2keyego, logits, tran_feat, new_sequence)
@@ -857,3 +916,169 @@ class BEVDet4DHotPath(BEVDetHotPath):
     def check_status(self, status_host):
         if int(status_host[0]):
             raise RuntimeError("BEVDet4D: an activation left fp16's range (|x| >= 65504) on the fp16-pair path")
+
+
+# ------------------------------------------------------------------------------------------ BEVDet4D from images
+# PARITY UNPINNED, as the configs it combines: BEVDet4D's BEV half (CONFIG_4D) behind BEVDet-R50's image half (CONFIG_IMG).
+CONFIG_4D_IMG = dict(CONFIG_4D, img_backbone=IMG_BACKBONE, img_neck=IMG_NECK, depth_net=DEPTH_NET)
+CONFIG_4D_IMG_BEVDET_NMS = dict(CONFIG_4D_IMG, test=TEST_CFG_BEVDET)
+BDA_IDENTITY = np.eye(3, dtype=np.float32)[None]  # the test pipeline's bda
+
+
+class BEVDet4DFromImages(BEVDet4D, BEVDetFromImages):
+    """BEVDet4D (CONFIG_4D_IMG) from six normalised camera images: BEVDetFromImages's image encoder and
+    p3d_lss_depth_feat_h16 in front of BEVDet4D's view transform, pre_process, shift, encoder, head and postprocess.
+    Batch 1.  Checks what both parents check (num_adj 1, input_size a multiple of 32, downsample 16, data_config's crop
+    equal to input_size).  Seeded weights equal both parents' for the same seed: the image encoder BEVDetFromImages's, the
+    BEV half and pre_process BEVDet4D's.  forward() from the depth net's output is BEVDet4D's; the methods whose
+    signatures differ between the parents are defined here."""
+
+    def __init__(self, model_cfg=None, accelerate=False, device="cuda"):
+        super().__init__(model_cfg or CONFIG_4D_IMG, accelerate, device)
+
+    def encoder_input(self, mats, prev_sensor2keyego, imgs, feat_prev=None):
+        """Eager: the concat rows [Y*X, 2*160] of a frame from imgs [N, 3, H, W] fp32 on the device."""
+        return self.concat_of(self.image_from_images(mats, imgs), mats, prev_sensor2keyego, feat_prev)
+
+    def forward_images(self, mats, prev_sensor2keyego, imgs, feat_prev=None):
+        """Eager frame from imgs [N, 3, H, W] fp32 on the device: ((boxes, scores, labels, counts), bev_feat) as
+        BEVDet4D.forward."""
+        return self.forward_concat(self.encoder_input(mats, prev_sensor2keyego, imgs, feat_prev))
+
+    def forward_frames(self, sensor2ego, cam2imgs, bda, frames, prev_sensor2keyego=None, feat_prev=None):
+        """Eager frame from decoded camera frames [N, H0, W0, 3] uint8 on the device: forward_images on
+        images_from_frames(frames) with test_mats (sensor2ego: this frame's sensor2keyego)."""
+        return self.forward_images(self.test_mats(sensor2ego, cam2imgs, bda), prev_sensor2keyego,
+                                   self.images_from_frames(frames), feat_prev)
+
+    def calibrate_heatmap_bias(self, mats, imgs, target_frac=0.014):
+        """BEVDet.calibrate_heatmap_bias on the start frame of a sequence with these images."""
+        x = self.encoder_input(mats, None, imgs)
+        self.head.calibrate_heatmap_bias(x, self.test_cfg["score_threshold"], target_frac, shape=self.enc_shape)
+        return self
+
+    def flops(self):
+        """BEVDet4D.flops plus BEVDetFromImages's image keys; frame_total = total (pre_process included) + img_total."""
+        out = super().flops()
+        out["frame_total"] = out["total"] + out["img_total"]
+        return out
+
+
+def drive_mats(items, test_mats):
+    """The pose bookkeeping of one drive, on the host: items = (frames, sensor2ego [N, 4, 4], ego2global [N, 4, 4],
+    cam2imgs [N, 3, 3]) per key frame (frames is not read) -> per item (mats, prev_sensor2keyego, new_sequence), what
+    BEVDet4DHotPath.launch takes.  mats = test_mats(sensor2keyego, cam2imgs, bda identity) with the frame's cameras in its
+    own key ego (ops.bev_pool_v2.sensor2keyegos; the current frame's camera 0 defines the key ego); prev_sensor2keyego
+    the previous frame's cameras in this frame's key ego (None on the first item, which starts the sequence)."""
+    prev = None
+    for _, s2e, e2g, k in items:
+        s2e, e2g = np.asarray(s2e, np.float64)[None], np.asarray(e2g, np.float64)[None]
+        curr = bp.sensor2keyegos(s2e, e2g, e2g)
+        prev_s2ke = None if prev is None else bp.sensor2keyegos(prev[0], prev[1], e2g)
+        yield test_mats(curr, np.asarray(k)[None], BDA_IDENTITY), prev_s2ke, prev is None
+        prev = (s2e, e2g)
+
+
+class BEVDet4DImageHotPath(ImageInput, BEVDet4DHotPath):
+    """BEVDet4DHotPath from camera images: both frame graphs ("start", "continue") begin with the image encoder ->
+    p3d_lss_depth_feat_h16 into the lane's depth / feat (ImageInput), then run BEVDet4DHotPath's frame unchanged (pool ->
+    pre_process -> shift -> history copy -> encoder -> head -> postprocess -> D2H).  Each graph holds its own copy of the
+    image encoder's activations (one private pool per graph).  Lanes, history and accelerate as in BEVDet4DHotPath."""
+
+    def __init__(self, model, device="cuda", stream=None):
+        super().__init__(model, device, stream)
+        self._init_images()
+
+    def launch(self, mats, prev_sensor2keyego=None, imgs=None, new_sequence=False):
+        """Enqueue one frame of this lane's sequence: BEVDet4DHotPath.launch with imgs [N, 3, H, W] (a device tensor
+        copied into the frame's input; None: already written there) in place of the depth net's output."""
+        self.check_sequence(new_sequence)
+        self._put_images(imgs)
+        BEVDet4DHotPath.launch(self, mats, prev_sensor2keyego, None, None, new_sequence)
+
+    def infer(self, mats, prev_sensor2keyego=None, imgs=None, new_sequence=False):
+        self.launch(mats, prev_sensor2keyego, imgs, new_sequence)
+        return self.result()
+
+
+class BEVDet4DFrameHotPath(FrameInput, BEVDet4DImageHotPath):
+    """BEVDet4DImageHotPath from decoded camera frames: p3d_image_prep_u8 from the lane's band at the head of both frame
+    graphs (FrameInput; frames as BEVDetFrameHotPath takes them).  infer_stream runs one drive from frames and ego poses
+    with the band's H2D off the critical path."""
+
+    def __init__(self, model, device="cuda", stream=None):
+        self.check_plan(model)
+        super().__init__(model, device, stream)
+        self._init_band()
+        self._copy_stream = None
+
+    def launch_frames(self, sensor2ego, cam2imgs, bda, frames, prev_sensor2keyego=None, new_sequence=False):
+        """Enqueue one frame of this lane's sequence from decoded camera frames [N, H0, W0, 3] uint8 (contiguous; on this
+        device, or in pinned host memory, which must stay unchanged until the frame's result is read); sensor2ego: this
+        frame's sensor2keyego; the rest as BEVDet4DImageHotPath.launch.  Pageable host memory raises ValueError."""
+        self.check_sequence(new_sequence)
+        self.check_frames(frames)
+        mats = self.model.test_mats(sensor2ego, cam2imgs, bda)
+        self._put_frames(frames)
+        self.launch(mats, prev_sensor2keyego, None, new_sequence)
+
+    def infer_frames(self, sensor2ego, cam2imgs, bda, frames, prev_sensor2keyego=None, new_sequence=False):
+        self.launch_frames(sensor2ego, cam2imgs, bda, frames, prev_sensor2keyego, new_sequence)
+        return self.result()
+
+    def infer_stream(self, items):
+        """One drive: items = (frames [N, H0, W0, 3] uint8 pinned, sensor2ego [N, 4, 4], ego2global [N, 4, 4], cam2imgs
+        [N, 3, 3]) per key frame, in order (frames as launch_frames takes them; each must stay unchanged until its result
+        is yielded).  The first item starts a sequence; bda is the identity; the matrices come from drive_mats.  Yields
+        (boxes, scores, labels) per item, in order, as clones.
+
+        The band of item j + 1 is copied on a copy stream into one of two device staging bands while frame j computes
+        (the copy is enqueued before the host waits for frame j), then moved into the lane's band by one D2D copy on the
+        lane's stream just before its replay; events order the reuse of each staging band (frame.in_flight's schedule on
+        one lane, its slot being the staging band)."""
+        if not self.graphs:
+            raise RuntimeError("infer_stream needs a captured lane: call capture() first")
+        if self._copy_stream is None:
+            self._copy_stream = torch.cuda.Stream(self.device)
+            self._staging = [torch.empty_like(self.band) for _ in range(2)]
+            self._staged = [torch.cuda.Event() for _ in range(2)]    # H2D into staging[k] done
+            self._consumed = [torch.cuda.Event() for _ in range(2)]  # staging[k] copied into the lane's band
+        a, b = itertools.tee(items)
+        plans = zip((item[0] for item in a), drive_mats(b, self.model.test_mats))
+        steps, held = {}, {}  # item -> its matrices until launched; its frames until its result is read
+        for kind, i, plan, _, k in in_flight(plans, 1):
+            if kind == "submit":
+                held[i], steps[i] = plan
+                self._stage(held[i], k, first_use=i < 2)
+                if i == 0:
+                    self._launch_staged(steps.pop(0), k)
+            else:
+                out = self.slot.read(self.check_status, self.done, clone=True)
+                del held[i]
+                if i + 1 in steps:
+                    self._launch_staged(steps.pop(i + 1), k ^ 1)
+                yield out
+
+    def _stage(self, frames, k, first_use):
+        """Check the frames of one item and enqueue the H2D of their band into staging band k on the copy stream."""
+        self.check_frames(frames)
+        cs = self._copy_stream
+        with torch.cuda.stream(cs):
+            if not first_use:
+                cs.wait_event(self._consumed[k])
+            self.copy_band(frames, out=self._staging[k])
+            if frames.is_cuda:
+                frames.record_stream(cs)
+            self._staged[k].record(cs)
+
+    def _launch_staged(self, step, k):
+        """Launch the frame whose band is in staging band k: wait for its H2D, one D2D copy into the lane's band on the
+        lane's stream, then the replay (BEVDet4DImageHotPath.launch).  step = (mats, prev_sensor2keyego, new_sequence)."""
+        mats, prev, new_sequence = step
+        st = self.stream
+        st.wait_stream(torch.cuda.current_stream(self.device))
+        with torch.cuda.stream(st):  # after the lane's previous frame, which read the band
+            st.wait_event(self._staged[k])
+            self.band.copy_(self._staging[k], non_blocking=True)
+            self._consumed[k].record(st)
+        self.launch(mats, prev, None, new_sequence)

@@ -3,6 +3,7 @@
 
   python tools/bevdet_bench.py [--steps K] [--warmup W] [--in-flight L] [--no-cpu-check] [--dump-outputs DIR]
   python tools/bevdet_bench.py --temporal [--steps K] [--warmup W] [--in-flight L] [--rounds R] [--no-cpu-check]
+  python tools/bevdet_bench.py --temporal --images | --raw-images [--steps K] [--warmup W] [--in-flight L] [--rounds R]
   python tools/bevdet_bench.py --bevdet-nms [--temporal] [--steps K] [--warmup W] [--in-flight L] [--rounds R]
 
 A frame = six cameras of 16 x 44 features (D = 118, C = 80) -> LSS view transform into the 128 x 128 x 96 pixel fp16-pair
@@ -33,6 +34,19 @@ band's H2D included, next to BEVDetImageHotPath on resident fp32 images, in roun
 rounds): frames/s in flight and one at a time; the host baseline (Pillow + OpenCV prep of the six cameras, one thread,
 timed on this host); the graph-timed prep kernel with its algorithmic bytes and GB/s; the band's H2D bytes and time; the
 node counts of both frame graphs; the card; and a frame-0 check that the device images equal the host pipeline's.
+
+--temporal --images: BEVDet4D from six normalised 256 x 704 camera images (bevdet.BEVDet4DImageHotPath: the image encoder
+and lss_depth_feat_h16 at the head of both the start and the continue graph) next to BEVDet4DHotPath fed that frame's own
+depth-net output (merged fp32 logits / tran_feat), in rounds that alternate the two (median of the rounds): frames/s with
+--in-flight lanes on independent drives and one at a time; the node counts of the start and continue graphs; the device
+memory reserved per lane by its buffers and by capture(); the card; and a frame-0 check against the CPU arm
+(bevdet_images_oracle.CpuBEVDetImages.image_encoder -> bevdet4d_oracle.CpuBEVDet4D, tests/).
+
+--temporal --raw-images: BEVDet4D from six decoded 900 x 1600 uint8 camera frames (bevdet.BEVDet4DFrameHotPath) fed from
+pinned host memory, the band's H2D included, next to BEVDet4DImageHotPath on resident fp32 images (frames/s in flight and
+one at a time); infer_stream over one drive of --steps key frames next to a loop of launch_frames + result over the same
+items (frames/s); the node counts of the start and continue graphs; memory per lane; the band's H2D bytes and time; the
+card.  Rounds alternate the arms (median of the rounds).
 
 --bevdet-nms: the frames with BEVDet's own box decode (bevdet.CONFIG_BEVDET_NMS, with --temporal CONFIG_4D_BEVDET_NMS:
 top-K over class x cell, per-class scale-NMS / circle NMS) next to the same weights with the default decode
@@ -91,6 +105,8 @@ def main():
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("bevdet_bench.py needs a CUDA device (no CPU fallback exists)")
+    if args.temporal and (args.images or args.raw_images):
+        return temporal_images(args)
     if args.raw_images:
         return raw_images(args)
     if args.images:
@@ -558,6 +574,181 @@ def raw_images(args):
                         "GB_per_s": plan.band_bytes(n) / (h2d_ms * 1e-3) / 1e9,
                         "full_fp32_images_bytes": plan.out_bytes(n)}
     line["value"] = line["frames"]["fps_in_flight"]
+    print(json.dumps(line))
+
+
+def _lanes(make, n):
+    """n captured lanes (make() builds one) and the device memory each reserved: by its buffers, then by capture() (its
+    graphs' private pools; the first lane's also holds the warm-up's cached blocks, which later lanes reuse)."""
+    import torch
+    lanes, mem = [], []
+    for i in range(n):
+        torch.cuda.synchronize()
+        r0 = torch.cuda.memory_reserved()
+        ln = make()
+        r1 = torch.cuda.memory_reserved()
+        ln.capture(count_nodes=i == 0)
+        torch.cuda.synchronize()
+        r2 = torch.cuda.memory_reserved()
+        lanes.append(ln)
+        mem.append({"buffers_MiB": (r1 - r0) / 2 ** 20, "capture_MiB": (r2 - r1) / 2 ** 20})
+    return lanes, mem
+
+
+def temporal_images(args):
+    import torch
+    from paddle3d_b200 import bevdet as bd
+    from paddle3d_b200 import synth
+    from paddle3d_b200.frame import count_graph_nodes
+    from paddle3d_b200.ops import bev_pool_v2 as bp
+    from paddle3d_b200.ops import dense_conv as dc
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    m = bd.BEVDet4DFromImages(device=dev).init_weight(seed=args.seed, bn_gain=BN_GAIN)
+    vt = m.vt
+    # one drive of pinned camera frames on a rig turning at 0.15 rad per 0.5 s key frame (drive_mats' matrices); the
+    # lanes run it independently, each starting its sequence on its first frame
+    rig = synth.camera_rig(args.seed, bda=False)
+    L = 8
+    frames_host = [torch.from_numpy(synth.camera_frames(args.seed + i)).pin_memory() for i in range(2)]
+    items = [(frames_host[k % 2], rig["sensor2ego"][0], np.broadcast_to(p, (m.N, 4, 4)).copy(), rig["cam2imgs"][0])
+             for k, p in enumerate(synth.ego_poses(L, speed=10.0, yaw_rate=0.3))]
+    steps = list(bd.drive_mats(items, m.test_mats))
+    imgs = m.images_from_frames(frames_host[0].to(dev))
+    imgs_np = imgs.cpu().numpy()
+    m.calibrate_heatmap_bias(steps[0][0], imgs)
+    rows, rshape = m.image_encoder(imgs)
+    d = dc.pixel_h16_to_nchw(rows, rshape)
+    logits, tran = d[:, :vt.D].contiguous(), d[:, vt.D:vt.D + vt.out_channels].contiguous()
+    raw = args.raw_images
+    src = ("decoded 900 x 1600 uint8 camera frames in pinned host memory (band H2D -> resize / crop / normalise -> "
+           if raw else "256 x 704 camera images (")
+    line = {"metric": "BEVDet4D sequential frames/s from six " + src + "ResNet-50 + CustomFPN + depth net -> LSS -> "
+                      "pre_process + shift of the previous BEV -> CustomResNet(160) + FPN_LSS -> CenterHead -> boxes)",
+            "unit": "frames/s", "gpu": gpu_identity(0), "steps": args.steps, "warmup": args.warmup,
+            "gflop": {k: v / 1e9 for k, v in m.flops().items()}}
+    lanes_n = max(1, args.in_flight)
+    if raw:
+        arms = {"frames": bd.BEVDet4DFrameHotPath, "images": bd.BEVDet4DImageHotPath}
+    else:
+        arms = {"images": bd.BEVDet4DImageHotPath, "depth_net_output": bd.BEVDet4DHotPath}
+    runs, mem = {}, {}
+    for name, cls in arms.items():
+        runs[name], mem[name] = _lanes(lambda: cls(m, device=dev), lanes_n)
+    for ln in runs["images"]:  # resident inputs: the timed frames replay on them
+        ln.imgs.copy_(imgs)
+    for ln in runs.get("depth_net_output", []):
+        ln.logits.copy_(logits)
+        ln.tran_feat.copy_(tran)
+    torch.cuda.synchronize()
+    count = {}
+
+    def launch(name, lane_i, lane):
+        k = count.get((name, lane_i), 0)
+        count[(name, lane_i)] = k + 1
+        mats, prev, _ = steps[0 if k == 0 else 1 + (k - 1) % (L - 1)]
+        if name == "frames":
+            it = items[k % L]
+            lane.launch_frames(mats[0], mats[1], mats[4], it[0], prev, k == 0)
+        elif name == "images":
+            lane.launch(mats, prev, None, k == 0)
+        else:
+            lane.launch(mats, prev, None, None, k == 0)
+
+    def one(name, lane):
+        launch(name, 0, lane)
+        lane.result()
+    rates = {n: {"fps_in_flight": [], "fps_one_at_a_time": []} for n in runs}
+    for name, lanes in runs.items():
+        for i in range(args.warmup):
+            launch(name, i % lanes_n, lanes[i % lanes_n])
+    torch.cuda.synchronize()
+    if raw:  # one drive of --steps key frames: infer_stream against launch_frames + result per item
+        drive = [(frames_host[k % 2], rig["sensor2ego"][0], np.broadcast_to(p, (m.N, 4, 4)).copy(), rig["cam2imgs"][0])
+                 for k, p in enumerate(synth.ego_poses(args.steps, speed=10.0, yaw_rate=0.3))]
+        plan = list(bd.drive_mats(drive, m.test_mats))
+        stream_lane = runs["frames"][0]
+
+        def loop():
+            for it, (mats, prev, new) in zip(drive, plan):
+                stream_lane.infer_frames(mats[0], mats[1], mats[4], it[0], prev, new)
+
+        def drive_rate(fn):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            fn()
+            torch.cuda.synchronize()
+            return len(drive) / (time.perf_counter() - t0)
+        rates["drive"] = {"infer_stream": [], "launch_frames_result_loop": []}
+        for _ in stream_lane.infer_stream(drive[:args.warmup]):
+            pass
+    for _ in range(max(1, args.rounds)):  # alternate the arms so that clocks and temperature drift hit both
+        for name, lanes in runs.items():
+            rates[name]["fps_in_flight"].append(
+                _rate(lambda i: launch(name, i % lanes_n, lanes[i % lanes_n]), torch.cuda.synchronize, args.steps))
+            rates[name]["fps_one_at_a_time"].append(
+                _rate(lambda i: one(name, lanes[0]), torch.cuda.synchronize, args.steps))
+        if raw:
+            rates["drive"]["infer_stream"].append(drive_rate(lambda: [None for _ in stream_lane.infer_stream(drive)]))
+            rates["drive"]["launch_frames_result_loop"].append(drive_rate(loop))
+    for name, lanes in runs.items():
+        for ln in lanes:
+            ln.result()  # raises on an fp16-range overflow
+        r = {k: float(np.median(v)) for k, v in rates[name].items()}
+        r.update(rounds=rates[name], lanes=lanes_n, memory_reserved_per_lane=mem[name],
+                 graph_nodes={g: count_graph_nodes(x) for g, x in lanes[0].graphs.items()})
+        line[name] = r
+    if raw:
+        line["drive"] = dict({k: float(np.median(v)) for k, v in rates["drive"].items()}, rounds=rates["drive"],
+                             key_frames=len(drive), note="frames/s of one drive on one lane; frames of a drive are serial")
+    line["note_lanes"] = "lanes run independent drives (each owns its history); frames of one drive are serial"
+    hot = runs["images"][0]
+    got = [t.clone().numpy() for t in hot.infer(steps[0][0], None, imgs, new_sequence=True)]
+    line["boxes_frame0"] = int(len(got[0]))
+    if raw:
+        plan_ = m.prep_plan
+        st = torch.cuda.Stream(dev)
+        fh = runs["frames"][0]
+        with torch.cuda.stream(st):
+            fh.copy_band(frames_host[0])
+            st.synchronize()
+            s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            s.record(st)
+            for _ in range(20):
+                fh.copy_band(frames_host[0])
+            e.record(st)
+        e.synchronize()
+        h2d_ms = s.elapsed_time(e) / 20
+        line["band_h2d"] = {"bytes_per_frame": plan_.band_bytes(m.N), "ms": h2d_ms,
+                            "GB_per_s": plan_.band_bytes(m.N) / (h2d_ms * 1e-3) / 1e9}
+        line["value"] = line["frames"]["fps_in_flight"]
+        print(json.dumps(line))
+        return
+    if not args.no_cpu_check:
+        sys.path.insert(0, os.path.join(ROOT, "tests"))
+        from bevdet4d_oracle import CpuBEVDet4D
+        from bevdet_images_oracle import CpuBEVDetImages
+        w = m.export_numpy()
+        mats = steps[0][0]
+        cams = bp.unpack_cameras(bp.pack_cameras(*mats), 1, m.N)
+        axes = tuple(a.numpy() for a in vt.axes_host)
+        t0 = time.perf_counter()
+        cl, ct = CpuBEVDetImages(w, m.test_cfg, m.label_off).image_encoder(imgs_np)
+        cpu = CpuBEVDet4D(w, m.test_cfg, m.label_off).run(cams, axes, cl, ct, *vt.grid_args(),
+                                                          np.asarray(mats[0], np.float64),
+                                                          np.asarray(mats[4], np.float64), new_sequence=True)
+        s = time.perf_counter() - t0
+        paired = 0
+        for i in range(len(cpu["boxes"])):
+            if not len(got[0]):
+                break
+            j = int(np.argmin(np.abs(got[0][:, :3] - cpu["boxes"][i, :3]).max(1)))
+            e = (np.abs(got[0][j] - cpu["boxes"][i]) / np.maximum(1.0, np.abs(cpu["boxes"][i]))).max()
+            paired += int(e <= 1e-3 and got[2][j] == cpu["labels"][i])
+        line["cpu_check_frame0"] = {"gpu_boxes": int(len(got[0])), "cpu_boxes": int(len(cpu["boxes"])),
+                                    "paired_frac": paired / max(1, len(cpu["boxes"])), "cpu_oracle_s": s,
+                                    "kind": "fp64-accumulating numpy + OpenMP oracle, not a tuned CPU implementation"}
+    line["value"] = line["images"]["fps_in_flight"]
     print(json.dumps(line))
 
 
