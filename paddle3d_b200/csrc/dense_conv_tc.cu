@@ -6,8 +6,10 @@
 // the row format of the sparse-conv layers with row = pixel), so a 3x3 tap of 32 input channels for a 16 x 8 pixel
 // tile is one 4-D TMA box {32 ch, 16 x, 8 y, 1 b} at the shifted coordinate: zero padding is the tensor map's
 // out-of-bounds fill, a stride-2 conv is the map's element stride, and the box lands in shared memory as the
-// SWIZZLE_128B K-major operand tile (128 rows x 128 B).  3xTF32: A_hi x B_hi into one register accumulator,
-// A_lo x B_hi + A_hi x B_lo into a second (warpgroup g: rows 64g .. 64g+63 of the tile), weights of the use by cp.async.bulk,
+// SWIZZLE_128B K-major operand tile (128 rows x 128 B).  3xTF32: A_hi x B_hi into one register accumulator (one tap's
+// partial, added to an fp32 register total with round-to-nearest FADDs after the tap's last channel group: the tensor
+// core's own accumulation drifts over a whole 9 x Cin / 8 k-step chain), A_lo x B_hi + A_hi x B_lo into a second
+// (warpgroup g: rows 64g .. 64g+63 of the tile), weights of the use by cp.async.bulk,
 // BN/bias/ReLU epilogue writing split rows (at a column offset: channel concat for free) or fp32 NCHW planes (the head
 // outputs centerpoint_postprocess reads).
 //
@@ -130,12 +132,12 @@ __global__ void __launch_bounds__(kThreads, Cfg<N>::MIN_CTAS)
              static_cast<uint32_t>(C::B_STAGE), bar);
   };
   long long next = 0;  // thread 0: next step to load
-  float acc[C::ACC], accx[C::ACC];  // hi x hi | cross terms
+  float acc[C::ACC], accx[C::ACC], tot[C::ACC];  // hi x hi of the current tap | cross terms | hi x hi of done taps
   long long q = 0;
   for (long long w = blockIdx.x; w < n_work; w += gridDim.x) {
     const Item im = decode(w, p);
 #pragma unroll
-    for (int i = 0; i < C::ACC; ++i) acc[i] = accx[i] = 0.f;
+    for (int i = 0; i < C::ACC; ++i) acc[i] = accx[i] = tot[i] = 0.f;
     for (int u = 0; u < n_uses; ++u, ++q) {
       __syncthreads();  // the wgmma of step q - 1 have retired in both warpgroups: its slot is free
       if (tid == 0)
@@ -144,6 +146,7 @@ __global__ void __launch_bounds__(kThreads, Cfg<N>::MIN_CTAS)
       mbar_wait(smem_u32(&s_full[slot]), static_cast<uint32_t>((q / S) & 1));
       const uint32_t a_hi = ring + slot * C::STAGE + static_cast<uint32_t>(wg * 64 * 128), a_lo = a_hi + C::A_TILE;
       const uint32_t b_hi = ring + slot * C::STAGE + C::A_STAGE, b_lo = b_hi + N * 16;  // rows 0..N-1 = hi, N..2N-1 = lo
+      const uint32_t tap_first = (u % G) == 0;  // the tap's hi x hi partial starts over (scale_d = 0)
       wg_fence();
 #pragma unroll
       for (int j = 0; j < C::KC / 8; ++j) {
@@ -152,12 +155,16 @@ __global__ void __launch_bounds__(kThreads, Cfg<N>::MIN_CTAS)
         const uint64_t dbh = smem_desc(b_hi + bo, 2 * N * 16, 128), dbl = smem_desc(b_lo + bo, 2 * N * 16, 128);
         wg::mma_tf32<N>(accx, dal, dbh, 1u);
         wg::mma_tf32<N>(accx, dah, dbl, 1u);
-        wg::mma_tf32<N>(acc, dah, dbh, 1u);
+        wg::mma_tf32<N>(acc, dah, dbh, (tap_first && j == 0) ? 0u : 1u);
       }
       wg_commit();
       wg_wait<0>();
+      if (u % G == G - 1) {  // last channel group of the tap: its partial joins the total
+        wg_fence_acc<C::ACC>(acc);
+#pragma unroll
+        for (int i = 0; i < C::ACC; ++i) tot[i] += acc[i];
+      }
     }
-    wg_fence_acc<C::ACC>(acc);
     wg_fence_acc<C::ACC>(accx);
 
     // ---------------------------------------------------------------- epilogue (accumulator fragment)
@@ -172,7 +179,7 @@ __global__ void __launch_bounds__(kThreads, Cfg<N>::MIN_CTAS)
       float o[2];
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
-        float v = accx[i + e] + acc[i + e];
+        float v = accx[i + e] + tot[i + e];
         if (ch + e < p.cout) {
           if (scale) v = v * __ldg(scale + ch + e);
           if (shift) v = v + __ldg(shift + ch + e);

@@ -18,7 +18,11 @@
 //               STAGES - 1 uses ahead; thread 0 copies the packed [hi | lo] weight slice of the use with cp.async.bulk
 //               (mbarrier complete_tx).
 //   mma         3 wgmma kind tf32 per 8-wide k-step: lo x hi + hi x lo into one accumulator, hi x hi into a second one
-//               (the small cross terms keep their own rounding; the epilogue adds the two).
+//               (the small cross terms keep their own rounding; the epilogue adds the two).  The hi x hi accumulator
+//               holds one tap's partial sum only: after a tap's last channel chunk it is added to an fp32 register
+//               total with round-to-nearest FADDs.  The tensor core's own accumulation is not round-to-nearest, so one
+//               chain of 27 x Cin / 8 k-steps drifts (H100, 128 -> 128, K = 27: 1.5e-4 relative at 1e-2 x max, against
+//               1.4e-5 with the per-tap total); per tap, both row layouts still run the same sums.
 //   epilogue    BN scale/shift (+bias), residual, ReLU from the accumulator fragment.
 //   split-K     the wide layers (Cout >= 64) have few 128-row tiles (52 - 130 at the C3 sizes): given a workspace, their
 //               taps are spread over 2 CTAs per tile (split s owns the taps t == s mod splits), which write raw partial
@@ -202,9 +206,9 @@ __global__ void __launch_bounds__(kThreads, Cfg<CIN, COUT, SPLIT_ROWS>::MIN_CTAS
       }
     };
 
-    float acc[C::ACC], accx[C::ACC];  // hi x hi | cross terms
+    float acc[C::ACC], accx[C::ACC], tot[C::ACC];  // hi x hi of the current tap | cross terms | hi x hi of done taps
 #pragma unroll
-    for (int i = 0; i < C::ACC; ++i) acc[i] = accx[i] = 0.f;
+    for (int i = 0; i < C::ACC; ++i) acc[i] = accx[i] = tot[i] = 0.f;
     for (int q = 0; q < S - 1; ++q) {
       issue(q);
       if constexpr (SPLIT_ROWS) cp_async_commit();
@@ -217,6 +221,7 @@ __global__ void __launch_bounds__(kThreads, Cfg<CIN, COUT, SPLIT_ROWS>::MIN_CTAS
       __syncthreads();      // whole stage present; the wgmma of use u - 1 have retired in both warpgroups
       const uint32_t a_hi = ring + slot * C::STAGE + static_cast<uint32_t>(wg * 64 * (C::KC * 4)), a_lo = a_hi + C::A_TILE;
       const uint32_t b_hi = ring + slot * C::STAGE + C::A_STAGE, b_lo = b_hi + COUT * 16;  // rows 0..N-1 = hi, N..2N-1 = lo
+      const uint32_t tap_first = (u % C::G) == 0;  // the tap's hi x hi partial starts over (scale_d = 0)
       wg_fence();
 #pragma unroll
       for (int j = 0; j < C::KC / 8; ++j) {
@@ -227,14 +232,18 @@ __global__ void __launch_bounds__(kThreads, Cfg<CIN, COUT, SPLIT_ROWS>::MIN_CTAS
         const uint64_t dbh = smem_desc(b_hi + bo, 2 * COUT * 16, 128), dbl = smem_desc(b_lo + bo, 2 * COUT * 16, 128);
         wg::mma_tf32<COUT>(accx, dal, dbh, 1u);  // A_lo x B_hi
         wg::mma_tf32<COUT>(accx, dah, dbl, 1u);  // A_hi x B_lo
-        wg::mma_tf32<COUT>(acc, dah, dbh, 1u);   // A_hi x B_hi
+        wg::mma_tf32<COUT>(acc, dah, dbh, (tap_first && j == 0) ? 0u : 1u);  // A_hi x B_hi
       }
       wg_commit();
       issue(u + S - 1);  // the slot of use u - 1
       if constexpr (SPLIT_ROWS) cp_async_commit();
       wg_wait<0>();
+      if (u % C::G == C::G - 1) {  // last chunk of the tap: its partial joins the total
+        wg_fence_acc<C::ACC>(acc);
+#pragma unroll
+        for (int i = 0; i < C::ACC; ++i) tot[i] += acc[i];
+      }
     }
-    wg_fence_acc<C::ACC>(acc);
     wg_fence_acc<C::ACC>(accx);
     if constexpr (SPLIT_ROWS) cp_async_wait<0>();
     gu += static_cast<uint32_t>(n_uses);
@@ -245,7 +254,7 @@ __global__ void __launch_bounds__(kThreads, Cfg<CIN, COUT, SPLIT_ROWS>::MIN_CTAS
       const int r = wg * 64 + frag_row(i, wtid), c = frag_col(i, wtid);
       if (r >= rows) continue;
       const size_t orow = static_cast<size_t>(row0 + r);
-      float o[2] = {accx[i] + acc[i], accx[i + 1] + acc[i + 1]};
+      float o[2] = {accx[i] + tot[i], accx[i + 1] + tot[i + 1]};
       float res[2] = {0.f, 0.f};
       if (residual) {
         if constexpr (SPLIT_ROWS) {
