@@ -610,6 +610,40 @@ int p3d_merge_sweeps(const float *raw, int num_slots, int64_t slot_cap, int raw_
                      float sweep_remove_radius, float *out, int64_t cap, int32_t *n_out_dev, int32_t *status_dev,
                      void *workspace, size_t workspace_bytes, p3d_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Baseline JPEG decode to uint8 RGB rows, bit-identical to libjpeg-turbo's C paths (jpeg_idct_islow, fancy upsampling,
+ * ycc_rgb_convert) that PIL.Image.open runs.  Supported: SOF0 / SOF1 Huffman DCT, 8-bit, three components Y Cb Cr in
+ * one interleaved scan, chroma 1x1 and luma 1x1, 2x1 or 2x2, any restart interval and tables.  The host reads the
+ * markers (paddle3d_b200/ops/jpeg.parse) and fills one p3d_jpeg_desc per image; every size, offset and table is read on
+ * the device, so a captured graph serves any compressed lengths and tables.
+ *   data [data_bytes] uint8: the concatenated files; desc [N] (device).  Every image is H x W (desc->height / width).
+ *   out [N][y1 - y0][W][3] uint8: rows [y0, y1) of every image.  status_dev [N] int32 (device), one word per image:
+ *   bits are OR-ed in and never cleared here: 1 = an undefined Huffman code or a run past coefficient 63, 2 = a restart marker out of
+ *   sequence, missing or misplaced, 4 = the data ends before the last MCU, 8 = a marker other than RSTn (or a fill byte)
+ *   in the entropy-coded segment, 16 = a descriptor disagrees with the call (size, sampling, a segment outside data or
+ *   longer than max_bytes; that image is not decoded).  Corrupt data never reads outside its segment.
+ *   workspace: p3d_jpeg_decode_workspace_bytes(N, H, W, max_bytes) bytes, max_bytes = the largest entropy-coded
+ *   segment.  No allocation, no host synchronisation.
+ * Null pointers, a size < 1 or rows outside [0, H): P3D_ERR_INVALID_ARG.  N > 64, H or W > 8192 or max_bytes > 2^28:
+ * P3D_ERR_UNSUPPORTED.
+ * ------------------------------------------------------------------------------------------- */
+#define P3D_JPEG_MAX_IMAGES 64
+#define P3D_JPEG_MAX_SIDE 8192
+typedef struct p3d_jpeg_desc {
+  int64_t offset;            /* first byte of the entropy-coded segment in data */
+  int32_t length;            /* its bytes, up to the EOI marker */
+  int32_t height, width;
+  int32_t hs, vs;            /* luma sampling factors (chroma 1 x 1) */
+  int32_t restart_interval;  /* MCUs per restart interval, 0 = none */
+  uint16_t quant[3][64];     /* per component, natural order */
+  uint8_t dc_bits[3][16], dc_vals[3][16], ac_bits[3][16], ac_vals[3][256]; /* per component: BITS / HUFFVAL */
+} p3d_jpeg_desc;
+
+size_t p3d_jpeg_decode_workspace_bytes(int N, int H, int W, int64_t max_bytes);
+int p3d_jpeg_decode_u8(const uint8_t *data, int64_t data_bytes, const p3d_jpeg_desc *desc, int N, int H, int W, int y0,
+                       int y1, int64_t max_bytes, uint8_t *out, int32_t *status_dev, void *workspace,
+                       size_t workspace_bytes, p3d_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

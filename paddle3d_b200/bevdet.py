@@ -37,6 +37,7 @@ from .ops import bevdet_postprocess as bdp
 from .ops import centerpoint_postprocess as cpp
 from .ops import dense_conv as dc
 from .ops import image_prep as ip
+from .ops import jpeg
 from .ops import sparse_nn as sp
 
 # PARITY UNPINNED (see the module docstring)
@@ -1080,5 +1081,165 @@ class BEVDet4DFrameHotPath(FrameInput, BEVDet4DImageHotPath):
         with torch.cuda.stream(st):  # after the lane's previous frame, which read the band
             st.wait_event(self._staged[k])
             self.band.copy_(self._staging[k], non_blocking=True)
+            self._consumed[k].record(st)
+        self.launch(mats, prev, None, new_sequence)
+
+
+# ------------------------------------------------------------------------------------------ from JPEG camera files
+class JpegInput(FrameInput):
+    """FrameInput from the bytes of N JPEG files (ops/jpeg): the lane's _depth_feat stage clears the lane's JPEG status
+    words, decodes the plan's band of every camera from the lane's byte buffer into the band (p3d_jpeg_decode_u8,
+    bit-identical to Pillow's decode), copies the status words back with the frame, then runs FrameInput's stage.  The
+    compressed bytes and the descriptors go H2D from pinned staging before the replay; one graph serves any compressed
+    lengths and tables.  max_bytes: the lane's capacity per camera file.  A corrupt file fails that frame's result()
+    with a RuntimeError naming the camera; the lane's next frame is unaffected."""
+
+    DEFAULT_MAX_BYTES = 2 << 20
+
+    def _init_jpeg(self, max_bytes):
+        self.jpeg_max_bytes = int(max_bytes)
+        if self.jpeg_max_bytes < 1:
+            raise ValueError("%s: max_bytes %d" % (type(self).__name__, self.jpeg_max_bytes))
+        N = self.model.N
+        dev = self.device
+        self.jpeg_data = torch.zeros((N * self.jpeg_max_bytes,), dtype=torch.uint8, device=dev)
+        self.jpeg_desc = torch.zeros((N * jpeg.DESC_DTYPE.itemsize,), dtype=torch.uint8, device=dev)
+        self.jpeg_status = torch.zeros((N,), dtype=torch.int32, device=dev)
+        self.h_jpeg_data = torch.empty((N * self.jpeg_max_bytes,), dtype=torch.uint8).pin_memory()
+        self.h_jpeg_desc = torch.empty((N * jpeg.DESC_DTYPE.itemsize,), dtype=torch.uint8).pin_memory()
+        self.h_jpeg_status = torch.zeros((N,), dtype=torch.int32).pin_memory()
+        self._jpeg_copied = None  # event after the last H2D from the pinned staging
+
+    def _depth_feat(self):
+        plan = self.model.prep_plan
+        self.jpeg_status.zero_()
+        jpeg.jpeg_decode_u8(self.jpeg_data, self.jpeg_desc, self.model.N, plan.src_size, rows=plan.band, out=self.band,
+                            status=self.jpeg_status, max_bytes=self.jpeg_max_bytes)
+        self.h_jpeg_status.copy_(self.jpeg_status, non_blocking=True)
+        super()._depth_feat()
+
+    def check_status(self, status_host):
+        bad = [(i, int(s)) for i, s in enumerate(self.h_jpeg_status.tolist()) if s]
+        if bad:
+            raise RuntimeError("%s: JPEG decode failed: %s" % (type(self).__name__, "; ".join(
+                "camera %d: corrupt data (status 0x%x: %s)" % (i, s, jpeg.status_reason(s)) for i, s in bad)))
+        super().check_status(status_host)
+
+    def pack_jpegs(self, jpegs, data=None, desc=None):
+        """Parse N JPEG files (bytes or uint8 numpy arrays) and write their bytes and descriptors into the pinned
+        buffers data / desc (default: the lane's, once its previous H2D has read them).  Returns the bytes used.  ValueError (nothing enqueued) for a rejected
+        header, a size other than the plan's src_size, a wrong count or a file longer than max_bytes."""
+        name = type(self).__name__
+        N = self.model.N
+        if len(jpegs) != N:
+            raise ValueError("%s: %d JPEG files, want %d" % (name, len(jpegs), N))
+        blobs = [f if isinstance(f, bytes) else (f.tobytes() if isinstance(f, np.ndarray) else bytes(f)) for f in jpegs]
+        for i, b in enumerate(blobs):
+            if len(b) > self.jpeg_max_bytes:
+                raise ValueError("%s: camera %d: %d bytes exceed the lane's capacity of %d per file"
+                                 % (name, i, len(b), self.jpeg_max_bytes))
+        if data is None:
+            data, desc = self.h_jpeg_data, self.h_jpeg_desc
+            if self._jpeg_copied is not None:
+                self._jpeg_copied.synchronize()  # the previous H2D from the lane's staging has read it
+        try:
+            raw_data, d, _ = jpeg.batch(blobs, self.model.prep_plan.src_size, out=data.numpy())
+        except ValueError as e:
+            raise ValueError("%s: %s" % (name, e)) from None
+        desc.numpy()[:] = d.view(np.uint8)
+        return len(raw_data)
+
+    def _put_jpegs(self, nbytes):
+        """Enqueue the H2D of the packed bytes and descriptors into the lane's buffers on its stream."""
+        self.stream.wait_stream(torch.cuda.current_stream(self.device))
+        with torch.cuda.stream(self.stream):  # after the lane's previous frame, which read the buffers
+            self.jpeg_data[:nbytes].copy_(self.h_jpeg_data[:nbytes], non_blocking=True)
+            self.jpeg_desc.copy_(self.h_jpeg_desc, non_blocking=True)
+            self._jpeg_copied = torch.cuda.Event()
+            self._jpeg_copied.record(self.stream)
+
+
+class BEVDetJpegHotPath(JpegInput, BEVDetFrameHotPath):
+    """BEVDetFrameHotPath from the bytes of six JPEG camera files: the captured frame starts with the device JPEG decode
+    of the prep plan's band into the lane's band (JpegInput), then runs BEVDetFrameHotPath's frame.  Lanes, share_model
+    and accelerate as in BEVDetFrameHotPath."""
+
+    def __init__(self, model, device="cuda", stream=None, max_bytes=JpegInput.DEFAULT_MAX_BYTES):
+        super().__init__(model, device, stream)
+        self._init_jpeg(max_bytes)
+
+    def launch_jpegs(self, sensor2ego, cam2imgs, bda, jpegs):
+        """Enqueue one frame from N JPEG files (bytes or uint8 numpy arrays, in camera order); the camera matrices as
+        test_mats takes them.  The files are parsed and copied to pinned staging here (ValueError before anything is
+        enqueued when one is rejected or too long)."""
+        nbytes = self.pack_jpegs(jpegs)
+        mats = self.model.test_mats(sensor2ego, cam2imgs, bda)
+        self._put_jpegs(nbytes)
+        self._launch(mats, None, None, "frame")
+
+    def infer_jpegs(self, sensor2ego, cam2imgs, bda, jpegs):
+        self.launch_jpegs(sensor2ego, cam2imgs, bda, jpegs)
+        return self.result()
+
+
+class BEVDet4DJpegHotPath(JpegInput, BEVDet4DFrameHotPath):
+    """BEVDet4DFrameHotPath from the bytes of six JPEG camera files (JpegInput at the head of both frame graphs).
+    infer_stream runs one drive from JPEG files and ego poses with the H2D of the next item's bytes on a copy stream
+    while the current frame computes."""
+
+    def __init__(self, model, device="cuda", stream=None, max_bytes=JpegInput.DEFAULT_MAX_BYTES):
+        super().__init__(model, device, stream)
+        self._init_jpeg(max_bytes)
+
+    def launch_jpegs(self, sensor2ego, cam2imgs, bda, jpegs, prev_sensor2keyego=None, new_sequence=False):
+        """Enqueue one frame of this lane's sequence from N JPEG files; the rest as BEVDet4DFrameHotPath.launch_frames."""
+        self.check_sequence(new_sequence)
+        nbytes = self.pack_jpegs(jpegs)
+        mats = self.model.test_mats(sensor2ego, cam2imgs, bda)
+        self._put_jpegs(nbytes)
+        self.launch(mats, prev_sensor2keyego, None, new_sequence)
+
+    def infer_jpegs(self, sensor2ego, cam2imgs, bda, jpegs, prev_sensor2keyego=None, new_sequence=False):
+        self.launch_jpegs(sensor2ego, cam2imgs, bda, jpegs, prev_sensor2keyego, new_sequence)
+        return self.result()
+
+    def infer_stream(self, items):
+        """One drive: items = (jpegs, sensor2ego [N, 4, 4], ego2global [N, 4, 4], cam2imgs [N, 3, 3]) per key frame, in
+        order; BEVDet4DFrameHotPath.infer_stream's schedule, the staged payload being the files' bytes and descriptors
+        (two pinned and two device staging buffers)."""
+        if self._copy_stream is None and self.graphs:
+            self._copy_stream = torch.cuda.Stream(self.device)
+            self._staging = [(torch.empty_like(self.jpeg_data), torch.empty_like(self.jpeg_desc),
+                              torch.empty_like(self.h_jpeg_data).pin_memory(),
+                              torch.empty_like(self.h_jpeg_desc).pin_memory(), [0]) for _ in range(2)]
+            self._staged = [torch.cuda.Event() for _ in range(2)]
+            self._consumed = [torch.cuda.Event() for _ in range(2)]
+        return super().infer_stream(items)
+
+    def _stage(self, jpegs, k, first_use):
+        """Parse the files of one item into pinned staging k, then enqueue their H2D into device staging k."""
+        data, desc, h_data, h_desc, used = self._staging[k]
+        if not first_use:
+            self._staged[k].synchronize()  # the H2D of the item staged here before has read the pinned buffers
+        used[0] = self.pack_jpegs(jpegs, h_data, h_desc)
+        cs = self._copy_stream
+        with torch.cuda.stream(cs):
+            if not first_use:
+                cs.wait_event(self._consumed[k])
+            data[:used[0]].copy_(h_data[:used[0]], non_blocking=True)
+            desc.copy_(h_desc, non_blocking=True)
+            self._staged[k].record(cs)
+
+    def _launch_staged(self, step, k):
+        """Launch the frame whose files are in staging k: wait for their H2D, D2D copies into the lane's buffers on the
+        lane's stream, then the replay."""
+        mats, prev, new_sequence = step
+        data, desc, _, _, used = self._staging[k]
+        st = self.stream
+        st.wait_stream(torch.cuda.current_stream(self.device))
+        with torch.cuda.stream(st):  # after the lane's previous frame, which read the buffers
+            st.wait_event(self._staged[k])
+            self.jpeg_data[:used[0]].copy_(data[:used[0]], non_blocking=True)
+            self.jpeg_desc.copy_(desc, non_blocking=True)
             self._consumed[k].record(st)
         self.launch(mats, prev, None, new_sequence)

@@ -344,6 +344,22 @@ def camera_frames(seed, n_cams=6, H=900, W=1600):
     return np.ascontiguousarray(np.clip(np.rint(img), 0, 255).astype(np.uint8))
 
 
+def camera_jpegs(seed, n_cams=6, H=900, W=1600, **pillow_save_kwargs):
+    """camera_frames(seed, n_cams, H, W) encoded by Pillow as JPEG files: a list of n_cams bytes objects.
+    pillow_save_kwargs go to Image.save (quality, subsampling, optimize, restart_marker_blocks, ...).  Pillow is
+    imported here: the package itself does not depend on it."""
+    import io
+
+    from PIL import Image
+
+    out = []
+    for frame in camera_frames(seed, n_cams, H, W):
+        buf = io.BytesIO()
+        Image.fromarray(frame).save(buf, "JPEG", **pillow_save_kwargs)
+        out.append(buf.getvalue())
+    return out
+
+
 def lss_mats(rig):
     """(sensor2ego, cam2imgs, post_rots, post_trans, bda) of a camera_rig, the order LSSHotPath takes them in."""
     return rig["sensor2ego"], rig["cam2imgs"], rig["post_rots"], rig["post_trans"], rig["bda"]

@@ -4,6 +4,7 @@
   python tools/bevdet_bench.py [--steps K] [--warmup W] [--in-flight L] [--no-cpu-check] [--dump-outputs DIR]
   python tools/bevdet_bench.py --temporal [--steps K] [--warmup W] [--in-flight L] [--rounds R] [--no-cpu-check]
   python tools/bevdet_bench.py --temporal --images | --raw-images [--steps K] [--warmup W] [--in-flight L] [--rounds R]
+  python tools/bevdet_bench.py --jpeg [--temporal] [--steps K] [--warmup W] [--in-flight L] [--rounds R]
   python tools/bevdet_bench.py --bevdet-nms [--temporal] [--steps K] [--warmup W] [--in-flight L] [--rounds R]
 
 A frame = six cameras of 16 x 44 features (D = 118, C = 80) -> LSS view transform into the 128 x 128 x 96 pixel fp16-pair
@@ -47,6 +48,14 @@ pinned host memory, the band's H2D included, next to BEVDet4DImageHotPath on res
 one at a time); infer_stream over one drive of --steps key frames next to a loop of launch_frames + result over the same
 items (frames/s); the node counts of the start and continue graphs; memory per lane; the band's H2D bytes and time; the
 card.  Rounds alternate the arms (median of the rounds).
+
+--jpeg [--temporal]: BEVDet (BEVDet4D) from the bytes of six 900 x 1600 JPEG camera files (bevdet.BEVDetJpegHotPath,
+BEVDet4DJpegHotPath: the device JPEG decode of the prep plan's band at the head of the captured frame), Pillow-encoded at
+q95 4:2:0 by synth.camera_jpegs, the bytes' H2D included, next to the --raw-images arm (BEVDetFrameHotPath /
+BEVDet4DFrameHotPath) on Pillow's decode of the same files in pinned memory, in rounds that alternate the two (median):
+frames/s in flight and one at a time; the decode of the band, graph-timed (us, compressed MB/s, output GB/s); the H2D
+bytes and time per frame of both arms; the host baseline (Pillow's decode of the six files on one thread and on every
+core); the node counts of the frame graphs; the card; and a frame-0 check that the lane's band equals Pillow's rows.
 
 --bevdet-nms: the frames with BEVDet's own box decode (bevdet.CONFIG_BEVDET_NMS, with --temporal CONFIG_4D_BEVDET_NMS:
 top-K over class x cell, per-class scale-NMS / circle NMS) next to the same weights with the default decode
@@ -101,10 +110,15 @@ def main():
     ap.add_argument("--raw-images", action="store_true",
                     help="BEVDet from six decoded uint8 camera frames (image prep in the frame), alternated with the frame "
                          "from normalised images")
+    ap.add_argument("--jpeg", action="store_true",
+                    help="BEVDet (with --temporal BEVDet4D) from the bytes of six JPEG files (device decode in the frame), "
+                         "alternated with the frame from Pillow's decode of the same files")
     args = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("bevdet_bench.py needs a CUDA device (no CPU fallback exists)")
+    if args.jpeg:
+        return jpeg_files(args)
     if args.temporal and (args.images or args.raw_images):
         return temporal_images(args)
     if args.raw_images:
@@ -574,6 +588,141 @@ def raw_images(args):
                         "GB_per_s": plan.band_bytes(n) / (h2d_ms * 1e-3) / 1e9,
                         "full_fp32_images_bytes": plan.out_bytes(n)}
     line["value"] = line["frames"]["fps_in_flight"]
+    print(json.dumps(line))
+
+
+def jpeg_files(args):
+    import io
+    from concurrent.futures import ThreadPoolExecutor
+
+    import torch
+    from PIL import Image
+
+    from paddle3d_b200 import bevdet as bd
+    from paddle3d_b200 import synth
+    from paddle3d_b200.frame import count_graph_nodes
+    from paddle3d_b200.ops import jpeg
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    four = args.temporal
+    m = (bd.BEVDet4DFromImages if four else bd.BEVDetFromImages)(device=dev).init_weight(seed=args.seed, bn_gain=BN_GAIN)
+    plan = m.prep_plan
+    files = [synth.camera_jpegs(args.seed + i, quality=95, subsampling=2) for i in range(2)]
+
+    def pil(f):
+        return np.asarray(Image.open(io.BytesIO(f)).convert("RGB"))
+    frames_host = [torch.from_numpy(np.stack([pil(f) for f in fr])).pin_memory() for fr in files]
+    L = 8
+    if four:
+        rig = synth.camera_rig(args.seed, bda=False)
+        poses = synth.ego_poses(L, speed=10.0, yaw_rate=0.3)
+        items = [(None, rig["sensor2ego"][0], np.broadcast_to(p, (m.N, 4, 4)).copy(), rig["cam2imgs"][0]) for p in poses]
+        steps = list(bd.drive_mats(items, m.test_mats))
+        m.calibrate_heatmap_bias(steps[0][0], m.images_from_frames(frames_host[0].to(dev)))
+    else:
+        rigs = [synth.camera_rig(s) for s in range(4)]
+        cams = [(r["sensor2ego"], r["cam2imgs"], r["bda"]) for r in rigs]
+        m.calibrate_heatmap_bias(m.test_mats(*cams[0]), m.images_from_frames(frames_host[0].to(dev)))
+    line = {"metric": "BEVDet%s frames/s from the bytes of six 900 x 1600 JPEG camera files (q95 4:2:0; H2D of the bytes -> "
+                      "device JPEG decode of the band -> resize / crop / normalise -> ResNet-50 + CustomFPN + depth net -> "
+                      "LSS -> BEV encoder -> CenterHead -> boxes)" % ("4D sequential" if four else ""),
+            "unit": "frames/s", "gpu": gpu_identity(0), "steps": args.steps, "warmup": args.warmup,
+            "compressed_bytes_per_frame": [sum(len(f) for f in fr) for fr in files]}
+    lanes_n = max(1, args.in_flight)
+    arms = {"jpeg": bd.BEVDet4DJpegHotPath if four else bd.BEVDetJpegHotPath,
+            "frames": bd.BEVDet4DFrameHotPath if four else bd.BEVDetFrameHotPath}
+    runs = {n: [c(m, device=dev).capture(count_nodes=(i == 0)) for i in range(lanes_n)] for n, c in arms.items()}
+    torch.cuda.synchronize()
+    count = {}
+
+    def launch(name, lane_i, lane):
+        k = count.get((name, lane_i), 0)
+        count[(name, lane_i)] = k + 1
+        if four:
+            mats, prev, _ = steps[0 if k == 0 else 1 + (k - 1) % (L - 1)]
+            args_ = (mats[0], mats[1], mats[4])
+            extra = (prev, k == 0)
+        else:
+            args_, extra = cams[k % 4], ()
+        if name == "jpeg":
+            lane.launch_jpegs(*args_, files[k % 2], *extra)
+        else:
+            lane.launch_frames(*args_, frames_host[k % 2], *extra)
+
+    def one(name, lane):
+        launch(name, 0, lane)
+        lane.result()
+    rates = {n: {"fps_in_flight": [], "fps_one_at_a_time": []} for n in runs}
+    for name, lanes in runs.items():
+        for i in range(args.warmup):
+            launch(name, i % lanes_n, lanes[i % lanes_n])
+    torch.cuda.synchronize()
+    for _ in range(max(1, args.rounds)):  # alternate the arms so that clocks and temperature drift hit both
+        for name, lanes in runs.items():
+            rates[name]["fps_in_flight"].append(
+                _rate(lambda i: launch(name, i % lanes_n, lanes[i % lanes_n]), torch.cuda.synchronize, args.steps))
+            rates[name]["fps_one_at_a_time"].append(
+                _rate(lambda i: one(name, lanes[0]), torch.cuda.synchronize, args.steps))
+    for name, lanes in runs.items():
+        for ln in lanes:
+            ln.result()  # raises on a JPEG decode error or an fp16-range overflow
+        r = {k: float(np.median(v)) for k, v in rates[name].items()}
+        r.update(rounds=rates[name], lanes=lanes_n,
+                 graph_nodes={g: count_graph_nodes(x) for g, x in lanes[0].graphs.items()} if four else
+                 lanes[0].graph_nodes)
+        line[name] = r
+    hot = runs["jpeg"][0]
+    line["band_equals_pillow_frame"] = bool(np.array_equal(hot.band.cpu().numpy(),
+                                                           frames_host[(count[("jpeg", 0)] - 1) % 2].numpy()[
+                                                               :, plan.band[0]:plan.band[1]]))
+    # the decode of the band alone, graph-timed
+    st = torch.cuda.Stream(dev)
+    nbytes = hot.pack_jpegs(files[0])
+    hot.jpeg_data[:nbytes].copy_(hot.h_jpeg_data[:nbytes])
+    hot.jpeg_desc.copy_(hot.h_jpeg_desc)
+    status = torch.zeros(m.N, dtype=torch.int32, device=dev)
+    out = torch.empty_like(hot.band)
+    dec_ms = graph_time_ms(lambda: jpeg.jpeg_decode_u8(hot.jpeg_data, hot.jpeg_desc, m.N, plan.src_size, rows=plan.band,
+                                                       out=out, status=status, max_bytes=hot.jpeg_max_bytes), st, 50)
+    comp = line["compressed_bytes_per_frame"][0]
+    line["decode_band"] = {"us": dec_ms * 1e3, "compressed_MB_per_s": comp / (dec_ms * 1e-3) / 1e6,
+                           "output_GB_per_s": out.numel() / (dec_ms * 1e-3) / 1e9, "band_rows": plan.band_rows}
+
+    def h2d_ms(copy):
+        with torch.cuda.stream(st):
+            copy()
+            st.synchronize()
+            s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            s.record(st)
+            for _ in range(20):
+                copy()
+            e.record(st)
+        e.synchronize()
+        return s.elapsed_time(e) / 20
+
+    def jpeg_copy():
+        hot.jpeg_data[:nbytes].copy_(hot.h_jpeg_data[:nbytes], non_blocking=True)
+        hot.jpeg_desc.copy_(hot.h_jpeg_desc, non_blocking=True)
+    fh = runs["frames"][0]
+    line["h2d"] = {"jpeg": {"bytes_per_frame": nbytes + hot.jpeg_desc.numel(), "ms": h2d_ms(jpeg_copy)},
+                   "frames_band": {"bytes_per_frame": plan.band_bytes(m.N),
+                                   "ms": h2d_ms(lambda: fh.copy_band(frames_host[0]))}}
+    # host baseline: Pillow's decode of the six files, one thread and every core
+    reps = 5
+    t0 = time.perf_counter()
+    for i in range(reps):
+        for f in files[i % 2]:
+            pil(f)
+    one_s = (time.perf_counter() - t0) / reps
+    with ThreadPoolExecutor(os.cpu_count()) as ex:
+        list(ex.map(pil, files[0]))
+        t0 = time.perf_counter()
+        for i in range(reps):
+            list(ex.map(pil, files[i % 2]))
+        all_s = (time.perf_counter() - t0) / reps
+    line["host_decode"] = {"one_thread_s_per_frame": one_s, "all_cores_s_per_frame": all_s, "cpus": os.cpu_count(),
+                           "kind": "np.asarray(Image.open(f).convert('RGB')) of the six files (libjpeg-turbo)"}
+    line["value"] = line["jpeg"]["fps_in_flight"]
     print(json.dumps(line))
 
 
