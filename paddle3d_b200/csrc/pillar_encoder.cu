@@ -5,8 +5,10 @@
 //                               concat([x, x_max]) -> Linear(2 C1 -> C2) + BN + ReLU, max over the rows.
 // One block per pillar, the decorated rows (and the first layer's rows) staged in shared memory.  The reference runs this
 // as ~15 elementwise / matmul / argmax launches over the [N, M, F+5] and [N, M, C] intermediates; here only voxels
-// [N, M, F] is read and [N, C] written.  Checked by tests/test_gpu_voxelize.py::test_pillar_feature_net and
-// tests/test_gpu_centerpoint_pillars.py (1e-4 vs the oracle restatements).
+// [N, M, F] is read and [N, C] written.  Checked by tests/test_gpu_lidar_front_end.py::test_pillar_feature_net_one_layer
+// (one layer: F 3 .. 8, M 1 .. 64, C 1 .. 200, far pillars, padding rows deciding the max, rows beyond the count
+// untouched), tests/test_gpu_voxelize.py::test_pillar_feature_net and tests/test_gpu_centerpoint_pillars.py (two layers),
+// 1e-4 vs the oracle restatements; the argument limits by tests/test_lidar_front_end_oracle.py.
 #include "common.cuh"
 #include "p3d_b200.h"
 
