@@ -644,6 +644,63 @@ int p3d_jpeg_decode_u8(const uint8_t *data, int64_t data_bytes, const p3d_jpeg_d
                        int y1, int64_t max_bytes, uint8_t *out, int32_t *status_dev, void *workspace,
                        size_t workspace_bytes, p3d_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * BEVFusion (bevf_pp) entry points.  PARITY UNPINNED: recalled from mmdet3d v0.17 (HardVFE, Anchor3DHead,
+ * box3d_multiclass_nms) and ADLab's BEVFusion (SE_Block), not checked against either.
+ *
+ * p3d_hard_vfe: mmdet3d HardVFE(feat_channels [mid, out], with_cluster_center, with_voxel_center, no distance) as one
+ * launch, the two-layer kernel of p3d_pillar_feature_net2 with a wider decoration: per point the F raw values, xyz minus
+ * the pillar mean, xyz minus the voxel centre (coors * voxel_size + voxel_size / 2 + range_min, z included), F + 6
+ * features; padding rows zeroed; VFELayer 0 = Linear(F + 6 -> mid) + BN + ReLU concatenated with its max over the M rows
+ * (weight1 [F + 6, mid]; mid is not halved), VFELayer 1 = Linear(2 mid -> out) + BN + ReLU, max over the rows -> [n, out].
+ * voxel_size_host / point_cloud_range_host: 3 / 6 values.  Limits of p3d_pillar_feature_net2.
+ *
+ * p3d_se_gate_h16: BEVFusion's SE_Block on a pixel H16 image img_h16 [B, H, W, C] in place:
+ *   gate[b, o] = sigmoid(bias[o] + sum_c weight[o, c] * mean_hw(img[b, :, :, c])), x *= gate[b, c].
+ *   The mean: per-CTA partial sums in fp64, then summed in index order (no atomics: bit-reproducible).  The gate is
+ *   computed in fp64 and rounded to fp32 into gate_dev [B, C] (device).  The scale rebuilds each value from its pair in
+ *   fp32, multiplies by the fp32 gate and splits again; status bit 0 as p3d_dense_conv2d_f16.  weight [C, C] (the 1x1
+ *   conv's [out, in]), bias [C], device fp32.  C % 32 == 0, 16-byte aligned image (P3D_ERR_INVALID_ARG otherwise);
+ *   C <= 1024, B <= 65535 (P3D_ERR_UNSUPPORTED above).  workspace: p3d_se_gate_workspace_bytes(B, H, W, C).
+ *
+ * p3d_anchor3d_postprocess: Anchor3DHead.get_bboxes_single + box3d_multiclass_nms at batch 1, sigmoid scores, every
+ * class in the same launches, no host synchronisation.
+ *   head [R (C + 9 + 2), H, W] fp32 planes: cls [R x C] | reg [R x 9] | dir [R x 2]; channel a * K + k of a group belongs
+ *   to anchor (y * W + x) * R + a.  anchors [A, 9] (x, y, z, w, l, h, r, vx, vy), A = H * W * R.
+ *   1. score = max over the classes of sigmoid(cls) (NaN when a class is NaN); dir = argmax of the two dir logits, a tie
+ *      to bin 0.
+ *   2. A > nms_pre: the nms_pre anchors of highest score, in descending score order, ties by the lower anchor index, a
+ *      NaN score above every number (torch.topk's order).  A <= nms_pre: every anchor, in anchor order.  Only anchors
+ *      that can reach the output (a class score > score_thr, or a NaN score) are ranked: the others cannot enter the
+ *      output and rank below every one that can.
+ *   3. DeltaXYZWLHRBBoxCoder.decode: za += ha / 2, diag = sqrt(la^2 + wa^2), x = xt diag + xa, y = yt diag + ya,
+ *      z = zt ha + za, (w, l, h) = exp(t) * anchor, r = rt + ra, z -= h / 2, (vx, vy) = t + anchor; fp32, every
+ *      operation rounded on its own.
+ *   4. per class c in order: the kept anchors with sigmoid(cls_c) > score_thr, greedy NMS in descending class score
+ *      (ties by kept order) with suppression at BEV IoU > nms_thr, the IoU of box_geom.cuh on (x, y, w, l, r) taken
+ *      as (x, y, dx, dy, heading).  Which rotation convention the reference's NMS applies is unpinned.
+ *   5. more than max_num survivors over all classes: sorted by score, descending, ties in class-major order, the first
+ *      max_num kept; otherwise class-major order.
+ *   6. r = limit_period(r - dir_offset, dir_limit_offset, pi) + dir_offset + pi * dir, limit_period(v, o, p) =
+ *      v - floor(v / p + o) * p in fp32.
+ *   Outputs (device): boxes [max_num, 9], scores [max_num], labels int64 [max_num], count [1] int32 (rows written).
+ *   Limits (P3D_ERR_UNSUPPORTED): C <= 64, A < 2^31, nms_pre <= 4096.  workspace: p3d_anchor3d_postprocess_workspace_bytes.
+ * ------------------------------------------------------------------------------------------- */
+int p3d_hard_vfe(const float *voxels, const int32_t *num_points_per_voxel, const int32_t *coors,
+                 const int32_t *num_voxels_dev, int64_t n_cap, int max_points, int num_point_dim, int mid_channels,
+                 const float *weight1, const float *bn_scale1, const float *bn_shift1, int out_channels,
+                 const float *weight2, const float *bn_scale2, const float *bn_shift2, const float *voxel_size_host,
+                 const float *point_cloud_range_host, float *out, p3d_stream_t stream);
+size_t p3d_se_gate_workspace_bytes(int B, int H, int W, int C);
+int p3d_se_gate_h16(void *img_h16, int B, int H, int W, int C, const float *weight, const float *bias, float *gate_dev,
+                    int32_t *status_dev, void *workspace, size_t workspace_bytes, p3d_stream_t stream);
+size_t p3d_anchor3d_postprocess_workspace_bytes(int feat_h, int feat_w, int anchors_per_loc, int num_classes,
+                                                int nms_pre, int max_num);
+int p3d_anchor3d_postprocess(const float *head, int feat_h, int feat_w, int anchors_per_loc, int num_classes,
+                             const float *anchors, int nms_pre, float score_thr, float nms_thr, int max_num,
+                             float dir_offset, float dir_limit_offset, float *boxes, float *scores, int64_t *labels,
+                             int32_t *count, void *workspace, size_t workspace_bytes, p3d_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

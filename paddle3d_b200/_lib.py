@@ -121,6 +121,13 @@ SIGNATURES = {
                                 _vp]),
     "p3d_jpeg_decode_workspace_bytes": (_sz, [_int, _int, _int, _i64]),
     "p3d_jpeg_decode_u8": (_int, [_vp, _i64, _vp, _int, _int, _int, _int, _int, _i64, _vp, _vp, _vp, _sz, _vp]),
+    "p3d_hard_vfe": (_int, [_vp, _vp, _vp, _vp, _i64, _int, _int, _int, _vp, _vp, _vp, _int, _vp, _vp, _vp, _vp, _vp, _vp,
+                            _vp]),
+    "p3d_se_gate_workspace_bytes": (_sz, [_int, _int, _int, _int]),
+    "p3d_se_gate_h16": (_int, [_vp, _int, _int, _int, _int, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "p3d_anchor3d_postprocess_workspace_bytes": (_sz, [_int, _int, _int, _int, _int, _int]),
+    "p3d_anchor3d_postprocess": (_int, [_vp, _int, _int, _int, _int, _vp, _int, _f, _f, _int, _f, _f, _vp, _vp, _vp, _vp,
+                                        _vp, _sz, _vp]),
 }
 
 

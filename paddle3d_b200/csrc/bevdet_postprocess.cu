@@ -6,11 +6,9 @@
 //   B1 bdp_candidates  one pass over every heat-map value of every task: sigmoid, score > threshold, (class, cell)
 //                      candidates appended with warp-aggregated atomics as sortable 64-bit keys
 //                      (~score_bits << 32 | class * HW + cell).  Only the heat maps are read here.
-//   B2 bdp_select      one CTA per task: the max_num smallest keys in exact order.  With more than max_num candidates
-//                      an 8-bit radix select over the key finds the max_num-th smallest key (the digits between the
-//                      index's top bit and bit 32 are zero in every key and are skipped), the keys at or below it are
-//                      compacted and only those are ranked by counting: work is O(M) per digit + O(max_num^2), never
-//                      O(M^2).  Keys are unique, so equal scores order by ascending class * HW + cell.
+//   B2 bdp_select      one CTA per task: the max_num smallest keys in exact order (topk_select.cuh: radix select,
+//                      then a rank count of the keys at or below the cut).  Keys are unique, so equal scores order by
+//                      ascending class * HW + cell.
 //   B3 bdp_decode      box decode of the selected candidates, range test on the DECODED centre (a box with a non-finite
 //                      value is dropped as well), survivors compacted in score order with a block-wide scan.
 //   B4 bdp_mask        upper triangle of the suppression bit-matrix in 64 x 64 tiles: rotated IoU on boxes whose dx, dy
@@ -21,6 +19,7 @@
 #include "box_geom.cuh"
 #include "common.cuh"
 #include "nms_reduce.cuh"
+#include "topk_select.cuh"
 
 namespace p3d {
 namespace {
@@ -117,79 +116,11 @@ __global__ void __launch_bounds__(256) bdp_candidates_kernel(BdpTasks tk, BdpAtt
 }
 
 __global__ void __launch_bounds__(1024) bdp_select_kernel(BdpTasks tk, BdpAttrs at, BdpWs w) {
-  const int t = blockIdx.x, tid = threadIdx.x;
-  const int M = w.cnt[t];
-  const int K = min(M, at.max_num);
-  const unsigned long long *keys = w.keys + tk.key_off[t];
-  unsigned long long *sel = w.sel + static_cast<size_t>(t) * at.max_num;
-  __shared__ int s_hist[256];
-  __shared__ unsigned long long s_prefix;
-  __shared__ int s_k, s_n;
-  unsigned long long kth = ~0ull;
-  if (M > at.max_num) {  // the max_num-th smallest key, most significant digit first
-    if (tid == 0) {
-      s_prefix = 0ull;
-      s_k = at.max_num;
-    }
-    for (int shift = 56; shift >= 0; shift -= 8) {
-      if (shift < 32 && shift >= tk.low_bits[t]) continue;
-      if (tid < 256) s_hist[tid] = 0;
-      __syncthreads();
-      const unsigned long long prefix = s_prefix;
-      for (int j = tid; j < M; j += blockDim.x) {
-        const unsigned long long key = keys[j];
-        if (shift == 56 || ((key ^ prefix) >> (shift + 8)) == 0ull) atomicAdd(&s_hist[(key >> shift) & 255ull], 1);
-      }
-      __syncthreads();
-      if (tid < 32) {  // the bin holding the k-th key of this digit: 8 bins per lane
-        int loc[8], sum = 0;
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          loc[q] = s_hist[tid * 8 + q];
-          sum += loc[q];
-        }
-        int inc = sum;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-          const int v = __shfl_up_sync(0xffffffffu, inc, d);
-          if (tid >= d) inc += v;
-        }
-        const int k = s_k;
-        __syncwarp();
-        if (inc - sum < k && k <= inc) {  // exactly one lane
-          int kk = k - (inc - sum), bin = -1;
-#pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            if (bin < 0) {
-              if (loc[q] >= kk)
-                bin = q;
-              else
-                kk -= loc[q];
-            }
-          }
-          s_k = kk;
-          s_prefix = prefix | (static_cast<unsigned long long>(tid * 8 + bin) << shift);
-        }
-      }
-      __syncthreads();
-    }
-    kth = s_prefix;
-  }
-  if (tid == 0) s_n = 0;
-  __syncthreads();
-  for (int j = tid; j < M; j += blockDim.x) {
-    const unsigned long long key = keys[j];
-    if (key <= kth) sel[atomicAdd(&s_n, 1)] = key;  // exactly K of them: keys are unique
-  }
-  __syncthreads();
-  for (int j = tid; j < K; j += blockDim.x) {
-    const unsigned long long mine = sel[j];
-    int rank = 0;
-#pragma unroll 8
-    for (int k = 0; k < K; ++k) rank += (sel[k] < mine);
-    w.sorted[static_cast<size_t>(t) * at.max_num + rank] = mine;
-  }
-  if (tid == 0) w.nsel[t] = K;
+  const int t = blockIdx.x;
+  const size_t o = static_cast<size_t>(t) * at.max_num;
+  const int K = select_smallest_keys(w.keys + tk.key_off[t], w.cnt[t], at.max_num, tk.low_bits[t], w.sel + o,
+                                     w.sorted + o);
+  if (threadIdx.x == 0) w.nsel[t] = K;
 }
 
 __global__ void __launch_bounds__(256) bdp_decode_kernel(BdpTasks tk, BdpAttrs at, BdpWs w) {

@@ -134,9 +134,11 @@ class SecondTrunk:
     def export_numpy(self):
         return dict(blocks=[[c.np for c in blk] for blk in self.blocks], deblocks=[c.np for c in self.deblocks])
 
-    def __call__(self, x, shape, first=None):
+    def __call__(self, x, shape, first=None, out=None, out_channels=None, out_c0=0):
         """x: pixel rows [B*H*W, 2*C] (fp16 pairs or tf32 split) with shape = (B, H, W, C); first replaces the first conv.
-        Returns (concat image [B*oH*oW, 2*fpn_channels], (B, oH, oW, fpn_channels))."""
+        Returns (concat image [B*oH*oW, 2*fpn_channels], (B, oH, oW, fpn_channels)).  out: an existing image of
+        out_channels channels per row; the concat is written into its channels [out_c0, out_c0 + fpn_channels) and
+        (out, (B, oH, oW, out_channels)) returned."""
         b = shape[0]
         feats = []
         for bi, blk in enumerate(self.blocks):
@@ -151,13 +153,14 @@ class SecondTrunk:
             raise ValueError("the FPN deblocks give feature maps of different sizes %s; the concat needs one size"
                              % sorted(out_hws))
         out_hw = out_hws.pop()
-        cat = torch.empty((b * out_hw[0] * out_hw[1], 2 * self.fpn_channels),
-                          dtype=torch.float16 if self.f16 else torch.float32, device=x.device)
-        c0 = 0
+        oc = self.fpn_channels if out is None else int(out_channels)
+        cat = out if out is not None else torch.empty((b * out_hw[0] * out_hw[1], 2 * oc),
+                                                      dtype=torch.float16 if self.f16 else torch.float32, device=x.device)
+        c0 = 0 if out is None else int(out_c0)
         for (f, fshape), de in zip(feats, self.deblocks):
-            de(f, fshape, out_split=cat, out_channels=self.fpn_channels, out_c0=c0)
+            de(f, fshape, out_split=cat, out_channels=oc, out_c0=c0)
             c0 += de.cout
-        return cat, (b, out_hw[0], out_hw[1], self.fpn_channels)
+        return cat, (b, out_hw[0], out_hw[1], oc)
 
     @staticmethod
     def deblock_out_hw(de, h, w):

@@ -60,3 +60,37 @@ def pillar_feature_net2(voxels, num_points_per_voxel, coors, layers, voxel_size,
                                         c, ptr(w2), ptr(s2), ptr(t2), host_floats(voxel_size),
                                         host_floats(point_cloud_range), ptr(out), stream(dev)), "pillar_feature_net2")
     return out
+
+
+def hard_vfe(voxels, num_points_per_voxel, coors, layers, voxel_size, point_cloud_range, num_voxels=None, folded=None,
+             out=None):
+    """mmdet3d HardVFE (feat_channels [mid, out], with_cluster_center, with_voxel_center, no distance) as one launch
+    (p3d_hard_vfe): the decoration adds xyz minus the voxel centre, z included, and the first layer is not halved.
+    layers: two dicts of weight / gamma / beta / mean / var / eps, weight [F + 6, mid] then [2 mid, out] on the device.
+    voxel_size: 3 values, point_cloud_range: 6.  folded: the two (scale, shift) pairs of fold_bn.  out: an existing
+    [n, out] fp32 buffer (a captured frame keeps its address; rows past num_voxels are left as they are), default a new
+    zero-filled one.  Returns the [n, out] features."""
+    voxels = require_cuda(voxels, "voxels", torch.float32)
+    npv = require_cuda(num_points_per_voxel, "num_points_per_voxel", torch.int32)
+    coors = require_cuda(coors, "coors", torch.int32)
+    w1 = require_cuda(layers[0]["weight"], "layers[0].weight", torch.float32)
+    w2 = require_cuda(layers[1]["weight"], "layers[1].weight", torch.float32)
+    n, m, f = voxels.shape
+    mid, c = w1.shape[1], w2.shape[1]
+    if w1.shape[0] != f + 6 or w2.shape[0] != 2 * mid:
+        raise ValueError("weights must be [F + 6, mid] and [2 mid, out]")
+    if len(voxel_size) != 3 or len(point_cloud_range) != 6:
+        raise ValueError("voxel_size needs 3 values and point_cloud_range 6")
+    dev = voxels.device
+    if folded is None:
+        folded = [fold_bn(l["gamma"], l["beta"], l["mean"], l["var"], l["eps"], dev) for l in layers]
+    (s1, t1), (s2, t2) = folded
+    if out is None:
+        out = torch.zeros((n, c), dtype=torch.float32, device=dev)
+    elif tuple(out.shape) != (n, c) or out.dtype != torch.float32 or not out.is_cuda or not out.is_contiguous():
+        raise ValueError("out must be a contiguous [n, out] fp32 device tensor")
+    nump = ptr(require_cuda(num_voxels, "num_voxels", torch.int32)) if num_voxels is not None else ptr(None)
+    check(lib().p3d_hard_vfe(ptr(voxels), ptr(npv), ptr(coors), nump, n, m, f, mid, ptr(w1), ptr(s1), ptr(t1), c, ptr(w2),
+                             ptr(s2), ptr(t2), host_floats(voxel_size), host_floats(point_cloud_range), ptr(out),
+                             stream(dev)), "hard_vfe")
+    return out
