@@ -48,6 +48,8 @@ constexpr int kSmemBudget = (227 - 6) * 1024;  // 227 KB per CTA less alignment 
 constexpr int kDenseThreads = 384;      // producer warpgroup + two consumer warpgroups
 constexpr uint32_t kConsumerWarps = 8;  // arrivals that release a slot: one per consumer warp
 constexpr uint32_t kEpiThreads = 96;    // warps 1-3 of the producer warpgroup: the epilogue warps
+constexpr int kFlush = 9;               // steps (18 k-steps) per hi x hi partial before it joins the fp32 total
+constexpr int kFlushTerms = 8192;       // products per output above which a launch flushes (FLUSH instantiations)
 
 struct Params {
   int B, H, W, Cin;           // input image (pixel H16 rows [B*H*W][4 * Cin bytes])
@@ -379,7 +381,7 @@ __device__ __forceinline__ void epilogue_pairs(const Params &p, const CUtensorMa
 // RES (pair tile, up == 1): each consumer thread adds the residual of its own fragment elements, read from global memory
 // (the hi and lo' halves of two adjacent channels: 4 + 4 bytes), before ReLU; the residual-free instantiations compile
 // to the code they have without it.
-template <int N, int MT, bool HALO, bool FUSE_P = false, bool RES = false>
+template <int N, int MT, bool HALO, bool FUSE_P = false, bool RES = false, bool FLUSH = false>
 __global__ void __launch_bounds__(kDenseThreads, 1)
     dense_conv_f16_kernel(const __grid_constant__ CUtensorMap in_map, const __grid_constant__ CUtensorMap out_map,
                           const KParams<FUSE_P, RES> p) {
@@ -431,6 +433,7 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
   // steps / activation units per item: HALO: one unit per group, 9 taps each; TAP: one unit per (tap, group)
   const int taps_item = p.up > 1 ? 1 : p.taps;
   const int units_item = HALO ? G : taps_item * G;
+  const int steps_item = units_item * C::SPU;
   // Ring positions advance by one slot per fill / use; the phase bit flips when the slot index wraps.  The consumers wait
   // for full[slot] to complete the phase of the current pass; the producer waits for empty[slot] to complete the phase
   // of the previous pass (parity ph ^ 1: on the first pass that is the phase before the barrier's first, which counts as
@@ -506,13 +509,21 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
     if (warp_leader) mbar_arrive(smem_u32(&s_bar[base + slot]));
   };
   uint32_t a_slot = 0, a_ph = 0, b_slot = 0, b_ph = 0;
-  float acc[C::ACC];
+  // acc: per M tile the hi x hi products since the last flush [0, H), then the cross products [H, N); tot: the hi x hi
+  // products of the flushed steps.  The tensor core's own accumulation does not round to nearest and drifts over a long
+  // chain, so every kFlush steps (HALO: one 32-channel group's 9 taps) the hi partial is added into tot with
+  // round-to-nearest FADDs and the next step's first hi wgmma starts it over (scale_d = 0).  Only the FLUSH instantiations
+  // do this, for chains longer than kFlushTerms: tot costs 32 to 64 registers (spills in the N = 128 and MT = 2 ones) and
+  // every flush drains the wgmma pipeline, so the shorter chains keep the single accumulator.
+  float acc[C::ACC], tot[MT * H];
   bool ovf = false;  // fp16 range overflow of the pair tile (status bit 0)
   Trace tr;
   const long long t_start = tr.now();
   for (long long idx = 0; idx < n_items; ++idx) {
 #pragma unroll
     for (int i = 0; i < C::ACC; ++i) acc[i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < MT * H; ++i) tot[i] = 0.f;
     const Item im = decode(idx, p, TH);
     // pair tile: the item's scale / shift columns are staged in shared memory while the K loop runs, in one of two
     // buffers (item parity) after the warpgroup's pair blocks; its epilogue reads them after a warpgroup barrier
@@ -529,6 +540,8 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
     uint32_t prev_b = 0;
     int prev_a = -1;
     bool pending = false;
+    int step = 0;             // steps of the item issued so far
+    uint32_t hi_scale = 1u;   // 0: the step's first hi wgmma starts the hi partial over
     for (int ua = 0; ua < units_item; ++ua) {
       long long t0 = tr.now();
       mbar_wait(smem_u32(&s_bar[kAF + a_slot]), a_ph);
@@ -556,15 +569,27 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
             }
             const uint64_t dah = desc_sw128(a0 + kb * 32, sbo), dal = desc_sw128(a0 + (2 + kb) * 32, sbo);
             float *d = acc + mt * N;
-            wg::mma_f16<N>(d, dah, dbh, 1u);      // A_hi x B_hi
+            wg::mma_f16<N>(d, dah, dbh, kb == 0 ? hi_scale : 1u);  // A_hi x B_hi
             wg::mma_f16<N>(d + H, dah, dbl, 1u);  // A_hi x B_lo'
             wg::mma_f16<N>(d + H, dal, dbh, 1u);  // A_lo' x B_hi
           }
         }
         wg_commit();
         t0 = tr.now();
-        wg_wait<1>();  // the previous step's group has retired: its slots go back to the producer
+        const bool flush = FLUSH && ++step % kFlush == 0 && step < steps_item;
+        if (flush)
+          wg_wait<0>();  // this step's group has retired too: the hi partial can be read
+        else
+          wg_wait<1>();  // the previous step's group has retired: its slots go back to the producer
         tr.add(kTrMma, t0);
+        if (flush) {
+          wg_fence_acc<C::ACC>(acc);
+#pragma unroll
+          for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+            for (int i = 0; i < H; ++i) tot[mt * H + i] += acc[mt * N + i];
+        }
+        hi_scale = flush ? 0u : 1u;
         if (pending) {
           release(kBE, prev_b);
           if (prev_a >= 0) release(kAE, static_cast<uint32_t>(prev_a));
@@ -583,6 +608,10 @@ __global__ void __launch_bounds__(kDenseThreads, 1)
     release(kBE, prev_b);
     release(kAE, static_cast<uint32_t>(prev_a));  // the item's last step ends a unit
     wg_fence_acc<C::ACC>(acc);
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+      for (int i = 0; i < H; ++i) acc[mt * N + i] += tot[mt * H + i];  // the last partial joins the total
     // fill this warpgroup's staging tile once the epilogue warps have drained the previous item from it, and go on with
     // the next item
     tr.add(kTrEpi, t0);
@@ -855,7 +884,9 @@ int launch(const CUtensorMap &map, const CUtensorMap &out_map, const KParams<FUS
   using C = Cfg<N, MT, HALO>;
   const size_t smem = static_cast<size_t>(C::NA) * C::A_BYTES + static_cast<size_t>(C::NB) * C::B_BYTES + C::STG_BYTES + 1024;
   if (smem > static_cast<size_t>(kSmemBudget)) return P3D_ERR_UNSUPPORTED;
-  auto kern = dense_conv_f16_kernel<N, MT, HALO, FUSE_P, RES>;
+  // a chain of more than kFlushTerms products per output drifts in one wgmma accumulator: the FLUSH instantiation
+  const bool flush = static_cast<long long>(p.Cin) * (p.up > 1 ? 1 : p.taps) > kFlushTerms;
+  auto kern = flush ? dense_conv_f16_kernel<N, MT, HALO, FUSE_P, RES, !FUSE_P> : dense_conv_f16_kernel<N, MT, HALO, FUSE_P, RES>;
   P3D_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   const long long work = static_cast<long long>(p.B) * p.tiles_y * p.tiles_x * p.n_ntiles * (p.up > 1 ? p.up * p.up : 1);
   cudaLaunchConfig_t cfg = {};

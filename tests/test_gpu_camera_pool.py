@@ -514,14 +514,17 @@ GEOMETRIES = {
     "b_ds8_b2": ((256, 704), 8, synth.LSS_BEVDET, 80, 2),
     "c_z8_c32": ((256, 704), 16, dict(synth.LSS_BEVDET, z=[-5.0, 3.0, 1.0]), 32, 1),
     "d_c160": ((256, 704), 16, synth.LSS_BEVDET, 160, 1),
+    # BEVFusion (bevf_pp): 900 / 8 = 112.5 feature rows (floored), 41 depth bins, a 200 x 200 x 16 grid, 1024 channels
+    "e_bevf_pp_900x1600_z16": ((900, 1600), 8, dict(synth.LSS_C4, z=[-5.0, 3.0, 0.5], depth=[4.0, 45.0, 1.0]), 64, 1),
 }
 
 
 @pytest.mark.parametrize("geom", sorted(GEOMETRIES))
 def test_view_transform_geometry(cuda, oracle_mod, geom):
     """coor bit-equal to the fp32 oracle, ranks = voxel_pooling_prepare_v2 of it, depth within the ulp rules, the BEV
-    bit-equal to the oracle's pool of the device's depth and feat, within 1e-4 / 1e-5 of oracle.lss.view_transform end
-    to end, and the captured frame equal to the eager forward."""
+    and the pixel-row fp16-pair pool image (bev_pool_v2_dev_h16, the image the camera encoders read) bit-equal to the
+    oracle's pool of the device's depth and feat, within 1e-4 / 1e-5 of oracle.lss.view_transform end to end, and the
+    captured frame equal to the eager forward."""
     import torch
     from oracle import lss
     from paddle3d_b200.lss import LSSHotPath, LSSViewTransformer
@@ -548,10 +551,13 @@ def test_view_transform_geometry(cuda, oracle_mod, geom):
         assert np.array_equal(g[:len(r)].cpu().numpy(), r), name
     # depth, feat and the pool of the device's own depth and feat
     depth, feat = bp.lss_depth_feat(tl, tt)
+    rows = bp.bev_pool_v2_dev_h16(depth, feat, got, vt.bev_feat_shape(B))
     depth, feat = depth.cpu().numpy(), feat.cpu().numpy()
     _depth_ulp_check(depth, lss.depth_softmax(logits))
     assert _bits_equal(feat, lss.feat_permute(tran))
     pool = collapse(oracle_mod.bev_pool_v2(depth, feat, rd, rf, rb, ln, st, (B, Z, Y, X, C), use_fma=True))
+    assert _bits_equal(rows, pixel_rows(pool, (Z * C + 31) // 32 * 32)), "pool image != split_h16 of the oracle's pool"
+    del rows
     inputs = [torch.zeros((B, 6, 1, 1, 1))] + [rig[n] for n in ("sensor2ego", "ego2global", "cam2imgs", "post_rots",
                                                                    "post_trans", "bda")]
     eager = vt.forward(inputs, tl, tt)

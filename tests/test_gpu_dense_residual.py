@@ -202,6 +202,21 @@ def error_stats(got, want):
     return float(err.std()) / scale, float(err[~big].max()) / scale, float((err[big] / want[big].abs()).max())
 
 
+def decomposition_runs(case):
+    """(N tile, mode, m_tiles) of a full-size layer's every-decomposition runs: the frame's N tile with the MT rule's
+    choice, N = 64 with both M tilings where the layer has at least 128 channels (else the other M tiling), and for the
+    3x3 stride-1 layers the forced per-tap loads."""
+    nt = _n_tile(case.cout)
+    runs = [(nt, 0, 0)]
+    if case.cout >= 128:
+        runs += [(64, 0, 1), (64, 0, 2)]
+    else:
+        runs += [(64, 0, 3 - case.plan(_sms(), 64).inst[1])]
+    if case.up == 1 and case.k == 3 and case.stride == 1:
+        runs.append((nt, 1, 0))
+    return runs
+
+
 # BEVDet's encoder (bevdet.BEVDetEncoder) at full size: (name, H, W, cin, cout, k, stride, pad, relu, bias_only,
 # residual, cin_real).  Per stage: the first block's conv1 and identity conv (3x3 stride 2 with bias, no ReLU) on the
 # previous stage's output, conv1 of the second block, conv2 with the residual; then FPN_LSS and the head's shared conv.
@@ -243,15 +258,7 @@ def test_bevdet_layer_every_decomposition(cuda, layer):
         case = DenseCase(cuda, 1, H, W, cin, cout, k, stride, pad, 1, seed, relu=relu, bias_only=bias_only)
         if cin_real is not None:
             zero_pad_input(case, cin_real)
-    nt = _n_tile(cout)
-    runs = [(nt, 0, 0)]
-    if cout >= 128:
-        runs += [(64, 0, 1), (64, 0, 2)]
-    else:
-        runs += [(64, 0, 3 - case.plan(_sms(), 64).inst[1])]
-    if k == 3 and stride == 1:
-        runs.append((nt, 1, 0))
-    for i, (n, mode, mt) in enumerate(runs):
+    for i, (n, mode, mt) in enumerate(decomposition_runs(case)):
         label = "bevdet %s N%d mode%d MT%d" % (name, n, mode, mt)
         if res:
             p, img, out_C = run_residual(label, case, n, mode, mt, c0=0, guards=i == 0)

@@ -312,7 +312,15 @@ def bar(terms):
     1e-2 floor: std 1.5e-7 / 2.1e-7 x max (stage-3 conv1 / lateral1), at most 1.3e-6 / 1.2e-6 x max below 5e-2 x max,
     so 1.15e-4 / 1.2e-4 relative at the 1e-2 floor, and relative error above 5e-2 x max at most 2.8e-5 / 2.7e-5, the
     same bits in every decomposition; 1024 terms: std 5.5e-8 to 8.3e-8 x max, at most 9.1e-7 x max below 5e-2 x max.
-    A lost tap or cross product would show a constant relative error instead, which the guards check."""
+    BEVFusion's full-size layers (test_gpu_bevfusion_full_size.py, same card and power limit, every decomposition):
+    4608 terms std 4.4e-7 x max, relative error above 5e-2 x max at most 4.4e-5; 5760 terms (reduc_conv, seeded input
+    and the frame's fusion image) std 6.2e-7 / 6.7e-7 x max, at most 3.8e-6 x max below 5e-2 x max, relative at most
+    6.7e-5; 9216 terms (the camera encoder's 1024-channel convs) std 8.9e-7 / 9.6e-7 x max, at most 6.3e-6 x max below,
+    relative 9.4e-5 to 1.001e-4 with the whole A_hi x B_hi chain of an item (576 k-steps) in one wgmma accumulator: at
+    and past the bar, and not flat (the std doubles from 4608 to 9216 terms).  The tensor core's accumulation does not
+    round to nearest, so a launch whose chain is longer than 8192 terms adds the hi partial of every 9 steps into a
+    round-to-nearest fp32 total (dcf::kFlush, the FLUSH instantiations); the figures up to 7200 terms are of the single
+    accumulator, which those launches keep.  A lost tap or cross product would show a constant relative error instead, which the guards check."""
     return (1e-2, 2e-6) if terms < 2048 else (5e-2, 1e-5)
 
 
@@ -453,13 +461,16 @@ class DenseCase:
         return pl, st
 
 
-def run_dense(name, case, n_tile, mode=0, m_tiles=0, c0=32, h16=True, guards=True):
+def run_dense(name, case, n_tile, mode=0, m_tiles=0, c0=32, h16=True, guards=True, out_C=None):
     """Launch a layer into a sentinel-filled wider fp16-pair image at channel offset c0 and into NaN-filled planes, check
-    both against the reference, the sentinels, the status word and a second launch (same bits).  Returns (plan, image,
-    planes)."""
+    both against the reference, the sentinels, the status word and a second launch (same bits).  out_C: the image's
+    channels (default: 32 more than c0 + cout rounded up to 32).  Returns (plan, image, planes)."""
     import torch
     p = case.plan(_sms(), n_tile, mode, m_tiles)
-    out_C = _cdiv(c0 + case.cout, 32) * 32 + 32 if h16 else 0
+    if not h16:
+        out_C = 0
+    elif out_C is None:
+        out_C = _cdiv(c0 + case.cout, 32) * 32 + 32
     n_px = case.B * p.out_H * p.out_W
 
     def once():

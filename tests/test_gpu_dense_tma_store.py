@@ -28,12 +28,14 @@ def _image_pair(case, n_tile, mode, m_tiles, out_C, c0, scale=None):
     return img, int(st[0]), ref, pl, int(st_ref[0])
 
 
-def run_pairs(name, case, n_tile, mode=0, m_tiles=0, c0=32, reference=True):
+def run_pairs(name, case, n_tile, mode=0, m_tiles=0, c0=32, reference=True, out_C=None):
     """H16-only launch against the launch with planes (same bits, same status), sentinels untouched, a second H16-only
-    launch gives the same bits; with `reference` also the fp64 bar.  Returns (plan, H16-only image, out_C)."""
+    launch gives the same bits; with `reference` also the fp64 bar.  out_C: the image's channels (default: 32 more than
+    c0 + cout rounded up to 32).  Returns (plan, H16-only image, out_C)."""
     import torch
     p = case.plan(_sms(), n_tile, mode, m_tiles)
-    out_C = _cdiv(c0 + case.cout, 32) * 32 + 32
+    if out_C is None:
+        out_C = _cdiv(c0 + case.cout, 32) * 32 + 32
     n_px = case.B * p.out_H * p.out_W
     img, st, ref, _, st_ref = _image_pair(case, n_tile, mode, m_tiles, out_C, c0)
     assert st == 0 and st_ref == 0, "%s: status %d / %d" % (name, st, st_ref)
