@@ -23,6 +23,7 @@ pipeline's resize, crop and normalisation (ops.image_prep, bit-identical to Pill
 BEVDet4DFromImages / BEVDet4DImageHotPath / BEVDet4DFrameHotPath (CONFIG_4D_IMG) do the same for BEVDet4D: the image
 encoder (and the image prep) at the head of both temporal graphs; BEVDet4DFrameHotPath.infer_stream runs a drive from
 frames and ego poses (drive_mats)."""
+import functools
 import itertools
 
 import numpy as np
@@ -30,7 +31,7 @@ import torch
 
 from . import raw, synth
 from .dense_head import DenseRPNHead, _Conv
-from .frame import ResultSlot, ResultSlotOwner, copy_rows, in_flight
+from .frame import ResultSlot, ResultSlotOwner, StagedUpload, copy_rows, in_flight
 from .lss import CameraFrame, LSSViewTransformer
 from .ops import bev_pool_v2 as bp
 from .ops import bevdet_postprocess as bdp
@@ -1011,7 +1012,7 @@ class BEVDet4DFrameHotPath(FrameInput, BEVDet4DImageHotPath):
         self.check_plan(model)
         super().__init__(model, device, stream)
         self._init_band()
-        self._copy_stream = None
+        self._upload = None
 
     def launch_frames(self, sensor2ego, cam2imgs, bda, frames, prev_sensor2keyego=None, new_sequence=False):
         """Enqueue one frame of this lane's sequence from decoded camera frames [N, H0, W0, 3] uint8 (contiguous; on this
@@ -1035,53 +1036,45 @@ class BEVDet4DFrameHotPath(FrameInput, BEVDet4DImageHotPath):
 
         The band of item j + 1 is copied on a copy stream into one of two device staging bands while frame j computes
         (the copy is enqueued before the host waits for frame j), then moved into the lane's band by one D2D copy on the
-        lane's stream just before its replay; events order the reuse of each staging band (frame.in_flight's schedule on
-        one lane, its slot being the staging band)."""
+        lane's stream just before its replay; events order the reuse of each staging band (frame.StagedUpload;
+        frame.in_flight's schedule on one lane, its slot being the staging band)."""
         if not self.graphs:
             raise RuntimeError("infer_stream needs a captured lane: call capture() first")
-        if self._copy_stream is None:
-            self._copy_stream = torch.cuda.Stream(self.device)
-            self._staging = [torch.empty_like(self.band) for _ in range(2)]
-            self._staged = [torch.cuda.Event() for _ in range(2)]    # H2D into staging[k] done
-            self._consumed = [torch.cuda.Event() for _ in range(2)]  # staging[k] copied into the lane's band
+        if self._upload is None:
+            self._upload = self._new_upload()
         a, b = itertools.tee(items)
         plans = zip((item[0] for item in a), drive_mats(b, self.model.test_mats))
         steps, held = {}, {}  # item -> its matrices until launched; its frames until its result is read
         for kind, i, plan, _, k in in_flight(plans, 1):
             if kind == "submit":
                 held[i], steps[i] = plan
-                self._stage(held[i], k, first_use=i < 2)
+                self._upload.stage(k, functools.partial(self._fill, held[i]), first_use=i < 2)
                 if i == 0:
-                    self._launch_staged(steps.pop(0), k)
+                    self._launch_step(steps.pop(0), k)
             else:
                 out = self.slot.read(self.check_status, self.done, clone=True)
                 del held[i]
                 if i + 1 in steps:
-                    self._launch_staged(steps.pop(i + 1), k ^ 1)
+                    self._launch_step(steps.pop(i + 1), k ^ 1)
                 yield out
 
-    def _stage(self, frames, k, first_use):
-        """Check the frames of one item and enqueue the H2D of their band into staging band k on the copy stream."""
-        self.check_frames(frames)
-        cs = self._copy_stream
-        with torch.cuda.stream(cs):
-            if not first_use:
-                cs.wait_event(self._consumed[k])
-            self.copy_band(frames, out=self._staging[k])
-            if frames.is_cuda:
-                frames.record_stream(cs)
-            self._staged[k].record(cs)
+    def _new_upload(self):
+        """The staged upload of infer_stream: two staging bands."""
+        return StagedUpload([self.band])
 
-    def _launch_staged(self, step, k):
-        """Launch the frame whose band is in staging band k: wait for its H2D, one D2D copy into the lane's band on the
-        lane's stream, then the replay (BEVDet4DImageHotPath.launch).  step = (mats, prev_sensor2keyego, new_sequence)."""
+    def _fill(self, frames, dev, host):
+        """StagedUpload fill of one drive item: check its frames and enqueue the H2D of their band into dev."""
+        self.check_frames(frames)
+        self.copy_band(frames, out=dev[0])
+        if frames.is_cuda:
+            frames.record_stream(torch.cuda.current_stream(self.device))
+
+    def _launch_step(self, step, k):
+        """Launch the frame whose input is in staging set k: its D2D into the lane's input on the lane's stream, then the
+        replay (BEVDet4DImageHotPath.launch).  step = (mats, prev_sensor2keyego, new_sequence)."""
         mats, prev, new_sequence = step
-        st = self.stream
-        st.wait_stream(torch.cuda.current_stream(self.device))
-        with torch.cuda.stream(st):  # after the lane's previous frame, which read the band
-            st.wait_event(self._staged[k])
-            self.band.copy_(self._staging[k], non_blocking=True)
-            self._consumed[k].record(st)
+        self.stream.wait_stream(torch.cuda.current_stream(self.device))
+        self._upload.unstage(k, self.stream)  # after the lane's previous frame, which read the input
         self.launch(mats, prev, None, new_sequence)
 
 
@@ -1185,7 +1178,7 @@ class BEVDetJpegHotPath(JpegInput, BEVDetFrameHotPath):
 class BEVDet4DJpegHotPath(JpegInput, BEVDet4DFrameHotPath):
     """BEVDet4DFrameHotPath from the bytes of six JPEG camera files (JpegInput at the head of both frame graphs).
     infer_stream runs one drive from JPEG files and ego poses with the H2D of the next item's bytes on a copy stream
-    while the current frame computes."""
+    while the current frame computes: its items carry N JPEG files (as launch_jpegs takes them) in place of the frames."""
 
     def __init__(self, model, device="cuda", stream=None, max_bytes=JpegInput.DEFAULT_MAX_BYTES):
         super().__init__(model, device, stream)
@@ -1203,43 +1196,14 @@ class BEVDet4DJpegHotPath(JpegInput, BEVDet4DFrameHotPath):
         self.launch_jpegs(sensor2ego, cam2imgs, bda, jpegs, prev_sensor2keyego, new_sequence)
         return self.result()
 
-    def infer_stream(self, items):
-        """One drive: items = (jpegs, sensor2ego [N, 4, 4], ego2global [N, 4, 4], cam2imgs [N, 3, 3]) per key frame, in
-        order; BEVDet4DFrameHotPath.infer_stream's schedule, the staged payload being the files' bytes and descriptors
-        (two pinned and two device staging buffers)."""
-        if self._copy_stream is None and self.graphs:
-            self._copy_stream = torch.cuda.Stream(self.device)
-            self._staging = [(torch.empty_like(self.jpeg_data), torch.empty_like(self.jpeg_desc),
-                              torch.empty_like(self.h_jpeg_data).pin_memory(),
-                              torch.empty_like(self.h_jpeg_desc).pin_memory(), [0]) for _ in range(2)]
-            self._staged = [torch.cuda.Event() for _ in range(2)]
-            self._consumed = [torch.cuda.Event() for _ in range(2)]
-        return super().infer_stream(items)
+    def _new_upload(self):
+        """The staged upload of infer_stream: the files' bytes and descriptors through pinned and device staging."""
+        return StagedUpload([self.jpeg_data, self.jpeg_desc], pinned=True)
 
-    def _stage(self, jpegs, k, first_use):
-        """Parse the files of one item into pinned staging k, then enqueue their H2D into device staging k."""
-        data, desc, h_data, h_desc, used = self._staging[k]
-        if not first_use:
-            self._staged[k].synchronize()  # the H2D of the item staged here before has read the pinned buffers
-        used[0] = self.pack_jpegs(jpegs, h_data, h_desc)
-        cs = self._copy_stream
-        with torch.cuda.stream(cs):
-            if not first_use:
-                cs.wait_event(self._consumed[k])
-            data[:used[0]].copy_(h_data[:used[0]], non_blocking=True)
-            desc.copy_(h_desc, non_blocking=True)
-            self._staged[k].record(cs)
-
-    def _launch_staged(self, step, k):
-        """Launch the frame whose files are in staging k: wait for their H2D, D2D copies into the lane's buffers on the
-        lane's stream, then the replay."""
-        mats, prev, new_sequence = step
-        data, desc, _, _, used = self._staging[k]
-        st = self.stream
-        st.wait_stream(torch.cuda.current_stream(self.device))
-        with torch.cuda.stream(st):  # after the lane's previous frame, which read the buffers
-            st.wait_event(self._staged[k])
-            self.jpeg_data[:used[0]].copy_(data[:used[0]], non_blocking=True)
-            self.jpeg_desc.copy_(desc, non_blocking=True)
-            self._consumed[k].record(st)
-        self.launch(mats, prev, None, new_sequence)
+    def _fill(self, jpegs, dev, host):
+        """StagedUpload fill of one drive item: parse its files into the pinned buffers host, then enqueue the H2D of the
+        bytes used and of the descriptors into dev."""
+        n = self.pack_jpegs(jpegs, *host)
+        dev[0][:n].copy_(host[0][:n], non_blocking=True)
+        dev[1].copy_(host[1], non_blocking=True)
+        return n, len(host[1])

@@ -90,6 +90,46 @@ class ResultSlotOwner:
     h_status = property(lambda self: self.slot.status)
 
 
+class StagedUpload:
+    """The double-buffered input upload of a lane whose frames are in flight: the H2D of frame i + 1's inputs runs on a
+    copy stream while frame i computes.  Two staging sets shaped like the lane's input buffers `bufs` on the device and,
+    with pinned=True, two on the host; `staged[k]` is recorded after the H2D into set k, `consumed[k]` after unstage has
+    copied set k into bufs."""
+
+    def __init__(self, bufs, pinned=False):
+        self.bufs = list(bufs)
+        self.stream = torch.cuda.Stream(self.bufs[0].device)
+        self.dev = [[torch.empty_like(b) for b in self.bufs] for _ in range(2)]
+        self.host = [[torch.empty(b.shape, dtype=b.dtype, pin_memory=True) for b in self.bufs] for _ in range(2)] \
+            if pinned else None
+        self.rows = [None, None]  # per set: the leading rows of each buffer its payload fills
+        self._staged = [torch.cuda.Event() for _ in range(2)]
+        self._consumed = [torch.cuda.Event() for _ in range(2)]
+
+    def stage(self, k, fill, first_use):
+        """Enqueue the H2D of one payload into set k on the copy stream: fill(dev, host) enqueues the copies into the
+        set's device buffers dev on the current stream (host: the set's pinned buffers, which fill writes first; None
+        without them) and returns the leading rows of each buffer it wrote (None: all).  Unless first_use (the set's
+        first use since the lane last drained), the copy stream first waits until the set's previous payload is consumed
+        and, with pinned staging, the host until that payload's H2D has read the pinned buffers."""
+        if not first_use and self.host is not None:
+            self._staged[k].synchronize()
+        with torch.cuda.stream(self.stream):
+            if not first_use:
+                self.stream.wait_event(self._consumed[k])
+            rows = fill(self.dev[k], None if self.host is None else self.host[k])
+            self._staged[k].record(self.stream)
+        self.rows[k] = [len(b) for b in self.bufs] if rows is None else rows
+
+    def unstage(self, k, stream):
+        """Enqueue on `stream` (the lane's) the wait for set k's H2D and the D2D copies of the rows it holds into bufs."""
+        with torch.cuda.stream(stream):
+            stream.wait_event(self._staged[k])
+            for dst, src, n in zip(self.bufs, self.dev[k], self.rows[k]):
+                dst[:n].copy_(src[:n], non_blocking=True)
+            self._consumed[k].record(stream)
+
+
 def in_flight(items, lanes):
     """The schedule of frames in flight over `lanes` lanes: item i runs on lane i % lanes into its result slot
     (i // lanes) & 1; at most lanes + 1 frames are outstanding, and the result of a frame is always read before its
@@ -187,7 +227,7 @@ class CapturedFrame(ResultSlotOwner, GraphFrame):
         self.n = int(num_points or self.cfg["num_points"])
         self.F = self.cfg["point_dim"]
         self.points = torch.zeros((self.n, self.F), dtype=torch.float32, device=self.device)  # static input
-        self.graph = None
+        self.graph = self._upload = None
         self.sweep_input = self.ring = None
         if sweep_input is not None:
             self._init_sweep_input(dict(SWEEP_INPUT, **sweep_input), sweep_ring)
@@ -239,33 +279,26 @@ class CapturedFrame(ResultSlotOwner, GraphFrame):
 
     # ---- public end-to-end call for a sweep of frames: same per-frame work, copies overlapped with compute
     def prepare_sweep(self):
-        """Copy stream, staging buffers, pinned result slots and events of infer_many (allocated once; pinned allocations
+        """Staged upload of the points, pinned result slots and events of infer_many (allocated once; pinned allocations
         cost milliseconds, so callers that time a sweep call this first)."""
-        if getattr(self, "_copy_stream", None) is not None:
+        if self._upload is not None:
             return self
-        self._copy_stream = torch.cuda.Stream(self.device)
-        self._staging = [torch.empty_like(self.points) for _ in range(2)]
+        self._upload = StagedUpload([self.points])
         self._slots = [ResultSlot(*self.slot.shape) for _ in range(2)]
-        self._staged = [torch.cuda.Event() for _ in range(2)]    # H2D into staging[k] done
-        self._consumed = [torch.cuda.Event() for _ in range(2)]  # staging[k] copied into the graph's input
-        self._done = [torch.cuda.Event() for _ in range(2)]      # results of slot k are on the host
+        self._done = [torch.cuda.Event() for _ in range(2)]  # results of slot k are on the host
         return self
 
     def _submit(self, pts, k, first_use):
-        """Enqueue one frame of a sweep into slot k: H2D on the copy stream, graph replay, D2H of the results."""
-        cs, st = self._copy_stream, self.stream
-        with torch.cuda.stream(cs):
-            if not first_use:
-                cs.wait_event(self._consumed[k])
-            self._staging[k].copy_(pts, non_blocking=True)
-            self._staged[k].record(cs)
-        with torch.cuda.stream(st):
-            st.wait_event(self._staged[k])
-            self.points.copy_(self._staging[k], non_blocking=True)
-            self._consumed[k].record(st)
+        """Enqueue one frame of a sweep into slot k: H2D into staging set k on the copy stream, its D2D into the points,
+        graph replay, D2H of the results."""
+        def fill(dev, host):
+            dev[0].copy_(pts, non_blocking=True)
+        self._upload.stage(k, fill, first_use)
+        self._upload.unstage(k, self.stream)
+        with torch.cuda.stream(self.stream):
             self.graph.replay()
             self._slots[k].copy_from(self.out)
-            self._done[k].record(st)
+            self._done[k].record(self.stream)
 
     def _result(self, k):
         return self._slots[k].read(self.check_status, self._done[k], clone=True)
