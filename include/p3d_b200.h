@@ -187,13 +187,21 @@ int p3d_bevdet_postprocess(int num_tasks, const float *const *hm, const int32_t 
  *   p3d_sparse_rulebook_subm : nbr [n_cap, K] int32, nbr[i][k] = input row at coord(i) - pad + k or -1
  *                              (K = kD*kH*kW, pad = k/2; shared by every SubM layer of a stage).
  *   p3d_sparse_rulebook_conv : strided Conv3D: writes the output coordinate list out_coords
- *                              [out_cap, 4] (site order is unspecified), the device counters
- *                              n_out_dev (int32[4]) and nbr [out_cap, K] with
- *                              nbr[o][k] = input row at o*stride - pad + k or -1.
+ *                              [out_cap, 4], the device counters n_out_dev (int32[4]) and
+ *                              nbr [out_cap, K] with nbr[o][k] = input row at o*stride - pad + k or -1.
+ *   Output site order: first appearance.  Walk the input rows in row order and, within a row, the
+ *   taps k = (kz*kH + ky)*kW + kx in order; a site is appended the first time it is generated
+ *   (output o from input c under tap k when c = o*stride - pad + k).  The order depends only on
+ *   the input index set: the same in every run, on every stream, eager or captured, and from both
+ *   strided entry points.  Malformed input: of rows sharing a coordinate the LAST stands for it
+ *   (it is the row nbr names) and the others generate no sites; rows outside the input grid
+ *   (batch or spatial) generate no sites and are in no map.  When out_cap is too small the rows
+ *   kept are the first out_cap sites of this order (while the output table, sized for 2*out_cap
+ *   rows, holds every site: n_out_dev[3] = 0).
  *   n_in_dev / n_out_dev are device scalars so the whole backbone runs without a host sync.
  *   n_out_dev[0] = number of output sites (clamped to out_cap), n_out_dev[1] = 1 if sites were
  *   dropped because out_cap was too small, n_out_dev[2] = unclamped count (a lower bound once the
- *   dedup table itself is full), n_out_dev[3] = internal table-full flag.
+ *   output table itself is full), n_out_dev[3] = internal table-full flag.
  * ------------------------------------------------------------------------------------------- */
 size_t p3d_sparse_rulebook_workspace_bytes(int64_t n_in_cap, int64_t n_out_cap);
 int p3d_sparse_rulebook_subm(const int32_t *coords, const int32_t *n_in_dev, int64_t n_in_cap, int batch,
@@ -207,7 +215,8 @@ int p3d_sparse_rulebook_conv(const int32_t *coords, const int32_t *n_in_dev, int
 /* Caller-owned coordinate tables (one per index set / resolution level): the same rulebooks with every level's
  * table built exactly once per frame (the two calls above run this path on tables carved out of their workspace).
  * p3d_sparse_table_build hashes an index set's coordinates; p3d_sparse_rulebook_subm_t only looks neighbours up in it.
- * Tables are p3d_sparse_table_bytes(rows_cap) bytes, 16-byte aligned. */
+ * Tables are p3d_sparse_table_bytes(rows_cap) bytes, 16-byte aligned; the size includes the scratch a strided level
+ * numbering its sites into the table uses. */
 size_t p3d_sparse_table_bytes(int64_t rows_cap);
 int p3d_sparse_table_build(const int32_t *coords, const int32_t *n_dev, int64_t n_cap, int batch,
                            const int *spatial_host, void *table, size_t table_bytes, p3d_stream_t stream);

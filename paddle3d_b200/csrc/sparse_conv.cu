@@ -19,6 +19,8 @@
 // for the 5-channel input layer); the wgmma 3xTF32 path lives in sparse_conv_tc.cu.
 #include <cuda_fp16.h>
 
+#include <algorithm>
+
 #include "common.cuh"
 #include "h16.cuh"
 
@@ -47,7 +49,7 @@ __device__ __forceinline__ int lookup(const unsigned long long *__restrict__ tab
     if (e == kEmpty) return -1;
     if (static_cast<uint32_t>(e >> 32) == key) {
       const uint32_t row = static_cast<uint32_t>(e);
-      return row >= 0x7fffffffu ? -1 : static_cast<int>(row);  // site enumerated beyond the capacity: no row
+      return row >= 0x7fffffffu ? -1 : static_cast<int>(row);  // a site beyond the capacity or not numbered yet: no row
     }
     h = (h + 1) & mask;
   }
@@ -103,85 +105,202 @@ __global__ void __launch_bounds__(256) rb_neighbors_kernel(const int32_t *__rest
   }
 }
 
-// Strided conv: enumerate output sites.  Thread (i, k): candidate o = (in + pad - k) / stride.  The warp's winners (first
-// claim of a site) are numbered with ONE atomicAdd per warp iteration.
-__global__ void __launch_bounds__(256) rb_outputs_kernel(const int32_t *__restrict__ coords,
-                                                         const int32_t *__restrict__ n_dev, long long n_cap, Dims d,
-                                                         unsigned long long *__restrict__ tab_out, uint32_t mask,
-                                                         uint32_t shift, int32_t *__restrict__ out_coords,
-                                                         int32_t *__restrict__ n_out_dev, int out_cap) {
-  const int K = d.kd * d.kh * d.kw;
+// Strided conv: output site o of input row coord c under tap k, where c = o*stride - pad + k.
+__device__ __forceinline__ bool strided_site(const int4 &c, int k, const Dims &d, int4 *o) {
+  const int kz = k / (d.kh * d.kw), ky = (k / d.kw) % d.kh, kx = k % d.kw;
+  int oz = c.y + d.pd - kz, oy = c.z + d.ph - ky, ox = c.w + d.pw - kx;
+  if (oz < 0 || oy < 0 || ox < 0 || oz % d.sd || oy % d.sh || ox % d.sw) return false;
+  oz /= d.sd;
+  oy /= d.sh;
+  ox /= d.sw;
+  if (oz >= d.oD || oy >= d.oH || ox >= d.oW) return false;
+  *o = make_int4(c.x, oz, oy, ox);
+  return true;
+}
+
+// Input row under tap k of output site o's window, or -1.
+__device__ __forceinline__ int window_row(const unsigned long long *__restrict__ tab, uint32_t mask, uint32_t shift,
+                                          const int4 &o, int k, const Dims &d) {
+  const int kz = k / (d.kh * d.kw), ky = (k / d.kw) % d.kh, kx = k % d.kw;
+  const int iz = o.y * d.sd - d.pd + kz, iy = o.z * d.sh - d.ph + ky, ix = o.w * d.sw - d.pw + kx;
+  if (iz < 0 || iz >= d.D || iy < 0 || iy >= d.H || ix < 0 || ix >= d.W) return -1;
+  return lookup(tab, mask, shift, lin(o.x, iz, iy, ix, d.D, d.H, d.W));
+}
+
+// Strided conv: number the output sites in first-appearance order (input rows in row order, within a row the taps in
+// tap order) in one pass.  The owner of a site is the smallest input row generating it; listed by (row, tap), the owners
+// are the sites in first-appearance order.  Tiles of tile_rows input rows, taken by ticket, one thread per (row, tap):
+//   A. every candidate site marks its table entry with the smallest generating row (atomicMin on kPending | row);
+//   B. once every earlier tile has passed A (a look-back over zero aggregates), the entry holds the site's owner unless
+//      a later tile's row generates it too, and those rows are larger: a candidate whose row the entry holds owns it;
+//   C. the tile's owned sites get their ids from a block scan and a second decoupled look-back and are listed in id
+//      order; one thread per site writes its coordinates and table entry (the id, or 0x7fffffff past out_cap), one
+//      thread per (site, tap) its strided neighbour-map row.
+// The grid is persistent: a block takes tickets until its tile starts past the last row, so no block waits on a tile
+// that has not started.  desc: [0] the ticket, [1 + t] tile t's descriptor for B, [1 + tiles + t] for C, all zero before
+// the launch.  s_own holds the tile's owned-tap masks (row r, tap k: bit k & 31 of word r * W + k / 32), s_off each
+// row's first id within the tile, s_site the sites (r * K + k) of one chunk of ids.
+constexpr int kSiteThreads = 256, kSiteMaskWords = 4096, kSiteMaxRows = 1024, kSiteList = 1024;
+constexpr uint32_t kPending = 0x80000000u;
+
+__device__ __forceinline__ uint32_t out_slot(const unsigned long long *tab, uint32_t mask, uint32_t shift, uint32_t key) {
+  uint32_t h = hash32(key) >> shift;
+  while (static_cast<uint32_t>(__ldcg(tab + h) >> 32) != key) h = (h + 1) & mask;
+  return h;
+}
+
+__global__ void __launch_bounds__(kSiteThreads) rb_sites_kernel(
+    const int32_t *__restrict__ coords, const int32_t *__restrict__ n_dev, long long n_cap, Dims d,
+    const unsigned long long *__restrict__ tab_in, uint32_t mask_in, uint32_t shift_in, unsigned long long *tab_out,
+    uint32_t mask_out, uint32_t shift_out, int32_t *__restrict__ out_coords, int32_t *__restrict__ n_out_dev,
+    int out_cap, int32_t *__restrict__ nbr, unsigned long long *desc, int tiles, int tile_rows) {
+  __shared__ uint32_t s_own[kSiteMaskWords];
+  __shared__ int s_off[kSiteMaxRows];
+  __shared__ int s_warp[kSiteThreads / 32];
+  __shared__ unsigned int s_tile;
+  __shared__ int s_prefix, s_total;
+  __shared__ int s_site[kSiteList];
+  const int K = d.kd * d.kh * d.kw, W = (K + 31) >> 5;
   const long long n = n_dev ? min(static_cast<long long>(n_dev[0]), n_cap) : n_cap;
-  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
-  const int lane = threadIdx.x & 31;
-  // warp-uniform trip count (q0 = the warp's first query): the ballot below needs all 32 lanes
-  for (long long q0 = static_cast<long long>(blockIdx.x) * blockDim.x + (threadIdx.x & ~31); q0 < n * K; q0 += stride) {
-    const long long q = q0 + lane;
-    bool won = false;
-    uint32_t h = 0, key = 0;
-    int4 oc = make_int4(0, 0, 0, 0);
-    if (q < n * K) {
-      const int i = static_cast<int>(q / K), k = static_cast<int>(q - static_cast<long long>(i) * K);
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  while (true) {
+    __syncthreads();  // the previous tile's shared state is consumed
+    if (threadIdx.x == 0) s_tile = static_cast<unsigned int>(atomicAdd(&desc[0], 1ull));
+    __syncthreads();
+    const unsigned int tile = s_tile;
+    const long long tile0 = static_cast<long long>(tile) * tile_rows;
+    if (tile0 >= n) return;  // past the last row: no later tile waits on this one
+    const int rows = static_cast<int>(min(static_cast<long long>(tile_rows), n - tile0));
+    for (int q = threadIdx.x; q < tile_rows * W; q += kSiteThreads) s_own[q] = 0u;
+    // A: mark each candidate's site with the smallest generating row
+    for (int q = threadIdx.x; q < rows * K; q += kSiteThreads) {
+      const int r = q / K, k = q - r * K;
+      const long long i = tile0 + r;
       const int4 c = *reinterpret_cast<const int4 *>(coords + static_cast<size_t>(i) * 4);
-      const int kz = k / (d.kh * d.kw), ky = (k / d.kw) % d.kh, kx = k % d.kw;
-      int oz = c.y + d.pd - kz, oy = c.z + d.ph - ky, ox = c.w + d.pw - kx;
-      bool cand = !(oz < 0 || oy < 0 || ox < 0 || oz % d.sd || oy % d.sh || ox % d.sw);
-      if (cand) {
-        oz /= d.sd;
-        oy /= d.sh;
-        ox /= d.sw;
-        cand = oz < d.oD && oy < d.oH && ox < d.oW;
+      if (c.x < 0 || c.x >= d.B || c.y < 0 || c.y >= d.D || c.z < 0 || c.z >= d.H || c.w < 0 || c.w >= d.W) continue;
+      int4 o;
+      if (!strided_site(c, k, d, &o)) continue;
+      // a duplicate coordinate: the row the table holds (the later one) stands for it
+      if (lookup(tab_in, mask_in, shift_in, lin(c.x, c.y, c.z, c.w, d.D, d.H, d.W)) != i) continue;
+      const uint32_t key = lin(o.x, o.y, o.z, o.w, d.oD, d.oH, d.oW);
+      const unsigned long long want = (static_cast<unsigned long long>(key) << 32) | kPending | static_cast<uint32_t>(i);
+      uint32_t h = hash32(key) >> shift_out;
+      for (uint32_t probes = 0;; ++probes) {
+        if (probes > mask_out) {  // table full (far more sites than out_cap): flag it, the site is not numbered
+          n_out_dev[3] = 1;
+          break;
+        }
+        unsigned long long cur = __ldcg(tab_out + h);
+        if (cur == kEmpty) {
+          cur = atomicCAS(&tab_out[h], kEmpty, want);
+          if (cur == kEmpty) break;
+        }
+        if (static_cast<uint32_t>(cur >> 32) == key) {
+          atomicMin(&tab_out[h], want);
+          break;
+        }
+        h = (h + 1) & mask_out;
       }
-      if (cand) {
-        key = lin(c.x, oz, oy, ox, d.oD, d.oH, d.oW);
-        oc = make_int4(c.x, oz, oy, ox);
-        h = hash32(key) >> shift;
-        for (uint32_t probes = 0;; ++probes) {
-          if (probes > mask) {  // table full (far more sites than out_cap): cannot dedupe any more, flag overflow
-            n_out_dev[3] = 1;
-            break;
-          }
-          unsigned long long cur = tab_out[h];
-          if (cur == kEmpty) {
-            // claim the slot; the winner numbers the site below
-            const unsigned long long want = (static_cast<unsigned long long>(key) << 32) | 0xfffffffeu;
-            cur = atomicCAS(&tab_out[h], kEmpty, want);
-            if (cur == kEmpty) {
-              won = true;
-              break;
-            }
-          }
-          if (static_cast<uint32_t>(cur >> 32) == key) break;
-          h = (h + 1) & mask;
+    }
+    __threadfence();
+    __syncthreads();
+    if (wid == 0) lookback_exclusive_prefix(desc + 1, tile, 0);  // returns once every earlier tile has passed A
+    __syncthreads();
+    // B: a candidate owns its site when the entry still holds its row
+    for (int q = threadIdx.x; q < rows * K; q += kSiteThreads) {
+      const int r = q / K, k = q - r * K;
+      const long long i = tile0 + r;
+      const int4 c = *reinterpret_cast<const int4 *>(coords + static_cast<size_t>(i) * 4);
+      if (c.x < 0 || c.x >= d.B || c.y < 0 || c.y >= d.D || c.z < 0 || c.z >= d.H || c.w < 0 || c.w >= d.W) continue;
+      int4 o;
+      if (!strided_site(c, k, d, &o)) continue;
+      const uint32_t key = lin(o.x, o.y, o.z, o.w, d.oD, d.oH, d.oW);
+      uint32_t h = hash32(key) >> shift_out;
+      for (uint32_t probes = 0; probes <= mask_out; ++probes, h = (h + 1) & mask_out) {
+        const unsigned long long e = __ldcg(tab_out + h);
+        if (e == kEmpty) break;
+        if (static_cast<uint32_t>(e >> 32) == key) {
+          if (static_cast<uint32_t>(e) == (kPending | static_cast<uint32_t>(i))) atomicOr(&s_own[r * W + (k >> 5)], 1u << (k & 31));
+          break;
         }
       }
     }
-    const unsigned int winners = __ballot_sync(0xffffffffu, won);
-    if (winners) {
-      int base = 0;
-      if (lane == __ffs(winners) - 1) base = atomicAdd(&n_out_dev[2], __popc(winners));  // raw counter (clamped copy: [0])
-      base = __shfl_sync(0xffffffffu, base, __ffs(winners) - 1);
-      if (won) {
-        const int id = base + __popc(winners & ((1u << lane) - 1u));
-        if (id < out_cap) {
-          *reinterpret_cast<int4 *>(out_coords + static_cast<size_t>(id) * 4) = oc;
-          // publish the row id: this table doubles as the coordinate table of the OUTPUT index set (same key, one
-          // aligned 8-byte store; concurrent probes only compare the key half)
-          tab_out[h] = (static_cast<unsigned long long>(key) << 32) | static_cast<uint32_t>(id);
-        }
+    __syncthreads();
+    // C: ids in (row, tap) order: per-row offsets from a block scan, the tile's offset from the look-back
+    const int rpt = (tile_rows + kSiteThreads - 1) / kSiteThreads, r0 = threadIdx.x * rpt;
+    int cnt = 0;
+    for (int r = r0; r < r0 + rpt && r < rows; ++r)
+      for (int w = 0; w < W; ++w) cnt += __popc(s_own[r * W + w]);
+    int inc = cnt;
+  #pragma unroll
+    for (int s = 1; s < 32; s <<= 1) {
+      const int t = __shfl_up_sync(0xffffffffu, inc, s);
+      if (lane >= s) inc += t;
+    }
+    if (lane == 31) s_warp[wid] = inc;
+    __syncthreads();
+    if (wid == 0) {
+      const int v = lane < kSiteThreads / 32 ? s_warp[lane] : 0;
+      int winc = v;
+  #pragma unroll
+      for (int s = 1; s < 32; s <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, winc, s);
+        if (lane >= s) winc += t;
       }
+      if (lane < kSiteThreads / 32) s_warp[lane] = winc - v;
+      const int aggregate = __shfl_sync(0xffffffffu, winc, 31);
+      const int prefix = lookback_exclusive_prefix(desc + 1 + tiles, tile, aggregate);
+      if (lane == 0) {
+        s_prefix = prefix;
+        s_total = aggregate;
+        if (tile0 + tile_rows >= n) n_out_dev[2] = prefix + aggregate;  // the last tile: raw count (clamped copy: [0])
+      }
+    }
+    __syncthreads();
+    int off = s_warp[wid] + inc - cnt;
+    for (int r = r0; r < r0 + rpt && r < rows; ++r) {
+      s_off[r] = off;
+      for (int w = 0; w < W; ++w) off += __popc(s_own[r * W + w]);
+    }
+    const int prefix = s_prefix, total = s_total;
+    for (int base = 0; base < total; base += kSiteList) {
+      const int m = min(kSiteList, total - base);
+      for (int r = r0; r < r0 + rpt && r < rows; ++r) {
+        int j = s_off[r] - base;
+        for (int w = 0; w < W && j < m; ++w)
+          for (uint32_t bits = s_own[r * W + w]; bits && j < m; bits &= bits - 1u, ++j)
+            if (j >= 0) s_site[j] = r * K + (w << 5) + __ffs(bits) - 1;
+      }
+      __syncthreads();
+      for (int j = threadIdx.x; j < m; j += kSiteThreads) {
+        const int r = s_site[j] / K, k = s_site[j] - r * K, id = prefix + base + j;
+        int4 o;
+        strided_site(*reinterpret_cast<const int4 *>(coords + static_cast<size_t>(tile0 + r) * 4), k, d, &o);
+        const uint32_t key = lin(o.x, o.y, o.z, o.w, d.oD, d.oH, d.oW);
+        // the entry now names the site's row of the OUTPUT index set: this table is that set's coordinate table
+        atomicExch(&tab_out[out_slot(tab_out, mask_out, shift_out, key)],
+                   (static_cast<unsigned long long>(key) << 32) | static_cast<uint32_t>(id < out_cap ? id : 0x7fffffff));
+        if (id < out_cap) *reinterpret_cast<int4 *>(out_coords + static_cast<size_t>(id) * 4) = o;
+      }
+      for (int q = threadIdx.x; q < m * K; q += kSiteThreads) {
+        const int j = q / K, k2 = q - j * K, id = prefix + base + j;
+        if (id >= out_cap) break;  // ids grow with q
+        const int r = s_site[j] / K, k = s_site[j] - r * K;
+        const long long i = tile0 + r;
+        int4 o;
+        strided_site(*reinterpret_cast<const int4 *>(coords + static_cast<size_t>(i) * 4), k, d, &o);
+        nbr[static_cast<size_t>(id) * K + k2] = k2 == k ? static_cast<int>(i) : window_row(tab_in, mask_in, shift_in, o, k2, d);
+      }
+      __syncthreads();
     }
   }
 }
 
-// One launch per resolution level after rb_outputs: publishes the clamped output count / overflow flag and fills BOTH
-// neighbour maps of the new index set: the strided conv's (rows of the input level, through tab_in) and, when nbr_m is
-// given, the 3-D SubM map of the level's residual blocks (rows of the output level, through tab_out, which rb_outputs
-// completed).  Query q < n * Ks: strided; else SubM.
+// One launch per resolution level after rb_sites: publishes the clamped output count / overflow flag and, when nbr_m
+// is given, fills the 3-D SubM map of the level's residual blocks (rows of the output level, through tab_out, which
+// rb_sites completed).
 __global__ void __launch_bounds__(256) rb_level_neighbors_kernel(const int32_t *__restrict__ out_coords,
-                                                                 int32_t *__restrict__ n_out_dev, long long out_cap, Dims ds,
-                                                                 const unsigned long long *__restrict__ tab_in,
-                                                                 uint32_t mask_in, uint32_t shift_in, int32_t *__restrict__ nbr_s,
+                                                                 int32_t *__restrict__ n_out_dev, long long out_cap,
                                                                  Dims dm, const unsigned long long *__restrict__ tab_out,
                                                                  uint32_t mask_out, uint32_t shift_out,
                                                                  int32_t *__restrict__ nbr_m) {
@@ -191,33 +310,21 @@ __global__ void __launch_bounds__(256) rb_level_neighbors_kernel(const int32_t *
     n_out_dev[0] = static_cast<int32_t>(n);
     n_out_dev[1] = (raw > out_cap || n_out_dev[3]) ? 1 : 0;
   }
-  const int Ks = ds.kd * ds.kh * ds.kw, Km = nbr_m ? dm.kd * dm.kh * dm.kw : 0;
-  const long long total = n * (Ks + Km), split = n * Ks;
+  if (!nbr_m) return;
+  const int Km = dm.kd * dm.kh * dm.kw;
   const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
-  for (long long q = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; q < total; q += stride) {
-    if (q < split) {
-      const int o = static_cast<int>(q / Ks), k = static_cast<int>(q - static_cast<long long>(o) * Ks);
-      const int4 c = *reinterpret_cast<const int4 *>(out_coords + static_cast<size_t>(o) * 4);
-      const int kz = k / (ds.kh * ds.kw), ky = (k / ds.kw) % ds.kh, kx = k % ds.kw;
-      const int iz = c.y * ds.sd - ds.pd + kz, iy = c.z * ds.sh - ds.ph + ky, ix = c.w * ds.sw - ds.pw + kx;
-      int r = -1;
-      if (iz >= 0 && iz < ds.D && iy >= 0 && iy < ds.H && ix >= 0 && ix < ds.W)
-        r = lookup(tab_in, mask_in, shift_in, lin(c.x, iz, iy, ix, ds.D, ds.H, ds.W));
-      nbr_s[q] = r;
-    } else {
-      const long long qm = q - split;
-      const int o = static_cast<int>(qm / Km), k = static_cast<int>(qm - static_cast<long long>(o) * Km);
-      const int4 c = *reinterpret_cast<const int4 *>(out_coords + static_cast<size_t>(o) * 4);
-      const int kz = k / (dm.kh * dm.kw), ky = (k / dm.kw) % dm.kh, kx = k % dm.kw;
-      const int iz = c.y - dm.pd + kz, iy = c.z - dm.ph + ky, ix = c.w - dm.pw + kx;
-      int r = -1;
-      if (kz == dm.kd / 2 && ky == dm.kh / 2 && kx == dm.kw / 2) {
-        r = o;
-      } else if (iz >= 0 && iz < dm.D && iy >= 0 && iy < dm.H && ix >= 0 && ix < dm.W) {
-        r = lookup(tab_out, mask_out, shift_out, lin(c.x, iz, iy, ix, dm.D, dm.H, dm.W));
-      }
-      nbr_m[qm] = r;
+  for (long long q = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; q < n * Km; q += stride) {
+    const int o = static_cast<int>(q / Km), k = static_cast<int>(q - static_cast<long long>(o) * Km);
+    const int4 c = *reinterpret_cast<const int4 *>(out_coords + static_cast<size_t>(o) * 4);
+    const int kz = k / (dm.kh * dm.kw), ky = (k / dm.kw) % dm.kh, kx = k % dm.kw;
+    const int iz = c.y - dm.pd + kz, iy = c.z - dm.ph + ky, ix = c.w - dm.pw + kx;
+    int r = -1;
+    if (kz == dm.kd / 2 && ky == dm.kh / 2 && kx == dm.kw / 2) {
+      r = o;
+    } else if (iz >= 0 && iz < dm.D && iy >= 0 && iy < dm.H && ix >= 0 && ix < dm.W) {
+      r = lookup(tab_out, mask_out, shift_out, lin(c.x, iz, iy, ix, dm.D, dm.H, dm.W));
     }
+    nbr_m[q] = r;
   }
 }
 
@@ -534,21 +641,32 @@ extern "C" int p3d_sparse_affine_act(const float *x, const int32_t *n_dev, int64
 // the next strided conv look coordinates up in — so every level's table is built exactly once per frame.  The
 // scratch-workspace entry points run the same code on tables carved out of their workspace.
 namespace {
+// A table of rows_cap rows: `cap` 64-bit entries (2x the rows, a power of two), then the site numbering's scratch of a
+// strided conv writing into it: a ticket and `tiles` look-back descriptors (two per input tile), at least one per 64
+// entries and never fewer than kMinTiles, so that a tile's rows and owned-tap masks fit rb_sites' shared memory for any
+// input capacity check_level accepts (2^24 rows, 125 taps: 1024 rows of 4 mask words).
+constexpr uint32_t kMinTiles = 32768;
 struct Tab {
   unsigned long long *p;
-  uint32_t cap, shift;
+  uint32_t cap, shift, tiles;
+  unsigned long long *scratch() const { return p + cap; }
 };
+uint32_t tab_cap(int64_t rows_cap) { return next_pow2(static_cast<uint64_t>(rows_cap > 512 ? rows_cap : 512) * 2); }
+uint32_t tab_tiles(uint32_t cap) { return cap / 64 > kMinTiles ? cap / 64 : kMinTiles; }
+
+size_t tab_bytes(int64_t rows_cap) {
+  const uint32_t cap = tab_cap(rows_cap);
+  return align_up((static_cast<size_t>(cap) + 1 + tab_tiles(cap)) * 8);
+}
+
 bool tab_of(void *mem, size_t bytes, int64_t rows_cap, Tab *t) {
   if (rows_cap > kMaxRows) return false;
-  t->cap = next_pow2(static_cast<uint64_t>(rows_cap > 512 ? rows_cap : 512) * 2);
+  t->cap = tab_cap(rows_cap);
+  t->tiles = tab_tiles(t->cap);
   t->shift = 32;
   for (uint32_t x = t->cap; x > 1; x >>= 1) --t->shift;
   t->p = static_cast<unsigned long long *>(mem);
-  return mem && bytes >= static_cast<size_t>(t->cap) * 8 && !(reinterpret_cast<uintptr_t>(mem) & 15);
-}
-
-size_t tab_bytes(int64_t rows_cap) {
-  return align_up(static_cast<size_t>(next_pow2(static_cast<uint64_t>(rows_cap > 512 ? rows_cap : 512) * 2)) * 8);
+  return mem && bytes >= tab_bytes(rows_cap) && !(reinterpret_cast<uintptr_t>(mem) & 15);
 }
 
 // The tables of p3d_sparse_rulebook_workspace_bytes(n_in_cap, n_out_cap): input set first, then output set.
@@ -603,22 +721,32 @@ int subm_map(const int32_t *coords, const int32_t *n_dev, int64_t n_cap, const D
   return P3D_OK;
 }
 
-// One resolution level in two launches: output sites + table `to` of the strided conv d (inputs looked up in `ti`), its
-// neighbour map and, when nbr_subm is given, the SubM map dm of the new level.
+// One resolution level in two launches: output sites + table `to` of the strided conv d (inputs looked up in `ti`) with
+// its neighbour map, then the counters and, when nbr_subm is given, the SubM map dm of the new level.
 int level_maps(const int32_t *coords, const int32_t *n_in_dev, int64_t n_in_cap, const Dims &d, const Tab &ti,
                int32_t *out_coords, int32_t *n_out_dev, int64_t out_cap, const Tab &to, int32_t *nbr, const Dims &dm,
                int32_t *nbr_subm, cudaStream_t st) {
-  const int K = d.kd * d.kh * d.kw, Km = nbr_subm ? dm.kd * dm.kh * dm.kw : 0;
+  const int Km = nbr_subm ? dm.kd * dm.kh * dm.kw : 0;
   P3D_CUDA_CHECK(cudaMemsetAsync(to.p, 0xff, static_cast<size_t>(to.cap) * 8, st));
   P3D_CUDA_CHECK(cudaMemsetAsync(n_out_dev, 0, sizeof(int32_t) * 4, st));
   if (n_in_cap > 0) {
-    rb_outputs_kernel<<<persistent_grid(n_in_cap * K), 256, 0, st>>>(coords, n_in_dev, n_in_cap, d, to.p, to.cap - 1,
-                                                                    to.shift, out_coords, n_out_dev,
-                                                                    static_cast<int>(out_cap));
+    // 32 input rows per tile (one thread per (row, tap)), wider when the tiles would not fit the scratch
+    const int words = (d.kd * d.kh * d.kw + 31) / 32;
+    const long long half = to.tiles / 2;
+    int rows = static_cast<int>(((n_in_cap + half - 1) / half + 31) / 32 * 32);
+    if (rows < 32) rows = 32;
+    if (rows > kSiteMaxRows || rows * words > kSiteMaskWords) return P3D_ERR_UNSUPPORTED;
+    const unsigned int tiles = div_up(n_in_cap, rows);
+    P3D_CUDA_CHECK(cudaMemsetAsync(to.scratch(), 0, (2 * static_cast<size_t>(tiles) + 1) * 8, st));
+    const unsigned int grid = std::min(tiles, static_cast<unsigned int>(num_sms()) * 8);
+    rb_sites_kernel<<<grid, kSiteThreads, 0, st>>>(coords, n_in_dev, n_in_cap, d, ti.p, ti.cap - 1, ti.shift, to.p,
+                                                    to.cap - 1, to.shift, out_coords, n_out_dev,
+                                                    static_cast<int>(out_cap), nbr, to.scratch(),
+                                                    static_cast<int>(tiles), rows);
     P3D_LAUNCH_CHECK();
   }
-  rb_level_neighbors_kernel<<<persistent_grid(out_cap * (K + Km)), 256, 0, st>>>(
-      out_coords, n_out_dev, out_cap, d, ti.p, ti.cap - 1, ti.shift, nbr, dm, to.p, to.cap - 1, to.shift, nbr_subm);
+  rb_level_neighbors_kernel<<<persistent_grid(out_cap * Km), 256, 0, st>>>(out_coords, n_out_dev, out_cap, dm, to.p,
+                                                                          to.cap - 1, to.shift, nbr_subm);
   P3D_LAUNCH_CHECK();
   return P3D_OK;
 }

@@ -163,7 +163,8 @@ class SparseCooTensor:
         return self.get(ROWS_F32)
 
     def indices(self):
-        """[4, cap] like paddle (columns beyond nnz() are padding)."""
+        """[4, cap] like paddle (columns beyond nnz() are padding).  The output of a strided Conv3D lists its sites in
+        first-appearance order (see Conv3D), not sorted as Paddle's does."""
         return self.index.coords.t()
 
     def nnz(self):
@@ -476,6 +477,11 @@ class SubmConv3D(_ConvBase):
 
 
 class Conv3D(_ConvBase):
+    """paddle.sparse.nn.Conv3D (strided).  The output's rows are its sites in first-appearance order: the input rows in
+    row order and, within a row, the kernel taps in order k = (kz kH + ky) kW + kx, each site listed the first time one
+    of them generates it.  The order depends only on the input index set, so the same input gives the same rows and the
+    same bits in every run; Paddle's returns the sites sorted by linear key instead.  Of input rows sharing a coordinate
+    the last stands for it; rows outside the grid generate no sites."""
     subm = False
 
 
