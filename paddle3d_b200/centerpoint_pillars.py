@@ -57,6 +57,7 @@ class CenterPointPillars:
         self.test_cfg = dict(mc["test"])
         self.label_off = synth.label_offsets(list(h["tasks"]))
         self.feat_hw, self.cat_hw = self._feature_sizes()
+        self.pfn = [dict(eps=mc["pfn"]["bn_eps"]) for _ in range(2)]  # parameters: init_weight or load_state_dict
         self.device = None
 
     def _feature_sizes(self):
@@ -78,16 +79,41 @@ class CenterPointPillars:
         rng = np.random.default_rng(seed)
         eps = self.mc["pfn"]["bn_eps"]
         self.pfn = []
-        for fan_in, c in ((self.F + 5, self.pfn_channels[0]), (2 * self.pfn_channels[0], self.pfn_channels[1])):
+        for fan_in, c in self.pfn_shapes():
             self.pfn.append(dict(weight=synth.kaiming_uniform(rng, (fan_in, c), fan_in),
                                  gamma=np.full(c, bn_gain, np.float32), beta=np.zeros(c, np.float32),
                                  mean=np.zeros(c, np.float32), var=np.ones(c, np.float32), eps=eps))
         self.head.init_weight(seed=seed + 1, device=device, bn_gain=bn_gain)
+        return self.derive(device)
+
+    def derive(self, device):
+        """The device images of the PFN parameters (self.pfn: per layer Linear weight [in, out] and BatchNorm1D
+        statistics): the weights and the folded BN.  Called after new parameters, seeded or loaded; the head derives its
+        own (DenseRPNHead.derive)."""
         self.device = None if device is None else torch.device(device)
         if device is not None:
             self.pfn_dev = [dict(l, weight=torch.from_numpy(l["weight"]).to(device)) for l in self.pfn]
             self.pfn_folded = [pe.fold_bn(l["gamma"], l["beta"], l["mean"], l["var"], l["eps"], device) for l in self.pfn]
         return self
+
+    def pfn_shapes(self):
+        """Linear weight shapes [in, out] of the two PFN layers."""
+        return [(self.F + 5, self.pfn_channels[0]), (2 * self.pfn_channels[0], self.pfn_channels[1])]
+
+    def state_dict(self):
+        """Parameters under Paddle3D's names and in its layouts (checkpoint.centerpoint_pillars)."""
+        from . import checkpoint
+        return checkpoint.state_dict(checkpoint.centerpoint_pillars(self))
+
+    def load_state_dict(self, sd, device=None):
+        """Load Paddle3D parameters (checkpoint.load_state_dict: all checked before any is assigned) and re-derive every
+        device image on `device` (default: the model's; None keeps numpy parameters only)."""
+        from . import checkpoint
+        device = self.device if device is None else device
+        checkpoint.load_state_dict(checkpoint.centerpoint_pillars(self), sd, device)
+        self.head.derive(device)
+        self.head.loaded = True
+        return self.derive(device)
 
     def export_numpy(self):
         return dict(self.head.export_numpy(), pfn=self.pfn)
@@ -115,7 +141,11 @@ class CenterPointPillars:
 
     def calibrate_heatmap_bias(self, points, target_frac=0.014):
         """DenseRPNHead.calibrate_heatmap_bias on this frame's pixel image: ~1.4 % of the cells above the score
-        threshold (SURVEY.md §8d).  Weights stay seeded and are exported unchanged to the CPU arm."""
+        threshold (SURVEY.md §8d).  Weights stay seeded and are exported unchanged to the CPU arm.  Raises on weights
+        loaded from a checkpoint."""
+        if self.head.loaded:
+            raise RuntimeError("calibrate_heatmap_bias moves the heat-map biases of seeded random weights; this model's "
+                               "weights were loaded from a checkpoint and are kept as trained")
         image, shape, _, _ = self.encode(points)
         self.head.calibrate_heatmap_bias(image, self.test_cfg["score_threshold"], target_frac, shape=shape)
         return self
@@ -145,12 +175,20 @@ class CenterPointPillarsHotPath(CapturedFrame):
     (fp16-range overflow of the pair path, with sweep input the merge's status bits)."""
 
     def __init__(self, cfg=None, device="cuda:0", seed=0, num_points=None, bn_gain=1.0, model_cfg=None,
-                 sweep_input=None, sweep_ring=None):
+                 sweep_input=None, sweep_ring=None, weights=None, share=None):
         """cfg: the point-cloud config (synth.CP_PILLARS by default); sweep_input / sweep_ring: as
-        pipeline.CenterPointHotPath (the merged columns are x, y, z, intensity and the time lag: F = 5)."""
+        pipeline.CenterPointHotPath (the merged columns are x, y, z, intensity and the time lag: F = 5).  weights: a
+        Paddle3D CenterPoint-pillars checkpoint (a `.pdparams` path or a state dict, see checkpoint.py) instead of the
+        seeded weights.  share: another frame whose model this one uses (CenterPointSweep's lanes)."""
         super().__init__(cfg or synth.CP_PILLARS, device, num_points, sweep_input, sweep_ring)
-        m = self.model = CenterPointPillars(self.cfg, model_cfg).init_weight(seed=seed, device=self.device,
-                                                                             bn_gain=bn_gain)
+        if share is not None:
+            self.share_model(share)
+        elif weights is None:
+            self.model = CenterPointPillars(self.cfg, model_cfg).init_weight(seed=seed, device=self.device, bn_gain=bn_gain)
+        else:
+            from .checkpoint import as_state_dict
+            self.model = CenterPointPillars(self.cfg, model_cfg).load_state_dict(as_state_dict(weights), self.device)
+        m = self.model
         self.slot = ResultSlot(len(m.label_off) * m.test_cfg["nms_post_max_size"], 9, len(m.label_off) + 1,
                                1 if self.sweep_input is None else 2)
 
@@ -168,6 +206,17 @@ class CenterPointPillarsHotPath(CapturedFrame):
 
     def _calibrate(self):
         self.model.calibrate_heatmap_bias(self.points)
+
+    def state_dict(self):
+        return self.model.state_dict()
+
+    def load_state_dict(self, sd):
+        """CenterPointPillars.load_state_dict on the frame's device.  Before capture(): a captured graph reads the images
+        it was captured with."""
+        if self.graph is not None:
+            raise RuntimeError("load_state_dict after capture(): load the weights first, then capture")
+        self.model.load_state_dict(sd, self.device)
+        return self
 
     def check_status(self, status_host):
         """Raise when the frame's status word reports dropped rows or an activation outside fp16's range (never a silent

@@ -38,14 +38,12 @@ class _Conv:
         """Seeded parameters (numpy); with a device also the packed tensor-core image and the folded epilogue."""
         cin, cout, k = self.cin, self.cout, self.k
         bound = 1.0 / np.sqrt(cin * k * k)  # build_conv_layer "uniform" (second_backbone.py:43-48)
-        shape = (cin, cout, k, k) if self.transposed else (cout, cin, k, k)
-        w = rng.uniform(-bound, bound, size=shape).astype(np.float32)
+        w = rng.uniform(-bound, bound, size=self.weight_shape()).astype(np.float32)
         b = None
         if self.has_bias:
             b = (np.full(cout, bias_value, np.float32) if bias_value is not None
                  else rng.uniform(-bound, bound, size=cout).astype(np.float32))
-        p = dict(weight=w, bias=b, stride=self.stride, padding=self.padding, up=self.up, relu=self.relu, bn=None,
-                 transposed=self.transposed)
+        bn = None
         if self.bn_eps is not None:
             if randomize_bn:
                 g, bt = rng.uniform(0.5, 1.5, cout), rng.uniform(-0.2, 0.2, cout)
@@ -53,9 +51,26 @@ class _Conv:
             else:
                 g, bt, m, v = np.ones(cout), np.zeros(cout), np.zeros(cout), np.ones(cout)
             g = g * bn_gain
-            p["bn"] = dict(gamma=g.astype(np.float32), beta=bt.astype(np.float32), mean=m.astype(np.float32),
-                           var=v.astype(np.float32), eps=self.bn_eps)
+            bn = dict(gamma=g.astype(np.float32), beta=bt.astype(np.float32), mean=m.astype(np.float32),
+                      var=v.astype(np.float32))
+        return self.set_parameters(w, b, bn, device)
+
+    def weight_shape(self):
+        """Paddle's weight layout: [Cin, Cout, k, k] for a Conv2DTranspose, [Cout, Cin, k, k] for a Conv2D."""
+        return (self.cin, self.cout, self.k, self.k) if self.transposed else (self.cout, self.cin, self.k, self.k)
+
+    def set_parameters(self, w, b=None, bn=None, device=None):
+        """Parameters in Paddle's layouts, float32 numpy: weight (weight_shape()), bias [Cout] (with bias), bn dict gamma /
+        beta / mean / var [Cout] (with BatchNorm).  They become self.np and, with a device, the packed tensor-core image
+        and the folded epilogue (self.dev); without one self.dev is left as it is."""
+        cout, shape = self.cout, self.weight_shape()
+        p = dict(weight=w, bias=b, stride=self.stride, padding=self.padding, up=self.up, relu=self.relu, bn=None,
+                 transposed=self.transposed)
+        if self.bn_eps is not None:
+            p["bn"] = dict(bn, eps=self.bn_eps)
         self.np = p
+        if device is None:
+            return self
         # fold: y = conv * s + ((bias - mean) * s + beta), s = gamma / sqrt(var + eps)   (fp64 on the host)
         s = np.ones(cout)
         t = np.zeros(cout) if b is None else b.astype(np.float64)
@@ -63,17 +78,15 @@ class _Conv:
             bn = p["bn"]
             s = bn["gamma"].astype(np.float64) / np.sqrt(bn["var"].astype(np.float64) + bn["eps"])
             t = (t - bn["mean"]) * s + bn["beta"]
-        if device is None:
-            return self
         if self.f16:
             pack = dc.pack_deconv_weight_f16 if self.transposed else dc.pack_conv_weight_f16
         else:
             pack = dc.pack_deconv_weight if self.transposed else dc.pack_conv_weight
         wd = w
-        if self.cin_pad and self.cin_pad > cin:
+        if self.cin_pad and self.cin_pad > self.cin:
             ax = 0 if self.transposed else 1
             wd = np.zeros(shape[:ax] + (self.cin_pad,) + shape[ax + 1:], np.float32)
-            wd[(slice(None),) * ax + (slice(0, cin),)] = w
+            wd[(slice(None),) * ax + (slice(0, self.cin),)] = w
         if self.cout_pad and self.cout_pad > cout:
             if self.transposed:
                 raise ValueError("cout_pad: Conv2D weights only")
@@ -207,6 +220,7 @@ class DenseRPNHead:
                            conv(share_conv_channel, c, 3, 1, 1, bias=True, relu=False)))
             self.heads.append(hs)
         self._batched = None
+        self.loaded = False  # parameters from a checkpoint (checkpoint.load_state_dict), not seeded
 
     def all_convs(self):
         out = self.trunk.convs() + [self.shared]
@@ -237,11 +251,21 @@ class DenseRPNHead:
         gamma (sqrt(6) keeps the activations O(1) through the stack, see sparse_nn.BatchNorm.init_parameters)."""
         rng = np.random.default_rng(seed)
         hm_finals = {id(b) for hs in self.heads for name, _, b in hs if name == "hm"}
-        finals = {id(b) for hs in self.heads for _, _, b in hs}
+        finals = {id(b) for b in self.finals()}
         for c in self.all_convs():  # hm bias = -2.19 (center_head.py:113-117)
             # the 1-3 channel output convs have no per-conv image in f16 mode: they run in one tap-as-N launch
             dev = None if (self.f16 and id(c) in finals) else device
             c.init(rng, dev, randomize_bn, bias_value=-2.19 if id(c) in hm_finals else None, bn_gain=bn_gain)
+        return self.derive(device)
+
+    def finals(self):
+        """The output convs: in f16 mode they have no per-conv device image (they run in one tap-as-N launch)."""
+        return [f for hs in self.heads for _, _, f in hs]
+
+    def derive(self, device):
+        """The device state that is derived from the whole model's parameters (each conv's own image comes from
+        _Conv.set_parameters): the permuted first conv of the (z, c) pixel input, and (on the next forward) the batched
+        ConvModule conv and the tap-as-N output-conv images.  Called after new parameters, seeded or loaded."""
         self._batched = None
         self._first_zc = None
         # bev_depth 1 (pillars): the (z, c) order is the (c, z) order, the first conv reads the pixel rows as it is
@@ -380,6 +404,9 @@ class DenseRPNHead:
         every task's heat-map conv so that `target_frac` of the cells of `bev`'s frame score above `score_threshold`
         (weights stay seeded and are exported unchanged to the CPU arm).  bev: as forward() takes it (with `shape`, pixel
         fp16-pair rows)."""
+        if self.loaded:
+            raise RuntimeError("calibrate_heatmap_bias moves the heat-map biases of seeded random weights; this head's "
+                               "weights were loaded from a checkpoint and are kept as trained")
         out = self.forward(bev, shape)
         logit_thr = float(np.log(score_threshold / (1.0 - score_threshold)))
         for t, hs in enumerate(self.heads):

@@ -4,7 +4,8 @@
     Predictor(...).run(points)                      infer.py:163-189  -> (box3d_lidar [K, 9], label_preds [K], scores [K]) on the host
     parse_result(box3d_lidar, label_preds, scores)  infer.py:139-160  the reference's text format, fake rows (score -1) skipped
 
-The predictor is `CenterPointHotPath` behind the reference's three-output contract (the exported model's outputs are
+The predictor is `CenterPointHotPath` (with the weights of a `.pdparams` checkpoint, or seeded ones) behind the
+reference's three-output contract (the exported model's outputs are
 box3d_lidar, label_preds, scores in that order, infer.py:180-188).  A frame may hold fewer points than the capacity the
 pipeline was captured for: the tail of the device buffer is filled with NaN rows, which `hard_voxelize` drops exactly
 like the reference drops out-of-range points (voxelize_op.cc:37-45 -> csrc/voxelize.cu cell_of).  Host code, as in the
@@ -63,7 +64,9 @@ class Predictor:
 
     def __init__(self, cfg=None, device="cuda:0", max_points=None, seed=0, precision=None, with_head=True, weights=None,
                  sweep_input=None):
-        """sweep_input: see CenterPointHotPath; the predictor then takes raw sweeps (run_sweeps) instead of points."""
+        """weights: a trained Paddle3D CenterPoint-voxel checkpoint, a `.pdparams` path or a state dict (checkpoint.py;
+        needs with_head=True), in place of the seeded weights of `seed`.  sweep_input: see CenterPointHotPath; the
+        predictor then takes raw sweeps (run_sweeps) instead of points."""
         import torch
         from . import synth
         from .ops import sparse_nn as sp
@@ -71,7 +74,7 @@ class Predictor:
         self.torch = torch
         self.cfg = dict(cfg or synth.C3)
         self.pipe = CenterPointHotPath(self.cfg, device, precision=sp.F16X3 if precision is None else precision, seed=seed,
-                                       num_points=max_points, with_head=with_head, sweep_input=sweep_input)
+                                       num_points=max_points, with_head=with_head, sweep_input=sweep_input, weights=weights)
         self.host = torch.empty((self.pipe.n, self.pipe.F), dtype=torch.float32).pin_memory()
         self.captured = False
 

@@ -366,10 +366,18 @@ class _ConvBase(_Layer):
         fan_in = self.in_channels * kd * kh * kw
         bound = math.sqrt(6.0 / ((1 + 5.0) * fan_in))
         w = rng.uniform(-bound, bound, size=(kd, kh, kw, self.in_channels, self.out_channels)).astype(np.float32)
-        self.weight = torch.from_numpy(w).to(device)
+        b = None
         if self.bias is not None:
             b = rng.uniform(-1 / math.sqrt(fan_in), 1 / math.sqrt(fan_in), size=(self.out_channels,)).astype(np.float32)
-            self.bias = torch.from_numpy(b).to(device)
+        return self.assign_parameters(torch.from_numpy(w).to(device), None if b is None else torch.from_numpy(b).to(device))
+
+    def assign_parameters(self, weight, bias):
+        """New parameter tensors on any device (weight [kD, kH, kW, Cin, Cout], bias [Cout] or None for a layer without
+        one).  The packed images of the old weights are dropped: their cache key, the weight's data_ptr, can come back
+        for a new tensor at a reused address."""
+        self.weight, self.bias = weight, bias
+        for attr in ("_packed", "_packed_f16", "_packed_wm"):
+            self.__dict__.pop(attr, None)
         return self
 
     def _packed_weight(self, K, f16=False, wm=False):
@@ -400,9 +408,8 @@ class _ConvBase(_Layer):
         return pk[1]
 
     def set_parameters(self, weight, bias=None):
-        self.weight = require_cuda(weight, "weight", torch.float32)
-        self.bias = require_cuda(bias, "bias", torch.float32) if bias is not None else None
-        return self
+        return self.assign_parameters(require_cuda(weight, "weight", torch.float32),
+                                      require_cuda(bias, "bias", torch.float32) if bias is not None else None)
 
     def build_index(self, src):
         """Strided conv: output site set + neighbour map of `src` under this layer's geometry (cached on `src`)."""
@@ -510,6 +517,7 @@ class BatchNorm(_Layer):
 
     def set_parameters(self, weight, bias, mean, variance):
         self.weight, self.bias, self._mean, self._variance = weight, bias, mean, variance
+        self._bias_fold = {}  # keyed on the conv bias' data_ptr, which a new tensor can reuse
         # fold once, in fp64 on the host side of the parameters (tiny): y = x*scale + shift
         w, b, m, v = [t.double() for t in (weight, bias, mean, variance)]
         scale = w / torch.sqrt(v + self.epsilon)

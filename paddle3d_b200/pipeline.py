@@ -22,25 +22,42 @@ from .ops import voxelize as vox
 
 class CenterPointHotPath(CapturedFrame):
     def __init__(self, cfg=None, device="cuda:0", precision=sp.FP32, seed=0, num_points=None, level_caps=None,
-                 head_seed=0, with_head=False, keep_bev=True, bn_gain=1.0, sweep_input=None, sweep_ring=None):
-        """sweep_input / sweep_ring: see frame.CapturedFrame."""
+                 head_seed=0, with_head=False, keep_bev=True, bn_gain=1.0, sweep_input=None, sweep_ring=None, weights=None,
+                 share=None):
+        """sweep_input / sweep_ring: see frame.CapturedFrame.  weights: a Paddle3D CenterPoint-voxel checkpoint (a
+        `.pdparams` path or a state dict, see checkpoint.py) instead of the seeded weights; needs with_head=True.
+        share: another CenterPointHotPath whose model (weights, packed images) this frame uses, built by it (weights,
+        seed, bn_gain and precision are then ignored; CenterPointSweep's lanes)."""
         super().__init__(cfg or synth.C3, device, num_points, sweep_input, sweep_ring)
+        if weights is not None and not with_head:
+            raise ValueError("weights: a CenterPoint checkpoint holds the dense RPN / neck / CenterHead as well; build the "
+                             "frame with with_head=True")
         self.test_cfg = dict(synth.CENTERPOINT_TEST_CFG)
         self.label_off = synth.label_offsets()
-        self.net = SparseResNet3D(self.F, self.cfg["voxel_size"], self.cfg["point_cloud_range"])
-        self.net.init_weight(seed=seed, device=self.device, bn_gain=bn_gain).set_precision(precision)
-        V = self.cfg["max_voxels"]
-        self.net.set_level_caps(level_caps or [3 * V, 3 * V, 2 * V, V])
         h = synth.centerpoint_head_outputs(head_seed)
         self.head_host = h
         self.head = {k: [torch.from_numpy(x).to(self.device) for x in v] for k, v in h.items()}
         # with_head: run the dense RPN / neck / CenterHead (dense_head.DenseRPNHead, SURVEY §8f-1) on the BEV tensor and
         # feed ITS outputs to the postprocess instead of the resident synthetic head tensors (parity-green per layer and
         # as a small network; this whole-frame composition has not been timed yet, hence off by default)
-        self.dense = None
-        if with_head:
-            from .dense_head import DenseRPNHead
-            self.dense = DenseRPNHead(in_channels=128 * 2).init_weight(seed=seed + 1, device=self.device, bn_gain=bn_gain)
+        if share is not None:
+            self.share_model(share)
+        else:
+            self.net = SparseResNet3D(self.F, self.cfg["voxel_size"], self.cfg["point_cloud_range"])
+            self.dense = None
+            if with_head:
+                from .dense_head import DenseRPNHead
+                self.dense = DenseRPNHead(in_channels=128 * 2)
+            if weights is None:
+                self.net.init_weight(seed=seed, device=self.device, bn_gain=bn_gain)
+                if self.dense is not None:
+                    self.dense.init_weight(seed=seed + 1, device=self.device, bn_gain=bn_gain)
+            else:
+                from .checkpoint import as_state_dict
+                self.load_state_dict(as_state_dict(weights))
+            self.net.set_precision(precision)
+            V = self.cfg["max_voxels"]
+            self.net.set_level_caps(level_caps or [3 * V, 3 * V, 2 * V, V])
         # keep_bev=False (with the fp16-pair dense head): the sparse rows go straight into the pixel fp16-pair image the RPN
         # reads; the reference's fp32 NCHW BEV tensor is then not materialised in the frame (bev_nchw() rebuilds it on demand)
         self.keep_bev = keep_bev or self.dense is None or not self.dense.f16
@@ -69,7 +86,7 @@ class CenterPointHotPath(CapturedFrame):
         boxes, scores, labels, counts = cpp.centerpoint_postprocess_heads(h, cfg["voxel_size"][:2], cfg["point_cloud_range"],
                                                                           self.test_cfg, self.label_off)
         return dict(bev=bev, bev_h16=bev_h16, boxes=boxes, scores=scores, labels=labels, counts=counts, num_voxels=nv,
-                    coors=coors, mean=mean, status=status)
+                    coors=coors, mean=mean, status=status, head=h)
 
     def bev_nchw(self):
         """The dense BEV tensor [1, 256, H, W] fp32 of the last frame (rebuilt from the pixel fp16-pair image when the
@@ -91,9 +108,12 @@ class CenterPointHotPath(CapturedFrame):
     def calibrate_head(self, points_dev):
         """Shift the heat-map biases of the (randomly initialised) dense head so that ~1.4 % of the BEV cells of this frame
         score above the threshold, as SURVEY.md §8d specifies for the synthetic workload (see
-        DenseRPNHead.calibrate_heatmap_bias).  Call before capture()."""
+        DenseRPNHead.calibrate_heatmap_bias).  Call before capture(); raises on weights loaded from a checkpoint."""
         if self.dense is None:
             return self
+        if self.dense.loaded:
+            raise RuntimeError("calibrate_head moves the heat-map biases of seeded random weights; this frame's weights "
+                               "were loaded from a checkpoint and are kept as trained")
         cfg = self.cfg
         with torch.cuda.stream(self.stream):
             self.points.copy_(points_dev)
@@ -120,6 +140,26 @@ class CenterPointHotPath(CapturedFrame):
 
     def share_model(self, other):
         self.net, self.dense = other.net, other.dense
+
+    def state_dict(self):
+        """The model's parameters under Paddle3D's names and in its layouts (checkpoint.centerpoint_voxel)."""
+        from . import checkpoint
+        if self.dense is None:
+            raise ValueError("state_dict: a frame without the dense head (with_head=False) is not a whole CenterPoint")
+        return checkpoint.state_dict(checkpoint.centerpoint_voxel(self.net, self.dense))
+
+    def load_state_dict(self, sd):
+        """Load Paddle3D CenterPoint-voxel parameters (checkpoint.load_state_dict: all checked before any is assigned)
+        and re-derive every device image.  Before capture(): a captured graph reads the images it was captured with."""
+        from . import checkpoint
+        if self.dense is None:
+            raise ValueError("load_state_dict: a frame without the dense head (with_head=False) is not a whole CenterPoint")
+        if self.graph is not None:
+            raise RuntimeError("load_state_dict after capture(): load the weights first, then capture")
+        checkpoint.load_state_dict(checkpoint.centerpoint_voxel(self.net, self.dense), sd, self.device)
+        self.dense.derive(self.device)
+        self.dense.loaded = True
+        return self
 
     def export_weights_numpy(self):
         """Weights as plain numpy dicts for the CPU arm (oracle.cpu_reference.CpuFrame)."""
@@ -152,11 +192,14 @@ class CenterPointSweep:
     """
 
     def __init__(self, lanes=2, frame_cls=None, **kw):
-        """frame_cls: the hot-path class of each lane (default CenterPointHotPath; pointpillars.PointPillarsHotPath)."""
+        """frame_cls: the hot-path class of each lane (default CenterPointHotPath; pointpillars.PointPillarsHotPath,
+        centerpoint_pillars.CenterPointPillarsHotPath).  kw: the frame's arguments; weights= (a checkpoint) is loaded
+        once, into lane 0's model, which every lane shares."""
         if lanes < 1:
             raise ValueError("lanes >= 1")
         frame_cls = frame_cls or CenterPointHotPath
-        first = frame_cls(**kw)
+        first = frame_cls(**kw)  # weights= (a checkpoint path) is read here, once
+        kw.pop("weights", None)
         if kw.get("sweep_input") is not None and kw.get("sweep_ring") is None:
             # one ring for all lanes, K + lanes slots: a slot is reused only after its last reader's result was read
             from .sweep_ring import SweepRing
@@ -165,9 +208,8 @@ class CenterPointSweep:
             kw = dict(kw, sweep_ring=first.ring)
         self.lanes = [first]
         for _ in range(lanes - 1):
-            p = frame_cls(**kw)
-            p.share_model(first)  # one model: calibration / weight loading happens once, on lane 0
-            self.lanes.append(p)
+            # one model: built, loaded and calibrated once, on lane 0; the other lanes build none
+            self.lanes.append(frame_cls(share=first, **kw))
         self.device = first.device
 
     def __len__(self):

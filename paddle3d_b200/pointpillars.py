@@ -127,7 +127,9 @@ class PointPillars:
             raise ValueError("model config: one anchor generator per class, anchors_per_loc anchors per location")
         self.corners_np = anchor_voxel_corners(self.anchors_np, self.cfg["voxel_size"], self.cfg["point_cloud_range"],
                                                self.grid)
+        self.pfn = dict(eps=mc["pfn_bn_eps"])  # parameters: init_weight or load_state_dict
         self.device = None
+        self.loaded = False  # parameters from a checkpoint (load_state_dict), not seeded
 
     def init_weight(self, seed=0, device="cuda", bn_gain=1.0):
         """device=None: numpy parameters only (enough for export_numpy / the CPU arm).  bn_gain multiplies every
@@ -140,6 +142,12 @@ class PointPillars:
         for c in self.trunk.convs():
             c.init(rng, device, bn_gain=bn_gain)
         self.head.init(rng, device)
+        return self.derive(device)
+
+    def derive(self, device):
+        """The device images of the PFN parameters (self.pfn: Linear weight [in, out] and BatchNorm1D statistics), and the
+        constant anchors.  Called after new parameters, seeded or loaded; each conv derives its own
+        (_Conv.set_parameters)."""
         self.device = None if device is None else torch.device(device)
         if device is not None:
             p = self.pfn
@@ -148,6 +156,25 @@ class PointPillars:
             self.anchors = torch.from_numpy(np.ascontiguousarray(self.anchors_np)).to(device)
             self.corners = torch.from_numpy(np.ascontiguousarray(self.corners_np)).to(device)
         return self
+
+    def head_splits(self):
+        """(name, output channels) of the SSD head's three convs in the order the one head conv concatenates them."""
+        R, mc = self.mc["anchors_per_loc"], self.mc
+        return [("cls", R * self.num_classes), ("box", R * mc["box_code_size"]), ("dir", R * mc["num_dir_bins"])]
+
+    def state_dict(self):
+        """Parameters under Paddle3D's names and in its layouts (checkpoint.pointpillars)."""
+        from . import checkpoint
+        return checkpoint.state_dict(checkpoint.pointpillars(self))
+
+    def load_state_dict(self, sd, device=None):
+        """Load Paddle3D parameters (checkpoint.load_state_dict: all checked before any is assigned) and re-derive every
+        device image on `device` (default: the model's; None keeps numpy parameters only)."""
+        from . import checkpoint
+        device = self.device if device is None else device
+        checkpoint.load_state_dict(checkpoint.pointpillars(self), sd, device)
+        self.loaded = True
+        return self.derive(device)
 
     def export_numpy(self):
         return dict(self.trunk.export_numpy(), pfn=self.pfn, head=self.head.np)
@@ -187,6 +214,9 @@ class PointPillars:
         all anchors pass the anchor mask AND the threshold in that class on this frame (at most 2 % together; about 2.1k
         for the car): more than nms_pre_max_size = 1000, so the top-k cut runs, and every class has candidates, so every
         label reaches the output.  Weights stay seeded and are exported unchanged to the CPU arm."""
+        if self.loaded:
+            raise RuntimeError("calibrate_cls_bias moves the cls biases of seeded random weights; this model's weights "
+                               "were loaded from a checkpoint and are kept as trained")
         image, shape, coors, nv = self.encode(points)
         planes = self.dense(image, shape)
         mask = torch.empty((self.anchors.shape[0],), dtype=torch.uint8, device=planes.device)
@@ -229,11 +259,20 @@ class PointPillarsHotPath(CapturedFrame):
     """One PointPillars frame on one GPU: H2D -> [captured: hard_voxelize -> PFN -> pixel image -> trunk -> head conv ->
     anchor postprocess] -> D2H of boxes [300, 7], scores, labels, counts (candidates, rows) and the status word."""
 
-    def __init__(self, cfg=None, device="cuda:0", seed=0, num_points=None, bn_gain=1.0, model_cfg=None):
+    def __init__(self, cfg=None, device="cuda:0", seed=0, num_points=None, bn_gain=1.0, model_cfg=None, weights=None,
+                 share=None):
         """cfg: the point-cloud config (synth.C2 by default); model_cfg: the model config (CONFIG by default; synth.C2 with
-        CONFIG is the car model, synth.C2_PED_CYCLIST with CONFIG_PED_CYCLIST the cyclist / pedestrian one)."""
+        CONFIG is the car model, synth.C2_PED_CYCLIST with CONFIG_PED_CYCLIST the cyclist / pedestrian one).  weights: a
+        Paddle3D PointPillars checkpoint of that model (a `.pdparams` path or a state dict, see checkpoint.py) instead of
+        the seeded weights.  share: another frame whose model this one uses (pipeline.CenterPointSweep's lanes)."""
         super().__init__(cfg or synth.C2, device, num_points)
-        self.model = PointPillars(self.cfg, model_cfg).init_weight(seed=seed, device=self.device, bn_gain=bn_gain)
+        if share is not None:
+            self.share_model(share)
+        elif weights is None:
+            self.model = PointPillars(self.cfg, model_cfg).init_weight(seed=seed, device=self.device, bn_gain=bn_gain)
+        else:
+            from .checkpoint import as_state_dict
+            self.model = PointPillars(self.cfg, model_cfg).load_state_dict(as_state_dict(weights), self.device)
         self.slot = ResultSlot(self.model.mc["test"]["nms_post_max_size"], 7, 2, 1)
 
     def forward_device(self):
@@ -247,6 +286,17 @@ class PointPillarsHotPath(CapturedFrame):
 
     def _calibrate(self):
         self.model.calibrate_cls_bias(self.points)
+
+    def state_dict(self):
+        return self.model.state_dict()
+
+    def load_state_dict(self, sd):
+        """PointPillars.load_state_dict on the frame's device.  Before capture(): a captured graph reads the images it
+        was captured with."""
+        if self.graph is not None:
+            raise RuntimeError("load_state_dict after capture(): load the weights first, then capture")
+        self.model.load_state_dict(sd, self.device)
+        return self
 
     @staticmethod
     def check_status(status_host):
