@@ -619,6 +619,22 @@ int p3d_merge_sweeps(const float *raw, int num_slots, int64_t slot_cap, int raw_
                      float sweep_remove_radius, float *out, int64_t cap, int32_t *n_out_dev, int32_t *status_dev,
                      void *workspace, size_t workspace_bytes, p3d_stream_t stream);
 
+/* merge_sweeps_frustum  p3d_merge_sweeps of one entry (the key cloud, no transform, no removal square) that also drops
+ *                   every row outside the KITTI left colour camera's view frustum: Paddle3D's
+ *                   RemoveCameraInvisiblePointsKITTI, SECOND's remove_outside_points (host oracle and plane builder:
+ *                   paddle3d_b200/kitti.py).
+ *   planes_dev [6][4] fp64 (device, 8-byte aligned), read on every launch: (a, b, c, d) per plane, normals outward.
+ *   A row is kept iff for every plane  ((x * a + y * b) + z * c) + d < 0  is not false, i.e. !(v >= 0): x, y, z are the
+ *   selected columns 0..2 widened from fp32, each product and sum rounded in fp64 (no FMA contraction).  So a row with
+ *   a NaN coordinate is KEPT (hard_voxelize drops it later) and a row exactly on a plane is DROPPED.  Kept rows keep
+ *   their order.  num_entries != 1 returns P3D_ERR_UNSUPPORTED.  Capacity, NaN tail, n_out and the status bits are
+ *   p3d_merge_sweeps': bit 0 = more than cap rows were kept (the rows beyond cap dropped), bit 1 = a bad entry. */
+int p3d_merge_sweeps_frustum(const float *raw, int num_slots, int64_t slot_cap, int raw_dim, const p3d_sweep_desc *desc,
+                             int num_entries, const int32_t *use_dim_host, int n_use_dim, int use_time_lag,
+                             float sweep_remove_radius, float *out, int64_t cap, int32_t *n_out_dev,
+                             int32_t *status_dev, void *workspace, size_t workspace_bytes, p3d_stream_t stream,
+                             const double *planes_dev);
+
 /* ---------------------------------------------------------------------------------------------
  * Baseline JPEG decode to uint8 RGB rows, bit-identical to libjpeg-turbo's C paths (jpeg_idct_islow, fancy upsampling,
  * ycc_rgb_convert) that PIL.Image.open runs.  Supported: SOF0 / SOF1 Huffman DCT, 8-bit, three components Y Cb Cr in

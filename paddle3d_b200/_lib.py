@@ -119,6 +119,8 @@ SIGNATURES = {
     "p3d_merge_sweeps_workspace_bytes": (_sz, [_int, _i64]),
     "p3d_merge_sweeps": (_int, [_vp, _int, _i64, _int, _vp, _int, _vp, _int, _int, _f, _vp, _i64, _vp, _vp, _vp, _sz,
                                 _vp]),
+    "p3d_merge_sweeps_frustum": (_int, [_vp, _int, _i64, _int, _vp, _int, _vp, _int, _int, _f, _vp, _i64, _vp, _vp, _vp,
+                                        _sz, _vp, _vp]),
     "p3d_jpeg_decode_workspace_bytes": (_sz, [_int, _int, _int, _i64]),
     "p3d_jpeg_decode_u8": (_int, [_vp, _i64, _vp, _int, _int, _int, _int, _int, _i64, _vp, _vp, _vp, _sz, _vp]),
     "p3d_hard_vfe": (_int, [_vp, _vp, _vp, _vp, _i64, _int, _int, _int, _vp, _vp, _vp, _int, _vp, _vp, _vp, _vp, _vp, _vp,

@@ -14,6 +14,11 @@
 //                    streams them out as 16-byte stores.
 //   K2 merge_tail    (PDL) NaN rows from n_out to cap - hard_voxelize drops them - and the status word.
 //
+// The frustum instantiation (p3d_merge_sweeps_frustum, one entry) is the KITTI camera cull of Paddle3D's
+// RemoveCameraInvisiblePointsKITTI / SECOND's remove_outside_points: the keep stage also tests each row against six
+// planes read from the device on every launch (one captured graph serves every calibration and image size), in the
+// reference's fp64 arithmetic, unfused; paddle3d_b200/kitti.py remove_camera_invisible is its oracle.
+//
 // Bandwidth-bound: 4 * raw_dim * rows bytes read, 4 * F * cap bytes written.
 #include <math.h>
 
@@ -50,6 +55,7 @@ MergeWs carve_merge(void *ws, long long tiles) {
   return w;
 }
 
+template <bool kFrustum>
 __global__ void __launch_bounds__(kMergeBlock) merge_sweeps_kernel(const float *__restrict__ raw, int num_slots,
                                                                    long long slot_cap,
                                                                    const p3d_sweep_desc *__restrict__ desc,
@@ -57,9 +63,11 @@ __global__ void __launch_bounds__(kMergeBlock) merge_sweeps_kernel(const float *
                                                                    float *__restrict__ out, long long cap,
                                                                    unsigned long long *__restrict__ scan,
                                                                    int32_t *__restrict__ flags,
-                                                                   int32_t *__restrict__ n_out) {
+                                                                   int32_t *__restrict__ n_out,
+                                                                   const double *__restrict__ planes) {
   extern __shared__ __align__(16) float s_mem[];
   __shared__ double s_m[12];
+  __shared__ double s_pl[kFrustum ? 24 : 1];  // frustum: six (a, b, c, d) planes, outward normals
   __shared__ int s_col[kMaxCols];
   __shared__ int s_cnt[kMergeItems * kMergeWarps];
   __shared__ unsigned int s_bid;
@@ -92,6 +100,7 @@ __global__ void __launch_bounds__(kMergeBlock) merge_sweeps_kernel(const float *
   __syncthreads();
   const int e = s_entry, nr = s_nr;
   if (tid < 12) s_m[tid] = desc[e].ref_from_curr[tid];  // read after the next barrier
+  if (kFrustum && tid < 24) s_pl[tid] = planes[tid];
   // stage the tile's raw rows: 16-byte loads (slot_cap % 4 == 0, tiles start at multiples of 1024 rows)
   if (nr > 0) {
     const float *src = raw + s_src;
@@ -111,6 +120,17 @@ __global__ void __launch_bounds__(kMergeBlock) merge_sweeps_kernel(const float *
     if (keep && e > 0) {
       const float x = s_in[r * RD + s_col[0]], y = s_in[r * RD + s_col[1]];
       keep = !(fabsf(x) < R && fabsf(y) < R);  // reader.py:143-150, NaN rows are kept as numpy keeps them
+    }
+    if (kFrustum && keep) {
+      // points_in_convex_polygon_3d_jit: fp32 x, y, z widened to fp64, ((x a + y b) + z c) + d per plane, no FMA
+      // contraction; a row is dropped when any plane gives >= 0, so NaN rows are kept and rows on a plane dropped
+      const double x = s_in[r * RD + s_col[0]], y = s_in[r * RD + s_col[1]], z = s_in[r * RD + s_col[2]];
+#pragma unroll
+      for (int p = 0; p < 6; ++p) {
+        const double *q = s_pl + 4 * p;
+        const double v = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(x, q[0]), __dmul_rn(y, q[1])), __dmul_rn(z, q[2])), q[3]);
+        keep = keep && !(v >= 0.0);
+      }
     }
     ball[k] = __ballot_sync(0xffffffffu, keep);
     if (lane == 0) s_cnt[k * kMergeWarps + wid] = __popc(ball[k]);
@@ -209,16 +229,21 @@ extern "C" size_t p3d_merge_sweeps_workspace_bytes(int num_entries, int64_t slot
   return carve_merge(nullptr, merge_tiles(num_entries, slot_cap)).bytes;
 }
 
-extern "C" int p3d_merge_sweeps(const float *raw, int num_slots, int64_t slot_cap, int raw_dim,
-                                const p3d_sweep_desc *desc, int num_entries, const int32_t *use_dim_host, int n_use_dim,
-                                int use_time_lag, float sweep_remove_radius, float *out, int64_t cap, int32_t *n_out_dev,
-                                int32_t *status_dev, void *workspace, size_t workspace_bytes, p3d_stream_t stream) {
+namespace {
+
+template <bool kFrustum>
+int merge_sweeps_impl(const float *raw, int num_slots, int64_t slot_cap, int raw_dim, const p3d_sweep_desc *desc,
+                      int num_entries, const int32_t *use_dim_host, int n_use_dim, int use_time_lag,
+                      float sweep_remove_radius, float *out, int64_t cap, int32_t *n_out_dev, int32_t *status_dev,
+                      void *workspace, size_t workspace_bytes, p3d_stream_t stream, const double *planes_dev) {
   if (!desc || !out || !n_out_dev || !status_dev || !workspace || num_entries < 1 || num_slots < 1 || slot_cap < 0 ||
       raw_dim < 3 || n_use_dim < 0 || cap < 0 || (n_use_dim && !use_dim_host) || (!raw && slot_cap))
     return P3D_ERR_INVALID_ARG;
   if ((slot_cap & 3) || (reinterpret_cast<uintptr_t>(raw) & 15) || (reinterpret_cast<uintptr_t>(out) & 15) ||
       (reinterpret_cast<uintptr_t>(workspace) & 255))
     return P3D_ERR_INVALID_ARG;
+  if (kFrustum && (!planes_dev || (reinterpret_cast<uintptr_t>(planes_dev) & 7))) return P3D_ERR_INVALID_ARG;
+  if (kFrustum && num_entries != 1) return P3D_ERR_UNSUPPORTED;  // the cull is defined on one untransformed cloud
   MergeAttrs a;
   a.raw_dim = raw_dim;
   a.ncol = n_use_dim ? n_use_dim : raw_dim;
@@ -242,12 +267,33 @@ extern "C" int p3d_merge_sweeps(const float *raw, int num_slots, int64_t slot_ca
   const int tpe = static_cast<int>(tiles / num_entries);
   P3D_CUDA_CHECK(cudaMemsetAsync(workspace, 0, w.bytes, st));
   const size_t smem = static_cast<size_t>(kMergeTile) * (raw_dim + a.F) * sizeof(float);
-  P3D_CUDA_CHECK(launch_pdl(merge_sweeps_kernel, dim3(static_cast<unsigned int>(tiles)), dim3(kMergeBlock), smem, st, raw,
-                            num_slots, static_cast<long long>(slot_cap), desc, tpe, a, out, static_cast<long long>(cap),
-                            w.scan, w.flags, n_out_dev));
+  P3D_CUDA_CHECK(launch_pdl(merge_sweeps_kernel<kFrustum>, dim3(static_cast<unsigned int>(tiles)), dim3(kMergeBlock), smem,
+                            st, raw, num_slots, static_cast<long long>(slot_cap), desc, tpe, a, out,
+                            static_cast<long long>(cap), w.scan, w.flags, n_out_dev, planes_dev));
   const long long tail = (cap * a.F + 4 * 256 - 1) / (4 * 256);
   const unsigned int tail_blocks = static_cast<unsigned int>(tail < 1 ? 1 : (tail > num_sms() * 4 ? num_sms() * 4 : tail));
   P3D_CUDA_CHECK(launch_pdl(merge_tail_kernel, dim3(tail_blocks), dim3(256), 0, st, out, static_cast<long long>(cap), a.F,
                             static_cast<const int32_t *>(n_out_dev), static_cast<const int32_t *>(w.flags), status_dev));
   return P3D_OK;
+}
+
+}  // namespace
+
+extern "C" int p3d_merge_sweeps(const float *raw, int num_slots, int64_t slot_cap, int raw_dim,
+                                const p3d_sweep_desc *desc, int num_entries, const int32_t *use_dim_host, int n_use_dim,
+                                int use_time_lag, float sweep_remove_radius, float *out, int64_t cap, int32_t *n_out_dev,
+                                int32_t *status_dev, void *workspace, size_t workspace_bytes, p3d_stream_t stream) {
+  return merge_sweeps_impl<false>(raw, num_slots, slot_cap, raw_dim, desc, num_entries, use_dim_host, n_use_dim,
+                                  use_time_lag, sweep_remove_radius, out, cap, n_out_dev, status_dev, workspace,
+                                  workspace_bytes, stream, nullptr);
+}
+
+extern "C" int p3d_merge_sweeps_frustum(const float *raw, int num_slots, int64_t slot_cap, int raw_dim,
+                                        const p3d_sweep_desc *desc, int num_entries, const int32_t *use_dim_host,
+                                        int n_use_dim, int use_time_lag, float sweep_remove_radius, float *out,
+                                        int64_t cap, int32_t *n_out_dev, int32_t *status_dev, void *workspace,
+                                        size_t workspace_bytes, p3d_stream_t stream, const double *planes_dev) {
+  return merge_sweeps_impl<true>(raw, num_slots, slot_cap, raw_dim, desc, num_entries, use_dim_host, n_use_dim,
+                                 use_time_lag, sweep_remove_radius, out, cap, n_out_dev, status_dev, workspace,
+                                 workspace_bytes, stream, planes_dev);
 }

@@ -10,6 +10,7 @@ import torch
 
 from . import raw
 
+_IDENTITY = np.eye(4)
 
 def count_graph_nodes(graph):
     """Node counts by type of a torch.cuda.CUDAGraph captured with keep_graph=True, {"kernel": .., "memcpy": ..,
@@ -164,6 +165,18 @@ def infer_in_flight(lanes, frames_host):
     yield from run_in_flight(lanes, frames_host, lambda p, i, pts, k: p._submit(pts, k, i < 2 * len(lanes)))
 
 
+def kitti_frames(lanes, ring, items):
+    """One frame per (cloud [n, 4] fp32 raw scan, planes [6, 4] (kitti.frustum_planes)) over the captured lanes sharing
+    `ring` (in_flight), each culled to its camera frustum inside the graph; the H2D of scan j + 1 runs on the ring's copy
+    stream while frame j computes.  Yields (boxes, scores, labels) per scan, in order."""
+    for p in lanes:
+        if p.graph is None or p.ring is not ring or not p.sweep_input["frustum"]:
+            raise RuntimeError("infer_kitti_many needs captured lanes with KITTI_INPUT sharing one ring")
+        p.prepare_sweep()
+    ring.reset()
+    yield from run_in_flight(lanes, items, lambda p, i, item, k: p._submit_kitti(item, k))
+
+
 def stream_frames(lanes, ring, items):
     """One frame per pushed sweep (cloud, global_from_lidar, timestamp) over the captured lanes sharing `ring` (in_flight);
     the H2D of sweep j + 1 runs on the ring's copy stream while frame j computes.  Yields (boxes, scores, labels) per
@@ -206,7 +219,14 @@ class GraphFrame:
 # sweep_input of the LiDAR frames: ten nuScenes sweeps of 5 values per point, of which x, y, z, intensity are kept and the
 # time lag appended (the 5 columns deploy.preprocess gives the model), close points of earlier sweeps removed within 1 m;
 # slot_cap None = 2 x the mean rows per sweep of num_points
-SWEEP_INPUT = dict(max_sweeps=10, raw_dim=5, use_dim=4, use_time_lag=True, remove_radius=1.0, slot_cap=None)
+SWEEP_INPUT = dict(max_sweeps=10, raw_dim=5, use_dim=4, use_time_lag=True, remove_radius=1.0, slot_cap=None,
+                   frustum=False)
+# sweep_input of the KITTI PointPillars frames on raw `velodyne/*.bin` scans (infer_kitti / infer_kitti_many): one sweep of
+# x, y, z, reflectance, culled on the device to the left colour camera's view frustum (kitti.frustum_planes; Paddle3D's
+# RemoveCameraInvisiblePointsKITTI) into the frame's points.  A raw HDL-64E scan holds ~120k points; slot_cap is the
+# largest raw scan a frame takes.
+KITTI_INPUT = dict(max_sweeps=1, raw_dim=4, use_dim=4, use_time_lag=False, remove_radius=1.0, slot_cap=196608,
+                   frustum=True)
 
 
 class CapturedFrame(ResultSlotOwner, GraphFrame):
@@ -323,6 +343,8 @@ class CapturedFrame(ResultSlotOwner, GraphFrame):
             raise ValueError("sweep_input gives %d columns per point, the model reads %d"
                              % (len(si["use_dim"]) + bool(si["use_time_lag"]), self.F))
         K = int(si["max_sweeps"])
+        if si["frustum"] and (K != 1 or si["use_time_lag"]):
+            raise ValueError("the camera frustum cull takes one sweep without a time lag")
         if si["slot_cap"] is None:
             si["slot_cap"] = -(-2 * self.n // K // 4) * 4
         if ring is None:
@@ -335,6 +357,9 @@ class CapturedFrame(ResultSlotOwner, GraphFrame):
         self._desc_host = [torch.zeros((nb,), dtype=torch.uint8).pin_memory() for _ in range(3)]
         self._n_merged = torch.zeros((1,), dtype=torch.int32, device=self.device)
         self._merge_status = torch.zeros((1,), dtype=torch.int32, device=self.device)
+        if si["frustum"]:  # the six frustum planes the captured cull reads, staged like the descriptor
+            self._planes = torch.zeros((6, 4), dtype=torch.float64, device=self.device)
+            self._planes_host = [torch.zeros((6, 4), dtype=torch.float64).pin_memory() for _ in range(3)]
 
     def _desc_view(self, k):
         from .ops import sweep_merge as sm
@@ -386,6 +411,64 @@ class CapturedFrame(ResultSlotOwner, GraphFrame):
             self._done[k].record(st)
         self.ring.mark_read(read, self._done[k])
 
+    def _kitti_input(self, cloud, planes):
+        """Checked (cloud, planes) of a KITTI frame: nothing is enqueued for a refused one."""
+        from . import kitti
+        if self.sweep_input is None or not self.sweep_input["frustum"]:
+            raise RuntimeError("KITTI frames need a pipeline built with sweep_input=frame.KITTI_INPUT")
+        cloud = np.ascontiguousarray(cloud, np.float32)
+        if cloud.ndim != 2 or cloud.shape[1] != self.ring.raw_dim or len(cloud) > self.ring.slot_cap:
+            raise ValueError("a raw scan must be [n <= %d, %d], got %s" % (self.ring.slot_cap, self.ring.raw_dim,
+                                                                           cloud.shape))
+        return cloud, kitti.check_planes(planes)
+
+    def infer_kitti(self, cloud, planes):
+        """One frame from a raw KITTI scan, latency mode: cloud [n, 4] fp32 (a `velodyne/*.bin`), planes [6, 4] float64
+        (kitti.frustum_planes of its calib and image shape).  The rows outside the camera frustum are dropped on the
+        device; returns what infer() returns for the culled cloud (LiDAR-frame boxes; kitti.to_kitti makes labels)."""
+        cloud, planes = self._kitti_input(cloud, planes)
+        from .ops import sweep_merge as sm
+        desc = self._desc_view(2)
+        self.stream.synchronize()  # the previous frame no longer reads the staging
+        desc[:] = np.zeros(1, sm.DESC_DTYPE)
+        self._planes_host[2].numpy()[:] = planes
+        self.ring.reset()
+        self.ring.load(0, cloud, self.stream)
+        sm.set_entry(desc[0], 0, len(cloud))
+
+        def upload():
+            self._sweep_desc.copy_(self._desc_host[2], non_blocking=True)
+            self._planes.copy_(self._planes_host[2], non_blocking=True)
+        out = self._infer(upload)
+        ev = torch.cuda.Event()
+        ev.record(self.stream)
+        self.ring.mark_read([0], ev)
+        return out
+
+    def infer_kitti_many(self, items):
+        """items: iterable of (cloud, planes) as infer_kitti takes them.  Yields (boxes, scores, labels) per scan, in
+        order; the H2D of the next scan overlaps the current frame (as infer_many)."""
+        if self.graph is None:
+            raise RuntimeError("infer_kitti_many needs a captured pipeline: call capture() first")
+        return kitti_frames([self], self.ring, items)
+
+    def _submit_kitti(self, item, k):
+        """Enqueue the frame of one raw scan into result slot k: scan H2D into the ring, descriptor and plane H2D, graph
+        replay, D2H of the results."""
+        cloud, planes = self._kitti_input(*item)
+        j = self.ring.push(cloud, _IDENTITY, 0.0)
+        self._planes_host[k].numpy()[:] = planes  # slot k's previous frame was read back: its H2D is done
+        read, pushed = self.ring.describe(j, self._desc_view(k))
+        st = self.stream
+        with torch.cuda.stream(st):
+            st.wait_event(pushed)
+            self._sweep_desc.copy_(self._desc_host[k], non_blocking=True)
+            self._planes.copy_(self._planes_host[k], non_blocking=True)
+            self.graph.replay()
+            self._slots[k].copy_from(self.out)
+            self._done[k].record(st)
+        self.ring.mark_read(read, self._done[k])
+
     def merged_rows(self):
         """Rows of the last merged cloud (device scalar read back; sweep input only)."""
         self.stream.synchronize()
@@ -395,6 +478,10 @@ class CapturedFrame(ResultSlotOwner, GraphFrame):
         """Enqueue the device merge (ops.sweep_merge) of the frame's sweeps in the ring into self.points."""
         from .ops import sweep_merge as sm
         si = self.sweep_input
+        if si["frustum"]:
+            sm.merge_frustum_into(self.ring.buf, self._sweep_desc, self._planes, si["use_dim"], self.points,
+                                  self._n_merged, self._merge_status)
+            return
         sm.merge_into(self.ring.buf, self._sweep_desc, si["max_sweeps"], si["use_dim"], si["use_time_lag"],
                       si["remove_radius"], self.points, self._n_merged, self._merge_status)
 

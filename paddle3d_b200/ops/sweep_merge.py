@@ -1,6 +1,7 @@
 """Multi-sweep merge on the device (csrc/sweep_merge.cu): LoadPointCloud.__call__ (paddle3d/transforms/reader.py:116-167)
 as one kernel pass over raw sweep rows already on the GPU.  The reference has no op for it (it is a data transform);
-`io.merge_sweeps` is the host restatement every result here is compared against."""
+`io.merge_sweeps` is the host restatement every result here is compared against.  The same pass with the KITTI camera
+frustum cull (merge_frustum_into / frustum_cull_device) has `kitti.remove_camera_invisible` as its host restatement."""
 import numpy as np
 import torch
 
@@ -54,6 +55,48 @@ def merge_into(raw, desc_dev, num_entries, cols, use_time_lag, sweep_remove_radi
     check(L.p3d_merge_sweeps(ptr(raw), slots, slot_cap, raw_dim, ptr(desc_dev), num_entries, host_ints(cols), len(cols),
                              int(bool(use_time_lag)), float(np.float32(sweep_remove_radius)), ptr(out), cap, ptr(n_out),
                              ptr(status), ptr(ws), ws.numel(), stream(raw.device)), "merge_sweeps")
+
+
+def merge_frustum_into(raw, desc_dev, planes_dev, cols, out, n_out, status, num_entries=1):
+    """merge_into of the one entry of desc_dev with the camera frustum cull (p3d_merge_sweeps_frustum): rows outside the
+    six planes of planes_dev [6, 4] fp64 (device; kitti.frustum_planes) are dropped, order kept.  No time lag, no
+    removal square.  num_entries != 1 is refused by the library (P3DError)."""
+    slots, slot_cap, raw_dim = raw.shape
+    cap, F = out.shape
+    if F != len(cols) or desc_dev.numel() < num_entries * DESC_DTYPE.itemsize:
+        raise ValueError("merge_sweeps_frustum: output has %d columns, descriptor %d bytes" % (F, desc_dev.numel()))
+    if planes_dev.dtype != torch.float64 or planes_dev.numel() != 24 or not planes_dev.is_contiguous():
+        raise ValueError("merge_sweeps_frustum: planes must be a contiguous [6, 4] float64 device tensor")
+    L = lib()
+    ws = workspace(L.p3d_merge_sweeps_workspace_bytes(num_entries, slot_cap), raw.device, "sweep_merge")
+    check(L.p3d_merge_sweeps_frustum(ptr(raw), slots, slot_cap, raw_dim, ptr(desc_dev), num_entries, host_ints(cols),
+                                     len(cols), 0, 0.0, ptr(out), cap, ptr(n_out), ptr(status), ptr(ws), ws.numel(),
+                                     stream(raw.device), ptr(planes_dev)), "merge_sweeps_frustum")
+
+
+def frustum_cull_device(cloud, planes, cap=None, use_dim=None, device="cuda"):
+    """kitti.remove_camera_invisible on the GPU: cloud [n, raw_dim] fp32, planes [6, 4] (kitti.frustum_planes).  Returns
+    (points [cap, F] fp32 on the device, NaN rows from n_out on, n_out [1] int32, status [1] int32: OVERFLOW when more than
+    cap rows were kept).  cap defaults to n."""
+    cloud = np.ascontiguousarray(cloud, np.float32)
+    if cloud.ndim != 2:
+        raise ValueError("cloud must be [n, raw_dim]")
+    raw_dim = cloud.shape[1]
+    cols = columns(use_dim, raw_dim)
+    slot_cap = max(4, -(-len(cloud) // 4) * 4)
+    host = np.zeros((1, slot_cap, raw_dim), np.float32)
+    host[0, :len(cloud)] = cloud
+    desc = np.zeros(1, DESC_DTYPE)
+    set_entry(desc[0], 0, len(cloud))
+    dev = torch.device(device)
+    cap = len(cloud) if cap is None else int(cap)
+    out = torch.empty((cap, len(cols)), dtype=torch.float32, device=dev)
+    n_out = torch.empty((1,), dtype=torch.int32, device=dev)
+    status = torch.empty((1,), dtype=torch.int32, device=dev)
+    raw = torch.from_numpy(host).to(dev)
+    planes_dev = torch.from_numpy(np.ascontiguousarray(planes, np.float64).reshape(6, 4)).to(dev)
+    merge_frustum_into(raw, torch.from_numpy(desc.view(np.uint8)).to(dev), planes_dev, cols, out, n_out, status)
+    return out, n_out, status
 
 
 def merge_sweeps_device(key, sweeps=(), use_dim=None, use_time_lag=False, sweep_remove_radius=1.0, order=None, cap=None,

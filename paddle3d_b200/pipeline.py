@@ -13,7 +13,8 @@ CenterHead.predict_by_custom_op (center_head.py:294-339).
 import torch
 
 from . import synth
-from .frame import SWEEP_INPUT, CapturedFrame, ResultSlot, infer_in_flight, in_flight, stream_frames  # noqa: F401
+from .frame import (SWEEP_INPUT, CapturedFrame, ResultSlot, infer_in_flight, in_flight, kitti_frames,  # noqa: F401
+                    stream_frames)
 from .layers import SparseResNet3D
 from .ops import centerpoint_postprocess as cpp
 from .ops import sparse_nn as sp
@@ -254,6 +255,12 @@ class CenterPointSweep:
         """As CenterPointHotPath.infer_stream (one result per pushed sweep, in order), with the lanes sharing one sweep
         ring and len(self) frames computing concurrently."""
         return stream_frames(self.lanes, self.lanes[0].ring, items)
+
+    def infer_kitti_many(self, items):
+        """As PointPillarsHotPath.infer_kitti_many ((raw scan, frustum planes) items in, host results out, in order), with
+        the lanes (built with sweep_input=frame.KITTI_INPUT) sharing one ring and len(self) frames computing
+        concurrently."""
+        return kitti_frames(self.lanes, self.lanes[0].ring, items)
 
     def infer_many(self, frames_host):
         """As CenterPointHotPath.infer_many (pinned host frames in, host results out, in order), with len(self) frames

@@ -9,7 +9,8 @@ repository's kernels:
     (cls | box | dir as ONE 1x1 conv, fp32 planes) -> anchor_head_postprocess (csrc/anchor_postprocess.cu) -> boxes
 
 PointPillarsHotPath captures everything between the H2D copy of the points and the D2H copy of the boxes as one CUDA graph
-(frame.CapturedFrame).  Anchors are constant per model and built once on the host (create_anchors_3d_stride, SECOND's
+(frame.CapturedFrame).  With sweep_input=frame.KITTI_INPUT the graph starts with the camera frustum cull of a raw KITTI
+scan (infer_kitti / infer_kitti_many; kitti.py builds the planes and writes the label files).  Anchors are constant per model and built once on the host (create_anchors_3d_stride, SECOND's
 box_np_ops), as are the voxel-index corners of each anchor's near box (anchor_voxel_corners) the anchor mask reads."""
 import numpy as np
 import torch
@@ -256,16 +257,19 @@ class PointPillars:
 
 
 class PointPillarsHotPath(CapturedFrame):
-    """One PointPillars frame on one GPU: H2D -> [captured: hard_voxelize -> PFN -> pixel image -> trunk -> head conv ->
-    anchor postprocess] -> D2H of boxes [300, 7], scores, labels, counts (candidates, rows) and the status word."""
+    """One PointPillars frame on one GPU: H2D -> [captured: (camera frustum cull) -> hard_voxelize -> PFN -> pixel image ->
+    trunk -> head conv -> anchor postprocess] -> D2H of boxes [300, 7], scores, labels, counts (candidates, rows) and the
+    status word (fp16-range overflow of the pair path, with sweep input the cull's status bits)."""
 
     def __init__(self, cfg=None, device="cuda:0", seed=0, num_points=None, bn_gain=1.0, model_cfg=None, weights=None,
-                 share=None):
+                 share=None, sweep_input=None, sweep_ring=None):
         """cfg: the point-cloud config (synth.C2 by default); model_cfg: the model config (CONFIG by default; synth.C2 with
         CONFIG is the car model, synth.C2_PED_CYCLIST with CONFIG_PED_CYCLIST the cyclist / pedestrian one).  weights: a
         Paddle3D PointPillars checkpoint of that model (a `.pdparams` path or a state dict, see checkpoint.py) instead of
-        the seeded weights.  share: another frame whose model this one uses (pipeline.CenterPointSweep's lanes)."""
-        super().__init__(cfg or synth.C2, device, num_points)
+        the seeded weights.  share: another frame whose model this one uses (pipeline.CenterPointSweep's lanes).
+        sweep_input / sweep_ring: frame.KITTI_INPUT to run on raw KITTI scans (infer_kitti, infer_kitti_many), culled
+        to the camera frustum on the device into the num_points rows the model reads."""
+        super().__init__(cfg or synth.C2, device, num_points, sweep_input, sweep_ring)
         if share is not None:
             self.share_model(share)
         elif weights is None:
@@ -273,14 +277,19 @@ class PointPillarsHotPath(CapturedFrame):
         else:
             from .checkpoint import as_state_dict
             self.model = PointPillars(self.cfg, model_cfg).load_state_dict(as_state_dict(weights), self.device)
-        self.slot = ResultSlot(self.model.mc["test"]["nms_post_max_size"], 7, 2, 1)
+        self.slot = ResultSlot(self.model.mc["test"]["nms_post_max_size"], 7, 2, 1 if self.sweep_input is None else 2)
 
     def forward_device(self):
         m = self.model
+        if self.sweep_input is not None:
+            self._merge_sweeps()
         image, shape, coors, nv = m.encode(self.points)
         planes = m.dense(image, shape)
         boxes, scores, labels, counts = m.postprocess(planes, coors, nv)
-        status = sp.status_tensor(self.device).clone()
+        if self.sweep_input is None:
+            status = sp.status_tensor(self.device).clone()
+        else:
+            status = torch.stack([sp.status_tensor(self.device)[0], self._merge_status[0]])
         return dict(boxes=boxes, scores=scores, labels=labels, counts=counts, num_voxels=nv, coors=coors, planes=planes,
                     status=status)
 
@@ -298,8 +307,10 @@ class PointPillarsHotPath(CapturedFrame):
         self.model.load_state_dict(sd, self.device)
         return self
 
-    @staticmethod
-    def check_status(status_host):
-        """Raise when the frame's status word reports that an activation left fp16's range (never a silent wrong result)."""
+    def check_status(self, status_host):
+        """Raise when the frame's status word reports that an activation left fp16's range, or with sweep input that the
+        cull kept more rows than num_points (never a silent wrong result)."""
+        if len(status_host) > 1:
+            self._check_merge_status(int(status_host[1]))
         if int(status_host[0]):
             raise RuntimeError("PointPillars: an activation left fp16's range (|x| >= 65504) on the fp16-pair path")

@@ -127,6 +127,51 @@ def sweep_sequence(n_sweeps, seed, points_per_sweep=29500, speed=10.0, yaw_rate=
     return out
 
 
+# A KITTI object-split calib file (the 2011_09_26 drive's camera and LiDAR calibration, as in training/calib/000000.txt)
+KITTI_CALIB = """P0: 7.215377e+02 0.000000e+00 6.095593e+02 0.000000e+00 0.000000e+00 7.215377e+02 1.728540e+02 0.000000e+00 0.000000e+00 0.000000e+00 1.000000e+00 0.000000e+00
+P1: 7.215377e+02 0.000000e+00 6.095593e+02 -3.875744e+02 0.000000e+00 7.215377e+02 1.728540e+02 0.000000e+00 0.000000e+00 0.000000e+00 1.000000e+00 0.000000e+00
+P2: 7.215377e+02 0.000000e+00 6.095593e+02 4.485728e+01 0.000000e+00 7.215377e+02 1.728540e+02 2.163791e-01 0.000000e+00 0.000000e+00 1.000000e+00 2.745884e-03
+P3: 7.215377e+02 0.000000e+00 6.095593e+02 -3.395242e+02 0.000000e+00 7.215377e+02 1.728540e+02 2.199936e+00 0.000000e+00 0.000000e+00 1.000000e+00 2.729905e-03
+R0_rect: 9.999239e-01 9.837760e-03 -7.445048e-03 -9.869795e-03 9.999421e-01 -4.278459e-03 7.402527e-03 4.351614e-03 9.999631e-01
+Tr_velo_to_cam: 7.533745e-03 -9.999714e-01 -6.166020e-04 -4.069766e-03 1.480249e-02 7.280733e-04 -9.998902e-01 -7.631618e-02 9.998621e-01 7.523790e-03 1.480755e-02 -2.717806e-01
+Tr_imu_to_velo: 9.999976e-01 7.553071e-04 -2.035826e-03 -8.086759e-01 -7.854027e-04 9.998898e-01 -1.482298e-02 3.195559e-01 2.024406e-03 1.482454e-02 9.998881e-01 -7.997231e-01
+"""
+
+
+def kitti_raw_cloud(seed, beams=64, max_range=80.0, height=1.73):
+    """A raw KITTI `velodyne/*.bin`-like scan: (cloud [n, 4] fp32 (x, y, z, reflectance), ~120k points over 360 degrees
+    from an HDL-64E-like sensor (64 beams from +2 to -24.8 degrees, ~1900 azimuth steps, ~3 % dropped returns) over a
+    ground plane `height` m below it and 96 seeded boxes, in azimuth order; the calib dict of KITTI_CALIB
+    (kitti.parse_calib); the image shape (H, W) of the reference's default).  About a quarter of the points lie in the
+    camera's view."""
+    from . import kitti
+    rng = np.random.default_rng(seed)
+    az_steps = 1850 + int(rng.integers(0, 100))
+    az = rng.uniform(0, 2 * np.pi) + np.linspace(0, 2 * np.pi, az_steps, endpoint=False)
+    elev = np.deg2rad(np.linspace(2.0, -24.8, beams))
+    a, e = np.meshgrid(az, elev, indexing="ij")  # azimuth-major: one column of 64 beams after another
+    dx, dy, dz = np.cos(e) * np.cos(a), np.cos(e) * np.sin(a), np.sin(e)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        t = np.where(dz < -1e-3, -height / dz, np.inf)
+    nb = 96
+    bc = rng.uniform(-60.0, 60.0, size=(nb, 2))
+    bs = rng.uniform(0.5, 3.0, size=(nb, 2))
+    bh = rng.uniform(1.0, 3.5, size=(nb,))
+    for k in range(nb):
+        with np.errstate(divide="ignore", invalid="ignore"):
+            tx1, tx2 = (bc[k, 0] - bs[k, 0]) / dx, (bc[k, 0] + bs[k, 0]) / dx
+            ty1, ty2 = (bc[k, 1] - bs[k, 1]) / dy, (bc[k, 1] + bs[k, 1]) / dy
+        tn = np.maximum(np.minimum(tx1, tx2), np.minimum(ty1, ty2))
+        tf = np.minimum(np.maximum(tx1, tx2), np.maximum(ty1, ty2))
+        zz = tn * dz
+        hit = (tn > 1.0) & (tn < tf) & (zz > -height) & (zz < bh[k] - height)
+        t = np.where(hit & (tn < t), tn, t)
+    ok = (t < max_range) & (rng.uniform(size=t.shape) > 0.03)
+    p = np.stack([(t * dx)[ok], (t * dy)[ok], (t * dz)[ok]], 1) + rng.normal(0, 0.02, size=(int(ok.sum()), 3))
+    cloud = np.concatenate([p, rng.uniform(0, 1, size=(len(p), 1))], 1).astype(np.float32)
+    return cloud, kitti.parse_calib(KITTI_CALIB, "synth.KITTI_CALIB"), kitti.DEFAULT_IMAGE_SHAPE
+
+
 def random_boxes(n, seed, extent=40.0, clustered=True):
     """[x,y,z,dx,dy,dz,heading] boxes; clustered centres so that rotated overlaps are common."""
     rng = np.random.default_rng(seed)

@@ -2,13 +2,13 @@
 """tools/pointpillars_bench.py — PointPillars KITTI frames/s on an H100 (BASELINE config 2).
 
   python tools/pointpillars_bench.py [--config car|ped_cyclist] [--steps K] [--warmup W] [--in-flight L]
-                                     [--no-cpu-baseline] [--dump-outputs DIR]
+                                     [--no-cpu-baseline] [--dump-outputs DIR] [--kitti-raw]
 
 A step = one 20k x 4-point synth.lidar_cloud frame through pointpillars.PointPillarsHotPath: hard_voxelize ->
 PillarFeatureNet -> pixel fp16-pair image -> SecondBackbone + SecondFPN + SSD head conv -> anchor_head_postprocess ->
 boxes.  --config car (default): synth.C2 with pointpillars.CONFIG, a 496 x 432 image, 66.2 GFLOP dense; ped_cyclist:
 synth.C2_PED_CYCLIST with pointpillars.CONFIG_PED_CYCLIST (two classes), a 248 x 296 image with a stride-1 first block.
-Prints one JSON line.  The timing harness (CenterPointSweep lanes, e2e through
+--kitti-raw times raw KITTI scans instead (run_kitti_raw).  Prints one JSON line.  The timing harness (CenterPointSweep lanes, e2e through
 infer_many / infer, graph-timed stages) is bench.py's, imported from it, so both models are measured the same way.
 """
 import argparse
@@ -188,6 +188,98 @@ def run(args):
     print(json.dumps(line))
 
 
+KITTI_RAW_POINTS = 40000  # rows a frame takes after the camera cull (tools/infer_kitti.py's default)
+
+
+def run_kitti_raw(args):
+    """Raw KITTI scans (synth.kitti_raw_cloud: ~115k points over 360 degrees, ~14.5k in the camera's view) end to end,
+    host arrays in, host boxes out, at 1 and --in-flight frames in flight:
+      device  the raw scan uploaded, culled to the camera frustum inside the captured frame (frame.KITTI_INPUT,
+              infer_kitti_many);
+      host    the same scan culled on the host by kitti.remove_camera_invisible, padded to the frame's rows and uploaded
+              reduced (infer_many), the cull inside the timed loop.
+    Also: the cull kernel alone (CUDA events over 200 launches on a full-size scan), the H2D bytes per frame of each
+    path, and that frame 0's boxes, scores and labels are bit-equal between the two."""
+    import torch
+    from paddle3d_b200 import frame, kitti, synth
+    from paddle3d_b200.ops import sweep_merge as sm
+    from paddle3d_b200.pipeline import CenterPointSweep
+    from paddle3d_b200.pointpillars import CONFIG, CONFIG_PED_CYCLIST, PointPillarsHotPath
+    if not torch.cuda.is_available():
+        raise SystemExit("pointpillars_bench.py needs a CUDA device (no CPU fallback exists)")
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    car = args.config == "car"
+    cfg, model_cfg = (synth.C2, CONFIG) if car else (synth.C2_PED_CYCLIST, CONFIG_PED_CYCLIST)
+    n = KITTI_RAW_POINTS
+    scans = [synth.kitti_raw_cloud(s) for s in range(POOL)]
+    items = [(c, kitti.frustum_planes(cal, shape)) for c, cal, shape in scans]
+
+    def reduced(item):
+        kept = kitti.remove_camera_invisible(*item)
+        full = np.full((n, 4), np.nan, np.float32)
+        full[:len(kept)] = kept
+        return torch.from_numpy(full)
+
+    ident = gpu_identity(0)
+    kw = dict(cfg=cfg, model_cfg=model_cfg, device=dev, seed=0, bn_gain=BN_GAIN, num_points=n)
+    calib_pts = reduced(items[0]).to(dev)
+    out = {}
+    for lanes in sorted({1, max(1, args.in_flight)}):
+        raw = CenterPointSweep(lanes, frame_cls=PointPillarsHotPath, sweep_input=frame.KITTI_INPUT, **kw)
+        host = CenterPointSweep(lanes, frame_cls=PointPillarsHotPath, **kw)
+        raw.calibrate_head(calib_pts)
+        host.calibrate_head(calib_pts)
+        for p in raw.lanes:
+            p.infer_kitti(*items[0])
+            p.capture()
+        host.capture(calib_pts)
+        if lanes == 1:
+            got_raw = [t.clone() for t in raw.lanes[0].infer_kitti(*items[0])]
+            got_host = host.lanes[0].infer(reduced(items[0]).pin_memory())
+            out["frame0_bit_equal"] = all(torch.equal(a, b) for a, b in zip(got_raw, got_host))
+            out["frame0_boxes"] = int(len(got_raw[0]))
+        seq = [items[i % len(items)] for i in range(args.steps)]
+        warm = [items[i % len(items)] for i in range(args.warmup)]
+        row = {}
+        for name, run_items in (("device_cull", lambda it: raw.infer_kitti_many(iter(it))),
+                                ("host_cull", lambda it: host.infer_many(reduced(x) for x in it))):
+            list(run_items(warm))
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            k = sum(1 for _ in run_items(seq))
+            row[name] = k / (time.perf_counter() - t0)
+        out["frames_per_s_%d_in_flight" % lanes] = row
+        if lanes == 1:
+            p = raw.lanes[0]
+            st = p.stream
+            big = max(range(len(items)), key=lambda i: len(items[i][0]))
+            p.infer_kitti(*items[big])
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+            with torch.cuda.stream(st):
+                for _ in range(20):
+                    p._merge_sweeps()
+                ev[0].record(st)
+                for _ in range(200):
+                    p._merge_sweeps()
+                ev[1].record(st)
+            ev[1].synchronize()
+            out["cull_kernel_us"] = {"mean": 1e3 * ev[0].elapsed_time(ev[1]) / 200, "raw_points": int(len(items[big][0])),
+                                     "what": "p3d_merge_sweeps_frustum: workspace memset + merge_sweeps_kernel<true> + "
+                                             "merge_tail_kernel, eager launches"}
+        del raw, host
+        torch.cuda.empty_cache()
+    mean_raw = float(np.mean([len(c) for c, _ in items]))
+    mean_kept = float(np.mean([len(kitti.remove_camera_invisible(*it)) for it in items]))
+    out["h2d_bytes_per_frame"] = {"device_cull": mean_raw * 16 + sm.DESC_DTYPE.itemsize + 6 * 4 * 8,
+                                  "host_cull": n * 4 * 4, "mean_raw_points": mean_raw, "mean_kept_points": mean_kept}
+    line = {"metric": "PointPillars KITTI frames/sec on raw scans, camera cull on the device vs on the host",
+            "model": "pointpillars_%s" % args.config, "unit": UNIT, "steps": args.steps, "warmup": args.warmup,
+            "data": "synthetic raw scans (synth.kitti_raw_cloud, %d seeds), num_points %d" % (len(items), n),
+            "gpu": ident, **out}
+    print(json.dumps(line))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--config", choices=sorted(CLASS_NAMES), default="car",
@@ -198,9 +290,11 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--dump-outputs", metavar="DIR", default=None,
                     help="after the timed steps, write the boxes / scores / labels of the last timed frame to DIR/*.npy")
+    ap.add_argument("--kitti-raw", action="store_true",
+                    help="raw KITTI scans: camera frustum cull inside the frame vs on the host (run_kitti_raw)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
-    run(args)
+    (run_kitti_raw if args.kitti_raw else run)(args)
 
 
 if __name__ == "__main__":
