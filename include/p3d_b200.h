@@ -564,6 +564,15 @@ int p3d_pillar_feature_net2(const float *voxels, const int32_t *num_points_per_v
                             int out_channels, const float *weight2, const float *bn_scale2, const float *bn_shift2,
                             const float *voxel_size_host, const float *point_cloud_range_host, float *out,
                             p3d_stream_t stream);
+/* p3d_pillar_feature_net2 for up to 128 points per pillar (CenterPoint-pillars KITTI reads 100): the same kernel with
+ * twice the shared-memory staging, so on every input both accept the two give the same bits.  M <= 128, mid <= 64,
+ * F <= 8 (P3D_ERR_UNSUPPORTED above). */
+int p3d_pillar_feature_net2_wide(const float *voxels, const int32_t *num_points_per_voxel, const int32_t *coors,
+                                 const int32_t *num_voxels_dev, int64_t n_cap, int max_points, int num_point_dim,
+                                 int mid_channels, const float *weight1, const float *bn_scale1, const float *bn_shift1,
+                                 int out_channels, const float *weight2, const float *bn_scale2,
+                                 const float *bn_shift2, const float *voxel_size_host,
+                                 const float *point_cloud_range_host, float *out, p3d_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
  * anchor_head_postprocess      SECOND v1.5 VoxelNet.predict (the path SSDHead.post_process -> rotate_nms_pcdet ports)

@@ -77,6 +77,8 @@ SIGNATURES = {
     "p3d_pillar_feature_net": (_int, [_vp, _vp, _vp, _vp, _i64, _int, _int, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "p3d_pillar_feature_net2": (_int, [_vp, _vp, _vp, _vp, _i64, _int, _int, _int, _vp, _vp, _vp, _int, _vp, _vp, _vp, _vp,
                                        _vp, _vp, _vp]),
+    "p3d_pillar_feature_net2_wide": (_int, [_vp, _vp, _vp, _vp, _i64, _int, _int, _int, _vp, _vp, _vp, _int, _vp, _vp, _vp,
+                                            _vp, _vp, _vp, _vp]),
     "p3d_head_final_conv": (_int, [_vp, _int, _int, _int, _int, _int, _int, _vp, _vp, _vp, _vp, _int, _vp, _vp]),
     "p3d_nchw_to_pixel_h16": (_int, [_vp, _int, _int, _int, _int, _vp, _vp, _vp]),
     "p3d_pixel_h16_to_nchw": (_int, [_vp, _int, _int, _int, _int, _vp, _vp]),

@@ -1,5 +1,6 @@
-"""CenterPoint-pillars nuScenes inference on one GPU (configs/centerpoint/centerpoint_pillars_02voxel_nuscenes_10sweep.yml,
-synth.CP_PILLARS with CONFIG), composed from this repository's kernels:
+"""CenterPoint-pillars inference on one GPU, nuScenes (configs/centerpoint/centerpoint_pillars_02voxel_nuscenes_10sweep.yml,
+synth.CP_PILLARS with CONFIG) and KITTI (configs/centerpoint/centerpoint_pillars_016voxel_kitti.yml, synth.CP_PILLARS_KITTI
+with CONFIG_KITTI), composed from this repository's kernels (the nuScenes sizes shown):
 
     hard_voxelize (0.2 m pillars, 20 points) -> PillarFeatureNet with two PFNLayers (one fused launch) -> pillar rows as
     fp16 pairs -> pixel fp16-pair image [512 x 512 x 64] -> SecondBackbone + SecondFPN (a 2x2 stride-2 conv, a 1x1 conv
@@ -7,16 +8,22 @@ synth.CP_PILLARS with CONFIG), composed from this repository's kernels:
     -> centerpoint_postprocess_device -> boxes
 
 CenterPointPillarsHotPath captures everything between the H2D copy of the points and the D2H copy of the boxes as one
-CUDA graph (frame.CapturedFrame), optionally starting with the device merge of raw sweeps (sweep_input).
+CUDA graph (frame.CapturedFrame), optionally starting with the device merge of raw sweeps (sweep_input), or for the KITTI
+model with the camera frustum cull of a raw scan (sweep_input=frame.KITTI_INPUT: infer_kitti, infer_kitti_many; the
+boxes become KITTI labels through kitti.centerpoint_to_lidar_boxes and kitti.to_kitti).
+
+The KITTI model reads 100 points per pillar (pillar_feature_net2 then launches p3d_pillar_feature_net2_wide), has no
+velocity head (7-column boxes) and two tasks, [Car] and [Pedestrian, Cyclist]; its head runs at half the 432 x 496 grid.
 
 PARITY UNPINNED: the model values (CONFIG, synth.CP_PILLARS, synth.CENTERPOINT_PILLARS_TEST_CFG) are recalled from
 Paddle3D's yml and det3d's nusc_centerpoint_pp_02voxel_two_pfn_10sweep, which it descends from; they were not checked
-against either file."""
+against either file.  CONFIG_KITTI, synth.CP_PILLARS_KITTI and synth.CP_PILLARS_KITTI_TEST_CFG are recalled from
+centerpoint_pillars_016voxel_kitti.yml in the same way."""
 import numpy as np
 import torch
 
 from . import synth
-from .dense_head import DenseRPNHead, SecondTrunk
+from .dense_head import COMMON_HEADS, DenseRPNHead, SecondTrunk
 from .frame import CapturedFrame, ResultSlot
 from .ops import centerpoint_postprocess as cpp
 from .ops import pillar_encoder as pe
@@ -32,13 +39,27 @@ CONFIG = dict(
     head=dict(tasks=tuple(synth.CENTERPOINT_TASKS), share_conv_channel=64),
     test=synth.CENTERPOINT_PILLARS_TEST_CFG,
 )
+# PARITY UNPINNED (centerpoint_pillars_016voxel_kitti.yml, recalled): PillarFeatureNet(in 4, feat_channels [64, 64],
+# with_distance False); SecondBackbone out [64, 128, 256], layer_nums [3, 5, 5], strides [2, 2, 2]; SecondFPN out
+# [128, 128, 128], upsample strides [1, 2, 4]; CenterHead share_conv 64, tasks [Car], [Pedestrian, Cyclist], common_heads
+# reg 2, height 1, dim 3, rot 2 (no vel)
+CONFIG_KITTI = dict(
+    pfn=dict(feat_channels=(64, 64), bn_eps=1e-3),
+    backbone=dict(out_channels=(64, 128, 256), layer_nums=(3, 5, 5), downsample_strides=(2, 2, 2)),
+    fpn=dict(out_channels=(128, 128, 128), upsample_strides=(1, 2, 4), use_conv_for_no_stride=True),
+    head=dict(tasks=tuple(synth.CP_PILLARS_KITTI_TASKS), share_conv_channel=64,
+              common_heads=(("reg", 2), ("height", 1), ("dim", 3), ("rot", 2))),
+    test=synth.CP_PILLARS_KITTI_TEST_CFG,
+)
 
 
 class CenterPointPillars:
     """Seeded CenterPoint-pillars model: PillarFeatureNet(in 5, feat_channels [64, 64]): PFNLayer Linear(F + 5 -> 32) +
     BN + ReLU, concat with the pillar max to 64, PFNLayer Linear(64 -> 64) + BN + ReLU, max (no bias, BatchNorm1D eps
     1e-3); PointPillarsScatter to ny x nx x 64; DenseRPNHead (SecondBackbone [3, 5, 5] / strides [2, 2, 2], SecondFPN
-    upsample strides [0.5, 1, 2], CenterHead with 6 tasks) at a quarter of the grid."""
+    upsample strides [0.5, 1, 2], CenterHead with 6 tasks) at a quarter of the grid.  model_cfg=CONFIG_KITTI (with
+    synth.CP_PILLARS_KITTI) is the KITTI model: PFN in 4, FPN upsample strides [1, 2, 4], two velocity-free tasks, the head
+    at half the grid."""
 
     def __init__(self, cfg=None, model_cfg=None):
         self.cfg = dict(cfg or synth.CP_PILLARS)
@@ -53,7 +74,8 @@ class CenterPointPillars:
         self.head = DenseRPNHead(in_channels=self.C, out_channels=b["out_channels"], layer_nums=b["layer_nums"],
                                  downsample_strides=b["downsample_strides"], fpn_out_channels=f["out_channels"],
                                  upsample_strides=f["upsample_strides"], tasks=h["tasks"],
-                                 share_conv_channel=h["share_conv_channel"], bev_depth=1)
+                                 share_conv_channel=h["share_conv_channel"], bev_depth=1,
+                                 common_heads=h.get("common_heads", COMMON_HEADS))
         self.test_cfg = dict(mc["test"])
         self.label_off = synth.label_offsets(list(h["tasks"]))
         self.feat_hw, self.cat_hw = self._feature_sizes()
@@ -154,8 +176,8 @@ class CenterPointPillars:
         return self.head.head_planes()
 
     def flops(self):
-        """Algorithmic flops (2 x MACs) of the dense part at the model's grid: backbone, FPN and head (shared conv, the 36
-        ConvModules, the output convs)."""
+        """Algorithmic flops (2 x MACs) of the dense part at the model's grid: backbone, FPN and head (shared conv, the
+        ConvModules (36 nuScenes, 10 KITTI), the output convs)."""
         out = dict(backbone=0.0, fpn=0.0)
         h, w = self.grid[1], self.grid[0]
         for blk in self.head.blocks:
@@ -170,14 +192,17 @@ class CenterPointPillars:
 
 
 class CenterPointPillarsHotPath(CapturedFrame):
-    """One CenterPoint-pillars frame on one GPU: H2D -> [captured: (sweep merge) -> hard_voxelize -> PFN -> pixel image ->
-    trunk / head -> centerpoint postprocess] -> D2H of boxes [6 x 83, 9], scores, labels, counts and the status word
-    (fp16-range overflow of the pair path, with sweep input the merge's status bits)."""
+    """One CenterPoint-pillars frame on one GPU: H2D -> [captured: (sweep merge or camera frustum cull) -> hard_voxelize ->
+    PFN -> pixel image -> trunk / head -> centerpoint postprocess] -> D2H of boxes ([6 x 83, 9] nuScenes, [2 x 83, 7]
+    KITTI), scores, labels, counts and the status word (fp16-range overflow of the pair path, with sweep input the merge's
+    status bits)."""
 
     def __init__(self, cfg=None, device="cuda:0", seed=0, num_points=None, bn_gain=1.0, model_cfg=None,
                  sweep_input=None, sweep_ring=None, weights=None, share=None):
         """cfg: the point-cloud config (synth.CP_PILLARS by default); sweep_input / sweep_ring: as
-        pipeline.CenterPointHotPath (the merged columns are x, y, z, intensity and the time lag: F = 5).  weights: a
+        pipeline.CenterPointHotPath (the merged columns are x, y, z, intensity and the time lag: F = 5), or for the KITTI
+        model (cfg=synth.CP_PILLARS_KITTI, model_cfg=CONFIG_KITTI) frame.KITTI_INPUT: raw scans culled to the camera
+        frustum on the device (infer_kitti, infer_kitti_many).  weights: a
         Paddle3D CenterPoint-pillars checkpoint (a `.pdparams` path or a state dict, see checkpoint.py) instead of the
         seeded weights.  share: another frame whose model this one uses (CenterPointSweep's lanes)."""
         super().__init__(cfg or synth.CP_PILLARS, device, num_points, sweep_input, sweep_ring)
@@ -189,7 +214,8 @@ class CenterPointPillarsHotPath(CapturedFrame):
             from .checkpoint import as_state_dict
             self.model = CenterPointPillars(self.cfg, model_cfg).load_state_dict(as_state_dict(weights), self.device)
         m = self.model
-        self.slot = ResultSlot(len(m.label_off) * m.test_cfg["nms_post_max_size"], 9, len(m.label_off) + 1,
+        self.slot = ResultSlot(len(m.label_off) * m.test_cfg["nms_post_max_size"], 9 if m.head.with_velocity else 7,
+                               len(m.label_off) + 1,
                                1 if self.sweep_input is None else 2)
 
     def forward_device(self):

@@ -9,19 +9,22 @@
 // (one layer: F 3 .. 8, M 1 .. 64, C 1 .. 200, far pillars, padding rows deciding the max, rows beyond the count
 // untouched), tests/test_gpu_voxelize.py::test_pillar_feature_net and tests/test_gpu_centerpoint_pillars.py (two layers),
 // tests/test_gpu_bevfusion.py::test_hard_vfe_matches_fp64 (HardVFE),
-// 1e-4 vs the oracle restatements; the argument limits by tests/test_lidar_front_end_oracle.py.
+// 1e-4 vs the oracle restatements; the argument limits by tests/test_lidar_front_end_oracle.py.  The wide two-layer
+// instantiation (kMaxRows = 128, p3d_pillar_feature_net2_wide, CenterPoint-pillars KITTI's 100 points per pillar) by
+// tests/test_gpu_centerpoint_pillars_kitti.py, its limits by tests/test_centerpoint_pillars_kitti.py.
 #include "common.cuh"
 #include "p3d_b200.h"
 
 namespace p3d {
 namespace {
 
-constexpr int kMaxM = 64, kMaxF = 8, kMaxMid = 64;
+constexpr int kMaxM = 64, kMaxMWide = 128, kMaxF = 8, kMaxMid = 64;
 
 // kLayers = 1: C1 = C is the output width and (C2, w2, scale2, shift2) are unused.  kLayers = 2: C1 is the first
 // layer's width (<= kMaxMid), w2 is [2 C1, C2].  kVoxelZ (HardVFE, with kLayers = 2): the decoration also carries
-// z - (coors_z * vz + z_off), so a row has F + 6 features.
-template <int kLayers, bool kVoxelZ = false>
+// z - (coors_z * vz + z_off), so a row has F + 6 features.  kMaxRows: the most points per pillar the shared-memory
+// staging holds (M <= kMaxRows); it sizes the arrays only, the arithmetic and its order do not depend on it.
+template <int kLayers, bool kVoxelZ = false, int kMaxRows = kMaxM>
 __global__ void pfn_kernel(const float *__restrict__ voxels, const int32_t *__restrict__ npv,
                            const int32_t *__restrict__ coors, const int32_t *__restrict__ num_dev, int n_cap, int M, int F,
                            int C1, const float *__restrict__ weight, const float *__restrict__ scale,
@@ -29,7 +32,7 @@ __global__ void pfn_kernel(const float *__restrict__ voxels, const int32_t *__re
                            const float *__restrict__ scale2, const float *__restrict__ shift2, float vx, float vy,
                            float x_off, float y_off, float *__restrict__ out, float vz = 0.f, float z_off = 0.f) {
   constexpr int kExtra = kVoxelZ ? 6 : 5;
-  __shared__ float s_f[kMaxM][kMaxF + kExtra];
+  __shared__ float s_f[kMaxRows][kMaxF + kExtra];
   __shared__ float s_mean[3];
   const int n = num_dev ? min(num_dev[0], n_cap) : n_cap;
   const int i = blockIdx.x;
@@ -73,7 +76,7 @@ __global__ void pfn_kernel(const float *__restrict__ voxels, const int32_t *__re
       out[static_cast<size_t>(i) * C1 + c] = best;
     }
   } else {
-    __shared__ float s_x[kMaxM][kMaxMid];
+    __shared__ float s_x[kMaxRows][kMaxMid];
     __shared__ float s_xmax[kMaxMid];
     // Every padding row has the same (zero) decorated input, so the first padding row (row cnt, when cnt < M) stands
     // for all of them: in layer 1 its value ReLU(shift1) enters x_max, in layer 2 its output enters the final max.
@@ -137,28 +140,55 @@ extern "C" int p3d_pillar_feature_net(const float *voxels, const int32_t *num_po
   return P3D_OK;
 }
 
+namespace {
+
+template <int kMaxRows>
+int launch_pfn2(const float *voxels, const int32_t *num_points_per_voxel, const int32_t *coors,
+                const int32_t *num_voxels_dev, int64_t n_cap, int max_points, int num_point_dim, int mid_channels,
+                const float *weight1, const float *bn_scale1, const float *bn_shift1, int out_channels,
+                const float *weight2, const float *bn_scale2, const float *bn_shift2, const float *voxel_size_host,
+                const float *point_cloud_range_host, float *out, p3d_stream_t stream) {
+  if (!voxels || !num_points_per_voxel || !coors || !weight1 || !bn_scale1 || !bn_shift1 || !weight2 || !bn_scale2 ||
+      !bn_shift2 || !voxel_size_host || !point_cloud_range_host || !out || n_cap < 0 || mid_channels < 1 ||
+      out_channels < 1)
+    return P3D_ERR_INVALID_ARG;
+  if (max_points < 1 || max_points > kMaxRows || num_point_dim < 3 || num_point_dim > kMaxF || mid_channels > kMaxMid)
+    return P3D_ERR_UNSUPPORTED;
+  if (n_cap == 0) return P3D_OK;
+  const float vx = voxel_size_host[0], vy = voxel_size_host[1];
+  const float x_off = vx / 2 + point_cloud_range_host[0], y_off = vy / 2 + point_cloud_range_host[1];
+  const int threads = out_channels <= 64 ? 64 : 128;
+  pfn_kernel<2, false, kMaxRows><<<static_cast<unsigned int>(n_cap), threads, 0, static_cast<cudaStream_t>(stream)>>>(
+      voxels, num_points_per_voxel, coors, num_voxels_dev, static_cast<int>(n_cap), max_points, num_point_dim,
+      mid_channels, weight1, bn_scale1, bn_shift1, out_channels, weight2, bn_scale2, bn_shift2, vx, vy, x_off, y_off,
+      out);
+  P3D_LAUNCH_CHECK();
+  return P3D_OK;
+}
+
+}  // namespace
+
 extern "C" int p3d_pillar_feature_net2(const float *voxels, const int32_t *num_points_per_voxel, const int32_t *coors,
                                        const int32_t *num_voxels_dev, int64_t n_cap, int max_points, int num_point_dim,
                                        int mid_channels, const float *weight1, const float *bn_scale1,
                                        const float *bn_shift1, int out_channels, const float *weight2,
                                        const float *bn_scale2, const float *bn_shift2, const float *voxel_size_host,
                                        const float *point_cloud_range_host, float *out, p3d_stream_t stream) {
-  if (!voxels || !num_points_per_voxel || !coors || !weight1 || !bn_scale1 || !bn_shift1 || !weight2 || !bn_scale2 ||
-      !bn_shift2 || !voxel_size_host || !point_cloud_range_host || !out || n_cap < 0 || mid_channels < 1 ||
-      out_channels < 1)
-    return P3D_ERR_INVALID_ARG;
-  if (max_points < 1 || max_points > kMaxM || num_point_dim < 3 || num_point_dim > kMaxF || mid_channels > kMaxMid)
-    return P3D_ERR_UNSUPPORTED;
-  if (n_cap == 0) return P3D_OK;
-  const float vx = voxel_size_host[0], vy = voxel_size_host[1];
-  const float x_off = vx / 2 + point_cloud_range_host[0], y_off = vy / 2 + point_cloud_range_host[1];
-  const int threads = out_channels <= 64 ? 64 : 128;
-  pfn_kernel<2><<<static_cast<unsigned int>(n_cap), threads, 0, static_cast<cudaStream_t>(stream)>>>(
-      voxels, num_points_per_voxel, coors, num_voxels_dev, static_cast<int>(n_cap), max_points, num_point_dim,
-      mid_channels, weight1, bn_scale1, bn_shift1, out_channels, weight2, bn_scale2, bn_shift2, vx, vy, x_off, y_off,
-      out);
-  P3D_LAUNCH_CHECK();
-  return P3D_OK;
+  return launch_pfn2<kMaxM>(voxels, num_points_per_voxel, coors, num_voxels_dev, n_cap, max_points, num_point_dim,
+                            mid_channels, weight1, bn_scale1, bn_shift1, out_channels, weight2, bn_scale2, bn_shift2,
+                            voxel_size_host, point_cloud_range_host, out, stream);
+}
+
+extern "C" int p3d_pillar_feature_net2_wide(const float *voxels, const int32_t *num_points_per_voxel,
+                                            const int32_t *coors, const int32_t *num_voxels_dev, int64_t n_cap,
+                                            int max_points, int num_point_dim, int mid_channels, const float *weight1,
+                                            const float *bn_scale1, const float *bn_shift1, int out_channels,
+                                            const float *weight2, const float *bn_scale2, const float *bn_shift2,
+                                            const float *voxel_size_host, const float *point_cloud_range_host,
+                                            float *out, p3d_stream_t stream) {
+  return launch_pfn2<kMaxMWide>(voxels, num_points_per_voxel, coors, num_voxels_dev, n_cap, max_points, num_point_dim,
+                                mid_channels, weight1, bn_scale1, bn_shift1, out_channels, weight2, bn_scale2,
+                                bn_shift2, voxel_size_host, point_cloud_range_host, out, stream);
 }
 
 extern "C" int p3d_hard_vfe(const float *voxels, const int32_t *num_points_per_voxel, const int32_t *coors,

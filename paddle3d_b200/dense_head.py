@@ -186,16 +186,24 @@ class SecondTrunk:
 class DenseRPNHead:
     def __init__(self, in_channels=256, out_channels=(128, 256), layer_nums=(5, 5), downsample_strides=(1, 2),
                  fpn_out_channels=(256, 256), upsample_strides=(1, 2), tasks=(1, 2, 2, 1, 2, 2), share_conv_channel=64,
-                 f16=True, with_velocity=True, bev_depth=2, trunk=None):
+                 f16=True, with_velocity=None, bev_depth=2, trunk=None, common_heads=COMMON_HEADS):
         """trunk: the network between the BEV image and the shared conv (None: SecondBackbone + SecondFPN from the
         arguments above); another object with SecondTrunk's __call__(x, shape, first=None) / fpn_channels / convs() /
-        export_numpy() contract, on pixel fp16-pair rows with bev_depth 1 (bevdet.BEVDetEncoder)."""
+        export_numpy() contract, on pixel fp16-pair rows with bev_depth 1 (bevdet.BEVDetEncoder).  common_heads: the
+        CenterHead's (name, channels) heads of every task before its "hm" (CenterHead common_heads); with_velocity
+        (default: whether "vel" is among them) decides whether the box decode reads a velocity head."""
         if trunk is not None and (not f16 or bev_depth > 1):
             raise ValueError("a custom trunk runs on the fp16-pair path with bev_depth 1")
         self.tasks = list(tasks)
         self.in_channels, self.bev_depth = in_channels, bev_depth
         self.num_classes = list(tasks)        # CenterHead.num_classes (center_head.py:64)
-        self.with_velocity = with_velocity    # 'vel' in common_heads (center_head.py:77)
+        self.common_heads = tuple((str(n), int(c)) for n, c in common_heads)
+        has_vel = any(n == "vel" for n, _ in self.common_heads)
+        if with_velocity is None:
+            with_velocity = has_vel
+        if with_velocity and not has_vel:
+            raise ValueError("with_velocity needs a 'vel' head in common_heads")
+        self.with_velocity = bool(with_velocity)  # 'vel' in common_heads (center_head.py:77)
         self.f16 = f16
         if f16 and (share_conv_channel % 32 or not 32 <= share_conv_channel <= 320):
             raise ValueError("the fp16-pair head output convs need share_conv_channel a multiple of 32 and at most 320 "
@@ -215,7 +223,7 @@ class DenseRPNHead:
         self.heads = []  # per task: list of (name, ConvModule 64->64, final conv 64->classes)
         for ncls in self.tasks:
             hs = []
-            for name, c in list(COMMON_HEADS) + [("hm", ncls)]:
+            for name, c in list(self.common_heads) + [("hm", ncls)]:
                 hs.append((name, conv(share_conv_channel, share_conv_channel, 3, 1, 1, bias=True, bn_eps=bn5),
                            conv(share_conv_channel, c, 3, 1, 1, bias=True, relu=False)))
             self.heads.append(hs)
@@ -230,8 +238,9 @@ class DenseRPNHead:
         return out
 
     def head_planes(self):
-        """Output planes of the CenterHead: per task 2 + 1 + 3 + 2 + 2 + classes (70 for the six nuScenes tasks)."""
-        return sum(sum(c for _, c in COMMON_HEADS) + n for n in self.tasks)
+        """Output planes of the CenterHead: per task the common heads' channels (2 + 1 + 3 + 2 + 2 by default) + classes
+        (70 for the six nuScenes tasks)."""
+        return sum(sum(c for _, c in self.common_heads) + n for n in self.tasks)
 
     def head_flops(self, h, w):
         """Algorithmic flops (2 x MACs) of the CenterHead on an h x w map: the shared conv, the ConvModules and the output

@@ -1,4 +1,4 @@
-"""KITTI object-split geometry and formats around the PointPillars frames (numpy, float64).
+"""KITTI object-split geometry and formats around the PointPillars and CenterPoint-pillars KITTI frames (numpy, float64).
 
 PARITY UNPINNED: every convention here is recalled from the references below, not checked against a checkout of them.
 
@@ -15,6 +15,11 @@ PARITY UNPINNED: every convention here is recalled from the references below, no
                            box_lidar_to_camera, center_to_corner_box3d (origin (0.5, 1.0, 0.5), axis 1), the 2-D box of
                            the corners projected through P2 (homogeneous coordinate 1), dropped when wholly outside the
                            image and clipped to it, alpha = -arctan2(-y_lidar, x_lidar) + r.
+  centerpoint_to_lidar_boxes
+                           Paddle3D CenterPoint._parse_results_to_sample (paddle3d/models/detection/centerpoint/
+                           centerpoint.py) and the KITTI metric's box conversion: the centerpoint_postprocess op's
+                           (x, y, z_centre, d0, d1, d2, rot) with dims[0:2] swapped, rot -> -(rot + pi / 2) and the box
+                           declared centred (origin (0.5, 0.5, 0.5)), so z drops by h / 2 to the bottom face.
   format_label_lines       kitti_common.kitti_result_line (4 decimals): the 16-field KITTI result line; truncation and
                            occlusion are written as 0.
 """
@@ -24,8 +29,9 @@ import numpy as np
 
 DEFAULT_IMAGE_SHAPE = (375, 1242)  # (H, W) the reference assumes when no image is read
 NEAR_CLIP, FAR_CLIP = 0.001, 100.0
-# KITTI type names in label order of the two PointPillars models
-CLASS_NAMES = {"car": ("Car",), "ped_cyclist": ("Cyclist", "Pedestrian")}
+# KITTI type names in label order of the two PointPillars models and of CenterPoint-pillars KITTI (tasks [Car],
+# [Pedestrian, Cyclist]: synth.CP_PILLARS_KITTI_TASKS)
+CLASS_NAMES = {"car": ("Car",), "ped_cyclist": ("Cyclist", "Pedestrian"), "centerpoint": ("Car", "Pedestrian", "Cyclist")}
 
 _CALIB_KEYS = {"P0": (3, 4), "P1": (3, 4), "P2": (3, 4), "P3": (3, 4), "R0_rect": (3, 3), "Tr_velo_to_cam": (3, 4)}
 
@@ -203,6 +209,14 @@ def to_kitti(boxes, scores, labels, calib, shape=DEFAULT_IMAGE_SHAPE, class_name
     return dict(name=np.array([class_names[int(c)] for c in labels[keep]], dtype=object),
                 alpha=-np.arctan2(-lid[:, 1], lid[:, 0]) + cam[:, 6], bbox=bbox, dimensions=cam[:, [4, 5, 3]],
                 location=cam[:, :3], rotation_y=cam[:, 6], score=scores[keep])
+
+
+def centerpoint_to_lidar_boxes(boxes):
+    """CenterPoint boxes [K, 7] (x, y, z_centre, d0, d1, d2, rot), as the centerpoint_postprocess op and the velocity-free
+    CenterPoint-pillars KITTI frame return them, -> the LiDAR boxes [K, 7] (x, y, z_bottom, w, l, h, theta) to_kitti
+    takes: (x, y, z - d2 / 2, d1, d0, d2, -(rot + pi / 2)), float64."""
+    b = np.asarray(boxes, np.float64).reshape(-1, 7)
+    return np.stack([b[:, 0], b[:, 1], b[:, 2] - b[:, 5] / 2, b[:, 4], b[:, 3], b[:, 5], -(b[:, 6] + np.pi / 2)], axis=1)
 
 
 def format_label_lines(annos):

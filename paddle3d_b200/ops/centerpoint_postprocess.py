@@ -46,13 +46,15 @@ def centerpoint_postprocess_device(hm, reg, height, dim, vel, rot, voxel_size, p
 
 
 def centerpoint_postprocess_heads(h, voxel_size, point_cloud_range, test_cfg, label_offsets):
-    """centerpoint_postprocess_device (with velocity) of a CenterHead output h = dict name -> [tensor per task], with the
-    range limit, down ratio, threshold and NMS settings of test_cfg and the tasks' label offsets."""
+    """centerpoint_postprocess_device of a CenterHead output h = dict name -> [tensor per task], with the range limit,
+    down ratio, threshold and NMS settings of test_cfg and the tasks' label offsets.  With a "vel" head the boxes have 9
+    columns (x, y, z, d0, d1, d2, vx, vy, rot), without one 7."""
     tc = test_cfg
+    with_velocity = "vel" in h
     return centerpoint_postprocess_device(
-        h["hm"], h["reg"], h["height"], h["dim"], h["vel"], h["rot"], voxel_size, point_cloud_range,
-        tc["post_center_limit_range"], label_offsets, tc["down_ratio"], tc["score_threshold"], tc["nms_iou_threshold"],
-        tc["nms_pre_max_size"], tc["nms_post_max_size"], True)
+        h["hm"], h["reg"], h["height"], h["dim"], h["vel"] if with_velocity else h["reg"], h["rot"], voxel_size,
+        point_cloud_range, tc["post_center_limit_range"], label_offsets, tc["down_ratio"], tc["score_threshold"],
+        tc["nms_iou_threshold"], tc["nms_pre_max_size"], tc["nms_post_max_size"], with_velocity)
 
 
 def centerpoint_postprocess(hm, reg, height, dim, vel, rot, voxel_size, point_cloud_range, post_center_range,

@@ -6,6 +6,8 @@ import torch
 from .._lib import check, host_floats, lib
 from .._mem import ptr, require_cuda, stream
 
+WIDE_FROM = 65  # points per pillar from which pillar_feature_net2 launches p3d_pillar_feature_net2_wide
+
 
 def fold_bn(bn_gamma, bn_beta, bn_mean, bn_var, bn_eps, device):
     """BatchNorm1D(eval) as (scale, shift) device tensors, folded on the host in fp64: do this once per model."""
@@ -40,7 +42,9 @@ def pillar_feature_net2(voxels, num_points_per_voxel, coors, layers, voxel_size,
                         folded=None):
     """PillarFeatureNet with two PFNLayers (CenterPoint-pillars, feat_channels [64, 64]) as one launch.  layers: two dicts
     of weight / gamma / beta / mean / var / eps, weight [F + 5, mid] then [2 mid, out] on the device.  folded: the two
-    (scale, shift) pairs of fold_bn, to keep host->device copies out of the per-frame path.  Returns [n, out]."""
+    (scale, shift) pairs of fold_bn, to keep host->device copies out of the per-frame path.  Returns [n, out].  Up to 64
+    points per pillar run on p3d_pillar_feature_net2, 65 to 128 on p3d_pillar_feature_net2_wide (same arithmetic, more
+    shared memory per pillar)."""
     voxels = require_cuda(voxels, "voxels", torch.float32)
     npv = require_cuda(num_points_per_voxel, "num_points_per_voxel", torch.int32)
     coors = require_cuda(coors, "coors", torch.int32)
@@ -56,9 +60,9 @@ def pillar_feature_net2(voxels, num_points_per_voxel, coors, layers, voxel_size,
     (s1, t1), (s2, t2) = folded
     out = torch.zeros((n, c), dtype=torch.float32, device=dev)
     nump = ptr(require_cuda(num_voxels, "num_voxels", torch.int32)) if num_voxels is not None else ptr(None)
-    check(lib().p3d_pillar_feature_net2(ptr(voxels), ptr(npv), ptr(coors), nump, n, m, f, mid, ptr(w1), ptr(s1), ptr(t1),
-                                        c, ptr(w2), ptr(s2), ptr(t2), host_floats(voxel_size),
-                                        host_floats(point_cloud_range), ptr(out), stream(dev)), "pillar_feature_net2")
+    fn = lib().p3d_pillar_feature_net2 if m < WIDE_FROM else lib().p3d_pillar_feature_net2_wide
+    check(fn(ptr(voxels), ptr(npv), ptr(coors), nump, n, m, f, mid, ptr(w1), ptr(s1), ptr(t1), c, ptr(w2), ptr(s2), ptr(t2),
+             host_floats(voxel_size), host_floats(point_cloud_range), ptr(out), stream(dev)), "pillar_feature_net2")
     return out
 
 

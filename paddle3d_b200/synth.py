@@ -40,6 +40,18 @@ CENTERPOINT_TEST_CFG = dict(  # yml:163-172
 # the same test config for CenterPoint-pillars, whose head runs at a quarter of the 512 x 512 grid (PARITY UNPINNED)
 CENTERPOINT_PILLARS_TEST_CFG = dict(CENTERPOINT_TEST_CFG, down_ratio=4)
 
+# CenterPoint-pillars KITTI, configs/centerpoint/centerpoint_pillars_016voxel_kitti.yml (PARITY UNPINNED: recalled from the
+# yml and its deploy command line `--max_points_in_voxel 100`, not checked against either): 0.16 m pillars over the KITTI
+# camera range -> 432 x 496, 100 points per pillar, 40000 pillars at test time (the yml's test max_num_voxels).
+# num_points: the rows a frame takes after the camera cull (tools/infer_kitti.py's default).
+CP_PILLARS_KITTI = dict(name="centerpoint_pillars_016_kitti", num_points=40000, point_dim=4, voxel_size=[0.16, 0.16, 4.0],
+                        point_cloud_range=[0.0, -39.68, -3.0, 69.12, 39.68, 1.0], max_points=100, max_voxels=40000)
+CP_PILLARS_KITTI_TASKS = [1, 2]  # [Car], [Pedestrian, Cyclist] (yml tasks; the order is recalled)
+# the yml's test_cfg (PARITY UNPINNED): the head runs at half the 432 x 496 grid
+CP_PILLARS_KITTI_TEST_CFG = dict(
+    post_center_limit_range=[-10.0, -50.0, -10.0, 80.0, 50.0, 10.0], nms_pre_max_size=1000, nms_post_max_size=83,
+    nms_iou_threshold=0.1, score_threshold=0.1, down_ratio=2)
+
 
 def uniform_cloud(cfg, seed, num_points=None, margin=0.02):
     """Worst case for hashing: x,y,z ~ U(range, slightly overshooting so some points fall outside)."""

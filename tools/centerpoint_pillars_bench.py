@@ -1,8 +1,10 @@
 #!/usr/bin/env python
-"""tools/centerpoint_pillars_bench.py — CenterPoint-pillars nuScenes frames/s on an H100.
+"""tools/centerpoint_pillars_bench.py — CenterPoint-pillars nuScenes or KITTI frames/s on an H100.
 
   python tools/centerpoint_pillars_bench.py [--steps K] [--warmup W] [--in-flight L] [--no-cpu-baseline] [--stream]
                                             [--dump-outputs DIR]
+  python tools/centerpoint_pillars_bench.py --config kitti [--kitti-raw] [--steps K] [--warmup W] [--in-flight L]
+                                            [--no-cpu-baseline]
 
 A step = one 300k x 5-point synth.lidar_cloud frame (synth.CP_PILLARS) through
 centerpoint_pillars.CenterPointPillarsHotPath: hard_voxelize (0.2 m pillars, 20 points) -> two-layer PillarFeatureNet ->
@@ -11,6 +13,11 @@ pixel fp16-pair image 512 x 512 x 64 -> SecondBackbone + SecondFPN + CenterHead 
 graph-timed stages) is bench.py's, imported from it, so every model is measured the same way.  --stream adds frames/s
 through CenterPointSweep.infer_stream over a 70-sweep synth.sweep_sequence (10 sweeps per frame, merged on the device),
 measured as tools/sweep_bench.py measures the voxel model.
+
+--config kitti runs centerpoint_pillars_016voxel_kitti (synth.CP_PILLARS_KITTI, CONFIG_KITTI: 100 points per pillar,
+432 x 496 grid, two velocity-free tasks, the head at 248 x 216) on synth.kitti_raw_cloud scans: culled to the camera
+frustum on the host and NaN-padded to the frame's 40000 rows (infer_many), or with --kitti-raw the raw scans culled inside
+the captured frame (frame.KITTI_INPUT, infer_kitti_many).  See run_kitti.
 """
 import argparse
 import json
@@ -203,8 +210,138 @@ def run(args):
     print(json.dumps(line))
 
 
+KITTI_SCANS = 8  # distinct synth.kitti_raw_cloud scans cycled through
+
+
+def run_kitti(args):
+    """CenterPoint-pillars KITTI: frames/s with 1 and --in-flight frames in flight (host arrays in, host boxes out), next
+    to the card's name and power limit; frame 0 against the CPU arm (tests/centerpoint_pillars_kitti_oracle.py); the
+    stages graph-timed on frame 0 (hard_voxelize at P = 100, the wide pillar encoder, the pixel image, the dense part, the
+    postprocess), with the bytes of the [40000, 100, 4] padded-voxel tensor hard_voxelize zero-fills per frame."""
+    import torch
+    from paddle3d_b200 import frame, kitti, synth
+    from paddle3d_b200.centerpoint_pillars import CONFIG_KITTI, CenterPointPillarsHotPath
+    from paddle3d_b200.ops import pillar_encoder as pe
+    from paddle3d_b200.ops import sparse_nn as sp
+    from paddle3d_b200.ops import voxelize as vox
+    from paddle3d_b200.pipeline import CenterPointSweep
+    if not torch.cuda.is_available():
+        raise SystemExit("centerpoint_pillars_bench.py needs a CUDA device (no CPU fallback exists)")
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    cfg = synth.CP_PILLARS_KITTI
+    n = cfg["num_points"]
+    scans = [synth.kitti_raw_cloud(s) for s in range(KITTI_SCANS)]
+    items = [(c, kitti.frustum_planes(cal, shape)) for c, cal, shape in scans]
+    kept = [kitti.remove_camera_invisible(*it) for it in items]
+
+    def padded(k):
+        full = np.full((n, 4), np.nan, np.float32)
+        full[:len(k)] = k
+        return full
+    frames = [padded(k) for k in kept]
+    host_frames = [torch.from_numpy(f).pin_memory() for f in frames]
+    calib_pts = torch.from_numpy(frames[0]).to(dev)
+    ident = gpu_identity(0)
+    kw = dict(cfg=cfg, model_cfg=CONFIG_KITTI, device=dev, seed=0, bn_gain=BN_GAIN)
+    if args.kitti_raw:
+        kw["sweep_input"] = frame.KITTI_INPUT
+    rates, first = {}, None
+    for lanes in sorted({1, max(1, args.in_flight)}):
+        sweep = CenterPointSweep(lanes, frame_cls=CenterPointPillarsHotPath, **kw)
+        sweep.calibrate_head(calib_pts)
+        for p in sweep.lanes:
+            if args.kitti_raw:
+                p.infer_kitti(*items[0])
+            else:
+                p.points.copy_(calib_pts)
+            p.capture(count_nodes=p is sweep.lanes[0])
+        if args.kitti_raw:
+            def run_items(seq):
+                return sweep.infer_kitti_many(iter(seq))
+            src = items
+        else:
+            def run_items(seq):
+                return sweep.infer_many(iter(seq))
+            src = host_frames
+        list(run_items([src[i % len(src)] for i in range(args.warmup)]))
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        k = sum(1 for _ in run_items([src[i % len(src)] for i in range(args.steps)]))
+        rates["frames_per_s_%d_in_flight" % lanes] = k / (time.perf_counter() - t0)
+        if first is None:
+            first = sweep
+        else:
+            del sweep
+    pipe = first.lanes[0]
+    m = pipe.model
+    got = [t.clone() for t in (pipe.infer_kitti(*items[0]) if args.kitti_raw else pipe.infer(host_frames[0]))]
+    line = {"metric": "CenterPoint-pillars KITTI frames/sec (centerpoint_pillars_016voxel_kitti), %s" % (
+                "raw scans, camera cull inside the frame" if args.kitti_raw else "host-culled scans"),
+            "model": "centerpoint_pillars_kitti", "unit": UNIT, "steps": args.steps, "warmup": args.warmup,
+            "data": "synthetic scans (synth.kitti_raw_cloud, %d seeds; %.0f of %.0f points in the camera's view), "
+                    "num_points %d" % (len(items), np.mean([len(k) for k in kept]), np.mean([len(c) for c, _ in items]), n),
+            "dtype": "f16x3 (fp16 hi/lo' pairs, f32 accumulation) dense; fp32 encoder and postprocess",
+            "gpu": ident, **rates, "gpu_launches_per_step": pipe.graph_nodes["kernel"] if pipe.graph_nodes else None,
+            "boxes_frame0": int(len(got[0])), "boxes_per_task_frame0": [int(v) for v in pipe.h_counts[:-1]],
+            "reference_figure": "Paddle3D's docs/models/centerpoint/README.md gives 43.96 FPS (fp32) and 74.21 FPS (fp16) "
+                                "for this config on a V100 with TensorRT: the reference's own figure on other hardware, "
+                                "not a like-for-like comparison"}
+    # stages on frame 0, each graph-timed on the frame's stream
+    st = pipe.stream
+    P, V = cfg["max_points"], cfg["max_voxels"]
+    nx, ny = m.grid
+    pts = torch.from_numpy(frames[0]).to(dev)
+    with torch.cuda.stream(st):
+        voxels, co, npv, nv = vox.hard_voxelize(pts, cfg["voxel_size"], cfg["point_cloud_range"], P, V)
+        coors = torch.nn.functional.pad(co, (1, 0))
+        feats = pe.pillar_feature_net2(voxels, npv, coors, m.pfn_dev, cfg["voxel_size"], cfg["point_cloud_range"],
+                                       num_voxels=nv, folded=m.pfn_folded)
+        image, shape = sp.sparse_coo_tensor(coors, feats, [1, 1, ny, nx, m.C], num=nv).to_pixel_h16()
+        h = m.dense(image, shape)
+    st.synchronize()
+    n_pillars = int(nv.item())
+    stage = {
+        "hard_voxelize (P = 100)": graph_time_ms(lambda: vox.hard_voxelize(pts, cfg["voxel_size"], cfg["point_cloud_range"],
+                                                                          P, V), st, 20),
+        "pillar_feature_net2 (p3d_pillar_feature_net2_wide)": graph_time_ms(
+            lambda: pe.pillar_feature_net2(voxels, npv, coors, m.pfn_dev, cfg["voxel_size"], cfg["point_cloud_range"],
+                                           num_voxels=nv, folded=m.pfn_folded), st, 20),
+        "pixel_image": graph_time_ms(lambda: sp.sparse_coo_tensor(coors, feats, [1, 1, ny, nx, m.C],
+                                                                  num=nv).to_pixel_h16(), st, 20),
+        "dense (backbone + FPN + CenterHead)": graph_time_ms(lambda: m.dense(image, shape), st, 5),
+        "centerpoint_postprocess": graph_time_ms(lambda: m.postprocess(h), st, 20),
+    }
+    fl = m.flops()
+    dense_flops = fl["backbone"] + fl["fpn"] + fl["head"]
+    pts_in = int(npv[:n_pillars].sum().item())
+    line.update(stage_ms_graph=stage, num_pillars_frame0=n_pillars, points_in_pillars_frame0=pts_in,
+                dense={"gflop": {k: round(v / 1e9, 2) for k, v in fl.items()}, "algorithmic_flops": dense_flops,
+                       "achieved_TFLOP_per_s": dense_flops / (stage["dense (backbone + FPN + CenterHead)"] * 1e-3) / 1e12},
+                voxelize={"padded_voxel_bytes": V * P * cfg["point_dim"] * 4,
+                          "note": "hard_voxelize writes the whole [max_voxels, max_points, 4] fp32 tensor, zero rows "
+                                  "included, every frame; the pillar encoder reads the pillars' rows of it"})
+    if not args.no_cpu_baseline:
+        sys.path.insert(0, os.path.join(ROOT, "tests"))
+        import oracle
+        from centerpoint_pillars_kitti_oracle import CpuCenterPointPillarsHeads
+        cpu = CpuCenterPointPillarsHeads(cfg, m.export_numpy(), m.test_cfg, m.label_off)
+        t0 = time.perf_counter()
+        r = cpu.run(kept[0])
+        cpu_s = time.perf_counter() - t0
+        line["cpu_baseline"] = {"value": 1.0 / cpu_s, "unit": UNIT, "cores": oracle.num_threads(), "stage_s": r["times"]}
+        chk = frame_check(got, r, [int(v) for v in pipe.h_counts[:-1]], m.test_cfg)
+        chk["pillars_gpu"] = n_pillars
+        line["frame0_check"] = chk
+    print(json.dumps(line))
+
+
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--config", choices=("nuscenes", "kitti"), default="nuscenes",
+                    help="nuscenes: centerpoint_pillars_02voxel_nuscenes_10sweep; kitti: centerpoint_pillars_016voxel_kitti")
+    ap.add_argument("--kitti-raw", action="store_true",
+                    help="with --config kitti: raw scans, the camera frustum cull inside the captured frame")
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--in-flight", type=int, default=4, help="frames computing concurrently (CenterPointSweep lanes)")
@@ -214,7 +351,9 @@ def main():
                     help="after the timed steps, write the boxes / scores / labels of the last timed frame to DIR/*.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
-    run(args)
+    if args.kitti_raw and args.config != "kitti":
+        ap.error("--kitti-raw needs --config kitti")
+    (run_kitti if args.config == "kitti" else run)(args)
 
 
 if __name__ == "__main__":

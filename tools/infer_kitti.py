@@ -1,15 +1,16 @@
 #!/usr/bin/env python
-"""tools/infer_kitti.py — PointPillars on a KITTI object split, raw scans in, KITTI label files out.
+"""tools/infer_kitti.py — PointPillars or CenterPoint-pillars on a KITTI object split, raw scans in, KITTI label files out.
 
-  python tools/infer_kitti.py --model X.pdparams --config car|ped_cyclist --root <split dir> [--ids list.txt]
+  python tools/infer_kitti.py --model X.pdparams --config car|ped_cyclist|centerpoint --root <split dir> [--ids list.txt]
                               --out DIR [--lanes L] [--num-points N] [--device cuda:0]
 
 <split dir> is a KITTI object split (e.g. training/ or testing/) with velodyne/<id>.bin (raw HDL-64E scans, x y z
 reflectance fp32), calib/<id>.txt and image_2/<id>.png (only the PNG header is read, for the image size; without the
 image the reference's 375 x 1242 is used).  --ids: a file of frame ids, one per line (default: every velodyne/*.bin).
 Each scan is culled to the left colour camera's view frustum inside the captured frame (frame.KITTI_INPUT), L frames
-run in flight (pipeline.CenterPointSweep), and DIR/<id>.txt gets one KITTI result line per box (kitti.to_kitti), the
-format the KITTI devkit's evaluate_object reads.
+run in flight (pipeline.CenterPointSweep), and DIR/<id>.txt gets one KITTI result line per box (kitti.to_kitti; the
+CenterPoint boxes through kitti.centerpoint_to_lidar_boxes first), the format the KITTI devkit's evaluate_object reads.
+--config centerpoint is centerpoint_pillars_016voxel_kitti (centerpoint_pillars.CONFIG_KITTI).
 """
 import argparse
 import collections
@@ -43,9 +44,12 @@ def load_frame(root, fid):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", required=True, help="a Paddle3D PointPillars checkpoint (.pdparams) of --config")
+    ap.add_argument("--model", required=True,
+                    help="a Paddle3D checkpoint (.pdparams) of --config: PointPillars (car, ped_cyclist) or "
+                         "CenterPoint-pillars (centerpoint)")
     ap.add_argument("--config", choices=sorted(kitti.CLASS_NAMES), default="car",
-                    help="car: pointpillars_xyres16_kitti_car; ped_cyclist: the cyclist / pedestrian model")
+                    help="car: pointpillars_xyres16_kitti_car; ped_cyclist: the cyclist / pedestrian model; "
+                         "centerpoint: centerpoint_pillars_016voxel_kitti")
     ap.add_argument("--root", required=True, help="KITTI object split directory (velodyne/, calib/, image_2/)")
     ap.add_argument("--ids", default=None, help="file of frame ids, one per line")
     ap.add_argument("--out", required=True, help="directory for the <id>.txt label files")
@@ -57,15 +61,19 @@ def main():
 
     import torch
     from paddle3d_b200 import frame, synth
+    from paddle3d_b200.centerpoint_pillars import CONFIG_KITTI, CenterPointPillarsHotPath
     from paddle3d_b200.pipeline import CenterPointSweep
     from paddle3d_b200.pointpillars import CONFIG, CONFIG_PED_CYCLIST, PointPillarsHotPath
     if not torch.cuda.is_available():
         raise SystemExit("infer_kitti.py needs a CUDA device (no CPU fallback exists)")
-    cfg, model_cfg = (synth.C2, CONFIG) if args.config == "car" else (synth.C2_PED_CYCLIST, CONFIG_PED_CYCLIST)
+    frame_cls, cfg, model_cfg = {"car": (PointPillarsHotPath, synth.C2, CONFIG),
+                                 "ped_cyclist": (PointPillarsHotPath, synth.C2_PED_CYCLIST, CONFIG_PED_CYCLIST),
+                                 "centerpoint": (CenterPointPillarsHotPath, synth.CP_PILLARS_KITTI, CONFIG_KITTI)}[args.config]
+    centerpoint = frame_cls is CenterPointPillarsHotPath
     names = kitti.CLASS_NAMES[args.config]
     ids = frame_ids(args.root, args.ids)
     os.makedirs(args.out, exist_ok=True)
-    sweep = CenterPointSweep(max(1, args.lanes), frame_cls=PointPillarsHotPath, cfg=cfg, model_cfg=model_cfg,
+    sweep = CenterPointSweep(max(1, args.lanes), frame_cls=frame_cls, cfg=cfg, model_cfg=model_cfg,
                              device=torch.device(args.device), num_points=args.num_points, weights=args.model,
                              sweep_input=frame.KITTI_INPUT)
     if not ids:
@@ -84,7 +92,8 @@ def main():
 
     for boxes, scores, labels in sweep.infer_kitti_many(items()):
         fid, calib, shape = meta.popleft()
-        annos = kitti.to_kitti(boxes.numpy(), scores.numpy(), labels.numpy(), calib, shape, names)
+        boxes = kitti.centerpoint_to_lidar_boxes(boxes.numpy()) if centerpoint else boxes.numpy()
+        annos = kitti.to_kitti(boxes, scores.numpy(), labels.numpy(), calib, shape, names)
         kitti.write_label_file(os.path.join(args.out, fid + ".txt"), annos)
     print("wrote %d label files to %s" % (len(ids), args.out))
 
